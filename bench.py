@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- Mfeatures/s (extract + match) of the B200 feature hot path.
+"""bench.py -- Mfeatures/s (extract + match) of the H100 feature hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {2,3,4}] [--frames F] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config {2,3,4}] [--frames F] [--impl reference] [--dump-outputs DIR]
 
 --config 2 (default, the configuration BASELINE.json's metric is quoted on): a stream of 3-fisheye 754x480 multi-camera frames,
     8-level pyramid (scale 1.2), 2000 features per camera, mdBRIEF-256 with masks; every (frame, camera) is brute-force matched
@@ -18,9 +18,14 @@
 One step = one pass over one batch of F frames per GPU (synthetic, seeded).  `value` times the step with the inputs already
 resident in HBM (CUDA events on the launching stream, max over ranks); `e2e` times the same work through the public API with
 pinned HOST buffers, H2D and D2H inside the timed region.  `roofline` is the fused pyramid+blur+FAST kernel (K1): algorithmic
-bytes per launch / CUDA-event time / measured HBM peak.  `cpu_baseline` / --impl reference: the reference's own extractor and
-matcher (oracle/_ref/libmcs_ref.so, compiled from /root/reference where that exists) on the host cores over a bounded sample,
-else the oracle port.
+bytes per launch / CUDA-event time / the H100 SXM data-sheet HBM3 bandwidth.  `cpu_baseline` / --impl reference: the reference's
+own extractor and matcher (oracle/_ref/libmcs_ref.so, built where MCS_REFERENCE_DIR names a reference checkout) on the host cores
+over a bounded sample, else the oracle port.
+
+--dump-outputs DIR: after the timed steps, what the last timed step computed -- the arrays a caller of the timed path receives --
+as DIR/<name>.npy (float32 / float64): per-image feature counts (and greedy match counts) of the whole batch, and the keypoints,
+descriptors, descriptor masks and matches of a fixed sample of images.  The inputs are seeded, so two builds can be compared
+output for output.
 """
 import argparse
 import json
@@ -49,10 +54,39 @@ CONFIGS = {
 
 
 def hbm_peak():
-    p = ROOT / "MEASURED_PEAKS.json"
-    if p.exists():
-        return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet (HBM3, 3.35 TB/s); not a measured figure"
+
+
+DUMP_IMAGES = 32          # images of the batch whose per-feature outputs --dump-outputs writes (seeded choice)
+
+
+def dump_outputs(path, outputs, n_images):
+    """outputs: name -> per-image vector [n_images] or per-feature array [n_images, capacity, ...], with the feature counts under
+    "counts"; float32 / float64 .npy files under `path`.  Rows at or beyond an image's count are buffer padding a caller never
+    reads: they are written as -1 (match / map-point indices) or 0 (everything else), so that dumps compare real outputs only."""
+    path = pathlib.Path(path)
+    path.mkdir(parents=True, exist_ok=True)
+    host = {k: (v.cpu().numpy() if hasattr(v, "cpu") else np.asarray(v)) for k, v in outputs.items()}
+    pick = np.sort(np.random.default_rng(0).choice(n_images, min(DUMP_IMAGES, n_images), replace=False))
+    arrays = {"sample_images": pick.astype(np.float64)}
+
+    def per_feature(name, a):
+        a = a[pick].astype(np.float64 if a.dtype.itemsize > 4 else np.float32)
+        pad = np.arange(a.shape[1])[None, :] >= host["counts"][pick][:, None]
+        a[pad] = -1 if ("match" in name or "mappoint" in name) else 0
+        return a
+    for name, a in host.items():
+        if a.dtype.names:                                   # keypoints: one file per field
+            for f in a.dtype.names:
+                arrays[f"{name}_{f}"] = per_feature(name, a[f])
+        elif a.ndim == 1 and len(a) == n_images:
+            arrays[name] = a.astype(np.float64)
+        else:
+            arrays[name] = per_feature(name, a)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, f"--dump-outputs would write {total / 2**20:.0f} MB"
+    for name, a in arrays.items():
+        np.save(path / f"{name}.npy", a)
 
 
 def rig_cams(cfg):
@@ -71,7 +105,7 @@ def make_stream(cams, cam_ids, n_frames, seed0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -96,6 +130,7 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         sm = [float(r[1]) for r in self.rows if len(r) >= 9 and r[1].replace(".", "").isdigit()]
         mx = [float(r[2]) for r in self.rows if len(r) >= 9 and r[2].replace(".", "").isdigit()]
         reasons = set()
@@ -330,9 +365,12 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--ref-frames", type=int, default=8, help="frames per step of the CPU reference arm (config 2)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     cfg_id, cfg = args.config, CONFIGS[args.config]
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what the GPU path computed; it has no meaning with --impl reference")
         return run_reference(args, cfg_id, cfg)
 
     import torch
@@ -347,7 +385,7 @@ def main():
     dev = torch.device("cuda", local)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    assert api.device_count() > 0, "no sm_100 device"
+    assert api.device_count() > 0, "no sm_90 (H100) device"
     F = args.frames or cfg["frames"]
     W, H, NF = cfg["w"], cfg["h"], cfg["nfeatures"]
     cams = rig_cams(cfg)
@@ -366,11 +404,12 @@ def main():
     PITCH = (W + 63) // 64 * 64                                                # 16-byte aligned rows: K1 stages by TMA
     dev_images = torch.zeros((B, H, PITCH), dtype=torch.uint8, device=dev)
     dev_images[:, :, :W] = host_images.to(dev, non_blocking=True).view(B, H, W)
-    # L2 rule: a step must not find its inputs in the 126 MB L2 from the step before.  Config 2 streams 139 MB of images per step
-    # (larger than L2 by itself); the small rig configs rotate through enough copies of their input that > 140 MB of other
+    # L2 rule: a step must not find its inputs in the 50 MB L2 of the H100 from the step before.  Config 2 streams 142 MB of images
+    # per step (larger than L2 by itself); the small rig configs rotate through enough copies of their input that > 60 MB of other
     # input is read before a copy comes round again.
+    L2_MB = 50
     in_bytes = B * H * PITCH
-    n_rot = 1 if in_bytes > 130e6 else int(np.ceil(140e6 / in_bytes)) + 1
+    n_rot = 1 if in_bytes > 55e6 else int(np.ceil(60e6 / in_bytes)) + 1
     rot_images = [dev_images] + [dev_images.clone() for _ in range(n_rot - 1)]
 
     ex = api.mdBRIEFextractorOct(nfeatures=NF, nlevels=NLEVELS, do_dBrief=True, learnMasks=True)
@@ -436,9 +475,11 @@ def main():
         t_c = time.perf_counter()
         mp = api.MapPoints(np.zeros(len(scene["world"]), np.uint8), iv, lv, px, py, vc, scene["mp_desc"], scene["mp_dmask"])
         mt = api.cORBmatcher(0.8, False, ds, True)
-        n, _ = mt.SearchByProjection(Fr, mp, 3.0)
+        n, frame_mp = mt.SearchByProjection(Fr, mp, 3.0)
         t_d = time.perf_counter()
         stats["matches"] = n
+        stats["outputs"] = {"frame_mappoints": np.concatenate([np.pad(frame_mp[o:o + c], (0, cap - c), constant_values=-1)[None]
+                                                              for o, c in zip(np.cumsum(counts) - counts, counts)])}
         stats["match_call_ms"] = (t_d - t_m3) * 1e3
         stats["parts_ms"] = {"wait_extract+d2h": (t_a - t_m3) * 1e3, "frame_view": (t_b - t_a) * 1e3, "mcs_project_mappoints": (t_c - t_b) * 1e3,
                              "mcs_search_by_projection": (t_d - t_c) * 1e3}
@@ -449,9 +490,10 @@ def main():
         valid1 = (np.arange(cap)[None, :] < counts[:, None]).astype(np.uint8).reshape(-1)
         # every key frame of the batch against the database as its own SearchByBoW(KF1, KF2): independent "already matched" state
         # per frame, the K-best lists of all frames from one launch
-        nms, _ = api.match_bruteforce_batch_device(v["desc"].view(B * cap, ds), v["dmask"].view(B * cap, ds), valid1, np.arange(B + 1) * cap,
-                                                   scene["db_t"], scene["dbm_t"], None, m.TH_LOW_, 0.9, stream=stream)
+        nms, m12_db = api.match_bruteforce_batch_device(v["desc"].view(B * cap, ds), v["dmask"].view(B * cap, ds), valid1, np.arange(B + 1) * cap,
+                                                        scene["db_t"], scene["dbm_t"], None, m.TH_LOW_, 0.9, stream=stream)
         stats["matches"] = int(nms.sum())
+        stats["outputs"] = {"nmatches": nms, "matches12": m12_db.reshape(B, cap)}
         stats["match_call_ms"] = (time.perf_counter() - t_m) * 1e3      # includes waiting for this step's extraction (the counts read)
 
     step_no = [0]
@@ -530,6 +572,11 @@ def main():
         e1.record(stream)
         barrier()
         ms = e0.elapsed_time(e1)
+        if args.dump_outputs and rank == 0:
+            res = {"counts": out["counts"], "kps": out["kps"].cpu().numpy().view(api.KEYPOINT_DTYPE).reshape(B, cap),
+                   "desc": out["desc"], "dmask": out["dmask"]}
+            res.update({"matches12": m12, "nmatches": nmat} if cfg_id == 2 else stats["outputs"])
+            dump_outputs(args.dump_outputs, res, B)
     clocks = sampler.stop() if rank == 0 else None
     feats_rank = int(out["counts"].sum().item())
     redo_n = int(redo.sum().item()) if cfg_id == 2 else 0
@@ -630,26 +677,21 @@ def main():
         peak, peak_src = hbm_peak()
         achieved = alg_bytes_img * B / (k_ms[0] * 1e-3) / 1e9                  # all 8 level launches together
         achieved_blur = (alg_bytes_img + P) * B / (k_ms[0] * 1e-3) / 1e9       # counting the fused blurred output (SURVEY 8d: +P)
-        traffic, traffic_note = None, "no committed ncu capture found"
-        tp = ROOT / "profiles" / "k1_traffic.json"
-        if tp.exists():        # DRAM bytes of K1 from the committed `ncu --set full` capture, per image; scaled to this batch
-            tj = json.loads(tp.read_text())
-            traffic = tj["dram_bytes_per_image"] * B / NLEVELS
-            traffic_note = f"bytes per launch (average of the 8 level launches), from {tj['source']} ({tj.get('images', '?')} images in the capture)"
         roof = {"kernel": "pyr_fast_kernel (K1, 8 launches/step, one per level)", "bound": "hbm", "achieved": achieved, "peak": peak,
-                "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_note": traffic_note,
+                "unit": "GB/s", "frac": achieved / peak,
                 "achieved_counting_blurred_output": achieved_blur, "frac_counting_blurred_output": achieved_blur / peak,
                 "algorithmic_bytes_per_launch_avg": alg_bytes_img * B / NLEVELS, "peak_source": peak_src,
                 "algorithmic_bytes_per_camera_frame": alg_bytes_img, "ms_per_launch_avg": k_ms[0] / NLEVELS,
                 "stage_ms": {"k1_pyr_blur_fast": k_ms[0], "k2_octree": k_ms[1], "k3_angle_describe": k_ms[2], "m2_match_greedy": match_ms}}
         n_feat = int(feats_rank)
-        other = {"k3_describe_kernel": {"bound": "fp32 issue (tier 1) / FP64 (tiers 2, 3); see profiles/", "algorithmic_GB_per_s":
+        other = {"k3_describe_kernel": {"bound": "fp32 issue (tier 1) / FP64 (tiers 2, 3)", "algorithmic_GB_per_s":
                                         n_feat * (845 + 51 * 51 + 28 + 64) / (k_ms[2] * 1e-3) / 1e9},
                  "k2_octree_kernel": {"bound": "latency (one CTA per image-level, serial passes)", "ms": k_ms[1]}}
         if cfg_id == 2 and match_ms:
             pairs = float((B - NC) if B > NC else 0) * NF * NF
-            sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
-            popc_rate = 148 * 16 * sm_mhz * 1e6                   # POPC issues on the XU pipe: 16 lanes / clk / SM (DESIGN.md section 7)
+            sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0
+            sms = torch.cuda.get_device_properties(dev).multi_processor_count
+            popc_rate = sms * 16 * sm_mhz * 1e6                   # POPC: 16 results / clk / SM on sm_90 (CUDA C++ Programming Guide, arithmetic instruction throughput)
             # mcs_match_stream_greedy_device = K-best lists (entries beyond the relevance bound of the acceptance rule left out) +
             # greedy replay; timed next to it: the plain K-best lists and the replay over them
             other["m2_match_stream_greedy"] = {
@@ -684,10 +726,10 @@ def main():
             "warmup": max(args.warmup, 3), "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": "u8", "data": "synthetic",
             "config": bench_config(cfg_id, cfg),
-            "run": bench_run(cfg, F, NC, world, features_per_step=int(feats.item()), matches_per_step_rank0=matches_rank, matcher_stats={k: v for k, v in stats.items() if k != 'matches'},
+            "run": bench_run(cfg, F, NC, world, features_per_step=int(feats.item()), matches_per_step_rank0=matches_rank, matcher_stats={k: v for k, v in stats.items() if k not in ('matches', 'outputs')},
                              greedy_replay_redo_images=redo_n,
-                             l2=(f"inputs {in_bytes / 1e6:.0f} MB per step, larger than the 126 MB L2" if n_rot == 1 else
-                                 f"inputs {in_bytes / 1e6:.0f} MB per step, rotated through {n_rot} copies ({n_rot * in_bytes / 1e6:.0f} MB > 126 MB L2) so no step "
+                             l2=(f"inputs {in_bytes / 1e6:.0f} MB per step, larger than the {L2_MB} MB L2" if n_rot == 1 else
+                                 f"inputs {in_bytes / 1e6:.0f} MB per step, rotated through {n_rot} copies ({n_rot * in_bytes / 1e6:.0f} MB > {L2_MB} MB L2) so no step "
                                  f"finds its input cached") + f"; pyramid + blurred pyramid written and re-read within a step: {2 * P * B / 1e6:.0f} MB"),
             "e2e": {"value": e2e_val, "unit": "Mfeatures/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h, "api": e2e_api, "steps": e2e_steps},
             "gpu_launches": args.steps * launches, "clocks": clocks, "roofline": roof, "cpu_baseline": cpu,

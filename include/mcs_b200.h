@@ -1,5 +1,5 @@
 /*
- * mcs_b200.h -- C ABI of the B200-native MultiCol-SLAM feature hot path.
+ * mcs_b200.h -- C ABI of the H100-native (sm_90a) MultiCol-SLAM feature hot path.
  *
  * One shared library (libmcs_b200.so) replaces the arithmetic behind
  *   mdBRIEFextractorOct::operator()            (ref include/mdBRIEFextractorOct.h:355-361,
@@ -34,7 +34,7 @@ extern "C" {
 #define MCS_ERR_UNSUPPORTED  -2   /* option of the reference that is not built (AGAST) */
 #define MCS_ERR_CUDA         -3   /* CUDA runtime error; see mcs_last_error()          */
 #define MCS_ERR_CAPACITY     -4   /* caller buffer too small                           */
-#define MCS_ERR_NO_DEVICE    -5   /* no usable sm_100 device: there is NO CPU fallback */
+#define MCS_ERR_NO_DEVICE    -5   /* no usable sm_90 (H100) device: there is NO CPU fallback */
 
 #define MCS_MAX_LEVELS       16
 #define MCS_FRAME_GRID_COLS  64   /* ref include/cMultiFrame.h:48 */
@@ -92,7 +92,7 @@ typedef struct mcs_extractor_info {
 typedef struct mcs_extractor mcs_extractor;   /* opaque; one per (camera, thread), not re-entrant */
 
 const char* mcs_last_error(void);             /* thread-local message of the last failure */
-int  mcs_device_count(void);                  /* number of visible sm_100 devices (0 -> none) */
+int  mcs_device_count(void);                  /* number of visible sm_90 (H100) devices (0 -> none) */
 void mcs_params_default(mcs_extractor_params* p);
 
 /* ---- camera model (C1) ------------------------------------------------------------------- */

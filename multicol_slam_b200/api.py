@@ -7,7 +7,7 @@ operator/matcher interface for this path:
         SearchByBoW(KF1, KF2)   (ref include/cORBmatcher.h:58-158, src/cORBmatcher.cpp:46-166, 579-726, 885-966)
 
 There is no CPU fallback: the shared library must be present (build it with `python __graft_entry__.py`)
-and every compute call needs an sm_100 device, otherwise it raises.
+and every compute call needs an sm_90 (H100) device, otherwise it raises.
 """
 import ctypes as C
 import math

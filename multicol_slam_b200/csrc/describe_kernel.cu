@@ -96,8 +96,9 @@ constexpr int kLutDeg = 9;                        // degree of the per-centre po
 #define MCS_K3_V3 1                  // round-2 instruction diet (0 restores the previous forms for A/B builds): IC-angle disc read from a
 #endif                               // shared-memory copy, warp mean by one integer REDUX, tie / range test as running maxima
 #ifndef MCS_K3_MINB
-#define MCS_K3_MINB 5                // resident CTAs per SM the register budget is cut for: 5 -> 96 registers, no local-memory reload left in
-                                     // the hot loops (4.91 ms per 384 images); 6 -> 80 registers, 1 + 3 reloads per iteration (5.07 ms)
+#define MCS_K3_MINB 5                // resident CTAs per SM the register budget is cut for.  sm_90a, H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs,
+                                     // K3 ms per 384 images: 4 -> 126-128 registers, no spills: 5.49 / 5.90; 5 -> 96 registers,
+                                     // 80-144 B spilled: 5.39 / 5.51; 6 -> 80 registers: 5.81 / 5.85
 #endif
 #ifndef MCS_K3_U1
 #define MCS_K3_U1 4                  // unroll of tier-1 pass 1 (m-form), points per iteration   (A/B builds)
@@ -124,7 +125,8 @@ __host__ __device__ inline double t1m_centre(int i) { return (double)i * (double
 __host__ __device__ inline double t1m_halfwidth(int i) { return 2.0 * kLutReach * (double)i; }
 
 // Rare path: one pattern of one keypoint with the reference's exact operation sequence (two projection passes;
-// per-lane partial sums + butterfly: within ~1e-13 of the reference's sequential sum, see DESIGN.md).
+// per-lane partial sums + butterfly: within ~1e-13 of the reference's sequential sum; the tier-1 guard band below keeps every
+// pattern whose rounding that difference could change on this path, see DESIGN.md "K3 tiers").
 // Returns the descriptor byte(s) of this lane for that pattern, byte bb in bits [8bb, 8bb+8).
 template <int PPL>
 __device__ __noinline__ unsigned exact_pattern(const mcs_ocam* cam, const float2* s_pat, double angle, double ukx,
@@ -360,8 +362,8 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
     __shared__ WarpCtx s_ctx[kDescWarps];
     __shared__ __align__(8) float2 s_patf[PPL * 32];      // [j][lane] : point 16*byte + k with byte = lane + 32*(j/16), k = j%16, as floats
     // tier 1 parks the projected coordinates of the current pattern here between its two passes ([point][lane], this lane's own
-    // slots only): with rolled loops the kernel body stays inside the instruction cache -- the fully unrolled form stalled on
-    // instruction fetch for 5.6 of every 8.5 stalled warp-cycles (profiles/r2_k3_*.md)
+    // slots only): with rolled loops the kernel body stays inside the instruction cache -- the fully unrolled form spent most of
+    // its stalled cycles waiting on instruction fetch
     extern __shared__ __align__(8) float2 s_park_dyn[];          // [kDescWarps][PPL * 32], dynamic: 16 KB (descSize <= 32) / 32 KB
     __shared__ __align__(16) uint8_t s_patch[kDescWarps][(2 * kPatchR + 1) * kPatchS];
     const int ds = geom->desc_size;
@@ -371,7 +373,7 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
     __syncthreads();
 
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    // one warp per slot (a persistent grid-stride variant measured 4 % slower: static imbalance + 60 B more spills)
+    // one warp per slot (a persistent grid-stride variant was slower: static imbalance and more spills)
     const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int sel_total = geom->sel_total;
     const int b = warp_global / sel_total;
@@ -501,7 +503,7 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
     // Everything that is warp-uniform and only needed again in the rare paths or at the very end is parked in this warp's context in
     // shared memory instead of living in registers across the pattern loops: at 80 registers (6 CTAs per SM) the compiler otherwise
     // spills the INVARIANTS OF THE HOT LOOPS, and with 212 KB of the SM's 256 KB configured as shared memory those reloads miss the
-    // small L1 (measured: 3 local-memory loads for every global load, L1 hit rate 45 %, long-scoreboard the top stall reason).
+    // small L1, and the kernel then waits on local-memory loads.
     WarpCtx& cx = s_ctx[wib];
     const int ci = cam_of_image[b];
     const bool masks = geom->learn_masks != 0, dbrief = geom->do_dbrief != 0 || masks;
@@ -983,7 +985,8 @@ cudaError_t launch_describe(const PyramidGeom& G, const PyramidGeom* G_dev, int 
                             cudaStream_t st) {
     const long long warps = (long long)n_images * G.sel_total;
     const int blocks = (int)std::max<long long>(1, (warps + kDescWarps - 1) / kDescWarps);
-    // 96 registers, 5 CTAs of 4 warps per SM (MCS_K3_MINB): the budget at which no local-memory reload is left in the hot loops, see DESIGN.md
+    // 96 registers, 5 CTAs of 4 warps per SM (MCS_K3_MINB, measured against 4 and 6 there); the warp context in shared memory keeps
+    // the hot-loop invariants out of the spilled set
     const size_t park16 = (size_t)kDescWarps * 16 * 32 * sizeof(float2), park32 = 2 * park16;
     if (G.desc_size > 32) {        // static 23 KB + 32 KB parked coordinates: above the 48 KB default
         cudaError_t e = cudaFuncSetAttribute(describe_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)park32);

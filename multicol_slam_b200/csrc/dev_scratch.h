@@ -1,6 +1,6 @@
 // dev_scratch.h -- RAII device scratch for the stateless matcher / bag-of-words entry points.
-// Those calls are made once per frame with a handful of small buffers each; cudaMalloc + cudaFree cost ~0.1-0.2 ms per
-// buffer, more than the kernels they feed (profiles/r1_bow_kernels.md: 12 us of kernel in a 0.7 ms call).  Freed blocks
+// Those calls are made once per frame with a handful of small buffers each; a cudaMalloc + cudaFree pair per buffer costs
+// more than the microsecond-scale kernels those buffers feed.  Freed blocks
 // therefore go to a per-thread, per-device free list (best fit, at most 2x oversize, 1 GiB held at most) instead of back
 // to the driver.  Every entry point synchronises before it returns, so a block is idle when its Dev dies.
 #pragma once

@@ -1,4 +1,4 @@
-// extract_kernels.cu -- sm_100a kernels of the extractor half of the hot path.
+// extract_kernels.cu -- sm_90a kernels of the extractor half of the hot path.
 //
 //   (K1, fused pyramid + blur + FAST, lives in pyr_fast_kernel.cu)
 //   K2 octree_kernel     : DistributeOctTree, one CTA per (image, level)   (ref :569-861)

@@ -44,8 +44,8 @@ cudaError_t launch_hamming_stream(const uint8_t* desc, const uint8_t* dmask, con
 // (best <= th_low - 1).  A database entry at distance >= b can neither be an accepted best nor make a ratio test fail, so the
 // K-best kernels may leave it out of their lists (`bound` argument; 0xFFFFFFFF = keep everything) without changing any decision.
 // cudaMallocAsync scratch: by default the device pool hands freed memory back to the driver at the next synchronisation, which
-// turns every call's stream-ordered allocation into a real cudaMalloc (measured: 36 ms per mcs_match_stream_greedy_device call
-// instead of 7).  Keep freed blocks in the pool.
+// turns every call's stream-ordered allocation into a real cudaMalloc, which costs several times the kernels of a
+// mcs_match_stream_greedy_device call.  Keep freed blocks in the pool.
 inline cudaError_t keep_pool_memory() {
     static bool done[64] = {};
     int dev = 0;

@@ -1,4 +1,4 @@
-// match_kernels.cu -- sm_100a kernels of the matcher half of the hot path.
+// match_kernels.cu -- sm_90a kernels of the matcher half of the hot path.
 //
 //   M2 hamming_topk_kernel : all-pairs bit-level Hamming distance (ref src/cORBmatcher.cpp:2438-2474)
 //                            of nq queries against nd database descriptors, K best (distance, index)
@@ -20,7 +20,7 @@ constexpr int kTopkThreads = 128;
 
 
 // ---- bit-sliced population count (Harley-Seal carry-save adders) -------------------------------------------------
-// POPC issues on the XU pipe of sm_100 at 16 lanes/clk/SM (4x slower than LOP3), which makes a plain popcount loop
+// POPC issues at 16 lanes/clk/SM on sm_90 (4x slower than LOP3), which makes a plain popcount loop
 // the bottleneck of brute-force Hamming.  A carry-save adder (2 LOP3) turns three words into a "ones" and a "twos"
 // word; reducing 16 (8) words this way needs 9 (4) POPC instead of 16 (8).
 // (a ^ b) & c in one LOP3 (immLut = (0xF0 ^ 0xCC) & 0xAA); the compiler otherwise keeps the shared xor separate
@@ -41,9 +41,9 @@ __device__ __forceinline__ unsigned popc_sum8(const uint32_t (&w)[8]) {
     csa(c0, c1, c2, t0, d0);
     return __popc(s2) + __popc(w[7]) + 2 * __popc(t0) + 4 * __popc(d0);
 }
-// 16 words (masked distance): two carry-save levels on the ones, none on the twos -- 14 LOP3 + 9 POPC.  ALU (LOP3/IADD, 64 lanes/clk/SM)
-// and XU (POPC, 16 lanes/clk/SM) run concurrently, so the cheapest split loads both about equally; measured on the stream
-// matcher (381 x 2000 x 2000 masked pairs): full tree 22 LOP3 + 5 POPC 4.62 ms, one level 10 + 11 4.33 ms, this one 4.08 ms.
+// 16 words (masked distance): two carry-save levels on the ones, none on the twos -- 14 LOP3 + 9 POPC.  LOP3 (64 lanes/clk/SM)
+// and POPC (16 lanes/clk/SM) issue concurrently, so the cheapest split loads both about equally.  Greedy stream matcher,
+// H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs: this split 6.71 / 6.69 ms, MCS_M2_TREE=1 7.27 / 7.03 ms, =2 7.07 / 7.00 ms.
 #ifndef MCS_M2_TREE
 #define MCS_M2_TREE 0                // 0: 7 carry-save adders + 9 POPC, 1: 5 + 11, 2: 6 + 10 (A/B builds)
 #endif
@@ -106,8 +106,7 @@ __device__ __forceinline__ unsigned hamming_words(const uint32_t (&qw)[WORDS], c
 }
 
 // (Parking candidates in a per-thread shared-memory queue and inserting them with all lanes together -- the insertion below runs
-// with 1.4 active lanes on average and is 17 % of the warp instructions of the greedy stream matcher -- was measured: 6.24 ms
-// against 4.66 ms; the vote + queue traffic per pair costs more than the divergent insertions.)
+// with few active lanes -- was tried and was slower: the vote + queue traffic per pair costs more than the divergent insertions.)
 // Keys are 32 bits: distance << kTopkShift | database index (index < 2^21, distance <= 512), the list length KT is a compile-time
 // constant (4 or 8): see hamming_stream_kernel.
 constexpr int kTopkShift = 21;
@@ -207,7 +206,7 @@ cudaError_t launch_hamming_topk(const uint8_t* q, const uint8_t* qmask, int nq, 
     if (K < 1 || K > kTopKMax || (dim != 16 && dim != 32 && dim != 64) || nd >= (1 << kTopkShift)) return cudaErrorInvalidValue;
     if (nq <= 0) return cudaSuccess;
     const int qblocks = (nq + kTopkThreads - 1) / kTopkThreads;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     // enough CTAs for ~4 waves; database chunks are multiples of the tile
@@ -417,9 +416,9 @@ __device__ __forceinline__ void replay_scan(const uint32_t* __restrict__ qd, con
     }
 }
 
-// Queries served by one pass over the previous image.  3 (the pass also serving the next undecided queries of the chunk) was measured on
-// the Lafida stream: 2.33 ms against 2.14 ms with 1 -- a pass is not purely latency-bound (8 entries x 50 instructions per thread and
-// query), and the look-ahead results are often invalidated by the matches in between.  The code path stays (R is a template parameter).
+// Queries served by one pass over the previous image.  3 (the pass also serving the next undecided queries of the chunk) was slower
+// than 1 on the Lafida stream -- a pass is not purely latency-bound (8 entries x 50 instructions per thread and query), and the
+// look-ahead results are often invalidated by the matches in between.  The code path stays (R is a template parameter).
 constexpr int kRescanBatch = 1;
 // decision of one query from its K-best list under the current matched bits, evaluated by a single lane (look-ahead only)
 __device__ __forceinline__ int list_code(const int* li, const int* ld, const int K, const unsigned* s_taken, const int th_low, const double nnratio) {
@@ -703,13 +702,12 @@ stream_replay_kernel(const int* __restrict__ list_idx, const int* __restrict__ l
     if (tid == 0) { nmatches[img] = nm; redo[img] = 0; }
 }
 
-// The same walk with the previous image's descriptors (and masks) RESIDENT IN SHARED MEMORY: a rescan then costs ~1.5 us instead
-// of ~6 us (its 8 x 64 bytes per thread come from shared memory instead of L2), at the price of one CTA per SM (capacity x 2 x dim
+// The same walk with the previous image's descriptors (and masks) RESIDENT IN SHARED MEMORY: a rescan then reads its 8 x 64 bytes
+// per thread from shared memory instead of L2, a fraction of the latency, at the price of one CTA per SM (capacity x 2 x dim
 // bytes, 129 KB for 2016 slots of mdBRIEF-256).  Used when the launch holds no more images than the device has SMs -- a chunk of the
 // host-facing stream pipeline, whose last acceptance launch is the un-overlapped tail of the call; a full 384-image step keeps the
 // kernel above (2.6 CTAs per SM in flight hide each other's latency, and the extraction kernels of the next step share the SMs).
-// (256 threads as in the kernel above; 1024 -- more warps of its own for the CTA that is alone on its SM -- measured no better:
-// e2e 44.7 against 46.0 Mfeatures/s)
+// (256 threads as in the kernel above; 1024 -- more warps of its own for the CTA that is alone on its SM -- was no better)
 constexpr int kSmemReplayThreads = kReplayThreads;
 template <int WORDS, bool MASKED>
 __global__ void __launch_bounds__(kSmemReplayThreads, 1)

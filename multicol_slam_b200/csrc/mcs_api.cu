@@ -279,7 +279,7 @@ int ensure_batch(mcs_extractor* ex, int B) {
 
 // Small per-call host inputs (masks, camera models, distortion tables, status word).  They travel over the same
 // H2D copy engine as the image chunks of the stream call, so they must be enqueued BEFORE any large copy: a 1 MB
-// mask upload queued behind 100 MB of images stalls the compute stream for the whole transfer (measured: +5 ms).
+// mask upload queued behind 100 MB of images stalls the compute stream for the whole transfer.
 int upload_small_inputs(mcs_extractor* ex, int W, int H, const uint8_t* masks, const mcs_ocam* cams, int n_cams, cudaStream_t st) {
     CK(ex->masks.ensure((size_t)n_cams * W * H));
     CK(ex->cams.ensure(n_cams));
@@ -366,9 +366,8 @@ int enqueue_kernels(mcs_extractor* ex, int n_images, const uint8_t* images_dev, 
     }
     CK(cudaGetLastError());
     if (ex->profiling) CK(cudaEventRecord(ex->ev[1], st));
-    // (K2 forked per level onto a second stream behind K1 of the same level was measured for the per-frame path: the per-level
-    // launches serialise on that stream, 0.64 ms per 3-camera frame against 0.48 ms with the single launch whose 8 x n CTAs run
-    // side by side)
+    // (K2 forked per level onto a second stream behind K1 of the same level was slower for the per-frame path: the per-level
+    // launches serialise on that stream, while the single launch runs its 8 x n CTAs side by side)
     CK(launch_octree(G, ex->G_dev.p, n_images, ex->raw.p, ex->raw_count.p, ex->node_of.p, ex->sel_xys.p, ex->sel_count.p,
                      ex->status.p, st));
     CK(cudaGetLastError());
@@ -475,7 +474,7 @@ int mcs_device_count(void) {
     int ok = 0;
     for (int i = 0; i < n; ++i) {
         int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) ++ok;
+        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 9) ++ok;
     }
     return ok;
 }
@@ -520,7 +519,7 @@ int mcs_extractor_create(const mcs_extractor_params* p, mcs_extractor** out) {
         if (e != cudaSuccess) { cudaGetLastError(); return fail(MCS_ERR_NO_DEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e)); }
         int major = 0;
         cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-        if (major != 10) return fail(MCS_ERR_NO_DEVICE, "device is not sm_100 (B200); this library has no other code path");
+        if (major != 9) return fail(MCS_ERR_NO_DEVICE, "device is not sm_90 (H100); this library has no other code path");
     }
     int rc = upload_consts_once(dev);
     if (rc) return rc;
@@ -904,7 +903,9 @@ int mcs_match_stream_greedy_device(const uint8_t* desc_dev, const uint8_t* dmask
     if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535) return fail(MCS_ERR_INVALID, "bad sizes (capacity must be 1..65535)");
     if (dim != 16 && dim != 32 && dim != 64) return fail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
     cudaStream_t st = (cudaStream_t)stream;
-    constexpr int K = 4;      // measured on the Lafida stream: K = 8 saves 0.9 ms of rescans in the replay and costs 1.2 ms in the list kernel
+    // K-best list length (the acceptance is exact for any K; K only sets how often the replay rescans).  H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs:
+    // K = 8 16.08 / 16.15 ms per 384-image step (47.9 Mfeatures/s) against 16.85 / 16.79 ms with K = 4.
+    constexpr int K = 8;
     const size_t n = (size_t)n_frames * n_cams * capacity;
     int *li = nullptr, *ld = nullptr, *redo = nullptr;
     CK(keep_pool_memory());

@@ -1,4 +1,4 @@
-// mcs_common.cuh -- shared host/device definitions of the sm_100a feature pipeline.
+// mcs_common.cuh -- shared host/device definitions of the sm_90a feature pipeline.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -7,13 +7,13 @@
 // loads, the tile (+4 px ring, REFLECT_101 at the image border) is resized once and kept in three shared forms:
 // bytes (for the stores) and two 16-bit-per-pixel copies offset by one pixel, so that ANY horizontally adjacent
 // pixel pair is one aligned 32-bit word.  Blur and FAST then run on pixel PAIRS with the packed 16x2 integer
-// SIMD of sm_100a (VIADD.16x2, VIMNMX3.S16x2):
+// SIMD of sm_90a (16x2 adds, DPX three-way min / max):
 //   * box blur: 5 packed loads + 4 packed adds give the horizontal 5-sums of two pixels;
 //   * FAST: E_k = ring_k - centre (packed), 9-arc minima / maxima by two 3-input min (max) levels
 //     (M3_k = min3(E_k,E_k+1,E_k+2), M9_k = min3(M3_k,M3_k+3,M3_k+6)), branch-free exact cornerScore for every
 //     pixel pair: score = max over arcs of max(min9(E), -max9(E)) - 1, corner iff that maximum exceeds the threshold.
-// The kernel is bound by integer issue rate, not by HBM (see DESIGN.md): ~100 thread-instructions per pixel
-// against ~2.5 bytes of DRAM traffic.
+// The kernel is bound by integer issue rate, not by HBM (DESIGN.md, K1): on the order of a hundred thread-instructions per
+// pixel against a few bytes of DRAM traffic.
 #include <cstring>
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -315,8 +315,8 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
     if (!fast_on) return;                                   // uniform for the CTA: no corner can come out of this tile
     const uint8_t* m0p = mask0 + (size_t)cam_b * mask_bytes;
     // A warp owns one tile row per pass (32 pixel pairs), every lane evaluates its pair branch-free and the warp VOTES: two
-    // ballots give the number of surviving corners and each lane's slot in the warp's own list segment (the per-corner divergent
-    // append this replaces was 23 % of the kernel's instructions at 2.5 active lanes; a per-pass shared atomic still 6 %).  The
+    // ballots give the number of surviving corners and each lane's slot in the warp's own list segment (a per-corner divergent
+    // append runs with few active lanes, and a per-pass shared atomic still costs a visible share of the instructions).  The
     // level-0 mask is only consulted when the row segment holds a strict maximum at all.
     int wn = 0;                                             // corners this warp has collected (warp-uniform)
 #pragma unroll

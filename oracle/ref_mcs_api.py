@@ -3,6 +3,7 @@
 against the stand-in OpenCV header oracle/ref_mcs/stub.  TEST INFRASTRUCTURE: pins oracle/mcs_oracle.cpp's extractor
 restatement and generates tests/golden/ref_extract_*.npz (tests/golden/make_ref_extract_golden.py)."""
 import ctypes as C
+import os
 import pathlib
 import sys
 
@@ -13,6 +14,13 @@ sys.path.insert(0, str(_HERE.parent))
 from multicol_slam_b200.ctypes_defs import KEYPOINT_DTYPE, Ocam, make_ocam, make_params  # noqa: E402
 
 SO = _HERE / "_ref" / "libmcs_ref.so"
+# the reference checkout `make -C oracle ref` compiles from (same default as oracle/Makefile)
+REFERENCE_DIR = pathlib.Path(os.environ.get("MCS_REFERENCE_DIR", "/root/reference"))
+
+
+def reference_present():
+    """a readable reference checkout (os.path.isdir is False, not an error, where the path cannot be reached)"""
+    return os.path.isdir(REFERENCE_DIR / "include") and os.access(REFERENCE_DIR / "include", os.R_OK | os.X_OK)
 _lib = None
 
 

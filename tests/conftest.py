@@ -9,7 +9,7 @@ sys.path.insert(0, str(ROOT / "oracle"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (sm_100) device")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90) device")
 
 
 @pytest.fixture(scope="session")

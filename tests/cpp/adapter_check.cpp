@@ -101,7 +101,7 @@ template <class V> static bool same_ids(const V& a, const V& b) {
 }
 
 int main() {
-    if (mcs_device_count() < 1) { std::printf("adapter_check: no sm_100 device\n"); return 3; }
+    if (mcs_device_count() < 1) { std::printf("adapter_check: no sm_90 device\n"); return 3; }
     int fails = 0;
     for (int masks = 0; masks < 2; ++masks) {
         std::mt19937 rng(17 + masks);

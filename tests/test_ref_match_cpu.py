@@ -1,7 +1,7 @@
-"""CPU: the matcher restatements (oracle/mcs_oracle.cpp) pinned by the REFERENCE'S OWN matcher -- /root/reference/src/cORBmatcher.cpp
+"""CPU: the matcher restatements (oracle/mcs_oracle.cpp) pinned by the REFERENCE'S OWN matcher -- the reference's src/cORBmatcher.cpp
 compiled where it lies into oracle/_ref/libmcs_ref.so (oracle/ref_mcs/wrap_match.cpp; the three SLAM container classes it reads are
-data-only stand-ins, oracle/ref_mcs/stub_slam.h).  Skipped where the library is absent (it needs /root/reference to build; it
-travels prebuilt to the GPU box)."""
+data-only stand-ins, oracle/ref_mcs/stub_slam.h).  The library's results are stored in tests/golden/ref_tape_ref_match_cpu.*
+(oracle/ref_tape.py), recorded live where the library is built and replayed everywhere else."""
 import pathlib
 import sys
 
@@ -13,12 +13,13 @@ sys.path.insert(0, str(ROOT / "oracle"))
 SIZES = [(754, 480)] * 3
 
 
+TAPE_LIMIT = 1 << 20       # results stored whole: the tests compute on them
+
+
 @pytest.fixture(scope="module")
 def rm():
-    import ref_match_api
-    if not ref_match_api.available():
-        pytest.skip("oracle/_ref/libmcs_ref.so not built (needs /root/reference)")
-    return ref_match_api
+    import ref_tape
+    return ref_tape.module("ref_match_api", "ref_match_cpu", TAPE_LIMIT)
 
 
 @pytest.fixture(scope="module")
@@ -383,7 +384,8 @@ def test_window_search_triangulation_and_bow_frame_equal_reference(oa, rm, api, 
     k2 = rm.KF(F2, cams, M_c=sc["M_c"], M_t=M_t2, mp=np.where(free2, -1, 0).astype(np.int32), rays=rays2)
     rn, rpairs = rm.search_for_triangulation_raw(k1, k2, rm.MPTable(3, np.zeros((1, 32), np.uint8)), 0.6, masks)
     r1, r2 = api.Rig(cams, sc["M_c"], sc["M_t"]), api.Rig(cams, sc["M_c"], M_t2)
-    import ref_mcs_api as ra
+    import ref_tape
+    ra = ref_tape.module("ref_mcs_api", "ref_match_cpu", TAPE_LIMIT)
     E = np.zeros((3, 3, 3, 3))
     for i in range(3):
         for j in range(3):

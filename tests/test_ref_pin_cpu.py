@@ -1,33 +1,31 @@
 """CPU: the extractor restatement (oracle/mcs_oracle.cpp) pinned by outputs of the REFERENCE'S OWN code.
 
 1. against the committed fixtures tests/golden/ref_extract_*.npz, written by tests/golden/make_ref_extract_golden.py from
-   oracle/_ref/libmcs_ref.so (= /root/reference/src/mdBRIEFextractorOct.cpp, cam_model_omni.cpp, misc.cpp compiled in place);
-2. live against that library where it exists (build container and GPU box; it is git-ignored and travels prebuilt): more
-   seeds and parameter corners, DistributeOctTree alone on adversarial tie-heavy corner lists, the camera model, the
-   epipolar test of misc.cpp;
+   oracle/_ref/libmcs_ref.so (= the reference's src/mdBRIEFextractorOct.cpp, cam_model_omni.cpp, misc.cpp compiled in place);
+2. against that library's results stored in tests/golden/ref_tape_ref_pin_cpu.* (oracle/ref_tape.py; recorded live where the
+   library is built): more seeds and parameter corners, DistributeOctTree alone on adversarial tie-heavy corner lists, the
+   camera model, the epipolar test of misc.cpp;
 3. the stand-in OpenCV primitives underneath the reference build against the real cv2 (only where cv2 is importable).
 """
 import glob
 import json
 import pathlib
-import zlib
 
 import numpy as np
 import pytest
+from ref_tape import crc32, same
 
 GOLD = pathlib.Path(__file__).resolve().parent / "golden"
 FIXTURES = sorted(glob.glob(str(GOLD / "ref_extract_*.npz")))
 
 
 def crc(a):
-    return zlib.crc32(np.ascontiguousarray(a).tobytes())
+    return crc32(a)             # an array's CRC-32, or the one stored with a replayed reference result
 
 
 def _ra():
-    import ref_mcs_api as ra
-    if not ra.available():
-        pytest.skip("oracle/_ref/libmcs_ref.so not built (needs /root/reference)")
-    return ra
+    import ref_tape
+    return ref_tape.module("ref_mcs_api", "ref_pin_cpu", scalar_digests=True)
 
 
 def load_case(path):
@@ -44,7 +42,7 @@ def check_against_fixture(g, k, d, m):
     assert len(k) == int(g["n"])
     assert crc(k) == int(g["kps_crc"]) and crc(d) == int(g["desc_crc"]) and crc(m) == int(g["dmask_crc"])
     if "kps" in g.files:
-        assert k.tobytes() == g["kps"].tobytes() and np.array_equal(d, g["desc"]) and np.array_equal(m, g["dmask"])
+        assert same(k, g["kps"]) and same(d, g["desc"]) and same(m, g["dmask"])
 
 
 def test_fixture_set_is_complete():
@@ -68,7 +66,9 @@ def test_oracle_equals_reference_fixture(oa, path):
 
 @pytest.mark.parametrize("path", FIXTURES[::4], ids=lambda p: pathlib.Path(p).stem[12:])
 def test_reference_library_reproduces_fixture(path):
-    """the fixtures really are what oracle/_ref returns (guards against a stale or hand-edited fixture)"""
+    """the fixtures really are what oracle/_ref returns (guards against a stale or hand-edited fixture).  While the tape is recorded
+    this runs the reference library itself; on replay it is a consistency check of two committed files: the fixture against the
+    digest (incl. CRC-32) of the library's result stored in the tape."""
     ra = _ra()
     g, cam, kw, img, mask = load_case(path)
     check_against_fixture(g, *ra.RefExtractor(**kw).extract(img, mask, cam))
@@ -96,8 +96,8 @@ def test_oracle_equals_reference_live(oa, cams, seed):
     mask = synth.mirror_mask(cam)
     rk, rd, rm = ra.RefExtractor(**kw).extract(img, mask, cam)
     ok, od, om = oa.OracleExtractor(**kw).extract(img, mask, cam)
-    assert len(rk) == len(ok) and rk.tobytes() == ok.tobytes()
-    assert np.array_equal(rd, od) and np.array_equal(rm, om)
+    assert len(rk) == len(ok) and same(rk, ok)
+    assert same(rd, od) and same(rm, om)
 
 
 def test_constructor_tables_equal_reference(oa):
@@ -131,7 +131,7 @@ def test_octree_equals_reference_with_ties(oa, seed):
     N = int(rng.integers(10, 1500))
     r = ra.RefExtractor(nfeatures=1000).octree(xyr, 22, 22 + W, 22, 22 + H, N)
     o = oa.octree(xyr, 22, 22 + W, 22, 22 + H, N)
-    assert r.shape == o.shape and np.array_equal(r, o)
+    assert same(r, o)
 
 
 def test_camera_model_equals_reference(oa, cams, api):
@@ -144,8 +144,8 @@ def test_camera_model_equals_reference(oa, cams, api):
     rng = np.random.default_rng(3)
     for cam in list(cams) + [synth.scaled_cam(cams[1], 1920, 1080)]:
         oc = make_ocam(cam)
-        assert np.array_equal(ra.mirror_mask(cam), synth.mirror_mask(cam))
-        assert np.array_equal(ra.mirror_mask(cam), api.mirror_mask(cam))
+        assert same(ra.mirror_mask(cam), synth.mirror_mask(cam))
+        assert same(ra.mirror_mask(cam), api.mirror_mask(cam))
         for _ in range(200):
             X = rng.normal(size=3) * [1.0, 1.0, 0.6]
             u, v = C.c_double(), C.c_double()
@@ -162,7 +162,7 @@ def test_camera_model_equals_reference(oa, cams, api):
         inside = (ur < cam["width"]) & (ur > 0) & (vr < cam["height"]) & (vr > 0)
         exp = np.zeros(500, np.uint8)
         exp[inside] = m[vr[inside], ur[inside]] > 0
-        assert np.array_equal(ra.points_in_mask(cam, uv), exp)
+        assert same(ra.points_in_mask(cam, uv), exp)
 
 
 def test_epipolar_check_equals_reference(oa):
@@ -200,17 +200,17 @@ def test_stub_resize_and_border_vs_cv2(cams):
     src = synth.frame(cams[0], 7)
     for (w, h) in [(628, 400), (524, 333), (436, 278), (364, 231), (303, 193), (253, 161), (210, 134)]:
         ref = cv2.resize(src, (w, h), interpolation=cv2.INTER_LINEAR)
-        assert np.array_equal(ref, ra.cv_resize(src, w, h, 1))
+        assert same(ref, ra.cv_resize(src, w, h, 1))
         mk = (rng.integers(0, 2, size=src.shape) * 255).astype(np.uint8)
-        assert np.array_equal(cv2.resize(mk, (w, h), interpolation=cv2.INTER_NEAREST), ra.cv_resize(mk, w, h, 0))
+        assert same(cv2.resize(mk, (w, h), interpolation=cv2.INTER_NEAREST), ra.cv_resize(mk, w, h, 0))
         src = ref
     for (sw, sh, dw, dh) in [(101, 77, 84, 64), (1920, 1080, 1600, 900), (1280, 720, 1067, 600), (64, 64, 53, 53), (97, 31, 40, 13)]:
         s = rng.integers(0, 256, size=(sh, sw)).astype(np.uint8)
-        assert np.array_equal(cv2.resize(s, (dw, dh), interpolation=cv2.INTER_LINEAR), ra.cv_resize(s, dw, dh, 1))
-        assert np.array_equal(cv2.resize(s, (dw, dh), interpolation=cv2.INTER_NEAREST), ra.cv_resize(s, dw, dh, 0))
+        assert same(cv2.resize(s, (dw, dh), interpolation=cv2.INTER_LINEAR), ra.cv_resize(s, dw, dh, 1))
+        assert same(cv2.resize(s, (dw, dh), interpolation=cv2.INTER_NEAREST), ra.cv_resize(s, dw, dh, 0))
     s = rng.integers(0, 256, size=(40, 57)).astype(np.uint8)
-    assert np.array_equal(cv2.copyMakeBorder(s, 25, 25, 25, 25, cv2.BORDER_REFLECT_101), ra.cv_make_border(s, 25, True))
-    assert np.array_equal(cv2.copyMakeBorder(s, 25, 25, 25, 25, cv2.BORDER_CONSTANT, value=0), ra.cv_make_border(s, 25, False))
+    assert same(cv2.copyMakeBorder(s, 25, 25, 25, 25, cv2.BORDER_REFLECT_101), ra.cv_make_border(s, 25, True))
+    assert same(cv2.copyMakeBorder(s, 25, 25, 25, 25, cv2.BORDER_CONSTANT, value=0), ra.cv_make_border(s, 25, False))
 
 
 def test_stub_box_filter_vs_cv2(cams):
@@ -223,7 +223,7 @@ def test_stub_box_filter_vs_cv2(cams):
         mine = ra.cv_box5_roi(b, 25, 25, s.shape[1], s.shape[0])
         roi = b[25:-25, 25:-25]
         cv2.boxFilter(roi, -1, (5, 5), roi, (-1, -1), True, cv2.BORDER_REFLECT_101)
-        assert np.array_equal(b, mine)
+        assert same(b, mine)
         # a ROI whose surroundings are NOT its reflection: the C++ API filters a sub-matrix with the parent's pixels
         # (FilterEngine::apply with wholeSize / ofs).  cv2's Python binding cannot express this -- a numpy view arrives as a
         # stand-alone Mat -- so the expectation is the plain 5x5 sum over the parent, (S + 12) / 25 (SURVEY Appendix A.3)
@@ -232,10 +232,10 @@ def test_stub_box_filter_vs_cv2(cams):
         S = sum(big[7 + dy:37 + dy, 3 + dx:43 + dx].astype(np.int64) for dy in range(-2, 3) for dx in range(-2, 3))
         exp = big.copy()
         exp[7:37, 3:43] = (S + 12) // 25
-        assert np.array_equal(exp, mine)
+        assert same(exp, mine)
         # whole image: border extrapolation
         whole = ra.cv_box5_roi(s, 0, 0, s.shape[1], s.shape[0])
-        assert np.array_equal(cv2.boxFilter(s, -1, (5, 5), None, (-1, -1), True, cv2.BORDER_REFLECT_101), whole)
+        assert same(cv2.boxFilter(s, -1, (5, 5), None, (-1, -1), True, cv2.BORDER_REFLECT_101), whole)
 
 
 def test_stub_fast_and_atan2_vs_cv2(cams):
@@ -244,9 +244,9 @@ def test_stub_fast_and_atan2_vs_cv2(cams):
     rng = np.random.default_rng(4)
     for _ in range(3000):
         y, x = (np.float32(v) for v in rng.normal(size=2) * rng.choice([1, 1e3, 1e6]))
-        assert np.float32(ra.cv_fast_atan2(y, x)) == np.float32(cv2.fastAtan2(float(y), float(x)))
+        assert ra.cv_fast_atan2(y, x) == np.float32(cv2.fastAtan2(float(y), float(x)))     # the library returns a float
     for y, x in [(0, 0), (0, -5), (1, 1), (3, -4), (-7, 2), (5, 0), (-5, 0)]:
-        assert np.float32(ra.cv_fast_atan2(y, x)) == np.float32(cv2.fastAtan2(y, x))
+        assert ra.cv_fast_atan2(y, x) == np.float32(cv2.fastAtan2(y, x))
     img = synth.frame(cams[2], 5)
     mask = synth.mirror_mask(cams[2])
     for th in (5, 20, 40):
@@ -257,10 +257,10 @@ def test_stub_fast_and_atan2_vs_cv2(cams):
             cell, mcell = img[y0:y0 + h, x0:x0 + w], mask[y0:y0 + h, x0:x0 + w]
             kp = fd.detect(cell, mcell)
             exp = np.array([[k.pt[0], k.pt[1], k.response] for k in kp], np.float32).reshape(-1, 3)
-            assert np.array_equal(ra.cv_fast(cell, mcell, th), exp)
+            assert same(ra.cv_fast(cell, mcell, th), exp)
         kp = fd.detect(img, None)
         exp = np.array([[k.pt[0], k.pt[1], k.response] for k in kp], np.float32).reshape(-1, 3)
-        assert np.array_equal(ra.cv_fast(img, None, th), exp)
+        assert same(ra.cv_fast(img, None, th), exp)
     for v in rng.normal(size=500) * 100:
         assert ra.lib().mcsref_cv_round(float(v)) == cv2.cvRound(float(v)) if hasattr(cv2, "cvRound") else True
     for v in (0.5, 1.5, 2.5, -0.5, -1.5, 3.5):

@@ -1,6 +1,6 @@
 """GPU parity against outputs of the REFERENCE'S OWN extractor: the CUDA path (through the C ABI) vs the fixtures
 tests/golden/ref_extract_*.npz, which tests/golden/make_ref_extract_golden.py wrote from oracle/_ref/libmcs_ref.so
-(/root/reference/src/mdBRIEFextractorOct.cpp, cam_model_omni.cpp, misc.cpp compiled in place).  Bit-exact: keypoint
+(the reference's src/mdBRIEFextractorOct.cpp, cam_model_omni.cpp, misc.cpp compiled in place).  Bit-exact: keypoint
 bytes (incl. the IC angle float), descriptor and mask bytes, pyramid and mask-pyramid levels.  Covers the configuration the
 reference ships (plain ORB, 400 features), its init extractor, BASELINE.json configs 1-4 and parameter corners."""
 import glob
@@ -49,14 +49,14 @@ def test_gpu_equals_reference_fixture(api, path):
 
 
 def test_gpu_equals_reference_live(api, cams):
-    """where oracle/_ref travelled to this box: the reference library itself, on fresh seeds, next to the CUDA path"""
-    import ref_mcs_api as ra
-    if not ra.available():
-        pytest.skip("oracle/_ref/libmcs_ref.so not present")
+    """the reference library itself (live, or its results stored in tests/golden/ref_tape_ref_pin_gpu.*) on fresh seeds, next to
+    the CUDA path"""
+    import ref_tape
+    ra = ref_tape.module("ref_mcs_api", "ref_pin_gpu")
     from multicol_slam_b200 import synth
-    for seed, (mode, nf) in enumerate([(dict(), 400), (dict(do_dbrief=True), 900), (dict(do_dbrief=True, learn_masks=True), 2000)]):
-        cam = cams[seed]
-        img, mask = synth.frame(cam, 900 + seed), synth.mirror_mask(cam)
-        rk, rd, rm = ra.RefExtractor(nfeatures=nf, **mode).extract(img, mask, cam)
+    cases = [(dict(), 400), (dict(do_dbrief=True), 900), (dict(do_dbrief=True, learn_masks=True), 2000)]
+    inputs = [(cams[seed], synth.frame(cams[seed], 900 + seed), synth.mirror_mask(cams[seed])) for seed in range(len(cases))]
+    ref = [ra.RefExtractor(nfeatures=nf, **mode).extract(img, mask, cam) for (mode, nf), (cam, img, mask) in zip(cases, inputs)]
+    for (mode, nf), (cam, img, mask), (rk, rd, rm) in zip(cases, inputs, ref):
         k, d, m = api.mdBRIEFextractorOct(nfeatures=nf, do_dBrief=mode.get("do_dbrief", False), learnMasks=mode.get("learn_masks", False))(img, mask, cam)
-        assert k.tobytes() == rk.tobytes() and np.array_equal(d, rd) and np.array_equal(m, rm)
+        assert ref_tape.same(k, rk) and ref_tape.same(d, rd) and ref_tape.same(m, rm)

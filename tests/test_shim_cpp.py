@@ -5,6 +5,7 @@ import subprocess
 
 import numpy as np
 import pytest
+import ref_mcs_api          # oracle/, on sys.path through tests/conftest.py (and build())
 
 ROOT = pathlib.Path(__file__).resolve().parents[1]
 EXE = ROOT / "tests" / "cpp" / "shim_smoke"
@@ -36,7 +37,7 @@ int use(MultiColSLAM::mdBRIEFextractorOct& ex, const MultiColSLAM::cCamModelGene
                            "-I" + str(ROOT / "include"), str(src)])
 
 
-REF = pathlib.Path("/root/reference")
+REF = ref_mcs_api.REFERENCE_DIR
 ADAPT = ROOT / "tests" / "cpp" / "adapter_check"
 
 
@@ -53,8 +54,8 @@ def build_adapter_check():
 
 
 def test_adapters_compile_against_reference_containers(api):
-    if not (REF.exists() and (ROOT / "oracle" / "_ref" / "obj" / "cORBmatcher.o").exists()):
-        pytest.skip("needs /root/reference and `make -C oracle ref`")
+    if not (ref_mcs_api.reference_present() and (ROOT / "oracle" / "_ref" / "obj" / "cORBmatcher.o").exists()):
+        pytest.skip("needs a reference checkout (MCS_REFERENCE_DIR) and `make -C oracle ref`")
     build_adapter_check()
     assert ADAPT.exists()
 
@@ -62,9 +63,9 @@ def test_adapters_compile_against_reference_containers(api):
 @pytest.mark.gpu
 def test_adapters_equal_reference_matcher():
     """C++ drop-in check: the reference's cORBmatcher::SearchByProjection / SearchForInitialization / SearchByBoW(KF,KF) and the
-    adapters over the C ABI leave the same reference-shaped containers in the same state (binary built where /root/reference exists)"""
+    adapters over the C ABI leave the same reference-shaped containers in the same state (binary built where the reference checkout is readable)"""
     if not ADAPT.exists():
-        pytest.skip("tests/cpp/adapter_check was not built (needs /root/reference)")
+        pytest.skip("tests/cpp/adapter_check was not built (needs a reference checkout, MCS_REFERENCE_DIR)")
     out = subprocess.run([str(ADAPT)], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0 and "adapter_check passed" in out.stdout, out.stdout + out.stderr
     assert out.stdout.count(" ok") == 6

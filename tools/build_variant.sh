@@ -5,7 +5,7 @@ NAME=$1; EXTRA=$2
 SRC=$(cd "$(dirname "$0")/../multicol_slam_b200/csrc" && pwd)
 OUT=/tmp/mcs_build_$NAME; mkdir -p $OUT
 NVCC=/usr/local/cuda/bin/nvcc
-ARCH="-gencode arch=compute_100a,code=sm_100a"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
 FLAGS="$ARCH $EXTRA -O3 -lineinfo -std=c++17 -fmad=false -Xcompiler -fPIC,-ffp-contract=off -Xptxas -v -I$SRC"
 pids=()
 for f in pyr_fast_kernel extract_kernels describe_kernel match_kernels bow_kernels mcs_api mcs_match_api mcs_bow_api mcs_comm; do

@@ -1,4 +1,4 @@
-# round-end evidence on one B200: ncu --set full of one bench step AT THE BENCH BATCH (128 frames x 3 cameras), launch list, the
+# profiling evidence on one GPU (the H100 the library targets): ncu --set full of one bench step AT THE BENCH BATCH (128 frames x 3 cameras), launch list, the
 # default bench run of every config and the reference arm.  Reports come back in gpurun_out/, summaries are made from them with
 # tools/profile_summary.py / ncu_lines.py / ncu_phases.py / make_k1_traffic.py and committed under profiles/.
 #   tools/final_capture.sh r3            config 2 in full + bench lines of configs 3 and 4

@@ -1,4 +1,4 @@
-// Repro + workarounds for a ptxas 12.9 (-O1 and above, sm_100a) miscompile found while writing the FAST
+// Repro + workarounds for a ptxas 12.9 (-O1 and above) miscompile, seen when targeting sm_100a, while writing the FAST
 // score: max(a, max(b, -c)) is folded into VIMNMX3 and the negation is lost.  Variants 1-3 are correct; the
 // original scalar form (removed) was wrong on the device and right on the host / with -Xptxas -O0.
 #include <cstdio>
