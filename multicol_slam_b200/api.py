@@ -11,7 +11,6 @@ and every compute call needs an sm_90 (H100) device, otherwise it raises.
 """
 import ctypes as C
 import math
-import os
 import pathlib
 
 import numpy as np
@@ -20,8 +19,7 @@ from .ctypes_defs import (ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DT
                           WINDOW_QUERY_DTYPE, make_ocam, make_params)
 
 _PKG = pathlib.Path(__file__).resolve().parent
-# MCS_B200_LIB: load another build of the same C ABI (kernel-variant experiments under tools/); never a CPU library
-_LIB_PATH = pathlib.Path(os.environ.get("MCS_B200_LIB", _PKG / "libmcs_b200.so"))
+_LIB_PATH = _PKG / "libmcs_b200.so"
 _lib = None
 
 MCS_OK, MCS_ERR_INVALID, MCS_ERR_UNSUPPORTED, MCS_ERR_CUDA, MCS_ERR_CAPACITY, MCS_ERR_NO_DEVICE = 0, -1, -2, -3, -4, -5

@@ -86,27 +86,12 @@ constexpr int kDescWarps = 4;
 constexpr int kPatchR = 25;                       // staged patch: rows/cols ky/kx -25 .. +25 (keypoints are >= 25 px inside the ROI)
 constexpr int kPatchS = 64;                       // bytes per staged patch row (4-byte aligned start + 51 columns)
 constexpr int kLutDeg = 9;                        // degree of the per-centre polynomial of R(r)  (kernels.h: DistortLut)
-#ifndef MCS_K3_T1
-#define MCS_K3_T1 1                  // 0: tier 1 off (A/B builds: everything goes through tier 2)
-#endif
-#ifndef MCS_K3_REPAIR
-#define MCS_K3_REPAIR 1              // 0: flagged tier-1 patterns go straight to tier 2 (A/B builds)
-#endif
-#ifndef MCS_K3_V3
-#define MCS_K3_V3 1                  // round-2 instruction diet (0 restores the previous forms for A/B builds): IC-angle disc read from a
-#endif                               // shared-memory copy, warp mean by one integer REDUX, tie / range test as running maxima
-#ifndef MCS_K3_MINB
-#define MCS_K3_MINB 5                // resident CTAs per SM the register budget is cut for.  sm_90a, H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs,
-                                     // K3 ms per 384 images: 4 -> 126-128 registers, no spills: 5.49 / 5.90; 5 -> 96 registers,
-                                     // 80-144 B spilled: 5.39 / 5.51; 6 -> 80 registers: 5.81 / 5.85
-#endif
-#ifndef MCS_K3_U1
-#define MCS_K3_U1 4                  // unroll of tier-1 pass 1 (m-form), points per iteration   (A/B builds)
-#endif
-#ifndef MCS_K3_U2
-#define MCS_K3_U2 2                  // unroll of tier-1 pass 2, point PAIRS per iteration        (A/B builds)
-#endif
-constexpr int kT1Unroll1 = MCS_K3_U1, kT1Unroll2 = MCS_K3_U2;
+// resident CTAs per SM the register budget is cut for.  sm_90a, H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs,
+// K3 ms per 384 images: 4 -> 126-128 registers, no spills: 5.49 / 5.90; 5 -> 96 registers, 80-144 B spilled: 5.39 / 5.51;
+// 6 -> 80 registers: 5.81 / 5.85
+constexpr int kDescMinBlocks = 5;
+constexpr int kT1Unroll1 = 4;                     // unroll of tier-1 pass 1 (m-form), points per iteration
+constexpr int kT1Unroll2 = 2;                     // unroll of tier-1 pass 2, point PAIRS per iteration
 constexpr int kT1Coef = 6;                        // tier 1: q(s') of degree 5, R(i + s) - R(i) = s' q(s'), s' = s / kT1Scale
 constexpr float kT1Scale = 32.f;
 constexpr double kT1MinRadius = 40.0;             // tier 1 needs r >= r_k - 21.3 well away from the pole of g at r = 0
@@ -114,11 +99,9 @@ constexpr float kT1Guard = 2.5e-5f;               // px; 5x the worst tier-1 err
 // doubles per centre: [0] tau offset, [1] tau scale, [2..11] kLutDeg + 1 coefficients (tier 2);
 // [12] R(i), [13] q0 (double), [14..16] q1..q5 as floats (+ one pad float), [17] 1.0 when the tier-1 entry is usable
 constexpr double kLutReach = 22.5;                // half-width of a centre's interval: pattern radius 15*sqrt(2) + 0.5 + margin
-// [18] G(c_i) (double), [19..22] a0..a7 of the m-form as floats, [23] 1.0 when the m-form entry is usable  (MCS_K3_MFORM)
+// [18] G(c_i) (double), [19..22] a0..a7 of the m-form as floats, [23] 1.0 when the m-form entry is usable
+// (tier 1 works in the variable m = r^2 where the centre's table allows it, otherwise in s)
 constexpr int kLutStride = 24;
-#ifndef MCS_K3_MFORM
-#define MCS_K3_MFORM 1               // tier 1 in the variable m = r^2 where the centre's table allows it (0: always the s-form; A/B builds)
-#endif
 constexpr int kT1MCoef = 8;                       // m-form: g(r) - G(c_i) = t P(t), P of degree 7, t = (r^2 - c_i) / hw_i
 // centre and half-width of centre i's window in m = r^2: r in [i - reach, i + reach]  (i >= reach, checked where the entry is built)
 __host__ __device__ inline double t1m_centre(int i) { return (double)i * (double)i + kLutReach * kLutReach; }
@@ -351,8 +334,8 @@ struct __align__(16) WarpCtx {
     uint32_t c;
     float angle;
 };
-template <int PPL /* pattern points per lane: 16 for descSize <= 32, 32 for descSize 64 */, int MINB = MCS_K3_MINB>
-__global__ void __launch_bounds__(kDescWarps * 32, MINB)
+template <int PPL /* pattern points per lane: 16 for descSize <= 32, 32 for descSize 64 */>
+__global__ void __launch_bounds__(kDescWarps * 32, kDescMinBlocks)
 describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, const mcs_ocam* __restrict__ cams,
                 const DistortLut* __restrict__ luts, const int* __restrict__ cam_of_image,
                 const uint32_t* __restrict__ sel_xys, const int* __restrict__ sel_count,
@@ -428,7 +411,6 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
 
     // ---- IC_Angle (ref :221-248): integer moments over the 845-pixel disc, lane = column u = lane-16 (+ u = 16) ----
     int m10 = 0, m01 = 0;
-#if MCS_K3_V3
     {
         // The 33 x 33 neighbourhood of the UNBLURRED level is copied with aligned word loads (3 rows x 10 words per warp
         // instruction) into this warp's slice of the parking buffer, which tier 1 only uses later; the moments are then summed from
@@ -472,32 +454,6 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
         }
         __syncwarp();                                       // the parking buffer is free again
     }
-#else
-    {
-        const uint8_t* ctr = uimg + (size_t)ky * pitch + kx;
-        const int u = lane - kHalfPatch;                    // -16 .. 15
-        const int au = u < 0 ? -u : u;
-        // |v| <= vmax(u): the disc is symmetric (umax table, ref :187-202); vmax(|u|) = umax[|u|]
-        const int vm = c_disc_u[au];                        // c_disc_u[0..16] doubles as umax[] (see upload_constants)
-#pragma unroll 11
-        for (int v = -kHalfPatch; v <= kHalfPatch; ++v) {
-            const int val = (v >= -vm && v <= vm) ? (int)ctr[v * pitch + u] : 0;
-            m10 += u * val;
-            m01 += v * val;
-        }
-        if (lane < 2 * c_disc_u[kHalfPatch] + 1) {          // column u = +16: rows |v| <= umax[16]
-            const int v = lane - c_disc_u[kHalfPatch];
-            const int val = ctr[v * pitch + kHalfPatch];
-            m10 += kHalfPatch * val;
-            m01 += v * val;
-        }
-#pragma unroll
-        for (int o = 16; o; o >>= 1) {
-            m10 += __shfl_xor_sync(0xffffffffu, m10, o);
-            m01 += __shfl_xor_sync(0xffffffffu, m01, o);
-        }
-    }
-#endif
     const float angle = fast_atan2_deg((float)m01, (float)m10);
 
     // Everything that is warp-uniform and only needed again in the rare paths or at the very end is parked in this warp's context in
@@ -585,8 +541,8 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
             const double* row = lut.coef + (size_t)ci_lut * kLutStride;
             if (lane == 0) { cx.ukx = ukx; cx.uky = uky; cx.row = row; }
             // ---- tier-1 set-up (per keypoint, all lanes redundantly; ~25 FP64 instructions against 48 points x 3 patterns) ----
-            t1 = MCS_K3_T1 && have_lut && rk >= kT1MinRadius && __ldg(row + 17) == 1.0;
-            mform = MCS_K3_MFORM && t1 && __ldg(row + 23) == 1.0;
+            t1 = have_lut && rk >= kT1MinRadius && __ldg(row + 17) == 1.0;
+            mform = t1 && __ldg(row + 23) == 1.0;
             if (mform) {
                 // m-form: t_k, K0 = t_k P(t_k), g_k = G(c_i) + K0 in double from the float coefficients the points will use
                 const float2 c01 = __ldg((const float2*)(row + 19)), c23 = __ldg((const float2*)(row + 20));
@@ -692,26 +648,15 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
                 }
                 // mean over the 16*ds points: lane partial sums in fp32 (16..32 terms)
                 const double inv_n = 1.0 / (double)(16 * ds);
-                bool flag = false;
-#if MCS_K3_V3
                 // ... and the warp sum as ONE integer REDUX per coordinate in 2^-17 px fixed point: a lane's rounding is <= 3.8e-6 px,
                 // the mean is off by <= 32 * 3.8e-6 / 512 = 2.4e-7 px (inside the tier-1 error budget, kT1Guard).  A lane sum of 500 px
                 // or more (or a NaN) cannot come from a sane pattern (|du| <= ~22 px) and sends the pattern on, so the 32-bit sum
                 // (< 32 * 500 * 2^17 = 2^31) never wraps.
-                flag = !(fabsf(su) < 500.f) | !(fabsf(sv) < 500.f);
+                bool flag = !(fabsf(su) < 500.f) | !(fabsf(sv) < 500.f);
                 const int iu = __reduce_add_sync(0xffffffffu, flag ? 0 : __float2int_rn(su * 131072.f));
                 const int iv = __reduce_add_sync(0xffffffffu, flag ? 0 : __float2int_rn(sv * 131072.f));
                 const float mu = (float)((double)iu * (inv_n * (1.0 / 131072.0))), mv = (float)((double)iv * (inv_n * (1.0 / 131072.0)));
                 float wf = 0.f, wt = 0.f;                                      // running maxima of |fraction - tie| and |offset|
-#else
-                double sud = (double)su, svd = (double)sv;
-#pragma unroll
-                for (int o = 16; o; o >>= 1) {
-                    sud += __shfl_xor_sync(0xffffffffu, sud, o);
-                    svd += __shfl_xor_sync(0xffffffffu, svd, o);
-                }
-                const float mu = (float)(sud * inv_n), mv = (float)(svd * inv_n);
-#endif
                 constexpr float kMagicF = 12582912.f;                          // 1.5 * 2^23: t + magic rounds t to the nearest even integer
                 unsigned bits = 0;                                             // descriptor byte(s) of this lane: points 0..15 | 16..31 << 8
 #pragma unroll kT1Unroll2
@@ -723,16 +668,10 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
                         const float tu = c.x - mu, tv = c.y - mv;
                         const float mu_r = tu + kMagicF, mv_r = tv + kMagicF;
                         const float fu = tu - (mu_r - kMagicF), fv = tv - (mv_r - kMagicF);
-                        // near a rounding tie, or outside the staged patch
-#if MCS_K3_V3
-                        // (running maxima, tested once after the loop; a NaN coordinate has already flagged the pattern through its lane sum)
+                        // near a rounding tie, or outside the staged patch: running maxima, tested once after the loop (a NaN
+                        // coordinate has already flagged the pattern through its lane sum)
                         wf = fmaxf(wf, fmaxf(fabsf(fu), fabsf(fv)));
                         wt = fmaxf(wt, fmaxf(fabsf(tu), fabsf(tv)));
-#else
-                        // (the comparisons are written so that a NaN flags too)
-                        flag |= !(fabsf(fu) < 0.5f - kT1Guard) | !(fabsf(fv) < 0.5f - kT1Guard) | !(fabsf(tu) < (float)kPatchR + 0.4f) |
-                                !(fabsf(tv) < (float)kPatchR + 0.4f);
-#endif
                         const int ix = __float_as_int(mu_r) - 0x4B400000, iy = __float_as_int(mv_r) - 0x4B400000;
                         // one clamp of the byte offset keeps the read inside the patch array; an offset that needed it belongs to a
                         // flagged coordinate (|t| >= 25.4) and the pattern is redone
@@ -741,14 +680,12 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
                     }
                     bits |= (unsigned)(smp[0] < smp[1]) << (j >> 1);          // point pair j/2: bits 0..7 = byte 0, 8..15 = byte 1
                 }
-#if MCS_K3_V3
                 flag |= !(wf < 0.5f - kT1Guard) | !(wt < (float)kPatchR + 0.4f);
-#endif
                 if (!__any_sync(0xffffffffu, flag && lane_valid)) {
                     put(qi, bits);
                     done = true;
                     if (args.tier_stats && lane == 0) atomicAdd(args.tier_stats, 1ull);
-                } else if (MCS_K3_REPAIR) {
+                } else {
                     int fail = 0;
                     const unsigned e = tier1_repair<PPL>(&cam, s_patf, park, cx.row, cx.ca[qi], cx.sa[qi], cx.ukx, cx.uky, lane, ds, patch, pofs, &fail);
                     if (!__any_sync(0xffffffffu, fail != 0)) {
@@ -985,7 +922,7 @@ cudaError_t launch_describe(const PyramidGeom& G, const PyramidGeom* G_dev, int 
                             cudaStream_t st) {
     const long long warps = (long long)n_images * G.sel_total;
     const int blocks = (int)std::max<long long>(1, (warps + kDescWarps - 1) / kDescWarps);
-    // 96 registers, 5 CTAs of 4 warps per SM (MCS_K3_MINB, measured against 4 and 6 there); the warp context in shared memory keeps
+    // 96 registers, 5 CTAs of 4 warps per SM (kDescMinBlocks, measured against 4 and 6 there); the warp context in shared memory keeps
     // the hot-loop invariants out of the spilled set
     const size_t park16 = (size_t)kDescWarps * 16 * 32 * sizeof(float2), park32 = 2 * park16;
     if (G.desc_size > 32) {        // static 23 KB + 32 KB parked coordinates: above the 48 KB default

@@ -43,10 +43,8 @@ __device__ __forceinline__ unsigned popc_sum8(const uint32_t (&w)[8]) {
 }
 // 16 words (masked distance): two carry-save levels on the ones, none on the twos -- 14 LOP3 + 9 POPC.  LOP3 (64 lanes/clk/SM)
 // and POPC (16 lanes/clk/SM) issue concurrently, so the cheapest split loads both about equally.  Greedy stream matcher,
-// H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs: this split 6.71 / 6.69 ms, MCS_M2_TREE=1 7.27 / 7.03 ms, =2 7.07 / 7.00 ms.
-#ifndef MCS_M2_TREE
-#define MCS_M2_TREE 0                // 0: 7 carry-save adders + 9 POPC, 1: 5 + 11, 2: 6 + 10 (A/B builds)
-#endif
+// H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs: this split (7 carry-save adders + 9 POPC) 6.71 / 6.69 ms,
+// 5 + 11: 7.27 / 7.03 ms, 6 + 10: 7.07 / 7.00 ms.
 __device__ __forceinline__ void popc_sum16(const uint32_t (&w)[16], unsigned& ones_out, unsigned& twos_out) {
     uint32_t s0, c0, s1, c1, s2, c2, s3, c3, s4, c4;
     csa(w[0], w[1], w[2], s0, c0);
@@ -54,21 +52,11 @@ __device__ __forceinline__ void popc_sum16(const uint32_t (&w)[16], unsigned& on
     csa(w[6], w[7], w[8], s2, c2);
     csa(w[9], w[10], w[11], s3, c3);
     csa(w[12], w[13], w[14], s4, c4);
-#if MCS_M2_TREE == 1
-    const unsigned ones = __popc(s0) + __popc(s1) + __popc(s2) + __popc(s3) + __popc(s4) + __popc(w[15]);
-    const unsigned twos = __popc(c0) + __popc(c1) + __popc(c2) + __popc(c3) + __popc(c4);
-#elif MCS_M2_TREE == 2
-    uint32_t a0, b0;
-    csa(s0, s1, s2, a0, b0);
-    const unsigned ones = __popc(a0) + __popc(s3) + __popc(s4) + __popc(w[15]);
-    const unsigned twos = __popc(c0) + __popc(c1) + __popc(c2) + __popc(c3) + __popc(c4) + __popc(b0);
-#else
     uint32_t a0, b0, a1, b1;
     csa(s0, s1, s2, a0, b0);
     csa(s3, s4, w[15], a1, b1);
     const unsigned ones = __popc(a0) + __popc(a1);
     const unsigned twos = __popc(c0) + __popc(c1) + __popc(c2) + __popc(c3) + __popc(c4) + __popc(b0) + __popc(b1);
-#endif
     ones_out += ones; twos_out += twos;
 }
 // sum over k of popc(x_k) [unmasked] or (popc(x_k & qm_k) + popc(x_k & dm_k)) / 2 [masked: the integer division of ref :2472
@@ -354,38 +342,30 @@ cudaError_t launch_hamming_stream(const uint8_t* desc, const uint8_t* dmask, con
 //   none is: rejected if dK >= th_low.
 // Otherwise the warp rescans the whole previous image for this one query (exact best / second among the unmatched entries), so
 // the result never depends on K; redo[] stays 0 and is kept for interface stability.
-#ifndef MCS_REPLAY_THREADS
-#define MCS_REPLAY_THREADS 256
-#endif
-constexpr int kReplayThreads = MCS_REPLAY_THREADS;   // stream matcher: <= 65535 database entries per image, many images in flight
+constexpr int kReplayThreads = 256;         // stream matcher: <= 65535 database entries per image, many images in flight
 constexpr int kBfReplayThreads = 1024;       // key-frame database: one CTA per query set scans up to ~1.5 M entries per rescan
 constexpr int kKeyShift = 21;                // rescan keys = distance << 21 | index (index < 2^21, distance <= 512)
 
 template <int THREADS>
 __device__ __forceinline__ void named_bar(int id) { asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(THREADS) : "memory"); }
 
-// One pass over this thread's share of the unmatched database entries for up to R queries at once (rows[0..n)): per query the two
-// smallest (distance << kKeyShift | index) keys.  The database words are loaded once per entry whatever n is; a rescan is bound
-// by the latency of those loads, so the extra queries ride along almost for free.
-template <int WORDS, bool MASKED, int THREADS, int R>
-__device__ __forceinline__ void replay_scan(const uint32_t* __restrict__ qd, const uint32_t* __restrict__ qmk, const int* rows, const int n,
+// One pass over this thread's share of the unmatched database entries for query row `row`: the two smallest
+// (distance << kKeyShift | index) keys of the warp.
+template <int WORDS, bool MASKED, int THREADS>
+__device__ __forceinline__ void replay_scan(const uint32_t* __restrict__ qd, const uint32_t* __restrict__ qmk, const int row,
                                             const uint32_t* __restrict__ dd, const uint32_t* __restrict__ dm, const int id_lo,
                                             const int id_hi, const unsigned* s_taken /* bit (id - id_lo) */, const int tid,
-                                            unsigned (&k1)[R], unsigned (&k2)[R]) {
-    uint32_t qw[R][WORDS], qm[R][MASKED ? WORDS : 1];
+                                            unsigned& k1, unsigned& k2) {
+    uint32_t qw[WORDS], qm[MASKED ? WORDS : 1];
+    const uint4* qp = reinterpret_cast<const uint4*>(qd + (size_t)row * WORDS);
 #pragma unroll
-    for (int r = 0; r < R; ++r) {
-        const int row = rows[r < n ? r : 0];
-        const uint4* qp = reinterpret_cast<const uint4*>(qd + (size_t)row * WORDS);
+    for (int k = 0; k < WORDS / 4; ++k) { const uint4 t = qp[k]; qw[4 * k] = t.x; qw[4 * k + 1] = t.y; qw[4 * k + 2] = t.z; qw[4 * k + 3] = t.w; }
+    if (MASKED) {
+        const uint4* qmp = reinterpret_cast<const uint4*>(qmk + (size_t)row * WORDS);
 #pragma unroll
-        for (int k = 0; k < WORDS / 4; ++k) { const uint4 t = qp[k]; qw[r][4 * k] = t.x; qw[r][4 * k + 1] = t.y; qw[r][4 * k + 2] = t.z; qw[r][4 * k + 3] = t.w; }
-        if (MASKED) {
-            const uint4* qmp = reinterpret_cast<const uint4*>(qmk + (size_t)row * WORDS);
-#pragma unroll
-            for (int k = 0; k < WORDS / 4; ++k) { const uint4 t = qmp[k]; qm[r][4 * k] = t.x; qm[r][4 * k + 1] = t.y; qm[r][4 * k + 2] = t.z; qm[r][4 * k + 3] = t.w; }
-        }
-        k1[r] = 0xFFFFFFFFu; k2[r] = 0xFFFFFFFFu;
+        for (int k = 0; k < WORDS / 4; ++k) { const uint4 t = qmp[k]; qm[4 * k] = t.x; qm[4 * k + 1] = t.y; qm[4 * k + 2] = t.z; qm[4 * k + 3] = t.w; }
     }
+    k1 = 0xFFFFFFFFu; k2 = 0xFFFFFFFFu;
 #pragma unroll 2
     for (int id = id_lo + tid; id < id_hi; id += THREADS) {
         if (s_taken[(id - id_lo) >> 5] >> ((id - id_lo) & 31) & 1u) continue;
@@ -397,52 +377,24 @@ __device__ __forceinline__ void replay_scan(const uint32_t* __restrict__ qd, con
             const uint4 t = dp[k]; dw[4 * k] = t.x; dw[4 * k + 1] = t.y; dw[4 * k + 2] = t.z; dw[4 * k + 3] = t.w;
             if (MASKED) { const uint4 u = mp[k]; mw[4 * k] = u.x; mw[4 * k + 1] = u.y; mw[4 * k + 2] = u.z; mw[4 * k + 3] = u.w; }
         }
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            if (r >= n) break;
-            // the list kernels' distance (carry-save popcount: 9 POPC instead of 16 per masked 256-bit pair -- a rescan is bound by the
-            // POPC rate of the SM as soon as the descriptors come from shared memory)
-            const unsigned dist = hamming_words<WORDS, MASKED>(qw[r], qm[r], dw, mw);
-            const unsigned key = (dist << kKeyShift) | (unsigned)id;
-            if (key < k1[r]) { k2[r] = k1[r]; k1[r] = key; } else if (key < k2[r]) k2[r] = key;
-        }
+        // the list kernels' distance (carry-save popcount: 9 POPC instead of 16 per masked 256-bit pair -- a rescan is bound by the
+        // POPC rate of the SM as soon as the descriptors come from shared memory)
+        const unsigned dist = hamming_words<WORDS, MASKED>(qw, qm, dw, mw);
+        const unsigned key = (dist << kKeyShift) | (unsigned)id;
+        if (key < k1) { k2 = k1; k1 = key; } else if (key < k2) k2 = key;
     }
-    // warp: smallest and second smallest of the 64 keys per query (keys are unique: the index is part of the key)
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-        const unsigned B = __reduce_min_sync(0xffffffffu, k1[r]);
-        const unsigned S = __reduce_min_sync(0xffffffffu, k1[r] == B ? k2[r] : k1[r]);
-        k1[r] = B; k2[r] = S;
-    }
+    // warp: smallest and second smallest of the 64 keys (keys are unique: the index is part of the key)
+    const unsigned B = __reduce_min_sync(0xffffffffu, k1);
+    const unsigned S = __reduce_min_sync(0xffffffffu, k1 == B ? k2 : k1);
+    k1 = B; k2 = S;
 }
 
-// Queries served by one pass over the previous image.  3 (the pass also serving the next undecided queries of the chunk) was slower
-// than 1 on the Lafida stream -- a pass is not purely latency-bound (8 entries x 50 instructions per thread and query), and the
-// look-ahead results are often invalidated by the matches in between.  The code path stays (R is a template parameter).
-constexpr int kRescanBatch = 1;
-// decision of one query from its K-best list under the current matched bits, evaluated by a single lane (look-ahead only)
-__device__ __forceinline__ int list_code(const int* li, const int* ld, const int K, const unsigned* s_taken, const int th_low, const double nnratio) {
-    int best1 = 0x7FFFFFFF, best2 = 0x7FFFFFFF, found = 0, dK = 0x7FFFFFFF;
-    bool complete = false;
-    for (int k = 0; k < K; ++k) {
-        const int id = li[k];
-        if (id < 0) { complete = true; break; }
-        dK = ld[k];
-        if (s_taken[id >> 5] >> (id & 31) & 1u) continue;
-        if (found == 0) best1 = ld[k]; else best2 = ld[k];
-        if (++found == 2) break;
-    }
-    if (found == 2 || complete) return (best1 < th_low && (double)best1 < nnratio * (double)best2) ? 1 : 0;
-    if (found == 1) return !(best1 < th_low) ? 0 : ((double)best1 < nnratio * (double)dK ? 1 : 2);
-    return !(dK < th_low) ? 0 : 2;
-}
-
+// A pass serves one query.  Letting it also serve the next undecided queries of the chunk (look-ahead) was slower on the Lafida
+// stream, and the look-ahead results are often invalidated by the matches in between.
 struct ReplayShared {
-    int cmd;                                  // queries in the published batch (>= 1), -1 = the walk is over
-    int bq[kRescanBatch];                     // their rows
-    unsigned k1[32][kRescanBatch], k2[32][kRescanBatch];      // per warp: two smallest keys per batch query
-    int pq[kRescanBatch];                     // look-ahead results of the last batch: query row (-1 = none), best, second
-    unsigned pB[kRescanBatch], pS[kRescanBatch];
+    int cmd;                                  // 0 while the walk runs, -1 once it is over (helper CTAs: the rescan sequence)
+    int bq;                                   // the rescan's query row
+    unsigned k1[32], k2[32];                  // per warp: the two smallest keys
 };
 
 // Several CTAs per query set (key-frame database): the leader CTA walks the queries; for a rescan it publishes the query in global
@@ -463,10 +415,7 @@ struct CoopLeader { CoopSeg* seg; int* log; int helpers; int shard_hi; };   // h
 // "already matched" bits live in s_taken.  Warp 0 walks the queries in order (lane 0 decides from the list); the other warps
 // sleep on a named barrier and wake only for a rescan, where all THREADS threads split the database.  Every thread of the CTA
 // must call this; returns the number of matches in warp 0 (other warps: 0).
-// R > 1: a rescan pass also serves the next queries of the current 32-query chunk that cannot be decided from their lists right
-// now (look-ahead).  Such a result stays exact as long as neither its best nor its second entry has been matched in between (the
-// minimum and second minimum of a set do not change when OTHER elements leave it); that is checked when the walk gets there.
-template <int WORDS, bool MASKED, int THREADS, int R>
+template <int WORDS, bool MASKED, int THREADS>
 __device__ __forceinline__ int replay_core(const int* __restrict__ list_idx, const int* __restrict__ list_dist, const int K, const int nq,
                                            const uint8_t* __restrict__ valid1, const uint32_t* __restrict__ qd,
                                            const uint32_t* __restrict__ qmk, const uint32_t* __restrict__ dd,
@@ -486,18 +435,14 @@ __device__ __forceinline__ int replay_core(const int* __restrict__ list_idx, con
             named_bar<THREADS>(1);
             const int cmd = *(volatile int*)&sh->cmd;
             if (cmd < 0) return 0;
-            unsigned k1[R], k2[R];
-            replay_scan<WORDS, MASKED, THREADS, R>(s_qd, s_qm, sh->bq, cmd, dd, dmk, 0, scan_hi, s_taken, tid, k1, k2);
-            if (lane == 0) {
-#pragma unroll
-                for (int r = 0; r < R; ++r) { sh->k1[warp][r] = k1[r]; sh->k2[warp][r] = k2[r]; }
-            }
+            unsigned k1, k2;
+            replay_scan<WORDS, MASKED, THREADS>(s_qd, s_qm, sh->bq, dd, dmk, 0, scan_hi, s_taken, tid, k1, k2);
+            if (lane == 0) { sh->k1[warp] = k1; sh->k2[warp] = k2; }
             named_bar<THREADS>(2);
         }
     }
     int nm = 0;
-    if (lane < kRescanBatch) sh->pq[lane] = -1;
-    __syncwarp();
+    if (lane == 0) sh->cmd = 0;
     for (int q0 = 0; q0 < nq; q0 += 32) {
         const int nchunk = min(32, nq - q0);
         for (int i = lane; i < nchunk * K; i += 32) {
@@ -537,71 +482,35 @@ __device__ __forceinline__ int replay_core(const int* __restrict__ list_idx, con
                 else code = !(dK < th_low) ? 0 : 2;
             }
             if (code == 2) {
-                unsigned B = 0xFFFFFFFFu, S = 0xFFFFFFFFu;
-                bool have = false;
-                if (R > 1) {                                // a look-ahead result of an earlier pass, still exact?
-#pragma unroll
-                    for (int r = 1; r < R; ++r)
-                        if (sh->pq[r] == q0 + t) {
-                            const unsigned pb = sh->pB[r], ps = sh->pS[r];
-                            const unsigned bi = pb & ((1u << kKeyShift) - 1u), si = ps & ((1u << kKeyShift) - 1u);
-                            const bool gone = (pb != 0xFFFFFFFFu && (s_taken[bi >> 5] >> (bi & 31) & 1u)) ||
-                                              (ps != 0xFFFFFFFFu && (s_taken[si >> 5] >> (si & 31) & 1u));
-                            if (!gone) { B = pb; S = ps; have = true; }
-                        }
+                // exact rescan of the database: two smallest (distance, index) keys among the unmatched entries
+                if (lane == 0) {
+                    sh->bq = t;                            // chunk-relative row (see s_qd)
+                    if (coop.helpers) {                     // publish the rescan to the helper CTAs before scanning shard 0 here
+                        coop.seg->cmd_query = q0 + t;
+                        coop.seg->log_len = nlog;
+                        __threadfence();
+                        atomicExch(&coop.seg->cmd_seq, ++seq);
+                    }
                 }
-                if (!have) {
-                    // exact rescan of the database: two smallest (distance, index) keys among the unmatched entries, for this query
-                    // and (R > 1) for the next queries of the chunk that are undecided under the current matched bits
-                    int n = 1;
-                    unsigned cand = 0u;
-                    if (R > 1) {
-                        int c = 0;
-                        if (lane > t && lane < nchunk && !(valid1 && !valid1[q0 + lane]))
-                            c = list_code(s_li + lane * K, s_ld + lane * K, K, s_taken, th_low, nnratio);
-                        cand = __ballot_sync(0xffffffffu, c == 2);
-                        n += min(__popc(cand), R - 1);
-                    }
+                named_bar<THREADS>(1);
+                unsigned k1, k2;
+                replay_scan<WORDS, MASKED, THREADS>(s_qd, s_qm, t, dd, dmk, 0, scan_hi, s_taken, tid, k1, k2);
+                if (lane == 0) { sh->k1[0] = k1; sh->k2[0] = k2; }
+                named_bar<THREADS>(2);
+                const unsigned w1 = lane < THREADS / 32 ? sh->k1[lane] : 0xFFFFFFFFu;
+                const unsigned w2 = lane < THREADS / 32 ? sh->k2[lane] : 0xFFFFFFFFu;
+                unsigned B = __reduce_min_sync(0xffffffffu, w1);
+                unsigned S = __reduce_min_sync(0xffffffffu, w1 == B ? w2 : w1);
+                if (coop.helpers) {                         // fold the helpers' partial minima (lanes 0..helpers-1), own shard in lane 31
                     if (lane == 0) {
-                        sh->cmd = n;
-                        sh->bq[0] = t;                     // chunk-relative rows (see s_qd)
-                        unsigned cm = cand;
-                        for (int r = 1; r < n; ++r) { sh->bq[r] = __ffs(cm) - 1; cm &= cm - 1u; }
-                        if (coop.helpers) {                 // publish the rescan to the helper CTAs before scanning shard 0 here (R == 1)
-                            coop.seg->cmd_query = q0 + t;
-                            coop.seg->log_len = nlog;
-                            __threadfence();
-                            atomicExch(&coop.seg->cmd_seq, ++seq);
-                        }
+                        while (*(volatile int*)&coop.seg->done < seq * coop.helpers) {}
+                        __threadfence();
                     }
-                    named_bar<THREADS>(1);
-                    unsigned k1[R], k2[R];
-                    replay_scan<WORDS, MASKED, THREADS, R>(s_qd, s_qm, sh->bq, n, dd, dmk, 0, scan_hi, s_taken, tid, k1, k2);
-                    if (lane == 0) {
-#pragma unroll
-                        for (int r = 0; r < R; ++r) { sh->k1[0][r] = k1[r]; sh->k2[0][r] = k2[r]; }
-                    }
-                    named_bar<THREADS>(2);
-#pragma unroll
-                    for (int r = 0; r < R; ++r) {
-                        const unsigned a1 = lane < THREADS / 32 ? sh->k1[lane][r] : 0xFFFFFFFFu;
-                        const unsigned a2 = lane < THREADS / 32 ? sh->k2[lane][r] : 0xFFFFFFFFu;
-                        const unsigned Br = __reduce_min_sync(0xffffffffu, a1);
-                        const unsigned Sr = __reduce_min_sync(0xffffffffu, a1 == Br ? a2 : a1);
-                        if (r == 0) { B = Br; S = Sr; }
-                        else if (lane == 0) { sh->pq[r] = r < n ? q0 + sh->bq[r] : -1; sh->pB[r] = Br; sh->pS[r] = Sr; }
-                    }
-                    if (coop.helpers) {                     // fold the helpers' partial minima (lanes 0..helpers-1), own shard in lane 31
-                        if (lane == 0) {
-                            while (*(volatile int*)&coop.seg->done < seq * coop.helpers) {}
-                            __threadfence();
-                        }
-                        __syncwarp();
-                        const unsigned a1 = lane < coop.helpers ? *(volatile unsigned*)&coop.seg->partial[2 * lane] : (lane == 31 ? B : 0xFFFFFFFFu);
-                        const unsigned a2 = lane < coop.helpers ? *(volatile unsigned*)&coop.seg->partial[2 * lane + 1] : (lane == 31 ? S : 0xFFFFFFFFu);
-                        B = __reduce_min_sync(0xffffffffu, a1);
-                        S = __reduce_min_sync(0xffffffffu, a1 == B ? a2 : a1);
-                    }
+                    __syncwarp();
+                    const unsigned a1 = lane < coop.helpers ? *(volatile unsigned*)&coop.seg->partial[2 * lane] : (lane == 31 ? B : 0xFFFFFFFFu);
+                    const unsigned a2 = lane < coop.helpers ? *(volatile unsigned*)&coop.seg->partial[2 * lane + 1] : (lane == 31 ? S : 0xFFFFFFFFu);
+                    B = __reduce_min_sync(0xffffffffu, a1);
+                    S = __reduce_min_sync(0xffffffffu, a1 == B ? a2 : a1);
                 }
                 const int best1 = B == 0xFFFFFFFFu ? 0x7FFFFFFF : (int)(B >> kKeyShift), best2 = S == 0xFFFFFFFFu ? 0x7FFFFFFF : (int)(S >> kKeyShift);
                 bestIdx = (int)(B & ((1u << kKeyShift) - 1u));
@@ -652,15 +561,13 @@ __device__ __forceinline__ void replay_helper(CoopSeg* cs, const int* log, const
         }
         applied = len;
         __syncthreads();
-        unsigned k1[1], k2[1];
-        if (tid == 0) sh->bq[0] = q;
-        __syncthreads();
-        replay_scan<WORDS, MASKED, THREADS, 1>(qd, qmk, sh->bq, 1, dd, dmk, lo, hi, s_taken, tid, k1, k2);
-        if (lane == 0) { sh->k1[warp][0] = k1[0]; sh->k2[warp][0] = k2[0]; }
+        unsigned k1, k2;
+        replay_scan<WORDS, MASKED, THREADS>(qd, qmk, q, dd, dmk, lo, hi, s_taken, tid, k1, k2);
+        if (lane == 0) { sh->k1[warp] = k1; sh->k2[warp] = k2; }
         __syncthreads();
         if (warp == 0) {
-            const unsigned a1 = lane < THREADS / 32 ? sh->k1[lane][0] : 0xFFFFFFFFu;
-            const unsigned a2 = lane < THREADS / 32 ? sh->k2[lane][0] : 0xFFFFFFFFu;
+            const unsigned a1 = lane < THREADS / 32 ? sh->k1[lane] : 0xFFFFFFFFu;
+            const unsigned a2 = lane < THREADS / 32 ? sh->k2[lane] : 0xFFFFFFFFu;
             const unsigned B = __reduce_min_sync(0xffffffffu, a1);
             const unsigned S = __reduce_min_sync(0xffffffffu, a1 == B ? a2 : a1);
             if (lane == 0) {
@@ -695,7 +602,7 @@ stream_replay_kernel(const int* __restrict__ list_idx, const int* __restrict__ l
     for (int i = tid; i < (capacity + 31) / 32; i += kReplayThreads) s_taken[i] = 0u;
     for (int i = tid; i < capacity; i += kReplayThreads) matches12[q_row0 + i] = -1;
     __syncthreads();
-    const int nm = replay_core<WORDS, MASKED, kReplayThreads, kRescanBatch>(list_idx + q_row0 * K, list_dist + q_row0 * K, K, nq, nullptr, desc + q_row0 * WORDS,
+    const int nm = replay_core<WORDS, MASKED, kReplayThreads>(list_idx + q_row0 * K, list_dist + q_row0 * K, K, nq, nullptr, desc + q_row0 * WORDS,
                                                               MASKED ? dmask + q_row0 * WORDS : nullptr, desc + d_row0 * WORDS,
                                                               MASKED ? dmask + d_row0 * WORDS : nullptr, nd, th_low, nnratio,
                                                               matches12 + q_row0, s_li, s_ld, s_taken, &sh, s_qc);
@@ -739,7 +646,7 @@ stream_replay_smem_kernel(const int* __restrict__ list_idx, const int* __restric
         }
     }
     __syncthreads();
-    const int nm = replay_core<WORDS, MASKED, kSmemReplayThreads, kRescanBatch>(list_idx + q_row0 * K, list_dist + q_row0 * K, K, nq, nullptr, desc + q_row0 * WORDS,
+    const int nm = replay_core<WORDS, MASKED, kSmemReplayThreads>(list_idx + q_row0 * K, list_dist + q_row0 * K, K, nq, nullptr, desc + q_row0 * WORDS,
                                                               MASKED ? dmask + q_row0 * WORDS : nullptr, s_db, MASKED ? s_dbm : nullptr, nd, th_low,
                                                               nnratio, matches12 + q_row0, s_li, s_ld, s_taken, &sh, s_qc);
     if (tid == 0) { nmatches[img] = nm; redo[img] = 0; }
@@ -818,7 +725,7 @@ bruteforce_replay_kernel(const int* __restrict__ list_idx, const int* __restrict
         return;
     }
     const CoopLeader cl{helpers ? coop_seg + s : nullptr, helpers ? coop_log + q0 : nullptr, helpers, helpers ? hi : nd};
-    const int nm = replay_core<WORDS, MASKED, kBfReplayThreads, 1>(list_idx + (size_t)q0 * K, list_dist + (size_t)q0 * K, K, nq, valid1 ? valid1 + q0 : nullptr,
+    const int nm = replay_core<WORDS, MASKED, kBfReplayThreads>(list_idx + (size_t)q0 * K, list_dist + (size_t)q0 * K, K, nq, valid1 ? valid1 + q0 : nullptr,
                                                                 q + (size_t)q0 * WORDS, MASKED ? qm + (size_t)q0 * WORDS : nullptr, d, dm, nd, th_low,
                                                                 nnratio, matches12 + q0, s_li, s_ld, s_taken, &sh, s_qc, cl);
     if (tid == 0) nmatches[s] = nm;

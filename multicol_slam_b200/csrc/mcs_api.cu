@@ -967,18 +967,6 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
         const int nc = std::min(std::max(n_frames / 8, 1), 4), each = (n_frames + nc - 1) / nc;
         for (int c = 0; c <= nc; ++c) chunk_lo.push_back(std::min(c * each, n_frames));
     }
-#ifdef MCS_DEBUG_KNOBS                                                  // experiment knobs exist only in -DMCS_DEBUG_KNOBS builds
-    if (const char* plan = getenv("MCS_STREAM_CHUNKS")) {               // comma-separated frames per chunk
-        std::vector<int> lo(1, 0);
-        for (const char* q = plan; *q && lo.back() < n_frames;) {
-            lo.push_back(std::min(n_frames, lo.back() + std::max(1, atoi(q))));
-            while (*q && *q != ',') ++q;
-            if (*q == ',') ++q;
-        }
-        if (lo.back() < n_frames) lo.push_back(n_frames);
-        chunk_lo = lo;
-    }
-#endif
     const int n_chunks = (int)chunk_lo.size() - 1;
     int fpc = 0;
     for (int c = 0; c < n_chunks; ++c) fpc = std::max(fpc, chunk_lo[c + 1] - chunk_lo[c]);
@@ -1018,18 +1006,13 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
             return e;
         }
     } events;
-    std::vector<cudaEvent_t> ev_in(n_chunks), ev_free(n_chunks), ev_feat(n_chunks), ev_done(n_chunks), tev;
+    std::vector<cudaEvent_t> ev_in(n_chunks), ev_free(n_chunks), ev_feat(n_chunks), ev_done(n_chunks);
     for (int c = 0; c < n_chunks; ++c) {
         CK(events.add(&ev_in[c], cudaEventDisableTiming));
         CK(events.add(&ev_free[c], cudaEventDisableTiming));
         CK(events.add(&ev_feat[c], cudaEventDisableTiming));
         CK(events.add(&ev_done[c], cudaEventDisableTiming));
     }
-#ifdef MCS_DEBUG_KNOBS
-    static const bool trace = getenv("MCS_TRACE_STREAM") != nullptr;    // per-chunk timeline on stderr
-#else
-    constexpr bool trace = false;
-#endif
     // Everything asynchronous happens inside enqueue(); whatever it returns, the three streams are drained before this
     // function returns, because the copies read caller memory and the local cam-of-image table.
     auto enqueue = [&]() -> int {
@@ -1040,27 +1023,21 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
     CK(ex->coi_all.ensure(n_images));
     CK(cudaMemcpyAsync(ex->coi_all.p, coi.data(), sizeof(int) * n_images, cudaMemcpyHostToDevice, st));
     const uint8_t* dmask_for_match = ex->p.learn_masks ? dmask_d : nullptr;
-    // MCS_TRACE_STREAM=1: per-chunk timeline on stderr (H2D begin/end, compute begin/features/end, D2H end), ms from the first H2D
-    auto mark = [&](cudaStream_t s_) { if (trace) { cudaEvent_t e; if (events.add(&e, cudaEventDefault) == cudaSuccess) { cudaEventRecord(e, s_); tev.push_back(e); } } };
     for (int c = 0; c < n_chunks && rc == MCS_OK; ++c) {
         const int img_lo = chunk_lo[c] * n_cams, nimg = (chunk_lo[c + 1] - chunk_lo[c]) * n_cams;
         if (nimg <= 0) continue;
         uint8_t* tight = ex->in_tight.p + (size_t)(c & 1) * tight_img * ipc;
         if (c >= 2) CK(cudaStreamWaitEvent(ex->s_copy, ev_free[c - 2], 0));          // staging buffer consumed
-        mark(ex->s_copy);
         CK(cudaMemcpyAsync(tight, images + (size_t)img_lo * tight_img, tight_img * nimg - (c == n_chunks - 1 ? (size_t)(stride - width) : 0),
                            cudaMemcpyHostToDevice, ex->s_copy));
-        mark(ex->s_copy);
         CK(cudaEventRecord(ev_in[c], ex->s_copy));
         CK(cudaStreamWaitEvent(st, ev_in[c], 0));
-        mark(st);
         launch_repitch(tight, stride, ex->in_images.p, dpitch, width, (size_t)height * nimg, st);
         CK(cudaEventRecord(ev_free[c], st));
         rc = run_pipeline(ex, nimg, ex->in_images.p, width, height, dpitch, masks, cams, n_cams, coi.data() + img_lo,
                           kps_d + (size_t)img_lo * capacity, desc_d + (size_t)img_lo * capacity * ds,
                           dmask_d + (size_t)img_lo * capacity * ds, counts_d + img_lo, capacity, st, false, ex->coi_all.p + img_lo);
         if (rc) break;
-        mark(st);
         CK(cudaEventRecord(ev_feat[c], st));                              // features of the chunk are final: their D2H overlaps the matching
         // the matching of chunk c runs on its own stream, so that K1..K3 of chunk c+1 (on `st`) fill the SMs behind its tail;
         // it reads descriptors of this chunk and of the last frame of the previous one, both final at ev_feat[c]
@@ -1071,7 +1048,6 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
         if (replay)     // greedy acceptance of SearchByBoW(KF1, KF2) over the lists of this chunk, still on the device
             CK(launch_stream_replay(ex->match_idx.p, ex->match_dist.p, counts_d, desc_d, dmask_for_match, ds, img_lo, nimg, n_cams, capacity, K,
                                     th_low, nnratio, ex->m12.p, ex->nmat.p, ex->redo.p, ex->s_match));
-        mark(ex->s_match);
         CK(cudaEventRecord(ev_done[c], ex->s_match));
         cudaStream_t so = ex->s_out;
         CK(cudaStreamWaitEvent(so, ev_feat[c], 0));
@@ -1094,21 +1070,12 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
             CK(cudaMemcpyAsync(nmatches_out + img_lo, ex->nmat.p + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
             CK(cudaMemcpyAsync(redo_out + img_lo, ex->redo.p + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
         }
-        mark(so);
     }
     return rc;
     };
     const int rc = enqueue();
     cudaError_t e1 = cudaStreamSynchronize(ex->s_copy), e2 = cudaStreamSynchronize(st), e3 = cudaStreamSynchronize(ex->s_out);
     { const cudaError_t e4 = cudaStreamSynchronize(ex->s_match); if (e2 == cudaSuccess) e2 = e4; }
-    if (trace && !tev.empty()) {
-        for (size_t i = 0; i + 5 < tev.size(); i += 6) {
-            float t[6];
-            for (int k = 0; k < 6 && i + k < tev.size(); ++k) cudaEventElapsedTime(&t[k], tev[0], tev[i + k]);
-            fprintf(stderr, "[mcs stream] chunk %zu: h2d %.2f-%.2f  compute %.2f  features %.2f  matched %.2f  d2h done %.2f ms\n", i / 6,
-                    t[0], t[1], t[2], t[3], t[4], t[5]);
-        }
-    }
     if (rc) return rc;
     CK(e1); CK(e2); CK(e3);
     ex->last_n_images = (chunk_lo[n_chunks] - chunk_lo[n_chunks - 1]) * n_cams;

@@ -51,12 +51,7 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, i
                  ::"r"(smem_u32(dst)), "l"((unsigned long long)map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
 }
 
-#ifndef MCS_K1_MINB
-#define MCS_K1_MINB 6                        // resident CTAs per SM the register budget is cut for (6 needs <= 40 registers)
-#endif
-#ifndef MCS_K1_TMA
-#define MCS_K1_TMA 1                         // 0: stage the source region with __ldg + st.shared (A/B builds)
-#endif
+constexpr int kMinBlocks = 6;               // resident CTAs per SM the register budget is cut for (6 needs <= 40 registers)
 constexpr int kThreads = 256;
 constexpr int kSrcWB = 176;                 // staged source row stride (bytes, multiple of 16)
 constexpr int kT8S = 80;                    // byte tile row stride
@@ -94,7 +89,7 @@ __device__ __forceinline__ unsigned fast_margin2(unsigned C, const unsigned (&E)
     return __vmaxs2(__vsub2(bright, C), __vsub2(C, darkn)); // values in 0..255: no 16-bit overflow
 }
 
-__global__ void __launch_bounds__(kThreads, MCS_K1_MINB)
+__global__ void __launch_bounds__(kThreads, kMinBlocks)
 pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
                 const LevelGeom g, const int level, const int nlevels, const int fast_th, const int src_aligned,
                 const uint8_t* __restrict__ src, const size_t src_img_bytes,
@@ -387,11 +382,11 @@ void launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_
     dim3 grid(g.tiles_x, g.tiles_y, n_images);
     const int aligned = (((uintptr_t)src & 15) == 0 && (g.spitch & 15) == 0 && (src_img_bytes & 15) == 0) ? 1 : 0;
     // tensor map of the source: (row bytes, rows, images), box = the level's staged region.  Encoding is a host-side table fill
-    // (no driver round trip), done per launch because the base address and the batch size are per call.
+    // (no driver round trip), done per launch because the base address and the batch size are per call.  Sources with an
+    // unaligned base or stride, and boxes larger than the staging buffer, are staged with __ldg instead (use_tma = 0).
     CUtensorMap map;
     std::memset(&map, 0, sizeof(map));
     int use_tma = 0;
-#if MCS_K1_TMA
     static PFN_cuTensorMapEncodeTiled_v12000 encode = [] {
         void* fn = nullptr;
         cudaDriverEntryPointQueryResult qr;
@@ -406,7 +401,6 @@ void launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_
         use_tma = encode(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)src, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
     }
-#endif
     pyr_fast_kernel<<<grid, kThreads, 0, st>>>(map, use_tma, g, level, G.nlevels, G.fast_threshold, aligned, src, src_img_bytes, dst, dst_blur,
                                                mask0, mask_w, mask_bytes, cam_of_image, tile_flags, G.tiles_total, raw, G.raw_total,
                                                raw_count);

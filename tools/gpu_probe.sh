@@ -1,7 +1,6 @@
-# one GPU visit: smoke, stage times (+ A/B builds given as arguments), all GPU tests, the bench at every config, ncu captures
+# one GPU visit: smoke, stage times, all GPU tests, the bench at every config, ncu captures
 timeout 90 python -c "import __graft_entry__ as g; g.smoke()" 2>&1 | tail -1 || { echo "SMOKE FAILED OR HUNG"; exit 1; }
-echo "== default"; timeout 200 python tools/stage_probe.py 128 stats 2>&1 | grep -E "images:|tiers"; timeout 100 python tools/stage_probe.py 1 2>&1 | grep -E "images:"
-for v in "$@"; do echo "== $v"; MCS_B200_LIB=$PWD/multicol_slam_b200/libmcs_b200_$v.so timeout 200 python tools/stage_probe.py 128 2>&1 | grep -E "images:"; done
+timeout 200 python tools/stage_probe.py 128 stats 2>&1 | grep -E "images:|tiers"; timeout 100 python tools/stage_probe.py 1 2>&1 | grep -E "images:"
 timeout 900 python -m pytest tests -m gpu -q > gpurun_out/gpu_tests.log 2>&1; tail -4 gpurun_out/gpu_tests.log
 for CFG in 2 3 4; do
 timeout 400 python bench.py --steps 6 --warmup 3 --no-cpu-baseline --config $CFG > gpurun_out/bench_c$CFG.json 2> gpurun_out/bench_c$CFG.err

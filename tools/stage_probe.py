@@ -1,5 +1,5 @@
-"""stage_probe.py -- K1/K2/K3 stage times of one extractor batch (CUDA events inside the library), for A/B builds selected with
-MCS_B200_LIB.   python tools/stage_probe.py [frames] [tier_stats]"""
+"""stage_probe.py -- K1/K2/K3 stage times of one extractor batch (CUDA events inside the library).
+python tools/stage_probe.py [frames] [tier_stats]"""
 import pathlib
 import sys
 
