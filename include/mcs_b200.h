@@ -266,7 +266,9 @@ int  mcs_hamming_topk_device(const uint8_t* q_dev, const uint8_t* qmask_dev, int
 /* cORBmatcher::SearchByBoW(KF1, KF2, matches12) semantics (ref :885-966): all-pairs scan,
  * best/second best, `best < th_low`, `best < nnratio*second`, every KF2 entry used at most once,
  * queries visited in index order.  valid1/valid2: 1 where the keypoint carries a good map point
- * (NULL = all valid).  matches12[nq] = matched database index or -1.  Returns via *nmatches. */
+ * (NULL = all valid).  matches12[nq] = matched database index or -1.  Returns via *nmatches.
+ * nd <= 1 622 016 per call for this entry point and the two below (the acceptance kernel keeps one "used" bit per database
+ * entry in shared memory); a larger database returns MCS_ERR_UNSUPPORTED without launching a kernel. */
 int  mcs_match_bruteforce(const uint8_t* q, const uint8_t* qmask, const uint8_t* valid1, int32_t nq,
                           const uint8_t* d, const uint8_t* dmask, const uint8_t* valid2, int32_t nd,
                           int32_t dim, int32_t th_low, double nnratio,

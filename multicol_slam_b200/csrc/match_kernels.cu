@@ -736,8 +736,8 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
                                      int th_low, double nnratio, int* matches12, int* nmatches, cudaStream_t st) {
     if (n_seg < 1) return cudaSuccess;
     if (nd >= (1 << kKeyShift) || (dim != 16 && dim != 32 && dim != 64)) return cudaErrorInvalidValue;
-    const size_t smem = (size_t)64 * K * 4 + (size_t)((nd + 31) / 32) * 4;
-    if (smem > 200 * 1024) return cudaErrorInvalidValue;
+    const size_t smem = bruteforce_replay_smem(K, nd);
+    if (smem > kBfReplaySmemMax) return cudaErrorInvalidValue;
     const bool masked = qm && dm;
     int dev = 0, sms = 0, coop_ok = 0;
     cudaError_t e = cudaGetDevice(&dev);

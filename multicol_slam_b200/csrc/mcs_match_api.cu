@@ -235,7 +235,10 @@ static int bruteforce_core(const uint8_t* q_dev, const uint8_t* qm_dev, const ui
     constexpr int K = 8;
     const int one_seg[2] = {0, nq};
     if (!seg) { seg = one_seg; n_seg = 1; }
-    if (nd >= (1 << 21)) return mfail(MCS_ERR_UNSUPPORTED, "more than 2^21 database descriptors in one call");
+    // the acceptance kernel keeps one bit per database entry in shared memory (kernels.h: bruteforce_replay_smem): at most
+    // 1 622 016 entries.  Checked here so that a larger database is refused before anything is launched.
+    if (nd > bruteforce_max_nd(K))
+        return mfail(MCS_ERR_UNSUPPORTED, "more than " + std::to_string(bruteforce_max_nd(K)) + " database descriptors in one call");
     Dev ds, di, dt, dv1, dseg, dm12, dnm;
     MCK(ds.alloc(nd)); MCK(di.alloc((size_t)nq * K * 4)); MCK(dt.alloc((size_t)nq * K * 4));
     MCK(dv1.alloc(nq)); MCK(dseg.alloc((size_t)(n_seg + 1) * 4)); MCK(dm12.alloc((size_t)nq * 4)); MCK(dnm.alloc((size_t)n_seg * 4));

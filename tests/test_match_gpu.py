@@ -15,13 +15,12 @@ def rand_desc(rng, n, dim=32):
     return rng.integers(0, 256, (n, dim)).astype(np.uint8)
 
 
-@pytest.mark.parametrize("dim", [16, 32, 64])
+@pytest.mark.parametrize("dim,K", [(16, 4), (32, 4), (64, 4), (16, 5), (64, 7)], ids=["16", "32", "64", "16-K5", "64-K7"])
 @pytest.mark.parametrize("masked", [False, True])
-def test_topk_vs_numpy(api, dim, masked):
+def test_topk_vs_numpy(api, dim, masked, K):
     rng = np.random.default_rng(dim + masked)
     q, d = rand_desc(rng, 300, dim), rand_desc(rng, 1777, dim)
-    d[5] = d[900] = q[7]                        # exact duplicates: ties must keep the lower index
-    K = 4
+    d[5] = d[900] = q[7]                        # exact duplicates in different database splits: ties must keep the lower index
     if masked:
         qm, dm = rand_desc(rng, 300, dim) | rand_desc(rng, 300, dim), rand_desc(rng, 1777, dim) | rand_desc(rng, 1777, dim)
         x = np.bitwise_xor(q[:, None, :], d[None, :, :])

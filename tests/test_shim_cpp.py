@@ -8,17 +8,18 @@ import pytest
 import ref_mcs_api          # oracle/, on sys.path through tests/conftest.py (and build())
 
 ROOT = pathlib.Path(__file__).resolve().parents[1]
-EXE = ROOT / "tests" / "cpp" / "shim_smoke"
 
 
-def build():
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-o", str(EXE), str(ROOT / "tests/cpp/shim_smoke.cpp"),
+def build(out_dir):
+    """compile tests/cpp/shim_smoke.cpp into out_dir (the checkout itself may be read-only); -> path of the program"""
+    exe = pathlib.Path(out_dir) / "shim_smoke"
+    subprocess.check_call(["g++", "-O1", "-std=c++17", "-o", str(exe), str(ROOT / "tests/cpp/shim_smoke.cpp"),
                            "-L" + str(ROOT / "multicol_slam_b200"), "-lmcs_b200", "-Wl,-rpath," + str(ROOT / "multicol_slam_b200")])
+    return exe
 
 
-def test_shim_compiles_and_links(api):
-    build()
-    assert EXE.exists()
+def test_shim_compiles_and_links(api, tmp_path):
+    assert build(tmp_path).exists()
 
 
 def test_shim_opencv_branch_compiles(tmp_path):
@@ -74,7 +75,7 @@ def test_adapters_equal_reference_matcher():
 @pytest.mark.gpu
 def test_shim_extract_and_match(api, oa, cams, tmp_path):
     from multicol_slam_b200 import synth
-    build()
+    exe = build(tmp_path)
     cam = cams[0]
     img, mask = synth.frame(cam, 4), synth.mirror_mask(cam)
     (tmp_path / "i.raw").write_bytes(img.tobytes())
@@ -84,7 +85,7 @@ def test_shim_extract_and_match(api, oa, cams, tmp_path):
     from extract_vocabulary import write_text
     voc = np.load(ROOT / "tests" / "golden" / "voc_small_9_6.npz")
     write_text({k: voc[k] for k in voc.files}, tmp_path / "voc.txt")
-    out = subprocess.run([str(EXE), str(tmp_path / "i.raw"), str(tmp_path / "m.raw"), "754", "480", str(tmp_path / "voc.txt")],
+    out = subprocess.run([str(exe), str(tmp_path / "i.raw"), str(tmp_path / "m.raw"), "754", "480", str(tmp_path / "voc.txt")],
                          capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
     kv = dict(t.split("=") for t in out.stdout.split()[1:])
