@@ -2,9 +2,9 @@
 //
 //   M2 hamming_topk_kernel : all-pairs bit-level Hamming distance (ref src/cORBmatcher.cpp:2438-2474)
 //                            of nq queries against nd database descriptors, K best (distance, index)
-//                            per query.  One thread owns one query (descriptor words in registers),
-//                            database tiles are staged in shared memory with 128-bit loads and broadcast.
-//                            Bound by the POPC issue rate, not HBM (SURVEY.md 7, hard part 7).
+//                            per query, as binary matrix products on the tensor cores (BMMA AND.POPC, see
+//                            "K-best lists on the binary tensor cores" below).  A warp owns 32 queries (fragments in
+//                            registers), database tiles are staged in shared memory.  Not bound by HBM.
 //   M1/M3 window_search_kernel : GetFeaturesInArea (ref src/cMultiFrame.cpp:272-340) + distance to every
 //                            candidate, one warp per query, candidates emitted in the reference's visiting
 //                            order (cell-x outer, cell-y inner, insertion order inside a cell).
@@ -93,73 +93,240 @@ __device__ __forceinline__ unsigned hamming_words(const uint32_t (&qw)[WORDS], c
     return dist;
 }
 
-// (Parking candidates in a per-thread shared-memory queue and inserting them with all lanes together -- the insertion below runs
-// with few active lanes -- was tried and was slower: the vote + queue traffic per pair costs more than the divergent insertions.)
-// Keys are 32 bits: distance << kTopkShift | database index (index < 2^21, distance <= 512), the list length KT is a compile-time
-// constant (4 or 8): see hamming_stream_kernel.
+// ---- K-best lists on the binary tensor cores -------------------------------------------------------------------------------------
+// Query a (mask m1) against database entry b (mask m2), x = a ^ b, [u|v].[s|t] = popc(u & s) + popc(v & t) (AND-popcount over
+// the concatenation):
+//   masked:   T = popc(a&m1) + popc(b&m2) + [m1|a].[b|m2] - 2 [a&m1|a].[b|b&m2] = popc(x&m1) + popc(x&m2),  dist = T >> 1
+//             (the integer division of ref :2472)
+//   unmasked: dist = popc(a) + popc(b) - 2 a.b
+// The dot products of 16 queries x 8 entries are one mma.sync.m16n8k256 .b1 AND.POPC (BMMA) per 256 bits of operand: masked
+// 2 / 4 / 8 BMMAs per 16x8 tile at 16 / 32 / 64 bytes, unmasked 1 / 1 / 2 (the second half of a 16-byte k256 step is zero).
+// .xor.popc would give popc(x) directly, but sm_90 lowers it to two AND BMMAs plus inversions.  Measured rate (tools/bmma_rate.cu,
+// H100 80GB HBM3, 400 W limit): 0.66 BMMA/clk/SM with 8 or more warps of 4 independent chains, i.e. 21 masked 32-byte pairs/clk/SM,
+// where the carry-save popcount on the CUDA cores (popc_sum16) is capped near 1.8 by the POPC issue rate.
+// Operand layout: the k dimension is a sequence of 128-bit half chunks (word w of a descriptor is word t = w % 4 of half chunk
+// w / 4); a k256 step takes two of them, and lane (g, t) holds word t of both for rows g and g + 8 (A) and column g (B).  A warp
+// owns 32 queries (two m16 tiles) and keeps their fragments in registers; database tiles are staged in shared memory with each
+// row's words permuted so that a lane's words of all half chunks are adjacent (one 32/64/128-bit load, the warp reads one
+// contiguous block: no bank conflicts).  b & m2 is formed in registers.
+// Epilogue: 3 integer instructions per pair (value, compare); one warp vote skips the list insertions when no lane has a pair
+// below its threshold.  Each lane keeps a partial K-best list for each of its 4 query rows over the 2 of every 8 columns it sees
+// (visited in increasing index order, so `<` keeps the earlier index on equal distance); the 4 lanes of a quad merge their lists
+// at the end.  Keys are unique (the index is part of the key), so the merge is exact.
+// Keys are 32 bits: distance << SHIFT | index (SHIFT 16 for the stream matcher's slots, kTopkShift for the key-frame database).
 constexpr int kTopkShift = 21;
+constexpr unsigned kColOff = 0x40000u;       // cd of a column that is not listed (beyond the database, skipped): its value exceeds
+                                             // every threshold (<= 2 * 0xFFFF) whatever the stale operand bits contribute
+// CTAs per SM the list kernels are compiled for (a register budget: 128 per thread, 168 for the 64-byte masked fragments).  Without
+// it ptxas kept some instantiations at 72 registers and reloaded A fragments from local memory in the inner loop.
+template <int WORDS, bool MASKED>
+constexpr int kListMinBlocks = (MASKED && WORDS == 16) ? 3 : 4;
+template <int WORDS, bool MASKED>
+struct BmmaTile {                            // one staged database tile, rows permuted (see above)
+    uint32_t b[kDbTile * WORDS];
+    uint32_t m[MASKED ? kDbTile * WORDS : 4];
+    unsigned cd[kDbTile];                    // popc(b & m2) (masked) / popc(b), kColOff for a column that is not listed
+};
+
+__device__ __forceinline__ void bmma_and_popc(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+    asm("mma.sync.aligned.m16n8k256.row.col.s32.b1.b1.s32.and.popc {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+template <int H>
+__device__ __forceinline__ void lds_words(const uint32_t* p, uint32_t (&w)[H]) {
+    if constexpr (H == 4) { const uint4 v = *reinterpret_cast<const uint4*>(p); w[0] = v.x; w[1] = v.y; w[2] = v.z; w[3] = v.w; }
+    else if constexpr (H == 2) { const uint2 v = *reinterpret_cast<const uint2*>(p); w[0] = v.x; w[1] = v.y; }
+    else w[0] = p[0];
+}
+
+// Database entries [t0, t0 + tn) of d (dm) into the tile; skip[i] != 0 leaves entry i out of the lists.
+template <int WORDS, bool MASKED>
+__device__ __forceinline__ void bmma_stage(BmmaTile<WORDS, MASKED>& s, const uint32_t* __restrict__ d, const uint32_t* __restrict__ dm,
+                                           const uint8_t* __restrict__ skip, const int t0, const int tn) {
+    constexpr int H = WORDS / 4;
+    for (int j = threadIdx.x; j < kDbTile; j += kTopkThreads) {
+        unsigned cd = kColOff;
+        if (j < tn && !(skip && skip[t0 + j])) {
+            uint32_t w[WORDS], mw[WORDS];
+            const uint4* src = reinterpret_cast<const uint4*>(d + (size_t)(t0 + j) * WORDS);
+            const uint4* msrc = MASKED ? reinterpret_cast<const uint4*>(dm + (size_t)(t0 + j) * WORDS) : nullptr;
+#pragma unroll
+            for (int k = 0; k < H; ++k) {
+                const uint4 v = src[k]; w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+                if (MASKED) { const uint4 u = msrc[k]; mw[4 * k] = u.x; mw[4 * k + 1] = u.y; mw[4 * k + 2] = u.z; mw[4 * k + 3] = u.w; }
+            }
+            cd = 0;
+#pragma unroll
+            for (int k = 0; k < WORDS; ++k) cd += __popc(MASKED ? (w[k] & mw[k]) : w[k]);
+            uint32_t pw[WORDS], pm[WORDS];                       // word 4h + t at t * H + h
+#pragma unroll
+            for (int k = 0; k < WORDS; ++k) { pw[(k & 3) * H + (k >> 2)] = w[k]; pm[(k & 3) * H + (k >> 2)] = mw[k]; }
+#pragma unroll
+            for (int k = 0; k < H; ++k) {
+                reinterpret_cast<uint4*>(s.b + j * WORDS)[k] = make_uint4(pw[4 * k], pw[4 * k + 1], pw[4 * k + 2], pw[4 * k + 3]);
+                if (MASKED) reinterpret_cast<uint4*>(s.m + j * WORDS)[k] = make_uint4(pm[4 * k], pm[4 * k + 1], pm[4 * k + 2], pm[4 * k + 3]);
+            }
+        }
+        s.cd[j] = cd;
+    }
+}
+
+// The K-best lists of the CTA's 128 queries (rows 0 .. nq_cta - 1 of q / qm; rows beyond are not listed) against database entries
+// [j0, j1) of d / dm that skip does not exclude, listing only distances below worst0.  Every thread of the CTA must call this.
+// emit(row, k, key) receives, from lane t == 0 of each quad, key k < KT of the CTA row (kNone past the list's end).
+template <int WORDS, bool MASKED, int KT, int SHIFT, class Emit>
+__device__ __forceinline__ void bmma_klists(const uint32_t* __restrict__ q, const uint32_t* __restrict__ qm, const int nq_cta,
+                                            const uint32_t* __restrict__ d, const uint32_t* __restrict__ dm, const uint8_t* __restrict__ skip,
+                                            const int j0, const int j1, const int K, const unsigned worst0, BmmaTile<WORDS, MASKED>& s,
+                                            Emit&& emit) {
+    constexpr int H = WORDS / 4;                                   // 128-bit half chunks of a descriptor
+    constexpr int STEPS = MASKED ? H : (H + 1) / 2;                // k256 steps per product
+    constexpr unsigned kNone = 0xFFFFFFFFu;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
+    // rows r = 0..3 of this lane: m-tile r >> 1, row g + 8 * (r & 1) of it
+    uint32_t qa[4][H], qx[4][H], qam[4][H];         // a, m1, a & m1: word t of every half chunk
+    unsigned cq[4], thr[4];                                        // popc(a & m1) / popc(a); value threshold (2 * worst masked)
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int row = warp * 32 + (r >> 1) * 16 + (r & 1) * 8 + g;
+        const bool act = row < nq_cta;
+        unsigned c = 0;
+#pragma unroll
+        for (int h = 0; h < H; ++h) {
+            qa[r][h] = act ? q[(size_t)row * WORDS + 4 * h + t] : 0u;
+            if constexpr (MASKED) {
+                qx[r][h] = act ? qm[(size_t)row * WORDS + 4 * h + t] : 0u;
+                qam[r][h] = qa[r][h] & qx[r][h];
+                c += __popc(qam[r][h]);
+            } else {
+                c += __popc(qa[r][h]);
+            }
+        }
+        c += __shfl_xor_sync(0xffffffffu, c, 1);
+        c += __shfl_xor_sync(0xffffffffu, c, 2);
+        cq[r] = c;
+        thr[r] = act ? (MASKED ? 2 * worst0 : worst0) : 0u;
+    }
+    unsigned best[4][KT];
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int k = 0; k < KT; ++k) best[r][k] = kNone;
+
+    for (int t0 = j0; t0 < j1; t0 += kDbTile) {
+        const int tn = min(kDbTile, j1 - t0);
+        __syncthreads();
+        bmma_stage<WORDS, MASKED>(s, d, dm, skip, t0, tn);
+        __syncthreads();
+        for (int n0 = 0; n0 < tn; n0 += 8) {
+            uint32_t bw[H], mw[H], bmw[H];
+            lds_words<H>(s.b + (n0 + g) * WORDS + t * H, bw);
+            if constexpr (MASKED) {
+                lds_words<H>(s.m + (n0 + g) * WORDS + t * H, mw);
+#pragma unroll
+                for (int h = 0; h < H; ++h) bmw[h] = bw[h] & mw[h];
+            }
+            const uint2 cd = *reinterpret_cast<const uint2*>(s.cd + n0 + 2 * t);
+            unsigned v[4][2];                                      // row r, column 2t + c
+            bool any = false;
+#pragma unroll
+            for (int mt = 0; mt < 2; ++mt) {
+                const int r0 = 2 * mt, r1 = 2 * mt + 1;
+                int c1[4] = {0, 0, 0, 0};
+#pragma unroll
+                for (int st = 0; st < STEPS; ++st) {
+                    // half chunks 2st, 2st + 1 of A = [m1|a] (masked) / [a], B = [b|m2] / [b]
+                    const int h0 = 2 * st, h1 = 2 * st + 1;
+                    if constexpr (MASKED) {
+                        bmma_and_popc(c1, h0 < H ? qx[r0][h0] : qa[r0][h0 - H], h0 < H ? qx[r1][h0] : qa[r1][h0 - H],
+                                      h1 < H ? qx[r0][h1] : qa[r0][h1 - H], h1 < H ? qx[r1][h1] : qa[r1][h1 - H],
+                                      h0 < H ? bw[h0] : mw[h0 - H], h1 < H ? bw[h1] : mw[h1 - H]);
+                    } else {
+                        bmma_and_popc(c1, qa[r0][h0], qa[r1][h0], h1 < H ? qa[r0][h1] : 0u, h1 < H ? qa[r1][h1] : 0u,
+                                      bw[h0], h1 < H ? bw[h1] : 0u);
+                    }
+                }
+                if constexpr (MASKED) {
+                    int c2[4] = {0, 0, 0, 0};                      // [a&m1|a].[b|b&m2]
+#pragma unroll
+                    for (int st = 0; st < STEPS; ++st) {
+                        const int h0 = 2 * st, h1 = 2 * st + 1;
+                        bmma_and_popc(c2, h0 < H ? qam[r0][h0] : qa[r0][h0 - H], h0 < H ? qam[r1][h0] : qa[r1][h0 - H],
+                                      h1 < H ? qam[r0][h1] : qa[r0][h1 - H], h1 < H ? qam[r1][h1] : qa[r1][h1 - H],
+                                      h0 < H ? bw[h0] : bmw[h0 - H], h1 < H ? bw[h1] : bmw[h1 - H]);
+                    }
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) c1[i] -= 2 * c2[i];
+                }
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int r = 2 * mt + (i >> 1);
+                    const unsigned val = cq[r] + (i & 1 ? cd.y : cd.x) + (MASKED ? c1[i] : -2 * c1[i]);
+                    v[r][i & 1] = val;
+                    any |= val < thr[r];
+                }
+            }
+            if (__any_sync(0xffffffffu, any)) {
+#pragma unroll
+                for (int r = 0; r < 4; ++r)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        // one vote per (row, column) slot: the warp runs only the insertions some lane needs, not all 8
+                        if (!__any_sync(0xffffffffu, v[r][c] < thr[r])) continue;
+                        if (v[r][c] < thr[r]) {                    // strict: equal distances keep the earlier index
+                            unsigned key = ((MASKED ? v[r][c] >> 1 : v[r][c]) << SHIFT) | (unsigned)(t0 + n0 + 2 * t + c);
+#pragma unroll
+                            for (int k = 0; k < KT; ++k) {
+                                if (k < K) { const unsigned lo = min(key, best[r][k]); key = max(key, best[r][k]); best[r][k] = lo; }
+                            }
+                            unsigned w = best[r][0];
+#pragma unroll
+                            for (int k = 1; k < KT; ++k) if (k < K) w = best[r][k];
+                            if (w != kNone) thr[r] = min(thr[r], MASKED ? 2 * (w >> SHIFT) : w >> SHIFT);
+                        }
+                    }
+            }
+        }
+    }
+    // quad merge: K rounds of "smallest head of the four lists", popped by the lane that holds it
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+        const int row = warp * 32 + (r >> 1) * 16 + (r & 1) * 8 + g;
+#pragma unroll
+        for (int k = 0; k < KT; ++k) {
+            unsigned m = kNone;
+            if (k < K) {
+                const unsigned h = best[r][0];
+                m = min(h, __shfl_xor_sync(0xffffffffu, h, 1));
+                m = min(m, __shfl_xor_sync(0xffffffffu, m, 2));
+                if (h == m) {
+#pragma unroll
+                    for (int j = 0; j + 1 < KT; ++j) best[r][j] = best[r][j + 1];
+                    best[r][KT - 1] = kNone;
+                }
+            }
+            if (t == 0) emit(row, k, m);
+        }
+    }
+}
+
 template <int WORDS, bool MASKED, int KT>
-__global__ void __launch_bounds__(kTopkThreads)
+__global__ void __launch_bounds__(kTopkThreads, kListMinBlocks<WORDS, MASKED>)
 hamming_topk_kernel(const uint32_t* __restrict__ q, const uint32_t* __restrict__ qmask, const int nq,
                     const uint32_t* __restrict__ d, const uint32_t* __restrict__ dmask, const int nd,
                     const uint8_t* __restrict__ skip, const int K, const int chunk, const unsigned bound,
                     unsigned* __restrict__ part /* [splits][nq][kTopKMax] */) {
-    __shared__ __align__(16) uint32_t s_d[kDbTile * WORDS];
-    __shared__ __align__(16) uint32_t s_m[MASKED ? kDbTile * WORDS : 4];
-    __shared__ uint8_t s_skip[kDbTile];
-
-    const int qi = blockIdx.x * kTopkThreads + threadIdx.x;
-    const bool active = qi < nq;
-    uint32_t qw[WORDS], qm[MASKED ? WORDS : 1];
-#pragma unroll
-    for (int k = 0; k < WORDS; ++k) {
-        qw[k] = active ? q[(size_t)qi * WORDS + k] : 0u;
-        if (MASKED) qm[k] = active ? qmask[(size_t)qi * WORDS + k] : 0u;
-    }
-    constexpr unsigned kNone = 0xFFFFFFFFu;
-    unsigned best[KT];
-#pragma unroll
-    for (int k = 0; k < KT; ++k) best[k] = kNone;
-    unsigned worst = min(bound, 0x7FFu);   // a pair is listed only below the K-th best so far and the caller's bound
-
+    __shared__ __align__(16) BmmaTile<WORDS, MASKED> s;
+    const int qb = blockIdx.x * kTopkThreads;
     const int j0 = blockIdx.y * chunk, j1 = min(j0 + chunk, nd);
-    for (int t0 = j0; t0 < j1; t0 += kDbTile) {
-        const int tn = min(kDbTile, j1 - t0);
-        __syncthreads();
-        {   // 128-bit coalesced staging of the database tile
-            const uint4* src = (const uint4*)(d + (size_t)t0 * WORDS);
-            uint4* dst = (uint4*)s_d;
-            for (int i = threadIdx.x; i < tn * WORDS / 4; i += kTopkThreads) dst[i] = src[i];
-            if (MASKED) {
-                const uint4* msrc = (const uint4*)(dmask + (size_t)t0 * WORDS);
-                uint4* mdst = (uint4*)s_m;
-                for (int i = threadIdx.x; i < tn * WORDS / 4; i += kTopkThreads) mdst[i] = msrc[i];
-            }
-            for (int i = threadIdx.x; i < tn; i += kTopkThreads) s_skip[i] = skip ? skip[t0 + i] : 0;
-        }
-        __syncthreads();
-        for (int j = 0; j < tn; ++j) {
-            if (s_skip[j]) continue;       // uniform across the CTA
-            // bit-level Hamming distance; masked form = (popc(x&ma) + popc(x&mb)) / 2, integer division (ref :2472)
-            const unsigned dist = hamming_words<WORDS, MASKED>(qw, qm, s_d + j * WORDS, s_m + j * WORDS);
-            if (dist < worst) {            // strict: equal distances keep the earlier index; entries at or beyond `bound` are not listed
-                unsigned key = (dist << kTopkShift) | (unsigned)(t0 + j);
-#pragma unroll
-                for (int k = 0; k < KT; ++k) {
-                    if (k < K) { const unsigned lo = min(key, best[k]); key = max(key, best[k]); best[k] = lo; }
-                }
-                unsigned w = best[0];
-#pragma unroll
-                for (int k = 1; k < KT; ++k) if (k < K) w = best[k];
-                if (w != kNone) worst = min(worst, w >> kTopkShift);
-            }
-        }
-    }
-    if (active) {
-        unsigned* o = part + ((size_t)blockIdx.y * nq + qi) * kTopKMax;
-#pragma unroll
-        for (int k = 0; k < kTopKMax; ++k) o[k] = k < KT ? best[k < KT ? k : 0] : kNone;
-    }
+    bmma_klists<WORDS, MASKED, KT, kTopkShift>(q + (size_t)qb * WORDS, MASKED ? qmask + (size_t)qb * WORDS : nullptr, nq - qb, d, dmask,
+                                               skip, j0, j1, K, min(bound, 0x7FFu), s, [=](int row, int k, unsigned key) {
+        if (qb + row >= nq) return;
+        unsigned* o = part + ((size_t)blockIdx.y * nq + qb + row) * kTopKMax;
+        o[k] = key;
+        if (k == KT - 1)
+            for (int j = KT; j < kTopKMax; ++j) o[j] = 0xFFFFFFFFu;
+    });
 }
 
 __global__ void topk_merge_kernel(const unsigned* __restrict__ part, const int splits, const int nq, const int K,
@@ -229,24 +396,23 @@ cudaError_t launch_hamming_topk(const uint8_t* q, const uint8_t* qmask, int nq, 
 
 // Stream matching: image i = (frame f, camera c) is matched against image i - n_cams = (f-1, c); both live in
 // fixed-size slots of `capacity` descriptors, the valid counts are read on the device (no host sync).
-// One thread owns one query; the (<= capacity) database descriptors of the previous frame are staged tile by
-// tile in shared memory.  Output: K best (index, distance) per query slot, (-1, INT_MAX) where none.
-// The per-thread list holds 32-bit keys (distance << 16 | slot; slots < 65536, distances <= 512) and its length KT is a compile-time
-// constant (4 or 8): the sorted insertion -- executed by the one or two lanes of a warp that have a candidate -- is 3 instructions
-// per list position instead of ~6 on 64-bit keys over all 8 positions.
+// A CTA lists 128 query slots against the (<= capacity) database descriptors of the previous frame, staged tile by tile in
+// shared memory (bmma_klists).  Output: K best (index, distance) per query slot, (-1, INT_MAX) where none.
+// Keys are 32 bits (distance << 16 | slot; slots < 65536, distances <= 512) and the list length KT is a compile-time constant
+// (4 or 8): the sorted insertion is 3 instructions per list position instead of ~6 on 64-bit keys over all 8 positions.
 template <int WORDS, bool MASKED, int KT>
-__global__ void __launch_bounds__(kTopkThreads)
+__global__ void __launch_bounds__(kTopkThreads, kListMinBlocks<WORDS, MASKED>)
 hamming_stream_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const int* __restrict__ counts,
                       const int n_cams, const int capacity, const int K, const int img_lo, const unsigned bound,
                       int* __restrict__ out_idx, int* __restrict__ out_dist) {
-    __shared__ __align__(16) uint32_t s_d[kDbTile * WORDS];
-    __shared__ __align__(16) uint32_t s_m[MASKED ? kDbTile * WORDS : 4];
+    __shared__ __align__(16) BmmaTile<WORDS, MASKED> s;
     const int img = blockIdx.y + img_lo;
-    const int qi = blockIdx.x * kTopkThreads + threadIdx.x;
+    const int qb = blockIdx.x * kTopkThreads;
     const bool has_prev = img >= n_cams;                 // frame 0 has no predecessor
     const int nq = has_prev ? min(counts[img], capacity) : 0;
     const int nd = has_prev ? min(counts[img - n_cams], capacity) : 0;
-    if ((int)(blockIdx.x * kTopkThreads) >= nq) {        // nothing to match in this block: mark the slots empty
+    if (qb >= nq) {                                      // nothing to match in this block: mark the slots empty
+        const int qi = qb + threadIdx.x;
         if (qi < capacity)
             for (int k = 0; k < K; ++k) {
                 out_idx[((size_t)img * capacity + qi) * K + k] = -1;
@@ -254,65 +420,15 @@ hamming_stream_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restr
             }
         return;
     }
-    const bool active = qi < nq;
-    const uint32_t* q = desc + ((size_t)img * capacity + qi) * WORDS;
-    const uint32_t* qmk = MASKED ? dmask + ((size_t)img * capacity + qi) * WORDS : nullptr;
-    uint32_t qw[WORDS], qm[MASKED ? WORDS : 1];
-#pragma unroll
-    for (int k = 0; k < WORDS; ++k) {
-        qw[k] = active ? q[k] : 0u;
-        if (MASKED) qm[k] = active ? qmk[k] : 0u;
-    }
-    constexpr unsigned kNone = 0xFFFFFFFFu;
-    unsigned best[KT];
-#pragma unroll
-    for (int k = 0; k < KT; ++k) best[k] = kNone;
-    unsigned worst = min(bound, 0xFFFFu);                // a pair is listed only below the K-th best so far and the caller's bound
-    const uint32_t* dbase = desc + (size_t)(img - n_cams) * capacity * WORDS;
-    const uint32_t* mbase = MASKED ? dmask + (size_t)(img - n_cams) * capacity * WORDS : nullptr;
-    for (int t0 = 0; t0 < nd; t0 += kDbTile) {
-        const int tn = min(kDbTile, nd - t0);
-        __syncthreads();
-        {
-            const uint4* src = (const uint4*)(dbase + (size_t)t0 * WORDS);
-            uint4* dst = (uint4*)s_d;
-            for (int i = threadIdx.x; i < tn * WORDS / 4; i += kTopkThreads) dst[i] = src[i];
-            if (MASKED) {
-                const uint4* msrc = (const uint4*)(mbase + (size_t)t0 * WORDS);
-                uint4* mdst = (uint4*)s_m;
-                for (int i = threadIdx.x; i < tn * WORDS / 4; i += kTopkThreads) mdst[i] = msrc[i];
-            }
-        }
-        __syncthreads();
-#pragma unroll 2
-        for (int j = 0; j < tn; ++j) {
-            // bit-level Hamming distance; masked form = (popc(x&ma) + popc(x&mb)) / 2, integer division (ref :2472)
-            const unsigned dist = hamming_words<WORDS, MASKED>(qw, qm, s_d + j * WORDS, s_m + j * WORDS);
-            if (dist < worst) {                          // strict: equal distances keep the earlier slot
-                unsigned key = (dist << 16) | (unsigned)(t0 + j);
-#pragma unroll
-                for (int k = 0; k < KT; ++k) {
-                    if (k < K) { const unsigned lo = min(key, best[k]); key = max(key, best[k]); best[k] = lo; }
-                }
-                unsigned w = best[0];
-#pragma unroll
-                for (int k = 1; k < KT; ++k) if (k < K) w = best[k];
-                if (w != kNone) worst = min(worst, w >> 16);
-            }
-        }
-    }
-    if (qi < capacity) {
-        int* oi = out_idx + ((size_t)img * capacity + qi) * K;
-        int* od = out_dist + ((size_t)img * capacity + qi) * K;
-#pragma unroll
-        for (int k = 0; k < KT; ++k) {
-            if (k < K) {
-                const bool none = !active || best[k] == kNone;
-                oi[k] = none ? -1 : (int)(best[k] & 0xFFFFu);
-                od[k] = none ? 0x7FFFFFFF : (int)(best[k] >> 16);
-            }
-        }
-    }
+    const size_t q_row0 = (size_t)img * capacity + qb, d_row0 = (size_t)(img - n_cams) * capacity;
+    bmma_klists<WORDS, MASKED, KT, 16>(desc + q_row0 * WORDS, MASKED ? dmask + q_row0 * WORDS : nullptr, nq - qb, desc + d_row0 * WORDS,
+                                       MASKED ? dmask + d_row0 * WORDS : nullptr, nullptr, 0, nd, K, min(bound, 0xFFFFu), s,
+                                       [=](int row, int k, unsigned key) {
+        if (qb + row >= capacity || k >= K) return;
+        const bool none = qb + row >= nq || key == 0xFFFFFFFFu;
+        out_idx[(q_row0 + row) * K + k] = none ? -1 : (int)(key & 0xFFFFu);
+        out_dist[(q_row0 + row) * K + k] = none ? 0x7FFFFFFF : (int)(key >> 16);
+    });
 }
 
 cudaError_t launch_hamming_stream(const uint8_t* desc, const uint8_t* dmask, const int* counts, int img_lo, int img_count,
