@@ -109,10 +109,16 @@ __device__ __forceinline__ unsigned hamming_words(const uint32_t (&qw)[WORDS], c
 // owns 32 queries (two m16 tiles) and keeps their fragments in registers; database tiles are staged in shared memory with each
 // row's words permuted so that a lane's words of all half chunks are adjacent (one 32/64/128-bit load, the warp reads one
 // contiguous block: no bank conflicts).  b & m2 is formed in registers.
-// Epilogue: 3 integer instructions per pair (value, compare); one warp vote skips the list insertions when no lane has a pair
-// below its threshold.  Each lane keeps a partial K-best list for each of its 4 query rows over the 2 of every 8 columns it sees
+// Epilogue: 3 integer instructions per pair (value, compare); one warp vote skips the rest when no lane has a pair below its
+// threshold.  Each lane keeps a partial K-best list for each of its 4 query rows over the 2 of every 8 columns it sees
 // (visited in increasing index order, so `<` keeps the earlier index on equal distance); the 4 lanes of a quad merge their lists
-// at the end.  Keys are unique (the index is part of the key), so the merge is exact.
+// at the end.  Keys are unique (the index is part of the key), so the merge is exact.  Pairs below the threshold are appended to
+// the lane's candidate buffer and folded into the lists in batches, so that the warp runs as many insertions as its busiest lane
+// needs rather than one per (row, column) slot in which any lane has a candidate; the threshold is the tighter of the lane's own
+// K-th distance and the best K-th distance of its quad.  H100 80GB HBM3, 700 W limit, bench.py config 2, the greedy matcher's
+// list kernel (tools/m2_split.py): 3.92 ms with one insertion per slot and no quad bound, 3.90 / 3.63 ms with the quad bound
+// refreshed every 8 / 32 column steps, 1.76 ms with the candidate buffer (quad bound refreshed at each fold); 0.75-0.77 ms when
+// nothing is listed (th_low = 0).
 // Keys are 32 bits: distance << SHIFT | index (SHIFT 16 for the stream matcher's slots, kTopkShift for the key-frame database).
 constexpr int kTopkShift = 21;
 constexpr unsigned kColOff = 0x40000u;       // cd of a column that is not listed (beyond the database, skipped): its value exceeds
@@ -121,11 +127,15 @@ constexpr unsigned kColOff = 0x40000u;       // cd of a column that is not liste
 // it ptxas kept some instantiations at 72 registers and reloaded A fragments from local memory in the inner loop.
 template <int WORDS, bool MASKED>
 constexpr int kListMinBlocks = (MASKED && WORDS == 16) ? 3 : 4;
+// Candidate keys a lane buffers per query row before the warp folds them into the lists (bmma_klists).  7 keeps the 64-byte masked
+// kernels' static shared memory under 48 KB.
+constexpr int kCandDepth = 7;
 template <int WORDS, bool MASKED>
 struct BmmaTile {                            // one staged database tile, rows permuted (see above)
     uint32_t b[kDbTile * WORDS];
     uint32_t m[MASKED ? kDbTile * WORDS : 4];
     unsigned cd[kDbTile];                    // popc(b & m2) (masked) / popc(b), kColOff for a column that is not listed
+    unsigned cand[kTopkThreads / 32][4][kCandDepth][32];    // [warp][row r][entry][lane]: the lanes' candidate buffers
 };
 
 __device__ __forceinline__ void bmma_and_popc(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
@@ -212,6 +222,36 @@ __device__ __forceinline__ void bmma_klists(const uint32_t* __restrict__ q, cons
     for (int r = 0; r < 4; ++r)
 #pragma unroll
         for (int k = 0; k < KT; ++k) best[r][k] = kNone;
+    unsigned* cand = &s.cand[warp][0][0][lane];                    // row r, entry i at cand[(r * kCandDepth + i) * 32]
+    int cnt[4] = {0, 0, 0, 0};
+    // Fold the buffered candidates into the lists (the whole warp, every lane its own), then tighten each row's threshold to
+    //   own:  value < 2 dK (masked) / dK -- strict, dK this lane's K-th distance: within a lane columns arrive in index order, so a
+    //         later column at distance dK cannot displace an entry;
+    //   quad: value < 2 dq + 2 / dq + 1 -- inclusive, dq the smallest K-th distance of the quad's full lists (the 4 lanes list the
+    //         same rows over disjoint columns): a pair farther than dq has K smaller keys in that lane's list; one at dq is kept,
+    //         since across lanes the index order of the columns is not the order in which they are visited.
+    // The quad bound changes only when a list changes, i.e. here.
+    auto fold = [&]() {
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            for (int i = 0; i < cnt[r]; ++i) {
+                unsigned key = cand[(r * kCandDepth + i) * 32];
+#pragma unroll
+                for (int k = 0; k < KT; ++k) {
+                    if (k < K) { const unsigned lo = min(key, best[r][k]); key = max(key, best[r][k]); best[r][k] = lo; }
+                }
+            }
+            cnt[r] = 0;
+            unsigned w = best[r][0];
+#pragma unroll
+            for (int k = 1; k < KT; ++k) if (k < K) w = best[r][k];
+            const unsigned own = w == kNone ? kNone : (MASKED ? 2 * (w >> SHIFT) : w >> SHIFT);
+            unsigned quad = w == kNone ? kNone : own + (MASKED ? 2 : 1);
+            quad = min(quad, __shfl_xor_sync(0xffffffffu, quad, 1));
+            quad = min(quad, __shfl_xor_sync(0xffffffffu, quad, 2));
+            thr[r] = min(thr[r], min(own, quad));
+        }
+    };
 
     for (int t0 = j0; t0 < j1; t0 += kDbTile) {
         const int tn = min(kDbTile, j1 - t0);
@@ -266,28 +306,24 @@ __device__ __forceinline__ void bmma_klists(const uint32_t* __restrict__ q, cons
                     any |= val < thr[r];
                 }
             }
+            // candidates below the threshold go to this lane's buffer, in column order; the warp folds them in when some lane's
+            // buffer for a row could not take another step's two columns.  A step where no lane has a candidate costs one vote.
             if (__any_sync(0xffffffffu, any)) {
+                if (any) {
 #pragma unroll
-                for (int r = 0; r < 4; ++r)
+                    for (int r = 0; r < 4; ++r)
 #pragma unroll
-                    for (int c = 0; c < 2; ++c) {
-                        // one vote per (row, column) slot: the warp runs only the insertions some lane needs, not all 8
-                        if (!__any_sync(0xffffffffu, v[r][c] < thr[r])) continue;
-                        if (v[r][c] < thr[r]) {                    // strict: equal distances keep the earlier index
-                            unsigned key = ((MASKED ? v[r][c] >> 1 : v[r][c]) << SHIFT) | (unsigned)(t0 + n0 + 2 * t + c);
-#pragma unroll
-                            for (int k = 0; k < KT; ++k) {
-                                if (k < K) { const unsigned lo = min(key, best[r][k]); key = max(key, best[r][k]); best[r][k] = lo; }
+                        for (int c = 0; c < 2; ++c)
+                            if (v[r][c] < thr[r]) {
+                                cand[(r * kCandDepth + cnt[r]) * 32] = ((MASKED ? v[r][c] >> 1 : v[r][c]) << SHIFT) | (unsigned)(t0 + n0 + 2 * t + c);
+                                ++cnt[r];
                             }
-                            unsigned w = best[r][0];
-#pragma unroll
-                            for (int k = 1; k < KT; ++k) if (k < K) w = best[r][k];
-                            if (w != kNone) thr[r] = min(thr[r], MASKED ? 2 * (w >> SHIFT) : w >> SHIFT);
-                        }
-                    }
+                }
+                if (__any_sync(0xffffffffu, max(max(cnt[0], cnt[1]), max(cnt[2], cnt[3])) > kCandDepth - 2)) fold();
             }
         }
     }
+    fold();
     // quad merge: K rounds of "smallest head of the four lists", popped by the lane that holds it
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
