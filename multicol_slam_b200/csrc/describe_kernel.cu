@@ -1,4 +1,4 @@
-// describe_kernel.cu -- K3: orientation + descriptor, one warp per selected keypoint.
+// describe_kernel.cu -- K3: orientation + descriptor, one warp per batch of 32 selected keypoints.
 //
 //   IC_Angle            ref src/mdBRIEFextractorOct.cpp:221-248   integer moments over the 845-px disc, fastAtan2
 //   undistortPointsOcam ref :1306-1317, include/cam_model_omni.h:127-138
@@ -6,11 +6,14 @@
 //   compute_ORB / compute_dBRIEF / compute_mdBRIEF   ref :303-554
 //   output assembly     ref :1327-1335  (pt *= scale for levels > 0)
 //
-// Layout of the work: lane b of the warp owns descriptor byte b, i.e. the 16 pattern points 16b..16b+15 (8 test
-// pairs).  For the distorted variants the lane parks the 16 projected points of one pattern in its own shared-memory
-// slots, the warp reduces their sum (the reference subtracts the mean of all 512 projected points, :262-281), then every
-// lane rounds and samples its own points: no shuffles, no second projection pass.  Warp-uniform state that is only needed
-// again in the rare paths or at the end lives in a per-warp context in shared memory (WarpCtx), not in registers.
+// Layout of the work: a warp takes 32 consecutive selected slots of one image.  First lane i sets up keypoint i (corner, output
+// index, undistortion, table row, tier-1 constants) into a per-keypoint context in shared memory (KpCtx); then the warp stages the
+// IC neighbourhoods three keypoints per round trip and sums their moments; then lane i computes keypoint i's angle and writes its
+// keypoint record; then the warp walks the batch, one keypoint at a time, staging the blurred patch and evaluating the patterns.
+// In the pattern work lane b owns descriptor byte b, i.e. the 16 pattern points 16b..16b+15 (8 test pairs).  For the distorted
+// variants the lane parks the 16 projected points of one pattern in its own shared-memory slots, the warp reduces their sum
+// (the reference subtracts the mean of all 512 projected points, :262-281), then every lane rounds and samples its own points:
+// no shuffles, no second projection pass.
 //
 // Fisheye projection cost.  cCamModelGeneral_::WorldToImg evaluates, per pattern point, sqrt + 3 divisions +
 // atan + a 12-term Horner in double (~250 FP64 instructions; 1536 points per mdBRIEF keypoint).  Because the
@@ -86,10 +89,11 @@ constexpr int kDescWarps = 4;
 constexpr int kPatchR = 25;                       // staged patch: rows/cols ky/kx -25 .. +25 (keypoints are >= 25 px inside the ROI)
 constexpr int kPatchS = 64;                       // bytes per staged patch row (4-byte aligned start + 51 columns)
 constexpr int kLutDeg = 9;                        // degree of the per-centre polynomial of R(r)  (kernels.h: DistortLut)
-// resident CTAs per SM the register budget is cut for.  sm_90a, H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs,
-// K3 ms per 384 images: 4 -> 126-128 registers, no spills: 5.49 / 5.90; 5 -> 96 registers, 80-144 B spilled: 5.39 / 5.51;
-// 6 -> 80 registers: 5.81 / 5.85
-constexpr int kDescMinBlocks = 5;
+// resident CTAs per SM the register budget is cut for.  The 32 keypoint contexts per warp (16 KB per CTA) leave room for 4 CTAs
+// (50 KB each with descSize <= 32); 4 -> 128 registers, no spills in the descSize <= 32 instantiation.  (One warp per keypoint,
+// without the contexts, measured on an H100 80GB HBM3 at 400 W, bench.py config 2, K3 ms: 4 CTAs 5.49 / 5.90, 5 CTAs 5.39 / 5.51,
+// 6 CTAs 5.81 / 5.85.)
+constexpr int kDescMinBlocks = 4;
 constexpr int kT1Unroll1 = 4;                     // unroll of tier-1 pass 1 (m-form), points per iteration
 constexpr int kT1Unroll2 = 2;                     // unroll of tier-1 pass 2, point PAIRS per iteration
 constexpr int kT1Coef = 6;                        // tier 1: q(s') of degree 5, R(i + s) - R(i) = s' q(s'), s' = s / kT1Scale
@@ -325,15 +329,30 @@ __device__ __noinline__ unsigned tier1_repair(const mcs_ocam* camp, const float2
     return out;
 }
 
-// warp-uniform values of the keypoint a warp works on, kept in shared memory across the pattern loops (see the kernel)
-struct __align__(16) WarpCtx {
-    float t1[16];                   // tier-1 constants of the keypoint: q[0..7], K0f, gkf, s0f, rk2f, rkf, auk, avk
-    double ukx, uky, a_base, ca[3], sa[3];
-    const double* row;
-    int kx, ky, oidx, b, level;
-    uint32_t c;
-    float angle;
+// per-keypoint values of a warp's batch, computed with one keypoint per lane and kept in shared memory while the warp walks the batch
+struct __align__(16) KpCtx {
+    float t1[16];                   // tier-1 constants: q[0..7], K0f, gkf, s0f, rk2f, rkf, auk, avk; [15] the IC angle
+    double ukx, uky, c0, s0;        // undistorted keypoint; cos / sin of the pattern angle a0
+    const double* row;              // the keypoint's distortion-table row
+    uint32_t c;                     // packed corner
+    int oidx, level, flags;         // output index, pyramid level, kKpLut | kKpT1 | kKpMForm
 };
+constexpr int kKpLut = 1, kKpT1 = 2, kKpMForm = 4;
+constexpr int kIcBatch = 3;         // IC neighbourhoods staged per round trip (3 x 33 rows x 40 bytes fit one warp's parking slice)
+
+// pattern angle a0 of the reference: angle / RHOf for mdBRIEF (ref :425), angle * DEG2RADf otherwise (ref :313,367)
+__device__ __forceinline__ double pattern_base_angle(float angle, bool masks) {
+    return masks ? (double)__fdiv_rn(angle, 57.2957763671875f) : (double)__fmul_rn(angle, 0.01745329238474369f);
+}
+// cos / sin of pattern qi's angle: a0, a0 + 20 deg, a0 - 20 deg (20 / RHOd, ref :424) by the addition theorems (1e-16 away from
+// cos/sin(a0 +- rot); the exact path uses the reference's own cos(angle +- rot) / sin(angle +- rot))
+__device__ __forceinline__ void pattern_rotation(double c0, double s0, int qi, double& ca, double& sa) {
+    const double c20 = 0.93969262078590838405, s20 = 0.34202014332566873304;
+    if (qi == 0) { ca = c0; sa = s0; }
+    else if (qi == 1) { ca = fma(c0, c20, -s0 * s20); sa = fma(s0, c20, c0 * s20); }
+    else { ca = fma(c0, c20, s0 * s20); sa = fma(s0, c20, -c0 * s20); }
+}
+
 template <int PPL /* pattern points per lane: 16 for descSize <= 32, 32 for descSize 64 */>
 __global__ void __launch_bounds__(kDescWarps * 32, kDescMinBlocks)
 describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, const mcs_ocam* __restrict__ cams,
@@ -342,7 +361,7 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
                 mcs_keypoint* __restrict__ kps_out, uint8_t* __restrict__ desc_out, uint8_t* __restrict__ dmask_out,
                 int* __restrict__ counts_out, const int capacity, const int n_images) {
     __shared__ mcs_ocam s_cam[kDescWarps];
-    __shared__ WarpCtx s_ctx[kDescWarps];
+    __shared__ KpCtx s_kp[kDescWarps][32];
     __shared__ __align__(8) float2 s_patf[PPL * 32];      // [j][lane] : point 16*byte + k with byte = lane + 32*(j/16), k = j%16, as floats
     // tier 1 parks the projected coordinates of the current pattern here between its two passes ([point][lane], this lane's own
     // slots only): with rolled loops the kernel body stays inside the instruction cache -- the fully unrolled form spent most of
@@ -355,194 +374,64 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
     for (int i = threadIdx.x; i < PPL * 32; i += kDescWarps * 32) s_patf[i] = g_patf[i];
     __syncthreads();
 
+    // A warp describes a batch of 32 consecutive selected slots of one image (level-major, so a batch may cross levels).  The
+    // warp-uniform set-up of a keypoint (undistortion, table row, tier-1 constants, angle) is computed with one keypoint per lane,
+    // then the warp walks the batch doing only patch staging and pattern work.
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    // one warp per slot (a persistent grid-stride variant was slower: static imbalance and more spills)
-    const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int sel_total = geom->sel_total;
-    const int b = warp_global / sel_total;
+    const int wpi = (sel_total + 31) >> 5;                      // warps per image
+    const int warp_global = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int b = warp_global / wpi;
     if (b >= n_images) return;
-    const int slot = warp_global - b * sel_total;
     const int L = geom->nlevels;
-    int level = 0, off = 0;
-    for (int l = 0; l < L; ++l)
-        if (slot >= geom->lv[l].sel_off) level = l;
-    for (int l = 0; l < level; ++l) off += sel_count[b * L + l];
-    const LevelGeom& g = geom->lv[level];
-    const int p = slot - g.sel_off;
-    const int cnt = sel_count[b * L + level];
-    if (slot == 0 && lane == 0) {
+    const int slot = (warp_global - b * wpi) * 32 + lane;
+    if (slot == 0) {
         int tot = 0;
         for (int l = 0; l < L; ++l) tot += sel_count[b * L + l];
         counts_out[b] = min(tot, capacity);
     }
-    if (p >= cnt) return;
-    const int oidx = off + p;
-    if (oidx >= capacity) return;
-    const uint32_t c = sel_xys[(size_t)b * sel_total + slot];
-    const int kx = corner_x(c), ky = corner_y(c);
-    const uint8_t* uimg = args.lvl[level] + (size_t)b * g.img_bytes;
-    const uint8_t* bimg = args.blur[level] + (size_t)b * g.img_bytes;
-    const int pitch = g.pitch;
-
-    // ---- stage the blurred 51x51 patch: 2 rows per warp instruction, 15 aligned words per row ----
-    uint8_t* patch = s_patch[wib];
-    const int x0 = (kx - kPatchR) & ~3;                    // >= 0: keypoints lie >= 25 px inside the level
-    {
-        const int half = lane >> 4, w = lane & 15;
-        const uint32_t* gp = (const uint32_t*)(bimg + (size_t)(ky - kPatchR + half) * pitch + x0) + w;
-        uint32_t* sp = (uint32_t*)(patch + half * kPatchS) + w;
-        // all loads of a batch are issued before the first store (memory-level parallelism)
-#pragma unroll
-        for (int k0 = 0; k0 < 26; k0 += 13) {
-            uint32_t t[13];
-#pragma unroll
-            for (int k = 0; k < 13; ++k) {
-                const int r = half + 2 * (k0 + k);
-                t[k] = (w < 15 && r < 2 * kPatchR + 1) ? __ldg(gp + (size_t)(k0 + k) * (pitch / 2)) : 0u;
-            }
-#pragma unroll
-            for (int k = 0; k < 13; ++k) {
-                const int r = half + 2 * (k0 + k);
-                if (w < 15 && r < 2 * kPatchR + 1) sp[(k0 + k) * (2 * kPatchS / 4)] = t[k];
-            }
-        }
-    }
-    const int pofs = kPatchR * kPatchS + (kx - x0);        // patch byte offset of the keypoint itself
-
-    // ---- IC_Angle (ref :221-248): integer moments over the 845-pixel disc, lane = column u = lane-16 (+ u = 16) ----
-    int m10 = 0, m01 = 0;
-    {
-        // The 33 x 33 neighbourhood of the UNBLURRED level is copied with aligned word loads (3 rows x 10 words per warp
-        // instruction) into this warp's slice of the parking buffer, which tier 1 only uses later; the moments are then summed from
-        // shared memory with compile-time offsets: row pairs +-k share one disc test, m01 += k (val(+k) - val(-k)).
-        constexpr int kIcS = 40;                            // bytes per staged row: 4-byte aligned start + 33 columns
-        uint8_t* ic = reinterpret_cast<uint8_t*>(s_park_dyn + wib * (PPL * 32));
-        const int xs = (kx - kHalfPatch) & ~3;              // >= 0: keypoints lie >= 25 px inside the level
-        {
-            const int rr = lane / 10, w = lane - rr * 10;
-            const uint32_t* gp = (const uint32_t*)(uimg + (size_t)(ky - kHalfPatch + rr) * pitch + xs) + w;
-            uint32_t* sp = (uint32_t*)(ic + rr * kIcS) + w;
-            uint32_t t[11];
-#pragma unroll
-            for (int k = 0; k < 11; ++k) t[k] = (lane < 30) ? __ldg(gp + (size_t)k * 3 * (pitch / 4)) : 0u;
-#pragma unroll
-            for (int k = 0; k < 11; ++k) if (lane < 30) sp[k * 3 * (kIcS / 4)] = t[k];
-        }
-        __syncwarp();
-        const int u = lane - kHalfPatch;                    // -16 .. 15
-        const int au = u < 0 ? -u : u;
-        const int vm = c_disc_u[au];                        // |v| <= vmax(|u|) = umax[|u|]: the disc is symmetric (ref :187-202)
-        const uint8_t* col = ic + kHalfPatch * kIcS + (kx - kHalfPatch - xs) + lane;
-        int sum = col[0];
-#pragma unroll
-        for (int k = 1; k <= kHalfPatch; ++k) {
-            const int a = col[k * kIcS], bb = col[-k * kIcS];
-            if (vm >= k) { sum += a + bb; m01 += k * (a - bb); }
-        }
-        m10 = u * sum;
-        const int um = c_disc_u[kHalfPatch];
-        if (lane < 2 * um + 1) {                            // column u = +16: rows |v| <= umax[16]
-            const int v = lane - um;
-            const int val = ic[(kHalfPatch + v) * kIcS + (kx - kHalfPatch - xs) + 2 * kHalfPatch];
-            m10 += kHalfPatch * val;
-            m01 += v * val;
-        }
-#pragma unroll
-        for (int o = 16; o; o >>= 1) {
-            m10 += __shfl_xor_sync(0xffffffffu, m10, o);
-            m01 += __shfl_xor_sync(0xffffffffu, m01, o);
-        }
-        __syncwarp();                                       // the parking buffer is free again
-    }
-    const float angle = fast_atan2_deg((float)m01, (float)m10);
-
-    // Everything that is warp-uniform and only needed again in the rare paths or at the very end is parked in this warp's context in
-    // shared memory instead of living in registers across the pattern loops: at 80 registers (6 CTAs per SM) the compiler otherwise
-    // spills the INVARIANTS OF THE HOT LOOPS, and with 212 KB of the SM's 256 KB configured as shared memory those reloads miss the
-    // small L1, and the kernel then waits on local-memory loads.
-    WarpCtx& cx = s_ctx[wib];
+    int level = 0, off = 0;
+    for (int l = 0; l < L; ++l)
+        if (slot >= geom->lv[l].sel_off) level = l;
+    for (int l = 0; l < level; ++l) off += sel_count[b * L + l];
+    const int p = slot - geom->lv[level].sel_off;
+    const bool valid = slot < sel_total && p < sel_count[b * L + level] && off + p < capacity;
+    const unsigned vmask = __ballot_sync(0xffffffffu, valid);
+    if (vmask == 0u) return;
+    const int nk = __popc(vmask);                               // keypoints of the batch, compacted to kp[0 .. nk)
+    KpCtx* kp = s_kp[wib];
     const int ci = cam_of_image[b];
     const bool masks = geom->learn_masks != 0, dbrief = geom->do_dbrief != 0 || masks;
     const int npat = masks ? 3 : 1;
-    {
-        double a0, s0, c0;
-        if (masks) a0 = (double)__fdiv_rn(angle, 57.2957763671875f);              // angle / RHOf      (ref :425)
-        else a0 = (double)__fmul_rn(angle, 0.01745329238474369f);                   // angle * DEG2RADf  (ref :313,367)
-        sincos(a0, &s0, &c0);
-        if (lane == 0) {
-            cx.kx = kx; cx.ky = ky; cx.oidx = oidx; cx.b = b; cx.level = level; cx.c = c; cx.angle = angle; cx.a_base = a0;
-            // angle +- 20 deg (20 / RHOd, ref :424) by the addition theorems (1e-16 away from cos/sin(a0 +- rot); the exact path uses
-            // the reference's own cos(angle +- rot) / sin(angle +- rot))
-            const double c20 = 0.93969262078590838405, s20 = 0.34202014332566873304;
-            cx.ca[0] = c0; cx.sa[0] = s0;
-            cx.ca[1] = fma(c0, c20, -s0 * s20); cx.sa[1] = fma(s0, c20, c0 * s20);
-            cx.ca[2] = fma(c0, c20, s0 * s20);  cx.sa[2] = fma(s0, c20, -c0 * s20);
-        }
-    }
-    constexpr int BPL = PPL / 16;                 // descriptor bytes per lane
-    unsigned v0[BPL], vdiff[BPL];                 // bits of the pattern at the keypoint's angle; bits that differ in a +-20 degree re-test
-#pragma unroll
-    for (int bb = 0; bb < BPL; ++bb) { v0[bb] = 0u; vdiff[bb] = 0u; }
-    auto put = [&](int qi, unsigned e /* byte bb in bits [8bb, 8bb+8) */) {
-#pragma unroll
-        for (int bb = 0; bb < BPL; ++bb) {
-            const unsigned v = (e >> (8 * bb)) & 0xFFu;
-            if (qi == 0) v0[bb] = v; else vdiff[bb] |= v ^ v0[bb];
-        }
-    };
-    __syncwarp();                                 // patch staged, context written
-    if (!dbrief) {
-        // ---- ORB: rotatePattern (ref :285-301) ----
-        const double ca0 = cx.ca[0], sa0 = cx.sa[0];
-        int ix[PPL], iy[PPL];
-        bool far = false;
-#pragma unroll
-        for (int j = 0; j < PPL; ++j) {
-            const float2 pp = s_patf[j * 32 + lane];
-            const double px = (double)pp.x, py = (double)pp.y;
-            ix[j] = __double2int_rn(px * ca0 - py * sa0);
-            iy[j] = __double2int_rn(px * sa0 + py * ca0);
-            far |= (unsigned)(ix[j] + kPatchR) > 2u * kPatchR || (unsigned)(iy[j] + kPatchR) > 2u * kPatchR;
-        }
-        if (__any_sync(0xffffffffu, far)) {
-            put(0, orb_pattern_global<PPL>(s_patf, ca0, sa0, lane, bimg, uimg, &g, kx, ky));
-        } else {
-            unsigned e = 0;
-#pragma unroll
-            for (int bb = 0; bb < BPL; ++bb) {
-#pragma unroll
-                for (int bit = 0; bit < 8; ++bit) {
-                    const int j0 = 16 * bb + 2 * bit;
-                    const int s0 = patch[pofs + iy[j0] * kPatchS + ix[j0]], s1 = patch[pofs + iy[j0 + 1] * kPatchS + ix[j0 + 1]];
-                    e |= (unsigned)(s0 < s1) << (8 * bb + bit);
-                }
-            }
-            put(0, e);
-        }
-    } else {
-        // ---- dBRIEF / mdBRIEF: rotateAndDistortPattern (ref :250-283) ----
-        if (lane < (int)(sizeof(mcs_ocam) / 8)) ((double*)&s_cam[wib])[lane] = ((const double*)&cams[ci])[lane];
-        __syncwarp();
-        const mcs_ocam& cam = s_cam[wib];
-        const bool lane_valid = (PPL == 32) || (lane < ds);      // descSize 16: lanes 16..31 own no byte
-        bool have_lut, t1, mform;
-        {
+    if (dbrief && lane < (int)(sizeof(mcs_ocam) / 8)) ((double*)&s_cam[wib])[lane] = ((const double*)&cams[ci])[lane];
+    __syncwarp();
+    const mcs_ocam& cam = s_cam[wib];
+
+    // ---- set-up, one keypoint per lane: corner, output index, undistortion, table row, tier-1 constants ----
+    if (valid) {
+        KpCtx& cx = kp[__popc(vmask & ((1u << lane) - 1u))];
+        const uint32_t c = sel_xys[(size_t)b * sel_total + slot];
+        const int kx = corner_x(c), ky = corner_y(c);
+        cx.c = c; cx.oidx = off + p; cx.level = level;
+        int flags = 0;
+        if (dbrief) {
             float q[kT1MCoef], K0f = 0.f, gkf = 0.f, s0f = 0.f, rk2f = 0.f, rkf = 0.f, auk = 0.f, avk = 0.f;
 #pragma unroll
             for (int k = 0; k < kT1MCoef; ++k) q[k] = 0.f;
             const DistortLut lut = luts[ci];
-            const float scale = g.scale;
+            const float scale = geom->lv[level].scale;
             double ukx, uky;   // undistortPointsOcam(pt.x*scale, pt.y*scale, a0)  (ref :1306-1317)
             cam_undistort(cam, (double)__fmul_rn((float)kx, scale), (double)__fmul_rn((float)ky, scale), cam.pol[0], ukx, uky);
             // the table row of this keypoint: centre i = rn(r_k); its polynomials are valid for every pattern point (|r - r_k| <= 21.3)
             const double rk = sqrt(ukx * ukx + uky * uky);
-            have_lut = rk < (double)(lut.n - 1);                  // false for NaN as well -> exact path
+            const bool have_lut = rk < (double)(lut.n - 1);       // false for NaN as well -> exact path
             const int ci_lut = have_lut ? __double2int_rn(rk) : 0;
             const double* row = lut.coef + (size_t)ci_lut * kLutStride;
-            if (lane == 0) { cx.ukx = ukx; cx.uky = uky; cx.row = row; }
-            // ---- tier-1 set-up (per keypoint, all lanes redundantly; ~25 FP64 instructions against 48 points x 3 patterns) ----
-            t1 = have_lut && rk >= kT1MinRadius && __ldg(row + 17) == 1.0;
-            mform = t1 && __ldg(row + 23) == 1.0;
+            cx.ukx = ukx; cx.uky = uky; cx.row = row;
+            // ---- tier-1 set-up ----
+            const bool t1 = have_lut && rk >= kT1MinRadius && __ldg(row + 17) == 1.0;
+            const bool mform = t1 && __ldg(row + 23) == 1.0;
+            flags = (have_lut ? kKpLut : 0) | (t1 ? kKpT1 : 0) | (mform ? kKpMForm : 0);
             if (mform) {
                 // m-form: t_k, K0 = t_k P(t_k), g_k = G(c_i) + K0 in double from the float coefficients the points will use
                 const float2 c01 = __ldg((const float2*)(row + 19)), c23 = __ldg((const float2*)(row + 20));
@@ -574,168 +463,324 @@ describe_kernel(const PyramidGeom* __restrict__ geom, const DescribeArgs args, c
                 rk2f = (float)(rk * rk); rkf = (float)rk;
                 auk = (float)(cam.c * ukx + cam.d * uky); avk = (float)(cam.e * ukx + uky);      // A X_k
             }
-            // the tier-1 constants go to the context as well: they are needed in pass 1 of every pattern only, and re-reading them
-            // there (four broadcast LDS.128) keeps 15 registers free across pass 2 and the rare-path calls
-            if (lane == 0) {
-                float4* tp = reinterpret_cast<float4*>(cx.t1);
-                tp[0] = make_float4(q[0], q[1], q[2], q[3]); tp[1] = make_float4(q[4], q[5], q[6], q[7]);
-                tp[2] = make_float4(K0f, gkf, s0f, rk2f);    tp[3] = make_float4(rkf, auk, avk, 0.f);
+            // pass 1 of every pattern re-reads them with four broadcast LDS.128
+            float4* tp = reinterpret_cast<float4*>(cx.t1);
+            tp[0] = make_float4(q[0], q[1], q[2], q[3]); tp[1] = make_float4(q[4], q[5], q[6], q[7]);
+            tp[2] = make_float4(K0f, gkf, s0f, rk2f);    tp[3].x = rkf; tp[3].y = auk; tp[3].z = avk;
+        }
+        cx.flags = flags;
+    }
+    __syncwarp();                                 // contexts of the batch complete
+
+    // ---- IC_Angle (ref :221-248): integer moments over the 845-pixel disc, lane = column u = lane-16 (+ u = 16) ----
+    // The 33 x 33 neighbourhoods of the UNBLURRED level of kIcBatch keypoints are copied with aligned word loads (3 rows x 10 words
+    // per warp instruction) into this warp's slice of the parking buffer, which tier 1 only uses later; the moments are then summed
+    // from shared memory with compile-time offsets: row pairs +-k share one disc test, m01 += k (val(+k) - val(-k)).  Lane k keeps
+    // the moments of keypoint k.
+    int my_m10 = 0, my_m01 = 0;
+    {
+        constexpr int kIcS = 40;                                // bytes per staged row: 4-byte aligned start + 33 columns
+        constexpr int kIcBytes = (2 * kHalfPatch + 1) * kIcS;
+        static_assert(kIcBatch * kIcBytes <= 16 * 32 * (int)sizeof(float2), "IC neighbourhoods exceed the parking slice");
+        uint8_t* icw = reinterpret_cast<uint8_t*>(s_park_dyn + wib * (PPL * 32));
+        const int rr = lane / 10, w = lane - rr * 10;
+        const int u = lane - kHalfPatch;                        // -16 .. 15
+        const int au = u < 0 ? -u : u;
+        const int vm = c_disc_u[au];                            // |v| <= vmax(|u|) = umax[|u|]: the disc is symmetric (ref :187-202)
+        const int um = c_disc_u[kHalfPatch];
+#pragma unroll 1
+        for (int k0 = 0; k0 < nk; k0 += kIcBatch) {
+            uint32_t t[kIcBatch][11];
+#pragma unroll
+            for (int e = 0; e < kIcBatch; ++e) {
+                const int k = min(k0 + e, nk - 1);
+                const uint32_t c = kp[k].c;
+                const int lv = kp[k].level, kx = corner_x(c), ky = corner_y(c);
+                const LevelGeom& g = geom->lv[lv];
+                const uint8_t* uimg = args.lvl[lv] + (size_t)b * g.img_bytes;
+                const int xs = (kx - kHalfPatch) & ~3;          // >= 0: keypoints lie >= 25 px inside the level
+                const uint32_t* gp = (const uint32_t*)(uimg + (size_t)(ky - kHalfPatch + rr) * g.pitch + xs) + w;
+#pragma unroll
+                for (int k = 0; k < 11; ++k) t[e][k] = (lane < 30) ? __ldg(gp + (size_t)k * 3 * (g.pitch / 4)) : 0u;
+            }
+#pragma unroll
+            for (int e = 0; e < kIcBatch; ++e) {
+                uint32_t* sp = (uint32_t*)(icw + e * kIcBytes + rr * kIcS) + w;
+#pragma unroll
+                for (int k = 0; k < 11; ++k) if (lane < 30) sp[k * 3 * (kIcS / 4)] = t[e][k];
+            }
+            __syncwarp();
+#pragma unroll
+            for (int e = 0; e < kIcBatch; ++e) {
+                if (k0 + e >= nk) break;
+                const int kx = corner_x(kp[k0 + e].c);
+                const int xo = kx - kHalfPatch - ((kx - kHalfPatch) & ~3);
+                const uint8_t* ic = icw + e * kIcBytes;
+                int m10 = 0, m01 = 0;
+                const uint8_t* col = ic + kHalfPatch * kIcS + xo + lane;
+                int sum = col[0];
+#pragma unroll
+                for (int k = 1; k <= kHalfPatch; ++k) {
+                    const int a = col[k * kIcS], bb = col[-k * kIcS];
+                    if (vm >= k) { sum += a + bb; m01 += k * (a - bb); }
+                }
+                m10 = u * sum;
+                if (lane < 2 * um + 1) {                        // column u = +16: rows |v| <= umax[16]
+                    const int v = lane - um;
+                    const int val = ic[(kHalfPatch + v) * kIcS + xo + 2 * kHalfPatch];
+                    m10 += kHalfPatch * val;
+                    m01 += v * val;
+                }
+#pragma unroll
+                for (int o = 16; o; o >>= 1) {
+                    m10 += __shfl_xor_sync(0xffffffffu, m10, o);
+                    m01 += __shfl_xor_sync(0xffffffffu, m01, o);
+                }
+                if (lane == k0 + e) { my_m10 = m10; my_m01 = m01; }
+            }
+            __syncwarp();                                       // the parking slice is free again
+        }
+    }
+    // ---- angle, one keypoint per lane; the keypoint record is complete here ----
+    if (lane < nk) {
+        KpCtx& cx = kp[lane];
+        const float angle = fast_atan2_deg((float)my_m01, (float)my_m10);
+        double s0, c0;
+        sincos(pattern_base_angle(angle, masks), &s0, &c0);
+        cx.t1[15] = angle; cx.c0 = c0; cx.s0 = s0;
+        const int lv = cx.level;
+        const LevelGeom& go = geom->lv[lv];
+        const float scale = go.scale;
+        mcs_keypoint k;
+        k.x = lv ? __fmul_rn((float)corner_x(cx.c), scale) : (float)corner_x(cx.c);      // pt *= scale for l > 0 (ref :1327-1332)
+        k.y = lv ? __fmul_rn((float)corner_y(cx.c), scale) : (float)corner_y(cx.c);
+        k.size = go.patch_size; k.angle = angle; k.response = (float)corner_s(cx.c);
+        k.octave = lv; k.class_id = -1;
+        kps_out[(size_t)b * capacity + cx.oidx] = k;
+    }
+    __syncwarp();
+
+    constexpr int BPL = PPL / 16;                 // descriptor bytes per lane
+    const bool lane_valid = (PPL == 32) || (lane < ds);      // descSize 16: lanes 16..31 own no byte
+    uint8_t* patch = s_patch[wib];
+    float2* park = s_park_dyn + wib * (PPL * 32);
+#pragma unroll 1
+    for (int kk = 0; kk < nk; ++kk) {
+        const KpCtx& cx = kp[kk];
+        const int kx = corner_x(cx.c), ky = corner_y(cx.c), level = cx.level;
+        const LevelGeom& g = geom->lv[level];
+        const uint8_t* uimg = args.lvl[level] + (size_t)b * g.img_bytes;
+        const uint8_t* bimg = args.blur[level] + (size_t)b * g.img_bytes;
+        const int pitch = g.pitch;
+
+        // ---- stage the blurred 51x51 patch: 2 rows per warp instruction, 15 aligned words per row ----
+        const int x0 = (kx - kPatchR) & ~3;                    // >= 0: keypoints lie >= 25 px inside the level
+        {
+            const int half = lane >> 4, w = lane & 15;
+            const uint32_t* gp = (const uint32_t*)(bimg + (size_t)(ky - kPatchR + half) * pitch + x0) + w;
+            uint32_t* sp = (uint32_t*)(patch + half * kPatchS) + w;
+            // all loads of a batch are issued before the first store (memory-level parallelism)
+#pragma unroll
+            for (int k0 = 0; k0 < 26; k0 += 13) {
+                uint32_t t[13];
+#pragma unroll
+                for (int k = 0; k < 13; ++k) {
+                    const int r = half + 2 * (k0 + k);
+                    t[k] = (w < 15 && r < 2 * kPatchR + 1) ? __ldg(gp + (size_t)(k0 + k) * (pitch / 2)) : 0u;
+                }
+#pragma unroll
+                for (int k = 0; k < 13; ++k) {
+                    const int r = half + 2 * (k0 + k);
+                    if (w < 15 && r < 2 * kPatchR + 1) sp[(k0 + k) * (2 * kPatchS / 4)] = t[k];
+                }
             }
         }
-        __syncwarp();                             // context complete
-#pragma unroll 1                         // one copy of the pattern body: the kernel has to fit the instruction cache
-        for (int qi = 0; qi < npat; ++qi) {
-            bool done = false;
-            float2* park = s_park_dyn + wib * (PPL * 32);
-            if (t1) {
-                // ---- tier 1: fp32, relative to the keypoint (see the header) ----
-                // rotation folded into per-pattern constants (double -> float once): with p the pattern point and d = Rot p,
-                //   n = r^2 - r_k^2 = |p|^2 + 2 (Rot^T X_k).p            (|d| = |p|: no rotated point needed for n)
-                //   u - u_k = g (A Rot p).x + dg (A X_k).x               (A = affine part [c d; e 1])
-                float nx, ny, axx, axy, ayx, ayy;
-                {
-                    const double caq = cx.ca[qi], saq = cx.sa[qi], ukx = cx.ukx, uky = cx.uky;
-                    nx = (float)(2.0 * (ukx * caq + uky * saq)); ny = (float)(2.0 * (uky * caq - ukx * saq));
-                    axx = (float)(cam.c * caq + cam.d * saq); axy = (float)(cam.d * caq - cam.c * saq);
-                    ayx = (float)(cam.e * caq + saq); ayy = (float)(caq - cam.e * saq);
+        const int pofs = kPatchR * kPatchS + (kx - x0);        // patch byte offset of the keypoint itself
+
+        unsigned v0[BPL], vdiff[BPL];                 // bits of the pattern at the keypoint's angle; bits that differ in a +-20 degree re-test
+#pragma unroll
+        for (int bb = 0; bb < BPL; ++bb) { v0[bb] = 0u; vdiff[bb] = 0u; }
+        auto put = [&](int qi, unsigned e /* byte bb in bits [8bb, 8bb+8) */) {
+#pragma unroll
+            for (int bb = 0; bb < BPL; ++bb) {
+                const unsigned v = (e >> (8 * bb)) & 0xFFu;
+                if (qi == 0) v0[bb] = v; else vdiff[bb] |= v ^ v0[bb];
+            }
+        };
+        __syncwarp();                                 // patch staged
+        if (!dbrief) {
+            // ---- ORB: rotatePattern (ref :285-301) ----
+            const double ca0 = cx.c0, sa0 = cx.s0;
+            int ix[PPL], iy[PPL];
+            bool far = false;
+#pragma unroll
+            for (int j = 0; j < PPL; ++j) {
+                const float2 pp = s_patf[j * 32 + lane];
+                const double px = (double)pp.x, py = (double)pp.y;
+                ix[j] = __double2int_rn(px * ca0 - py * sa0);
+                iy[j] = __double2int_rn(px * sa0 + py * ca0);
+                far |= (unsigned)(ix[j] + kPatchR) > 2u * kPatchR || (unsigned)(iy[j] + kPatchR) > 2u * kPatchR;
+            }
+            if (__any_sync(0xffffffffu, far)) {
+                put(0, orb_pattern_global<PPL>(s_patf, ca0, sa0, lane, bimg, uimg, &g, kx, ky));
+            } else {
+                unsigned e = 0;
+#pragma unroll
+                for (int bb = 0; bb < BPL; ++bb) {
+#pragma unroll
+                    for (int bit = 0; bit < 8; ++bit) {
+                        const int j0 = 16 * bb + 2 * bit;
+                        const int s0 = patch[pofs + iy[j0] * kPatchS + ix[j0]], s1 = patch[pofs + iy[j0 + 1] * kPatchS + ix[j0 + 1]];
+                        e |= (unsigned)(s0 < s1) << (8 * bb + bit);
+                    }
                 }
-                float su = 0.f, sv = 0.f;
-                {
-                const float4* tp = reinterpret_cast<const float4*>(cx.t1);
-                const float4 tA = tp[0], tB = tp[1], tC = tp[2], tD = tp[3];
-                const float q[kT1MCoef] = {tA.x, tA.y, tA.z, tA.w, tB.x, tB.y, tB.z, tB.w};
-                const float K0f = tC.x, gkf = tC.y, s0f = tC.z, rk2f = tC.w, rkf = tD.x, auk = tD.y, avk = tD.z;
-                if (mform) {
+                put(0, e);
+            }
+        } else {
+            // ---- dBRIEF / mdBRIEF: rotateAndDistortPattern (ref :250-283) ----
+            const int flags = cx.flags;
+            const bool have_lut = (flags & kKpLut) != 0, t1 = (flags & kKpT1) != 0, mform = (flags & kKpMForm) != 0;
+#pragma unroll 1                         // one copy of the pattern body: the kernel has to fit the instruction cache
+            for (int qi = 0; qi < npat; ++qi) {
+                bool done = false;
+                double caq, saq;
+                pattern_rotation(cx.c0, cx.s0, qi, caq, saq);
+                if (t1) {
+                    // ---- tier 1: fp32, relative to the keypoint (see the header) ----
+                    // rotation folded into per-pattern constants (double -> float once): with p the pattern point and d = Rot p,
+                    //   n = r^2 - r_k^2 = |p|^2 + 2 (Rot^T X_k).p            (|d| = |p|: no rotated point needed for n)
+                    //   u - u_k = g (A Rot p).x + dg (A X_k).x               (A = affine part [c d; e 1])
+                    float nx, ny, axx, axy, ayx, ayy;
+                    {
+                        const double ukx = cx.ukx, uky = cx.uky;
+                        nx = (float)(2.0 * (ukx * caq + uky * saq)); ny = (float)(2.0 * (uky * caq - ukx * saq));
+                        axx = (float)(cam.c * caq + cam.d * saq); axy = (float)(cam.d * caq - cam.c * saq);
+                        ayx = (float)(cam.e * caq + saq); ayy = (float)(caq - cam.e * saq);
+                    }
+                    float su = 0.f, sv = 0.f;
+                    {
+                    const float4* tp = reinterpret_cast<const float4*>(cx.t1);
+                    const float4 tA = tp[0], tB = tp[1], tC = tp[2], tD = tp[3];
+                    const float q[kT1MCoef] = {tA.x, tA.y, tA.z, tA.w, tB.x, tB.y, tB.z, tB.w};
+                    const float K0f = tC.x, gkf = tC.y, s0f = tC.z, rk2f = tC.w, rkf = tD.x, auk = tD.y, avk = tD.z;
+                    if (mform) {
 #pragma unroll kT1Unroll1
+                        for (int j = 0; j < PPL; ++j) {
+                            const float2 pp = s_patf[j * 32 + lane];
+                            const float n = fmaf(pp.x, nx, fmaf(pp.y, ny, fmaf(pp.x, pp.x, pp.y * pp.y)));   // m - m_k
+                            const float t = fmaf(n, rk2f, s0f);                       // (m - c_i) / hw_i
+                            float pl = q[kT1MCoef - 1];
+#pragma unroll
+                            for (int k = kT1MCoef - 2; k >= 0; --k) pl = fmaf(pl, t, q[k]);
+                            const float dg = fmaf(t, pl, -K0f);                        // g(r) - g(r_k)
+                            const float g = gkf + dg;
+                            const float du = fmaf(g, fmaf(pp.x, axx, pp.y * axy), dg * auk);   // u - u_k
+                            const float dv = fmaf(g, fmaf(pp.x, ayx, pp.y * ayy), dg * avk);   // v - v_k
+                            park[j * 32 + lane] = make_float2(du, dv);
+                            if (lane_valid) { su += du; sv += dv; }
+                        }
+                    } else
+#pragma unroll 4
                     for (int j = 0; j < PPL; ++j) {
                         const float2 pp = s_patf[j * 32 + lane];
-                        const float n = fmaf(pp.x, nx, fmaf(pp.y, ny, fmaf(pp.x, pp.x, pp.y * pp.y)));   // m - m_k
-                        const float t = fmaf(n, rk2f, s0f);                       // (m - c_i) / hw_i
-                        float pl = q[kT1MCoef - 1];
-#pragma unroll
-                        for (int k = kT1MCoef - 2; k >= 0; --k) pl = fmaf(pl, t, q[k]);
-                        const float dg = fmaf(t, pl, -K0f);                        // g(r) - g(r_k)
+                        const float n = fmaf(pp.x, nx, fmaf(pp.y, ny, fmaf(pp.x, pp.x, pp.y * pp.y)));
+                        const float r2 = rk2f + n;
+                        float y, z;
+                        asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(r2));   // MUFU + one Newton step each: ~1 ulp
+                        y = fmaf(0.5f * y, fmaf(-r2 * y, y, 1.f), y);              // 1 / r
+                        const float w = fmaf(r2, y, rkf);                          // r + r_k
+                        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(z) : "f"(w));
+                        z = fmaf(z, fmaf(-w, z, 1.f), z);
+                        const float delta = n * z;                                 // r - r_k without cancellation
+                        const float sp = fmaf(delta, 1.f / kT1Scale, s0f);
+                        float pl = q[5];
+                        pl = fmaf(pl, sp, q[4]); pl = fmaf(pl, sp, q[3]); pl = fmaf(pl, sp, q[2]);
+                        pl = fmaf(pl, sp, q[1]); pl = fmaf(pl, sp, q[0]);
+                        const float dg = fmaf(sp, pl, -K0f) * y;                   // g(r) - g(r_k)
                         const float g = gkf + dg;
                         const float du = fmaf(g, fmaf(pp.x, axx, pp.y * axy), dg * auk);   // u - u_k
                         const float dv = fmaf(g, fmaf(pp.x, ayx, pp.y * ayy), dg * avk);   // v - v_k
                         park[j * 32 + lane] = make_float2(du, dv);
                         if (lane_valid) { su += du; sv += dv; }
                     }
-                } else
-#pragma unroll 4
-                for (int j = 0; j < PPL; ++j) {
-                    const float2 pp = s_patf[j * 32 + lane];
-                    const float n = fmaf(pp.x, nx, fmaf(pp.y, ny, fmaf(pp.x, pp.x, pp.y * pp.y)));
-                    const float r2 = rk2f + n;
-                    float y, z;
-                    asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(r2));   // MUFU + one Newton step each: ~1 ulp
-                    y = fmaf(0.5f * y, fmaf(-r2 * y, y, 1.f), y);              // 1 / r
-                    const float w = fmaf(r2, y, rkf);                          // r + r_k
-                    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(z) : "f"(w));
-                    z = fmaf(z, fmaf(-w, z, 1.f), z);
-                    const float delta = n * z;                                 // r - r_k without cancellation
-                    const float sp = fmaf(delta, 1.f / kT1Scale, s0f);
-                    float pl = q[5];
-                    pl = fmaf(pl, sp, q[4]); pl = fmaf(pl, sp, q[3]); pl = fmaf(pl, sp, q[2]);
-                    pl = fmaf(pl, sp, q[1]); pl = fmaf(pl, sp, q[0]);
-                    const float dg = fmaf(sp, pl, -K0f) * y;                   // g(r) - g(r_k)
-                    const float g = gkf + dg;
-                    const float du = fmaf(g, fmaf(pp.x, axx, pp.y * axy), dg * auk);   // u - u_k
-                    const float dv = fmaf(g, fmaf(pp.x, ayx, pp.y * ayy), dg * avk);   // v - v_k
-                    park[j * 32 + lane] = make_float2(du, dv);
-                    if (lane_valid) { su += du; sv += dv; }
-                }
-                }
-                // mean over the 16*ds points: lane partial sums in fp32 (16..32 terms)
-                const double inv_n = 1.0 / (double)(16 * ds);
-                // ... and the warp sum as ONE integer REDUX per coordinate in 2^-17 px fixed point: a lane's rounding is <= 3.8e-6 px,
-                // the mean is off by <= 32 * 3.8e-6 / 512 = 2.4e-7 px (inside the tier-1 error budget, kT1Guard).  A lane sum of 500 px
-                // or more (or a NaN) cannot come from a sane pattern (|du| <= ~22 px) and sends the pattern on, so the 32-bit sum
-                // (< 32 * 500 * 2^17 = 2^31) never wraps.
-                bool flag = !(fabsf(su) < 500.f) | !(fabsf(sv) < 500.f);
-                const int iu = __reduce_add_sync(0xffffffffu, flag ? 0 : __float2int_rn(su * 131072.f));
-                const int iv = __reduce_add_sync(0xffffffffu, flag ? 0 : __float2int_rn(sv * 131072.f));
-                const float mu = (float)((double)iu * (inv_n * (1.0 / 131072.0))), mv = (float)((double)iv * (inv_n * (1.0 / 131072.0)));
-                float wf = 0.f, wt = 0.f;                                      // running maxima of |fraction - tie| and |offset|
-                constexpr float kMagicF = 12582912.f;                          // 1.5 * 2^23: t + magic rounds t to the nearest even integer
-                unsigned bits = 0;                                             // descriptor byte(s) of this lane: points 0..15 | 16..31 << 8
+                    }
+                    // mean over the 16*ds points: lane partial sums in fp32 (16..32 terms)
+                    const double inv_n = 1.0 / (double)(16 * ds);
+                    // ... and the warp sum as ONE integer REDUX per coordinate in 2^-17 px fixed point: a lane's rounding is <= 3.8e-6 px,
+                    // the mean is off by <= 32 * 3.8e-6 / 512 = 2.4e-7 px (inside the tier-1 error budget, kT1Guard).  A lane sum of 500 px
+                    // or more (or a NaN) cannot come from a sane pattern (|du| <= ~22 px) and sends the pattern on, so the 32-bit sum
+                    // (< 32 * 500 * 2^17 = 2^31) never wraps.
+                    bool flag = !(fabsf(su) < 500.f) | !(fabsf(sv) < 500.f);
+                    const int iu = __reduce_add_sync(0xffffffffu, flag ? 0 : __float2int_rn(su * 131072.f));
+                    const int iv = __reduce_add_sync(0xffffffffu, flag ? 0 : __float2int_rn(sv * 131072.f));
+                    const float mu = (float)((double)iu * (inv_n * (1.0 / 131072.0))), mv = (float)((double)iv * (inv_n * (1.0 / 131072.0)));
+                    float wf = 0.f, wt = 0.f;                                      // running maxima of |fraction - tie| and |offset|
+                    constexpr float kMagicF = 12582912.f;                          // 1.5 * 2^23: t + magic rounds t to the nearest even integer
+                    unsigned bits = 0;                                             // descriptor byte(s) of this lane: points 0..15 | 16..31 << 8
 #pragma unroll kT1Unroll2
-                for (int j = 0; j < PPL; j += 2) {
-                    int smp[2];
+                    for (int j = 0; j < PPL; j += 2) {
+                        int smp[2];
 #pragma unroll
-                    for (int e2 = 0; e2 < 2; ++e2) {
-                        const float2 c = park[(j + e2) * 32 + lane];           // this lane's own slot: no synchronisation needed
-                        const float tu = c.x - mu, tv = c.y - mv;
-                        const float mu_r = tu + kMagicF, mv_r = tv + kMagicF;
-                        const float fu = tu - (mu_r - kMagicF), fv = tv - (mv_r - kMagicF);
-                        // near a rounding tie, or outside the staged patch: running maxima, tested once after the loop (a NaN
-                        // coordinate has already flagged the pattern through its lane sum)
-                        wf = fmaxf(wf, fmaxf(fabsf(fu), fabsf(fv)));
-                        wt = fmaxf(wt, fmaxf(fabsf(tu), fabsf(tv)));
-                        const int ix = __float_as_int(mu_r) - 0x4B400000, iy = __float_as_int(mv_r) - 0x4B400000;
-                        // one clamp of the byte offset keeps the read inside the patch array; an offset that needed it belongs to a
-                        // flagged coordinate (|t| >= 25.4) and the pattern is redone
-                        const int ofs = min(max(iy * kPatchS + ix, -(kPatchR * kPatchS + kPatchR)), kPatchR * kPatchS + kPatchR);
-                        smp[e2] = patch[pofs + ofs];
+                        for (int e2 = 0; e2 < 2; ++e2) {
+                            const float2 c = park[(j + e2) * 32 + lane];           // this lane's own slot: no synchronisation needed
+                            const float tu = c.x - mu, tv = c.y - mv;
+                            const float mu_r = tu + kMagicF, mv_r = tv + kMagicF;
+                            const float fu = tu - (mu_r - kMagicF), fv = tv - (mv_r - kMagicF);
+                            // near a rounding tie, or outside the staged patch: running maxima, tested once after the loop (a NaN
+                            // coordinate has already flagged the pattern through its lane sum)
+                            wf = fmaxf(wf, fmaxf(fabsf(fu), fabsf(fv)));
+                            wt = fmaxf(wt, fmaxf(fabsf(tu), fabsf(tv)));
+                            const int ix = __float_as_int(mu_r) - 0x4B400000, iy = __float_as_int(mv_r) - 0x4B400000;
+                            // one clamp of the byte offset keeps the read inside the patch array; an offset that needed it belongs to a
+                            // flagged coordinate (|t| >= 25.4) and the pattern is redone
+                            const int ofs = min(max(iy * kPatchS + ix, -(kPatchR * kPatchS + kPatchR)), kPatchR * kPatchS + kPatchR);
+                            smp[e2] = patch[pofs + ofs];
+                        }
+                        bits |= (unsigned)(smp[0] < smp[1]) << (j >> 1);          // point pair j/2: bits 0..7 = byte 0, 8..15 = byte 1
                     }
-                    bits |= (unsigned)(smp[0] < smp[1]) << (j >> 1);          // point pair j/2: bits 0..7 = byte 0, 8..15 = byte 1
-                }
-                flag |= !(wf < 0.5f - kT1Guard) | !(wt < (float)kPatchR + 0.4f);
-                if (!__any_sync(0xffffffffu, flag && lane_valid)) {
-                    put(qi, bits);
-                    done = true;
-                    if (args.tier_stats && lane == 0) atomicAdd(args.tier_stats, 1ull);
-                } else {
-                    int fail = 0;
-                    const unsigned e = tier1_repair<PPL>(&cam, s_patf, park, cx.row, cx.ca[qi], cx.sa[qi], cx.ukx, cx.uky, lane, ds, patch, pofs, &fail);
-                    if (!__any_sync(0xffffffffu, fail != 0)) {
-                        put(qi, e);
+                    flag |= !(wf < 0.5f - kT1Guard) | !(wt < (float)kPatchR + 0.4f);
+                    if (!__any_sync(0xffffffffu, flag && lane_valid)) {
+                        put(qi, bits);
                         done = true;
-                        if (args.tier_stats && lane == 0) atomicAdd(args.tier_stats + 1, 1ull);
+                        if (args.tier_stats && lane == 0) atomicAdd(args.tier_stats, 1ull);
+                    } else {
+                        int fail = 0;
+                        const unsigned e = tier1_repair<PPL>(&cam, s_patf, park, cx.row, caq, saq, cx.ukx, cx.uky, lane, ds, patch, pofs, &fail);
+                        if (!__any_sync(0xffffffffu, fail != 0)) {
+                            put(qi, e);
+                            done = true;
+                            if (args.tier_stats && lane == 0) atomicAdd(args.tier_stats + 1, 1ull);
+                        }
                     }
                 }
-            }
-            if (!done) {
-                // ---- tier 2 (FP64 polynomial), then tier 3 (exact) where tier 2 cannot decide ----
-                unsigned e = 0;
-                int need_exact = have_lut ? 0 : 1;
-                if (have_lut) e = tier2_pattern<PPL>(&cam, s_patf, cx.row, cx.ca[qi], cx.sa[qi], cx.ukx, cx.uky, lane, ds, patch, pofs, &need_exact);
-                const bool exact = __any_sync(0xffffffffu, need_exact != 0);
-                if (exact) {
-                    const double rot = 20.0 / (180.0 / 3.1415926535897932384626433832795);      // 20 / RHOd         (ref :424)
-                    const double aq = qi == 0 ? cx.a_base : (qi == 1 ? cx.a_base + rot : cx.a_base - rot);
-                    const int lv = cx.level, bq = cx.b;
-                    const LevelGeom& gq = geom->lv[lv];
-                    e = exact_pattern<PPL>(&cam, s_patf, aq, cx.ukx, cx.uky, lane, ds, args.blur[lv] + (size_t)bq * gq.img_bytes,
-                                           args.lvl[lv] + (size_t)bq * gq.img_bytes, &gq, cx.kx, cx.ky);
+                if (!done) {
+                    // ---- tier 2 (FP64 polynomial), then tier 3 (exact) where tier 2 cannot decide ----
+                    unsigned e = 0;
+                    int need_exact = have_lut ? 0 : 1;
+                    if (have_lut) e = tier2_pattern<PPL>(&cam, s_patf, cx.row, caq, saq, cx.ukx, cx.uky, lane, ds, patch, pofs, &need_exact);
+                    const bool exact = __any_sync(0xffffffffu, need_exact != 0);
+                    if (exact) {
+                        const double rot = 20.0 / (180.0 / 3.1415926535897932384626433832795);      // 20 / RHOd         (ref :424)
+                        const double a0 = pattern_base_angle(cx.t1[15], masks);
+                        const double aq = qi == 0 ? a0 : (qi == 1 ? a0 + rot : a0 - rot);
+                        e = exact_pattern<PPL>(&cam, s_patf, aq, cx.ukx, cx.uky, lane, ds, bimg, uimg, &g, kx, ky);
+                    }
+                    if (args.tier_stats && lane == 0) atomicAdd(args.tier_stats + (exact ? 3 : 2), 1ull);
+                    put(qi, e);
                 }
-                if (args.tier_stats && lane == 0) atomicAdd(args.tier_stats + (exact ? 3 : 2), 1ull);
-                put(qi, e);
             }
         }
-    }
-    {
-        const int bo = cx.b, oo = cx.oidx;
+        const size_t ob = ((size_t)b * capacity + cx.oidx) * ds;
 #pragma unroll
         for (int bb = 0; bb < BPL; ++bb) {
             const int byte = lane + 32 * bb;
             if (byte < ds) {
-                desc_out[((size_t)bo * capacity + oo) * ds + byte] = (uint8_t)v0[bb];
+                desc_out[ob + byte] = (uint8_t)v0[bb];
                 // stable bit <=> both +-20 degree re-tests agree with the bit (ref :449-451 ...)
-                if (dmask_out) dmask_out[((size_t)bo * capacity + oo) * ds + byte] = (uint8_t)(masks ? (~vdiff[bb] & 0xFFu) : 0u);
+                if (dmask_out) dmask_out[ob + byte] = (uint8_t)(masks ? (~vdiff[bb] & 0xFFu) : 0u);
             }
         }
-        if (lane == 0) {
-            const int lv = cx.level, kxo = cx.kx, kyo = cx.ky;
-            const LevelGeom& go = geom->lv[lv];
-            const float scale = go.scale;
-            mcs_keypoint k;
-            k.x = lv ? __fmul_rn((float)kxo, scale) : (float)kxo;      // pt *= scale for l > 0 (ref :1327-1332)
-            k.y = lv ? __fmul_rn((float)kyo, scale) : (float)kyo;
-            k.size = go.patch_size; k.angle = cx.angle; k.response = (float)corner_s(cx.c);
-            k.octave = lv; k.class_id = -1;
-            kps_out[(size_t)bo * capacity + oo] = k;
-        }
+        __syncwarp();                                 // the patch is read by every lane before the next keypoint overwrites it
     }
 }
 
@@ -920,15 +965,15 @@ cudaError_t launch_describe(const PyramidGeom& G, const PyramidGeom* G_dev, int 
                             const mcs_ocam* cams, const DistortLut* luts, const int* cam_of_image, const uint32_t* sel_xys,
                             const int* sel_count, mcs_keypoint* kps, uint8_t* desc, uint8_t* dmask, int* counts, int capacity,
                             cudaStream_t st) {
-    const long long warps = (long long)n_images * G.sel_total;
+    const long long warps = (long long)n_images * ((G.sel_total + 31) / 32);      // a warp per 32 selected slots of an image
     const int blocks = (int)std::max<long long>(1, (warps + kDescWarps - 1) / kDescWarps);
-    // 96 registers, 5 CTAs of 4 warps per SM (kDescMinBlocks, measured against 4 and 6 there); the warp context in shared memory keeps
-    // the hot-loop invariants out of the spilled set
+    // 4 CTAs of 4 warps per SM (kDescMinBlocks); static shared memory (34 KB / 38 KB with the keypoint contexts) + the parked
+    // coordinates (16 KB / 32 KB) is above the 48 KB default for both instantiations
     const size_t park16 = (size_t)kDescWarps * 16 * 32 * sizeof(float2), park32 = 2 * park16;
-    if (G.desc_size > 32) {        // static 23 KB + 32 KB parked coordinates: above the 48 KB default
-        cudaError_t e = cudaFuncSetAttribute(describe_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)park32);
-        if (e != cudaSuccess) return e;
-    }
+    cudaError_t e = G.desc_size <= 32
+        ? cudaFuncSetAttribute(describe_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)park16)
+        : cudaFuncSetAttribute(describe_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)park32);
+    if (e != cudaSuccess) return e;
     if (G.desc_size <= 32)
         describe_kernel<16><<<blocks, kDescWarps * 32, park16, st>>>(G_dev, args, cams, luts, cam_of_image, sel_xys, sel_count, kps, desc,
                                                                dmask, counts, capacity, n_images);
