@@ -206,6 +206,8 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
         g.n_cols = (int)(width / 30.0); g.n_rows = (int)(height / 30.0);
         if (g.n_cols < 1 || g.n_rows < 1) return fail(MCS_ERR_UNSUPPORTED, "level too small for the 30 px cell grid");
         g.w_cell = (int)std::ceil(width / g.n_cols); g.h_cell = (int)std::ceil(height / g.n_rows);
+        // K1 sizes its per-warp corner segments for tile rows that cross at most 3 cell edges (kWarpCorners)
+        if (g.w_cell < 30) return fail(MCS_ERR_UNSUPPORTED, "FAST cells narrower than 30 px");
         if ((long long)g.n_cols * g.n_rows * g.w_cell * g.h_cell >= (1 << 24))
             return fail(MCS_ERR_UNSUPPORTED, "cell-order key overflow");
         for (int i = 0; i < g.n_rows; ++i) {
@@ -229,7 +231,18 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
         g.hX = (double)(maxBX - minB) / g.nodes_ini;
         g.sel_cap = std::max(g.quota + 3, 4 * g.nodes_ini);
         g.sel_off = sel_off; sel_off += g.sel_cap;
-        g.raw_cap = ((g.w - 2 * kEdge + 1) / 2 + 1) * ((g.h - 2 * kEdge + 1) / 2 + 1);
+        // raw corner capacity: a cell of w_c x h_c pixels holds at most ceil(w_c / 2) * ceil(h_c / 2) strict maxima (one per 2x2
+        // block, the per-cell NMS does not look across cells); the cells form a grid, so the sum over the cells factors per axis
+        auto half_cells = [](const std::vector<int16_t>& cell) {
+            int s = 0, run = 0;
+            for (size_t i = 0; i <= cell.size(); ++i) {
+                if (i < cell.size() && cell[i] >= 0 && (run == 0 || cell[i] == cell[i - 1])) { ++run; continue; }
+                s += (run + 1) / 2;
+                run = (i < cell.size() && cell[i] >= 0) ? 1 : 0;
+            }
+            return s;
+        };
+        g.raw_cap = half_cells(cellx) * half_cells(celly);
         g.raw_off = raw_off; raw_off += (size_t)((g.raw_cap + 3) & ~3);
         auto put = [&](const std::vector<int16_t>& v) { size_t o = blob.size(); blob.insert(blob.end(), v.begin(), v.end()); while (blob.size() & 7) blob.push_back(0); return o; };
         off[l] = {put(xofs), put(xa0), put(xa1), put(yofs), put(yb0), put(yb1), put(cellx), put(celly), put(mx), put(my)};

@@ -57,7 +57,11 @@ constexpr int kSrcWB = 176;                 // staged source row stride (bytes, 
 constexpr int kT8S = 80;                    // byte tile row stride
 constexpr int kT16S = 72;                   // 16-bit tile row stride (elements)
 constexpr int kScoreS = 68;                 // score tile row stride in 16-bit elements (66 used)
-constexpr int kWarpCorners = (kTH / (kThreads / 32)) * (kTW / 2);   // a warp owns kTH/8 rows; strict 3x3 maxima are never adjacent in a row
+// corner slots per warp: a warp owns kTH/8 tile rows.  Inside a FAST cell two strict 3x3 maxima are never adjacent in a row, but the
+// NMS counts a neighbour in another cell as 0, so the last pixel of a cell and the first of the next can both be maxima.  Cells are
+// at least 30 px wide (nCols = int(width / 30), checked by build_geometry), so a 64-px row meets at most 4 cells and holds at most
+// sum ceil(piece / 2) <= (64 + 4) / 2 = 34 maxima (tests/test_k1_bounds_cpu.py runs every level width)
+constexpr int kWarpCorners = (kTH / (kThreads / 32)) * (kTW / 2 + 2);
 
 __device__ __forceinline__ unsigned vneg2(unsigned a) { return __vadd2(~a, 0x00010001u); }
 

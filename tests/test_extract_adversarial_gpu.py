@@ -1,0 +1,316 @@
+"""GPU parity of the front of the extractor (K1 pyr_fast_kernel, K2 octree_kernel) on adversarial images: dense dot lattices that
+put strict per-cell maxima on both sides of FAST cell boundaries, lattices of equal responses, contrasts at the FAST threshold,
+saturated patterns, symmetric blobs and striped masks.  Natural-looking frames never come near these cases: corners there are
+sparse, responses spread out, and no 64-pixel tile row holds more than a handful of maxima.
+
+Every case compares every stage with the CPU oracle bit for bit (levels, blurred levels, masks, raw corners, keypoints including the
+IC angle bits, descriptors and descriptor masks); extract_batch raises on any capacity status of the kernels.  Each family also
+checks on the oracle's output that its images reach the edge they are built for, so that a change of a generator cannot quietly
+turn a case into an easy one."""
+import math
+
+import numpy as np
+import pytest
+
+pytestmark = pytest.mark.gpu
+
+MODES = {"orb": dict(do_dbrief=False, learn_masks=False), "dbrief": dict(do_dbrief=True, learn_masks=False),
+         "mdbrief": dict(do_dbrief=True, learn_masks=True)}
+EDGE = 25
+MIN_B = EDGE - 3
+TILE_W, TILE_H, WARPS = 64, 32, 8          # K1 tile and warps per CTA; warp w collects tile rows w, w + 8, w + 16, w + 24
+WARP_SEGMENT_BEFORE_FIX = 128              # corner slots per warp when K1 assumed one strict maximum per pixel pair of a row
+
+
+def axis_cells(n, x_axis):
+    """FAST cell index of every pixel along one axis of a level (-1 outside every cell) and the cell size, with the formulas of
+    oracle/pyref.py detect_level: minB = 22, nCols = int(width / 30), wCell = ceil(width / nCols); a cell is skipped when it starts
+    6 (columns) or 3 (rows) px before maxB, and cv::FAST reports nothing in the 3 px frame of the cell's image."""
+    max_b = n - EDGE + 3
+    size = max_b - MIN_B
+    ncell = int(size / 30.0)
+    wc = int(math.ceil(size / ncell))
+    out = np.full(n, -1, np.int64)
+    for j in range(ncell):
+        ini = MIN_B + j * wc
+        if ini >= max_b - (6 if x_axis else 3):
+            continue
+        out[ini + 3:min(ini + wc + 6, max_b) - 3] = j
+    return out, wc
+
+
+def cams_for(cams, w, h):
+    """the three Lafida cameras at size w x h, full masks (Camera.mirrorMask: 0)"""
+    from multicol_slam_b200 import synth
+    out = []
+    for c in cams:
+        c = dict(c) if (w, h) == (c["width"], c["height"]) else synth.scaled_cam(c, w, h)
+        c["mirror_mask"] = 0
+        out.append(c)
+    return out
+
+
+def run_batch(api, oa, imgs, masks, cams, coi, nf, mode, levels=True, **kw):
+    """extract_batch against the oracle image by image; returns the oracle's (keypoints, level-0 raw corners) per image"""
+    m = MODES[mode]
+    ex = api.mdBRIEFextractorOct(nfeatures=nf, do_dBrief=m["do_dbrief"], learnMasks=m["learn_masks"], **kw)
+    okw = {"fast_threshold": kw.get("fastThreshold", 20), "nlevels": kw.get("nlevels", 8)}
+    oe = oa.OracleExtractor(nfeatures=nf, **m, **okw)
+    kps, desc, dmask, counts = ex.extract_batch(np.ascontiguousarray(imgs), np.ascontiguousarray(masks), cams, coi)
+    out = []
+    for i, c in enumerate(coi):
+        ok, od, om = oe.extract(imgs[i], masks[c], cams[c])
+        if levels:
+            for l in range(ex.GetLevels()):
+                assert np.array_equal(ex.debug_read(l, 0, i), oe.debug_read(l, 0)), f"image {i}: pyramid level {l}"
+                assert np.array_equal(ex.debug_read(l, 1, i), oe.debug_read(l, 1)) or not np.any(ok["octave"] == l), \
+                    f"image {i}: blurred level {l}"
+                assert np.array_equal(ex.debug_read(l, 2, i), oe.debug_read(l, 2)), f"image {i}: mask level {l}"
+                assert np.array_equal(ex.debug_read(l, 3, i), oe.debug_read(l, 3)), f"image {i}: raw corners level {l}"
+        n = counts[i]
+        k = kps[i, :n]
+        assert n == len(ok), f"image {i}: {n} keypoints, oracle {len(ok)}"
+        for f in ("x", "y", "size", "response", "octave", "class_id"):
+            assert np.array_equal(k[f], ok[f]), f"image {i}: keypoint field {f}"
+        assert np.array_equal(k["angle"].view(np.uint32), ok["angle"].view(np.uint32)), f"image {i}: IC angle bits"
+        assert np.array_equal(desc[i, :n], od), f"image {i}: descriptor bits"
+        assert np.array_equal(dmask[i, :n], om), f"image {i}: descriptor mask bits"
+        out.append((ok, oe.debug_read(0, 3)))
+    return out
+
+
+# ---- 1. dense lattices at FAST cell boundaries -----------------------------------------------------------------------------------
+def dense_row(w):
+    """One row of dots that reaches the per-tile bound on strict per-cell 3x3 maxima in every even K1 tile: each piece of a FAST
+    cell inside a tile (a segment) holds dots at every other pixel from its first pixel on, ceil(length / 2) of them.  The per-cell
+    NMS treats a neighbour in another cell as 0, so the last pixel of a cell and the first pixel of the next can both be dots, and
+    a 64-pixel tile row holds 33 or 34 maxima where its segments have odd lengths.  Where a cell runs across a tile edge, two
+    dots would touch inside one cell and suppress each other: the even tile of the two keeps its dot."""
+    cx, _ = axis_cells(w, True)
+    x = np.arange(w)
+    first = (cx >= 0) & np.concatenate([[True], cx[1:] != cx[:-1]])
+    seg0 = np.maximum(np.maximum.accumulate(np.where(first, x, 0)), x // TILE_W * TILE_W)
+    dot = (cx >= 0) & ((x - seg0) % 2 == 0)
+    for x0 in range(TILE_W, w, TILE_W):
+        if dot[x0 - 1] and dot[x0] and cx[x0 - 1] == cx[x0]:
+            dot[x0 if (x0 // TILE_W) % 2 else x0 - 1] = False
+    return dot
+
+
+def boundary_lattice(w, h, variant=0):
+    """Dense rows (dense_row, dots of 255 on black) on the four rows of one K1 warp (w = variant) in every tile.  In the last of
+    them one dot makes room for a dot in the row below, which belongs to warp w + 1 of the same tile.  Every dot is an isolated
+    FAST corner of score 254, so K2 sees nothing but ties as well."""
+    dot = dense_row(w)
+    img = np.zeros((h, w), np.uint8)
+    img[variant::WARPS][:, dot] = 255
+    for y0 in range(0, h, TILE_H):
+        y = y0 + 3 * WARPS + variant                          # last row of warp `variant` in this tile
+        if y + 1 >= h:
+            continue
+        for x0 in range(0, w, TILE_W):
+            g = np.nonzero(dot[x0 + 30 + 2 * variant:x0 + TILE_W])[0]
+            if len(g):
+                g = x0 + 30 + 2 * variant + g[0]
+                img[y, g] = 0                                 # its neighbours in the row are empty already
+                img[y + 1, g] = 255
+    return img
+
+
+def warp_segments(raw):
+    """level-0 raw corners (x, y, score) -> {(tile x, tile y, warp): corners}, the way K1 collects them"""
+    seg = {}
+    for x, y, _ in raw:
+        key = (int(x) // TILE_W, int(y) // TILE_H, (int(y) % TILE_H) % WARPS)
+        seg[key] = seg.get(key, 0) + 1
+    return seg
+
+
+def overflowing_segments(raw):
+    """warp segments holding more corners than the old 128-slot segment while the next warp of the same tile holds corners too"""
+    seg = warp_segments(raw)
+    return [k for k, v in seg.items() if v > WARP_SEGMENT_BEFORE_FIX and seg.get((k[0], k[1], k[2] + 1), 0) > 0], seg
+
+
+@pytest.mark.parametrize("mode", ["orb", "dbrief", "mdbrief"])
+@pytest.mark.parametrize("nlevels", [1, 8])
+@pytest.mark.parametrize("w,h", [(754, 480), (1280, 720), (764, 480), (641, 479)])
+def test_dense_lattice_cell_boundaries(api, oa, cams, w, h, nlevels, mode):
+    cs = cams_for(cams, w, h)
+    imgs = np.stack([boundary_lattice(w, h, v) for v in range(3)])
+    masks = np.stack([np.ones((h, w), np.uint8)] * 3)
+    res = run_batch(api, oa, imgs, masks, cs, [0, 1, 2], 2000 if w > 1000 else 1000, mode, nlevels=nlevels)
+    for i, (_, raw) in enumerate(res):
+        hit, seg = overflowing_segments(raw)
+        assert hit, f"image {i}: no warp segment above {WARP_SEGMENT_BEFORE_FIX} with a non-empty next warp (max {max(seg.values())})"
+
+
+def test_dense_lattice_device_unaligned(api, oa, cams):
+    """the same lattices from a tight 754-byte-stride device batch: K1 stages such rows byte by byte instead of by TMA"""
+    import torch
+    w, h = 754, 480
+    cs = cams_for(cams, w, h)
+    imgs = np.stack([boundary_lattice(w, h, v) for v in range(3)])
+    masks = np.stack([np.ones((h, w), np.uint8)] * 3)
+    ex = api.mdBRIEFextractorOct(nfeatures=1000, do_dBrief=True, learnMasks=True)
+    oe = oa.OracleExtractor(nfeatures=1000, do_dbrief=True, learn_masks=True)
+    dev = torch.device("cuda", 0)
+    tight = torch.from_numpy(imgs).to(dev)
+    st = torch.cuda.Stream(dev)
+    with torch.cuda.stream(st):
+        out = ex.extract_batch_device(tight, masks, cs, [0, 1, 2], stream=st)
+    ex.check_status(st)
+    counts = out["counts"].cpu().numpy()
+    kps = out["kps"].cpu().numpy().view(api.KEYPOINT_DTYPE).reshape(3, -1)
+    for i in range(3):
+        ok, od, om = oe.extract(imgs[i], masks[i], cs[i])
+        assert overflowing_segments(oe.debug_read(0, 3))[0]
+        assert np.array_equal(ex.debug_read(0, 3, i), oe.debug_read(0, 3)), f"image {i}: raw corners level 0"
+        n = counts[i]
+        assert n == len(ok) and kps[i, :n].tobytes() == ok.tobytes()
+        assert np.array_equal(out["desc"][i, :n].cpu().numpy(), od)
+        assert np.array_equal(out["dmask"][i, :n].cpu().numpy(), om)
+
+
+# ---- 2. all-equal responses ------------------------------------------------------------------------------------------------------
+def dot_lattice(w, h, period, ox, oy, value=255, background=0):
+    img = np.full((h, w), background, np.uint8)
+    img[oy::period, ox::period] = value
+    return img
+
+
+@pytest.mark.parametrize("nf", [300, 1000, 2000])
+def test_equal_responses(api, oa, cams, nf):
+    """Isolated identical dots: every dot is a corner of score 254.  Periods 4, 5 and 7 do not divide the tile or cell sizes, so the
+    lattice phase differs from tile to tile and cell to cell; every "first maximum in reference order" choice of K2 and every
+    "largest first, later created first" order of its pass B is decided by a tie."""
+    w, h = 754, 480
+    cs = cams_for(cams, w, h)
+    imgs = np.stack([dot_lattice(w, h, 4, 1, 2), dot_lattice(w, h, 5, 3, 0), dot_lattice(w, h, 7, 2, 5)])
+    masks = np.stack([np.ones((h, w), np.uint8)] * 3)
+    res = run_batch(api, oa, imgs, masks, cs, [0, 1, 2], nf, "orb")
+    for ok, raw in res:
+        assert len(raw) > 2 * nf and np.all(raw[:, 2] == 254)
+        assert np.all(ok["response"][ok["octave"] == 0] == 254)
+
+
+# ---- 3. FAST threshold edge ------------------------------------------------------------------------------------------------------
+def threshold_dots(w, h, th, spacing=9):
+    """Bright and dark dots on mid-grey whose contrast cycles through th, th + 1, th + 2 -> (image, {(x, y): contrast})"""
+    img = np.full((h, w), 128, np.uint8)
+    dots = {}
+    k = 0
+    for y in range(4, h - 4, spacing):
+        for x in range(4 + (y // spacing) % 3, w - 4, spacing):
+            c = th + k % 3
+            img[y, x] = 128 + c if (k // 3) % 2 == 0 else 128 - c
+            dots[(x, y)] = c
+            k += 1
+    return img, dots
+
+
+@pytest.mark.parametrize("th", [20, 5])
+def test_fast_threshold_edge(api, oa, cams, th):
+    """A pixel is a corner iff its FAST margin exceeds the threshold, with score = margin - 1: dots of contrast th never appear,
+    th + 1 appear with response th, th + 2 with response th + 1"""
+    w, h = 754, 480
+    cs = cams_for(cams, w, h)
+    img, dots = threshold_dots(w, h, th)
+    imgs = np.stack([img, img[:, ::-1], 255 - img])
+    masks = np.stack([np.ones((h, w), np.uint8)] * 3)
+    res = run_batch(api, oa, imgs, masks, cs, [0, 1, 2], 1000, "dbrief", fastThreshold=th)
+    cx, _ = axis_cells(w, True)
+    cy, _ = axis_cells(h, False)
+    want = {(x, y, c - 1) for (x, y), c in dots.items() if c > th and cx[x] >= 0 and cy[y] >= 0}
+    got = {tuple(int(v) for v in r) for r in res[0][1]}
+    assert got == want
+    assert {th, th + 1} <= {int(r[2]) for r in res[0][1]}
+
+
+# ---- 4. saturation ---------------------------------------------------------------------------------------------------------------
+def saturated_images(w, h):
+    """0/255 checkerboards of square sizes 1..6 and uniform binary noise: FAST margins of 255, 5x5 blur sums of 6375, saturated
+    bilinear resizes on every level"""
+    y, x = np.mgrid[0:h, 0:w]
+    out = [(((x // s) + (y // s)) % 2 * 255).astype(np.uint8) for s in range(1, 7)]
+    out.append((np.random.default_rng(7).integers(0, 2, (h, w)) * 255).astype(np.uint8))
+    return np.stack(out)
+
+
+@pytest.mark.parametrize("w,h", [(754, 480), (641, 479)])
+def test_saturated_patterns(api, oa, cams, w, h):
+    cs = cams_for(cams, w, h)
+    imgs = saturated_images(w, h)
+    masks = np.stack([np.ones((h, w), np.uint8)] * 3)
+    res = run_batch(api, oa, imgs, masks, cs, [i % 3 for i in range(len(imgs))], 1000, "mdbrief")
+    assert any(np.any(raw[:, 2] == 254) for _, raw in res)                # margin 255 reached
+
+
+# ---- 5. symmetric blobs ----------------------------------------------------------------------------------------------------------
+BLOBS = [
+    [],                                        # lone dot: both moments 0 -> fastAtan2(0, 0)
+    [(8, 0, 255)], [(0, 8, 255)], [(-8, 0, 255)], [(0, -8, 255)],              # on an axis: 0, 90, 180, 270 degrees
+    [(8, 5, 255), (-8, -5, 255)],              # point-symmetric: both moments 0
+    [(6, 6, 255), (6, -6, 255)],               # symmetric about the x axis: m01 = 0
+    [(6, 6, 255), (-6, 6, 255)],               # symmetric about the y axis: m10 = 0
+    [(8, 0, 255), (0, -1, 1)],                 # just below 360
+    [(8, 0, 255), (0, 1, 1)],                  # just above 0
+    [(6, 6, 255)],                             # diagonal
+]
+
+
+def blob_image(w, h, shift=0, spacing=37):
+    img = np.zeros((h, w), np.uint8)
+    k = shift
+    for y in range(30, h - 30, spacing):
+        for x in range(30, w - 30, spacing):
+            img[y, x] = 255
+            for dx, dy, v in BLOBS[k % len(BLOBS)]:
+                img[y + dy, x + dx] = v
+            k += 1
+    return img
+
+
+@pytest.mark.parametrize("mode", ["orb", "mdbrief"])
+def test_symmetric_blobs(api, oa, cams, mode):
+    """IC moments exactly zero or on an axis: fastAtan2(0, 0), angles of exactly 0 / 90 / 180 / 270, wrap-around near 360, and the
+    mdBRIEF +-20 degree mask patterns around them"""
+    w, h = 754, 480
+    cs = cams_for(cams, w, h)
+    imgs = np.stack([blob_image(w, h, s) for s in range(3)])
+    masks = np.stack([np.ones((h, w), np.uint8)] * 3)
+    res = run_batch(api, oa, imgs, masks, cs, [0, 1, 2], 3000, mode)
+    ang =np.concatenate([ok["angle"][ok["octave"] == 0] for ok, _ in res])
+    for a in (0.0, 90.0, 180.0, 270.0):
+        assert np.any(ang == np.float32(a)), f"no keypoint at exactly {a} degrees"
+    assert np.any(ang > 359.0) and np.any((ang > 0.0) & (ang < 1.0))
+
+
+# ---- 6. mask stripes -------------------------------------------------------------------------------------------------------------
+def stripe_masks(w, h):
+    """1-pixel alternating columns, alternating rows, and holes on the cell boundaries: every K1 tile lies on the mask border"""
+    y, x = np.mgrid[0:h, 0:w]
+    cols = ((x % 2) * 255).astype(np.uint8)
+    rows = ((y % 2 == 0) * 255).astype(np.uint8)
+    cx, _ = axis_cells(w, True)
+    cy, _ = axis_cells(h, False)
+    holes = np.full((h, w), 255, np.uint8)
+    bx = np.nonzero((cx[1:] != cx[:-1]) & (cx[1:] >= 0) & (cx[:-1] >= 0))[0]      # last column of a cell
+    by = np.nonzero((cy[1:] != cy[:-1]) & (cy[1:] >= 0) & (cy[:-1] >= 0))[0]
+    holes[1::2, :][:, bx] = 0
+    holes[::2, :][:, bx + 1] = 0
+    holes[by, :] = np.where(x[0] % 3 == 0, 0, 255)
+    for yy in by:
+        for xx in bx:
+            holes[yy - 2:yy + 3, xx - 2:xx + 3] = 0
+    return np.stack([cols, rows, holes])
+
+
+def test_mask_stripes(api, oa, cams):
+    w, h = 754, 480
+    cs = cams_for(cams, w, h)
+    imgs = np.stack([boundary_lattice(w, h, v) for v in (0, 1, 2, 0, 1, 2)])
+    masks = stripe_masks(w, h)
+    res = run_batch(api, oa, imgs, masks, cs, [0, 1, 2, 1, 2, 0], 1000, "mdbrief")
+    for i, (_, raw) in enumerate(res):                                # every mask keeps some corners and drops others
+        assert 0 < len(raw) < np.count_nonzero(imgs[i]) * 0.95, f"image {i}: {len(raw)} corners"
