@@ -51,7 +51,15 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, i
                  ::"r"(smem_u32(dst)), "l"((unsigned long long)map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
 }
 
-constexpr int kMinBlocks = 6;               // resident CTAs per SM the register budget is cut for (6 needs <= 40 registers)
+// block index read from the special register where it is used: asm volatile keeps the compiler from holding the first read live
+// across the FAST phase, where it would be spilled at the 40-register budget
+__device__ __forceinline__ int ctaid_x() { int v; asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(v)); return v; }
+__device__ __forceinline__ int ctaid_y() { int v; asm volatile("mov.u32 %0, %%ctaid.y;" : "=r"(v)); return v; }
+__device__ __forceinline__ int ctaid_z() { int v; asm volatile("mov.u32 %0, %%ctaid.z;" : "=r"(v)); return v; }
+
+// resident CTAs per SM the register budget is cut for: 5 allows 48 registers, enough for FAST without spills (6 CTAs at 40
+// registers spilled and measured the same time on H100, DESIGN.md §6)
+constexpr int kMinBlocks = 5;
 constexpr int kThreads = 256;
 constexpr int kSrcWB = 176;                 // staged source row stride (bytes, multiple of 16)
 constexpr int kT8S = 80;                    // byte tile row stride
@@ -93,6 +101,23 @@ __device__ __forceinline__ unsigned fast_margin2(unsigned C, const unsigned (&E)
     return __vmaxs2(__vsub2(bright, C), __vsub2(C, darkn)); // values in 0..255: no 16-bit overflow
 }
 
+// packed FAST margins of the pixel pair (px, px+1), px odd: o = word of the odd copy holding the pair, e = word of the even copy
+// holding (px+1, px+2).  Even ring offsets dx read the odd copy, odd dx the even one.
+__device__ __forceinline__ unsigned fast_pair_margin(const uint32_t* o, const uint32_t* e) {
+    constexpr int S = kT16S / 2;                             // row stride in words
+    unsigned R[16];
+    R[0] = o[3 * S];       R[1] = e[3 * S];        R[2] = o[2 * S + 1];   R[3] = e[S + 1];
+    R[4] = e[1];           R[5] = e[-S + 1];       R[6] = o[-2 * S + 1];  R[7] = e[-3 * S];
+    R[8] = o[-3 * S];      R[9] = e[-3 * S - 1];   R[10] = o[-2 * S - 1]; R[11] = e[-S - 2];
+    R[12] = e[-2];         R[13] = e[S - 2];       R[14] = o[2 * S - 1];  R[15] = e[3 * S - 1];
+    return fast_margin2(o[0], R);
+}
+
+// score pair of packed margins m: margin - 1 where the margin exceeds th2 (the threshold in both 16-bit lanes), else 0
+__device__ __forceinline__ unsigned fast_pair_score(unsigned m, unsigned th2) {
+    return __vsub2(m, 0x00010001u) & __vcmpgts2(m, th2);
+}
+
 __global__ void __launch_bounds__(kThreads, kMinBlocks)
 pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
                 const LevelGeom g, const int level, const int nlevels, const int fast_th, const int src_aligned,
@@ -112,34 +137,26 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
     __shared__ int16_t s_ys0[kTileH], s_ys1[kTileH], s_yb0[kTileH], s_yb1[kTileH];
     __shared__ int16_t s_cellx[kTW + 2], s_celly[kTH + 2];
     __shared__ int16_t s_mx[kTW], s_my[kTH];                          // level-0 mask coordinates of the tile's pixels
-    __shared__ int s_wn[kThreads / 32], s_base;
+    __shared__ int s_wn[kThreads / 32], s_base, s_cam, s_flag;
 
-    // 16-bit score tiles (two copies offset by one pixel, like the pixel tiles); they reuse the source staging
-    // area, which is dead once the tile has been resized
+    // 16-bit score tile; it reuses the source staging area, which is dead once the tile has been resized.  The NMS forms the
+    // odd-aligned score pairs from two aligned words with a byte permute.
     uint16_t* s_s0 = (uint16_t*)s_src;                                  // s_s0[y][x] = score(x),   x = score-tile column
-    uint16_t* s_s1 = (uint16_t*)s_src + (kTH + 2) * kScoreS;            // s_s1[y][i] = score(i+1)
     // corner list, one segment per warp (no atomics while collecting): lives in the 16-bit pixel tile, which is dead once the FAST
     // margins are computed (phases b, c; the barrier before phase d separates them from phase e)
     uint32_t* s_list = (uint32_t*)s_a0;
     static_assert((kThreads / 32) * kWarpCorners * 4 <= kTileH * kT16S * 2, "corner list must fit into the dead pixel tile");
-    static_assert(2 * (kTH + 2) * kScoreS * 2 <= kSrcH * kSrcWB, "score tiles must fit into the staging area");
+    static_assert((kTH + 2) * kScoreS * 2 <= kSrcH * kSrcWB, "score tile must fit into the staging area");
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int b = blockIdx.z;
     const int X0 = blockIdx.x * kTW, Y0 = blockIdx.y * kTH;
     const uint8_t* simg = src + (size_t)b * src_img_bytes;
-    // FAST + NMS only where the tile holds at least one pixel inside the camera's mask: a corner is reported only if its own
-    // mask pixel is set (mask applied after NMS, SURVEY A.5), and the scores of its 8 neighbours come from this CTA's own halo
-    const int cam_b = cam_of_image[b];
-    const int tile_flag = tile_flags[(size_t)cam_b * tiles_total + g.tile_off + blockIdx.y * g.tiles_x + blockIdx.x];
-    const bool fast_on = tile_flag != 0, mask_full = tile_flag == 2;      // 2: every pixel of the tile is inside the mask
-
     // output-space range needed by this tile; after REFLECT_101 everything lies inside it
     const int xa = max(X0 - kHalo, 0), xb = min(X0 + kTW + kHalo, g.w) - 1;
     const int ya = max(Y0 - kHalo, 0), yb = min(Y0 + kTH + kHalo, g.h) - 1;
     const int sx_lo = g.xofs[xa], sx_hi = min(g.xofs[xb] + 1, g.sw - 1);
     const int sy_lo = min(max((int)g.yofs[ya], 0), g.sh - 1), sy_hi = min(max(g.yofs[yb] + 1, 0), g.sh - 1);
     const int sx_base = sx_lo & ~15;
-    const int wb = use_tma ? g.box_w : kSrcWB;                          // row stride of the staged region in bytes
     if (tid == 0) {
         if (use_tma) {
             // the barrier is initialised and armed by the same thread that issues the copy; every other thread first sees it
@@ -150,7 +167,18 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         }
     }
 
+    // FAST + NMS only where the tile holds at least one pixel inside the camera's mask: a corner is reported only if its own
+    // mask pixel is set (mask applied after NMS, SURVEY A.5), and the scores of its 8 neighbours come from this CTA's own halo.
+    // One thread reads the camera and the tile's flag; the other threads read them from shared memory where they are used,
+    // so that they hold no registers through FAST.
+    if (tid == 32) {
+        const int cam_b = cam_of_image[b];
+        s_cam = cam_b;
+        s_flag = tile_flags[(size_t)cam_b * tiles_total + g.tile_off + blockIdx.y * g.tiles_x + blockIdx.x];
+    }
+
     // ---- per-tile slices of the resize / cell tables ----
+    bool in_cells = true;                 // this thread's score-tile row / column lies inside a FAST cell
     if (tid < kTileW) {
         // rows/columns further than the ring beyond the image are never consumed: clamp them into the staged range
         const int rx = min(max(reflect101(X0 - kHalo + tid, g.w), xa), xb);
@@ -167,11 +195,15 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         s_yb0[t] = g.yb0[ry]; s_yb1[t] = g.yb1[ry];
     } else if (tid >= 144 && tid < 144 + kTW + 2) {
         const int x = X0 - 1 + tid - 144;
-        s_cellx[tid - 144] = (x >= 0 && x < g.w) ? g.cellx[x] : (int16_t)-1;
+        const int16_t c = (x >= 0 && x < g.w) ? g.cellx[x] : (int16_t)-1;
+        s_cellx[tid - 144] = c;
+        in_cells = c >= 0;
     }
     if (tid < kTH + 2) {
         const int y = Y0 - 1 + tid;
-        s_celly[tid] = (y >= 0 && y < g.h) ? g.celly[y] : (int16_t)-1;
+        const int16_t c = (y >= 0 && y < g.h) ? g.celly[y] : (int16_t)-1;
+        s_celly[tid] = c;
+        in_cells = in_cells && c >= 0;
     } else if (tid >= 64 && tid < 64 + kTW) {
         const int x = X0 + tid - 64;
         s_mx[tid - 64] = x < g.w ? g.mx0[x] : (int16_t)0;
@@ -205,11 +237,31 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
                 }
         }
     }
-    __syncthreads();
+    // every pixel of the score tile (tile + 1 ring) lies inside some FAST cell, and so inside the level: FAST needs no per-pixel test
+    const bool fast_inner = __syncthreads_and(in_cells);
     if (use_tma) mbar_wait(&s_bar, 0);
+    const int wb = use_tma ? g.box_w : kSrcWB;                          // row stride of the staged region in bytes
 
-    // ---- bilinear resize (OpenCV 11-bit fixed point) into the three tile forms; a thread owns a pixel-pair column ----
-    if (tid < (kTileW / 2) * 7) {
+    if (level == 0 && ctaid_x() * kTW >= kHalo && ctaid_x() * kTW + kTW + kHalo <= g.w) {
+        // ---- identity resize of a tile whose columns (with the ring) need no reflection: a word copy of the staged rows ----
+        // staged column X0 - kHalo lies at byte (X0 - kHalo) & 15 (sx_base = (X0 - kHalo) & ~15), a multiple of 4
+        static_assert(kTW % 16 == 0 && kHalo % 4 == 0 && kTileW % 4 == 0, "level-0 word copy needs word-aligned tile columns");
+        constexpr int kQ = kTileW / 4, kRG = kThreads / kQ;              // 18 words per row, 14 row groups
+        if (tid < kQ * kRG) {
+            const int q = tid % kQ;
+            const uint8_t* s_row = s_src + ((ctaid_x() * kTW - kHalo) & 15) + 4 * q;
+#pragma unroll
+            for (int ty = tid / kQ; ty < kTileH; ty += kRG) {
+                const uint32_t* r = (const uint32_t*)(s_row + s_ys0[ty] * wb);
+                const uint32_t w = r[0], wn = r[1];                         // pixels 4q .. 4q+3, 4q+4 .. 4q+7
+                const uint32_t a0 = __byte_perm(w, 0u, 0x4140), a1 = __byte_perm(w, 0u, 0x4342);
+                *(uint32_t*)(s_t8 + ty * kT8S + 4 * q) = w;
+                *(uint2*)(s_a0 + ty * kT16S + 4 * q) = make_uint2(a0, a1);
+                *(uint2*)(s_a1 + ty * kT16S + 4 * q) = make_uint2(__byte_perm(w, 0u, 0x4241), __byte_perm(a1, wn, 0x1412));
+            }
+        }
+    } else if (tid < (kTileW / 2) * 7) {
+        // ---- bilinear resize (OpenCV 11-bit fixed point) into the three tile forms; a thread owns a pixel-pair column ----
         const int pc = tid % (kTileW / 2), rg = tid / (kTileW / 2);      // 36 pair columns x 7 row groups
         const int tx = 2 * pc;
         const int xs00 = s_xs0[tx], xs01 = s_xs1[tx], xs10 = s_xs0[tx + 1], xs11 = s_xs1[tx + 1];
@@ -248,7 +300,6 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         s_md[y] = s_celly[y + 2] == s_celly[y + 1] ? 0xFFFFFFFFu : 0u;
     }
     uint8_t* dimg = dst + (size_t)b * g.img_bytes;
-    uint8_t* bimg = dst_blur + (size_t)b * g.img_bytes;
     // ---- (a) store the unblurred tile, 4 px per thread ----
 #pragma unroll
     for (int i = tid; i < kTH * (kTW / 4); i += kThreads) {
@@ -264,55 +315,65 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         const uint32_t* w1 = (const uint32_t*)(s_a1 + (y + kHalo - 2) * kT16S) + (kHalo / 2 + j);   // pair (x+1, x+2)
         s_h[i] = __vadd2(__vadd2(__vadd2(w0[-1], w1[-1]), __vadd2(w0[0], w1[0])), w0[1]);
     }
-    // ---- (c) FAST margins of pixel pairs on the tile + 1 ring; pairs start at tile column 3 (odd) ----
-    if (fast_on)
+    // ---- (c) FAST scores of pixel pairs on the tile + 1 ring: score-tile row y, pair j = score-tile columns 2j, 2j+1, centre
+    // pixel px = tile col 3+2j (odd) -> word j+1 of the odd copy, pair (px+1, px+2) -> word j+2 of the even copy ----
+    constexpr int kPJ = (kTW + 2) / 2;                          // 33 pairs per score-tile row
+    static_assert(kTH % 8 == 0 && kTW == 64, "FAST: one lane per pair column, a warp per score-tile row");
+    if (s_flag != 0) {                                          // CTA-uniform
+        const unsigned th2 = (unsigned)fast_th * 0x00010001u;   // 1 <= fast_th <= 254 (checked by the host)
+        // score of pair j on row y; pixels outside every FAST cell get a threshold no margin exceeds (margins are at most 255)
+        // rather than a mask on the score: one register less across the margin, which keeps FAST free of spills.  A warp skips
+        // the margins of a pair set outside the cells.  Tiles inside the cell grid (fast_inner, most of them) test nothing.
+        auto score = [&](const uint32_t* o, const uint32_t* e, unsigned in) -> unsigned {
+            return in ? fast_pair_score(fast_pair_margin(o, e), (th2 & in) | (0x7FFF7FFFu & ~in)) : 0u;
+        };
+        auto cells = [&](int y, int j) -> unsigned {
+            if (fast_inner) return ~0u;
+            return s_celly[y] < 0 ? 0u : (s_cellx[2 * j] >= 0 ? 0xFFFFu : 0u) | (s_cellx[2 * j + 1] >= 0 ? 0xFFFF0000u : 0u);
+        };
+        // lane = pair column 0..31 on rows wid, wid + 8, ..: addresses formed once, rows 8 apart are compile-time offsets
+        {
+            const uint32_t* o = (const uint32_t*)(s_a1 + (wid + kHalo - 1) * kT16S) + (lane + 1);
+            const uint32_t* e = (const uint32_t*)(s_a0 + (wid + kHalo - 1) * kT16S) + (lane + 2);
+            uint32_t* sc = (uint32_t*)(s_s0 + wid * kScoreS) + lane;
 #pragma unroll
-    for (int i = tid; i < (kTH + 2) * ((kTW + 2) / 2); i += kThreads) {
-        const int y = i / ((kTW + 2) / 2), j = i - y * ((kTW + 2) / 2);
-        const int sx = 2 * j;                                   // score-tile column of the first pixel of the pair
-        const bool in0 = s_cellx[sx] >= 0, in1 = s_cellx[sx + 1] >= 0, iny = s_celly[y] >= 0;
-        unsigned s0 = 0, s1 = 0;
-        if (iny && (in0 || in1)) {
-            // centre pair (px, px+1) with px = tile col 3+2j (odd) -> word j+1 of the odd copy; even dx -> odd copy, odd dx -> even copy
-            const uint32_t* o = (const uint32_t*)(s_a1 + (y + kHalo - 1) * kT16S) + (j + 1);
-            const uint32_t* e = (const uint32_t*)(s_a0 + (y + kHalo - 1) * kT16S) + (j + 2);   // pair starting at px+1
-            constexpr int S = kT16S / 2;                         // row stride in words
-            const unsigned C = o[0];
-            unsigned R[16];
-            R[0] = o[3 * S];       R[1] = e[3 * S];        R[2] = o[2 * S + 1];   R[3] = e[S + 1];
-            R[4] = e[1];           R[5] = e[-S + 1];       R[6] = o[-2 * S + 1];  R[7] = e[-3 * S];
-            R[8] = o[-3 * S];      R[9] = e[-3 * S - 1];   R[10] = o[-2 * S - 1]; R[11] = e[-S - 2];
-            R[12] = e[-2];         R[13] = e[S - 2];       R[14] = o[2 * S - 1];  R[15] = e[3 * S - 1];
-            const unsigned m = fast_margin2(C, R);
-            const int m0 = (int)(short)(m & 0xFFFFu), m1 = (int)(short)(m >> 16);
-            s0 = (in0 && m0 > fast_th) ? (unsigned)(m0 - 1) : 0u;
-            s1 = (in1 && m1 > fast_th) ? (unsigned)(m1 - 1) : 0u;
+            for (int k = 0; k < kTH / 8; ++k)                   // 8 rows further: 8 * kT16S / 2 words in the pixel tiles
+                sc[k * 4 * kScoreS] = score(o + k * 4 * kT16S, e + k * 4 * kT16S, cells(wid + 8 * k, lane));
         }
-        *(uint32_t*)(s_s0 + y * kScoreS + sx) = s0 | (s1 << 16);
-        if (sx > 0) s_s1[y * kScoreS + sx - 1] = (uint16_t)s0;
-        s_s1[y * kScoreS + sx] = (uint16_t)s1;
+        // the rest: rows 32, 33 (warps 0, 1) and pair column 32 of every row (threads 64 .. 97)
+        if (tid < 2 * 32 + kTH + 2) {
+            const int y = tid < 64 ? kTH + (tid >> 5) : tid - 64, j = tid < 64 ? lane : kPJ - 1;
+            const uint32_t* o = (const uint32_t*)(s_a1 + (y + kHalo - 1) * kT16S) + (j + 1);
+            const uint32_t* e = (const uint32_t*)(s_a0 + (y + kHalo - 1) * kT16S) + (j + 2);
+            *((uint32_t*)(s_s0 + y * kScoreS) + j) = score(o, e, cells(y, j));
+        }
     }
     __syncthreads();
+    const int tx0 = ctaid_x() * kTW, ty0 = ctaid_y() * kTH, img = ctaid_z();   // X0, Y0, b again (see ctaid_x)
+    uint8_t* bimg = dst_blur + (size_t)img * g.img_bytes;
 
     // ---- (d) blurred tile: vertical 5-sum of the packed row sums, (S+12)/25, 4 px per thread ----
 #pragma unroll
     for (int i = tid; i < kTH * (kTW / 4); i += kThreads) {
         const int y = i >> 4, q = i & 15;
-        if (Y0 + y < g.h && X0 + 4 * q < g.pitch) {
+        if (ty0 + y < g.h && tx0 + 4 * q < g.pitch) {
             const uint32_t* h = s_h + y * (kTW / 2) + 2 * q;
             const unsigned p0 = __vadd2(__vadd2(__vadd2(h[0], h[32]), __vadd2(h[64], h[96])), h[128]);
             const unsigned p1 = __vadd2(__vadd2(__vadd2(h[1], h[33]), __vadd2(h[65], h[97])), h[129]);
             // (S + 12) / 25 == ((S + 12) * 5243) >> 17 for S <= 6375 (checked exhaustively in tests)
             const unsigned o0 = (((p0 & 0xFFFFu) + 12u) * 5243u) >> 17, o1 = (((p0 >> 16) + 12u) * 5243u) >> 17;
             const unsigned o2 = (((p1 & 0xFFFFu) + 12u) * 5243u) >> 17, o3 = (((p1 >> 16) + 12u) * 5243u) >> 17;
-            *(uint32_t*)(bimg + (size_t)(Y0 + y) * g.pitch + X0 + 4 * q) = o0 | (o1 << 8) | (o2 << 16) | (o3 << 24);
+            *(uint32_t*)(bimg + (size_t)(ty0 + y) * g.pitch + tx0 + 4 * q) = o0 | (o1 << 8) | (o2 << 16) | (o3 << 24);
         }
     }
     // ---- (e) per-cell 3x3 non-max suppression on pixel pairs (packed 16x2), mask filter, tile-local compaction ----
-    // Pair j of row y = pixels x = 2j, 2j+1 = score-tile columns 2j+1, 2j+2: centre word from the odd copy, left /
-    // right neighbour pairs from the even copy.  A neighbour outside the pixel's FAST cell counts as 0 (cv::FAST runs per cell).
-    if (!fast_on) return;                                   // uniform for the CTA: no corner can come out of this tile
-    const uint8_t* m0p = mask0 + (size_t)cam_b * mask_bytes;
+    // Pair j of row y = pixels x = 2j, 2j+1 = score-tile columns 2j+1, 2j+2: the high half of word j and the low half of word j+1
+    // (one byte permute), left / right neighbour pairs are words j and j+1 themselves.  A neighbour outside the pixel's FAST cell
+    // counts as 0 (cv::FAST runs per cell).
+    const int tile_flag = s_flag;
+    if (tile_flag == 0) return;                             // uniform for the CTA: no corner can come out of this tile
+    const bool mask_full = tile_flag == 2;                  // 2: every pixel of the tile is inside the mask
+    const uint8_t* m0p = mask0 + (size_t)s_cam * mask_bytes;
     // A warp owns one tile row per pass (32 pixel pairs), every lane evaluates its pair branch-free and the warp VOTES: two
     // ballots give the number of surviving corners and each lane's slot in the warp's own list segment (a per-corner divergent
     // append runs with few active lanes, and a per-pass shared atomic still costs a visible share of the instructions).  The
@@ -322,13 +383,13 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
     for (int i = tid; i < kTH * (kTW / 2); i += kThreads) {
         const int y = i >> 5, j = i & 31;
         const uint32_t* e0 = (const uint32_t*)(s_s0 + y * kScoreS) + j;          // row y-1 of the interior row y (score row y)
-        const uint32_t* o0 = (const uint32_t*)(s_s1 + y * kScoreS) + j;
         constexpr int S = kScoreS / 2;
-        const unsigned C = o0[S];
+        const unsigned u0 = e0[0], u1 = e0[1], c0 = e0[S], c1 = e0[S + 1], d0 = e0[2 * S], d1 = e0[2 * S + 1];
+        const unsigned C = __byte_perm(c0, c1, 0x5432);
         const unsigned ml = s_ml[j], mr = s_mr[j], mu = s_mu[y], md = s_md[y];
-        const unsigned up = __vimax3_u16x2(e0[0] & ml & mu, o0[0] & mu, e0[1] & mr & mu);
-        const unsigned dn = __vimax3_u16x2(e0[2 * S] & ml & md, o0[2 * S] & md, e0[2 * S + 1] & mr & md);
-        const unsigned nm = __vimax3_u16x2(up, dn, __vmaxu2(e0[S] & ml, e0[S + 1] & mr));
+        const unsigned up = __vimax3_u16x2(u0 & ml & mu, __byte_perm(u0, u1, 0x5432) & mu, u1 & mr & mu);
+        const unsigned dn = __vimax3_u16x2(d0 & ml & md, __byte_perm(d0, d1, 0x5432) & md, d1 & mr & md);
+        const unsigned nm = __vimax3_u16x2(up, dn, __vmaxu2(c0 & ml, c1 & mr));
         const int sv0 = (int)(C & 0xFFFFu), sv1 = (int)(C >> 16);
         // strict maximum of its 3x3 (implies a non-zero score), then the mask of its own pixel (mask applied after NMS)
         bool k0 = sv0 > (int)(nm & 0xFFFFu), k1 = sv1 > (int)(nm >> 16);
@@ -342,8 +403,8 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
             const int n0 = __popc(b0);
             const unsigned lt = (1u << lane) - 1u;
             uint32_t* wl = s_list + wid * kWarpCorners + wn;
-            if (k0) wl[__popc(b0 & lt)] = pack_corner(X0 + 2 * j, Y0 + y, sv0);
-            if (k1) wl[n0 + __popc(b1 & lt)] = pack_corner(X0 + 2 * j + 1, Y0 + y, sv1);
+            if (k0) wl[__popc(b0 & lt)] = pack_corner(tx0 + 2 * j, ty0 + y, sv0);
+            if (k1) wl[n0 + __popc(b1 & lt)] = pack_corner(tx0 + 2 * j + 1, ty0 + y, sv1);
             wn += n0 + __popc(b1);
         }
     }
@@ -356,9 +417,9 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         n += s_wn[w];
     }
     if (n == 0) return;
-    if (tid == 0) s_base = atomicAdd(&raw_count[b * nlevels + level], n);
+    if (tid == 0) s_base = atomicAdd(&raw_count[img * nlevels + level], n);
     __syncthreads();
-    uint32_t* rlist = raw + (size_t)b * raw_img_stride + g.raw_off;
+    uint32_t* rlist = raw + (size_t)img * raw_img_stride + g.raw_off;
     for (int i = lane; i < wn; i += 32) {
         const int pos = s_base + my_off + i;
         if (pos < g.raw_cap) rlist[pos] = s_list[wid * kWarpCorners + i];
