@@ -386,6 +386,56 @@ int  mcs_project_mappoints(int32_t n_cams, const double* mtmc_inv, const double*
                            const double* min_dist, const double* max_dist, const double* scale_factors, int32_t n_levels,
                            uint8_t* in_view, int32_t* level, double* proj_x, double* proj_y, double* view_cos);
 
+/* ---- SearchReferencePointsInFrustum on the device (G1 / M1 without host round trips) ------------------------------------- */
+/* Both calls are asynchronous on `stream` (a cudaStream_t as void*; NULL = the default stream, and the call synchronises before
+ * returning).  With a stream given neither call waits for it.  Scratch comes from the stream-ordered memory pool.
+ *
+ * mcs_project_mappoints_device: mcs_project_mappoints with the map-point arrays and the outputs in device memory (the map points
+ * stay resident across frames like the cMapPoint members).  mtmc_inv, mtmc, cams and scale_factors are host memory; masks_dev holds
+ * the n_cams level-0 mirror masks.  skip_dev ([n_points] bytes, may be NULL): the outputs of a flagged point are left untouched --
+ * the reference skips points already matched or bad (ref src/cTracking.cpp:985-988), and SearchByProjection then reads their
+ * previous mbTrackInView.  Same kernel and arithmetic as mcs_project_mappoints; cameras of different sizes: MCS_ERR_UNSUPPORTED. */
+int  mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const double* mtmc, const mcs_ocam* cams,
+                                  const uint8_t* masks_dev, int32_t n_points, const double* world_pos_dev, const double* normal_dev,
+                                  const double* min_dist_dev, const double* max_dist_dev, const double* scale_factors, int32_t n_levels,
+                                  const uint8_t* skip_dev, uint8_t* in_view_dev, int32_t* level_dev, double* proj_x_dev,
+                                  double* proj_y_dev, double* view_cos_dev, void* stream);
+
+/* mcs_mappoint_view with every pointer in device memory (the arrays mcs_project_mappoints_device fills, plus bad / desc / dmask). */
+typedef struct mcs_mappoint_dev_view {
+    int32_t n_points;
+    const uint8_t* bad;             /* may be NULL: no point is bad */
+    const uint8_t* in_view;
+    const int32_t* level;
+    const double*  proj_x;
+    const double*  proj_y;
+    const double*  view_cos;
+    const uint8_t* desc;
+    const uint8_t* dmask;
+} mcs_mappoint_dev_view;
+
+/* cORBmatcher::SearchByProjection(F, vpMapPoints, th) (ref :67-166) with the frame in packed feature buffers and every output on
+ * the device; the result equals mcs_search_by_projection's.
+ *   Frame: camera c is global image first_image + c of packed_dev, which holds n_parts consecutive packed layouts of
+ *   part_images images each (mcs_packed_layout(part_images, capacity, dim) bytes apiece): n_parts = 1 is one extraction call's
+ *   buffer, n_parts = world with part_images = 1 what mcs_allgather_features leaves for a one-camera-per-GPU rig.  The masks
+ *   section is read when having_masks is set.  cam_width / cam_height [n_cams] (mnMaxX - mnMinX, ...) and scale_factors
+ *   [n_levels] are host memory.
+ *   frame_mp_dev [n_cams * capacity] in/out, indexed by slot c * capacity + j (keypoint j of camera c): -1 = free, accepted
+ *   slots receive the map-point index; slots at or beyond a camera's count are ignored.
+ *   nmatches_dev: number of acceptances.  status_dev: MCS_ERR_INVALID when an in-view entry of a non-bad point has a level
+ *   outside [0, n_levels) -- that query is skipped, the others are unaffected -- MCS_OK otherwise.
+ *   diag_dev (may be NULL): int32[4] = fixpoint rounds run, first query the sequential walk took over (-1 = none), queries,
+ *   decisions that rescanned their window (DESIGN.md section 4).
+ * capacity <= 65535, n_points * n_cams < 2^24. */
+int  mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int32_t part_images, int32_t first_image,
+                                     int32_t n_cams, int32_t capacity, int32_t dim, const int32_t* cam_width, const int32_t* cam_height,
+                                     int32_t n_levels, const double* scale_factors, const mcs_mappoint_dev_view* mps,
+                                     double th, double nnratio, int32_t th_high, int32_t having_masks,
+                                     int32_t* frame_mp_dev, int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev, void* stream);
+/* The number of fixpoint rounds mcs_search_by_projection_device runs before the sequential walk finishes the rest. */
+int  mcs_search_by_projection_max_rounds(void);
+
 /* Generic projection-window search: the shape shared by the remaining cORBmatcher searches (SURVEY 8a row M4).
  * Queries are visited in order; for each one the candidates of GetFeaturesInArea(cam, x, y, r, min_level, max_level)
  * that are not yet taken (assigned[idx] >= 0) are scanned in the reference's order, best / second best are tracked

@@ -15,7 +15,7 @@ import pathlib
 
 import numpy as np
 
-from .ctypes_defs import (ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointView, Ocam,
+from .ctypes_defs import (ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam,
                           WINDOW_QUERY_DTYPE, make_ocam, make_params)
 
 _PKG = pathlib.Path(__file__).resolve().parent
@@ -511,6 +511,78 @@ def project_mappoints(mtmc_inv, mtmc, cams, masks, world_pos, normal, min_dist, 
     return in_view, level, px, py, vc
 
 
+def _dptr(t):
+    return C.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _stream_handle(stream, dev):
+    import torch
+    return C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
+
+
+def project_mappoints_device(mtmc_inv, mtmc, cams, masks_t, world_t, normal_t, min_dist_t, max_dist_t, scale_factors, skip_t=None,
+                             out=None, stream=None):
+    """mcs_project_mappoints_device: project_mappoints with the map points resident on the GPU.  mtmc_inv / mtmc [n_cams,4,4] and
+    scale_factors on the host; masks_t [n_cams,H,W] u8, world_t / normal_t [n,3] f64, min/max_dist_t [n] f64 cuda tensors;
+    skip_t [n] u8 cuda or None (flagged points keep their previous entries in `out`).  Returns `out` = (in_view [n,n_cams] u8,
+    level i32, proj_x, proj_y, view_cos f64) cuda tensors, written asynchronously on `stream`."""
+    import torch
+    mi = np.ascontiguousarray(mtmc_inv, np.float64)
+    mm = np.ascontiguousarray(mtmc, np.float64)
+    sf = np.ascontiguousarray(scale_factors, np.float64)
+    nc, n, dev = len(cams), world_t.shape[0], world_t.device
+    ocs = (Ocam * nc)(*[as_ocam(c) for c in cams])
+    if out is None:
+        out = (torch.zeros((n, nc), dtype=torch.uint8, device=dev), torch.zeros((n, nc), dtype=torch.int32, device=dev),
+               *(torch.zeros((n, nc), dtype=torch.float64, device=dev) for _ in range(3)))
+    _check(lib().mcs_project_mappoints_device(nc, _p(mi), _p(mm), ocs, _dptr(masks_t), n, _dptr(world_t), _dptr(normal_t), _dptr(min_dist_t),
+                                              _dptr(max_dist_t), _p(sf), len(sf), _dptr(skip_t), *(_dptr(t) for t in out),
+                                              _stream_handle(stream, dev)))
+    return out
+
+
+class MapPointsDevice:
+    """MapPoints with every array a torch CUDA tensor (bad may be None); in_view / level / proj_x / proj_y / view_cos [n, n_cams]
+    as project_mappoints_device fills them, desc / dmask [n, dim] u8."""
+
+    def __init__(self, bad, in_view, level, proj_x, proj_y, view_cos, desc, dmask=None):
+        self.bad, self.in_view, self.level = bad, in_view, level
+        self.proj_x, self.proj_y, self.view_cos, self.desc, self.dmask = proj_x, proj_y, view_cos, desc, dmask
+
+    @staticmethod
+    def from_host(mps, device):
+        """MapPoints (host arrays) -> the same fields on `device`"""
+        import torch
+        t = lambda a: None if a is None else torch.from_numpy(np.ascontiguousarray(a)).to(device)  # noqa: E731
+        return MapPointsDevice(t(mps.bad), t(mps.in_view), t(mps.level), t(mps.proj_x), t(mps.proj_y), t(mps.view_cos), t(mps.desc),
+                               t(mps.dmask))
+
+    def view(self):
+        v = MapPointDevView()
+        v.n_points = self.desc.shape[0]
+        for k in ("bad", "in_view", "level", "proj_x", "proj_y", "view_cos", "desc", "dmask"):
+            t = getattr(self, k)
+            setattr(v, k, t.data_ptr() if t is not None else None)
+        return v
+
+
+def slots_to_contiguous(frame_mp_slots, counts, capacity):
+    """slot-indexed frame_mp [n_cams * capacity] (slot c * capacity + j) -> the contiguous keypoint order of Frame / cMultiFrame
+    (camera-major, ref src/cMultiFrame.cpp:168-184)"""
+    a = np.asarray(frame_mp_slots).reshape(-1, capacity)
+    return np.concatenate([a[c, :int(n)] for c, n in enumerate(counts)]).astype(np.int32)
+
+
+def contiguous_to_slots(frame_mp, counts, capacity, fill=-1):
+    """inverse of slots_to_contiguous; slots beyond a camera's count get `fill`"""
+    out = np.full((len(counts), capacity), fill, np.int32)
+    o = 0
+    for c, n in enumerate(counts):
+        out[c, :int(n)] = frame_mp[o:o + int(n)]
+        o += int(n)
+    return out.reshape(-1)
+
+
 RULE_RATIO, RULE_BEST, RULE_LEVEL_RATIO, RULE_BEST_FREE, RULE_FIRST_FREE, RULE_SCW = 0, 1, 2, 3, 4, 5
 
 
@@ -643,6 +715,27 @@ class cORBmatcher:
         _check(lib().mcs_search_by_projection(C.byref(fv), C.byref(mv), C.c_double(th), C.c_double(self.mfNNratio), self.TH_HIGH_,
                                               int(self.havingMasks), _p(frame_mp), C.byref(n)))
         return n.value, frame_mp
+
+    def SearchByProjectionDevice(self, packed_t, n_parts, part_images, first_image, n_cams, capacity, cam_sizes, scale_factors, mps_dev,
+                                 th, frame_mp_t, stream=None, out=None, diag=False):
+        """mcs_search_by_projection_device: SearchByProjection with the frame in packed feature buffers (packed_t: uint8 cuda tensor of
+        n_parts layouts of part_images images; camera c = image first_image + c) and the map points in a MapPointsDevice.  frame_mp_t:
+        int32 cuda tensor [n_cams * capacity] indexed by slot, updated in place.  Asynchronous on `stream`.  Returns (nmatches [1],
+        status [1], frame_mp_t), plus diag [4] when diag is set, as cuda tensors."""
+        import torch
+        dev = packed_t.device
+        dim = mps_dev.desc.shape[1]
+        cw = np.ascontiguousarray([s[0] for s in cam_sizes], np.int32)
+        ch = np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
+        sf = np.ascontiguousarray(scale_factors, np.float64)
+        if out is None:
+            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
+        mv = mps_dev.view()
+        _check(lib().mcs_search_by_projection_device(_dptr(packed_t), n_parts, part_images, first_image, n_cams, capacity, dim, _p(cw), _p(ch),
+                                                     len(sf), _p(sf), C.byref(mv), C.c_double(th), C.c_double(self.mfNNratio), self.TH_HIGH_,
+                                                     int(self.havingMasks), _dptr(frame_mp_t), _dptr(out[0]), _dptr(out[1]),
+                                                     _dptr(out[2]) if diag else None, _stream_handle(stream, dev)))
+        return (out[0], out[1], frame_mp_t) + ((out[2],) if diag else ())
 
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
         """ref :579-726.  vbPrevMatched [n1,2] float64 updated in place.  Returns (nmatches, vnMatches12)."""

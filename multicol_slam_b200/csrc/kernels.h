@@ -100,9 +100,31 @@ cudaError_t launch_compact_lists(const int* idx, const int* dist, const int* cou
 cudaError_t launch_frame_prepare(const mcs_keypoint* keys, const int* key_cam, int n_keys, const mcs_ocam* cams, int n_cams, float* kx,
                                  float* ky, int* koct, double* rays, int* cell_of, int* cursor, int* cell_start, int* cell_items,
                                  double* winv, double* hinv, cudaStream_t st);
+// skip (may be NULL): [n_points] bytes; the outputs of a flagged point are left untouched
 cudaError_t launch_frustum(int n_cams, const double* mtmc_inv, const double* mtmc, const mcs_ocam* cams, const uint8_t* masks,
                            int n_points, const double* pos, const double* nrm, const double* dmin, const double* dmax, const double* sf,
-                           int n_levels, uint8_t* in_view, int* level, double* px, double* py, double* vcos, cudaStream_t st);
+                           int n_levels, uint8_t* in_view, int* level, double* px, double* py, double* vcos, const uint8_t* skip,
+                           cudaStream_t st);
+
+// device-resident SearchByProjection (proj_search_kernels.cu)
+// Copies small host data into device memory in stream order through kernel parameters, so that the calling thread never waits
+// for the stream (a cudaMemcpyAsync from pageable memory may).
+cudaError_t stage_to_device(const void* host, size_t bytes, void* dev, cudaStream_t st);
+struct PsCamSlots {                     // camera c of the frame: its image slot inside the packed feature buffer
+    const int* count; const mcs_keypoint* kps; const uint8_t* desc; const uint8_t* dmask;
+};
+struct ProjSearchArgs {
+    int n_cams, capacity, dim, n_levels, n_points;
+    const PsCamSlots* cams;                                  // host [n_cams] (device pointers inside)
+    const int* cam_w; const int* cam_h; const double* sf;    // host
+    const uint8_t* bad; const uint8_t* in_view; const int* level;              // device map-point arrays
+    const double* px; const double* py; const double* vcos;
+    const uint8_t* mp_desc; const uint8_t* mp_dmask;
+    double th, nnratio; int th_high; bool masked;
+    int* frame_mp; int* nmatches; int* status; int* diag;    // device
+};
+cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st);
+int proj_search_max_rounds();
 
 // ---- bag of words (bow_kernels.cu) ----
 // vocabulary tree on the device: CSR children in the reference's order, 32-byte node descriptors as uint4 pairs

@@ -1141,10 +1141,11 @@ __global__ void frustum_kernel(const int n_cams, const double* __restrict__ mtmc
                                const double* __restrict__ pos, const double* __restrict__ nrm, const double* __restrict__ dmin,
                                const double* __restrict__ dmax, const double* __restrict__ sf, const int n_levels,
                                uint8_t* __restrict__ in_view, int* __restrict__ level, double* __restrict__ px, double* __restrict__ py,
-                               double* __restrict__ vcos) {
+                               double* __restrict__ vcos, const uint8_t* __restrict__ skip) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n_points * n_cams) return;
     const int i = t / n_cams, c = t - i * n_cams;
+    if (skip && skip[i]) return;                  // already matched / bad (ref src/cTracking.cpp:985-988): keeps its last entries
     in_view[t] = 0; level[t] = 0; px[t] = 0.0; py[t] = 0.0; vcos[t] = 0.0;
     const double P0 = pos[3 * i], P1 = pos[3 * i + 1], P2 = pos[3 * i + 2];
     // ptRot = MtMc_inv[c] * (P,1): cv::Matx product, s = 0 + a0 b0 + a1 b1 + a2 b2 + a3 b3 in this order, no FMA
@@ -1174,11 +1175,12 @@ __global__ void frustum_kernel(const int n_cams, const double* __restrict__ mtmc
 
 cudaError_t launch_frustum(int n_cams, const double* mtmc_inv, const double* mtmc, const mcs_ocam* cams, const uint8_t* masks,
                            int n_points, const double* pos, const double* nrm, const double* dmin, const double* dmax, const double* sf,
-                           int n_levels, uint8_t* in_view, int* level, double* px, double* py, double* vcos, cudaStream_t st) {
+                           int n_levels, uint8_t* in_view, int* level, double* px, double* py, double* vcos, const uint8_t* skip,
+                           cudaStream_t st) {
     const long long n = (long long)n_points * n_cams;
     if (n <= 0) return cudaSuccess;
     frustum_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n_cams, mtmc_inv, mtmc, cams, masks, n_points, pos, nrm, dmin, dmax, sf,
-                                                                n_levels, in_view, level, px, py, vcos);
+                                                                n_levels, in_view, level, px, py, vcos, skip);
     return cudaGetLastError();
 }
 

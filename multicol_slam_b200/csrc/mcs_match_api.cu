@@ -496,7 +496,7 @@ int mcs_project_mappoints(int32_t n_cams, const double* mtmc_inv, const double* 
     MCK(cudaMemcpy(dsf.p, scale_factors, n_levels * 8, cudaMemcpyHostToDevice));
     MCK(launch_frustum(n_cams, dmi.as<double>(), dm.as<double>(), dc.as<mcs_ocam>(), dk.as<uint8_t>(), n_points, dp.as<double>(),
                        dn.as<double>(), dmn.as<double>(), dmx.as<double>(), dsf.as<double>(), n_levels, div.as<uint8_t>(),
-                       dlv.as<int>(), dpx.as<double>(), dpy.as<double>(), dvc.as<double>(), nullptr));
+                       dlv.as<int>(), dpx.as<double>(), dpy.as<double>(), dvc.as<double>(), nullptr, nullptr));
     MCK(cudaMemcpy(in_view, div.p, n, cudaMemcpyDeviceToHost));
     MCK(cudaMemcpy(level, dlv.p, n * 4, cudaMemcpyDeviceToHost));
     MCK(cudaMemcpy(proj_x, dpx.p, n * 8, cudaMemcpyDeviceToHost));
@@ -618,6 +618,88 @@ int mcs_search_by_projection(const mcs_frame_view* f, const mcs_mappoint_view* m
     if (!having_masks) fv.dmask = nullptr;
     return mcs_search_windows(&fv, qs.data(), (int)qs.size(), mps->desc, having_masks ? mps->dmask : nullptr, tags.data(),
                               MCS_RULE_LEVEL_RATIO, nnratio, th_high, frame_mp, nmatches);
+}
+
+int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const double* mtmc, const mcs_ocam* cams, const uint8_t* masks_dev,
+                                 int32_t n_points, const double* world_pos_dev, const double* normal_dev, const double* min_dist_dev,
+                                 const double* max_dist_dev, const double* scale_factors, int32_t n_levels, const uint8_t* skip_dev,
+                                 uint8_t* in_view_dev, int32_t* level_dev, double* proj_x_dev, double* proj_y_dev, double* view_cos_dev,
+                                 void* stream) {
+    if (!mtmc_inv || !mtmc || !cams || !masks_dev || !world_pos_dev || !normal_dev || !min_dist_dev || !max_dist_dev || !scale_factors ||
+        !in_view_dev || !level_dev || !proj_x_dev || !proj_y_dev || !view_cos_dev)
+        return mfail(MCS_ERR_INVALID, "null argument");
+    if (n_cams < 1 || n_points < 0 || n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mfail(MCS_ERR_INVALID, "bad sizes");
+    for (int c = 0; c < n_cams; ++c)
+        if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
+            return mfail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
+    cudaStream_t st = (cudaStream_t)stream;
+    MCK(keep_pool_memory());
+    if (n_points == 0) return MCS_OK;
+    // poses, camera models and scale factors: one scratch block, staged in stream order
+    const size_t b_pose = (size_t)n_cams * 128, b_cam = sizeof(mcs_ocam) * n_cams, b_sf = 8 * (size_t)n_levels;
+    std::vector<uint8_t> h(2 * b_pose + b_cam + b_sf);
+    std::memcpy(h.data(), mtmc_inv, b_pose);
+    std::memcpy(h.data() + b_pose, mtmc, b_pose);
+    std::memcpy(h.data() + 2 * b_pose, cams, b_cam);
+    std::memcpy(h.data() + 2 * b_pose + b_cam, scale_factors, b_sf);
+    uint8_t* d = nullptr;
+    MCK(cudaMallocAsync((void**)&d, h.size(), st));
+    cudaError_t e = stage_to_device(h.data(), h.size(), d, st);
+    if (e == cudaSuccess)
+        e = launch_frustum(n_cams, (const double*)d, (const double*)(d + b_pose), (const mcs_ocam*)(d + 2 * b_pose), masks_dev, n_points,
+                           world_pos_dev, normal_dev, min_dist_dev, max_dist_dev, (const double*)(d + 2 * b_pose + b_cam), n_levels, in_view_dev,
+                           level_dev, proj_x_dev, proj_y_dev, view_cos_dev, skip_dev, st);
+    const cudaError_t ef = cudaFreeAsync(d, st);
+    MCK(e);
+    MCK(ef);
+    if (!stream) MCK(cudaStreamSynchronize(st));
+    return MCS_OK;
+}
+
+int mcs_search_by_projection_max_rounds(void) { return proj_search_max_rounds(); }
+
+int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int32_t part_images, int32_t first_image, int32_t n_cams,
+                                    int32_t capacity, int32_t dim, const int32_t* cam_width, const int32_t* cam_height, int32_t n_levels,
+                                    const double* scale_factors, const mcs_mappoint_dev_view* mps, double th, double nnratio, int32_t th_high,
+                                    int32_t having_masks, int32_t* frame_mp_dev, int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev,
+                                    void* stream) {
+    if (!packed_dev || !cam_width || !cam_height || !scale_factors || !mps || !frame_mp_dev || !nmatches_dev || !status_dev)
+        return mfail(MCS_ERR_INVALID, "null argument");
+    if (n_cams < 1 || n_parts < 1 || part_images < 1 || first_image < 0 || n_levels < 1 || n_levels > MCS_MAX_LEVELS || mps->n_points < 0)
+        return mfail(MCS_ERR_INVALID, "bad sizes");
+    if (capacity < 1 || capacity > 65535) return mfail(MCS_ERR_INVALID, "capacity must be 1..65535");
+    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    if ((long long)first_image + n_cams > (long long)n_parts * part_images)
+        return mfail(MCS_ERR_INVALID, "first_image + n_cams exceeds the images of the packed buffer");
+    if (!mps->in_view || !mps->level || !mps->proj_x || !mps->proj_y || !mps->view_cos || !mps->desc)
+        return mfail(MCS_ERR_INVALID, "null map-point array");
+    if (having_masks && !mps->dmask) return mfail(MCS_ERR_INVALID, "masks requested but not supplied");
+    for (int c = 0; c < n_cams; ++c)
+        if (cam_width[c] < 1 || cam_height[c] < 1) return mfail(MCS_ERR_INVALID, "camera sizes must be positive");
+    if ((long long)mps->n_points * n_cams >= (1LL << 24))
+        return mfail(MCS_ERR_UNSUPPORTED, "more than 2^24 - 1 (map point, camera) entries in one call");
+    cudaStream_t st = (cudaStream_t)stream;
+    MCK(keep_pool_memory());
+    // camera c = global image first_image + c = image (g mod part_images) of part g / part_images
+    size_t off[4];
+    const size_t part_bytes = mcs_packed_layout(part_images, capacity, dim, off);
+    std::vector<PsCamSlots> slots(n_cams);
+    for (int c = 0; c < n_cams; ++c) {
+        const int g = first_image + c, p = g / part_images, i = g - p * part_images;
+        const uint8_t* b = (const uint8_t*)packed_dev + (size_t)p * part_bytes;
+        slots[c] = PsCamSlots{(const int*)(b + off[0]) + i, (const mcs_keypoint*)(b + off[1]) + (size_t)i * capacity,
+                              b + off[2] + (size_t)i * capacity * dim, b + off[3] + (size_t)i * capacity * dim};
+    }
+    ProjSearchArgs a{};
+    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.n_levels = n_levels; a.n_points = mps->n_points;
+    a.cams = slots.data(); a.cam_w = cam_width; a.cam_h = cam_height; a.sf = scale_factors;
+    a.bad = mps->bad; a.in_view = mps->in_view; a.level = mps->level; a.px = mps->proj_x; a.py = mps->proj_y; a.vcos = mps->view_cos;
+    a.mp_desc = mps->desc; a.mp_dmask = having_masks ? mps->dmask : nullptr;
+    a.th = th; a.nnratio = nnratio; a.th_high = th_high; a.masked = having_masks != 0;
+    a.frame_mp = frame_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
+    MCK(launch_search_by_projection(a, st));
+    if (!stream) MCK(cudaStreamSynchronize(st));
+    return MCS_OK;
 }
 
 int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view* f2, double* prev_matched, int32_t window_size,

@@ -1,0 +1,497 @@
+// proj_search_kernels.cu -- SearchByProjection(F, vpMapPoints, th) (ref src/cORBmatcher.cpp:67-166) with every input and output
+// resident on the device: the frame comes straight from the packed feature buffer (mcs_packed_layout), the map points from
+// the arrays mcs_project_mappoints_device fills, and the reference's ordered greedy acceptance runs on the device.
+//
+//   ps_gather_kernel    the frame's keypoints / descriptors / masks in slot order (slot = cam * capacity + j); empty slots get a
+//                       position outside every image, so the unchanged frame_prepare_kernel leaves them out of the grid
+//   ps_count / ps_fill  the query array in the reference's order (map point outer, camera inner), a count / scan / fill over
+//                       in_view and bad
+//   ps_list_kernel      per query the K smallest (distance, visiting position) keys of its window and the true candidate count
+//   ps_round_kernel     one round of the fixpoint iteration of the ordered acceptance (DESIGN.md section 4)
+//   ps_walk_kernel      the sequential fallback past the round cap: one warp per camera walks the unsettled queries in order
+//
+// No kernel reads anything back to the host: every size that depends on the data (the number of queries, the rounds the
+// fixpoint needed, where the walk starts) lives in device memory and the kernels are launched for the upper bound.
+#include <algorithm>
+#include <climits>
+#include <cstring>
+#include <vector>
+
+#include "kernels.h"
+
+namespace mcs {
+
+// ------------------------------------------------------------------------------------------------
+// small host inputs, staged through a kernel parameter: a pageable cudaMemcpyAsync may wait for the stream
+// ------------------------------------------------------------------------------------------------
+namespace {
+constexpr int kStageBytes = 3968;
+struct StageBlob { unsigned char b[kStageBytes]; };
+__global__ void stage_kernel(const StageBlob blob, const int n, unsigned char* __restrict__ dst) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = blob.b[i];
+}
+}  // namespace
+
+cudaError_t stage_to_device(const void* host, size_t bytes, void* dev, cudaStream_t st) {
+    const unsigned char* src = (const unsigned char*)host;
+    for (size_t off = 0; off < bytes; off += kStageBytes) {
+        const int n = (int)std::min<size_t>(kStageBytes, bytes - off);
+        StageBlob blob;
+        std::memcpy(blob.b, src + off, n);
+        stage_kernel<<<1, 256, 0, st>>>(blob, n, (unsigned char*)dev + off);
+    }
+    return cudaGetLastError();
+}
+
+namespace {
+
+constexpr int kPsK = 8;                      // list length per query
+constexpr int kPsRounds = 8;                 // fixpoint rounds before the walk takes over
+constexpr unsigned kNoKey = 0xFFFFFFFFu;
+constexpr int kNoChange = 0x7F7F7F7F;        // memset(0x7F): no decision changed in that round
+constexpr int kQbThreads = 256, kQbPer = 8, kQbTile = kQbThreads * kQbPer;
+static_assert(kPsRounds < 255, "round versions live in the top byte of the owner words");
+
+// ---- frame view from the packed slots ----
+__global__ void ps_gather_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, const int dim,
+                                 const bool masked, mcs_keypoint* __restrict__ keys, int* __restrict__ key_cam,
+                                 uint8_t* __restrict__ desc, uint8_t* __restrict__ dmask) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_cams * capacity) return;
+    const int c = s / capacity, j = s - c * capacity;
+    const PsCamSlots cs = cams[c];
+    const int n = min(*cs.count, capacity);
+    key_cam[s] = c;
+    const int v4 = dim / 16;
+    if (j < n) {
+        keys[s] = cs.kps[j];
+        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = ((const uint4*)cs.desc)[(size_t)j * v4 + k];
+        if (masked)
+            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = ((const uint4*)cs.dmask)[(size_t)j * v4 + k];
+    } else {
+        mcs_keypoint e{};
+        e.x = e.y = -1.0e6f;                 // PosInGrid falls outside the image: never a candidate
+        keys[s] = e;
+        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = make_uint4(0, 0, 0, 0);
+        if (masked)
+            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = make_uint4(0, 0, 0, 0);
+    }
+}
+
+// ---- query build: entry k = point * n_cams + cam is a query when the point is not bad and in view ----
+struct QbArgs {
+    int n_cams, n_points, n_levels;
+    const uint8_t* bad; const uint8_t* in_view; const int* level;
+};
+__device__ __forceinline__ bool qb_valid(const QbArgs& a, long long k, int* status) {
+    if (k >= (long long)a.n_points * a.n_cams) return false;
+    const int i = (int)(k / a.n_cams);
+    if (a.bad && a.bad[i]) return false;
+    if (!a.in_view[k]) return false;
+    const int lvl = a.level[k];
+    if (lvl < 0 || lvl >= a.n_levels) {       // the host call refuses such input; here the query is dropped and flagged
+        if (status) *status = MCS_ERR_INVALID;
+        return false;
+    }
+    return true;
+}
+
+__global__ void __launch_bounds__(kQbThreads) ps_count_kernel(const QbArgs a, int* __restrict__ block_count, int* __restrict__ status) {
+    int total = 0;
+    for (int i = 0; i < kQbPer; ++i) {
+        const long long k = (long long)blockIdx.x * kQbTile + i * kQbThreads + threadIdx.x;
+        total += __syncthreads_count(qb_valid(a, k, status));
+    }
+    if (threadIdx.x == 0) block_count[blockIdx.x] = total;
+}
+
+// exclusive scan of the block counts (one CTA), total -> *nq
+__global__ void __launch_bounds__(1024) ps_scan_kernel(const int* __restrict__ block_count, const int nb, int* __restrict__ block_off,
+                                                       int* __restrict__ nq) {
+    __shared__ int s[1024];
+    int carry = 0;
+    for (int base = 0; base < nb; base += 1024) {
+        const int i = base + threadIdx.x;
+        const int v = i < nb ? block_count[i] : 0;
+        s[threadIdx.x] = v;
+        __syncthreads();
+        for (int o = 1; o < 1024; o <<= 1) {
+            const int t = threadIdx.x >= o ? s[threadIdx.x - o] : 0;
+            __syncthreads();
+            s[threadIdx.x] += t;
+            __syncthreads();
+        }
+        if (i < nb) block_off[i] = carry + s[threadIdx.x] - v;
+        carry += s[1023];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *nq = carry;
+}
+
+__global__ void __launch_bounds__(kQbThreads) ps_fill_kernel(const QbArgs a, const int* __restrict__ block_off, const double* __restrict__ proj_x,
+                                                             const double* __restrict__ proj_y, const double* __restrict__ view_cos,
+                                                             const double* __restrict__ sf, const double th, mcs_window_query* __restrict__ qry) {
+    __shared__ int s_w[kQbThreads / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int run = block_off[blockIdx.x];
+    for (int i = 0; i < kQbPer; ++i) {
+        const long long k = (long long)blockIdx.x * kQbTile + i * kQbThreads + threadIdx.x;
+        const bool v = qb_valid(a, k, nullptr);
+        const unsigned m = __ballot_sync(0xffffffffu, v);
+        if (lane == 0) s_w[w] = __popc(m);
+        __syncthreads();
+        int off = run, tot = 0;
+        for (int u = 0; u < kQbThreads / 32; ++u) { if (u < w) off += s_w[u]; tot += s_w[u]; }
+        if (v) {
+            const int lvl = a.level[k];
+            double r = view_cos[k] > 0.998 ? 2.5 : 4.0;      // RadiusByViewingCos (ref :169-175)
+            if (th != 1.0) r *= th;
+            mcs_window_query q;
+            q.cam = (int)(k % a.n_cams); q.min_level = lvl - 1; q.max_level = lvl; q.desc_index = (int)(k / a.n_cams);
+            q.x = proj_x[k]; q.y = proj_y[k]; q.r = r * sf[lvl];
+            qry[off + __popc(m & ((1u << lane) - 1u))] = q;
+        }
+        run += tot;
+        __syncthreads();
+    }
+}
+
+// ---- window search keeping the KB smallest (distance << 16 | visiting position) keys of the candidates not taken ----
+// Mirrors window_search_kernel (GetFeaturesInArea, ref src/cMultiFrame.cpp:272-340): same cell range, visiting order, level filter
+// and distance.  Every lane ends with the same sorted list.  Returns the number of candidates in the window (taken ones included).
+struct NoneTaken { __device__ bool operator()(int) const { return false; } };
+
+template <int WORDS, bool MASKED, int KB, class Taken>
+__device__ __forceinline__ int window_kbest(const WindowFrameDev& f, const mcs_window_query& qq, const uint32_t* __restrict__ qdesc,
+                                            const uint32_t* __restrict__ qmask, const Taken& taken, unsigned (&key)[KB], int (&slot)[KB]) {
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int k = 0; k < KB; ++k) { key[k] = kNoKey; slot[k] = -1; }
+    const int cam = qq.cam;
+    const double x = qq.x, y = qq.y, r = qq.r;
+    const double wi = f.winv[cam], hi = f.hinv[cam];
+    int cx0 = (int)floor((x - 0 - r) * wi); cx0 = max(0, cx0); if (cx0 >= MCS_FRAME_GRID_COLS) return 0;
+    int cx1 = (int)ceil((x - 0 + r) * wi);  cx1 = min(MCS_FRAME_GRID_COLS - 1, cx1); if (cx1 < 0) return 0;
+    int cy0 = (int)floor((y - 0 - r) * hi); cy0 = max(0, cy0); if (cy0 >= MCS_FRAME_GRID_ROWS) return 0;
+    int cy1 = (int)ceil((y - 0 + r) * hi);  cy1 = min(MCS_FRAME_GRID_ROWS - 1, cy1); if (cy1 < 0) return 0;
+    uint32_t qw[WORDS], qm[MASKED ? WORDS : 1];
+#pragma unroll
+    for (int k = 0; k < WORDS; ++k) {
+        qw[k] = qdesc[(size_t)qq.desc_index * WORDS + k];
+        if (MASKED) qm[k] = qmask[(size_t)qq.desc_index * WORDS + k];
+    }
+    const bool check = !(qq.min_level == -1 && qq.max_level == -1);
+    const bool same = check && qq.min_level == qq.max_level;
+    int count = 0;
+    for (int ix = cx0; ix <= cx1; ++ix)
+        for (int iy = cy0; iy <= cy1; ++iy) {
+            const int cell = (cam * MCS_FRAME_GRID_COLS + ix) * MCS_FRAME_GRID_ROWS + iy;
+            const int s = f.cell_start[cell], e = f.cell_start[cell + 1];
+            for (int base = s; base < e; base += 32) {
+                const int it = base + lane;
+                bool ok = it < e;
+                int id = 0;
+                if (ok) {
+                    id = f.cell_items[it];
+                    const int oct = f.koct[id];
+                    if (check && !same) ok = !(oct < qq.min_level || oct > qq.max_level);
+                    else if (same) ok = (oct == qq.min_level);
+                    if (ok) ok = !(fabs((double)f.kx[id] - x) > r || fabs((double)f.ky[id] - y) > r);
+                }
+                const unsigned m = __ballot_sync(0xffffffffu, ok);
+                const bool cand = ok && !taken(id);
+                unsigned kk = kNoKey;
+                if (cand) {
+                    const uint32_t* dd = (const uint32_t*)f.desc + (size_t)id * WORDS;
+                    unsigned dist = 0;
+                    if (MASKED) {
+                        const uint32_t* mm = (const uint32_t*)f.dmask + (size_t)id * WORDS;
+#pragma unroll
+                        for (int k = 0; k < WORDS; ++k) {
+                            const uint32_t xw = qw[k] ^ dd[k];
+                            dist += __popc(xw & qm[k]) + __popc(xw & mm[k]);
+                        }
+                        dist >>= 1;
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < WORDS; ++k) dist += __popc(qw[k] ^ dd[k]);
+                    }
+                    kk = (dist << 16) | (unsigned)(count + __popc(m & ((1u << lane) - 1u)));
+                }
+                unsigned ins = __ballot_sync(0xffffffffu, cand && kk < key[KB - 1]);
+                while (ins) {
+                    const int b = __ffs(ins) - 1;
+                    ins &= ins - 1;
+                    unsigned nk = __shfl_sync(0xffffffffu, kk, b);
+                    int ns = __shfl_sync(0xffffffffu, id, b);
+#pragma unroll
+                    for (int k = 0; k < KB; ++k)
+                        if (nk < key[k]) { const unsigned tk = key[k]; key[k] = nk; nk = tk; const int ts = slot[k]; slot[k] = ns; ns = ts; }
+                }
+                count += __popc(m);
+            }
+        }
+    return count;
+}
+
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(256) ps_list_kernel(const WindowFrameDev f, const mcs_window_query* __restrict__ qry, const int* __restrict__ nq_p,
+                                                      const uint32_t* __restrict__ qdesc, const uint32_t* __restrict__ qmask,
+                                                      unsigned* __restrict__ lkey, int* __restrict__ lslot, int* __restrict__ lcnt) {
+    const int lane = threadIdx.x & 31, nq = *nq_p;
+    const int stride = gridDim.x * (blockDim.x >> 5);
+    for (int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; q < nq; q += stride) {
+        unsigned key[kPsK]; int slot[kPsK];
+        const int n = window_kbest<WORDS, MASKED, kPsK>(f, qry[q], qdesc, qmask, NoneTaken{}, key, slot);
+#pragma unroll
+        for (int k = 0; k < kPsK; ++k)
+            if (lane == k) { lkey[(size_t)q * kPsK + k] = key[k]; lslot[(size_t)q * kPsK + k] = slot[k]; }
+        if (lane == 0) lcnt[q] = n;
+    }
+}
+
+// The decision of one query (warp-uniform) under a "keypoint already taken" predicate: best / second best free candidate by
+// (distance, visiting position) -- what the sequential strict-< update of ref :138-150 picks -- and the acceptance of :154-160.
+// The list decides when it holds two free entries or every candidate; otherwise the window is scanned again with the predicate.
+template <int WORDS, bool MASKED, class Taken>
+__device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_window_query& qq, const unsigned* lk, const int* ls, const int cnt,
+                                         const uint32_t* qdesc, const uint32_t* qmask, const Taken& taken, const int th_high,
+                                         const double nnratio, int* rescans) {
+    const int lane = threadIdx.x & 31;
+    unsigned k = kNoKey; int s = -1; bool fr = false;
+    if (lane < kPsK) { k = lk[lane]; s = ls[lane]; fr = k != kNoKey && !taken(s); }
+    const unsigned fm = __ballot_sync(0xffffffffu, fr);
+    unsigned k0 = kNoKey, k1 = kNoKey; int s0 = -1, s1 = -1;
+    if (__popc(fm) >= 2 || cnt <= kPsK) {
+        const int b0 = fm ? __ffs(fm) - 1 : 0;
+        const unsigned rest = fm & (fm - 1);
+        const int b1 = rest ? __ffs(rest) - 1 : 0;
+        const unsigned x0 = __shfl_sync(0xffffffffu, k, b0), x1 = __shfl_sync(0xffffffffu, k, b1);
+        const int y0 = __shfl_sync(0xffffffffu, s, b0), y1 = __shfl_sync(0xffffffffu, s, b1);
+        if (fm) { k0 = x0; s0 = y0; }
+        if (rest) { k1 = x1; s1 = y1; }
+    } else {
+        unsigned kk[2]; int ss[2];
+        window_kbest<WORDS, MASKED, 2>(f, qq, qdesc, qmask, taken, kk, ss);
+        k0 = kk[0]; s0 = ss[0]; k1 = kk[1]; s1 = ss[1];
+        if (lane == 0 && rescans) atomicAdd(rescans, 1);
+    }
+    if (s0 < 0) return -1;
+    const int d0 = (int)(k0 >> 16), l0 = f.koct[s0];
+    const int d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX, l1 = s1 >= 0 ? f.koct[s1] : -1;
+    const bool ok = d0 <= th_high && !(l0 == l1 && (double)d0 > nnratio * (double)d1);
+    return ok ? s0 : -1;
+}
+
+struct PsState {                 // device scratch shared by the acceptance kernels
+    const mcs_window_query* qry;
+    const unsigned* lkey; const int* lslot; const int* lcnt;
+    int* dec;                    // [2][Q] decisions of the last two rounds (accepted slot or -1)
+    unsigned* owner;             // [2][n_slots] ((kPsRounds - round) << 24 | smallest accepting query)
+    int* ctl;                    // [0] nq  [1] rounds run  [2] rescans  [3] walk start  [4 ..] first changed query of each round
+    int Q, n_slots, capacity, th_high;
+    double nnratio;
+};
+__device__ __forceinline__ int* ps_chg(const PsState& p) { return p.ctl + 4; }
+
+// Round r: every query not yet settled decides, treating a keypoint as taken when frame_mp had it on entry or a query with a
+// smaller index accepted it in round r - 1.  Queries below the first one whose decision changed in round r - 1 are final
+// (query p reads only decisions of queries < p) and only republish their keypoint.
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(256, 2) ps_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
+                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
+    const int* chg = ps_chg(p);
+    const int settled = r >= 2 ? chg[r - 1] : 0;
+    if (settled == kNoChange) return;                         // converged in an earlier round
+    const int lane = threadIdx.x & 31, nq = p.ctl[0];
+    if (blockIdx.x == 0 && threadIdx.x == 0) p.ctl[1] = r + 1;
+    int* dec_cur = p.dec + (size_t)(r & 1) * p.Q;
+    const int* dec_prev = p.dec + (size_t)((r + 1) & 1) * p.Q;
+    unsigned* own_cur = p.owner + (size_t)(r & 1) * p.n_slots;
+    const unsigned* own_prev = p.owner + (size_t)((r + 1) & 1) * p.n_slots;
+    const unsigned ver_cur = (unsigned)(kPsRounds - r) << 24, ver_prev = (unsigned)(kPsRounds - r + 1) << 24;
+    const int stride = gridDim.x * (blockDim.x >> 5);
+    for (int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; q < nq; q += stride) {
+        if (q < settled) {                                    // dec_cur[q] holds round r - 2, equal to round r - 1 below `settled`
+            if (lane == 0) { const int d = dec_cur[q]; if (d >= 0) atomicMin(&own_cur[d], ver_cur | (unsigned)q); }
+            continue;
+        }
+        auto taken = [=](int s) {
+            if (fmp_in[s] >= 0) return true;
+            if (r == 0) return false;
+            const unsigned v = own_prev[s];
+            return (v & 0xFF000000u) == ver_prev && (int)(v & 0xFFFFFFu) < q;
+        };
+        const int d = ps_decide<WORDS, MASKED>(f, p.qry[q], p.lkey + (size_t)q * kPsK, p.lslot + (size_t)q * kPsK, p.lcnt[q], qdesc, qmask,
+                                               taken, p.th_high, p.nnratio, p.ctl + 2);
+        if (lane == 0) {
+            dec_cur[q] = d;
+            if (d >= 0) atomicMin(&own_cur[d], ver_cur | (unsigned)q);
+            if (r >= 1 && d != dec_prev[q]) atomicMin(&p.ctl[4 + r], q);
+        }
+    }
+}
+
+// Writes the final decisions of the settled prefix into frame_mp and counts them; records where the walk has to start.
+__global__ void __launch_bounds__(256) ps_finalize_kernel(const PsState p, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
+    __shared__ int s_n;
+    const int nq = p.ctl[0], rl = p.ctl[1] - 1;
+    int S = rl >= 1 ? ps_chg(p)[rl] : 0;
+    if (S == kNoChange || S > nq) S = nq;
+    const int* dec = p.dec + (size_t)(rl & 1) * p.Q;
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    int n = 0;
+    for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < S; q += gridDim.x * blockDim.x) {
+        const int d = dec[q];
+        if (d >= 0) { frame_mp[d] = p.qry[q].desc_index; ++n; }
+    }
+    if (n) atomicAdd(&s_n, n);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        if (s_n) atomicAdd(nmatches, s_n);
+        if (blockIdx.x == 0) p.ctl[3] = S < nq ? S : -1;
+    }
+}
+
+// Fallback past the round cap: one warp per camera walks its queries from the first unsettled one in order, with the camera's
+// taken keypoints as a bitmap in shared memory.
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(32) ps_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
+                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
+    extern __shared__ unsigned s_bits[];
+    const int S = p.ctl[3];
+    if (S < 0) return;
+    const int c = blockIdx.x, lane = threadIdx.x, nq = p.ctl[0], cap = p.capacity;
+    const int* fmp = frame_mp + (size_t)c * cap;
+    for (int w = lane; w < (cap + 31) / 32; w += 32) {
+        unsigned b = 0;
+        for (int k = 0; k < 32 && w * 32 + k < cap; ++k) b |= (fmp[w * 32 + k] >= 0 ? 1u : 0u) << k;
+        s_bits[w] = b;
+    }
+    __syncwarp();
+    auto taken = [=](int s) { const int j = s - c * cap; return ((s_bits[j >> 5] >> (j & 31)) & 1u) != 0; };
+    int nm = 0;
+    for (int base = S; base < nq; base += 32) {
+        const int q = base + lane;
+        unsigned m = __ballot_sync(0xffffffffu, q < nq && p.qry[q].cam == c);
+        while (m) {
+            const int qi = base + __ffs(m) - 1;
+            m &= m - 1;
+            const mcs_window_query qq = p.qry[qi];
+            const int d = ps_decide<WORDS, MASKED>(f, qq, p.lkey + (size_t)qi * kPsK, p.lslot + (size_t)qi * kPsK, p.lcnt[qi], qdesc, qmask,
+                                                   taken, p.th_high, p.nnratio, p.ctl + 2);
+            if (d >= 0) {
+                if (lane == 0) {
+                    const int j = d - c * cap;
+                    s_bits[j >> 5] |= 1u << (j & 31);
+                    frame_mp[d] = qq.desc_index;
+                }
+                ++nm;
+            }
+            __syncwarp();
+        }
+    }
+    if (lane == 0 && nm) atomicAdd(nmatches, nm);
+}
+
+__global__ void ps_diag_kernel(const int* __restrict__ ctl, int* __restrict__ diag) {
+    diag[0] = ctl[1];        // fixpoint rounds run
+    diag[1] = ctl[1] ? ctl[3] : -1;   // first query of the walk, -1 = the rounds settled every query
+    diag[2] = ctl[0];        // queries
+    diag[3] = ctl[2];        // decisions that rescanned their window
+}
+
+size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+}  // namespace
+
+int proj_search_max_rounds() { return kPsRounds; }
+
+cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    const int ncell = a.n_cams * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
+    const long long Q = (long long)a.n_points * a.n_cams;
+    const int nb = (int)((Q + kQbTile - 1) / kQbTile);
+    const size_t db = (size_t)NS * a.dim;
+    // one stream-ordered scratch block, carved below
+    const size_t sizes[] = {
+        sizeof(mcs_ocam) * a.n_cams, sizeof(double) * a.n_levels, sizeof(PsCamSlots) * a.n_cams,          // staged host inputs
+        sizeof(mcs_keypoint) * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, db, a.masked ? db : 0,     // keys key_cam kx ky koct desc dmask
+        4ull * NS, 4ull * ncell, 4ull * (ncell + 1), 4ull * NS, 8ull * a.n_cams, 8ull * a.n_cams,          // cell_of cursor start items winv hinv
+        4ull * (nb + 1), 4ull * (nb + 1), 4ull * (4 + kPsRounds),                                          // block counts / offsets, ctl
+        sizeof(mcs_window_query) * Q, 4ull * Q * kPsK, 4ull * Q * kPsK, 4ull * Q, 8ull * Q, 8ull * NS};    // qry lkey lslot lcnt dec owner
+    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
+    size_t off[nsz], total = 0;
+    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
+    cudaError_t e = keep_pool_memory();
+    if (e != cudaSuccess) return e;
+    int dev = 0, sms = 132;
+    e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return e;
+    uint8_t* base = nullptr;
+    e = cudaMallocAsync((void**)&base, total, st);
+    if (e != cudaSuccess) return e;
+    auto at = [&](int i) { return (void*)(base + off[i]); };
+    mcs_ocam* cams = (mcs_ocam*)at(0); double* sf = (double*)at(1); PsCamSlots* slots = (PsCamSlots*)at(2);
+    mcs_keypoint* keys = (mcs_keypoint*)at(3); int* key_cam = (int*)at(4); float* kx = (float*)at(5); float* ky = (float*)at(6);
+    int* koct = (int*)at(7); uint8_t* desc = (uint8_t*)at(8); uint8_t* dmask = a.masked ? (uint8_t*)at(9) : nullptr;
+    int* cell_of = (int*)at(10); int* cursor = (int*)at(11); int* cell_start = (int*)at(12); int* cell_items = (int*)at(13);
+    double* winv = (double*)at(14); double* hinv = (double*)at(15);
+    int* bcount = (int*)at(16); int* boff = (int*)at(17); int* ctl = (int*)at(18);
+    mcs_window_query* qry = (mcs_window_query*)at(19); unsigned* lkey = (unsigned*)at(20); int* lslot = (int*)at(21); int* lcnt = (int*)at(22);
+    int* dec = (int*)at(23); unsigned* owner = (unsigned*)at(24);
+
+    std::vector<mcs_ocam> hc(a.n_cams);
+    std::memset(hc.data(), 0, sizeof(mcs_ocam) * a.n_cams);
+    for (int c = 0; c < a.n_cams; ++c) { hc[c].width = a.cam_w[c]; hc[c].height = a.cam_h[c]; }
+    if (e == cudaSuccess) e = stage_to_device(hc.data(), sizeof(mcs_ocam) * a.n_cams, cams, st);
+    if (e == cudaSuccess) e = stage_to_device(a.sf, sizeof(double) * a.n_levels, sf, st);
+    if (e == cudaSuccess) e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, slots, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.nmatches, 0, 4, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctl, 0, 16, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctl + 4, 0x7F, 4 * kPsRounds, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(owner, 0xFF, 8ull * NS, st);
+    if (e != cudaSuccess) { cudaFreeAsync(base, st); return e; }
+
+    // frame view in slot order and its grid (the kernel the host entry points build their grid with)
+    ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
+    e = launch_frame_prepare(keys, key_cam, NS, cams, a.n_cams, kx, ky, koct, nullptr, cell_of, cursor, cell_start, cell_items, winv, hinv, st);
+    // queries in the reference's order
+    const QbArgs qa{a.n_cams, a.n_points, a.n_levels, a.bad, a.in_view, a.level};
+    if (e == cudaSuccess && nb > 0) {
+        ps_count_kernel<<<nb, kQbThreads, 0, st>>>(qa, bcount, a.status);
+        ps_scan_kernel<<<1, 1024, 0, st>>>(bcount, nb, boff, ctl);
+        ps_fill_kernel<<<nb, kQbThreads, 0, st>>>(qa, boff, a.px, a.py, a.vcos, sf, a.th, qry);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && Q > 0) {
+        const WindowFrameDev f{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv};
+        const PsState p{qry, lkey, lslot, lcnt, dec, owner, ctl, (int)Q, NS, a.capacity, a.th_high, a.nnratio};
+        const uint32_t* qd = (const uint32_t*)a.mp_desc;
+        const uint32_t* qm = a.masked ? (const uint32_t*)a.mp_dmask : nullptr;
+        const int wblocks = (int)std::min<long long>((Q + 7) / 8, (long long)sms * 16);
+        const int fblocks = (int)std::min<long long>((Q + 255) / 256, (long long)sms * 4);
+        const size_t walk_smem = 4ull * ((a.capacity + 31) / 32);
+#define MCS_PS(W, M)                                                                                                   \
+        {                                                                                                              \
+            ps_list_kernel<W, M><<<wblocks, 256, 0, st>>>(f, qry, ctl, qd, qm, lkey, lslot, lcnt);                     \
+            for (int r = 0; r < kPsRounds; ++r) ps_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qm, a.frame_mp); \
+            ps_finalize_kernel<<<fblocks, 256, 0, st>>>(p, a.frame_mp, a.nmatches);                                    \
+            ps_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qm, a.frame_mp, a.nmatches);               \
+        }
+        if (a.dim == 16) { if (a.masked) MCS_PS(4, true) else MCS_PS(4, false) }
+        else if (a.dim == 32) { if (a.masked) MCS_PS(8, true) else MCS_PS(8, false) }
+        else { if (a.masked) MCS_PS(16, true) else MCS_PS(16, false) }
+#undef MCS_PS
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && a.diag) ps_diag_kernel<<<1, 1, 0, st>>>(ctl, a.diag);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    const cudaError_t ef = cudaFreeAsync(base, st);
+    return e != cudaSuccess ? e : ef;
+}
+
+}  // namespace mcs

@@ -42,6 +42,11 @@ class MapPointView(C.Structure):
                 ("dmask", C.c_void_p)]
 
 
+class MapPointDevView(C.Structure):
+    """mcs_mappoint_dev_view: the same fields as MapPointView, every pointer in device memory"""
+    _fields_ = MapPointView._fields_
+
+
 import numpy as np
 
 # numpy dtype binary-compatible with mcs_keypoint / cv::KeyPoint (28 bytes)
