@@ -25,7 +25,8 @@ GOLD = ROOT / "tests" / "golden"
 ORB, DBRIEF, MDBRIEF = dict(), dict(do_dbrief=True), dict(do_dbrief=True, learn_masks=True)
 
 # (name, camera spec, seed, constructor arguments, store full outputs?)
-#   camera spec: Lafida index, or (index, width, height) for a rescaled sensor, or (index, "nomask") for mirrorMask 0
+#   camera spec: Lafida index, or (index, width, height) for a rescaled sensor, or (index, "nomask") for mirrorMask 0, or the name
+#   of a calibration in tests/golden/synthetic_cams.json
 CASES = [
     # the configuration the reference ships: plain ORB, 400 features (Examples/Lafida/Slam_Settings_indoor1.yaml:12-27)
     ("shipped_orb400_cam0", 0, 11, dict(nfeatures=400, **ORB), True),
@@ -51,11 +52,26 @@ CASES = [
     ("cfg3_1280x720_mdbrief2000", (0, 1280, 720), 41, dict(nfeatures=2000, **MDBRIEF), False),
     ("cfg4_1920x1080_mdbrief4000", (1, 1920, 1080), 42, dict(nfeatures=4000, **MDBRIEF), False),
     ("small_333x211_l4_orb", (2, 333, 211), 43, dict(nfeatures=300, nlevels=4, **ORB), True),
+    # fisheye calibrations other than Lafida's (tests/golden/synthetic_cams.json): each drives the descriptor kernel down another path
+    ("syn_equidistant185_mdbrief1000", "equidistant185", 51, dict(nfeatures=1000, **MDBRIEF), False),
+    ("syn_equisolid230_dbrief1000", "equisolid230", 52, dict(nfeatures=1000, **DBRIEF), False),
+    ("syn_equisolid230_mdbrief300", "equisolid230", 53, dict(nfeatures=300, **MDBRIEF), True),
+    ("syn_stereographic170_orb400", "stereographic170", 54, dict(nfeatures=400, **ORB), True),
+    ("syn_stereographic170_mdbrief1000", "stereographic170", 55, dict(nfeatures=1000, **MDBRIEF), False),
+    ("syn_affine185_mdbrief1000", "affine185", 56, dict(nfeatures=1000, **MDBRIEF), False),
+    ("syn_affine185_mdbrief_desc16", "affine185", 57, dict(nfeatures=500, desc_size=16, **MDBRIEF), False),
+    ("syn_wide1920x1080_195_mdbrief4000", "wide1920x1080_195", 58, dict(nfeatures=4000, **MDBRIEF), False),
+    ("syn_narrow1280x720_120_dbrief2000", "narrow1280x720_120", 59, dict(nfeatures=2000, **DBRIEF), False),
+    ("syn_magnify130_mdbrief1000", "magnify130", 60, dict(nfeatures=1000, **MDBRIEF), False),
+    ("syn_magnify130_mdbrief_desc64", "magnify130", 61, dict(nfeatures=500, desc_size=64, **MDBRIEF), False),
+    ("syn_magnify130_dbrief300", "magnify130", 62, dict(nfeatures=300, **DBRIEF), True),
 ]
 
 
 def make_cam(spec):
     cams = synth.lafida_cams()
+    if isinstance(spec, str):
+        return next(c for c in json.loads((GOLD / "synthetic_cams.json").read_text()) if c["name"] == spec)
     if isinstance(spec, int):
         return dict(cams[spec])
     if spec[1] == "nomask":
@@ -69,8 +85,10 @@ def crc(a):
     return zlib.crc32(np.ascontiguousarray(a).tobytes())
 
 
-def main():
+def main(only=None):
     for name, spec, seed, kw, full in CASES:
+        if only and not name.startswith(only):
+            continue
         cam = make_cam(spec)
         img = synth.frame(cam, seed)
         mask = ra.mirror_mask(cam)                       # the reference's own CreateMirrorMask (or all ones)
@@ -94,4 +112,4 @@ def main():
 if __name__ == "__main__":
     if not ra.available():
         raise SystemExit("oracle/_ref/libmcs_ref.so is missing: run `make -C oracle ref` where /root/reference exists")
-    main()
+    main(sys.argv[1] if len(sys.argv) > 1 else None)

@@ -6,11 +6,17 @@ in numpy long double:  R(r) = rho(atan(-z / r)),  rho = the inverse polynomial o
   tier 1   s-form  R(i + s) - R(i) = s' q(s'), s' = s / 32                       |error| < 1e-6 px
            m-form  G(c_i + hw_i t) - G(c_i) = t P(t), G(m) = R(sqrt m) / sqrt m  |error| (i + 1) < 1e-6 px
 with the float coefficients exactly as the kernel reads them."""
+import json
+import pathlib
+
 import numpy as np
 import pytest
 
 LD = np.longdouble
 REACH = 22.5
+# fisheye calibrations unlike Lafida's (tests/golden/make_synthetic_cams.py), each meant for one path of the descriptor kernel
+SYNTHETIC = {c["name"]: c for c in json.loads((pathlib.Path(__file__).resolve().parent / "golden" / "synthetic_cams.json").read_text())}
+LAFIDA_M_START = range(62, 68)        # where the m-form rows start on the three Lafida cameras
 
 
 def horner(c, x):
@@ -29,10 +35,16 @@ def floats_of(row, first, count):
     return np.frombuffer(np.ascontiguousarray(row[first:first + (count + 1) // 2]).tobytes(), np.float32)[:count].astype(LD)
 
 
-@pytest.mark.parametrize("which", [0, 1, 2, "hd"])
+def form_start(T, col):
+    """first row from which every row but the last has the tier-1 form flagged in column col (17: s-form, 23: m-form)"""
+    on = T[:-1, col] == 1.0
+    return len(on) - int(np.argmin(on[::-1])) if not on.all() else 0
+
+
+@pytest.mark.parametrize("which", [0, 1, 2, "hd"] + list(SYNTHETIC))
 def test_tables_against_the_camera_model(api, cams, which):
     from multicol_slam_b200 import synth
-    cam = synth.scaled_cam(cams[1], 1920, 1080) if which == "hd" else cams[which]
+    cam = synth.scaled_cam(cams[1], 1920, 1080) if which == "hd" else SYNTHETIC[which] if which in SYNTHETIC else cams[which]
     T = api.distort_table(cam)
     n, stride = T.shape
     assert stride == 24 and 200 < n <= 8192
@@ -68,11 +80,21 @@ def test_tables_against_the_camera_model(api, cams, which):
             assert abs(float(G(np.array([c]))[0]) - row[18]) < 1e-14
             assert err * (i + 1) < 1.2e-6, (i, float(err * (i + 1)))
             n1m += 1
-    # coverage: tier 2 everywhere, the s-form from radius 40..54 on and the m-form from 62..67 on (Lafida cameras), never below 40
+    # coverage: tier 2 everywhere, tier 1 never below 39
     assert n2 > 100 and n1s > 80 and n1m > 60
     assert not np.isnan(T[:, 0]).any()
-    assert all(T[i, 17] == 1.0 for i in range(56, n - 1)) and all(T[i, 23] == 1.0 for i in range(72, n - 1))
     assert not any(T[i, 17] == 1.0 or T[i, 23] == 1.0 for i in range(0, 39))
+    if which not in SYNTHETIC:
+        # Lafida cameras: the s-form from radius 40..54 on and the m-form from 62..67 on
+        assert all(T[i, 17] == 1.0 for i in range(56, n - 1)) and all(T[i, 23] == 1.0 for i in range(72, n - 1))
+    elif which in ("equisolid230", "stereographic170"):
+        # strong and weak compression move the m-form boundary out of the Lafida range (to 79 and to 39)
+        assert form_start(T, 23) not in LAFIDA_M_START and form_start(T, 23) >= form_start(T, 17)
+    elif which == "wide1920x1080_195":
+        # corner pixels near 90 degrees incidence: the table stops at its cap (keypoints beyond it take the exact path)
+        assert n == 8192
+    elif which == "narrow1280x720_120":
+        assert form_start(T, 23) == 39                      # the m-form from the first tier-1 radius on
 
 
 def test_table_argument_validation(api, cams):

@@ -17,6 +17,7 @@ from ref_tape import crc32, same
 
 GOLD = pathlib.Path(__file__).resolve().parent / "golden"
 FIXTURES = sorted(glob.glob(str(GOLD / "ref_extract_*.npz")))
+SYNTHETIC_CAMS = json.loads((GOLD / "synthetic_cams.json").read_text())      # tests/golden/make_synthetic_cams.py
 
 
 def crc(a):
@@ -136,13 +137,14 @@ def test_octree_equals_reference_with_ties(oa, seed):
 
 def test_camera_model_equals_reference(oa, cams, api):
     """WorldToImg / ImgToWorld / undistortPointsOcam / CreateMirrorMask / isPointInMirrorMask of the reference
-    (src/cam_model_omni.cpp) vs the oracle and vs the product's host helpers (same double arithmetic, bit for bit)."""
+    (src/cam_model_omni.cpp) vs the oracle and vs the product's host helpers (same double arithmetic, bit for bit), on the Lafida
+    cameras and on the synthetic calibrations the descriptor tests use."""
     ra = _ra()
     import ctypes as C
     from multicol_slam_b200 import synth
     from multicol_slam_b200.ctypes_defs import make_ocam
     rng = np.random.default_rng(3)
-    for cam in list(cams) + [synth.scaled_cam(cams[1], 1920, 1080)]:
+    for cam in list(cams) + [synth.scaled_cam(cams[1], 1920, 1080)] + SYNTHETIC_CAMS:
         oc = make_ocam(cam)
         assert same(ra.mirror_mask(cam), synth.mirror_mask(cam))
         assert same(ra.mirror_mask(cam), api.mirror_mask(cam))
