@@ -85,6 +85,19 @@ class Grid:
                     out.append(k)
         return out
 
+    def features_in_area_kf(self, cam, x, y, r):
+        """the cMultiKeyFrame overload (src/cMultiKeyFrame.cpp:694-737): same cell range, no level filter, `<= r` in place of
+        `!(> r)`"""
+        x, y, r = float(x), float(y), float(r)
+        c0 = max(0, int(math.floor((x - 0 - r) * self.winv[cam])))
+        c1 = min(GRID_COLS - 1, int(math.ceil((x - 0 + r) * self.winv[cam])))
+        r0 = max(0, int(math.floor((y - 0 - r) * self.hinv[cam])))
+        r1 = min(GRID_ROWS - 1, int(math.ceil((y - 0 + r) * self.hinv[cam])))
+        if c0 >= GRID_COLS or c1 < 0 or r0 >= GRID_ROWS or r1 < 0:
+            return []
+        return [k for ix in range(c0, c1 + 1) for iy in range(r0, r1 + 1) for k in self.cells[cam][ix][iy]
+                if abs(float(self.keys["x"][k]) - x) <= r and abs(float(self.keys["y"][k]) - y) <= r]
+
 
 def radius_by_viewing_cos(view_cos):
     return 2.5 if view_cos > 0.998 else 4.0
