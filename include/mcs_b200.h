@@ -436,6 +436,39 @@ int  mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, in
 /* The number of fixpoint rounds mcs_search_by_projection_device runs before the sequential walk finishes the rest. */
 int  mcs_search_by_projection_max_rounds(void);
 
+/* A frame in packed feature buffers: camera c is global image first_image + c of packed_dev, which holds n_parts consecutive
+ * mcs_packed_layout(part_images, capacity, dim) layouts (see mcs_search_by_projection_device). */
+typedef struct mcs_packed_frame {
+    const void* packed_dev;
+    int32_t n_parts, part_images, first_image;
+} mcs_packed_frame;
+
+/* cORBmatcher::SearchByProjection(CurrentFrame, LastFrame, th) (ref :1990-2118, TrackWithMotionModel) with both frames in packed
+ * feature buffers and every output on the device.  Asynchronous like mcs_search_by_projection_device (same stream, scratch and
+ * staging rules; nothing is read back).
+ *   cur / last: the two frames, each in either packed layout; they may share one buffer.  cams [n_cams] host camera models (one
+ *   image size for all); masks_dev [n_cams][height][width] their level-0 mirror masks; scale_factors [n_levels] host
+ *   (CurrentFrame.mvScaleFactors); mtmc_inv [n_cams * 16] host, the CURRENT rig pose's MtMc_inv (row-major 4x4 per camera).
+ *   last_mp_dev [n_cams * capacity]: the last frame's map-point ids by slot (-1 = none), in the frame_mp format of
+ *   mcs_search_by_projection_device, so that call's output can be passed on unchanged.  last_outlier_dev (slot-indexed, may be
+ *   NULL: no outliers).  world_pos_dev [n_points * 3] and bad_dev [n_points] (may be NULL) are the map points.
+ *   For every last-frame keypoint in contiguous order (camera-major): skipped when it has no map point, the point is bad or the
+ *   keypoint is an outlier; else the point is projected with WorldToCamHom_fast into the keypoint's own camera and, inside the
+ *   mirror mask, searched in GetFeaturesInArea(cam, u, v, th * scale_factors[octave], octave - 1, octave + 1) of the current
+ *   frame.  The best candidate not yet assigned (strict < over the visiting order, distance from the last frame's descriptor and
+ *   mask) is accepted when its distance is <= th_high; cur_mp_dev receives the map-point id.  No ratio test, no rotation check.
+ *   cur_mp_dev [n_cams * capacity] in/out, slot-indexed like frame_mp_dev; slots at or beyond a camera's count are neither read
+ *   nor written, in either frame.  nmatches_dev: the acceptances of this call.  status_dev: MCS_ERR_INVALID when a map-point id
+ *   is >= n_points or an octave of a query lies outside [0, n_levels) -- that query is dropped, the others are unaffected --
+ *   MCS_OK otherwise.  diag_dev (may be NULL): int32[4] as for mcs_search_by_projection_device.
+ * capacity <= 65535, n_cams * capacity < 2^24 (MCS_ERR_UNSUPPORTED beyond); cameras of different sizes: MCS_ERR_UNSUPPORTED. */
+int  mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity,
+                                          int32_t dim, const mcs_ocam* cams, const uint8_t* masks_dev, int32_t n_levels,
+                                          const double* scale_factors, const double* mtmc_inv, const int32_t* last_mp_dev,
+                                          const uint8_t* last_outlier_dev, int32_t n_points, const double* world_pos_dev,
+                                          const uint8_t* bad_dev, double th, int32_t th_high, int32_t having_masks, int32_t* cur_mp_dev,
+                                          int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev, void* stream);
+
 /* Generic projection-window search: the shape shared by the remaining cORBmatcher searches (SURVEY 8a row M4).
  * Queries are visited in order; for each one the candidates of GetFeaturesInArea(cam, x, y, r, min_level, max_level)
  * that are not yet taken (assigned[idx] >= 0) are scanned in the reference's order, best / second best are tracked

@@ -15,8 +15,8 @@ import pathlib
 
 import numpy as np
 
-from .ctypes_defs import (ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam,
-                          WINDOW_QUERY_DTYPE, make_ocam, make_params)
+from .ctypes_defs import (ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam, PackedFrame,
+                          WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
 
 _PKG = pathlib.Path(__file__).resolve().parent
 _LIB_PATH = _PKG / "libmcs_b200.so"
@@ -40,6 +40,7 @@ def lib():
         _lib = C.CDLL(str(_LIB_PATH))
         _lib.mcs_last_error.restype = C.c_char_p
         _lib.mcs_slot_bytes.restype = C.c_size_t
+        set_prototypes(_lib)
     return _lib
 
 
@@ -736,6 +737,31 @@ class cORBmatcher:
                                                      int(self.havingMasks), _dptr(frame_mp_t), _dptr(out[0]), _dptr(out[1]),
                                                      _dptr(out[2]) if diag else None, _stream_handle(stream, dev)))
         return (out[0], out[1], frame_mp_t) + ((out[2],) if diag else ())
+
+    def SearchByProjectionLastDevice(self, cur, last, capacity, rig_cur, masks_t, scale_factors, last_mp_t, world_t, th, cur_mp_t,
+                                     bad_t=None, last_outlier_t=None, stream=None, out=None, diag=False):
+        """mcs_search_by_projection_last_device: SearchByProjection(CurrentFrame, LastFrame, th) (ref :1990-2118, motion model) with
+        both frames in packed feature buffers.  cur / last: (packed uint8 cuda tensor, n_parts, part_images, first_image); camera c =
+        image first_image + c.  rig_cur: a Rig at the current pose (its MtMc_inv and camera models); masks_t [n_cams,H,W] u8 cuda,
+        their mirror masks; scale_factors: CurrentFrame's.  last_mp_t / cur_mp_t: int32 cuda [n_cams * capacity] map-point ids by
+        slot (-1 none), cur_mp_t updated in place; world_t [n_points,3] f64 cuda; bad_t [n_points] / last_outlier_t [n_cams *
+        capacity] u8 cuda or None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4] when
+        diag is set, as cuda tensors."""
+        import torch
+        fc, fl = (PackedFrame(f[0].data_ptr(), *f[1:4]) for f in (cur, last))
+        dev = cur[0].device
+        nc = len(rig_cur.cams)
+        ocs = (Ocam * nc)(*[as_ocam(c) for c in rig_cur.cams])
+        sf = np.ascontiguousarray(scale_factors, np.float64)
+        mi = np.ascontiguousarray(rig_cur.MtMc_inv, np.float64)
+        if out is None:
+            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
+        _check(lib().mcs_search_by_projection_last_device(C.byref(fc), C.byref(fl), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t), len(sf),
+                                                          _p(sf), _p(mi), _dptr(last_mp_t), _dptr(last_outlier_t), world_t.shape[0],
+                                                          _dptr(world_t), _dptr(bad_t), th, self.TH_HIGH_, int(self.havingMasks),
+                                                          _dptr(cur_mp_t), _dptr(out[0]), _dptr(out[1]), _dptr(out[2]) if diag else None,
+                                                          _stream_handle(stream, dev)))
+        return (out[0], out[1], cur_mp_t) + ((out[2],) if diag else ())
 
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
         """ref :579-726.  vbPrevMatched [n1,2] float64 updated in place.  Returns (nmatches, vnMatches12)."""

@@ -30,6 +30,22 @@ MCS_HD void cam_world_to_img(const mcs_ocam& cam, double x, double y, double z, 
     v = uu * cam.e + vv + cam.v0;
 }
 
+#ifdef __CUDACC__
+// WorldToCamHom_fast (ref src/cam_system_omni.cpp:92-133) then isPointInMirrorMask(u, v, 0) (ref src/cam_model_omni.cpp:163-178).
+// M: the camera's MtMc_inv (row-major 4x4), mask: its level-0 mirror mask.  ptRot = M * (P, 1) is the cv::Matx product,
+// s = 0 + a0 b0 + a1 b1 + a2 b2 + a3 b3 in this order, no FMA.  Returns whether (u, v) lies in the mask.
+__device__ __forceinline__ bool cam_project_in_mask(const double* M, const mcs_ocam& cam, const uint8_t* mask, double P0, double P1,
+                                                    double P2, double& u, double& v) {
+    double r[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) r[k] = ((M[4 * k] * P0 + M[4 * k + 1] * P1) + M[4 * k + 2] * P2) + M[4 * k + 3] * 1.0;
+    cam_world_to_img(cam, r[0], r[1], r[2], u, v);
+    const int ur = __double2int_rn(u), vr = __double2int_rn(v);
+    if (ur >= cam.width || ur <= 0 || vr >= cam.height || vr <= 0) return false;
+    return mask[(size_t)vr * cam.width + ur] != 0;
+}
+#endif
+
 MCS_HD void cam_img_to_world(const mcs_ocam& cam, double u, double v, double& x, double& y, double& z) {
     const double inv_affine = cam.c - cam.d * cam.e;
     const double u_t = u - cam.u0;

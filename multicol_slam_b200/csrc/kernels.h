@@ -113,17 +113,31 @@ cudaError_t stage_to_device(const void* host, size_t bytes, void* dev, cudaStrea
 struct PsCamSlots {                     // camera c of the frame: its image slot inside the packed feature buffer
     const int* count; const mcs_keypoint* kps; const uint8_t* desc; const uint8_t* dmask;
 };
-struct ProjSearchArgs {
-    int n_cams, capacity, dim, n_levels, n_points;
+struct PsFrameArgs {                    // both searches: the frame searched, the acceptance threshold, the outputs
+    int n_cams, capacity, dim, n_levels;
     const PsCamSlots* cams;                                  // host [n_cams] (device pointers inside)
     const int* cam_w; const int* cam_h; const double* sf;    // host
+    int th_high; bool masked;
+    int* frame_mp; int* nmatches; int* status; int* diag;    // device
+};
+struct ProjSearchArgs : PsFrameArgs {   // SearchByProjection(F, vpMapPoints, th)
+    int n_points;
     const uint8_t* bad; const uint8_t* in_view; const int* level;              // device map-point arrays
     const double* px; const double* py; const double* vcos;
     const uint8_t* mp_desc; const uint8_t* mp_dmask;
-    double th, nnratio; int th_high; bool masked;
-    int* frame_mp; int* nmatches; int* status; int* diag;    // device
+    double th, nnratio;
 };
 cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st);
+struct ProjSearchLastArgs : PsFrameArgs {   // SearchByProjection(CurrentFrame, LastFrame, th): the frame searched is CurrentFrame
+    const PsCamSlots* last;                                  // host [n_cams]: LastFrame's image slots
+    const mcs_ocam* models; const double* mtmc_inv;          // host [n_cams], [n_cams * 16] (the current pose)
+    const uint8_t* masks;                                    // device [n_cams][h][w] level-0 mirror masks
+    int n_points;
+    const int* last_mp; const uint8_t* last_outlier;         // device [n_cams * capacity], slot-indexed (outlier may be NULL)
+    const double* world_pos; const uint8_t* bad;             // device [n_points * 3], [n_points] (bad may be NULL)
+    double th;
+};
+cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaStream_t st);
 int proj_search_max_rounds();
 
 // ---- bag of words (bow_kernels.cu) ----

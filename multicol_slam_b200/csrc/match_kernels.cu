@@ -1148,18 +1148,9 @@ __global__ void frustum_kernel(const int n_cams, const double* __restrict__ mtmc
     if (skip && skip[i]) return;                  // already matched / bad (ref src/cTracking.cpp:985-988): keeps its last entries
     in_view[t] = 0; level[t] = 0; px[t] = 0.0; py[t] = 0.0; vcos[t] = 0.0;
     const double P0 = pos[3 * i], P1 = pos[3 * i + 1], P2 = pos[3 * i + 2];
-    // ptRot = MtMc_inv[c] * (P,1): cv::Matx product, s = 0 + a0 b0 + a1 b1 + a2 b2 + a3 b3 in this order, no FMA
-    const double* M = mtmc_inv + 16 * c;
-    double r[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) r[k] = ((M[4 * k] * P0 + M[4 * k + 1] * P1) + M[4 * k + 2] * P2) + M[4 * k + 3] * 1.0;
     const mcs_ocam cam = cams[c];
     double u, v;
-    cam_world_to_img(cam, r[0], r[1], r[2], u, v);
-    // isPointInMirrorMask(u, v, 0)  (ref src/cam_model_omni.cpp:163-178)
-    const int ur = __double2int_rn(u), vr = __double2int_rn(v);
-    if (ur >= cam.width || ur <= 0 || vr >= cam.height || vr <= 0) return;
-    if (masks[(size_t)c * cam.width * cam.height + (size_t)vr * cam.width + ur] == 0) return;
+    if (!cam_project_in_mask(mtmc_inv + 16 * c, cam, masks + (size_t)c * cam.width * cam.height, P0, P1, P2, u, v)) return;
     // distance to the camera centre, scale-invariance region
     const double* T = mtmc + 16 * c;
     const double o0 = P0 - T[3], o1 = P1 - T[7], o2 = P2 - T[11];

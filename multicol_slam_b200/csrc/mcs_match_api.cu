@@ -658,6 +658,31 @@ int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const d
 
 int mcs_search_by_projection_max_rounds(void) { return proj_search_max_rounds(); }
 
+}  // extern "C"
+
+namespace {
+// camera c of a packed frame = global image first_image + c = image (g mod part_images) of part g / part_images
+std::vector<PsCamSlots> packed_slots(const mcs_packed_frame& fr, int n_cams, int capacity, int dim) {
+    size_t off[4];
+    const size_t part_bytes = mcs_packed_layout(fr.part_images, capacity, dim, off);
+    std::vector<PsCamSlots> slots(n_cams);
+    for (int c = 0; c < n_cams; ++c) {
+        const int g = fr.first_image + c, p = g / fr.part_images, i = g - p * fr.part_images;
+        const uint8_t* b = (const uint8_t*)fr.packed_dev + (size_t)p * part_bytes;
+        slots[c] = PsCamSlots{(const int*)(b + off[0]) + i, (const mcs_keypoint*)(b + off[1]) + (size_t)i * capacity,
+                              b + off[2] + (size_t)i * capacity * dim, b + off[3] + (size_t)i * capacity * dim};
+    }
+    return slots;
+}
+
+bool packed_frame_ok(const mcs_packed_frame* fr, int n_cams) {
+    return fr->packed_dev && fr->n_parts >= 1 && fr->part_images >= 1 && fr->first_image >= 0 &&
+           (long long)fr->first_image + n_cams <= (long long)fr->n_parts * fr->part_images;
+}
+}  // namespace
+
+extern "C" {
+
 int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int32_t part_images, int32_t first_image, int32_t n_cams,
                                     int32_t capacity, int32_t dim, const int32_t* cam_width, const int32_t* cam_height, int32_t n_levels,
                                     const double* scale_factors, const mcs_mappoint_dev_view* mps, double th, double nnratio, int32_t th_high,
@@ -680,16 +705,7 @@ int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int
         return mfail(MCS_ERR_UNSUPPORTED, "more than 2^24 - 1 (map point, camera) entries in one call");
     cudaStream_t st = (cudaStream_t)stream;
     MCK(keep_pool_memory());
-    // camera c = global image first_image + c = image (g mod part_images) of part g / part_images
-    size_t off[4];
-    const size_t part_bytes = mcs_packed_layout(part_images, capacity, dim, off);
-    std::vector<PsCamSlots> slots(n_cams);
-    for (int c = 0; c < n_cams; ++c) {
-        const int g = first_image + c, p = g / part_images, i = g - p * part_images;
-        const uint8_t* b = (const uint8_t*)packed_dev + (size_t)p * part_bytes;
-        slots[c] = PsCamSlots{(const int*)(b + off[0]) + i, (const mcs_keypoint*)(b + off[1]) + (size_t)i * capacity,
-                              b + off[2] + (size_t)i * capacity * dim, b + off[3] + (size_t)i * capacity * dim};
-    }
+    const std::vector<PsCamSlots> slots = packed_slots(mcs_packed_frame{packed_dev, n_parts, part_images, first_image}, n_cams, capacity, dim);
     ProjSearchArgs a{};
     a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.n_levels = n_levels; a.n_points = mps->n_points;
     a.cams = slots.data(); a.cam_w = cam_width; a.cam_h = cam_height; a.sf = scale_factors;
@@ -698,6 +714,44 @@ int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int
     a.th = th; a.nnratio = nnratio; a.th_high = th_high; a.masked = having_masks != 0;
     a.frame_mp = frame_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
     MCK(launch_search_by_projection(a, st));
+    if (!stream) MCK(cudaStreamSynchronize(st));
+    return MCS_OK;
+}
+
+int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity,
+                                         int32_t dim, const mcs_ocam* cams, const uint8_t* masks_dev, int32_t n_levels,
+                                         const double* scale_factors, const double* mtmc_inv, const int32_t* last_mp_dev,
+                                         const uint8_t* last_outlier_dev, int32_t n_points, const double* world_pos_dev, const uint8_t* bad_dev,
+                                         double th, int32_t th_high, int32_t having_masks, int32_t* cur_mp_dev, int32_t* nmatches_dev,
+                                         int32_t* status_dev, int32_t* diag_dev, void* stream) {
+    if (!cur || !last || !cams || !masks_dev || !scale_factors || !mtmc_inv || !last_mp_dev || !world_pos_dev || !cur_mp_dev ||
+        !nmatches_dev || !status_dev)
+        return mfail(MCS_ERR_INVALID, "null argument");
+    if (n_cams < 1 || n_levels < 1 || n_levels > MCS_MAX_LEVELS || n_points < 0) return mfail(MCS_ERR_INVALID, "bad sizes");
+    if (capacity < 1 || capacity > 65535) return mfail(MCS_ERR_INVALID, "capacity must be 1..65535");
+    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    if (!packed_frame_ok(cur, n_cams)) return mfail(MCS_ERR_INVALID, "current frame: no buffer, or first_image + n_cams exceeds its images");
+    if (!packed_frame_ok(last, n_cams)) return mfail(MCS_ERR_INVALID, "last frame: no buffer, or first_image + n_cams exceeds its images");
+    for (int c = 0; c < n_cams; ++c) {
+        if (cams[c].width < 1 || cams[c].height < 1) return mfail(MCS_ERR_INVALID, "camera sizes must be positive");
+        if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
+            return mfail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
+    }
+    if ((long long)n_cams * capacity >= (1LL << 24)) return mfail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    cudaStream_t st = (cudaStream_t)stream;
+    MCK(keep_pool_memory());
+    const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
+    std::vector<int> cw(n_cams), ch(n_cams);
+    for (int c = 0; c < n_cams; ++c) { cw[c] = cams[c].width; ch[c] = cams[c].height; }
+    ProjSearchLastArgs a{};
+    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.n_levels = n_levels;
+    a.cams = cs.data(); a.cam_w = cw.data(); a.cam_h = ch.data(); a.sf = scale_factors;
+    a.th_high = th_high; a.masked = having_masks != 0;
+    a.frame_mp = cur_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
+    a.last = ls.data(); a.models = cams; a.mtmc_inv = mtmc_inv; a.masks = masks_dev;
+    a.n_points = n_points; a.last_mp = last_mp_dev; a.last_outlier = last_outlier_dev; a.world_pos = world_pos_dev; a.bad = bad_dev;
+    a.th = th;
+    MCK(launch_search_by_projection_last(a, st));
     if (!stream) MCK(cudaStreamSynchronize(st));
     return MCS_OK;
 }

@@ -1,14 +1,17 @@
-// proj_search_kernels.cu -- SearchByProjection(F, vpMapPoints, th) (ref src/cORBmatcher.cpp:67-166) with every input and output
-// resident on the device: the frame comes straight from the packed feature buffer (mcs_packed_layout), the map points from
-// the arrays mcs_project_mappoints_device fills, and the reference's ordered greedy acceptance runs on the device.
+// proj_search_kernels.cu -- SearchByProjection(F, vpMapPoints, th) (ref src/cORBmatcher.cpp:67-166) and the motion-model
+// SearchByProjection(CurrentFrame, LastFrame, th) (ref :1990-2118) with every input and output resident on the device: the frames
+// come straight from packed feature buffers (mcs_packed_layout), the map points from device arrays, and the reference's ordered
+// greedy acceptance runs on the device.
 //
-//   ps_gather_kernel    the frame's keypoints / descriptors / masks in slot order (slot = cam * capacity + j); empty slots get a
+//   ps_gather_kernel    a frame's keypoints / descriptors / masks in slot order (slot = cam * capacity + j); empty slots get a
 //                       position outside every image, so the unchanged frame_prepare_kernel leaves them out of the grid
-//   ps_count / ps_fill  the query array in the reference's order (map point outer, camera inner), a count / scan / fill over
-//                       in_view and bad
+//   pl_project_kernel   motion model only: per last-frame slot, its map point projected with the current pose into its camera
+//   ps_count / ps_fill  the query array in the reference's order, a count / scan / fill over a query maker: map point outer,
+//                       camera inner over in_view and bad (MapPointQueries), or last-frame slot order (LastFrameQueries)
 //   ps_list_kernel      per query the K smallest (distance, visiting position) keys of its window and the true candidate count
 //   ps_round_kernel     one round of the fixpoint iteration of the ordered acceptance (DESIGN.md section 4)
 //   ps_walk_kernel      the sequential fallback past the round cap: one warp per camera walks the unsettled queries in order
+//   pl_round / pl_walk  the same two kernels under the motion model's acceptance rule (MCS_RULE_BEST)
 //
 // No kernel reads anything back to the host: every size that depends on the data (the number of queries, the rounds the
 // fixpoint needed, where the walk starts) lives in device memory and the kernels are launched for the upper bound.
@@ -17,6 +20,7 @@
 #include <cstring>
 #include <vector>
 
+#include "cam_model.cuh"
 #include "kernels.h"
 
 namespace mcs {
@@ -61,7 +65,7 @@ __global__ void ps_gather_kernel(const PsCamSlots* __restrict__ cams, const int 
     const int c = s / capacity, j = s - c * capacity;
     const PsCamSlots cs = cams[c];
     const int n = min(*cs.count, capacity);
-    key_cam[s] = c;
+    if (key_cam) key_cam[s] = c;          // NULL: a frame that is only read by slot, never through a grid
     const int v4 = dim / 16;
     if (j < n) {
         keys[s] = cs.kps[j];
@@ -78,29 +82,88 @@ __global__ void ps_gather_kernel(const PsCamSlots* __restrict__ cams, const int 
     }
 }
 
-// ---- query build: entry k = point * n_cams + cam is a query when the point is not bad and in view ----
-struct QbArgs {
-    int n_cams, n_points, n_levels;
-    const uint8_t* bad; const uint8_t* in_view; const int* level;
+// ---- motion model: which last-frame slots make a query (ref :1997-2029) ----
+// Slot s = c * capacity + j (j < camera c's count) queries when its map point exists, is not bad and s is not an outlier, and the
+// point, projected with the current pose into camera c (the keypoint's own camera), falls in c's mirror mask.  A map-point id
+// >= n_points or an octave outside [0, n_levels) drops the query and raises status.
+struct LastProjArgs {
+    const PsCamSlots* cams; int n_cams, capacity, n_levels, n_points;
+    const mcs_keypoint* keys;                                  // the last frame in slot order (ps_gather_kernel)
+    const int* last_mp; const uint8_t* outlier; const uint8_t* bad; const double* pos;
+    const mcs_ocam* models; const double* mtmc_inv; const uint8_t* masks;
 };
-__device__ __forceinline__ bool qb_valid(const QbArgs& a, long long k, int* status) {
-    if (k >= (long long)a.n_points * a.n_cams) return false;
-    const int i = (int)(k / a.n_cams);
-    if (a.bad && a.bad[i]) return false;
-    if (!a.in_view[k]) return false;
-    const int lvl = a.level[k];
-    if (lvl < 0 || lvl >= a.n_levels) {       // the host call refuses such input; here the query is dropped and flagged
-        if (status) *status = MCS_ERR_INVALID;
-        return false;
-    }
-    return true;
+__global__ void __launch_bounds__(256) pl_project_kernel(const LastProjArgs a, uint8_t* __restrict__ ok, double* __restrict__ u,
+                                                         double* __restrict__ v, int* __restrict__ status) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= a.n_cams * a.capacity) return;
+    const int c = s / a.capacity, j = s - c * a.capacity;
+    ok[s] = 0;
+    if (j >= min(*a.cams[c].count, a.capacity)) return;
+    const int i = a.last_mp[s];
+    if (i < 0) return;
+    if (i >= a.n_points) { *status = MCS_ERR_INVALID; return; }
+    if ((a.bad && a.bad[i]) || (a.outlier && a.outlier[s])) return;
+    const mcs_ocam cam = a.models[c];
+    double x, y;
+    if (!cam_project_in_mask(a.mtmc_inv + 16 * c, cam, a.masks + (size_t)c * cam.width * cam.height, a.pos[3 * i], a.pos[3 * i + 1],
+                             a.pos[3 * i + 2], x, y))
+        return;
+    const int oct = a.keys[s].octave;
+    if (oct < 0 || oct >= a.n_levels) { *status = MCS_ERR_INVALID; return; }
+    ok[s] = 1; u[s] = x; v[s] = y;
 }
 
-__global__ void __launch_bounds__(kQbThreads) ps_count_kernel(const QbArgs a, int* __restrict__ block_count, int* __restrict__ status) {
+// ---- query build: a count / scan / fill over the entries of a query maker, in the maker's order ----
+// A maker has size() entries; valid(k) says whether entry k is a query (and may raise status), make(k) builds it.  sf is the
+// staged scale-factor table, set by ps_search.
+struct MapPointQueries {         // SearchByProjection(F, vpMapPoints): entry k = point * n_cams + cam, when not bad and in view
+    int n_cams, n_points, n_levels;
+    const uint8_t* bad; const uint8_t* in_view; const int* level;
+    const double* px; const double* py; const double* vcos; const double* sf; double th;
+    __host__ __device__ long long size() const { return (long long)n_points * n_cams; }
+    __device__ bool valid(long long k, int* status) const {
+        if (k >= size()) return false;
+        const int i = (int)(k / n_cams);
+        if (bad && bad[i]) return false;
+        if (!in_view[k]) return false;
+        const int lvl = level[k];
+        if (lvl < 0 || lvl >= n_levels) {     // the host call refuses such input; here the query is dropped and flagged
+            if (status) *status = MCS_ERR_INVALID;
+            return false;
+        }
+        return true;
+    }
+    __device__ mcs_window_query make(long long k) const {
+        const int lvl = level[k];
+        double r = vcos[k] > 0.998 ? 2.5 : 4.0;      // RadiusByViewingCos (ref :169-175)
+        if (th != 1.0) r *= th;
+        mcs_window_query q;
+        q.cam = (int)(k % n_cams); q.min_level = lvl - 1; q.max_level = lvl; q.desc_index = (int)(k / n_cams);
+        q.x = px[k]; q.y = py[k]; q.r = r * sf[lvl];
+        return q;
+    }
+};
+
+struct LastFrameQueries {        // SearchByProjection(CurrentFrame, LastFrame, th): entry k = last-frame slot, as pl_project_kernel set it
+    int n_slots, capacity;
+    const uint8_t* ok; const double* u; const double* v; const mcs_keypoint* keys; const double* sf; double th;
+    __host__ __device__ long long size() const { return n_slots; }
+    __device__ bool valid(long long k, int*) const { return k < n_slots && ok[k]; }
+    __device__ mcs_window_query make(long long k) const {
+        const int oct = keys[k].octave;
+        mcs_window_query q;                          // GetFeaturesInArea(cam, u, v, th * sf[oct], oct - 1, oct + 1)  (ref :2027-2033)
+        q.cam = (int)(k / capacity); q.min_level = oct - 1; q.max_level = oct + 1; q.desc_index = (int)k;
+        q.x = u[k]; q.y = v[k]; q.r = th * sf[oct];
+        return q;
+    }
+};
+
+template <class QM>
+__global__ void __launch_bounds__(kQbThreads) ps_count_kernel(const QM a, int* __restrict__ block_count, int* __restrict__ status) {
     int total = 0;
     for (int i = 0; i < kQbPer; ++i) {
         const long long k = (long long)blockIdx.x * kQbTile + i * kQbThreads + threadIdx.x;
-        total += __syncthreads_count(qb_valid(a, k, status));
+        total += __syncthreads_count(a.valid(k, status));
     }
     if (threadIdx.x == 0) block_count[blockIdx.x] = total;
 }
@@ -128,29 +191,20 @@ __global__ void __launch_bounds__(1024) ps_scan_kernel(const int* __restrict__ b
     if (threadIdx.x == 0) *nq = carry;
 }
 
-__global__ void __launch_bounds__(kQbThreads) ps_fill_kernel(const QbArgs a, const int* __restrict__ block_off, const double* __restrict__ proj_x,
-                                                             const double* __restrict__ proj_y, const double* __restrict__ view_cos,
-                                                             const double* __restrict__ sf, const double th, mcs_window_query* __restrict__ qry) {
+template <class QM>
+__global__ void __launch_bounds__(kQbThreads) ps_fill_kernel(const QM a, const int* __restrict__ block_off, mcs_window_query* __restrict__ qry) {
     __shared__ int s_w[kQbThreads / 32];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     int run = block_off[blockIdx.x];
     for (int i = 0; i < kQbPer; ++i) {
         const long long k = (long long)blockIdx.x * kQbTile + i * kQbThreads + threadIdx.x;
-        const bool v = qb_valid(a, k, nullptr);
+        const bool v = a.valid(k, nullptr);
         const unsigned m = __ballot_sync(0xffffffffu, v);
         if (lane == 0) s_w[w] = __popc(m);
         __syncthreads();
         int off = run, tot = 0;
         for (int u = 0; u < kQbThreads / 32; ++u) { if (u < w) off += s_w[u]; tot += s_w[u]; }
-        if (v) {
-            const int lvl = a.level[k];
-            double r = view_cos[k] > 0.998 ? 2.5 : 4.0;      // RadiusByViewingCos (ref :169-175)
-            if (th != 1.0) r *= th;
-            mcs_window_query q;
-            q.cam = (int)(k % a.n_cams); q.min_level = lvl - 1; q.max_level = lvl; q.desc_index = (int)(k / a.n_cams);
-            q.x = proj_x[k]; q.y = proj_y[k]; q.r = r * sf[lvl];
-            qry[off + __popc(m & ((1u << lane) - 1u))] = q;
-        }
+        if (v) qry[off + __popc(m & ((1u << lane) - 1u))] = a.make(k);
         run += tot;
         __syncthreads();
     }
@@ -250,19 +304,23 @@ __global__ void __launch_bounds__(256) ps_list_kernel(const WindowFrameDev f, co
     }
 }
 
-// The decision of one query (warp-uniform) under a "keypoint already taken" predicate: best / second best free candidate by
-// (distance, visiting position) -- what the sequential strict-< update of ref :138-150 picks -- and the acceptance of :154-160.
-// The list decides when it holds two free entries or every candidate; otherwise the window is scanned again with the predicate.
-template <int WORDS, bool MASKED, class Taken>
+// The decision of one query (warp-uniform) under a "keypoint already taken" predicate.  MCS_RULE_LEVEL_RATIO: best / second best
+// free candidate by (distance, visiting position) -- what the sequential strict-< update of ref :138-150 picks -- and the
+// acceptance of :154-160.  MCS_RULE_BEST: the best free candidate alone (strict < over the visiting order, ref :2050-2068),
+// accepted when its distance is <= th_high (:2070).  The list decides when it holds as many free entries as the rule reads, or
+// every candidate; otherwise the window is scanned again with the predicate.
+template <int RULE, int WORDS, bool MASKED, class Taken>
 __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_window_query& qq, const unsigned* lk, const int* ls, const int cnt,
                                          const uint32_t* qdesc, const uint32_t* qmask, const Taken& taken, const int th_high,
                                          const double nnratio, int* rescans) {
+    static_assert(RULE == MCS_RULE_LEVEL_RATIO || RULE == MCS_RULE_BEST, "device acceptance rules");
+    constexpr int NB = RULE == MCS_RULE_BEST ? 1 : 2;       // free keys the rule reads
     const int lane = threadIdx.x & 31;
     unsigned k = kNoKey; int s = -1; bool fr = false;
     if (lane < kPsK) { k = lk[lane]; s = ls[lane]; fr = k != kNoKey && !taken(s); }
     const unsigned fm = __ballot_sync(0xffffffffu, fr);
     unsigned k0 = kNoKey, k1 = kNoKey; int s0 = -1, s1 = -1;
-    if (__popc(fm) >= 2 || cnt <= kPsK) {
+    if (__popc(fm) >= NB || cnt <= kPsK) {
         const int b0 = fm ? __ffs(fm) - 1 : 0;
         const unsigned rest = fm & (fm - 1);
         const int b1 = rest ? __ffs(rest) - 1 : 0;
@@ -271,12 +329,14 @@ __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_wind
         if (fm) { k0 = x0; s0 = y0; }
         if (rest) { k1 = x1; s1 = y1; }
     } else {
-        unsigned kk[2]; int ss[2];
-        window_kbest<WORDS, MASKED, 2>(f, qq, qdesc, qmask, taken, kk, ss);
-        k0 = kk[0]; s0 = ss[0]; k1 = kk[1]; s1 = ss[1];
+        unsigned kk[NB]; int ss[NB];
+        window_kbest<WORDS, MASKED, NB>(f, qq, qdesc, qmask, taken, kk, ss);
+        k0 = kk[0]; s0 = ss[0];
+        if constexpr (NB == 2) { k1 = kk[1]; s1 = ss[1]; }
         if (lane == 0 && rescans) atomicAdd(rescans, 1);
     }
     if (s0 < 0) return -1;
+    if constexpr (RULE == MCS_RULE_BEST) return (int)(k0 >> 16) <= th_high ? s0 : -1;
     const int d0 = (int)(k0 >> 16), l0 = f.koct[s0];
     const int d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX, l1 = s1 >= 0 ? f.koct[s1] : -1;
     const bool ok = d0 <= th_high && !(l0 == l1 && (double)d0 > nnratio * (double)d1);
@@ -291,15 +351,17 @@ struct PsState {                 // device scratch shared by the acceptance kern
     int* ctl;                    // [0] nq  [1] rounds run  [2] rescans  [3] walk start  [4 ..] first changed query of each round
     int Q, n_slots, capacity, th_high;
     double nnratio;
+    const int* tag;              // may be NULL: an accepted query writes tag[desc_index] into frame_mp, else desc_index itself
 };
+__device__ __forceinline__ int ps_tag(const PsState& p, const int desc_index) { return p.tag ? p.tag[desc_index] : desc_index; }
 __device__ __forceinline__ int* ps_chg(const PsState& p) { return p.ctl + 4; }
 
 // Round r: every query not yet settled decides, treating a keypoint as taken when frame_mp had it on entry or a query with a
 // smaller index accepted it in round r - 1.  Queries below the first one whose decision changed in round r - 1 are final
 // (query p reads only decisions of queries < p) and only republish their keypoint.
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(256, 2) ps_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
-                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
+template <int RULE, int WORDS, bool MASKED>
+__device__ __forceinline__ void ps_round(const WindowFrameDev& f, const PsState& p, const int r, const uint32_t* __restrict__ qdesc,
+                                         const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
     const int* chg = ps_chg(p);
     const int settled = r >= 2 ? chg[r - 1] : 0;
     if (settled == kNoChange) return;                         // converged in an earlier round
@@ -322,14 +384,25 @@ __global__ void __launch_bounds__(256, 2) ps_round_kernel(const WindowFrameDev f
             const unsigned v = own_prev[s];
             return (v & 0xFF000000u) == ver_prev && (int)(v & 0xFFFFFFu) < q;
         };
-        const int d = ps_decide<WORDS, MASKED>(f, p.qry[q], p.lkey + (size_t)q * kPsK, p.lslot + (size_t)q * kPsK, p.lcnt[q], qdesc, qmask,
-                                               taken, p.th_high, p.nnratio, p.ctl + 2);
+        const int d = ps_decide<RULE, WORDS, MASKED>(f, p.qry[q], p.lkey + (size_t)q * kPsK, p.lslot + (size_t)q * kPsK, p.lcnt[q], qdesc,
+                                                     qmask, taken, p.th_high, p.nnratio, p.ctl + 2);
         if (lane == 0) {
             dec_cur[q] = d;
             if (d >= 0) atomicMin(&own_cur[d], ver_cur | (unsigned)q);
             if (r >= 1 && d != dec_prev[q]) atomicMin(&p.ctl[4 + r], q);
         }
     }
+}
+// one kernel name per rule: MCS_RULE_LEVEL_RATIO (local map) and MCS_RULE_BEST (motion model)
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(256, 2) ps_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
+                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
+    ps_round<MCS_RULE_LEVEL_RATIO, WORDS, MASKED>(f, p, r, qdesc, qmask, fmp_in);
+}
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(256, 2) pl_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
+                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
+    ps_round<MCS_RULE_BEST, WORDS, MASKED>(f, p, r, qdesc, qmask, fmp_in);
 }
 
 // Writes the final decisions of the settled prefix into frame_mp and counts them; records where the walk has to start.
@@ -344,7 +417,7 @@ __global__ void __launch_bounds__(256) ps_finalize_kernel(const PsState p, int* 
     int n = 0;
     for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < S; q += gridDim.x * blockDim.x) {
         const int d = dec[q];
-        if (d >= 0) { frame_mp[d] = p.qry[q].desc_index; ++n; }
+        if (d >= 0) { frame_mp[d] = ps_tag(p, p.qry[q].desc_index); ++n; }
     }
     if (n) atomicAdd(&s_n, n);
     __syncthreads();
@@ -356,9 +429,9 @@ __global__ void __launch_bounds__(256) ps_finalize_kernel(const PsState p, int* 
 
 // Fallback past the round cap: one warp per camera walks its queries from the first unsettled one in order, with the camera's
 // taken keypoints as a bitmap in shared memory.
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(32) ps_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
-                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
+template <int RULE, int WORDS, bool MASKED>
+__device__ __forceinline__ void ps_walk(const WindowFrameDev& f, const PsState& p, const uint32_t* __restrict__ qdesc,
+                                        const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
     extern __shared__ unsigned s_bits[];
     const int S = p.ctl[3];
     if (S < 0) return;
@@ -379,13 +452,13 @@ __global__ void __launch_bounds__(32) ps_walk_kernel(const WindowFrameDev f, con
             const int qi = base + __ffs(m) - 1;
             m &= m - 1;
             const mcs_window_query qq = p.qry[qi];
-            const int d = ps_decide<WORDS, MASKED>(f, qq, p.lkey + (size_t)qi * kPsK, p.lslot + (size_t)qi * kPsK, p.lcnt[qi], qdesc, qmask,
-                                                   taken, p.th_high, p.nnratio, p.ctl + 2);
+            const int d = ps_decide<RULE, WORDS, MASKED>(f, qq, p.lkey + (size_t)qi * kPsK, p.lslot + (size_t)qi * kPsK, p.lcnt[qi], qdesc,
+                                                         qmask, taken, p.th_high, p.nnratio, p.ctl + 2);
             if (d >= 0) {
                 if (lane == 0) {
                     const int j = d - c * cap;
                     s_bits[j >> 5] |= 1u << (j & 31);
-                    frame_mp[d] = qq.desc_index;
+                    frame_mp[d] = ps_tag(p, qq.desc_index);
                 }
                 ++nm;
             }
@@ -393,6 +466,16 @@ __global__ void __launch_bounds__(32) ps_walk_kernel(const WindowFrameDev f, con
         }
     }
     if (lane == 0 && nm) atomicAdd(nmatches, nm);
+}
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(32) ps_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
+                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
+    ps_walk<MCS_RULE_LEVEL_RATIO, WORDS, MASKED>(f, p, qdesc, qmask, frame_mp, nmatches);
+}
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(32) pl_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
+                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
+    ps_walk<MCS_RULE_BEST, WORDS, MASKED>(f, p, qdesc, qmask, frame_mp, nmatches);
 }
 
 __global__ void ps_diag_kernel(const int* __restrict__ ctl, int* __restrict__ diag) {
@@ -408,10 +491,17 @@ size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 int proj_search_max_rounds() { return kPsRounds; }
 
-cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st) {
+namespace {
+
+// Both searches from the query maker on: the frame view of `a` in slot order and its grid, the queries in the maker's order, the
+// lists, the rounds and the walk under RULE.  qdesc / qmask: the query descriptors, row desc_index; tag: see PsState.  The caller
+// has zeroed a.nmatches and a.status.
+template <int RULE, class QM>
+cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const uint8_t* qdesc, const uint8_t* qmask, const int* tag,
+                      cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     const int ncell = a.n_cams * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
-    const long long Q = (long long)a.n_points * a.n_cams;
+    const long long Q = qm.size();
     const int nb = (int)((Q + kQbTile - 1) / kQbTile);
     const size_t db = (size_t)NS * a.dim;
     // one stream-ordered scratch block, carved below
@@ -449,8 +539,6 @@ cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st
     if (e == cudaSuccess) e = stage_to_device(hc.data(), sizeof(mcs_ocam) * a.n_cams, cams, st);
     if (e == cudaSuccess) e = stage_to_device(a.sf, sizeof(double) * a.n_levels, sf, st);
     if (e == cudaSuccess) e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, slots, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a.nmatches, 0, 4, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl, 0, 16, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl + 4, 0x7F, 4 * kPsRounds, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(owner, 0xFF, 8ull * NS, st);
@@ -460,27 +548,31 @@ cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st
     ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
     e = launch_frame_prepare(keys, key_cam, NS, cams, a.n_cams, kx, ky, koct, nullptr, cell_of, cursor, cell_start, cell_items, winv, hinv, st);
     // queries in the reference's order
-    const QbArgs qa{a.n_cams, a.n_points, a.n_levels, a.bad, a.in_view, a.level};
+    qm.sf = sf;
     if (e == cudaSuccess && nb > 0) {
-        ps_count_kernel<<<nb, kQbThreads, 0, st>>>(qa, bcount, a.status);
+        ps_count_kernel<<<nb, kQbThreads, 0, st>>>(qm, bcount, a.status);
         ps_scan_kernel<<<1, 1024, 0, st>>>(bcount, nb, boff, ctl);
-        ps_fill_kernel<<<nb, kQbThreads, 0, st>>>(qa, boff, a.px, a.py, a.vcos, sf, a.th, qry);
+        ps_fill_kernel<<<nb, kQbThreads, 0, st>>>(qm, boff, qry);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess && Q > 0) {
         const WindowFrameDev f{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv};
-        const PsState p{qry, lkey, lslot, lcnt, dec, owner, ctl, (int)Q, NS, a.capacity, a.th_high, a.nnratio};
-        const uint32_t* qd = (const uint32_t*)a.mp_desc;
-        const uint32_t* qm = a.masked ? (const uint32_t*)a.mp_dmask : nullptr;
+        const PsState p{qry, lkey, lslot, lcnt, dec, owner, ctl, (int)Q, NS, a.capacity, a.th_high, nnratio, tag};
+        const uint32_t* qd = (const uint32_t*)qdesc;
+        const uint32_t* qk = a.masked ? (const uint32_t*)qmask : nullptr;
         const int wblocks = (int)std::min<long long>((Q + 7) / 8, (long long)sms * 16);
         const int fblocks = (int)std::min<long long>((Q + 255) / 256, (long long)sms * 4);
         const size_t walk_smem = 4ull * ((a.capacity + 31) / 32);
 #define MCS_PS(W, M)                                                                                                   \
         {                                                                                                              \
-            ps_list_kernel<W, M><<<wblocks, 256, 0, st>>>(f, qry, ctl, qd, qm, lkey, lslot, lcnt);                     \
-            for (int r = 0; r < kPsRounds; ++r) ps_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qm, a.frame_mp); \
+            ps_list_kernel<W, M><<<wblocks, 256, 0, st>>>(f, qry, ctl, qd, qk, lkey, lslot, lcnt);                     \
+            for (int r = 0; r < kPsRounds; ++r) {                                                                      \
+                if constexpr (RULE == MCS_RULE_BEST) pl_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp); \
+                else ps_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp);                      \
+            }                                                                                                          \
             ps_finalize_kernel<<<fblocks, 256, 0, st>>>(p, a.frame_mp, a.nmatches);                                    \
-            ps_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qm, a.frame_mp, a.nmatches);               \
+            if constexpr (RULE == MCS_RULE_BEST) pl_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches); \
+            else ps_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches);          \
         }
         if (a.dim == 16) { if (a.masked) MCS_PS(4, true) else MCS_PS(4, false) }
         else if (a.dim == 32) { if (a.masked) MCS_PS(8, true) else MCS_PS(8, false) }
@@ -490,6 +582,59 @@ cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st
     }
     if (e == cudaSuccess && a.diag) ps_diag_kernel<<<1, 1, 0, st>>>(ctl, a.diag);
     if (e == cudaSuccess) e = cudaGetLastError();
+    const cudaError_t ef = cudaFreeAsync(base, st);
+    return e != cudaSuccess ? e : ef;
+}
+
+cudaError_t ps_zero_outputs(const PsFrameArgs& a, cudaStream_t st) {
+    cudaError_t e = cudaMemsetAsync(a.nmatches, 0, 4, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
+    return e;
+}
+
+}  // namespace
+
+cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st) {
+    const cudaError_t e = ps_zero_outputs(a, st);
+    if (e != cudaSuccess) return e;
+    const MapPointQueries qm{a.n_cams, a.n_points, a.n_levels, a.bad, a.in_view, a.level, a.px, a.py, a.vcos, nullptr, a.th};
+    return ps_search<MCS_RULE_LEVEL_RATIO>(a, qm, a.nnratio, a.mp_desc, a.mp_dmask, nullptr, st);
+}
+
+// The last frame in slot order (gather without a grid) and its queries (pl_project_kernel), then the current frame searched under
+// MCS_RULE_BEST with the last frame's descriptors as the query rows and last_mp as the tags.
+cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    const size_t db = (size_t)NS * a.dim;
+    const size_t sizes[] = {sizeof(PsCamSlots) * a.n_cams, sizeof(mcs_ocam) * a.n_cams, 128ull * a.n_cams,    // staged host inputs
+                            sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0, (size_t)NS, 8ull * NS, 8ull * NS}; // keys desc dmask ok u v
+    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
+    size_t off[nsz], total = 0;
+    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
+    cudaError_t e = keep_pool_memory();
+    if (e != cudaSuccess) return e;
+    uint8_t* base = nullptr;
+    e = cudaMallocAsync((void**)&base, total, st);
+    if (e != cudaSuccess) return e;
+    auto at = [&](int i) { return (void*)(base + off[i]); };
+    PsCamSlots* slots = (PsCamSlots*)at(0); mcs_ocam* models = (mcs_ocam*)at(1); double* mi = (double*)at(2);
+    mcs_keypoint* keys = (mcs_keypoint*)at(3); uint8_t* desc = (uint8_t*)at(4); uint8_t* dmask = a.masked ? (uint8_t*)at(5) : nullptr;
+    uint8_t* ok = (uint8_t*)at(6); double* u = (double*)at(7); double* v = (double*)at(8);
+    e = stage_to_device(a.last, sizeof(PsCamSlots) * a.n_cams, slots, st);
+    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
+    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, mi, st);
+    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
+    if (e == cudaSuccess) {
+        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, nullptr, desc, dmask);
+        const LastProjArgs pa{slots, a.n_cams, a.capacity, a.n_levels, a.n_points, keys, a.last_mp, a.last_outlier, a.bad, a.world_pos,
+                              models, mi, a.masks};
+        pl_project_kernel<<<(NS + 255) / 256, 256, 0, st>>>(pa, ok, u, v, a.status);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        const LastFrameQueries qm{NS, a.capacity, ok, u, v, keys, nullptr, a.th};
+        e = ps_search<MCS_RULE_BEST>(a, qm, 0.0, desc, dmask, a.last_mp, st);
+    }
     const cudaError_t ef = cudaFreeAsync(base, st);
     return e != cudaSuccess ? e : ef;
 }

@@ -47,6 +47,19 @@ class MapPointDevView(C.Structure):
     _fields_ = MapPointView._fields_
 
 
+class PackedFrame(C.Structure):
+    """mcs_packed_frame: camera c = global image first_image + c of n_parts consecutive packed layouts of part_images images"""
+    _fields_ = [("packed_dev", C.c_void_p), ("n_parts", C.c_int32), ("part_images", C.c_int32), ("first_image", C.c_int32)]
+
+
+def set_prototypes(lib):
+    """argument types of the entry points whose many arguments are easiest to get wrong from Python"""
+    P, I, D = C.c_void_p, C.c_int32, C.c_double
+    f = lib.mcs_search_by_projection_last_device
+    f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, I, P, P, P, P, I, P, P, D, I, I, P, P, P, P, P]
+    f.restype = C.c_int
+
+
 import numpy as np
 
 # numpy dtype binary-compatible with mcs_keypoint / cv::KeyPoint (28 bytes)
