@@ -50,7 +50,8 @@ static const signed char kPairs[2048] = {
 #include "../multicol_slam_b200/csrc/brief_pairs_64.inc"
 };
 
-inline int cv_round(double v) { return (int)lrint(v); }        // cvRound: round-half-even
+// cvRound: round half to even; as OpenCV's x86-64 path (cvtsd2si), NaN and values outside int give INT_MIN rather than wrapping
+inline int cv_round(double v) { const double r = std::nearbyint(v); return (r >= -2147483648.0 && r < 2147483648.0) ? (int)r : INT_MIN; }
 inline int cv_floor(double v) { int i = (int)v; return i - (i > v); }
 inline int cv_ceil(double v) { int i = (int)v; return i + (i < v); }
 

@@ -21,8 +21,11 @@ INT_MAX = 2**31 - 1
 
 
 def cv_round(v):
-    """cvRound(double): round half to even (lrint)"""
-    return int(np.rint(np.float64(v)))
+    """cvRound(double): round half to even (lrint); NaN and results outside int give INT_MIN (cvtsd2si on x86-64)"""
+    v = np.float64(v)
+    if not np.isfinite(v) or not -2.0 ** 31 <= np.rint(v) < 2.0 ** 31:
+        return -2 ** 31
+    return int(np.rint(v))
 
 
 def popcount_bytes(a):

@@ -41,8 +41,9 @@
 #define CV_PI 3.1415926535897932384626433832795
 #define CV_Assert(expr) do { if (!(expr)) throw cv::Exception(#expr); } while (0)
 
-// OpenCV core/fast_math.hpp: cvRound = round-half-to-even (lrint), cvFloor / cvCeil by truncation + correction
-inline int cvRound(double v) { return (int)lrint(v); }
+// OpenCV core/fast_math.hpp: cvRound = round-half-to-even (lrint), cvFloor / cvCeil by truncation + correction.  cvRound(double)
+// on x86-64 is cvtsd2si: NaN and values outside int give INT_MIN (a plain (int)lrint would wrap 2^32 + 5 to 5)
+inline int cvRound(double v) { const double r = nearbyint(v); return (r >= -2147483648.0 && r < 2147483648.0) ? (int)r : (-2147483647 - 1); }
 inline int cvRound(float v) { return (int)lrintf(v); }
 inline int cvRound(int v) { return v; }
 inline int cvFloor(double v) { int i = (int)v; return i - (i > v); }

@@ -113,6 +113,11 @@ def world_to_img(cam, x, y, z):
     return u.value, v.value
 
 
+def world_to_img_many(cam, xyz):
+    """world_to_img of each row of xyz [n,3] -> [n,2]"""
+    return np.array([world_to_img(cam, float(p[0]), float(p[1]), float(p[2])) for p in np.asarray(xyz, np.float64)]).reshape(-1, 2)
+
+
 def img_to_world(cam, u, v):
     x, y, z = C.c_double(), C.c_double(), C.c_double()
     lib().mcsref_cam_img_to_world(C.byref(_oc(cam)), C.c_double(u), C.c_double(v), C.byref(x), C.byref(y), C.byref(z))
