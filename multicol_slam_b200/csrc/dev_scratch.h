@@ -60,6 +60,16 @@ struct Dev {   // RAII device scratch buffer
         if (p) { DevCache::local().give(p, cap, dev); p = nullptr; }
         return DevCache::local().take(bytes, &p, &cap, &dev);
     }
+    // alloc(bytes), then copy `bytes` of host memory from `src` into the buffer with cudaMemcpy ...
+    cudaError_t upload(const void* src, size_t bytes) {
+        const cudaError_t e = alloc(bytes);
+        return e != cudaSuccess ? e : cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice);
+    }
+    // ... or with cudaMemcpyAsync on `st`
+    cudaError_t upload_async(const void* src, size_t bytes, cudaStream_t st) {
+        const cudaError_t e = alloc(bytes);
+        return e != cudaSuccess ? e : cudaMemcpyAsync(p, src, bytes, cudaMemcpyHostToDevice, st);
+    }
     template <typename T> T* as() { return (T*)p; }
 };
 

@@ -15,26 +15,17 @@
 #include <string>
 #include <vector>
 
+#include "api_check.h"
 #include "cam_model.cuh"
 #include "kernels.h"
 #include "mcs_common.cuh"
 
 using namespace mcs;
 
+static thread_local std::string g_err;
+int mcs_fail(int code, const std::string& msg) { g_err = msg; return code; }
+
 namespace {
-
-thread_local std::string g_err;
-int fail(int code, const std::string& msg) { g_err = msg; return code; }
-
-#define CK(expr)                                                                                       \
-    do {                                                                                               \
-        cudaError_t e__ = (expr);                                                                      \
-        if (e__ != cudaSuccess) {                                                                      \
-            cudaGetLastError();                                                                        \
-            return fail(e__ == cudaErrorNoDevice || e__ == cudaErrorInsufficientDriver ? MCS_ERR_NO_DEVICE : MCS_ERR_CUDA, \
-                        std::string(#expr) + ": " + cudaGetErrorString(e__));                          \
-        }                                                                                              \
-    } while (0)
 
 static const signed char kPairs[2048] = {
 #include "brief_pairs_64.inc"
@@ -132,7 +123,7 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
     G.nlevels = L; G.width = W; G.height = H;
     G.fast_threshold = ex->p.fast_threshold; G.desc_size = ex->p.desc_size;
     G.do_dbrief = ex->p.do_dbrief; G.learn_masks = ex->p.learn_masks;
-    if (W >= 4096 || H >= 4096) return fail(MCS_ERR_UNSUPPORTED, "images larger than 4095 px are not supported");
+    if (W >= 4096 || H >= 4096) return mcs_fail(MCS_ERR_UNSUPPORTED, "images larger than 4095 px are not supported");
 
     std::vector<int16_t> blob;     // all LUTs, int16
     struct Off { size_t xofs, xa0, xa1, yofs, yb0, yb1, cellx, celly, mx0, my0; } off[kMaxLevels];
@@ -144,7 +135,7 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
         g.w = cv_round((double)W * ex->isf[l]);
         g.h = cv_round((double)H * ex->isf[l]);
         if (g.w < 2 * kEdge + 8 || g.h < 2 * kEdge + 8)
-            return fail(MCS_ERR_UNSUPPORTED, "pyramid level smaller than 58 px");
+            return mcs_fail(MCS_ERR_UNSUPPORTED, "pyramid level smaller than 58 px");
         g.pitch = (g.w + 63) & ~63;
         g.img_bytes = (size_t)g.pitch * g.h;
         g.sw = l ? G.lv[l - 1].w : W; g.sh = l ? G.lv[l - 1].h : H;
@@ -158,7 +149,7 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
         if (l) {
             const double scale_x = 1.0 / ((double)g.w / g.sw), scale_y = 1.0 / ((double)g.h / g.sh);
             // the staged source region of a 72x40 tile must fit 176 x 88 bytes: (72*s + 17) <= 176, (40*s + 2) <= 88
-            if (scale_x > 2.08 || scale_y > 2.08) return fail(MCS_ERR_UNSUPPORTED, "scale factors above 2 are not supported");
+            if (scale_x > 2.08 || scale_y > 2.08) return mcs_fail(MCS_ERR_UNSUPPORTED, "scale factors above 2 are not supported");
             for (int dx = 0; dx < g.w; ++dx) {
                 float fx = (float)((dx + 0.5) * scale_x - 0.5);
                 int sx = cv_floor(fx);
@@ -204,12 +195,12 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
         const int minB = kEdge - 3, maxBX = g.w - kEdge + 3, maxBY = g.h - kEdge + 3;
         const double width = maxBX - minB, height = maxBY - minB;
         g.n_cols = (int)(width / 30.0); g.n_rows = (int)(height / 30.0);
-        if (g.n_cols < 1 || g.n_rows < 1) return fail(MCS_ERR_UNSUPPORTED, "level too small for the 30 px cell grid");
+        if (g.n_cols < 1 || g.n_rows < 1) return mcs_fail(MCS_ERR_UNSUPPORTED, "level too small for the 30 px cell grid");
         g.w_cell = (int)std::ceil(width / g.n_cols); g.h_cell = (int)std::ceil(height / g.n_rows);
         // K1 sizes its per-warp corner segments for tile rows that cross at most 3 cell edges (kWarpCorners)
-        if (g.w_cell < 30) return fail(MCS_ERR_UNSUPPORTED, "FAST cells narrower than 30 px");
+        if (g.w_cell < 30) return mcs_fail(MCS_ERR_UNSUPPORTED, "FAST cells narrower than 30 px");
         if ((long long)g.n_cols * g.n_rows * g.w_cell * g.h_cell >= (1 << 24))
-            return fail(MCS_ERR_UNSUPPORTED, "cell-order key overflow");
+            return mcs_fail(MCS_ERR_UNSUPPORTED, "cell-order key overflow");
         for (int i = 0; i < g.n_rows; ++i) {
             const double iniY = minB + i * g.h_cell;
             double maxY = iniY + g.h_cell + 6;
@@ -227,7 +218,7 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
         // a cell narrower/lower than 7 px yields nothing in cv::FAST; the ranges above are then empty.
         // octree roots (ref :640-642)
         g.nodes_ini = cv_round((double)(maxBX - minB) / (maxBY - minB));
-        if (g.nodes_ini < 1) return fail(MCS_ERR_UNSUPPORTED, "portrait images narrower than half their height");
+        if (g.nodes_ini < 1) return mcs_fail(MCS_ERR_UNSUPPORTED, "portrait images narrower than half their height");
         g.hX = (double)(maxBX - minB) / g.nodes_ini;
         g.sel_cap = std::max(g.quota + 3, 4 * g.nodes_ini);
         g.sel_off = sel_off; sel_off += g.sel_cap;
@@ -253,9 +244,9 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
     ex->tile_flags_valid = false;
     // kernels of an earlier *_device call on a caller-supplied stream may still read the tables about to be rewritten (a change of the
     // image size is rare: drain the device)
-    CK(cudaDeviceSynchronize());
-    CK(ex->lut_blob.ensure(blob.size() * sizeof(int16_t)));
-    CK(cudaMemcpyAsync(ex->lut_blob.p, blob.data(), blob.size() * sizeof(int16_t), cudaMemcpyHostToDevice, ex->stream));
+    CUDA_CHECK(cudaDeviceSynchronize());
+    CUDA_CHECK(ex->lut_blob.ensure(blob.size() * sizeof(int16_t)));
+    CUDA_CHECK(cudaMemcpyAsync(ex->lut_blob.p, blob.data(), blob.size() * sizeof(int16_t), cudaMemcpyHostToDevice, ex->stream));
     const int16_t* base = (const int16_t*)ex->lut_blob.p;
     for (int l = 0; l < L; ++l) {
         LevelGeom& g = G.lv[l];
@@ -264,9 +255,9 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
         g.cellx = base + off[l].cellx; g.celly = base + off[l].celly;
         g.mx0 = base + off[l].mx0; g.my0 = base + off[l].my0;
     }
-    CK(ex->G_dev.ensure(1));
-    CK(cudaMemcpyAsync(ex->G_dev.p, &G, sizeof(G), cudaMemcpyHostToDevice, ex->stream));
-    CK(cudaStreamSynchronize(ex->stream));     // blob / G are host temporaries
+    CUDA_CHECK(ex->G_dev.ensure(1));
+    CUDA_CHECK(cudaMemcpyAsync(ex->G_dev.p, &G, sizeof(G), cudaMemcpyHostToDevice, ex->stream));
+    CUDA_CHECK(cudaStreamSynchronize(ex->stream));     // blob / G are host temporaries
     ex->geom_w = W; ex->geom_h = H; ex->geom_stride = in_stride;
     ex->B_cap = 0;      // level buffers depend on the geometry
     return MCS_OK;
@@ -276,16 +267,16 @@ int ensure_batch(mcs_extractor* ex, int B) {
     if (B <= ex->B_cap) return MCS_OK;
     const PyramidGeom& G = ex->G;
     for (int l = 0; l < G.nlevels; ++l) {
-        CK(ex->lvl[l].ensure(G.lv[l].img_bytes * B + 256));
-        CK(ex->blur[l].ensure(G.lv[l].img_bytes * B + 256));
+        CUDA_CHECK(ex->lvl[l].ensure(G.lv[l].img_bytes * B + 256));
+        CUDA_CHECK(ex->blur[l].ensure(G.lv[l].img_bytes * B + 256));
     }
-    CK(ex->cam_of_image.ensure(B));
-    CK(ex->raw.ensure(G.raw_total * B));
-    CK(ex->node_of.ensure(G.raw_total * B));
-    CK(ex->raw_count.ensure((size_t)B * G.nlevels));
-    CK(ex->sel_count.ensure((size_t)B * G.nlevels));
-    CK(ex->sel_xys.ensure((size_t)B * G.sel_total));
-    CK(ex->status.ensure(1));
+    CUDA_CHECK(ex->cam_of_image.ensure(B));
+    CUDA_CHECK(ex->raw.ensure(G.raw_total * B));
+    CUDA_CHECK(ex->node_of.ensure(G.raw_total * B));
+    CUDA_CHECK(ex->raw_count.ensure((size_t)B * G.nlevels));
+    CUDA_CHECK(ex->sel_count.ensure((size_t)B * G.nlevels));
+    CUDA_CHECK(ex->sel_xys.ensure((size_t)B * G.sel_total));
+    CUDA_CHECK(ex->status.ensure(1));
     ex->B_cap = B;
     return MCS_OK;
 }
@@ -294,14 +285,14 @@ int ensure_batch(mcs_extractor* ex, int B) {
 // H2D copy engine as the image chunks of the stream call, so they must be enqueued BEFORE any large copy: a 1 MB
 // mask upload queued behind 100 MB of images stalls the compute stream for the whole transfer.
 int upload_small_inputs(mcs_extractor* ex, int W, int H, const uint8_t* masks, const mcs_ocam* cams, int n_cams, cudaStream_t st) {
-    CK(ex->masks.ensure((size_t)n_cams * W * H));
-    CK(ex->cams.ensure(n_cams));
+    CUDA_CHECK(ex->masks.ensure((size_t)n_cams * W * H));
+    CUDA_CHECK(ex->cams.ensure(n_cams));
     // the masks rarely change between calls (static mirror masks): a 1 MB compare is cheaper than a pageable upload
     const size_t mbytes = (size_t)n_cams * W * H;
     if (ex->masks_host.size() != mbytes || std::memcmp(ex->masks_host.data(), masks, mbytes) != 0) {
-        CK(cudaStreamSynchronize(st));                     // a previous call may still read the old masks
+        CUDA_CHECK(cudaStreamSynchronize(st));                     // a previous call may still read the old masks
         ex->masks_host.assign(masks, masks + mbytes);
-        CK(cudaMemcpyAsync(ex->masks.p, ex->masks_host.data(), mbytes, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(ex->masks.p, ex->masks_host.data(), mbytes, cudaMemcpyHostToDevice, st));
         ex->tile_flags_valid = false;
     }
     if (!ex->tile_flags_valid) {
@@ -328,13 +319,13 @@ int upload_small_inputs(mcs_extractor* ex, int W, int H, const uint8_t* masks, c
             }
         }
         for (size_t i = 0; i < flags.size(); ++i) flags[i] = flags[i] ? (all_in[i] ? 2 : 1) : 0;
-        CK(cudaStreamSynchronize(st));                     // a previous call may still read the old flags
-        CK(ex->tile_flags.ensure(flags.size()));
-        CK(cudaMemcpyAsync(ex->tile_flags.p, flags.data(), flags.size(), cudaMemcpyHostToDevice, st));
-        CK(cudaStreamSynchronize(st));                     // `flags` is a host temporary
+        CUDA_CHECK(cudaStreamSynchronize(st));                     // a previous call may still read the old flags
+        CUDA_CHECK(ex->tile_flags.ensure(flags.size()));
+        CUDA_CHECK(cudaMemcpyAsync(ex->tile_flags.p, flags.data(), flags.size(), cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));                     // `flags` is a host temporary
         ex->tile_flags_valid = true;
     }
-    CK(cudaMemcpyAsync(ex->cams.p, cams, sizeof(mcs_ocam) * n_cams, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->cams.p, cams, sizeof(mcs_ocam) * n_cams, cudaMemcpyHostToDevice, st));
     if ((ex->p.do_dbrief || ex->p.learn_masks) &&
         ((int)ex->lut_cams.size() != n_cams || std::memcmp(ex->lut_cams.data(), cams, sizeof(mcs_ocam) * n_cams) != 0)) {
         std::vector<double> all;
@@ -346,17 +337,17 @@ int upload_small_inputs(mcs_extractor* ex, int W, int H, const uint8_t* masks, c
             offs[c] = all.size();
             all.insert(all.end(), coef.begin(), coef.end());
         }
-        CK(cudaStreamSynchronize(st));                 // a previous call may still read the old tables
-        CK(ex->lut_coef.ensure(all.size()));
-        CK(ex->luts.ensure(n_cams));
+        CUDA_CHECK(cudaStreamSynchronize(st));                 // a previous call may still read the old tables
+        CUDA_CHECK(ex->lut_coef.ensure(all.size()));
+        CUDA_CHECK(ex->luts.ensure(n_cams));
         std::vector<DistortLut> h(n_cams);
         for (int c = 0; c < n_cams; ++c) h[c] = DistortLut{ex->lut_coef.p + offs[c], ns[c], 1.0};
-        CK(cudaMemcpyAsync(ex->lut_coef.p, all.data(), all.size() * sizeof(double), cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(ex->luts.p, h.data(), sizeof(DistortLut) * n_cams, cudaMemcpyHostToDevice, st));
-        CK(cudaStreamSynchronize(st));                 // host staging vectors die here
+        CUDA_CHECK(cudaMemcpyAsync(ex->lut_coef.p, all.data(), all.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(ex->luts.p, h.data(), sizeof(DistortLut) * n_cams, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));                 // host staging vectors die here
         ex->lut_cams.assign(cams, cams + n_cams);
     }
-    CK(cudaMemsetAsync(ex->status.p, 0, sizeof(int), st));
+    CUDA_CHECK(cudaMemsetAsync(ex->status.p, 0, sizeof(int), st));
 
     return MCS_OK;
 }
@@ -369,28 +360,28 @@ int enqueue_kernels(mcs_extractor* ex, int n_images, const uint8_t* images_dev, 
                     mcs_keypoint* kps_dev, uint8_t* desc_dev, uint8_t* dmask_dev, int* counts_dev, int capacity, cudaStream_t st) {
     const PyramidGeom& G = ex->G;
     ex->coi_last = coi_d;
-    CK(cudaMemsetAsync(ex->raw_count.p, 0, sizeof(int) * n_images * G.nlevels, st));
-    if (ex->profiling) CK(cudaEventRecord(ex->ev[0], st));
+    CUDA_CHECK(cudaMemsetAsync(ex->raw_count.p, 0, sizeof(int) * n_images * G.nlevels, st));
+    if (ex->profiling) CUDA_CHECK(cudaEventRecord(ex->ev[0], st));
     for (int l = 0; l < G.nlevels; ++l) {
         const uint8_t* src = l ? ex->lvl[l - 1].p : images_dev;
         const size_t src_bytes = l ? G.lv[l - 1].img_bytes : (size_t)stride * H;
         launch_pyr_fast(G, l, n_images, src, src_bytes, ex->lvl[l].p, ex->blur[l].p, ex->masks.p, W, (size_t)W * H,
                         coi_d, ex->tile_flags.p, ex->raw.p, ex->raw_count.p, st);
     }
-    CK(cudaGetLastError());
-    if (ex->profiling) CK(cudaEventRecord(ex->ev[1], st));
+    CUDA_CHECK(cudaGetLastError());
+    if (ex->profiling) CUDA_CHECK(cudaEventRecord(ex->ev[1], st));
     // (K2 forked per level onto a second stream behind K1 of the same level was slower for the per-frame path: the per-level
     // launches serialise on that stream, while the single launch runs its 8 x n CTAs side by side)
-    CK(launch_octree(G, ex->G_dev.p, n_images, ex->raw.p, ex->raw_count.p, ex->node_of.p, ex->sel_xys.p, ex->sel_count.p,
-                     ex->status.p, st));
-    CK(cudaGetLastError());
-    if (ex->profiling) CK(cudaEventRecord(ex->ev[2], st));
+    CUDA_CHECK(launch_octree(G, ex->G_dev.p, n_images, ex->raw.p, ex->raw_count.p, ex->node_of.p, ex->sel_xys.p, ex->sel_count.p,
+                             ex->status.p, st));
+    CUDA_CHECK(cudaGetLastError());
+    if (ex->profiling) CUDA_CHECK(cudaEventRecord(ex->ev[2], st));
     DescribeArgs a;
     for (int l = 0; l < kMaxLevels; ++l) { a.lvl[l] = ex->lvl[l].p; a.blur[l] = ex->blur[l].p; }
     a.tier_stats = ex->tier_on ? ex->tier.p : nullptr;
-    CK(launch_describe(G, ex->G_dev.p, n_images, a, ex->cams.p, ex->luts.p, coi_d, ex->sel_xys.p, ex->sel_count.p,
-                       kps_dev, desc_dev, dmask_dev, counts_dev, capacity, st));
-    if (ex->profiling) CK(cudaEventRecord(ex->ev[3], st));
+    CUDA_CHECK(launch_describe(G, ex->G_dev.p, n_images, a, ex->cams.p, ex->luts.p, coi_d, ex->sel_xys.p, ex->sel_count.p,
+                               kps_dev, desc_dev, dmask_dev, counts_dev, capacity, st));
+    if (ex->profiling) CUDA_CHECK(cudaEventRecord(ex->ev[3], st));
     ex->last_n_images = n_images;
     return MCS_OK;
 }
@@ -399,9 +390,9 @@ int enqueue_kernels(mcs_extractor* ex, int n_images, const uint8_t* images_dev, 
 // pageable host memory); *coi_d receives the device camera-of-image table the kernels should use.
 int prepare_inputs(mcs_extractor* ex, int n_images, int W, int H, int stride, const uint8_t* masks, const mcs_ocam* cams, int n_cams,
                    const int* cam_of_image, cudaStream_t st, bool first_chunk, const int* coi_dev, const int** coi_d) {
-    if (n_cams < 1 || n_cams > 64) return fail(MCS_ERR_INVALID, "n_cams must be in [1,64]");
+    if (n_cams < 1 || n_cams > 64) return mcs_fail(MCS_ERR_INVALID, "n_cams must be in [1,64]");
     for (int i = 0; i < n_images; ++i)
-        if (cam_of_image[i] < 0 || cam_of_image[i] >= n_cams) return fail(MCS_ERR_INVALID, "cam_of_image out of range");
+        if (cam_of_image[i] < 0 || cam_of_image[i] >= n_cams) return mcs_fail(MCS_ERR_INVALID, "cam_of_image out of range");
     int rc = build_geometry(ex, W, H, stride);
     if (rc) return rc;
     rc = ensure_batch(ex, n_images);
@@ -412,7 +403,7 @@ int prepare_inputs(mcs_extractor* ex, int n_images, int W, int H, int stride, co
     }
     *coi_d = coi_dev;
     if (!coi_dev) {
-        CK(cudaMemcpyAsync(ex->cam_of_image.p, cam_of_image, sizeof(int) * n_images, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(cudaMemcpyAsync(ex->cam_of_image.p, cam_of_image, sizeof(int) * n_images, cudaMemcpyHostToDevice, st));
         *coi_d = ex->cam_of_image.p;
     }
     ex->sf_valid = false;            // shared state (camera table, masks, tables) may now differ from what the cached graph assumes
@@ -431,11 +422,11 @@ int run_pipeline(mcs_extractor* ex, int n_images, const uint8_t* images_dev, int
 
 int check_status(mcs_extractor* ex, cudaStream_t st) {
     int s = 0;
-    CK(cudaMemcpyAsync(&s, ex->status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (s & 1) return fail(MCS_ERR_CAPACITY, "raw corner list overflow");
-    if (s & 2) return fail(MCS_ERR_CAPACITY, "octree node table overflow");
-    if (s & 4) return fail(MCS_ERR_CAPACITY, "selected keypoint slots overflow");
+    CUDA_CHECK(cudaMemcpyAsync(&s, ex->status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    if (s & 1) return mcs_fail(MCS_ERR_CAPACITY, "raw corner list overflow");
+    if (s & 2) return mcs_fail(MCS_ERR_CAPACITY, "octree node table overflow");
+    if (s & 4) return mcs_fail(MCS_ERR_CAPACITY, "selected keypoint slots overflow");
     return MCS_OK;
 }
 
@@ -459,22 +450,20 @@ int upload_consts_once(int dev) {
     signed char du[848] = {0}, dv[848] = {0};
     int n = 0;
     for (int v = -kHalfPatch; v <= kHalfPatch; ++v) n += 2 * (v == 0 ? kHalfPatch : umax[std::abs(v)]) + 1;
-    if (n != 845) return fail(MCS_ERR_INVALID, "disc table size");
+    if (n != 845) return mcs_fail(MCS_ERR_INVALID, "disc table size");
     for (int v = 0; v <= kHalfPatch; ++v) {
         du[v] = (signed char)(v == 0 ? kHalfPatch : umax[v]);
         // symmetry check: column |u| = v must hold rows |v'| <= umax[v]
         for (int w = 0; w <= kHalfPatch; ++w)
             if ((w <= (v == 0 ? kHalfPatch : umax[v])) != (v <= (w == 0 ? kHalfPatch : umax[w])))
-                return fail(MCS_ERR_INVALID, "IC_Angle disc is not symmetric");
+                return mcs_fail(MCS_ERR_INVALID, "IC_Angle disc is not symmetric");
     }
-    CK(upload_constants(kPairs, du, dv));
+    CUDA_CHECK(upload_constants(kPairs, du, dv));
     if (dev < 64) g_consts_uploaded[dev] = true;
     return MCS_OK;
 }
 
 }  // namespace
-
-void mcs_set_error_(const std::string& msg) { g_err = msg; }
 
 // ================================================================================================
 extern "C" {
@@ -504,7 +493,7 @@ void mcs_cam_img_to_world(const mcs_ocam* cam, double u, double v, double* x, do
     cam_img_to_world(*cam, u, v, *x, *y, *z);
 }
 int mcs_cam_mirror_mask(const mcs_ocam* cam, uint8_t* out) {
-    if (!cam || !out) return fail(MCS_ERR_INVALID, "null argument");
+    if (!cam || !out) return mcs_fail(MCS_ERR_INVALID, "null argument");
     const int w = cam->width, h = cam->height;
     if (cam->mirror_mask != 1) { std::memset(out, 1, (size_t)w * h); return MCS_OK; }
     // ref src/cam_model_omni.cpp:187-188 swaps the names on purpose (SURVEY Appendix C.9)
@@ -518,21 +507,21 @@ int mcs_cam_mirror_mask(const mcs_ocam* cam, uint8_t* out) {
 }
 
 int mcs_extractor_create(const mcs_extractor_params* p, mcs_extractor** out) {
-    if (!p || !out) return fail(MCS_ERR_INVALID, "null argument");
+    if (!p || !out) return mcs_fail(MCS_ERR_INVALID, "null argument");
     *out = nullptr;
-    if (p->use_agast) return fail(MCS_ERR_UNSUPPORTED, "AGAST detector is not built (north star: FAST-9)");
-    if (p->fast_agast_type != 2) return fail(MCS_ERR_UNSUPPORTED, "only FastFeatureDetector::TYPE_9_16 (type 2) is built");
-    if (p->nlevels < 1 || p->nlevels > kMaxLevels) return fail(MCS_ERR_INVALID, "nlevels must be in [1,16]");
-    if (p->desc_size != 16 && p->desc_size != 32 && p->desc_size != 64) return fail(MCS_ERR_INVALID, "desc_size must be 16, 32 or 64");
+    if (p->use_agast) return mcs_fail(MCS_ERR_UNSUPPORTED, "AGAST detector is not built (north star: FAST-9)");
+    if (p->fast_agast_type != 2) return mcs_fail(MCS_ERR_UNSUPPORTED, "only FastFeatureDetector::TYPE_9_16 (type 2) is built");
+    if (p->nlevels < 1 || p->nlevels > kMaxLevels) return mcs_fail(MCS_ERR_INVALID, "nlevels must be in [1,16]");
+    if (p->desc_size != 16 && p->desc_size != 32 && p->desc_size != 64) return mcs_fail(MCS_ERR_INVALID, "desc_size must be 16, 32 or 64");
     if (p->nfeatures < 1 || !(p->scale_factor > 1.0f) || p->fast_threshold < 1 || p->fast_threshold > 254)
-        return fail(MCS_ERR_INVALID, "bad nfeatures / scale_factor / fast_threshold");
+        return mcs_fail(MCS_ERR_INVALID, "bad nfeatures / scale_factor / fast_threshold");
     int dev = 0;
     {
         cudaError_t e = cudaGetDevice(&dev);
-        if (e != cudaSuccess) { cudaGetLastError(); return fail(MCS_ERR_NO_DEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e)); }
+        if (e != cudaSuccess) { cudaGetLastError(); return mcs_fail(MCS_ERR_NO_DEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e)); }
         int major = 0;
         cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-        if (major != 9) return fail(MCS_ERR_NO_DEVICE, "device is not sm_90 (H100); this library has no other code path");
+        if (major != 9) return mcs_fail(MCS_ERR_NO_DEVICE, "device is not sm_90 (H100); this library has no other code path");
     }
     int rc = upload_consts_once(dev);
     if (rc) return rc;
@@ -556,12 +545,12 @@ int mcs_extractor_create(const mcs_extractor_params* p, mcs_extractor** out) {
     ex->quota[p->nlevels - 1] = std::max(p->nfeatures - sum, 0);
     ex->capacity = 0;
     for (int l = 0; l < p->nlevels; ++l) {
-        if (ex->quota[l] + 8 > kMaxNodes) { delete ex; return fail(MCS_ERR_UNSUPPORTED, "nfeatures too large for the octree node table"); }
+        if (ex->quota[l] + 8 > kMaxNodes) { delete ex; return mcs_fail(MCS_ERR_UNSUPPORTED, "nfeatures too large for the octree node table"); }
         ex->capacity += std::max(ex->quota[l] + 2, 16);
     }
     if (cudaStreamCreateWithFlags(&ex->stream, cudaStreamNonBlocking) != cudaSuccess) {
         delete ex;
-        return fail(MCS_ERR_CUDA, "cudaStreamCreate failed");
+        return mcs_fail(MCS_ERR_CUDA, "cudaStreamCreate failed");
     }
     *out = ex;
     return MCS_OK;
@@ -589,7 +578,7 @@ void mcs_extractor_destroy(mcs_extractor* ex) {
 }
 
 int mcs_extractor_get_info(const mcs_extractor* ex, mcs_extractor_info* info) {
-    if (!ex || !info) return fail(MCS_ERR_INVALID, "null argument");
+    if (!ex || !info) return mcs_fail(MCS_ERR_INVALID, "null argument");
     std::memset(info, 0, sizeof(*info));
     info->nlevels = ex->p.nlevels; info->capacity = ex->capacity; info->desc_size = ex->p.desc_size;
     for (int l = 0; l < ex->p.nlevels; ++l) {
@@ -605,11 +594,11 @@ int mcs_extract_batch_device(mcs_extractor* ex, int32_t n_images, const uint8_t*
                              const int32_t* cam_of_image, mcs_keypoint* kps_dev, uint8_t* desc_dev, uint8_t* dmask_dev,
                              int32_t* counts_dev, int32_t capacity, void* stream) {
     if (!ex || !images_dev || !masks || !cams || !cam_of_image || !kps_dev || !desc_dev || !counts_dev)
-        return fail(MCS_ERR_INVALID, "null argument");
-    if (n_images < 1 || width < 1 || height < 1 || stride < width) return fail(MCS_ERR_INVALID, "bad image geometry");
-    if (capacity < ex->capacity) return fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
-    if (ex->p.learn_masks && !dmask_dev) return fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
-    CK(cudaSetDevice(ex->device));
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_images < 1 || width < 1 || height < 1 || stride < width) return mcs_fail(MCS_ERR_INVALID, "bad image geometry");
+    if (capacity < ex->capacity) return mcs_fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
+    if (ex->p.learn_masks && !dmask_dev) return mcs_fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
+    CUDA_CHECK(cudaSetDevice(ex->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : ex->stream;
     int rc = run_pipeline(ex, n_images, images_dev, width, height, stride, masks, cams, n_cams, cam_of_image, kps_dev, desc_dev,
                           dmask_dev, counts_dev, capacity, st);
@@ -624,7 +613,7 @@ int pin_ensure(uint8_t*& p, size_t& cap, size_t need, bool* moved) {
     if (need <= cap) return MCS_OK;
     if (p) cudaFreeHost(p);
     p = nullptr; cap = 0;
-    CK(cudaMallocHost((void**)&p, need));
+    CUDA_CHECK(cudaMallocHost((void**)&p, need));
     cap = need; *moved = true;
     return MCS_OK;
 }
@@ -645,16 +634,16 @@ SmallOut small_out_layout(int n, int capacity, int ds) {
 int enqueue_small(mcs_extractor* ex, int n, int W, int H, int stride, int dpitch, const int* coi_d, int capacity, bool with_dmask, cudaStream_t st) {
     const int ds = ex->p.desc_size;
     const SmallOut o = small_out_layout(n, capacity, ds);
-    CK(cudaMemcpyAsync(ex->in_tight.p, ex->pin_in, (size_t)stride * H * n, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->in_tight.p, ex->pin_in, (size_t)stride * H * n, cudaMemcpyHostToDevice, st));
     launch_repitch(ex->in_tight.p, stride, ex->in_images.p, dpitch, W, (size_t)H * n, st);
-    CK(cudaMemsetAsync(ex->status.p, 0, sizeof(int), st));
+    CUDA_CHECK(cudaMemsetAsync(ex->status.p, 0, sizeof(int), st));
     int rc = enqueue_kernels(ex, n, ex->in_images.p, W, H, dpitch, coi_d, ex->kps.p, ex->desc.p, ex->dmask.p, ex->counts.p, capacity, st);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ex->pin_out + o.status, ex->status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ex->pin_out + o.counts, ex->counts.p, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ex->pin_out + o.kps, ex->kps.p, sizeof(mcs_keypoint) * n * capacity, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(ex->pin_out + o.desc, ex->desc.p, (size_t)n * capacity * ds, cudaMemcpyDeviceToHost, st));
-    if (with_dmask) CK(cudaMemcpyAsync(ex->pin_out + o.dmask, ex->dmask.p, (size_t)n * capacity * ds, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.status, ex->status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.counts, ex->counts.p, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.kps, ex->kps.p, sizeof(mcs_keypoint) * n * capacity, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.desc, ex->desc.p, (size_t)n * capacity * ds, cudaMemcpyDeviceToHost, st));
+    if (with_dmask) CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.dmask, ex->dmask.p, (size_t)n * capacity * ds, cudaMemcpyDeviceToHost, st));
     return MCS_OK;
 }
 
@@ -664,30 +653,30 @@ int mcs_extract_batch(mcs_extractor* ex, int32_t n_images, const uint8_t* images
                       const uint8_t* masks, const mcs_ocam* cams, int32_t n_cams, const int32_t* cam_of_image,
                       mcs_keypoint* kps_out, uint8_t* desc_out, uint8_t* dmask_out, int32_t* counts_out, int32_t capacity) {
     if (!ex || !images || !masks || !cams || !cam_of_image || !kps_out || !desc_out || !counts_out)
-        return fail(MCS_ERR_INVALID, "null argument");
-    if (n_images < 1 || width < 1 || height < 1 || stride < width) return fail(MCS_ERR_INVALID, "bad image geometry");
-    if (capacity < ex->capacity) return fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
-    if (ex->p.learn_masks && !dmask_out) return fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
-    CK(cudaSetDevice(ex->device));
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_images < 1 || width < 1 || height < 1 || stride < width) return mcs_fail(MCS_ERR_INVALID, "bad image geometry");
+    if (capacity < ex->capacity) return mcs_fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
+    if (ex->p.learn_masks && !dmask_out) return mcs_fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
+    CUDA_CHECK(cudaSetDevice(ex->device));
     cudaStream_t st = ex->stream;
     const int ds = ex->p.desc_size;
     // device staging with a 64-byte-aligned pitch so that K1 can use 128-bit loads
     const int dpitch = (width + 63) & ~63;
     const size_t img_bytes = (size_t)dpitch * height;
     const void* before[6] = {ex->in_images.p, ex->kps.p, ex->desc.p, ex->dmask.p, ex->counts.p, ex->in_tight.p};
-    CK(ex->in_images.ensure(img_bytes * n_images + 256));
-    CK(ex->kps.ensure((size_t)n_images * capacity));
-    CK(ex->desc.ensure((size_t)n_images * capacity * ds));
-    CK(ex->dmask.ensure((size_t)n_images * capacity * ds));
-    CK(ex->counts.ensure(n_images));
+    CUDA_CHECK(ex->in_images.ensure(img_bytes * n_images + 256));
+    CUDA_CHECK(ex->kps.ensure((size_t)n_images * capacity));
+    CUDA_CHECK(ex->desc.ensure((size_t)n_images * capacity * ds));
+    CUDA_CHECK(ex->dmask.ensure((size_t)n_images * capacity * ds));
+    CUDA_CHECK(ex->counts.ensure(n_images));
     // linear H2D + device re-pitch (a 2-D DMA of short rows is several times slower)
-    CK(ex->in_tight.ensure((size_t)stride * height * n_images + 256));
+    CUDA_CHECK(ex->in_tight.ensure((size_t)stride * height * n_images + 256));
     const void* after[6] = {ex->in_images.p, ex->kps.p, ex->desc.p, ex->dmask.p, ex->counts.p, ex->in_tight.p};
     bool moved = std::memcmp(before, after, sizeof(before)) != 0;
 
     if (n_images <= kGraphMaxImages && !ex->profiling && !ex->tier_on) {
         // ---- per-frame call: pinned staging + the whole sequence as one graph launch once the inputs repeat ----
-        if (n_cams < 1 || n_cams > 64) return fail(MCS_ERR_INVALID, "n_cams must be in [1,64]");
+        if (n_cams < 1 || n_cams > 64) return mcs_fail(MCS_ERR_INVALID, "n_cams must be in [1,64]");
         const size_t in_bytes = (size_t)stride * height * n_images, mbytes = (size_t)n_cams * width * height;
         const SmallOut o = small_out_layout(n_images, capacity, ds);
         int rc = pin_ensure(ex->pin_in, ex->pin_in_bytes, in_bytes, &moved);
@@ -705,9 +694,9 @@ int mcs_extract_batch(mcs_extractor* ex, int32_t n_images, const uint8_t* images
         if (hit) {
             // the graph goes first and the 1 MB mask comparison runs while the GPU works; if the masks did change the result
             // is thrown away and the call starts over on the eager path (which uploads the new masks)
-            CK(cudaGraphLaunch(ex->sf_exec, st));
+            CUDA_CHECK(cudaGraphLaunch(ex->sf_exec, st));
             if (std::memcmp(ex->masks_host.data(), masks, mbytes) != 0) {
-                CK(cudaStreamSynchronize(st));
+                CUDA_CHECK(cudaStreamSynchronize(st));
                 hit = false;
             } else {
                 ++ex->sf_replays;
@@ -741,11 +730,11 @@ int mcs_extract_batch(mcs_extractor* ex, int32_t n_images, const uint8_t* images
                 cudaGetLastError();
             }
         }
-        CK(cudaStreamSynchronize(st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
         const int status = *(const int*)(ex->pin_out + o.status);
-        if (status & 1) return fail(MCS_ERR_CAPACITY, "raw corner list overflow");
-        if (status & 2) return fail(MCS_ERR_CAPACITY, "octree node table overflow");
-        if (status & 4) return fail(MCS_ERR_CAPACITY, "selected keypoint slots overflow");
+        if (status & 1) return mcs_fail(MCS_ERR_CAPACITY, "raw corner list overflow");
+        if (status & 2) return mcs_fail(MCS_ERR_CAPACITY, "octree node table overflow");
+        if (status & 4) return mcs_fail(MCS_ERR_CAPACITY, "selected keypoint slots overflow");
         const int* cnt = (const int*)(ex->pin_out + o.counts);
         for (int i = 0; i < n_images; ++i) {
             const size_t nused = (size_t)std::min(std::max(cnt[i], 0), capacity), row = (size_t)i * capacity;
@@ -757,24 +746,24 @@ int mcs_extract_batch(mcs_extractor* ex, int32_t n_images, const uint8_t* images
         return MCS_OK;
     }
 
-    CK(cudaMemcpyAsync(ex->in_tight.p, images, (size_t)stride * height * n_images - (size_t)(stride - width), cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->in_tight.p, images, (size_t)stride * height * n_images - (size_t)(stride - width), cudaMemcpyHostToDevice, st));
     launch_repitch(ex->in_tight.p, stride, ex->in_images.p, dpitch, width, (size_t)height * n_images, st);
     int rc = run_pipeline(ex, n_images, ex->in_images.p, width, height, dpitch, masks, cams, n_cams, cam_of_image, ex->kps.p,
                           ex->desc.p, ex->dmask.p, ex->counts.p, capacity, st);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(counts_out, ex->counts.p, sizeof(int) * n_images, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(kps_out, ex->kps.p, sizeof(mcs_keypoint) * n_images * capacity, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(desc_out, ex->desc.p, (size_t)n_images * capacity * ds, cudaMemcpyDeviceToHost, st));
-    if (dmask_out) CK(cudaMemcpyAsync(dmask_out, ex->dmask.p, (size_t)n_images * capacity * ds, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(counts_out, ex->counts.p, sizeof(int) * n_images, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(kps_out, ex->kps.p, sizeof(mcs_keypoint) * n_images * capacity, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(desc_out, ex->desc.p, (size_t)n_images * capacity * ds, cudaMemcpyDeviceToHost, st));
+    if (dmask_out) CUDA_CHECK(cudaMemcpyAsync(dmask_out, ex->dmask.p, (size_t)n_images * capacity * ds, cudaMemcpyDeviceToHost, st));
     return check_status(ex, st);
 }
 
 int mcs_extract(mcs_extractor* ex, const uint8_t* image, int32_t width, int32_t height, int32_t stride, const uint8_t* mask,
                 int32_t mask_stride, const mcs_ocam* cam, mcs_keypoint* kps_out, uint8_t* desc_out, uint8_t* dmask_out,
                 int32_t capacity, int32_t* n_out) {
-    if (!ex || !n_out) return fail(MCS_ERR_INVALID, "null argument");
+    if (!ex || !n_out) return mcs_fail(MCS_ERR_INVALID, "null argument");
     if (!image) return MCS_OK;   // empty image: silent return, outputs untouched (ref :1252-1253)
-    if (!mask || !cam) return fail(MCS_ERR_INVALID, "a mask and a camera model are mandatory (ref :913-917 throws on an empty mask)");
+    if (!mask || !cam) return mcs_fail(MCS_ERR_INVALID, "a mask and a camera model are mandatory (ref :913-917 throws on an empty mask)");
     std::vector<uint8_t> packed;
     const uint8_t* m = mask;
     if (mask_stride != width) {
@@ -793,41 +782,41 @@ int mcs_extract(mcs_extractor* ex, const uint8_t* image, int32_t width, int32_t 
 
 int mcs_extractor_debug_read(mcs_extractor* ex, int32_t image_index, int32_t level, int32_t what, void* out, size_t out_bytes,
                              int32_t* w_out, int32_t* h_out) {
-    if (!ex || !out || !w_out || !h_out) return fail(MCS_ERR_INVALID, "null argument");
+    if (!ex || !out || !w_out || !h_out) return mcs_fail(MCS_ERR_INVALID, "null argument");
     if (level < 0 || level >= ex->G.nlevels || image_index < 0 || image_index >= ex->last_n_images)
-        return fail(MCS_ERR_INVALID, "bad level / image index");
-    CK(cudaSetDevice(ex->device));
+        return mcs_fail(MCS_ERR_INVALID, "bad level / image index");
+    CUDA_CHECK(cudaSetDevice(ex->device));
     const LevelGeom& g = ex->G.lv[level];
     const int L = ex->G.nlevels;
     if (what == 0 || what == 1) {
         *w_out = g.w; *h_out = g.h;
-        if (out_bytes < (size_t)g.w * g.h) return fail(MCS_ERR_CAPACITY, "buffer too small");
+        if (out_bytes < (size_t)g.w * g.h) return mcs_fail(MCS_ERR_CAPACITY, "buffer too small");
         const uint8_t* src = (what == 0 ? ex->lvl[level].p : ex->blur[level].p) + (size_t)image_index * g.img_bytes;
-        CK(cudaMemcpy2D(out, g.w, src, g.pitch, g.w, g.h, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy2D(out, g.w, src, g.pitch, g.w, g.h, cudaMemcpyDeviceToHost));
         return MCS_OK;
     }
     if (what == 2) {   // the mask pyramid is never materialised: evaluate the composed nearest-neighbour maps
         *w_out = g.w; *h_out = g.h;
-        if (out_bytes < (size_t)g.w * g.h) return fail(MCS_ERR_CAPACITY, "buffer too small");
+        if (out_bytes < (size_t)g.w * g.h) return mcs_fail(MCS_ERR_CAPACITY, "buffer too small");
         std::vector<int16_t> mx(g.w), my(g.h);
         std::vector<int> coi(ex->last_n_images);
-        CK(cudaMemcpy(mx.data(), g.mx0, g.w * 2, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(my.data(), g.my0, g.h * 2, cudaMemcpyDeviceToHost));
-        CK(cudaMemcpy(coi.data(), ex->coi_last, sizeof(int) * ex->last_n_images, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(mx.data(), g.mx0, g.w * 2, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(my.data(), g.my0, g.h * 2, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(coi.data(), ex->coi_last, sizeof(int) * ex->last_n_images, cudaMemcpyDeviceToHost));
         std::vector<uint8_t> m0((size_t)ex->G.width * ex->G.height);
-        CK(cudaMemcpy(m0.data(), ex->masks.p + (size_t)coi[image_index] * m0.size(), m0.size(), cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(m0.data(), ex->masks.p + (size_t)coi[image_index] * m0.size(), m0.size(), cudaMemcpyDeviceToHost));
         for (int y = 0; y < g.h; ++y)
             for (int x = 0; x < g.w; ++x) ((uint8_t*)out)[(size_t)y * g.w + x] = m0[(size_t)my[y] * ex->G.width + mx[x]];
         return MCS_OK;
     }
     if (what == 3) {   // raw corners, sorted into the reference order (cell-row-major, then pixel-row-major)
         int n = 0;
-        CK(cudaMemcpy(&n, ex->raw_count.p + (size_t)image_index * L + level, sizeof(int), cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(&n, ex->raw_count.p + (size_t)image_index * L + level, sizeof(int), cudaMemcpyDeviceToHost));
         n = std::min(n, g.raw_cap);
         *w_out = n; *h_out = 3;
-        if (out_bytes < (size_t)n * 12) return fail(MCS_ERR_CAPACITY, "buffer too small");
+        if (out_bytes < (size_t)n * 12) return mcs_fail(MCS_ERR_CAPACITY, "buffer too small");
         std::vector<uint32_t> c(n);
-        CK(cudaMemcpy(c.data(), ex->raw.p + (size_t)image_index * ex->G.raw_total + g.raw_off, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(c.data(), ex->raw.p + (size_t)image_index * ex->G.raw_total + g.raw_off, sizeof(uint32_t) * n, cudaMemcpyDeviceToHost));
         auto key = [&](uint32_t v) {
             const int x = corner_x(v) - kEdge, y = corner_y(v) - kEdge;
             const int cj = x / g.w_cell, ci = y / g.h_cell;
@@ -838,43 +827,43 @@ int mcs_extractor_debug_read(mcs_extractor* ex, int32_t image_index, int32_t lev
         for (int i = 0; i < n; ++i) { o[3 * i] = corner_x(c[i]); o[3 * i + 1] = corner_y(c[i]); o[3 * i + 2] = corner_s(c[i]); }
         return MCS_OK;
     }
-    return fail(MCS_ERR_INVALID, "unknown `what`");
+    return mcs_fail(MCS_ERR_INVALID, "unknown `what`");
 }
 
 int mcs_extractor_set_profiling(mcs_extractor* ex, int32_t enable) {
-    if (!ex) return fail(MCS_ERR_INVALID, "null argument");
-    CK(cudaSetDevice(ex->device));
-    if (enable) for (int i = 0; i < 4; ++i) if (!ex->ev[i]) CK(cudaEventCreate(&ex->ev[i]));
+    if (!ex) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    CUDA_CHECK(cudaSetDevice(ex->device));
+    if (enable) for (int i = 0; i < 4; ++i) if (!ex->ev[i]) CUDA_CHECK(cudaEventCreate(&ex->ev[i]));
     ex->profiling = enable != 0;
     return MCS_OK;
 }
 
 int mcs_extractor_tier_stats(mcs_extractor* ex, int32_t enable, int64_t* counts4) {
-    if (!ex) return fail(MCS_ERR_INVALID, "null extractor");
-    CK(cudaSetDevice(ex->device));
-    CK(cudaDeviceSynchronize());
+    if (!ex) return mcs_fail(MCS_ERR_INVALID, "null extractor");
+    CUDA_CHECK(cudaSetDevice(ex->device));
+    CUDA_CHECK(cudaDeviceSynchronize());
     if (counts4) {
         counts4[0] = counts4[1] = counts4[2] = counts4[3] = 0;
-        if (ex->tier_on) CK(cudaMemcpy(counts4, ex->tier.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        if (ex->tier_on) CUDA_CHECK(cudaMemcpy(counts4, ex->tier.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     }
     if (enable && !ex->tier_on) {
-        CK(ex->tier.ensure(4));
-        CK(cudaMemset(ex->tier.p, 0, 4 * sizeof(unsigned long long)));
+        CUDA_CHECK(ex->tier.ensure(4));
+        CUDA_CHECK(cudaMemset(ex->tier.p, 0, 4 * sizeof(unsigned long long)));
     }
     ex->tier_on = enable != 0;
     return MCS_OK;
 }
 
 int mcs_extractor_check_status(mcs_extractor* ex, void* stream) {
-    if (!ex) return fail(MCS_ERR_INVALID, "null extractor");
+    if (!ex) return mcs_fail(MCS_ERR_INVALID, "null extractor");
     if (!ex->status.p) return MCS_OK;                       // nothing has run yet
-    CK(cudaSetDevice(ex->device));
+    CUDA_CHECK(cudaSetDevice(ex->device));
     return check_status(ex, stream ? (cudaStream_t)stream : ex->stream);
 }
 
 int mcs_cam_distort_table(const mcs_ocam* cam, double* rows_out, int32_t max_rows, int32_t* n_rows, int32_t* row_doubles) {
-    if (!cam || !n_rows || !row_doubles) return fail(MCS_ERR_INVALID, "null argument");
-    if (rows_out && max_rows < 0) return fail(MCS_ERR_INVALID, "negative max_rows");
+    if (!cam || !n_rows || !row_doubles) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (rows_out && max_rows < 0) return mcs_fail(MCS_ERR_INVALID, "negative max_rows");
     std::vector<double> coef;
     int n = 0;
     build_distort_lut(*cam, coef, n);
@@ -885,53 +874,53 @@ int mcs_cam_distort_table(const mcs_ocam* cam, double* rows_out, int32_t max_row
 }
 
 int mcs_extractor_graph_replays(mcs_extractor* ex, int64_t* n) {
-    if (!ex || !n) return fail(MCS_ERR_INVALID, "null argument");
+    if (!ex || !n) return mcs_fail(MCS_ERR_INVALID, "null argument");
     *n = ex->sf_replays;
     return MCS_OK;
 }
 
 int mcs_extractor_get_timings(mcs_extractor* ex, float* ms3) {
-    if (!ex || !ms3) return fail(MCS_ERR_INVALID, "null argument");
-    if (!ex->profiling || !ex->ev[3]) return fail(MCS_ERR_INVALID, "profiling is not enabled");
-    CK(cudaEventSynchronize(ex->ev[3]));
-    for (int i = 0; i < 3; ++i) CK(cudaEventElapsedTime(&ms3[i], ex->ev[i], ex->ev[i + 1]));
+    if (!ex || !ms3) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (!ex->profiling || !ex->ev[3]) return mcs_fail(MCS_ERR_INVALID, "profiling is not enabled");
+    CUDA_CHECK(cudaEventSynchronize(ex->ev[3]));
+    for (int i = 0; i < 3; ++i) CUDA_CHECK(cudaEventElapsedTime(&ms3[i], ex->ev[i], ex->ev[i + 1]));
     return MCS_OK;
 }
 
 int mcs_match_stream_device(const uint8_t* desc_dev, const uint8_t* dmask_dev, const int32_t* counts_dev, int32_t n_frames,
                             int32_t n_cams, int32_t capacity, int32_t dim, int32_t K, int32_t* match_idx_dev,
                             int32_t* match_dist_dev, void* stream) {
-    if (!desc_dev || !counts_dev || !match_idx_dev || !match_dist_dev) return fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || capacity < 1 || K < 1 || K > 8) return fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
-    if (dim != 16 && dim != 32 && dim != 64) return fail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    if (!desc_dev || !counts_dev || !match_idx_dev || !match_dist_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_frames < 1 || n_cams < 1 || capacity < 1 || K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
+    if (int rc = check_desc_dim(dim)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    CK(launch_hamming_stream(desc_dev, dmask_dev, counts_dev, 0, n_frames * n_cams, n_cams, capacity, dim, K, 0xFFFFFFFFu, match_idx_dev, match_dist_dev, st));
+    CUDA_CHECK(launch_hamming_stream(desc_dev, dmask_dev, counts_dev, 0, n_frames * n_cams, n_cams, capacity, dim, K, 0xFFFFFFFFu, match_idx_dev, match_dist_dev, st));
     return MCS_OK;
 }
 
 int mcs_match_stream_greedy_device(const uint8_t* desc_dev, const uint8_t* dmask_dev, const int32_t* counts_dev, int32_t n_frames,
                                    int32_t n_cams, int32_t capacity, int32_t dim, int32_t th_low, double nnratio,
                                    int32_t* matches12_dev, int32_t* nmatches_dev, void* stream) {
-    if (!desc_dev || !counts_dev || !matches12_dev || !nmatches_dev) return fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535) return fail(MCS_ERR_INVALID, "bad sizes (capacity must be 1..65535)");
-    if (dim != 16 && dim != 32 && dim != 64) return fail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    if (!desc_dev || !counts_dev || !matches12_dev || !nmatches_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535) return mcs_fail(MCS_ERR_INVALID, "bad sizes (capacity must be 1..65535)");
+    if (int rc = check_desc_dim(dim)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     // K-best list length (the acceptance is exact for any K; K only sets how often the replay rescans).  H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs:
     // K = 8 16.08 / 16.15 ms per 384-image step (47.9 Mfeatures/s) against 16.85 / 16.79 ms with K = 4.
     constexpr int K = 8;
     const size_t n = (size_t)n_frames * n_cams * capacity;
     int *li = nullptr, *ld = nullptr, *redo = nullptr;
-    CK(keep_pool_memory());
-    CK(cudaMallocAsync((void**)&li, n * K * sizeof(int), st));
-    CK(cudaMallocAsync((void**)&ld, n * K * sizeof(int), st));
-    CK(cudaMallocAsync((void**)&redo, (size_t)n_frames * n_cams * sizeof(int), st));
+    CUDA_CHECK(keep_pool_memory());
+    CUDA_CHECK(cudaMallocAsync((void**)&li, n * K * sizeof(int), st));
+    CUDA_CHECK(cudaMallocAsync((void**)&ld, n * K * sizeof(int), st));
+    CUDA_CHECK(cudaMallocAsync((void**)&redo, (size_t)n_frames * n_cams * sizeof(int), st));
     cudaError_t e = launch_hamming_stream(desc_dev, dmask_dev, counts_dev, 0, n_frames * n_cams, n_cams, capacity, dim, K,
                                           greedy_dist_bound(th_low, nnratio), li, ld, st);
     if (e == cudaSuccess)
         e = launch_stream_replay(li, ld, counts_dev, desc_dev, dmask_dev, dim, 0, n_frames * n_cams, n_cams, capacity, K, th_low, nnratio,
                                  matches12_dev, nmatches_dev, redo, st);
     cudaFreeAsync(li, st); cudaFreeAsync(ld, st); cudaFreeAsync(redo, st);
-    CK(e);
+    CUDA_CHECK(e);
     return MCS_OK;
 }
 
@@ -940,11 +929,11 @@ int mcs_match_stream_replay_device(const int32_t* match_idx_dev, const int32_t* 
                                    int32_t dim, int32_t K, int32_t th_low, double nnratio, int32_t* matches12_dev, int32_t* nmatches_dev,
                                    int32_t* redo_dev, void* stream) {
     if (!match_idx_dev || !match_dist_dev || !counts_dev || !desc_dev || !matches12_dev || !nmatches_dev || !redo_dev)
-        return fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535 || K < 1 || K > 8) return fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
-    if (dim != 16 && dim != 32 && dim != 64) return fail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
-    CK(launch_stream_replay(match_idx_dev, match_dist_dev, counts_dev, desc_dev, dmask_dev, dim, 0, n_frames * n_cams, n_cams, capacity, K,
-                            th_low, nnratio, matches12_dev, nmatches_dev, redo_dev, (cudaStream_t)stream));
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535 || K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
+    if (int rc = check_desc_dim(dim)) return rc;
+    CUDA_CHECK(launch_stream_replay(match_idx_dev, match_dist_dev, counts_dev, desc_dev, dmask_dev, dim, 0, n_frames * n_cams, n_cams, capacity, K,
+                                    th_low, nnratio, matches12_dev, nmatches_dev, redo_dev, (cudaStream_t)stream));
     return MCS_OK;
 }
 
@@ -956,16 +945,16 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
                              int32_t* match_idx_out, int32_t* match_dist_out, void* packed_dev, int32_t th_low = 0, double nnratio = 0.0,
                              int32_t* matches12_out = nullptr, int32_t* nmatches_out = nullptr, int32_t* redo_out = nullptr) {
     if (!ex || !images || !masks || !cams || !kps_out || !desc_out || !counts_out || !match_idx_out || !match_dist_out)
-        return fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || width < 1 || height < 1 || stride < width) return fail(MCS_ERR_INVALID, "bad geometry");
-    if (capacity < ex->capacity) return fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
-    if (ex->p.learn_masks && !dmask_out) return fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
-    if (K < 1 || K > 8) return fail(MCS_ERR_INVALID, "K must be 1..8");
-    CK(cudaSetDevice(ex->device));
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_frames < 1 || n_cams < 1 || width < 1 || height < 1 || stride < width) return mcs_fail(MCS_ERR_INVALID, "bad geometry");
+    if (capacity < ex->capacity) return mcs_fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
+    if (ex->p.learn_masks && !dmask_out) return mcs_fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
+    if (K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "K must be 1..8");
+    CUDA_CHECK(cudaSetDevice(ex->device));
     cudaStream_t st = ex->stream;
-    if (!ex->s_copy) CK(cudaStreamCreateWithFlags(&ex->s_copy, cudaStreamNonBlocking));
-    if (!ex->s_out) CK(cudaStreamCreateWithFlags(&ex->s_out, cudaStreamNonBlocking));
-    if (!ex->s_match) CK(cudaStreamCreateWithFlags(&ex->s_match, cudaStreamNonBlocking));
+    if (!ex->s_copy) CUDA_CHECK(cudaStreamCreateWithFlags(&ex->s_copy, cudaStreamNonBlocking));
+    if (!ex->s_out) CUDA_CHECK(cudaStreamCreateWithFlags(&ex->s_out, cudaStreamNonBlocking));
+    if (!ex->s_match) CUDA_CHECK(cudaStreamCreateWithFlags(&ex->s_match, cudaStreamNonBlocking));
     const int n_images = n_frames * n_cams, ds = ex->p.desc_size;
     const int dpitch = (width + 63) & ~63;
     // Software pipeline over chunks of frames: H2D (copy stream) | re-pitch + K1..K3 + matching (compute stream) |
@@ -987,8 +976,8 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
     const size_t tight_img = (size_t)stride * height, pitched_img = (size_t)dpitch * height;
     std::vector<int> coi(n_images);
     for (int i = 0; i < n_images; ++i) coi[i] = i % n_cams;
-    CK(ex->in_tight.ensure(2 * tight_img * ipc + 256));
-    CK(ex->in_images.ensure(pitched_img * ipc + 256));
+    CUDA_CHECK(ex->in_tight.ensure(2 * tight_img * ipc + 256));
+    CUDA_CHECK(ex->in_images.ensure(pitched_img * ipc + 256));
     // feature buffers: the extractor's own, or the caller's packed exchange buffer (mcs_packed_layout) when one is given
     mcs_keypoint* kps_d; uint8_t* desc_d; uint8_t* dmask_d; int* counts_d;
     if (packed_dev) {
@@ -997,18 +986,18 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
         uint8_t* base = (uint8_t*)packed_dev;
         counts_d = (int*)(base + off[0]); kps_d = (mcs_keypoint*)(base + off[1]); desc_d = base + off[2]; dmask_d = base + off[3];
     } else {
-        CK(ex->kps.ensure((size_t)n_images * capacity));
-        CK(ex->desc.ensure((size_t)n_images * capacity * ds));
-        CK(ex->dmask.ensure((size_t)n_images * capacity * ds));
-        CK(ex->counts.ensure(n_images));
+        CUDA_CHECK(ex->kps.ensure((size_t)n_images * capacity));
+        CUDA_CHECK(ex->desc.ensure((size_t)n_images * capacity * ds));
+        CUDA_CHECK(ex->dmask.ensure((size_t)n_images * capacity * ds));
+        CUDA_CHECK(ex->counts.ensure(n_images));
         kps_d = ex->kps.p; desc_d = ex->desc.p; dmask_d = ex->dmask.p; counts_d = ex->counts.p;
     }
-    CK(ex->match_idx.ensure((size_t)n_images * capacity * K));
-    CK(ex->match_dist.ensure((size_t)n_images * capacity * K));
+    CUDA_CHECK(ex->match_idx.ensure((size_t)n_images * capacity * K));
+    CUDA_CHECK(ex->match_dist.ensure((size_t)n_images * capacity * K));
     const bool replay = matches12_out != nullptr;
     if (replay) {
-        if (!nmatches_out || !redo_out) return fail(MCS_ERR_INVALID, "the greedy acceptance needs all three outputs");
-        CK(ex->m12.ensure((size_t)n_images * capacity)); CK(ex->nmat.ensure(n_images)); CK(ex->redo.ensure(n_images));
+        if (!nmatches_out || !redo_out) return mcs_fail(MCS_ERR_INVALID, "the greedy acceptance needs all three outputs");
+        CUDA_CHECK(ex->m12.ensure((size_t)n_images * capacity)); CUDA_CHECK(ex->nmat.ensure(n_images)); CUDA_CHECK(ex->redo.ensure(n_images));
     }
     struct Events {                       // destroyed on every path out of this function
         std::vector<cudaEvent_t> v;
@@ -1021,10 +1010,10 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
     } events;
     std::vector<cudaEvent_t> ev_in(n_chunks), ev_free(n_chunks), ev_feat(n_chunks), ev_done(n_chunks);
     for (int c = 0; c < n_chunks; ++c) {
-        CK(events.add(&ev_in[c], cudaEventDisableTiming));
-        CK(events.add(&ev_free[c], cudaEventDisableTiming));
-        CK(events.add(&ev_feat[c], cudaEventDisableTiming));
-        CK(events.add(&ev_done[c], cudaEventDisableTiming));
+        CUDA_CHECK(events.add(&ev_in[c], cudaEventDisableTiming));
+        CUDA_CHECK(events.add(&ev_free[c], cudaEventDisableTiming));
+        CUDA_CHECK(events.add(&ev_feat[c], cudaEventDisableTiming));
+        CUDA_CHECK(events.add(&ev_done[c], cudaEventDisableTiming));
     }
     // Everything asynchronous happens inside enqueue(); whatever it returns, the three streams are drained before this
     // function returns, because the copies read caller memory and the local cam-of-image table.
@@ -1033,55 +1022,55 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
     if (rc == MCS_OK) rc = ensure_batch(ex, ipc);
     if (rc == MCS_OK) rc = upload_small_inputs(ex, width, height, masks, cams, n_cams, st);     // before the first image copy, see there
     if (rc) return rc;
-    CK(ex->coi_all.ensure(n_images));
-    CK(cudaMemcpyAsync(ex->coi_all.p, coi.data(), sizeof(int) * n_images, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(ex->coi_all.ensure(n_images));
+    CUDA_CHECK(cudaMemcpyAsync(ex->coi_all.p, coi.data(), sizeof(int) * n_images, cudaMemcpyHostToDevice, st));
     const uint8_t* dmask_for_match = ex->p.learn_masks ? dmask_d : nullptr;
     for (int c = 0; c < n_chunks && rc == MCS_OK; ++c) {
         const int img_lo = chunk_lo[c] * n_cams, nimg = (chunk_lo[c + 1] - chunk_lo[c]) * n_cams;
         if (nimg <= 0) continue;
         uint8_t* tight = ex->in_tight.p + (size_t)(c & 1) * tight_img * ipc;
-        if (c >= 2) CK(cudaStreamWaitEvent(ex->s_copy, ev_free[c - 2], 0));          // staging buffer consumed
-        CK(cudaMemcpyAsync(tight, images + (size_t)img_lo * tight_img, tight_img * nimg - (c == n_chunks - 1 ? (size_t)(stride - width) : 0),
-                           cudaMemcpyHostToDevice, ex->s_copy));
-        CK(cudaEventRecord(ev_in[c], ex->s_copy));
-        CK(cudaStreamWaitEvent(st, ev_in[c], 0));
+        if (c >= 2) CUDA_CHECK(cudaStreamWaitEvent(ex->s_copy, ev_free[c - 2], 0));          // staging buffer consumed
+        CUDA_CHECK(cudaMemcpyAsync(tight, images + (size_t)img_lo * tight_img, tight_img * nimg - (c == n_chunks - 1 ? (size_t)(stride - width) : 0),
+                                   cudaMemcpyHostToDevice, ex->s_copy));
+        CUDA_CHECK(cudaEventRecord(ev_in[c], ex->s_copy));
+        CUDA_CHECK(cudaStreamWaitEvent(st, ev_in[c], 0));
         launch_repitch(tight, stride, ex->in_images.p, dpitch, width, (size_t)height * nimg, st);
-        CK(cudaEventRecord(ev_free[c], st));
+        CUDA_CHECK(cudaEventRecord(ev_free[c], st));
         rc = run_pipeline(ex, nimg, ex->in_images.p, width, height, dpitch, masks, cams, n_cams, coi.data() + img_lo,
                           kps_d + (size_t)img_lo * capacity, desc_d + (size_t)img_lo * capacity * ds,
                           dmask_d + (size_t)img_lo * capacity * ds, counts_d + img_lo, capacity, st, false, ex->coi_all.p + img_lo);
         if (rc) break;
-        CK(cudaEventRecord(ev_feat[c], st));                              // features of the chunk are final: their D2H overlaps the matching
+        CUDA_CHECK(cudaEventRecord(ev_feat[c], st));                              // features of the chunk are final: their D2H overlaps the matching
         // the matching of chunk c runs on its own stream, so that K1..K3 of chunk c+1 (on `st`) fill the SMs behind its tail;
         // it reads descriptors of this chunk and of the last frame of the previous one, both final at ev_feat[c]
-        CK(cudaStreamWaitEvent(ex->s_match, ev_feat[c], 0));
+        CUDA_CHECK(cudaStreamWaitEvent(ex->s_match, ev_feat[c], 0));
         // with the greedy acceptance on the device the lists only need the entries that can influence it (kernels.h: greedy_dist_bound)
-        CK(launch_hamming_stream(desc_d, dmask_for_match, counts_d, img_lo, nimg, n_cams, capacity, ds, K,
-                                 replay ? greedy_dist_bound(th_low, nnratio) : 0xFFFFFFFFu, ex->match_idx.p, ex->match_dist.p, ex->s_match));
+        CUDA_CHECK(launch_hamming_stream(desc_d, dmask_for_match, counts_d, img_lo, nimg, n_cams, capacity, ds, K,
+                                         replay ? greedy_dist_bound(th_low, nnratio) : 0xFFFFFFFFu, ex->match_idx.p, ex->match_dist.p, ex->s_match));
         if (replay)     // greedy acceptance of SearchByBoW(KF1, KF2) over the lists of this chunk, still on the device
-            CK(launch_stream_replay(ex->match_idx.p, ex->match_dist.p, counts_d, desc_d, dmask_for_match, ds, img_lo, nimg, n_cams, capacity, K,
-                                    th_low, nnratio, ex->m12.p, ex->nmat.p, ex->redo.p, ex->s_match));
-        CK(cudaEventRecord(ev_done[c], ex->s_match));
+            CUDA_CHECK(launch_stream_replay(ex->match_idx.p, ex->match_dist.p, counts_d, desc_d, dmask_for_match, ds, img_lo, nimg, n_cams, capacity, K,
+                                            th_low, nnratio, ex->m12.p, ex->nmat.p, ex->redo.p, ex->s_match));
+        CUDA_CHECK(cudaEventRecord(ev_done[c], ex->s_match));
         cudaStream_t so = ex->s_out;
-        CK(cudaStreamWaitEvent(so, ev_feat[c], 0));
-        CK(cudaMemcpyAsync(counts_out + img_lo, counts_d + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
-        CK(cudaMemcpyAsync(kps_out + (size_t)img_lo * capacity, kps_d + (size_t)img_lo * capacity,
-                           sizeof(mcs_keypoint) * (size_t)nimg * capacity, cudaMemcpyDeviceToHost, so));
-        CK(cudaMemcpyAsync(desc_out + (size_t)img_lo * capacity * ds, desc_d + (size_t)img_lo * capacity * ds,
-                           (size_t)nimg * capacity * ds, cudaMemcpyDeviceToHost, so));
+        CUDA_CHECK(cudaStreamWaitEvent(so, ev_feat[c], 0));
+        CUDA_CHECK(cudaMemcpyAsync(counts_out + img_lo, counts_d + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
+        CUDA_CHECK(cudaMemcpyAsync(kps_out + (size_t)img_lo * capacity, kps_d + (size_t)img_lo * capacity,
+                                   sizeof(mcs_keypoint) * (size_t)nimg * capacity, cudaMemcpyDeviceToHost, so));
+        CUDA_CHECK(cudaMemcpyAsync(desc_out + (size_t)img_lo * capacity * ds, desc_d + (size_t)img_lo * capacity * ds,
+                                   (size_t)nimg * capacity * ds, cudaMemcpyDeviceToHost, so));
         if (dmask_out)
-            CK(cudaMemcpyAsync(dmask_out + (size_t)img_lo * capacity * ds, dmask_d + (size_t)img_lo * capacity * ds,
-                               (size_t)nimg * capacity * ds, cudaMemcpyDeviceToHost, so));
-        CK(cudaStreamWaitEvent(so, ev_done[c], 0));
-        CK(cudaMemcpyAsync(match_idx_out + (size_t)img_lo * capacity * K, ex->match_idx.p + (size_t)img_lo * capacity * K,
-                           sizeof(int) * (size_t)nimg * capacity * K, cudaMemcpyDeviceToHost, so));
-        CK(cudaMemcpyAsync(match_dist_out + (size_t)img_lo * capacity * K, ex->match_dist.p + (size_t)img_lo * capacity * K,
-                           sizeof(int) * (size_t)nimg * capacity * K, cudaMemcpyDeviceToHost, so));
+            CUDA_CHECK(cudaMemcpyAsync(dmask_out + (size_t)img_lo * capacity * ds, dmask_d + (size_t)img_lo * capacity * ds,
+                                       (size_t)nimg * capacity * ds, cudaMemcpyDeviceToHost, so));
+        CUDA_CHECK(cudaStreamWaitEvent(so, ev_done[c], 0));
+        CUDA_CHECK(cudaMemcpyAsync(match_idx_out + (size_t)img_lo * capacity * K, ex->match_idx.p + (size_t)img_lo * capacity * K,
+                                   sizeof(int) * (size_t)nimg * capacity * K, cudaMemcpyDeviceToHost, so));
+        CUDA_CHECK(cudaMemcpyAsync(match_dist_out + (size_t)img_lo * capacity * K, ex->match_dist.p + (size_t)img_lo * capacity * K,
+                                   sizeof(int) * (size_t)nimg * capacity * K, cudaMemcpyDeviceToHost, so));
         if (replay) {
-            CK(cudaMemcpyAsync(matches12_out + (size_t)img_lo * capacity, ex->m12.p + (size_t)img_lo * capacity, sizeof(int) * (size_t)nimg * capacity,
-                               cudaMemcpyDeviceToHost, so));
-            CK(cudaMemcpyAsync(nmatches_out + img_lo, ex->nmat.p + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
-            CK(cudaMemcpyAsync(redo_out + img_lo, ex->redo.p + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
+            CUDA_CHECK(cudaMemcpyAsync(matches12_out + (size_t)img_lo * capacity, ex->m12.p + (size_t)img_lo * capacity, sizeof(int) * (size_t)nimg * capacity,
+                                       cudaMemcpyDeviceToHost, so));
+            CUDA_CHECK(cudaMemcpyAsync(nmatches_out + img_lo, ex->nmat.p + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
+            CUDA_CHECK(cudaMemcpyAsync(redo_out + img_lo, ex->redo.p + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
         }
     }
     return rc;
@@ -1090,7 +1079,7 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
     cudaError_t e1 = cudaStreamSynchronize(ex->s_copy), e2 = cudaStreamSynchronize(st), e3 = cudaStreamSynchronize(ex->s_out);
     { const cudaError_t e4 = cudaStreamSynchronize(ex->s_match); if (e2 == cudaSuccess) e2 = e4; }
     if (rc) return rc;
-    CK(e1); CK(e2); CK(e3);
+    CUDA_CHECK(e1); CUDA_CHECK(e2); CUDA_CHECK(e3);
     ex->last_n_images = (chunk_lo[n_chunks] - chunk_lo[n_chunks - 1]) * n_cams;
     return check_status(ex, st);
 }
@@ -1118,7 +1107,7 @@ int mcs_extract_match_stream_packed(mcs_extractor* ex, int32_t n_frames, int32_t
 int mcs_extract_batch_packed_device(mcs_extractor* ex, int32_t n_images, const uint8_t* images_dev, int32_t width, int32_t height,
                                     int32_t stride, const uint8_t* masks, const mcs_ocam* cams, int32_t n_cams,
                                     const int32_t* cam_of_image, void* packed_dev, int32_t capacity, void* stream) {
-    if (!ex || !packed_dev) return fail(MCS_ERR_INVALID, "null argument");
+    if (!ex || !packed_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
     size_t off[4];
     mcs_packed_layout(n_images, capacity, ex->p.desc_size, off);
     uint8_t* base = (uint8_t*)packed_dev;

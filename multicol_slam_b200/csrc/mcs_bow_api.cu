@@ -11,29 +11,11 @@
 #include <vector>
 #include <cuda_runtime.h>
 #include "../../include/mcs_b200.h"
+#include "api_check.h"
 #include "kernels.h"
 #include "dev_scratch.h"
 
 using namespace mcs;
-
-void mcs_set_error_(const std::string& msg);   // mcs_api.cu
-
-namespace {
-
-int bfail(int code, const std::string& msg) { mcs_set_error_(msg); return code; }
-
-#define BCK(expr)                                                                                      \
-    do {                                                                                               \
-        cudaError_t e__ = (expr);                                                                      \
-        if (e__ != cudaSuccess) {                                                                      \
-            cudaGetLastError();                                                                        \
-            return bfail(e__ == cudaErrorNoDevice || e__ == cudaErrorInsufficientDriver ? MCS_ERR_NO_DEVICE : MCS_ERR_CUDA, \
-                         std::string(#expr) + ": " + cudaGetErrorString(e__));                         \
-        }                                                                                              \
-    } while (0)
-
-
-}  // namespace
 
 struct mcs_vocabulary {
     int k = 0, L = 0, scoring = 0, weighting = 0, n_nodes = 0, n_words = 0, device = 0;
@@ -46,26 +28,26 @@ extern "C" {
 int mcs_vocabulary_create(int32_t k, int32_t L, int32_t scoring, int32_t weighting, int32_t n_nodes, const int32_t* parent,
                           const double* weight, const uint8_t* descriptors, const int32_t* node_order, int32_t n_words,
                           const int32_t* word_node, mcs_vocabulary** out) {
-    if (!out) return bfail(MCS_ERR_INVALID, "null argument");
+    if (!out) return mcs_fail(MCS_ERR_INVALID, "null argument");
     *out = nullptr;
-    if (!parent || !weight || !descriptors || !word_node) return bfail(MCS_ERR_INVALID, "null argument");
-    if (n_nodes < 2 || n_words < 1 || k < 1 || L < 1) return bfail(MCS_ERR_INVALID, "empty vocabulary");
-    if (scoring < 0 || scoring > 5 || weighting < 0 || weighting > 3) return bfail(MCS_ERR_INVALID, "unknown scoring / weighting type");
+    if (!parent || !weight || !descriptors || !word_node) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_nodes < 2 || n_words < 1 || k < 1 || L < 1) return mcs_fail(MCS_ERR_INVALID, "empty vocabulary");
+    if (scoring < 0 || scoring > 5 || weighting < 0 || weighting > 3) return mcs_fail(MCS_ERR_INVALID, "unknown scoring / weighting type");
     // children in the reference's push_back order (ref TemplatedVocabulary.h:1596-1608)
     std::vector<int> cnt(n_nodes + 1, 0), ids(n_nodes - 1), won(n_nodes, -1);
     std::vector<uint8_t> seen(n_nodes, 0);
     for (int i = 0; i + 1 < n_nodes; ++i) {
         const int nid = node_order ? node_order[i] : i + 1;
-        if (nid < 1 || nid >= n_nodes || seen[nid]) return bfail(MCS_ERR_INVALID, "node_order is not a permutation of 1..n_nodes-1");
+        if (nid < 1 || nid >= n_nodes || seen[nid]) return mcs_fail(MCS_ERR_INVALID, "node_order is not a permutation of 1..n_nodes-1");
         seen[nid] = 1;
         const int pid = parent[nid];
-        if (pid < 0 || pid >= n_nodes || pid == nid) return bfail(MCS_ERR_INVALID, "parent id out of range");
+        if (pid < 0 || pid >= n_nodes || pid == nid) return mcs_fail(MCS_ERR_INVALID, "parent id out of range");
         ++cnt[pid + 1];
     }
     for (int i = 0; i < n_nodes; ++i)
-        if (cnt[i + 1] > 65535) return bfail(MCS_ERR_UNSUPPORTED, "more than 65535 children under one node (the descent packs the child position in 16 bits)");
+        if (cnt[i + 1] > 65535) return mcs_fail(MCS_ERR_UNSUPPORTED, "more than 65535 children under one node (the descent packs the child position in 16 bits)");
     for (int i = 0; i < n_nodes; ++i) cnt[i + 1] += cnt[i];
-    if (cnt[1] == 0) return bfail(MCS_ERR_INVALID, "the root has no children");
+    if (cnt[1] == 0) return mcs_fail(MCS_ERR_INVALID, "the root has no children");
     std::vector<int> cur(cnt.begin(), cnt.end() - 1);
     for (int i = 0; i + 1 < n_nodes; ++i) {
         const int nid = node_order ? node_order[i] : i + 1;
@@ -74,36 +56,29 @@ int mcs_vocabulary_create(int32_t k, int32_t L, int32_t scoring, int32_t weighti
     for (int i = 1; i < n_nodes; ++i) {                  // every node must hang under the root: walk up at most n_nodes steps
         int a = i, steps = 0;
         while (a != 0 && steps <= n_nodes) { a = parent[a]; ++steps; }
-        if (a != 0) return bfail(MCS_ERR_INVALID, "parent links contain a cycle");
+        if (a != 0) return mcs_fail(MCS_ERR_INVALID, "parent links contain a cycle");
     }
     for (int w = 0; w < n_words; ++w) {
         const int nid = word_node[w];
-        if (nid < 1 || nid >= n_nodes || cnt[nid + 1] != cnt[nid]) return bfail(MCS_ERR_INVALID, "word_node must name leaves");
+        if (nid < 1 || nid >= n_nodes || cnt[nid + 1] != cnt[nid]) return mcs_fail(MCS_ERR_INVALID, "word_node must name leaves");
         won[nid] = w;
     }
     for (int i = 1; i < n_nodes; ++i)
-        if (cnt[i + 1] == cnt[i] && won[i] < 0) return bfail(MCS_ERR_INVALID, "a leaf has no word id");
+        if (cnt[i + 1] == cnt[i] && won[i] < 0) return mcs_fail(MCS_ERR_INVALID, "a leaf has no word id");
     int ndev = 0;
-    BCK(cudaGetDeviceCount(&ndev));
-    if (ndev == 0) return bfail(MCS_ERR_NO_DEVICE, "no CUDA device");
+    CUDA_CHECK(cudaGetDeviceCount(&ndev));
+    if (ndev == 0) return mcs_fail(MCS_ERR_NO_DEVICE, "no CUDA device");
     mcs_vocabulary* v = new mcs_vocabulary();
     v->k = k; v->L = L; v->scoring = scoring; v->weighting = weighting; v->n_nodes = n_nodes; v->n_words = n_words;
     cudaError_t e = cudaGetDevice(&v->device);
-    if (e == cudaSuccess) e = v->child_off.alloc((size_t)(n_nodes + 1) * 4);
-    if (e == cudaSuccess) e = v->child_ids.alloc((size_t)(n_nodes - 1) * 4);
-    if (e == cudaSuccess) e = v->desc.alloc((size_t)n_nodes * 32);
-    if (e == cudaSuccess) e = v->word_of_node.alloc((size_t)n_nodes * 4);
-    if (e == cudaSuccess) e = v->weight.alloc((size_t)n_nodes * 8);
-    if (e == cudaSuccess) e = cudaMemcpy(v->child_off.p, cnt.data(), (size_t)(n_nodes + 1) * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->child_ids.p, ids.data(), (size_t)(n_nodes - 1) * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->desc.p, descriptors, (size_t)n_nodes * 32, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->word_of_node.p, won.data(), (size_t)n_nodes * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(v->weight.p, weight, (size_t)n_nodes * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = v->child_off.upload(cnt.data(), (size_t)(n_nodes + 1) * 4);
+    if (e == cudaSuccess) e = v->child_ids.upload(ids.data(), (size_t)(n_nodes - 1) * 4);
+    if (e == cudaSuccess) e = v->desc.upload(descriptors, (size_t)n_nodes * 32);
+    if (e == cudaSuccess) e = v->word_of_node.upload(won.data(), (size_t)n_nodes * 4);
+    if (e == cudaSuccess) e = v->weight.upload(weight, (size_t)n_nodes * 8);
     if (e != cudaSuccess) {
         delete v;
-        cudaGetLastError();
-        return bfail(e == cudaErrorNoDevice || e == cudaErrorInsufficientDriver ? MCS_ERR_NO_DEVICE : MCS_ERR_CUDA,
-                     std::string("vocabulary upload: ") + cudaGetErrorString(e));
+        return mcs_cuda_fail(e, "vocabulary upload");
     }
     v->view = VocabularyDev{v->child_off.as<int>(), v->child_ids.as<int>(), v->desc.as<uint4>(), v->word_of_node.as<int>(),
                             v->weight.as<double>(), n_nodes, L};
@@ -115,31 +90,31 @@ void mcs_vocabulary_destroy(mcs_vocabulary* voc) { delete voc; }
 
 int mcs_bow_transform(const mcs_vocabulary* voc, const uint8_t* desc, int32_t n, int32_t levelsup, int32_t* word_id, double* weight,
                       int32_t* node_id) {
-    if (!voc || (n > 0 && !desc)) return bfail(MCS_ERR_INVALID, "null argument");
+    if (!voc || (n > 0 && !desc)) return mcs_fail(MCS_ERR_INVALID, "null argument");
     if (n <= 0) return MCS_OK;
     {   // the tree lives on the device that was current when the vocabulary was created: a call from a thread whose current
         // device differs would hand the kernel foreign pointers
         int cur = -1;
-        BCK(cudaGetDevice(&cur));
-        if (cur != voc->device) return bfail(MCS_ERR_INVALID, "vocabulary was created on another CUDA device than the current one");
+        CUDA_CHECK(cudaGetDevice(&cur));
+        if (cur != voc->device) return mcs_fail(MCS_ERR_INVALID, "vocabulary was created on another CUDA device than the current one");
     }
     Dev dd, dw, dwt, dn;
-    BCK(dd.alloc((size_t)n * 32)); BCK(dw.alloc((size_t)n * 4)); BCK(dwt.alloc((size_t)n * 8)); BCK(dn.alloc((size_t)n * 4));
-    BCK(cudaMemcpy(dd.p, desc, (size_t)n * 32, cudaMemcpyHostToDevice));
-    BCK(launch_bow_descend(voc->view, dd.as<uint8_t>(), n, levelsup, dw.as<int>(), dwt.as<double>(), dn.as<int>(), nullptr));
-    if (word_id) BCK(cudaMemcpy(word_id, dw.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
-    if (weight) BCK(cudaMemcpy(weight, dwt.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
-    if (node_id) BCK(cudaMemcpy(node_id, dn.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
-    BCK(cudaDeviceSynchronize());
+    CUDA_CHECK(dd.upload(desc, (size_t)n * 32));
+    CUDA_CHECK(dw.alloc((size_t)n * 4)); CUDA_CHECK(dwt.alloc((size_t)n * 8)); CUDA_CHECK(dn.alloc((size_t)n * 4));
+    CUDA_CHECK(launch_bow_descend(voc->view, dd.as<uint8_t>(), n, levelsup, dw.as<int>(), dwt.as<double>(), dn.as<int>(), nullptr));
+    if (word_id) CUDA_CHECK(cudaMemcpy(word_id, dw.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    if (weight) CUDA_CHECK(cudaMemcpy(weight, dwt.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    if (node_id) CUDA_CHECK(cudaMemcpy(node_id, dn.p, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaDeviceSynchronize());
     return MCS_OK;
 }
 
 int mcs_bow_vectors(const mcs_vocabulary* voc, const uint8_t* desc, int32_t n, int32_t levelsup, int32_t* bow_words,
                     double* bow_values, int32_t* n_bow, int32_t* fv_nodes, int32_t* fv_offsets, int32_t* n_fv, int32_t* fv_features) {
-    if (!voc || !n_bow || !n_fv || !fv_offsets) return bfail(MCS_ERR_INVALID, "null argument");
+    if (!voc || !n_bow || !n_fv || !fv_offsets) return mcs_fail(MCS_ERR_INVALID, "null argument");
     *n_bow = 0; *n_fv = 0; fv_offsets[0] = 0;
     if (n <= 0) return MCS_OK;
-    if (!bow_words || !bow_values || !fv_nodes || !fv_features) return bfail(MCS_ERR_INVALID, "null argument");
+    if (!bow_words || !bow_values || !fv_nodes || !fv_features) return mcs_fail(MCS_ERR_INVALID, "null argument");
     std::vector<int> word(n), node(n);
     std::vector<double> wt(n);
     const int rc = mcs_bow_transform(voc, desc, n, levelsup, word.data(), wt.data(), node.data());
@@ -189,7 +164,7 @@ int mcs_bow_vectors(const mcs_vocabulary* voc, const uint8_t* desc, int32_t n, i
 
 int mcs_bow_score(const mcs_vocabulary* voc, const int32_t* w1, const double* v1, int32_t n1, const int32_t* w2, const double* v2,
                   int32_t n2, double* score_out) {
-    if (!voc || !score_out || (n1 > 0 && (!w1 || !v1)) || (n2 > 0 && (!w2 || !v2))) return bfail(MCS_ERR_INVALID, "null argument");
+    if (!voc || !score_out || (n1 > 0 && (!w1 || !v1)) || (n2 > 0 && (!w2 || !v2))) return mcs_fail(MCS_ERR_INVALID, "null argument");
     const int kind = voc->scoring;
     const double log_eps = std::log(DBL_EPSILON);                              // GeneralScoring::LOG_EPS (ref ScoringObject.cpp:18)
     double acc = 0;
@@ -223,27 +198,27 @@ int mcs_search_by_bow(const uint8_t* desc1, const uint8_t* mask1, const uint8_t*
                       const int32_t* fv1_offsets, int32_t n_fv1, const int32_t* fv1_features, const uint8_t* desc2, const uint8_t* mask2,
                       int32_t n2, const int32_t* fv2_nodes, const int32_t* fv2_offsets, int32_t n_fv2, const int32_t* fv2_features,
                       int32_t dim, int32_t th_low, double nnratio, int32_t* match_of_2, int32_t* nmatches) {
-    if (!match_of_2 || !nmatches) return bfail(MCS_ERR_INVALID, "null argument");
-    if (dim != 16 && dim != 32 && dim != 64) return bfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    if (!match_of_2 || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_desc_dim(dim)) return rc;
     *nmatches = 0;
     for (int i = 0; i < n2; ++i) match_of_2[i] = -1;
     if (n1 <= 0 || n2 <= 0 || n_fv1 <= 0 || n_fv2 <= 0) return MCS_OK;
     if (!desc1 || !desc2 || !fv1_nodes || !fv1_offsets || !fv1_features || !fv2_nodes || !fv2_offsets || !fv2_features)
-        return bfail(MCS_ERR_INVALID, "null argument");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
     // feature vectors are std::map<NodeId, vector<unsigned>> in the reference: node ids strictly ascending, CSR offsets monotone
     for (int side = 0; side < 2; ++side) {
         const int32_t* nodes = side ? fv2_nodes : fv1_nodes;
         const int32_t* off = side ? fv2_offsets : fv1_offsets;
         const int n = side ? n_fv2 : n_fv1;
-        if (off[0] < 0) return bfail(MCS_ERR_INVALID, "feature-vector offsets must start at >= 0");
+        if (off[0] < 0) return mcs_fail(MCS_ERR_INVALID, "feature-vector offsets must start at >= 0");
         for (int i = 0; i < n; ++i) {
-            if (off[i + 1] < off[i]) return bfail(MCS_ERR_INVALID, "feature-vector offsets must be non-decreasing");
-            if (i > 0 && nodes[i] <= nodes[i - 1]) return bfail(MCS_ERR_INVALID, "feature-vector node ids must be strictly ascending");
+            if (off[i + 1] < off[i]) return mcs_fail(MCS_ERR_INVALID, "feature-vector offsets must be non-decreasing");
+            if (i > 0 && nodes[i] <= nodes[i - 1]) return mcs_fail(MCS_ERR_INVALID, "feature-vector node ids must be strictly ascending");
         }
     }
     const int nf1 = fv1_offsets[n_fv1], nf2 = fv2_offsets[n_fv2];
-    for (int i = fv1_offsets[0]; i < nf1; ++i) if (fv1_features[i] < 0 || fv1_features[i] >= n1) return bfail(MCS_ERR_INVALID, "feature index out of range");
-    for (int i = fv2_offsets[0]; i < nf2; ++i) if (fv2_features[i] < 0 || fv2_features[i] >= n2) return bfail(MCS_ERR_INVALID, "feature index out of range");
+    for (int i = fv1_offsets[0]; i < nf1; ++i) if (fv1_features[i] < 0 || fv1_features[i] >= n1) return mcs_fail(MCS_ERR_INVALID, "feature index out of range");
+    for (int i = fv2_offsets[0]; i < nf2; ++i) if (fv2_features[i] < 0 || fv2_features[i] >= n2) return mcs_fail(MCS_ERR_INVALID, "feature index out of range");
     const bool masked = mask1 && mask2;
     // queries in the reference's visiting order: common nodes ascending, key-frame keypoints in list order (ref :199-217)
     std::vector<GroupQuery> qs;
@@ -262,14 +237,12 @@ int mcs_search_by_bow(const uint8_t* desc1, const uint8_t* mask1, const uint8_t*
     }
     if (qs.empty()) return MCS_OK;
     Dev d1, m1, d2, m2, dc;
-    BCK(d1.alloc((size_t)n1 * dim)); BCK(d2.alloc((size_t)n2 * dim)); BCK(dc.alloc((size_t)nf2 * 4));
-    BCK(cudaMemcpy(d1.p, desc1, (size_t)n1 * dim, cudaMemcpyHostToDevice));
-    BCK(cudaMemcpy(d2.p, desc2, (size_t)n2 * dim, cudaMemcpyHostToDevice));
-    BCK(cudaMemcpy(dc.p, fv2_features, (size_t)nf2 * 4, cudaMemcpyHostToDevice));
+    CUDA_CHECK(d1.upload(desc1, (size_t)n1 * dim));
+    CUDA_CHECK(d2.upload(desc2, (size_t)n2 * dim));
+    CUDA_CHECK(dc.upload(fv2_features, (size_t)nf2 * 4));
     if (masked) {
-        BCK(m1.alloc((size_t)n1 * dim)); BCK(m2.alloc((size_t)n2 * dim));
-        BCK(cudaMemcpy(m1.p, mask1, (size_t)n1 * dim, cudaMemcpyHostToDevice));
-        BCK(cudaMemcpy(m2.p, mask2, (size_t)n2 * dim, cudaMemcpyHostToDevice));
+        CUDA_CHECK(m1.upload(mask1, (size_t)n1 * dim));
+        CUDA_CHECK(m2.upload(mask2, (size_t)n2 * dim));
     }
     // distance lists go through a bounded staging buffer: consecutive queries are cut into chunks of <= kChunk distances
     const size_t kChunk = (size_t)8 << 20;
@@ -281,16 +254,16 @@ int mcs_search_by_bow(const uint8_t* desc1, const uint8_t* mask1, const uint8_t*
         s = e;
     }
     Dev dq, dout;
-    BCK(dq.alloc(qs.size() * sizeof(GroupQuery))); BCK(dout.alloc(biggest * 4));
+    CUDA_CHECK(dq.alloc(qs.size() * sizeof(GroupQuery))); CUDA_CHECK(dout.alloc(biggest * 4));
     std::vector<int> dist(biggest);
     int nm = 0;
     for (size_t s = 0; s < qs.size();) {
         size_t tot = 0, e = s;
         while (e < qs.size() && (e == s || tot + qs[e].cand_count <= kChunk)) { qs[e].out_off = (int)tot; tot += qs[e].cand_count; ++e; }
-        BCK(cudaMemcpy(dq.as<GroupQuery>() + s, qs.data() + s, (e - s) * sizeof(GroupQuery), cudaMemcpyHostToDevice));
-        BCK(launch_group_distance(dq.as<GroupQuery>() + s, (int)(e - s), d1.as<uint8_t>(), masked ? m1.as<uint8_t>() : nullptr,
-                                  d2.as<uint8_t>(), masked ? m2.as<uint8_t>() : nullptr, dc.as<int>(), dim, dout.as<int>(), nullptr));
-        BCK(cudaMemcpy(dist.data(), dout.p, tot * 4, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(dq.as<GroupQuery>() + s, qs.data() + s, (e - s) * sizeof(GroupQuery), cudaMemcpyHostToDevice));
+        CUDA_CHECK(launch_group_distance(dq.as<GroupQuery>() + s, (int)(e - s), d1.as<uint8_t>(), masked ? m1.as<uint8_t>() : nullptr,
+                                         d2.as<uint8_t>(), masked ? m2.as<uint8_t>() : nullptr, dc.as<int>(), dim, dout.as<int>(), nullptr));
+        CUDA_CHECK(cudaMemcpy(dist.data(), dout.p, tot * 4, cudaMemcpyDeviceToHost));
         // host: the reference's sequential scan over the GPU distances (ref :226-279)
         for (size_t qi = s; qi < e; ++qi) {
             const GroupQuery& q = qs[qi];

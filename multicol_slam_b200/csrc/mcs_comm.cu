@@ -11,13 +11,11 @@
 #include <mutex>
 #include <string>
 
+#include "api_check.h"
 #include "kernels.h"
 #include "mcs_common.cuh"
 
-void mcs_set_error_(const std::string& msg);   // mcs_api.cu
-
 namespace {
-int cfail(int code, const std::string& msg) { mcs_set_error_(msg); return code; }
 
 // the slice of nccl.h this file needs (NCCL 2.x ABI)
 struct NcclUniqueId { char internal[128]; };
@@ -66,28 +64,28 @@ struct mcs_comm {
 extern "C" {
 
 int mcs_comm_unique_id(uint8_t* id128) {
-    if (!id128) return cfail(MCS_ERR_INVALID, "null argument");
+    if (!id128) return mcs_fail(MCS_ERR_INVALID, "null argument");
     Nccl& n = nccl();
-    if (!n.handle) return cfail(MCS_ERR_UNSUPPORTED, n.why);
+    if (!n.handle) return mcs_fail(MCS_ERR_UNSUPPORTED, n.why);
     NcclUniqueId id;
     const int rc = n.GetUniqueId(&id);
-    if (rc) return cfail(MCS_ERR_CUDA, nccl_err(rc));
+    if (rc) return mcs_fail(MCS_ERR_CUDA, nccl_err(rc));
     std::memcpy(id128, id.internal, 128);
     return MCS_OK;
 }
 
 int mcs_comm_create(const uint8_t* id128, int32_t rank, int32_t world, mcs_comm** out) {
-    if (!id128 || !out || world < 1 || rank < 0 || rank >= world) return cfail(MCS_ERR_INVALID, "bad communicator arguments");
+    if (!id128 || !out || world < 1 || rank < 0 || rank >= world) return mcs_fail(MCS_ERR_INVALID, "bad communicator arguments");
     Nccl& n = nccl();
-    if (!n.handle) return cfail(MCS_ERR_UNSUPPORTED, n.why);
+    if (!n.handle) return mcs_fail(MCS_ERR_UNSUPPORTED, n.why);
     mcs_comm* c = new mcs_comm();
     c->rank = rank; c->world = world;
     cudaError_t e = cudaGetDevice(&c->device);
-    if (e != cudaSuccess) { delete c; return cfail(MCS_ERR_NO_DEVICE, cudaGetErrorString(e)); }
+    if (e != cudaSuccess) { delete c; return mcs_fail(MCS_ERR_NO_DEVICE, cudaGetErrorString(e)); }
     NcclUniqueId id;
     std::memcpy(id.internal, id128, 128);
     const int rc = n.CommInitRank(&c->comm, world, id, rank);        // collective: every rank of the rig calls it
-    if (rc) { delete c; return cfail(MCS_ERR_CUDA, nccl_err(rc)); }
+    if (rc) { delete c; return mcs_fail(MCS_ERR_CUDA, nccl_err(rc)); }
     *out = c;
     return MCS_OK;
 }
@@ -99,7 +97,7 @@ void mcs_comm_destroy(mcs_comm* c) {
 }
 
 int mcs_comm_info(const mcs_comm* c, int32_t* rank, int32_t* world, int32_t* nccl_version) {
-    if (!c) return cfail(MCS_ERR_INVALID, "null communicator");
+    if (!c) return mcs_fail(MCS_ERR_INVALID, "null communicator");
     if (rank) *rank = c->rank;
     if (world) *world = c->world;
     if (nccl_version) { int v = 0; if (nccl().GetVersion) nccl().GetVersion(&v); *nccl_version = v; }
@@ -122,12 +120,12 @@ size_t mcs_packed_layout(int32_t n_images, int32_t capacity, int32_t dim, size_t
 size_t mcs_slot_bytes(int32_t capacity, int32_t dim) { return mcs_packed_layout(1, capacity, dim, nullptr); }
 
 int mcs_allgather_features(mcs_comm* c, const void* packed_dev, size_t bytes, void* gathered_dev, void* stream) {
-    if (!c || !packed_dev || !gathered_dev || bytes == 0) return cfail(MCS_ERR_INVALID, "null argument");
+    if (!c || !packed_dev || !gathered_dev || bytes == 0) return mcs_fail(MCS_ERR_INVALID, "null argument");
     int dev = -1;
     cudaGetDevice(&dev);
-    if (dev != c->device) return cfail(MCS_ERR_INVALID, "the communicator belongs to another CUDA device than the current one");
+    if (dev != c->device) return mcs_fail(MCS_ERR_INVALID, "the communicator belongs to another CUDA device than the current one");
     const int rc = nccl().AllGather(packed_dev, gathered_dev, bytes, kNcclUint8, c->comm, (cudaStream_t)stream);
-    if (rc) return cfail(MCS_ERR_CUDA, nccl_err(rc));
+    if (rc) return mcs_fail(MCS_ERR_CUDA, nccl_err(rc));
     return MCS_OK;
 }
 

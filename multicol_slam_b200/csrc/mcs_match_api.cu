@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 
+#include "api_check.h"
 #include "kernels.h"
 #include "dev_scratch.h"
 #include "mcs_common.cuh"
@@ -19,145 +20,103 @@ using namespace mcs;
 
 namespace {
 
-int mfail(int code, const std::string& msg);   // records the message for mcs_last_error() (mcs_api.cu)
+// a frame's keypoints on the device, sorted into the CSR grid of cMultiFrame
+struct FrameGrid {
+    Dev keys, key_cam, cams, cell, cursor;                      // inputs and scratch of launch_frame_prepare
+    Dev kx, ky, koct, cell_start, cell_items, winv, hinv;
+};
 
-#define MCK(expr)                                                                                      \
-    do {                                                                                               \
-        cudaError_t e__ = (expr);                                                                      \
-        if (e__ != cudaSuccess) {                                                                      \
-            cudaGetLastError();                                                                        \
-            return mfail(e__ == cudaErrorNoDevice || e__ == cudaErrorInsufficientDriver ? MCS_ERR_NO_DEVICE : MCS_ERR_CUDA, \
-                         std::string(#expr) + ": " + cudaGetErrorString(e__));                         \
-        }                                                                                              \
-    } while (0)
-
-
-inline int cv_round(double v) { return (int)lrint(v); }
+// Uploads the keypoints, their cameras and the camera records, and enqueues the grid build on `st`: SoA copies of the keypoints,
+// the grid cell of every keypoint, the CSR grid and, when `rays` is given, the keypoint bearing vectors.  The caller synchronises
+// `st` before it reads the results or `g` dies.
+int build_frame_grid(const mcs_keypoint* keys, const int* key_cam, int n, const mcs_ocam* cams, int nc, FrameGrid& g, Dev* rays,
+                     cudaStream_t st) {
+    for (int i = 0; i < n; ++i)
+        if (key_cam[i] < 0 || key_cam[i] >= nc) return mcs_fail(MCS_ERR_INVALID, "key_cam out of range");
+    const int ncell = nc * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
+    const size_t m = (size_t)std::max(n, 1);
+    CUDA_CHECK(g.keys.upload_async(keys, (size_t)n * sizeof(mcs_keypoint), st));
+    CUDA_CHECK(g.key_cam.upload_async(key_cam, (size_t)n * 4, st));
+    CUDA_CHECK(g.cams.upload_async(cams, nc * sizeof(mcs_ocam), st));
+    CUDA_CHECK(g.cell.alloc(m * 4)); CUDA_CHECK(g.cursor.alloc((size_t)ncell * 4));
+    CUDA_CHECK(g.kx.alloc(m * 4)); CUDA_CHECK(g.ky.alloc(m * 4)); CUDA_CHECK(g.koct.alloc(m * 4));
+    CUDA_CHECK(g.cell_start.alloc((size_t)(ncell + 1) * 4)); CUDA_CHECK(g.cell_items.alloc(m * 4));
+    CUDA_CHECK(g.winv.alloc(nc * 8)); CUDA_CHECK(g.hinv.alloc(nc * 8));
+    if (rays) CUDA_CHECK(rays->alloc(m * 24));
+    CUDA_CHECK(launch_frame_prepare(g.keys.as<mcs_keypoint>(), g.key_cam.as<int>(), n, g.cams.as<mcs_ocam>(), nc, g.kx.as<float>(),
+                                    g.ky.as<float>(), g.koct.as<int>(), rays ? rays->as<double>() : nullptr, g.cell.as<int>(),
+                                    g.cursor.as<int>(), g.cell_start.as<int>(), g.cell_items.as<int>(), g.winv.as<double>(),
+                                    g.hinv.as<double>(), st));
+    return MCS_OK;
+}
 
 // frame uploaded for window searches
 struct FrameDev {
-    Dev kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv, cam_first;
+    FrameGrid grid;
+    Dev desc, dmask, cam_first;
     WindowFrameDev view;
 };
 
 int upload_frame(const mcs_frame_view* f, FrameDev& d, cudaStream_t st) {
-    // keypoints go up as they are; SoA copies, grid cell of every keypoint and the CSR grid are built on the device
+    // keypoints go up as they are; the window searches need only the image size of each camera
     const int n = f->n_keys, nc = f->n_cams;
-    for (int i = 0; i < n; ++i)
-        if (f->key_cam[i] < 0 || f->key_cam[i] >= nc) return mfail(MCS_ERR_INVALID, "key_cam out of range");
     std::vector<mcs_ocam> cams(nc);
     std::memset(cams.data(), 0, sizeof(mcs_ocam) * nc);
     for (int c = 0; c < nc; ++c) { cams[c].width = f->cam_width[c]; cams[c].height = f->cam_height[c]; }
-    const int ncell = nc * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
+    const int rc = build_frame_grid(f->keys, f->key_cam, n, cams.data(), nc, d.grid, nullptr, st);
+    if (rc) return rc;
     const size_t db = (size_t)n * f->dim;
-    Dev dkeys, dkc, dcams, dcell, dcur;
-    MCK(dkeys.alloc((size_t)n * sizeof(mcs_keypoint))); MCK(dkc.alloc((size_t)n * 4)); MCK(dcams.alloc(nc * sizeof(mcs_ocam)));
-    MCK(dcell.alloc((size_t)n * 4)); MCK(dcur.alloc((size_t)ncell * 4));
-    MCK(d.kx.alloc(n * 4)); MCK(d.ky.alloc(n * 4)); MCK(d.koct.alloc(n * 4)); MCK(d.desc.alloc(db));
-    MCK(d.cell_start.alloc((ncell + 1) * 4)); MCK(d.cell_items.alloc((size_t)std::max(n, 1) * 4));
-    MCK(d.winv.alloc(nc * 8)); MCK(d.hinv.alloc(nc * 8));
-    MCK(cudaMemcpyAsync(dkeys.p, f->keys, (size_t)n * sizeof(mcs_keypoint), cudaMemcpyHostToDevice, st));
-    MCK(cudaMemcpyAsync(dkc.p, f->key_cam, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-    MCK(cudaMemcpyAsync(dcams.p, cams.data(), nc * sizeof(mcs_ocam), cudaMemcpyHostToDevice, st));
-    MCK(cudaMemcpyAsync(d.desc.p, f->desc, db, cudaMemcpyHostToDevice, st));
-    if (f->dmask) {
-        MCK(d.dmask.alloc(db));
-        MCK(cudaMemcpyAsync(d.dmask.p, f->dmask, db, cudaMemcpyHostToDevice, st));
-    }
-    MCK(launch_frame_prepare(dkeys.as<mcs_keypoint>(), dkc.as<int>(), n, dcams.as<mcs_ocam>(), nc, d.kx.as<float>(), d.ky.as<float>(),
-                             d.koct.as<int>(), nullptr, dcell.as<int>(), dcur.as<int>(), d.cell_start.as<int>(), d.cell_items.as<int>(),
-                             d.winv.as<double>(), d.hinv.as<double>(), st));
-    MCK(cudaStreamSynchronize(st));    // host staging vectors and the scratch buffers die with this scope
-    d.view = WindowFrameDev{nc, n, f->dim, d.kx.as<float>(), d.ky.as<float>(), d.koct.as<int>(), d.desc.as<uint8_t>(),
-                            f->dmask ? d.dmask.as<uint8_t>() : nullptr, d.cell_start.as<int>(), d.cell_items.as<int>(),
-                            d.winv.as<double>(), d.hinv.as<double>()};
+    CUDA_CHECK(d.desc.upload_async(f->desc, db, st));
+    if (f->dmask) CUDA_CHECK(d.dmask.upload_async(f->dmask, db, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));    // `cams` is a host temporary
+    FrameGrid& g = d.grid;
+    d.view = WindowFrameDev{nc, n, f->dim, g.kx.as<float>(), g.ky.as<float>(), g.koct.as<int>(), d.desc.as<uint8_t>(),
+                            f->dmask ? d.dmask.as<uint8_t>() : nullptr, g.cell_start.as<int>(), g.cell_items.as<int>(),
+                            g.winv.as<double>(), g.hinv.as<double>()};
     return MCS_OK;
 }
 
-// run the window-search kernel for host-side queries; grows max_cand until nothing overflows
-int window_search_host(const FrameDev& fd, const std::vector<mcs_window_query>& qs, const uint8_t* qdesc, const uint8_t* qmask,
-                       size_t qdesc_rows, int dim, std::vector<int>& cidx, std::vector<int>& cdist, std::vector<int>& ccount,
-                       int& max_cand, bool allow_grow, cudaStream_t st) {
-    const int nq = (int)qs.size();
-    ccount.assign(nq, 0);
-    if (nq == 0) return MCS_OK;
-    Dev dq, dqd, dqm;
-    MCK(dq.alloc(sizeof(mcs_window_query) * nq));
-    MCK(dqd.alloc(qdesc_rows * dim));
-    MCK(cudaMemcpyAsync(dq.p, qs.data(), sizeof(mcs_window_query) * nq, cudaMemcpyHostToDevice, st));
-    MCK(cudaMemcpyAsync(dqd.p, qdesc, qdesc_rows * dim, cudaMemcpyHostToDevice, st));
-    const bool masked = qmask && fd.view.dmask;
-    if (masked) {
-        MCK(dqm.alloc(qdesc_rows * dim));
-        MCK(cudaMemcpyAsync(dqm.p, qmask, qdesc_rows * dim, cudaMemcpyHostToDevice, st));
-    }
-    for (;;) {
-        Dev di, dd, dc;
-        MCK(di.alloc((size_t)nq * max_cand * 4)); MCK(dd.alloc((size_t)nq * max_cand * 4)); MCK(dc.alloc((size_t)nq * 4));
-        MCK(cudaMemsetAsync(di.p, 0xFF, (size_t)nq * max_cand * 4, st));      // unused list entries read back as -1
-        MCK(cudaMemsetAsync(dd.p, 0, (size_t)nq * max_cand * 4, st));
-        MCK(launch_window_search(fd.view, dq.as<mcs_window_query>(), nq, dqd.as<uint8_t>(), masked ? dqm.as<uint8_t>() : nullptr,
-                                 max_cand, di.as<int>(), dd.as<int>(), dc.as<int>(), st));
-        cidx.resize((size_t)nq * max_cand); cdist.resize((size_t)nq * max_cand);
-        MCK(cudaMemcpyAsync(ccount.data(), dc.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-        MCK(cudaMemcpyAsync(cidx.data(), di.p, (size_t)nq * max_cand * 4, cudaMemcpyDeviceToHost, st));
-        MCK(cudaMemcpyAsync(cdist.data(), dd.p, (size_t)nq * max_cand * 4, cudaMemcpyDeviceToHost, st));
-        MCK(cudaStreamSynchronize(st));
-        const int mx = *std::max_element(ccount.begin(), ccount.end());
-        if (mx <= max_cand) return MCS_OK;
-        if (!allow_grow) return MCS_ERR_CAPACITY;
-        max_cand = (mx + 31) & ~31;
-    }
-}
-
-// The same search with the candidates returned as ONE dense array in query order: candidates of query q are
-// cidx / cdist [coff[q] .. coff[q + 1]).  Only the counts and the candidates that exist cross PCIe.
+// Runs the window-search kernel for host-side queries and returns the candidates as ONE dense array in query order: candidates
+// of query q are cidx / cdist [coff[q] .. coff[q + 1]), in the kernel's visiting order.  Only the counts and the candidates that
+// exist cross PCIe.  The first pass keeps max_cand candidates per query; a longer list runs the search once more.
 int window_search_compact(const FrameDev& fd, const mcs_window_query* qs, const int nq, const uint8_t* qdesc, const uint8_t* qmask,
-                          size_t qdesc_rows, int dim, std::vector<int>& cidx, std::vector<int>& cdist, std::vector<int>& coff, cudaStream_t st) {
+                          size_t qdesc_rows, int dim, int max_cand, std::vector<int>& cidx, std::vector<int>& cdist, std::vector<int>& coff,
+                          cudaStream_t st) {
     coff.assign(nq + 1, 0);
     cidx.clear(); cdist.clear();
     if (nq == 0) return MCS_OK;
     Dev dq, dqd, dqm, dc, doff;
-    MCK(dq.alloc(sizeof(mcs_window_query) * nq));
-    MCK(dqd.alloc(qdesc_rows * dim));
-    MCK(dc.alloc((size_t)nq * 4)); MCK(doff.alloc((size_t)nq * 4));
-    MCK(cudaMemcpyAsync(dq.p, qs, sizeof(mcs_window_query) * nq, cudaMemcpyHostToDevice, st));
-    MCK(cudaMemcpyAsync(dqd.p, qdesc, qdesc_rows * dim, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(dq.upload_async(qs, sizeof(mcs_window_query) * nq, st));
+    CUDA_CHECK(dqd.upload_async(qdesc, qdesc_rows * dim, st));
+    CUDA_CHECK(dc.alloc((size_t)nq * 4)); CUDA_CHECK(doff.alloc((size_t)nq * 4));
     const bool masked = qmask && fd.view.dmask;
-    if (masked) {
-        MCK(dqm.alloc(qdesc_rows * dim));
-        MCK(cudaMemcpyAsync(dqm.p, qmask, qdesc_rows * dim, cudaMemcpyHostToDevice, st));
-    }
+    if (masked) CUDA_CHECK(dqm.upload_async(qmask, qdesc_rows * dim, st));
     std::vector<int> count(nq);
-    int max_cand = 32;
     for (;;) {
         Dev di, dd;
-        MCK(di.alloc((size_t)nq * max_cand * 4)); MCK(dd.alloc((size_t)nq * max_cand * 4));
-        MCK(launch_window_search(fd.view, dq.as<mcs_window_query>(), nq, dqd.as<uint8_t>(), masked ? dqm.as<uint8_t>() : nullptr,
-                                 max_cand, di.as<int>(), dd.as<int>(), dc.as<int>(), st));
-        MCK(cudaMemcpyAsync(count.data(), dc.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-        MCK(cudaStreamSynchronize(st));
+        CUDA_CHECK(di.alloc((size_t)nq * max_cand * 4)); CUDA_CHECK(dd.alloc((size_t)nq * max_cand * 4));
+        CUDA_CHECK(launch_window_search(fd.view, dq.as<mcs_window_query>(), nq, dqd.as<uint8_t>(), masked ? dqm.as<uint8_t>() : nullptr,
+                                        max_cand, di.as<int>(), dd.as<int>(), dc.as<int>(), st));
+        CUDA_CHECK(cudaMemcpyAsync(count.data(), dc.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
         const int mx = *std::max_element(count.begin(), count.end());
         if (mx > max_cand) { max_cand = (mx + 31) & ~31; continue; }        // a list overflowed: once more with room for the longest
         for (int q = 0; q < nq; ++q) coff[q + 1] = coff[q] + count[q];
         const int total = coff[nq];
         if (total == 0) return MCS_OK;
         Dev doi, dod;
-        MCK(doi.alloc((size_t)total * 4)); MCK(dod.alloc((size_t)total * 4));
-        MCK(cudaMemcpyAsync(doff.p, coff.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st));
-        MCK(launch_compact_lists(di.as<int>(), dd.as<int>(), dc.as<int>(), doff.as<int>(), nq, max_cand, doi.as<int>(), dod.as<int>(), st));
+        CUDA_CHECK(doi.alloc((size_t)total * 4)); CUDA_CHECK(dod.alloc((size_t)total * 4));
+        CUDA_CHECK(cudaMemcpyAsync(doff.p, coff.data(), (size_t)nq * 4, cudaMemcpyHostToDevice, st));
+        CUDA_CHECK(launch_compact_lists(di.as<int>(), dd.as<int>(), dc.as<int>(), doff.as<int>(), nq, max_cand, doi.as<int>(), dod.as<int>(), st));
         cidx.resize(total); cdist.resize(total);
-        MCK(cudaMemcpyAsync(cidx.data(), doi.p, (size_t)total * 4, cudaMemcpyDeviceToHost, st));
-        MCK(cudaMemcpyAsync(cdist.data(), dod.p, (size_t)total * 4, cudaMemcpyDeviceToHost, st));
-        MCK(cudaStreamSynchronize(st));
+        CUDA_CHECK(cudaMemcpyAsync(cidx.data(), doi.p, (size_t)total * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaMemcpyAsync(cdist.data(), dod.p, (size_t)total * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_CHECK(cudaStreamSynchronize(st));
         return MCS_OK;
     }
 }
 
 }  // namespace
-
-void mcs_set_error_(const std::string& msg);   // mcs_api.cu
-namespace { int mfail(int code, const std::string& msg) { mcs_set_error_(msg); return code; } }
 
 extern "C" {
 
@@ -181,37 +140,31 @@ int mcs_descriptor_distance64_masked(const uint64_t* a, const uint64_t* b, const
 int mcs_hamming_topk_device(const uint8_t* q_dev, const uint8_t* qmask_dev, int32_t nq, const uint8_t* d_dev,
                             const uint8_t* dmask_dev, int32_t nd, const uint8_t* db_skip_dev, int32_t dim, int32_t K,
                             int32_t* topk_idx_dev, int32_t* topk_dist_dev, void* stream) {
-    if (!q_dev || !d_dev || !topk_idx_dev || !topk_dist_dev) return mfail(MCS_ERR_INVALID, "null argument");
-    if (nq < 0 || nd < 0 || K < 1 || K > 8) return mfail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
-    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
-    if (nd >= (1 << 21)) return mfail(MCS_ERR_UNSUPPORTED, "more than 2^21 - 1 database descriptors in one call (split the database)");
-    MCK(launch_hamming_topk(q_dev, qmask_dev, nq, d_dev, dmask_dev, nd, db_skip_dev, dim, K, 0xFFFFFFFFu, topk_idx_dev, topk_dist_dev,
-                            (cudaStream_t)stream));
+    if (!q_dev || !d_dev || !topk_idx_dev || !topk_dist_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (nq < 0 || nd < 0 || K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
+    if (int rc = check_desc_dim(dim)) return rc;
+    if (nd >= (1 << 21)) return mcs_fail(MCS_ERR_UNSUPPORTED, "more than 2^21 - 1 database descriptors in one call (split the database)");
+    CUDA_CHECK(launch_hamming_topk(q_dev, qmask_dev, nq, d_dev, dmask_dev, nd, db_skip_dev, dim, K, 0xFFFFFFFFu, topk_idx_dev, topk_dist_dev,
+                                   (cudaStream_t)stream));
     return MCS_OK;
 }
 
 int mcs_hamming_topk(const uint8_t* q, const uint8_t* qmask, int32_t nq, const uint8_t* d, const uint8_t* dmask, int32_t nd,
                      const uint8_t* db_skip, int32_t dim, int32_t K, int32_t* topk_idx, int32_t* topk_dist) {
-    if (!q || !d || !topk_idx || !topk_dist) return mfail(MCS_ERR_INVALID, "null argument");
+    if (!q || !d || !topk_idx || !topk_dist) return mcs_fail(MCS_ERR_INVALID, "null argument");
     if (nq <= 0) return MCS_OK;
     const bool masked = qmask && dmask;
     Dev dq, dqm, dd, ddm, ds, di, dt;
-    MCK(dq.alloc((size_t)nq * dim)); MCK(dd.alloc((size_t)nd * dim));
-    MCK(di.alloc((size_t)nq * K * 4)); MCK(dt.alloc((size_t)nq * K * 4));
-    MCK(cudaMemcpy(dq.p, q, (size_t)nq * dim, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dd.p, d, (size_t)nd * dim, cudaMemcpyHostToDevice));
-    if (masked) {
-        MCK(dqm.alloc((size_t)nq * dim)); MCK(ddm.alloc((size_t)nd * dim));
-        MCK(cudaMemcpy(dqm.p, qmask, (size_t)nq * dim, cudaMemcpyHostToDevice));
-        MCK(cudaMemcpy(ddm.p, dmask, (size_t)nd * dim, cudaMemcpyHostToDevice));
-    }
-    if (db_skip) { MCK(ds.alloc(nd)); MCK(cudaMemcpy(ds.p, db_skip, nd, cudaMemcpyHostToDevice)); }
+    CUDA_CHECK(dq.upload(q, (size_t)nq * dim)); CUDA_CHECK(dd.upload(d, (size_t)nd * dim));
+    CUDA_CHECK(di.alloc((size_t)nq * K * 4)); CUDA_CHECK(dt.alloc((size_t)nq * K * 4));
+    if (masked) { CUDA_CHECK(dqm.upload(qmask, (size_t)nq * dim)); CUDA_CHECK(ddm.upload(dmask, (size_t)nd * dim)); }
+    if (db_skip) CUDA_CHECK(ds.upload(db_skip, nd));
     int rc = mcs_hamming_topk_device(dq.as<uint8_t>(), masked ? dqm.as<uint8_t>() : nullptr, nq, dd.as<uint8_t>(),
                                      masked ? ddm.as<uint8_t>() : nullptr, nd, db_skip ? ds.as<uint8_t>() : nullptr, dim, K,
                                      di.as<int>(), dt.as<int>(), nullptr);
     if (rc) return rc;
-    MCK(cudaMemcpy(topk_idx, di.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
-    MCK(cudaMemcpy(topk_dist, dt.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(topk_idx, di.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(topk_dist, dt.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
     return MCS_OK;
 }
 
@@ -238,41 +191,41 @@ static int bruteforce_core(const uint8_t* q_dev, const uint8_t* qm_dev, const ui
     // the acceptance kernel keeps one bit per database entry in shared memory (kernels.h: bruteforce_replay_smem): at most
     // 1 622 016 entries.  Checked here so that a larger database is refused before anything is launched.
     if (nd > bruteforce_max_nd(K))
-        return mfail(MCS_ERR_UNSUPPORTED, "more than " + std::to_string(bruteforce_max_nd(K)) + " database descriptors in one call");
-    Dev ds, di, dt, dv1, dseg, dm12, dnm;
-    MCK(ds.alloc(nd)); MCK(di.alloc((size_t)nq * K * 4)); MCK(dt.alloc((size_t)nq * K * 4));
-    MCK(dv1.alloc(nq)); MCK(dseg.alloc((size_t)(n_seg + 1) * 4)); MCK(dm12.alloc((size_t)nq * 4)); MCK(dnm.alloc((size_t)n_seg * 4));
+        return mcs_fail(MCS_ERR_UNSUPPORTED, "more than " + std::to_string(bruteforce_max_nd(K)) + " database descriptors in one call");
     std::vector<uint8_t> skip(nd, 0);
     if (valid2) for (int i = 0; i < nd; ++i) skip[i] = valid2[i] ? 0 : 1;
     g_bf_rounds = 1;
-    MCK(cudaMemcpyAsync(ds.p, skip.data(), nd, cudaMemcpyHostToDevice, st));
-    if (valid1) MCK(cudaMemcpyAsync(dv1.p, valid1, nq, cudaMemcpyHostToDevice, st));
-    MCK(cudaMemcpyAsync(dseg.p, seg, (size_t)(n_seg + 1) * 4, cudaMemcpyHostToDevice, st));
+    Dev ds, di, dt, dv1, dseg, dm12, dnm;
+    CUDA_CHECK(ds.upload_async(skip.data(), nd, st));
+    CUDA_CHECK(di.alloc((size_t)nq * K * 4)); CUDA_CHECK(dt.alloc((size_t)nq * K * 4)); CUDA_CHECK(dv1.alloc(nq));
+    if (valid1) CUDA_CHECK(cudaMemcpyAsync(dv1.p, valid1, nq, cudaMemcpyHostToDevice, st));
+    CUDA_CHECK(dseg.upload_async(seg, (size_t)(n_seg + 1) * 4, st));
+    CUDA_CHECK(dm12.alloc((size_t)nq * 4)); CUDA_CHECK(dnm.alloc((size_t)n_seg * 4));
     // Entries at or beyond the relevance bound of (th_low, nnratio) stay out of the lists: a list shorter than K then means "every
     // entry that can influence the decision is here".
-    MCK(launch_hamming_topk(q_dev, masked ? qm_dev : nullptr, nq, d_dev, masked ? dm_dev : nullptr, nd, ds.as<uint8_t>(), dim, K,
-                            greedy_dist_bound(th_low, nnratio), di.as<int>(), dt.as<int>(), st));
+    CUDA_CHECK(launch_hamming_topk(q_dev, masked ? qm_dev : nullptr, nq, d_dev, masked ? dm_dev : nullptr, nd, ds.as<uint8_t>(), dim, K,
+                                   greedy_dist_bound(th_low, nnratio), di.as<int>(), dt.as<int>(), st));
     // the replay kernel wants "valid" bytes for the database (1 = usable): reuse the skip buffer inverted on the fly is not worth a
     // kernel -- upload the caller's array when there is one
     Dev dv2;
-    if (valid2) { MCK(dv2.alloc(nd)); MCK(cudaMemcpyAsync(dv2.p, valid2, nd, cudaMemcpyHostToDevice, st)); }
-    MCK(launch_bruteforce_replay(di.as<int>(), dt.as<int>(), K, q_dev, masked ? qm_dev : nullptr, valid1 ? dv1.as<uint8_t>() : nullptr,
-                                 dseg.as<int>(), n_seg, nq, d_dev, masked ? dm_dev : nullptr, valid2 ? dv2.as<uint8_t>() : nullptr, nd, dim, th_low,
-                                 nnratio, dm12.as<int>(), dnm.as<int>(), st));
-    MCK(cudaMemcpyAsync(matches12, dm12.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
-    MCK(cudaMemcpyAsync(nmatches, dnm.p, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, st));
-    MCK(cudaStreamSynchronize(st));
+    if (valid2) CUDA_CHECK(dv2.upload_async(valid2, nd, st));
+    CUDA_CHECK(launch_bruteforce_replay(di.as<int>(), dt.as<int>(), K, q_dev, masked ? qm_dev : nullptr, valid1 ? dv1.as<uint8_t>() : nullptr,
+                                        dseg.as<int>(), n_seg, nq, d_dev, masked ? dm_dev : nullptr, valid2 ? dv2.as<uint8_t>() : nullptr, nd, dim, th_low,
+                                        nnratio, dm12.as<int>(), dnm.as<int>(), st));
+    CUDA_CHECK(cudaMemcpyAsync(matches12, dm12.p, (size_t)nq * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(nmatches, dnm.p, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
     return MCS_OK;
 }
 
 int mcs_match_bruteforce_batch_device(const uint8_t* q_dev, const uint8_t* qmask_dev, const uint8_t* valid1, const int32_t* seg_start,
                                       int32_t n_seg, const uint8_t* d_dev, const uint8_t* dmask_dev, const uint8_t* valid2, int32_t nd,
                                       int32_t dim, int32_t th_low, double nnratio, int32_t* matches12, int32_t* nmatches, void* stream) {
-    if (!q_dev || !d_dev || !matches12 || !nmatches || !seg_start) return mfail(MCS_ERR_INVALID, "null argument");
-    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
-    if (n_seg < 1 || seg_start[0] != 0) return mfail(MCS_ERR_INVALID, "seg_start must begin at 0 and hold n_seg + 1 offsets");
+    if (!q_dev || !d_dev || !matches12 || !nmatches || !seg_start) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_desc_dim(dim)) return rc;
+    if (n_seg < 1 || seg_start[0] != 0) return mcs_fail(MCS_ERR_INVALID, "seg_start must begin at 0 and hold n_seg + 1 offsets");
     for (int s = 0; s < n_seg; ++s)
-        if (seg_start[s + 1] < seg_start[s]) return mfail(MCS_ERR_INVALID, "seg_start must be non-decreasing");
+        if (seg_start[s + 1] < seg_start[s]) return mcs_fail(MCS_ERR_INVALID, "seg_start must be non-decreasing");
     const int nq = seg_start[n_seg];
     for (int s = 0; s < n_seg; ++s) nmatches[s] = 0;
     for (int i = 0; i < nq; ++i) matches12[i] = -1;
@@ -284,8 +237,8 @@ int mcs_match_bruteforce_batch_device(const uint8_t* q_dev, const uint8_t* qmask
 int mcs_match_bruteforce_device(const uint8_t* q_dev, const uint8_t* qmask_dev, const uint8_t* valid1, int32_t nq, const uint8_t* d_dev,
                                 const uint8_t* dmask_dev, const uint8_t* valid2, int32_t nd, int32_t dim, int32_t th_low, double nnratio,
                                 int32_t* matches12, int32_t* nmatches, void* stream) {
-    if (!q_dev || !d_dev || !matches12 || !nmatches) return mfail(MCS_ERR_INVALID, "null argument");
-    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    if (!q_dev || !d_dev || !matches12 || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_desc_dim(dim)) return rc;
     *nmatches = 0;
     for (int i = 0; i < nq; ++i) matches12[i] = -1;
     if (nq <= 0 || nd <= 0) return MCS_OK;
@@ -296,21 +249,15 @@ int mcs_match_bruteforce_device(const uint8_t* q_dev, const uint8_t* qmask_dev, 
 int mcs_match_bruteforce(const uint8_t* q, const uint8_t* qmask, const uint8_t* valid1, int32_t nq, const uint8_t* d,
                          const uint8_t* dmask, const uint8_t* valid2, int32_t nd, int32_t dim, int32_t th_low, double nnratio,
                          int32_t* matches12, int32_t* nmatches) {
-    if (!q || !d || !matches12 || !nmatches) return mfail(MCS_ERR_INVALID, "null argument");
-    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    if (!q || !d || !matches12 || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_desc_dim(dim)) return rc;
     *nmatches = 0;
     for (int i = 0; i < nq; ++i) matches12[i] = -1;
     if (nq <= 0 || nd <= 0) return MCS_OK;
     const bool masked = qmask && dmask;
     Dev dq, dqm, dd, ddm;
-    MCK(dq.alloc((size_t)nq * dim)); MCK(dd.alloc((size_t)nd * dim));
-    MCK(cudaMemcpy(dq.p, q, (size_t)nq * dim, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dd.p, d, (size_t)nd * dim, cudaMemcpyHostToDevice));
-    if (masked) {
-        MCK(dqm.alloc((size_t)nq * dim)); MCK(ddm.alloc((size_t)nd * dim));
-        MCK(cudaMemcpy(dqm.p, qmask, (size_t)nq * dim, cudaMemcpyHostToDevice));
-        MCK(cudaMemcpy(ddm.p, dmask, (size_t)nd * dim, cudaMemcpyHostToDevice));
-    }
+    CUDA_CHECK(dq.upload(q, (size_t)nq * dim)); CUDA_CHECK(dd.upload(d, (size_t)nd * dim));
+    if (masked) { CUDA_CHECK(dqm.upload(qmask, (size_t)nq * dim)); CUDA_CHECK(ddm.upload(dmask, (size_t)nd * dim)); }
     return bruteforce_core(dq.as<uint8_t>(), masked ? dqm.as<uint8_t>() : nullptr, valid1, nq, dd.as<uint8_t>(),
                            masked ? ddm.as<uint8_t>() : nullptr, valid2, nd, dim, th_low, nnratio, matches12, nmatches, nullptr);
 }
@@ -333,17 +280,16 @@ int mcs_search_for_triangulation(const uint8_t* desc1, const uint8_t* mask1, con
                                  const uint8_t* free2, const double* rays2, int32_t n2, int32_t dim, int32_t th_low, const double* E,
                                  int32_t n_cams, double epi_thresh, int32_t* matches12, int32_t* nmatches) {
     if (!desc1 || !cam1 || !free1 || !rays1 || !desc2 || !cam2 || !free2 || !rays2 || !E || !matches12 || !nmatches)
-        return mfail(MCS_ERR_INVALID, "null argument");
-    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_desc_dim(dim)) return rc;
     *nmatches = 0;
     for (int i = 0; i < n1; ++i) matches12[i] = -1;
     if (n1 <= 0 || n2 <= 0) return MCS_OK;
     const bool masked = mask1 && mask2;
     constexpr int K = 8;
     Dev dd, ddm, ds;
-    MCK(dd.alloc((size_t)n2 * dim)); MCK(ds.alloc(n2));
-    MCK(cudaMemcpy(dd.p, desc2, (size_t)n2 * dim, cudaMemcpyHostToDevice));
-    if (masked) { MCK(ddm.alloc((size_t)n2 * dim)); MCK(cudaMemcpy(ddm.p, mask2, (size_t)n2 * dim, cudaMemcpyHostToDevice)); }
+    CUDA_CHECK(dd.upload(desc2, (size_t)n2 * dim)); CUDA_CHECK(ds.alloc(n2));
+    if (masked) CUDA_CHECK(ddm.upload(mask2, (size_t)n2 * dim));
     std::vector<uint8_t> matched2(n2, 0), skip(n2);
     int nm = 0;
     for (int c = 0; c < n_cams; ++c) {                 // queries of camera c only ever see database entries of camera c (ref :1043-1045)
@@ -357,19 +303,18 @@ int mcs_search_for_triangulation(const uint8_t* desc1, const uint8_t* mask1, con
             if (masked) std::memcpy(&qmk[(size_t)k * dim], mask1 + (size_t)q_idx[k] * dim, dim);
         }
         Dev dq, dqm, di, dt;
-        MCK(dq.alloc((size_t)nq * dim)); MCK(di.alloc((size_t)nq * K * 4)); MCK(dt.alloc((size_t)nq * K * 4));
-        MCK(cudaMemcpy(dq.p, qd.data(), (size_t)nq * dim, cudaMemcpyHostToDevice));
-        if (masked) { MCK(dqm.alloc((size_t)nq * dim)); MCK(cudaMemcpy(dqm.p, qmk.data(), (size_t)nq * dim, cudaMemcpyHostToDevice)); }
+        CUDA_CHECK(dq.upload(qd.data(), (size_t)nq * dim)); CUDA_CHECK(di.alloc((size_t)nq * K * 4)); CUDA_CHECK(dt.alloc((size_t)nq * K * 4));
+        if (masked) CUDA_CHECK(dqm.upload(qmk.data(), (size_t)nq * dim));
         std::vector<int> tidx((size_t)nq * K), tdist((size_t)nq * K);
         const double* Ecc = E + ((size_t)c * n_cams + c) * 9;
         // one GPU pass: the K best database entries (distance, index) of every query under the skip state at the start
         for (int i = 0; i < n2; ++i) skip[i] = (matched2[i] || !free2[i] || cam2[i] != c) ? 1 : 0;
-        MCK(cudaMemcpy(ds.p, skip.data(), n2, cudaMemcpyHostToDevice));
+        CUDA_CHECK(cudaMemcpy(ds.p, skip.data(), n2, cudaMemcpyHostToDevice));
         int rc = mcs_hamming_topk_device(dq.as<uint8_t>(), masked ? dqm.as<uint8_t>() : nullptr, nq, dd.as<uint8_t>(),
                                          masked ? ddm.as<uint8_t>() : nullptr, n2, ds.as<uint8_t>(), dim, K, di.as<int>(), dt.as<int>(), nullptr);
         if (rc) return rc;
-        MCK(cudaMemcpy(tidx.data(), di.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
-        MCK(cudaMemcpy(tdist.data(), dt.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(tidx.data(), di.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
+        CUDA_CHECK(cudaMemcpy(tdist.data(), dt.p, (size_t)nq * K * 4, cudaMemcpyDeviceToHost));
         std::vector<int> pi(K), pd(K), marked;
         for (int k = 0; k < nq; ++k) {                   // sequential replay (ref :1015-1107)
             const double* r1 = rays1 + 3 * (size_t)q_idx[k];
@@ -393,13 +338,13 @@ int mcs_search_for_triangulation(const uint8_t* desc1, const uint8_t* mask1, con
                 std::vector<uint8_t> sk(n2);
                 while (!done) {
                     for (int i = 0; i < n2; ++i) sk[i] = (matched2[i] || !free2[i] || cam2[i] != c || skip[i] == 2) ? 1 : 0;
-                    MCK(cudaMemcpy(ds.p, sk.data(), n2, cudaMemcpyHostToDevice));
+                    CUDA_CHECK(cudaMemcpy(ds.p, sk.data(), n2, cudaMemcpyHostToDevice));
                     rc = mcs_hamming_topk_device(dq.as<uint8_t>() + (size_t)k * dim, masked ? dqm.as<uint8_t>() + (size_t)k * dim : nullptr, 1,
                                                  dd.as<uint8_t>(), masked ? ddm.as<uint8_t>() : nullptr, n2, ds.as<uint8_t>(), dim, K,
                                                  di.as<int>(), dt.as<int>(), nullptr);
                     if (rc) return rc;
-                    MCK(cudaMemcpy(pi.data(), di.p, K * 4, cudaMemcpyDeviceToHost));
-                    MCK(cudaMemcpy(pd.data(), dt.p, K * 4, cudaMemcpyDeviceToHost));
+                    CUDA_CHECK(cudaMemcpy(pi.data(), di.p, K * 4, cudaMemcpyDeviceToHost));
+                    CUDA_CHECK(cudaMemcpy(pd.data(), dt.p, K * 4, cudaMemcpyDeviceToHost));
                     if (!walk(pi.data(), pd.data())) break;
                 }
             }
@@ -415,51 +360,51 @@ int mcs_search_for_triangulation(const uint8_t* desc1, const uint8_t* mask1, con
 int mcs_window_search(const mcs_frame_view* frame, const mcs_window_query* queries, int32_t nq, const uint8_t* qdesc,
                       const uint8_t* qmask, int32_t max_cand, int32_t* cand_idx, int32_t* cand_dist, int32_t* cand_count) {
     if (!frame || !queries || !qdesc || !cand_idx || !cand_dist || !cand_count || max_cand < 1)
-        return mfail(MCS_ERR_INVALID, "null argument");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
     if (nq <= 0) return MCS_OK;
     FrameDev fd;
     int rc = upload_frame(frame, fd, nullptr);
     if (rc) return rc;
     int rows = 0;
     for (int i = 0; i < nq; ++i) {
-        if (queries[i].cam < 0 || queries[i].cam >= frame->n_cams) return mfail(MCS_ERR_INVALID, "query camera out of range");
-        if (queries[i].desc_index < 0) return mfail(MCS_ERR_INVALID, "negative query descriptor index");
+        if (queries[i].cam < 0 || queries[i].cam >= frame->n_cams) return mcs_fail(MCS_ERR_INVALID, "query camera out of range");
+        if (queries[i].desc_index < 0) return mcs_fail(MCS_ERR_INVALID, "negative query descriptor index");
         rows = std::max(rows, queries[i].desc_index + 1);
     }
-    std::vector<mcs_window_query> qs(queries, queries + nq);
-    std::vector<int> ci, cd, cc;
-    int mc = max_cand;
-    rc = window_search_host(fd, qs, qdesc, qmask, rows, frame->dim, ci, cd, cc, mc, false, nullptr);
-    if (rc != MCS_OK && rc != MCS_ERR_CAPACITY) return rc;
-    std::memcpy(cand_count, cc.data(), sizeof(int) * nq);
-    std::memcpy(cand_idx, ci.data(), sizeof(int) * (size_t)nq * max_cand);
-    std::memcpy(cand_dist, cd.data(), sizeof(int) * (size_t)nq * max_cand);
-    if (rc == MCS_ERR_CAPACITY) return mfail(MCS_ERR_CAPACITY, "max_cand too small for at least one query");
+    std::vector<int> ci, cd, co;
+    rc = window_search_compact(fd, queries, nq, qdesc, qmask, rows, frame->dim, max_cand, ci, cd, co, nullptr);
+    if (rc) return rc;
+    // the kernel stores a candidate at its visiting position, so the first max_cand of a longer list are what a list of
+    // max_cand slots would hold
+    bool overflow = false;
+    for (int q = 0; q < nq; ++q) {
+        const int count = co[q + 1] - co[q], n = std::min(count, max_cand);
+        int32_t* idx = cand_idx + (size_t)q * max_cand;
+        int32_t* dist = cand_dist + (size_t)q * max_cand;
+        std::copy(ci.begin() + co[q], ci.begin() + co[q] + n, idx);
+        std::copy(cd.begin() + co[q], cd.begin() + co[q] + n, dist);
+        std::fill(idx + n, idx + max_cand, -1);
+        std::fill(dist + n, dist + max_cand, 0);
+        cand_count[q] = count;
+        overflow |= count > max_cand;
+    }
+    if (overflow) return mcs_fail(MCS_ERR_CAPACITY, "max_cand too small for at least one query");
     return MCS_OK;
 }
 
 int mcs_frame_prepare(const mcs_keypoint* keys, const int32_t* key_cam, int32_t n_keys, const mcs_ocam* cams, int32_t n_cams,
                       double* rays_out, int32_t* cell_start_out, int32_t* cell_items_out, int32_t* n_in_grid) {
     if (!keys || !key_cam || !cams || !rays_out || !cell_start_out || !cell_items_out || !n_in_grid)
-        return mfail(MCS_ERR_INVALID, "null argument");
-    if (n_keys < 0 || n_cams < 1) return mfail(MCS_ERR_INVALID, "bad sizes");
-    for (int i = 0; i < n_keys; ++i)
-        if (key_cam[i] < 0 || key_cam[i] >= n_cams) return mfail(MCS_ERR_INVALID, "key_cam out of range");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_keys < 0 || n_cams < 1) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    FrameGrid g;
+    Dev rays;
+    const int rc = build_frame_grid(keys, key_cam, n_keys, cams, n_cams, g, &rays, nullptr);
+    if (rc) return rc;
     const int ncell = n_cams * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
-    Dev dkeys, dkc, dcams, dcell, dcur, dkx, dky, dko, drays, dstart, ditems, dw, dh;
-    const size_t n = (size_t)std::max(n_keys, 1);
-    MCK(dkeys.alloc(n * sizeof(mcs_keypoint))); MCK(dkc.alloc(n * 4)); MCK(dcams.alloc(n_cams * sizeof(mcs_ocam)));
-    MCK(dcell.alloc(n * 4)); MCK(dcur.alloc((size_t)ncell * 4)); MCK(dkx.alloc(n * 4)); MCK(dky.alloc(n * 4)); MCK(dko.alloc(n * 4));
-    MCK(drays.alloc(n * 24)); MCK(dstart.alloc((size_t)(ncell + 1) * 4)); MCK(ditems.alloc(n * 4)); MCK(dw.alloc(n_cams * 8)); MCK(dh.alloc(n_cams * 8));
-    MCK(cudaMemcpy(dkeys.p, keys, (size_t)n_keys * sizeof(mcs_keypoint), cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dkc.p, key_cam, (size_t)n_keys * 4, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dcams.p, cams, n_cams * sizeof(mcs_ocam), cudaMemcpyHostToDevice));
-    MCK(launch_frame_prepare(dkeys.as<mcs_keypoint>(), dkc.as<int>(), n_keys, dcams.as<mcs_ocam>(), n_cams, dkx.as<float>(), dky.as<float>(),
-                             dko.as<int>(), drays.as<double>(), dcell.as<int>(), dcur.as<int>(), dstart.as<int>(), ditems.as<int>(),
-                             dw.as<double>(), dh.as<double>(), nullptr));
-    MCK(cudaMemcpy(rays_out, drays.p, (size_t)n_keys * 24, cudaMemcpyDeviceToHost));
-    MCK(cudaMemcpy(cell_start_out, dstart.p, (size_t)(ncell + 1) * 4, cudaMemcpyDeviceToHost));
-    MCK(cudaMemcpy(cell_items_out, ditems.p, (size_t)n_keys * 4, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(rays_out, rays.p, (size_t)n_keys * 24, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(cell_start_out, g.cell_start.p, (size_t)(ncell + 1) * 4, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(cell_items_out, g.cell_items.p, (size_t)n_keys * 4, cudaMemcpyDeviceToHost));
     *n_in_grid = cell_start_out[ncell];
     return MCS_OK;
 }
@@ -470,53 +415,46 @@ int mcs_project_mappoints(int32_t n_cams, const double* mtmc_inv, const double* 
                           double* proj_x, double* proj_y, double* view_cos) {
     if (!mtmc_inv || !mtmc || !cams || !masks || !world_pos || !normal || !min_dist || !max_dist || !scale_factors || !in_view ||
         !level || !proj_x || !proj_y || !view_cos)
-        return mfail(MCS_ERR_INVALID, "null argument");
-    if (n_cams < 1 || n_points < 0 || n_levels < 1) return mfail(MCS_ERR_INVALID, "bad sizes");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_cams < 1 || n_points < 0 || n_levels < 1) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     if (n_points == 0) return MCS_OK;
     size_t mask_bytes = 0;
     for (int c = 0; c < n_cams; ++c) {
         if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
-            return mfail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
+            return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
         mask_bytes += (size_t)cams[c].width * cams[c].height;
     }
     const size_t n = (size_t)n_points * n_cams;
     Dev dmi, dm, dc, dk, dp, dn, dmn, dmx, dsf, div, dlv, dpx, dpy, dvc;
-    MCK(dmi.alloc(n_cams * 128)); MCK(dm.alloc(n_cams * 128)); MCK(dc.alloc(n_cams * sizeof(mcs_ocam))); MCK(dk.alloc(mask_bytes));
-    MCK(dp.alloc((size_t)n_points * 24)); MCK(dn.alloc((size_t)n_points * 24)); MCK(dmn.alloc((size_t)n_points * 8));
-    MCK(dmx.alloc((size_t)n_points * 8)); MCK(dsf.alloc(n_levels * 8));
-    MCK(div.alloc(n)); MCK(dlv.alloc(n * 4)); MCK(dpx.alloc(n * 8)); MCK(dpy.alloc(n * 8)); MCK(dvc.alloc(n * 8));
-    MCK(cudaMemcpy(dmi.p, mtmc_inv, n_cams * 128, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dm.p, mtmc, n_cams * 128, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dc.p, cams, n_cams * sizeof(mcs_ocam), cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dk.p, masks, mask_bytes, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dp.p, world_pos, (size_t)n_points * 24, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dn.p, normal, (size_t)n_points * 24, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dmn.p, min_dist, (size_t)n_points * 8, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dmx.p, max_dist, (size_t)n_points * 8, cudaMemcpyHostToDevice));
-    MCK(cudaMemcpy(dsf.p, scale_factors, n_levels * 8, cudaMemcpyHostToDevice));
-    MCK(launch_frustum(n_cams, dmi.as<double>(), dm.as<double>(), dc.as<mcs_ocam>(), dk.as<uint8_t>(), n_points, dp.as<double>(),
-                       dn.as<double>(), dmn.as<double>(), dmx.as<double>(), dsf.as<double>(), n_levels, div.as<uint8_t>(),
-                       dlv.as<int>(), dpx.as<double>(), dpy.as<double>(), dvc.as<double>(), nullptr, nullptr));
-    MCK(cudaMemcpy(in_view, div.p, n, cudaMemcpyDeviceToHost));
-    MCK(cudaMemcpy(level, dlv.p, n * 4, cudaMemcpyDeviceToHost));
-    MCK(cudaMemcpy(proj_x, dpx.p, n * 8, cudaMemcpyDeviceToHost));
-    MCK(cudaMemcpy(proj_y, dpy.p, n * 8, cudaMemcpyDeviceToHost));
-    MCK(cudaMemcpy(view_cos, dvc.p, n * 8, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(dmi.upload(mtmc_inv, n_cams * 128)); CUDA_CHECK(dm.upload(mtmc, n_cams * 128));
+    CUDA_CHECK(dc.upload(cams, n_cams * sizeof(mcs_ocam))); CUDA_CHECK(dk.upload(masks, mask_bytes));
+    CUDA_CHECK(dp.upload(world_pos, (size_t)n_points * 24)); CUDA_CHECK(dn.upload(normal, (size_t)n_points * 24));
+    CUDA_CHECK(dmn.upload(min_dist, (size_t)n_points * 8)); CUDA_CHECK(dmx.upload(max_dist, (size_t)n_points * 8));
+    CUDA_CHECK(dsf.upload(scale_factors, n_levels * 8));
+    CUDA_CHECK(div.alloc(n)); CUDA_CHECK(dlv.alloc(n * 4)); CUDA_CHECK(dpx.alloc(n * 8)); CUDA_CHECK(dpy.alloc(n * 8)); CUDA_CHECK(dvc.alloc(n * 8));
+    CUDA_CHECK(launch_frustum(n_cams, dmi.as<double>(), dm.as<double>(), dc.as<mcs_ocam>(), dk.as<uint8_t>(), n_points, dp.as<double>(),
+                              dn.as<double>(), dmn.as<double>(), dmx.as<double>(), dsf.as<double>(), n_levels, div.as<uint8_t>(),
+                              dlv.as<int>(), dpx.as<double>(), dpy.as<double>(), dvc.as<double>(), nullptr, nullptr));
+    CUDA_CHECK(cudaMemcpy(in_view, div.p, n, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(level, dlv.p, n * 4, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(proj_x, dpx.p, n * 8, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(proj_y, dpy.p, n * 8, cudaMemcpyDeviceToHost));
+    CUDA_CHECK(cudaMemcpy(view_cos, dvc.p, n * 8, cudaMemcpyDeviceToHost));
     return MCS_OK;
 }
 
 int mcs_search_windows(const mcs_frame_view* f, const mcs_window_query* queries, int32_t nq, const uint8_t* qdesc,
                        const uint8_t* qmask, const int32_t* query_tag, int32_t rule, double nnratio, int32_t threshold,
                        int32_t* assigned, int32_t* nmatches) {
-    if (!f || !queries || !qdesc || !query_tag || !assigned || !nmatches) return mfail(MCS_ERR_INVALID, "null argument");
-    if (rule < 0 || rule > MCS_RULE_SCW) return mfail(MCS_ERR_INVALID, "unknown rule");
+    if (!f || !queries || !qdesc || !query_tag || !assigned || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (rule < 0 || rule > MCS_RULE_SCW) return mcs_fail(MCS_ERR_INVALID, "unknown rule");
     *nmatches = 0;
     if (nq <= 0) return MCS_OK;
     int rows = 0;
     for (int i = 0; i < nq; ++i) {
-        if (queries[i].cam < 0 || queries[i].cam >= f->n_cams) return mfail(MCS_ERR_INVALID, "query camera out of range");
-        if (query_tag[i] < 0) return mfail(MCS_ERR_INVALID, "query tags must be >= 0");
-        if (queries[i].desc_index < 0) return mfail(MCS_ERR_INVALID, "negative query descriptor index");
+        if (queries[i].cam < 0 || queries[i].cam >= f->n_cams) return mcs_fail(MCS_ERR_INVALID, "query camera out of range");
+        if (query_tag[i] < 0) return mcs_fail(MCS_ERR_INVALID, "query tags must be >= 0");
+        if (queries[i].desc_index < 0) return mcs_fail(MCS_ERR_INVALID, "negative query descriptor index");
         rows = std::max(rows, queries[i].desc_index + 1);
     }
     FrameDev fd;
@@ -527,16 +465,15 @@ int mcs_search_windows(const mcs_frame_view* f, const mcs_window_query* queries,
         // camera-major keypoint order of src/cMultiFrame.cpp:168-184
         std::vector<int> first(f->n_cams + 1, 0);
         for (int i = 0; i < f->n_keys; ++i) {
-            if (i && f->key_cam[i] < f->key_cam[i - 1]) return mfail(MCS_ERR_INVALID, "MCS_RULE_SCW needs camera-major keypoint order");
+            if (i && f->key_cam[i] < f->key_cam[i - 1]) return mcs_fail(MCS_ERR_INVALID, "MCS_RULE_SCW needs camera-major keypoint order");
             ++first[f->key_cam[i] + 1];
         }
         for (int c = 0; c < f->n_cams; ++c) first[c + 1] += first[c];
-        MCK(fd.cam_first.alloc(first.size() * 4));
-        MCK(cudaMemcpy(fd.cam_first.p, first.data(), first.size() * 4, cudaMemcpyHostToDevice));
+        CUDA_CHECK(fd.cam_first.upload(first.data(), first.size() * 4));
         fd.view.cam_first = fd.cam_first.as<int>();
     }
     std::vector<int> ci, cd, co;
-    rc = window_search_compact(fd, queries, nq, qdesc, qmask, rows, f->dim, ci, cd, co, nullptr);
+    rc = window_search_compact(fd, queries, nq, qdesc, qmask, rows, f->dim, 32, ci, cd, co, nullptr);
     if (rc) return rc;
     int nm = 0;
     for (int qi = 0; qi < nq; ++qi) {       // sequential greedy replay over the GPU-computed candidate lists
@@ -584,8 +521,8 @@ int mcs_search_windows(const mcs_frame_view* f, const mcs_window_query* queries,
 
 int mcs_search_by_projection(const mcs_frame_view* f, const mcs_mappoint_view* mps, double th, double nnratio, int32_t th_high,
                              int32_t having_masks, int32_t* frame_mp, int32_t* nmatches) {
-    if (!f || !mps || !frame_mp || !nmatches) return mfail(MCS_ERR_INVALID, "null argument");
-    if (having_masks && (!f->dmask || !mps->dmask)) return mfail(MCS_ERR_INVALID, "masks requested but not supplied");
+    if (!f || !mps || !frame_mp || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (having_masks && (!f->dmask || !mps->dmask)) return mcs_fail(MCS_ERR_INVALID, "masks requested but not supplied");
     *nmatches = 0;
     // queries in the reference's visiting order: map point outer, camera inner (ref :74-98)
     std::vector<mcs_window_query> qs;
@@ -603,7 +540,7 @@ int mcs_search_by_projection(const mcs_frame_view* f, const mcs_mappoint_view* m
             const size_t k = (size_t)i * f->n_cams + cam;
             if (!mps->in_view[k]) continue;
             const int lvl = mps->level[k];
-            if (lvl < 0 || lvl >= f->n_levels) return mfail(MCS_ERR_INVALID, "map point scale level out of range");
+            if (lvl < 0 || lvl >= f->n_levels) return mcs_fail(MCS_ERR_INVALID, "map point scale level out of range");
             double r = mps->view_cos[k] > 0.998 ? 2.5 : 4.0;   // RadiusByViewingCos (ref :169-175)
             if (bFactor) r *= th;
             mcs_window_query q;
@@ -627,13 +564,13 @@ int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const d
                                  void* stream) {
     if (!mtmc_inv || !mtmc || !cams || !masks_dev || !world_pos_dev || !normal_dev || !min_dist_dev || !max_dist_dev || !scale_factors ||
         !in_view_dev || !level_dev || !proj_x_dev || !proj_y_dev || !view_cos_dev)
-        return mfail(MCS_ERR_INVALID, "null argument");
-    if (n_cams < 1 || n_points < 0 || n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mfail(MCS_ERR_INVALID, "bad sizes");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_cams < 1 || n_points < 0 || n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     for (int c = 0; c < n_cams; ++c)
         if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
-            return mfail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
+            return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
     cudaStream_t st = (cudaStream_t)stream;
-    MCK(keep_pool_memory());
+    CUDA_CHECK(keep_pool_memory());
     if (n_points == 0) return MCS_OK;
     // poses, camera models and scale factors: one scratch block, staged in stream order
     const size_t b_pose = (size_t)n_cams * 128, b_cam = sizeof(mcs_ocam) * n_cams, b_sf = 8 * (size_t)n_levels;
@@ -643,16 +580,16 @@ int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const d
     std::memcpy(h.data() + 2 * b_pose, cams, b_cam);
     std::memcpy(h.data() + 2 * b_pose + b_cam, scale_factors, b_sf);
     uint8_t* d = nullptr;
-    MCK(cudaMallocAsync((void**)&d, h.size(), st));
+    CUDA_CHECK(cudaMallocAsync((void**)&d, h.size(), st));
     cudaError_t e = stage_to_device(h.data(), h.size(), d, st);
     if (e == cudaSuccess)
         e = launch_frustum(n_cams, (const double*)d, (const double*)(d + b_pose), (const mcs_ocam*)(d + 2 * b_pose), masks_dev, n_points,
                            world_pos_dev, normal_dev, min_dist_dev, max_dist_dev, (const double*)(d + 2 * b_pose + b_cam), n_levels, in_view_dev,
                            level_dev, proj_x_dev, proj_y_dev, view_cos_dev, skip_dev, st);
     const cudaError_t ef = cudaFreeAsync(d, st);
-    MCK(e);
-    MCK(ef);
-    if (!stream) MCK(cudaStreamSynchronize(st));
+    CUDA_CHECK(e);
+    CUDA_CHECK(ef);
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
     return MCS_OK;
 }
 
@@ -679,6 +616,18 @@ bool packed_frame_ok(const mcs_packed_frame* fr, int n_cams) {
     return fr->packed_dev && fr->n_parts >= 1 && fr->part_images >= 1 && fr->first_image >= 0 &&
            (long long)fr->first_image + n_cams <= (long long)fr->n_parts * fr->part_images;
 }
+
+// the arguments of the frame both device SearchByProjection calls search, and of the packed feature buffers the images of its
+// cameras come from (`last`: the motion-model search only)
+int check_packed_frames(int n_cams, int capacity, int dim, int n_levels, const mcs_packed_frame* cur, const mcs_packed_frame* last) {
+    if (n_cams < 1 || n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (capacity < 1 || capacity > 65535) return mcs_fail(MCS_ERR_INVALID, "capacity must be 1..65535");
+    if (int rc = check_desc_dim(dim)) return rc;
+    if (!packed_frame_ok(cur, n_cams)) return mcs_fail(MCS_ERR_INVALID, "current frame: no buffer, or first_image + n_cams exceeds its images");
+    if (last && !packed_frame_ok(last, n_cams))
+        return mcs_fail(MCS_ERR_INVALID, "last frame: no buffer, or first_image + n_cams exceeds its images");
+    return MCS_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -689,23 +638,20 @@ int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int
                                     int32_t having_masks, int32_t* frame_mp_dev, int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev,
                                     void* stream) {
     if (!packed_dev || !cam_width || !cam_height || !scale_factors || !mps || !frame_mp_dev || !nmatches_dev || !status_dev)
-        return mfail(MCS_ERR_INVALID, "null argument");
-    if (n_cams < 1 || n_parts < 1 || part_images < 1 || first_image < 0 || n_levels < 1 || n_levels > MCS_MAX_LEVELS || mps->n_points < 0)
-        return mfail(MCS_ERR_INVALID, "bad sizes");
-    if (capacity < 1 || capacity > 65535) return mfail(MCS_ERR_INVALID, "capacity must be 1..65535");
-    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
-    if ((long long)first_image + n_cams > (long long)n_parts * part_images)
-        return mfail(MCS_ERR_INVALID, "first_image + n_cams exceeds the images of the packed buffer");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    const mcs_packed_frame frame{packed_dev, n_parts, part_images, first_image};
+    if (int rc = check_packed_frames(n_cams, capacity, dim, n_levels, &frame, nullptr)) return rc;
+    if (mps->n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     if (!mps->in_view || !mps->level || !mps->proj_x || !mps->proj_y || !mps->view_cos || !mps->desc)
-        return mfail(MCS_ERR_INVALID, "null map-point array");
-    if (having_masks && !mps->dmask) return mfail(MCS_ERR_INVALID, "masks requested but not supplied");
+        return mcs_fail(MCS_ERR_INVALID, "null map-point array");
+    if (having_masks && !mps->dmask) return mcs_fail(MCS_ERR_INVALID, "masks requested but not supplied");
     for (int c = 0; c < n_cams; ++c)
-        if (cam_width[c] < 1 || cam_height[c] < 1) return mfail(MCS_ERR_INVALID, "camera sizes must be positive");
+        if (cam_width[c] < 1 || cam_height[c] < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
     if ((long long)mps->n_points * n_cams >= (1LL << 24))
-        return mfail(MCS_ERR_UNSUPPORTED, "more than 2^24 - 1 (map point, camera) entries in one call");
+        return mcs_fail(MCS_ERR_UNSUPPORTED, "more than 2^24 - 1 (map point, camera) entries in one call");
     cudaStream_t st = (cudaStream_t)stream;
-    MCK(keep_pool_memory());
-    const std::vector<PsCamSlots> slots = packed_slots(mcs_packed_frame{packed_dev, n_parts, part_images, first_image}, n_cams, capacity, dim);
+    CUDA_CHECK(keep_pool_memory());
+    const std::vector<PsCamSlots> slots = packed_slots(frame, n_cams, capacity, dim);
     ProjSearchArgs a{};
     a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.n_levels = n_levels; a.n_points = mps->n_points;
     a.cams = slots.data(); a.cam_w = cam_width; a.cam_h = cam_height; a.sf = scale_factors;
@@ -713,8 +659,8 @@ int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int
     a.mp_desc = mps->desc; a.mp_dmask = having_masks ? mps->dmask : nullptr;
     a.th = th; a.nnratio = nnratio; a.th_high = th_high; a.masked = having_masks != 0;
     a.frame_mp = frame_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
-    MCK(launch_search_by_projection(a, st));
-    if (!stream) MCK(cudaStreamSynchronize(st));
+    CUDA_CHECK(launch_search_by_projection(a, st));
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
     return MCS_OK;
 }
 
@@ -726,20 +672,17 @@ int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_
                                          int32_t* status_dev, int32_t* diag_dev, void* stream) {
     if (!cur || !last || !cams || !masks_dev || !scale_factors || !mtmc_inv || !last_mp_dev || !world_pos_dev || !cur_mp_dev ||
         !nmatches_dev || !status_dev)
-        return mfail(MCS_ERR_INVALID, "null argument");
-    if (n_cams < 1 || n_levels < 1 || n_levels > MCS_MAX_LEVELS || n_points < 0) return mfail(MCS_ERR_INVALID, "bad sizes");
-    if (capacity < 1 || capacity > 65535) return mfail(MCS_ERR_INVALID, "capacity must be 1..65535");
-    if (dim != 16 && dim != 32 && dim != 64) return mfail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
-    if (!packed_frame_ok(cur, n_cams)) return mfail(MCS_ERR_INVALID, "current frame: no buffer, or first_image + n_cams exceeds its images");
-    if (!packed_frame_ok(last, n_cams)) return mfail(MCS_ERR_INVALID, "last frame: no buffer, or first_image + n_cams exceeds its images");
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, n_levels, cur, last)) return rc;
+    if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     for (int c = 0; c < n_cams; ++c) {
-        if (cams[c].width < 1 || cams[c].height < 1) return mfail(MCS_ERR_INVALID, "camera sizes must be positive");
+        if (cams[c].width < 1 || cams[c].height < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
         if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
-            return mfail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
+            return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
     }
-    if ((long long)n_cams * capacity >= (1LL << 24)) return mfail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
     cudaStream_t st = (cudaStream_t)stream;
-    MCK(keep_pool_memory());
+    CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
     std::vector<int> cw(n_cams), ch(n_cams);
     for (int c = 0; c < n_cams; ++c) { cw[c] = cams[c].width; ch[c] = cams[c].height; }
@@ -751,16 +694,16 @@ int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_
     a.last = ls.data(); a.models = cams; a.mtmc_inv = mtmc_inv; a.masks = masks_dev;
     a.n_points = n_points; a.last_mp = last_mp_dev; a.last_outlier = last_outlier_dev; a.world_pos = world_pos_dev; a.bad = bad_dev;
     a.th = th;
-    MCK(launch_search_by_projection_last(a, st));
-    if (!stream) MCK(cudaStreamSynchronize(st));
+    CUDA_CHECK(launch_search_by_projection_last(a, st));
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
     return MCS_OK;
 }
 
 int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view* f2, double* prev_matched, int32_t window_size,
                                   double nnratio, int32_t th_low, int32_t having_masks, int32_t* matches12, int32_t* nmatches) {
-    if (!f1 || !f2 || !prev_matched || !matches12 || !nmatches) return mfail(MCS_ERR_INVALID, "null argument");
-    if (f1->dim != f2->dim) return mfail(MCS_ERR_INVALID, "descriptor sizes differ");
-    if (having_masks && (!f1->dmask || !f2->dmask)) return mfail(MCS_ERR_INVALID, "masks requested but not supplied");
+    if (!f1 || !f2 || !prev_matched || !matches12 || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (f1->dim != f2->dim) return mcs_fail(MCS_ERR_INVALID, "descriptor sizes differ");
+    if (having_masks && (!f1->dmask || !f2->dmask)) return mcs_fail(MCS_ERR_INVALID, "masks requested but not supplied");
     *nmatches = 0;
     const int n1 = f1->n_keys;
     for (int i = 0; i < n1; ++i) matches12[i] = -1;
@@ -769,7 +712,7 @@ int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view
     for (int i1 = 0; i1 < n1; ++i1) {
         mcs_window_query& q = qs[i1];
         q.cam = f1->key_cam[i1];
-        if (q.cam < 0 || q.cam >= f2->n_cams) return mfail(MCS_ERR_INVALID, "key_cam out of range");
+        if (q.cam < 0 || q.cam >= f2->n_cams) return mcs_fail(MCS_ERR_INVALID, "key_cam out of range");
         q.min_level = q.max_level = f1->keys[i1].octave;
         q.desc_index = i1;
         q.x = prev_matched[2 * i1]; q.y = prev_matched[2 * i1 + 1]; q.r = (double)window_size;
@@ -778,7 +721,7 @@ int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view
     int rc = upload_frame(f2, fd, nullptr);
     if (rc) return rc;
     std::vector<int> ci, cd, co;
-    rc = window_search_compact(fd, qs.data(), n1, f1->desc, having_masks ? f1->dmask : nullptr, n1, f1->dim, ci, cd, co, nullptr);
+    rc = window_search_compact(fd, qs.data(), n1, f1->desc, having_masks ? f1->dmask : nullptr, n1, f1->dim, 32, ci, cd, co, nullptr);
     if (rc) return rc;
     int nm = 0;
     std::vector<int> matchedDist(f2->n_keys, INT_MAX), matches21(f2->n_keys, -1);
