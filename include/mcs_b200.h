@@ -469,6 +469,43 @@ int  mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs
                                           const uint8_t* bad_dev, double th, int32_t th_high, int32_t having_masks, int32_t* cur_mp_dev,
                                           int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev, void* stream);
 
+/* TrackPreviousFrame's two searches (ref src/cTracking.cpp:724-788) with both frames in packed feature buffers and every output on
+ * the device, F1 = last, F2 = cur.  Same conventions as mcs_search_by_projection_last_device: asynchronous, host validation before
+ * any launch, both frames may share one buffer, last_mp_dev / cur_mp_dev [n_cams * capacity] slot-indexed map-point ids (-1 =
+ * none), slots at or beyond a camera's count neither read nor written in either frame, nmatches_dev / status_dev / diag_dev as
+ * there.  Acceptance is MCS_RULE_RATIO: the best candidate not yet assigned (strict < over the visiting order) is accepted when
+ * best <= second * nnratio (second = INT_MAX without one) and best <= th_high; cur_mp_dev receives the map-point id.  Neither call
+ * reads scale factors: -1 as an octave is "no level filter" and an octave >= the frame's levels finds no candidate, so octaves
+ * raise no status.
+ *
+ * mcs_window_search_device: WindowSearch(last, cur, window, ., min_level, max_level) (ref src/cORBmatcher.cpp:326-473).
+ *   cur_mp_dev is an output: every slot below a camera's count is first set to -1 (the reference starts from an all-NULL vector).
+ *   Each last-frame keypoint in contiguous order whose map point exists and is not bad, with min_level <= 0 or octave >=
+ *   min_level, and max_level == INT_MAX or octave <= max_level, searches GetFeaturesInArea(cam, x, y, window) of the same camera of
+ *   cur, all levels.  cam_width / cam_height [n_cams] host.  status_dev: MCS_ERR_INVALID when a map-point id is >= n_points (that
+ *   query is dropped).  n_cams * capacity < 2^24.
+ * mcs_search_by_projection_frames_device: SearchByProjection(last, cur, window, .) (ref :476-577).
+ *   cur_mp_dev is in/out and holds cur's map points on entry; the points it holds are "already found" and their keypoints are
+ *   taken.  A last-frame keypoint searches when its map point exists, is not bad, is not already found and the keypoint is the
+ *   first to carry it; the point is projected with WorldToCamHom_fast into EVERY camera c of the current pose (mtmc_inv [n_cams *
+ *   16] host, row-major MtMc_inv) and, inside c's mirror mask (masks_dev [n_cams][height][width]), searched in
+ *   GetFeaturesInArea(c, u, v, window, octave, octave).  Each camera's search may be accepted.  cams [n_cams] host, one image
+ *   size for all (MCS_ERR_UNSUPPORTED otherwise); world_pos_dev [n_points * 3], bad_dev [n_points] (may be NULL).
+ *   status_dev: MCS_ERR_INVALID when a last-frame map-point id is >= n_points (that keypoint is dropped); ids >= n_points in
+ *   cur_mp_dev mark their keypoint taken and find no point.  n_cams * n_cams * capacity < 2^24.
+ * capacity <= 65535; beyond the query bounds MCS_ERR_UNSUPPORTED. */
+int  mcs_window_search_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity, int32_t dim,
+                              const int32_t* cam_width, const int32_t* cam_height, const int32_t* last_mp_dev, int32_t n_points,
+                              const uint8_t* bad_dev, int32_t window, int32_t min_level, int32_t max_level, double nnratio,
+                              int32_t th_high, int32_t having_masks, int32_t* cur_mp_dev, int32_t* nmatches_dev, int32_t* status_dev,
+                              int32_t* diag_dev, void* stream);
+int  mcs_search_by_projection_frames_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity,
+                                            int32_t dim, const mcs_ocam* cams, const uint8_t* masks_dev, const double* mtmc_inv,
+                                            const int32_t* last_mp_dev, int32_t n_points, const double* world_pos_dev,
+                                            const uint8_t* bad_dev, int32_t window, double nnratio, int32_t th_high, int32_t having_masks,
+                                            int32_t* cur_mp_dev, int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev,
+                                            void* stream);
+
 /* Generic projection-window search: the shape shared by the remaining cORBmatcher searches (SURVEY 8a row M4).
  * Queries are visited in order; for each one the candidates of GetFeaturesInArea(cam, x, y, r, min_level, max_level)
  * that are not yet taken (assigned[idx] >= 0) are scanned in the reference's order, best / second best are tracked

@@ -763,6 +763,52 @@ class cORBmatcher:
                                                           _stream_handle(stream, dev)))
         return (out[0], out[1], cur_mp_t) + ((out[2],) if diag else ())
 
+    def WindowSearchDevice(self, cur, last, capacity, cam_sizes, last_mp_t, window, cur_mp_t, min_level=0, max_level=2**31 - 1, bad_t=None,
+                           stream=None, out=None, diag=False):
+        """mcs_window_search_device: WindowSearch(F1 = last, F2 = cur, window, ., min_level, max_level) (ref :326-473) with both
+        frames in packed feature buffers.  cur / last: (packed uint8 cuda tensor, n_parts, part_images, first_image); cam_sizes
+        [(w, h)] per camera.  last_mp_t: int32 cuda [n_cams * capacity] map-point ids by slot (-1 none); cur_mp_t: same shape,
+        overwritten (every slot below a camera's count starts at -1); bad_t [n_points] u8 cuda or None, n_points = len(bad_t) or
+        every id when None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4] when diag is set,
+        as cuda tensors."""
+        import torch
+        fc, fl = (PackedFrame(f[0].data_ptr(), *f[1:4]) for f in (cur, last))
+        dev = cur[0].device
+        nc = len(cam_sizes)
+        cw = np.ascontiguousarray([s[0] for s in cam_sizes], np.int32)
+        ch = np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
+        n_points = bad_t.shape[0] if bad_t is not None else 2**31 - 1
+        if out is None:
+            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
+        _check(lib().mcs_window_search_device(C.byref(fc), C.byref(fl), nc, capacity, self.mbFeatDim, _p(cw), _p(ch), _dptr(last_mp_t),
+                                              n_points, _dptr(bad_t), int(window), int(min_level), int(max_level), self.mfNNratio,
+                                              self.TH_HIGH_, int(self.havingMasks), _dptr(cur_mp_t), _dptr(out[0]), _dptr(out[1]),
+                                              _dptr(out[2]) if diag else None, _stream_handle(stream, dev)))
+        return (out[0], out[1], cur_mp_t) + ((out[2],) if diag else ())
+
+    def SearchByProjectionFramesDevice(self, cur, last, capacity, rig_cur, masks_t, last_mp_t, world_t, window, cur_mp_t, bad_t=None,
+                                       stream=None, out=None, diag=False):
+        """mcs_search_by_projection_frames_device: SearchByProjection(F1 = last, F2 = cur, window, .) (ref :476-577) with both frames
+        in packed feature buffers.  cur / last as for WindowSearchDevice; rig_cur: a Rig at the current pose (after
+        PoseOptimization); masks_t [n_cams,H,W] u8 cuda, its mirror masks.  last_mp_t / cur_mp_t: int32 cuda [n_cams * capacity]
+        map-point ids by slot (-1 none), cur_mp_t updated in place (its entries are "already found"); world_t [n_points,3] f64 cuda;
+        bad_t [n_points] u8 cuda or None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4]
+        when diag is set, as cuda tensors."""
+        import torch
+        fc, fl = (PackedFrame(f[0].data_ptr(), *f[1:4]) for f in (cur, last))
+        dev = cur[0].device
+        nc = len(rig_cur.cams)
+        ocs = (Ocam * nc)(*[as_ocam(c) for c in rig_cur.cams])
+        mi = np.ascontiguousarray(rig_cur.MtMc_inv, np.float64)
+        if out is None:
+            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
+        _check(lib().mcs_search_by_projection_frames_device(C.byref(fc), C.byref(fl), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t),
+                                                            _p(mi), _dptr(last_mp_t), world_t.shape[0], _dptr(world_t), _dptr(bad_t),
+                                                            int(window), self.mfNNratio, self.TH_HIGH_, int(self.havingMasks),
+                                                            _dptr(cur_mp_t), _dptr(out[0]), _dptr(out[1]), _dptr(out[2]) if diag else None,
+                                                            _stream_handle(stream, dev)))
+        return (out[0], out[1], cur_mp_t) + ((out[2],) if diag else ())
+
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
         """ref :579-726.  vbPrevMatched [n1,2] float64 updated in place.  Returns (nmatches, vnMatches12)."""
         prev = np.ascontiguousarray(vbPrevMatched, np.float64)

@@ -138,6 +138,23 @@ struct ProjSearchLastArgs : PsFrameArgs {   // SearchByProjection(CurrentFrame, 
     double th;
 };
 cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaStream_t st);
+// TrackPreviousFrame's searches, F1 = the last frame, F2 = the frame searched.  Neither reads scale factors (n_levels = 0, sf NULL).
+struct WindowSearchDevArgs : PsFrameArgs {   // WindowSearch(F1, F2, window, ., min_level, max_level): frame_mp is an output
+    const PsCamSlots* last;                                  // host [n_cams]: F1's image slots
+    int n_points;
+    const int* last_mp; const uint8_t* bad;                  // device, slot-indexed / [n_points] (bad may be NULL)
+    double window, nnratio; int min_level, max_level;
+};
+cudaError_t launch_window_search_device(const WindowSearchDevArgs& a, cudaStream_t st);
+struct SearchFramesDevArgs : PsFrameArgs {   // SearchByProjection(F1, F2, window, .): frame_mp holds F2.mvpMapPoints on entry
+    const PsCamSlots* last;                                  // host [n_cams]: F1's image slots
+    const mcs_ocam* models; const double* mtmc_inv;          // host [n_cams], [n_cams * 16] (F2's pose)
+    const uint8_t* masks;                                    // device [n_cams][h][w] level-0 mirror masks
+    int n_points;
+    const int* last_mp; const double* world_pos; const uint8_t* bad;   // device (bad may be NULL)
+    double window, nnratio;
+};
+cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cudaStream_t st);
 int proj_search_max_rounds();
 
 // ---- bag of words (bow_kernels.cu) ----

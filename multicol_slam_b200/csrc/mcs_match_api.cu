@@ -617,10 +617,10 @@ bool packed_frame_ok(const mcs_packed_frame* fr, int n_cams) {
            (long long)fr->first_image + n_cams <= (long long)fr->n_parts * fr->part_images;
 }
 
-// the arguments of the frame both device SearchByProjection calls search, and of the packed feature buffers the images of its
-// cameras come from (`last`: the motion-model search only)
-int check_packed_frames(int n_cams, int capacity, int dim, int n_levels, const mcs_packed_frame* cur, const mcs_packed_frame* last) {
-    if (n_cams < 1 || n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+// the arguments of the frame the device searches search, and of the packed feature buffers the images of its cameras come from
+// (`last`: the searches between two frames only)
+int check_packed_frames(int n_cams, int capacity, int dim, const mcs_packed_frame* cur, const mcs_packed_frame* last) {
+    if (n_cams < 1) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     if (capacity < 1 || capacity > 65535) return mcs_fail(MCS_ERR_INVALID, "capacity must be 1..65535");
     if (int rc = check_desc_dim(dim)) return rc;
     if (!packed_frame_ok(cur, n_cams)) return mcs_fail(MCS_ERR_INVALID, "current frame: no buffer, or first_image + n_cams exceeds its images");
@@ -640,7 +640,8 @@ int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int
     if (!packed_dev || !cam_width || !cam_height || !scale_factors || !mps || !frame_mp_dev || !nmatches_dev || !status_dev)
         return mcs_fail(MCS_ERR_INVALID, "null argument");
     const mcs_packed_frame frame{packed_dev, n_parts, part_images, first_image};
-    if (int rc = check_packed_frames(n_cams, capacity, dim, n_levels, &frame, nullptr)) return rc;
+    if (n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, &frame, nullptr)) return rc;
     if (mps->n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     if (!mps->in_view || !mps->level || !mps->proj_x || !mps->proj_y || !mps->view_cos || !mps->desc)
         return mcs_fail(MCS_ERR_INVALID, "null map-point array");
@@ -673,7 +674,8 @@ int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_
     if (!cur || !last || !cams || !masks_dev || !scale_factors || !mtmc_inv || !last_mp_dev || !world_pos_dev || !cur_mp_dev ||
         !nmatches_dev || !status_dev)
         return mcs_fail(MCS_ERR_INVALID, "null argument");
-    if (int rc = check_packed_frames(n_cams, capacity, dim, n_levels, cur, last)) return rc;
+    if (n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, cur, last)) return rc;
     if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     for (int c = 0; c < n_cams; ++c) {
         if (cams[c].width < 1 || cams[c].height < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
@@ -695,6 +697,68 @@ int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_
     a.n_points = n_points; a.last_mp = last_mp_dev; a.last_outlier = last_outlier_dev; a.world_pos = world_pos_dev; a.bad = bad_dev;
     a.th = th;
     CUDA_CHECK(launch_search_by_projection_last(a, st));
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
+    return MCS_OK;
+}
+
+int mcs_window_search_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity, int32_t dim,
+                             const int32_t* cam_width, const int32_t* cam_height, const int32_t* last_mp_dev, int32_t n_points,
+                             const uint8_t* bad_dev, int32_t window, int32_t min_level, int32_t max_level, double nnratio, int32_t th_high,
+                             int32_t having_masks, int32_t* cur_mp_dev, int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev,
+                             void* stream) {
+    if (!cur || !last || !cam_width || !cam_height || !last_mp_dev || !cur_mp_dev || !nmatches_dev || !status_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, cur, last)) return rc;
+    if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    for (int c = 0; c < n_cams; ++c)
+        if (cam_width[c] < 1 || cam_height[c] < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
+    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_CHECK(keep_pool_memory());
+    const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
+    WindowSearchDevArgs a{};
+    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim;
+    a.cams = cs.data(); a.cam_w = cam_width; a.cam_h = cam_height;
+    a.th_high = th_high; a.masked = having_masks != 0;
+    a.frame_mp = cur_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
+    a.last = ls.data(); a.n_points = n_points; a.last_mp = last_mp_dev; a.bad = bad_dev;
+    a.window = window; a.nnratio = nnratio; a.min_level = min_level; a.max_level = max_level;
+    CUDA_CHECK(launch_window_search_device(a, st));
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
+    return MCS_OK;
+}
+
+int mcs_search_by_projection_frames_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity,
+                                           int32_t dim, const mcs_ocam* cams, const uint8_t* masks_dev, const double* mtmc_inv,
+                                           const int32_t* last_mp_dev, int32_t n_points, const double* world_pos_dev, const uint8_t* bad_dev,
+                                           int32_t window, double nnratio, int32_t th_high, int32_t having_masks, int32_t* cur_mp_dev,
+                                           int32_t* nmatches_dev, int32_t* status_dev, int32_t* diag_dev, void* stream) {
+    if (!cur || !last || !cams || !masks_dev || !mtmc_inv || !last_mp_dev || !world_pos_dev || !cur_mp_dev || !nmatches_dev || !status_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, cur, last)) return rc;
+    if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    for (int c = 0; c < n_cams; ++c) {
+        if (cams[c].width < 1 || cams[c].height < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
+        if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
+            return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
+    }
+    // one query per (last-frame slot, camera): the owner words hold a 24-bit query index
+    if ((long long)n_cams * n_cams * capacity >= (1LL << 24))
+        return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * n_cams * capacity must stay below 2^24");
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_CHECK(keep_pool_memory());
+    const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
+    std::vector<int> cw(n_cams), ch(n_cams);
+    for (int c = 0; c < n_cams; ++c) { cw[c] = cams[c].width; ch[c] = cams[c].height; }
+    SearchFramesDevArgs a{};
+    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim;
+    a.cams = cs.data(); a.cam_w = cw.data(); a.cam_h = ch.data();
+    a.th_high = th_high; a.masked = having_masks != 0;
+    a.frame_mp = cur_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
+    a.last = ls.data(); a.models = cams; a.mtmc_inv = mtmc_inv; a.masks = masks_dev;
+    a.n_points = n_points; a.last_mp = last_mp_dev; a.world_pos = world_pos_dev; a.bad = bad_dev;
+    a.window = window; a.nnratio = nnratio;
+    CUDA_CHECK(launch_search_by_projection_frames(a, st));
     if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
     return MCS_OK;
 }

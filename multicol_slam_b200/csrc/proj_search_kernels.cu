@@ -1,17 +1,23 @@
-// proj_search_kernels.cu -- SearchByProjection(F, vpMapPoints, th) (ref src/cORBmatcher.cpp:67-166) and the motion-model
-// SearchByProjection(CurrentFrame, LastFrame, th) (ref :1990-2118) with every input and output resident on the device: the frames
-// come straight from packed feature buffers (mcs_packed_layout), the map points from device arrays, and the reference's ordered
-// greedy acceptance runs on the device.
+// proj_search_kernels.cu -- SearchByProjection(F, vpMapPoints, th) (ref src/cORBmatcher.cpp:67-166), the motion-model
+// SearchByProjection(CurrentFrame, LastFrame, th) (ref :1990-2118) and TrackPreviousFrame's WindowSearch(F1, F2) (:326-473) and
+// SearchByProjection(F1, F2, window) (:476-577) with every input and output resident on the device: the frames come straight from
+// packed feature buffers (mcs_packed_layout), the map points from device arrays, and the reference's ordered greedy acceptance
+// runs on the device.
 //
 //   ps_gather_kernel    a frame's keypoints / descriptors / masks in slot order (slot = cam * capacity + j); empty slots get a
 //                       position outside every image, so the unchanged frame_prepare_kernel leaves them out of the grid
 //   pl_project_kernel   motion model only: per last-frame slot, its map point projected with the current pose into its camera
+//   pw_clear_kernel     WindowSearch only: the searched frame's assignments start free
+//   pf_flag / pf_project  SearchByProjection(F1, F2) only: "already found" and first-slot flags per map point, then per
+//                       (last-frame slot, camera) the slot's map point projected with the current pose into that camera
 //   ps_count / ps_fill  the query array in the reference's order, a count / scan / fill over a query maker: map point outer,
-//                       camera inner over in_view and bad (MapPointQueries), or last-frame slot order (LastFrameQueries)
+//                       camera inner over in_view and bad (MapPointQueries), last-frame slot order (LastFrameQueries,
+//                       WindowQueries), or last-frame slot outer, camera inner (FramesQueries)
 //   ps_list_kernel      per query the K smallest (distance, visiting position) keys of its window and the true candidate count
 //   ps_round_kernel     one round of the fixpoint iteration of the ordered acceptance (DESIGN.md section 4)
 //   ps_walk_kernel      the sequential fallback past the round cap: one warp per camera walks the unsettled queries in order
 //   pl_round / pl_walk  the same two kernels under the motion model's acceptance rule (MCS_RULE_BEST)
+//   pr_round / pr_walk  the same two kernels under the previous-frame searches' ratio rule (MCS_RULE_RATIO)
 //
 // No kernel reads anything back to the host: every size that depends on the data (the number of queries, the rounds the
 // fixpoint needed, where the walk starts) lives in device memory and the kernels are launched for the upper bound.
@@ -113,6 +119,61 @@ __global__ void __launch_bounds__(256) pl_project_kernel(const LastProjArgs a, u
     ok[s] = 1; u[s] = x; v[s] = y;
 }
 
+// ---- previous frame: WindowSearch(F1 = last, F2 = cur) starts from an all-free F2 (ref :333) ----
+__global__ void pw_clear_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, int* __restrict__ frame_mp) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_cams * capacity) return;
+    const int c = s / capacity, j = s - c * capacity;
+    if (j < min(*cams[c].count, capacity)) frame_mp[s] = -1;
+}
+
+// ---- previous frame: the skip rules of SearchByProjection(F1 = last, F2 = cur, window) (ref :481-500) ----
+// found[p]: p is held by a slot of cur on entry (spMapPointsAlreadyFound).  first[p]: the smallest last-frame slot carrying p
+// (mapPt_2_obs_idx); slot order is the reference's visiting order, so the atomicMin picks the keypoint the reference keeps.  Ids of
+// cur >= n_points match no valid p and are left out; ids of last >= n_points raise status (their slot is dropped by pf_project).
+__global__ void pf_flag_kernel(const PsCamSlots* __restrict__ cur, const PsCamSlots* __restrict__ last, const int n_cams, const int capacity,
+                               const int n_points, const int* __restrict__ cur_mp, const int* __restrict__ last_mp, uint8_t* __restrict__ found,
+                               int* __restrict__ first, int* __restrict__ status) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_cams * capacity) return;
+    const int c = s / capacity, j = s - c * capacity;
+    if (j < min(*cur[c].count, capacity)) {
+        const int p = cur_mp[s];
+        if (p >= 0 && p < n_points) found[p] = 1;
+    }
+    if (j < min(*last[c].count, capacity)) {
+        const int p = last_mp[s];
+        if (p >= n_points) *status = MCS_ERR_INVALID;
+        else if (p >= 0) atomicMin(&first[p], s);
+    }
+}
+
+// Entry k = s * n_cams + c: last-frame slot s qualifies when its point p is valid, not bad, not already found and s is its first
+// slot; p is then projected with the current pose into EVERY camera c (ref :509-513), and makes a query where it falls in c's mask.
+struct FramesProjArgs {
+    const PsCamSlots* last; int n_cams, capacity, n_points;
+    const int* last_mp; const uint8_t* bad; const uint8_t* found; const int* first; const double* pos;
+    const mcs_ocam* models; const double* mtmc_inv; const uint8_t* masks;
+};
+__global__ void __launch_bounds__(256) pf_project_kernel(const FramesProjArgs a, uint8_t* __restrict__ ok, double* __restrict__ u,
+                                                         double* __restrict__ v) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= (long long)a.n_cams * a.n_cams * a.capacity) return;
+    const int s = (int)(k / a.n_cams), c = (int)(k - (long long)s * a.n_cams);
+    ok[k] = 0;
+    const int cl = s / a.capacity;
+    if (s - cl * a.capacity >= min(*a.last[cl].count, a.capacity)) return;
+    const int i = a.last_mp[s];
+    if (i < 0 || i >= a.n_points) return;
+    if ((a.bad && a.bad[i]) || a.found[i] || a.first[i] != s) return;
+    const mcs_ocam cam = a.models[c];
+    double x, y;
+    if (!cam_project_in_mask(a.mtmc_inv + 16 * c, cam, a.masks + (size_t)c * cam.width * cam.height, a.pos[3 * i], a.pos[3 * i + 1],
+                             a.pos[3 * i + 2], x, y))
+        return;
+    ok[k] = 1; u[k] = x; v[k] = y;
+}
+
 // ---- query build: a count / scan / fill over the entries of a query maker, in the maker's order ----
 // A maker has size() entries; valid(k) says whether entry k is a query (and may raise status), make(k) builds it.  sf is the
 // staged scale-factor table, set by ps_search.
@@ -154,6 +215,49 @@ struct LastFrameQueries {        // SearchByProjection(CurrentFrame, LastFrame, 
         mcs_window_query q;                          // GetFeaturesInArea(cam, u, v, th * sf[oct], oct - 1, oct + 1)  (ref :2027-2033)
         q.cam = (int)(k / capacity); q.min_level = oct - 1; q.max_level = oct + 1; q.desc_index = (int)k;
         q.x = u[k]; q.y = v[k]; q.r = th * sf[oct];
+        return q;
+    }
+};
+
+struct WindowQueries {           // WindowSearch(F1 = last, F2 = cur, window, ., min_level, max_level): entry k = last-frame slot (ref :344-368)
+    int n_slots, capacity, n_points, min_level, max_level;
+    const PsCamSlots* last; const mcs_keypoint* keys; const int* last_mp; const uint8_t* bad;
+    const double* sf; double window;                         // sf: unused, no level is looked up
+    __host__ __device__ long long size() const { return n_slots; }
+    __device__ bool valid(long long k, int* status) const {
+        if (k >= n_slots) return false;
+        const int c = (int)(k / capacity);
+        if ((int)k - c * capacity >= min(*last[c].count, capacity)) return false;
+        const int p = last_mp[k];
+        if (p < 0) return false;
+        if (p >= n_points) {
+            if (status) *status = MCS_ERR_INVALID;
+            return false;
+        }
+        if (bad && bad[p]) return false;
+        const int oct = keys[k].octave;
+        if (min_level > 0 && oct < min_level) return false;
+        return !(max_level < INT_MAX && oct > max_level);
+    }
+    __device__ mcs_window_query make(long long k) const {
+        mcs_window_query q;                          // GetFeaturesInArea(cam, kp1.pt.x, kp1.pt.y, windowSize)  (ref :366-368)
+        q.cam = (int)(k / capacity); q.min_level = -1; q.max_level = -1; q.desc_index = (int)k;
+        q.x = (double)keys[k].x; q.y = (double)keys[k].y; q.r = window;
+        return q;
+    }
+};
+
+struct FramesQueries {           // SearchByProjection(F1 = last, F2 = cur, window): entry k = slot * n_cams + cam, as pf_project_kernel set it
+    int n_slots, n_cams;
+    const uint8_t* ok; const double* u; const double* v; const mcs_keypoint* keys;
+    const double* sf; double window;                         // sf: unused, the octave is a level filter only
+    __host__ __device__ long long size() const { return (long long)n_slots * n_cams; }
+    __device__ bool valid(long long k, int*) const { return k < size() && ok[k]; }
+    __device__ mcs_window_query make(long long k) const {
+        const int s = (int)(k / n_cams), oct = keys[s].octave;
+        mcs_window_query q;                          // GetFeaturesInArea(c, u, v, windowSize, level1, level1)  (ref :515-516)
+        q.cam = (int)(k - (long long)s * n_cams); q.min_level = oct; q.max_level = oct; q.desc_index = s;
+        q.x = u[k]; q.y = v[k]; q.r = window;
         return q;
     }
 };
@@ -307,13 +411,15 @@ __global__ void __launch_bounds__(256) ps_list_kernel(const WindowFrameDev f, co
 // The decision of one query (warp-uniform) under a "keypoint already taken" predicate.  MCS_RULE_LEVEL_RATIO: best / second best
 // free candidate by (distance, visiting position) -- what the sequential strict-< update of ref :138-150 picks -- and the
 // acceptance of :154-160.  MCS_RULE_BEST: the best free candidate alone (strict < over the visiting order, ref :2050-2068),
-// accepted when its distance is <= th_high (:2070).  The list decides when it holds as many free entries as the rule reads, or
-// every candidate; otherwise the window is scanned again with the predicate.
+// accepted when its distance is <= th_high (:2070).  MCS_RULE_RATIO: best / second best free candidate, accepted when
+// best <= second * nnratio and best <= th_high (WindowSearch :405-416, SearchByProjection(F1, F2) :553-566), in the double form of
+// the host replay.  The list decides when it holds as many free entries as the rule reads, or every candidate; otherwise the window
+// is scanned again with the predicate.
 template <int RULE, int WORDS, bool MASKED, class Taken>
 __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_window_query& qq, const unsigned* lk, const int* ls, const int cnt,
                                          const uint32_t* qdesc, const uint32_t* qmask, const Taken& taken, const int th_high,
                                          const double nnratio, int* rescans) {
-    static_assert(RULE == MCS_RULE_LEVEL_RATIO || RULE == MCS_RULE_BEST, "device acceptance rules");
+    static_assert(RULE == MCS_RULE_LEVEL_RATIO || RULE == MCS_RULE_BEST || RULE == MCS_RULE_RATIO, "device acceptance rules");
     constexpr int NB = RULE == MCS_RULE_BEST ? 1 : 2;       // free keys the rule reads
     const int lane = threadIdx.x & 31;
     unsigned k = kNoKey; int s = -1; bool fr = false;
@@ -337,6 +443,10 @@ __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_wind
     }
     if (s0 < 0) return -1;
     if constexpr (RULE == MCS_RULE_BEST) return (int)(k0 >> 16) <= th_high ? s0 : -1;
+    if constexpr (RULE == MCS_RULE_RATIO) {
+        const int d0 = (int)(k0 >> 16), d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX;
+        return (double)d0 <= (double)d1 * nnratio && d0 <= th_high ? s0 : -1;
+    }
     const int d0 = (int)(k0 >> 16), l0 = f.koct[s0];
     const int d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX, l1 = s1 >= 0 ? f.koct[s1] : -1;
     const bool ok = d0 <= th_high && !(l0 == l1 && (double)d0 > nnratio * (double)d1);
@@ -393,7 +503,7 @@ __device__ __forceinline__ void ps_round(const WindowFrameDev& f, const PsState&
         }
     }
 }
-// one kernel name per rule: MCS_RULE_LEVEL_RATIO (local map) and MCS_RULE_BEST (motion model)
+// one kernel name per rule: MCS_RULE_LEVEL_RATIO (local map), MCS_RULE_BEST (motion model), MCS_RULE_RATIO (previous frame)
 template <int WORDS, bool MASKED>
 __global__ void __launch_bounds__(256, 2) ps_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
                                                        const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
@@ -403,6 +513,11 @@ template <int WORDS, bool MASKED>
 __global__ void __launch_bounds__(256, 2) pl_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
                                                        const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
     ps_round<MCS_RULE_BEST, WORDS, MASKED>(f, p, r, qdesc, qmask, fmp_in);
+}
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(256, 2) pr_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
+                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
+    ps_round<MCS_RULE_RATIO, WORDS, MASKED>(f, p, r, qdesc, qmask, fmp_in);
 }
 
 // Writes the final decisions of the settled prefix into frame_mp and counts them; records where the walk has to start.
@@ -476,6 +591,11 @@ template <int WORDS, bool MASKED>
 __global__ void __launch_bounds__(32) pl_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
                                                      const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
     ps_walk<MCS_RULE_BEST, WORDS, MASKED>(f, p, qdesc, qmask, frame_mp, nmatches);
+}
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(32) pr_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
+                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
+    ps_walk<MCS_RULE_RATIO, WORDS, MASKED>(f, p, qdesc, qmask, frame_mp, nmatches);
 }
 
 __global__ void ps_diag_kernel(const int* __restrict__ ctl, int* __restrict__ diag) {
@@ -568,10 +688,12 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
             ps_list_kernel<W, M><<<wblocks, 256, 0, st>>>(f, qry, ctl, qd, qk, lkey, lslot, lcnt);                     \
             for (int r = 0; r < kPsRounds; ++r) {                                                                      \
                 if constexpr (RULE == MCS_RULE_BEST) pl_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp); \
+                else if constexpr (RULE == MCS_RULE_RATIO) pr_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp); \
                 else ps_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp);                      \
             }                                                                                                          \
             ps_finalize_kernel<<<fblocks, 256, 0, st>>>(p, a.frame_mp, a.nmatches);                                    \
             if constexpr (RULE == MCS_RULE_BEST) pl_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches); \
+            else if constexpr (RULE == MCS_RULE_RATIO) pr_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches); \
             else ps_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches);          \
         }
         if (a.dim == 16) { if (a.masked) MCS_PS(4, true) else MCS_PS(4, false) }
@@ -634,6 +756,86 @@ cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaSt
     if (e == cudaSuccess) {
         const LastFrameQueries qm{NS, a.capacity, ok, u, v, keys, nullptr, a.th};
         e = ps_search<MCS_RULE_BEST>(a, qm, 0.0, desc, dmask, a.last_mp, st);
+    }
+    const cudaError_t ef = cudaFreeAsync(base, st);
+    return e != cudaSuccess ? e : ef;
+}
+
+// WindowSearch: cur_mp cleared below each camera's count, the last frame in slot order, then the current frame searched under
+// MCS_RULE_RATIO with one query per qualifying last-frame slot and last_mp as the tags.
+cudaError_t launch_window_search_device(const WindowSearchDevArgs& a, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    const size_t db = (size_t)NS * a.dim;
+    const size_t sizes[] = {sizeof(PsCamSlots) * a.n_cams, sizeof(PsCamSlots) * a.n_cams,        // staged host inputs: cur, last
+                            sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0};                  // keys desc dmask
+    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
+    size_t off[nsz], total = 0;
+    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
+    cudaError_t e = keep_pool_memory();
+    if (e != cudaSuccess) return e;
+    uint8_t* base = nullptr;
+    e = cudaMallocAsync((void**)&base, total, st);
+    if (e != cudaSuccess) return e;
+    auto at = [&](int i) { return (void*)(base + off[i]); };
+    PsCamSlots* cur = (PsCamSlots*)at(0); PsCamSlots* last = (PsCamSlots*)at(1);
+    mcs_keypoint* keys = (mcs_keypoint*)at(2); uint8_t* desc = (uint8_t*)at(3); uint8_t* dmask = a.masked ? (uint8_t*)at(4) : nullptr;
+    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, cur, st);
+    if (e == cudaSuccess) e = stage_to_device(a.last, sizeof(PsCamSlots) * a.n_cams, last, st);
+    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
+    if (e == cudaSuccess) {
+        pw_clear_kernel<<<(NS + 255) / 256, 256, 0, st>>>(cur, a.n_cams, a.capacity, a.frame_mp);
+        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(last, a.n_cams, a.capacity, a.dim, a.masked, keys, nullptr, desc, dmask);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        const WindowQueries qm{NS, a.capacity, a.n_points, a.min_level, a.max_level, last, keys, a.last_mp, a.bad, nullptr, a.window};
+        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, desc, dmask, a.last_mp, st);
+    }
+    const cudaError_t ef = cudaFreeAsync(base, st);
+    return e != cudaSuccess ? e : ef;
+}
+
+// SearchByProjection(F1 = last, F2 = cur): the skip flags (pf_flag_kernel), the last frame in slot order, the (slot, camera)
+// projections (pf_project_kernel), then the current frame searched under MCS_RULE_RATIO with last_mp as the tags.
+cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    const size_t NK = (size_t)NS * a.n_cams;
+    const size_t db = (size_t)NS * a.dim;
+    const size_t sizes[] = {sizeof(PsCamSlots) * a.n_cams, sizeof(PsCamSlots) * a.n_cams, sizeof(mcs_ocam) * a.n_cams,  // staged: cur last
+                            128ull * a.n_cams,                                                                         // models mtmc_inv
+                            (size_t)a.n_points, 4ull * a.n_points,                                                     // found first
+                            sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0, NK, 8 * NK, 8 * NK};                    // keys desc dmask ok u v
+    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
+    size_t off[nsz], total = 0;
+    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
+    cudaError_t e = keep_pool_memory();
+    if (e != cudaSuccess) return e;
+    uint8_t* base = nullptr;
+    e = cudaMallocAsync((void**)&base, total, st);
+    if (e != cudaSuccess) return e;
+    auto at = [&](int i) { return (void*)(base + off[i]); };
+    PsCamSlots* cur = (PsCamSlots*)at(0); PsCamSlots* last = (PsCamSlots*)at(1); mcs_ocam* models = (mcs_ocam*)at(2); double* mi = (double*)at(3);
+    uint8_t* found = (uint8_t*)at(4); int* first = (int*)at(5);
+    mcs_keypoint* keys = (mcs_keypoint*)at(6); uint8_t* desc = (uint8_t*)at(7); uint8_t* dmask = a.masked ? (uint8_t*)at(8) : nullptr;
+    uint8_t* ok = (uint8_t*)at(9); double* u = (double*)at(10); double* v = (double*)at(11);
+    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, cur, st);
+    if (e == cudaSuccess) e = stage_to_device(a.last, sizeof(PsCamSlots) * a.n_cams, last, st);
+    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
+    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, mi, st);
+    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
+    if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(found, 0, a.n_points, st);
+    if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(first, 0x7F, 4ull * a.n_points, st);     // above every slot
+    if (e == cudaSuccess) {
+        pf_flag_kernel<<<(NS + 255) / 256, 256, 0, st>>>(cur, last, a.n_cams, a.capacity, a.n_points, a.frame_mp, a.last_mp, found, first,
+                                                         a.status);
+        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(last, a.n_cams, a.capacity, a.dim, a.masked, keys, nullptr, desc, dmask);
+        const FramesProjArgs pa{last, a.n_cams, a.capacity, a.n_points, a.last_mp, a.bad, found, first, a.world_pos, models, mi, a.masks};
+        pf_project_kernel<<<(unsigned)((NK + 255) / 256), 256, 0, st>>>(pa, ok, u, v);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) {
+        const FramesQueries qm{NS, a.n_cams, ok, u, v, keys, nullptr, a.window};
+        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, desc, dmask, a.last_mp, st);
     }
     const cudaError_t ef = cudaFreeAsync(base, st);
     return e != cudaSuccess ? e : ef;

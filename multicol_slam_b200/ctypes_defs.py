@@ -58,6 +58,12 @@ def set_prototypes(lib):
     f = lib.mcs_search_by_projection_last_device
     f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, I, P, P, P, P, I, P, P, D, I, I, P, P, P, P, P]
     f.restype = C.c_int
+    f = lib.mcs_window_search_device
+    f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, P, I, P, I, I, I, D, I, I, P, P, P, P, P]
+    f.restype = C.c_int
+    f = lib.mcs_search_by_projection_frames_device
+    f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, P, P, I, P, P, I, D, I, I, P, P, P, P, P]
+    f.restype = C.c_int
 
 
 import numpy as np
