@@ -599,6 +599,67 @@ int  mcs_search_by_bow(const uint8_t* desc1, const uint8_t* mask1, const uint8_t
                        const int32_t* fv2_nodes, const int32_t* fv2_offsets, int32_t n_fv2, const int32_t* fv2_features,
                        int32_t dim, int32_t th_low, double nnratio, int32_t* match_of_2, int32_t* nmatches);
 
+/* ---- Relocalisation's bag-of-words step on the device (ref src/cTracking.cpp:1125-1312): ComputeBoW and SearchByBoW(KF, F) on
+ * frames that stay in their packed feature buffers.  Conventions of mcs_search_by_projection_last_device: frames as
+ * mcs_packed_frame, everything per keypoint indexed by slot c * capacity + j, asynchronous on `stream` (NULL = the default
+ * stream, synchronised before returning), scratch from the stream-ordered pool, every argument checked on the host before any
+ * launch, results and status in device memory, nothing read back.  Slot order is the reference's contiguous keypoint order
+ * (camera-major, ref src/cMultiFrame.cpp:168-184), so "ascending feature index" in DBoW2's containers is "ascending slot". */
+
+/* The largest number of distinct node ids a FeatureVector built with `levelsup` can hold: the nodes at depth
+ * max(L - levelsup, 0) plus the leaves shallower than that (see mcs_bow_transform).  Sizes fv_nodes / fv_offsets and max_nodes
+ * below.  Host arithmetic. */
+int  mcs_vocabulary_level_nodes(const mcs_vocabulary* voc, int32_t levelsup, int32_t* n_nodes);
+
+/* transform(features, BowVector&, FeatureVector&, levelsup) (ref TemplatedVocabulary.h:1126-1194; ComputeBoW, ref
+ * src/cMultiFrame.cpp:356-363, src/cMultiKeyFrame.cpp:105-114) over the descriptors of the n_cams cameras of `frame`, each
+ * camera's slots below its device-side count, in camera order.  The values equal mcs_bow_vectors on the concatenated descriptors
+ * bit for bit, feature indices being slots.  All outputs are device memory:
+ *   word_dev / weight_dev / node_dev [n_cams * capacity] (each may be NULL): what mcs_bow_transform returns, per slot; untouched
+ *     at or beyond a camera's count.
+ *   FeatureVector as CSR: fv_nodes_dev [max_nodes] ascending node ids, fv_offsets_dev [max_nodes + 1], n_fv_dev [1],
+ *     fv_features_dev [n_cams * capacity] slots, ascending inside a node; fv_offsets_dev[*n_fv_dev] entries are written.
+ *   BowVector: bow_words_dev / bow_values_dev [n_cams * capacity] ascending word ids and their values, n_bow_dev [1].
+ *   status_dev [1]: MCS_OK, or MCS_ERR_CAPACITY when the frame holds more than max_nodes nodes: the FeatureVector then holds the
+ *     max_nodes smallest node ids, complete and consistent, and nothing is written beyond the arrays.  The BowVector is unaffected.
+ * dim must be 32 (FORB::L; MCS_ERR_UNSUPPORTED otherwise); the vocabulary's device must be current (MCS_ERR_INVALID otherwise);
+ * capacity <= 65535, n_cams * capacity < 2^24.  Scratch: 4 bytes per vocabulary node and 8 per word, cleared per call. */
+int  mcs_bow_vectors_device(const mcs_vocabulary* voc, const mcs_packed_frame* frame, int32_t n_cams, int32_t capacity, int32_t dim,
+                            int32_t levelsup, int32_t max_nodes, int32_t* word_dev, double* weight_dev, int32_t* node_dev,
+                            int32_t* fv_nodes_dev, int32_t* fv_offsets_dev, int32_t* n_fv_dev, int32_t* fv_features_dev,
+                            int32_t* bow_words_dev, double* bow_values_dev, int32_t* n_bow_dev, int32_t* status_dev, void* stream);
+
+/* A frame or key frame whose FeatureVector is on the device (mcs_bow_vectors_device's CSR outputs, or arrays of the same form). */
+typedef struct mcs_bow_frame {
+    mcs_packed_frame frame;
+    const int32_t* fv_nodes_dev;        /* [<= max_nodes] strictly ascending node ids          */
+    const int32_t* fv_offsets_dev;      /* [*n_fv_dev + 1] non-decreasing                      */
+    const int32_t* n_fv_dev;            /* [1]; entries beyond max_nodes are not visited       */
+    const int32_t* fv_features_dev;     /* slots                                               */
+    const int32_t* mp_dev;              /* [n_cams * capacity] slot-indexed map-point ids, -1 = none; NULL for the current frame */
+} mcs_bow_frame;
+
+/* cORBmatcher::SearchByBoW(pKF, F, vpMapPointMatches) (ref src/cORBmatcher.cpp:179-324, mbCheckOrientation compile-time false)
+ * for n_kf key frames against one current frame, as Relocalisation calls it for every candidate (ref src/cTracking.cpp:1170-1177).
+ * Per key frame k, independently of the others (n_kf key frames in one call give what n_kf calls with one key frame give):
+ *   match_mp_dev [n_kf][n_cams * capacity]: the map-point id matched to each current-frame slot, -1 = none; match_slot_dev (same
+ *   shape, may be NULL): the key-frame slot it came from.  Both are first set to -1 below each camera's count of `cur`; slots at
+ *   or beyond a count are neither read nor written, in any frame.
+ *   For every node id both feature vectors hold, ascending, and every key-frame slot of that node in list order whose mp_dev is
+ *   >= 0 and not bad: best and second-best distance (strict <, in list order) over the current frame's slots of that node that no
+ *   earlier keypoint of this key frame has taken; accepted when best <= th_low and (double)best < nnratio * (double)second
+ *   (second = INT_MAX without one).  Distances are DescriptorDistance64 / DescriptorDistance64Masked (having_masks) between the
+ *   packed descriptor rows, dim 16 / 32 / 64.
+ *   nmatches_dev [n_kf].  status_dev [1]: MCS_ERR_INVALID when a map-point id is >= n_points or a feature-vector entry is no
+ *   keypoint of its frame -- that keypoint is dropped, the others are unaffected -- MCS_OK otherwise.  bad_dev [n_points] may be NULL.
+ * The key frames may live in different packed buffers from each other and from `cur`, or share one.  max_nodes bounds the node
+ * lists visited (mcs_vocabulary_level_nodes); the grid is sized from n_kf * max_nodes.  n_kf = 0 is a successful no-op.
+ * capacity <= 65535, n_cams * capacity < 2^24 (MCS_ERR_UNSUPPORTED beyond). */
+int  mcs_search_by_bow_device(const mcs_bow_frame* kfs, int32_t n_kf, const mcs_bow_frame* cur, int32_t n_cams, int32_t capacity,
+                              int32_t dim, int32_t max_nodes, int32_t n_points, const uint8_t* bad_dev, int32_t th_low, double nnratio,
+                              int32_t having_masks, int32_t* match_mp_dev, int32_t* match_slot_dev, int32_t* nmatches_dev,
+                              int32_t* status_dev, void* stream);
+
 /* ---- multi-GPU: one camera (or stream chunk) per GPU, ONE allgather of the packed feature buffer (SURVEY 8e) -------------- */
 /* Packed feature buffer of a batch of n_images images: the four output arrays of the batched extractor in one allocation,
  *   [ counts int32[n_images] | mcs_keypoint[n_images][capacity] | desc u8[n_images][capacity][dim] | dmask u8[n_images][capacity][dim] ]

@@ -15,7 +15,7 @@ import pathlib
 
 import numpy as np
 
-from .ctypes_defs import (ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam, PackedFrame,
+from .ctypes_defs import (BowFrame, ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam, PackedFrame,
                           WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
 
 _PKG = pathlib.Path(__file__).resolve().parent
@@ -1207,6 +1207,62 @@ class cORBmatcher:
                                        _p(out), C.byref(n)))
         return n.value, out
 
+    def SearchByBoWDevice(self, kfs, cur, n_points, bad_t=None, max_nodes=None, stream=None, out=None):
+        """mcs_search_by_bow_device: SearchByBoW(pKF, F, vpMapPointMatches) (ref :179-324) for every candidate key frame of a
+        relocalisation in one call, all frames in packed feature buffers.  kfs: [(DeviceBoW, mp_t)] with mp_t the key frame's int32
+        cuda [n_cams * capacity] map-point ids by slot (-1 none); cur: the current frame's DeviceBoW (ORBVocabulary.transform_device,
+        or built by hand from CSR tensors).  bad_t [n_points] u8 cuda or None; max_nodes: the node lists visited, by default the
+        largest max_nodes of the frames.  Asynchronous on `stream`.  Returns (match_mp [n_kf, n_cams * capacity], match_slot (same
+        shape), nmatches [n_kf], status [1]) as int32 cuda tensors: per current-frame slot the matched map-point id and the
+        key-frame slot it came from, -1 = none; slots at or beyond a camera's count are not written."""
+        import torch
+        dev = cur.packed[0].device
+        nk, ns = len(kfs), cur.n_cams * cur.capacity
+        if max_nodes is None:
+            max_nodes = max([cur.max_nodes] + [b.max_nodes for b, _ in kfs])
+        if out is None:
+            with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(dev)):     # the fills run on `stream` too
+                out = (torch.full((nk, ns), -1, dtype=torch.int32, device=dev), torch.full((nk, ns), -1, dtype=torch.int32, device=dev),
+                       torch.zeros(nk, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev))
+        frames = (BowFrame * max(nk, 1))(*[b.bow_frame(mp_t) for b, mp_t in kfs])
+        fc = cur.bow_frame()
+        _check(lib().mcs_search_by_bow_device(frames, nk, C.byref(fc), cur.n_cams, cur.capacity, self.mbFeatDim, max_nodes, n_points,
+                                              _dptr(bad_t), self.TH_LOW_, C.c_double(self.mfNNratio), int(self.havingMasks),
+                                              _dptr(out[0]), _dptr(out[1]), _dptr(out[2]), _dptr(out[3]), _stream_handle(stream, dev)))
+        return out
+
+
+class DeviceBoW:
+    """What ComputeBoW leaves on the device for one frame (ORBVocabulary.transform_device): packed = (uint8 cuda tensor, n_parts,
+    part_images, first_image); the FeatureVector as CSR over slots (fv_nodes [max_nodes], fv_offsets [max_nodes + 1], n_fv [1],
+    fv_features [n_cams * capacity]); the BowVector (bow_words, bow_values [n_cams * capacity], n_bow [1]); status [1]; word /
+    weight / node per slot when they were asked for.  The tensors a search does not read may be None."""
+
+    def __init__(self, packed, n_cams, capacity, fv_nodes, fv_offsets, n_fv, fv_features, bow_words=None, bow_values=None, n_bow=None,
+                 status=None, word=None, weight=None, node=None):
+        self.packed, self.n_cams, self.capacity = packed, n_cams, capacity
+        self.fv_nodes, self.fv_offsets, self.n_fv, self.fv_features = fv_nodes, fv_offsets, n_fv, fv_features
+        self.bow_words, self.bow_values, self.n_bow, self.status = bow_words, bow_values, n_bow, status
+        self.word, self.weight, self.node = word, weight, node
+        self.max_nodes = fv_nodes.shape[0]
+
+    def bow_frame(self, mp_t=None):
+        """the mcs_bow_frame of this frame; mp_t: its map-point ids by slot (a key frame's)"""
+        f = BowFrame()
+        f.frame = PackedFrame(self.packed[0].data_ptr(), *self.packed[1:4])
+        f.fv_nodes_dev, f.fv_offsets_dev, f.n_fv_dev = self.fv_nodes.data_ptr(), self.fv_offsets.data_ptr(), self.n_fv.data_ptr()
+        f.fv_features_dev = self.fv_features.data_ptr()
+        f.mp_dev = mp_t.data_ptr() if mp_t is not None else None
+        return f
+
+    def host(self):
+        """(bow_words, bow_values, (fv_nodes, fv_offsets, fv_features)) as ORBVocabulary.transform returns them, feature indices
+        being slots (synchronises)"""
+        nb, nf = int(self.n_bow.item()), int(self.n_fv.item())
+        fo = self.fv_offsets[:nf + 1].cpu().numpy()
+        return (self.bow_words[:nb].cpu().numpy(), self.bow_values[:nb].cpu().numpy(),
+                (self.fv_nodes[:nf].cpu().numpy(), fo, self.fv_features[:int(fo[nf])].cpu().numpy()))
+
 
 class ORBVocabulary:
     """Mirror of ORBVocabulary = DBoW2::TemplatedVocabulary<FORB::TDescriptor, FORB> (ref include/cORBVocabulary.h:34) for the
@@ -1296,6 +1352,33 @@ class ORBVocabulary:
         _check(lib().mcs_bow_vectors(self._h, _p(desc), n, levelsup, _p(bw), _p(bv), C.byref(nb), _p(fn), _p(fo), C.byref(nf), _p(ff)))
         k = nf.value
         return bw[:nb.value].copy(), bv[:nb.value].copy(), (fn[:k].copy(), fo[:k + 1].copy(), ff[:fo[k]].copy())
+
+    def level_nodes(self, levelsup=4):
+        """mcs_vocabulary_level_nodes: the most node ids a FeatureVector built with `levelsup` can hold"""
+        n = C.c_int32(0)
+        _check(lib().mcs_vocabulary_level_nodes(self._h, levelsup, C.byref(n)))
+        return n.value
+
+    def transform_device(self, packed, n_cams, capacity, levelsup=4, max_nodes=None, per_slot=False, stream=None):
+        """mcs_bow_vectors_device: ComputeBoW on a frame that stays in its packed feature buffer.  packed = (uint8 cuda tensor,
+        n_parts, part_images, first_image); camera c = image first_image + c.  max_nodes defaults to level_nodes(levelsup);
+        per_slot also returns word / weight / node per slot.  Asynchronous on `stream`.  Returns a DeviceBoW of cuda tensors."""
+        import torch
+        dev = packed[0].device
+        ns = n_cams * capacity
+        if max_nodes is None:
+            max_nodes = self.level_nodes(levelsup)
+        i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=dev)  # noqa: E731
+        f64 = lambda n: torch.zeros(n, dtype=torch.float64, device=dev)  # noqa: E731
+        with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(dev)):         # the fills run on `stream` too
+            b = DeviceBoW(packed, n_cams, capacity, i32(max_nodes), i32(max_nodes + 1), i32(1), i32(ns), i32(ns), f64(ns), i32(1), i32(1),
+                          *((i32(ns), f64(ns), i32(ns)) if per_slot else ()))
+        fr = PackedFrame(packed[0].data_ptr(), *packed[1:4])
+        _check(lib().mcs_bow_vectors_device(self._h, C.byref(fr), n_cams, capacity, 32, levelsup, max_nodes, _dptr(b.word), _dptr(b.weight),
+                                            _dptr(b.node), _dptr(b.fv_nodes), _dptr(b.fv_offsets), _dptr(b.n_fv), _dptr(b.fv_features),
+                                            _dptr(b.bow_words), _dptr(b.bow_values), _dptr(b.n_bow), _dptr(b.status),
+                                            _stream_handle(stream, dev)))
+        return b
 
     def score(self, v1, v2):
         """score(BowVector, BowVector) with the vocabulary's scoring type; v = (words, values)."""

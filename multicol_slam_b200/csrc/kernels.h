@@ -174,4 +174,31 @@ struct GroupQuery { int feature, cand_start, cand_count, out_off; };
 cudaError_t launch_group_distance(const GroupQuery* queries, int nq, const uint8_t* desc1, const uint8_t* mask1, const uint8_t* desc2,
                                   const uint8_t* mask2, const int* cand, int dim, int* out, cudaStream_t st);
 
+// ComputeBoW on a frame in packed feature buffers (mcs_bow_vectors_device): every output in device memory, slot-indexed
+struct BowVectorsDevArgs {
+    int n_cams, capacity, levelsup, max_nodes;
+    int n_words, scoring, weighting;                           // of the vocabulary
+    const PsCamSlots* cams;                                    // host [n_cams] (device pointers inside)
+    int* word; double* weight; int* node;                      // [n_cams * capacity], each may be NULL
+    int* fv_nodes; int* fv_offsets; int* n_fv; int* fv_features;
+    int* bow_words; double* bow_values; int* n_bow; int* status;
+};
+cudaError_t launch_bow_vectors_device(const VocabularyDev& v, const BowVectorsDevArgs& a, cudaStream_t st);
+
+// SearchByBoW(KF_i, F) for a batch of key frames (mcs_search_by_bow_device)
+struct BowFrameDev {                                           // the device arrays of one mcs_bow_frame
+    const int* fv_nodes; const int* fv_offsets; const int* n_fv; const int* fv_features; const int* mp;
+};
+struct BowSearchDevArgs {
+    int n_kf, n_cams, capacity, dim, max_nodes, n_points, th_low;
+    double nnratio; bool masked;
+    const PsCamSlots* kf_cams;                                 // host [n_kf * n_cams]
+    const PsCamSlots* cur_cams;                                // host [n_cams]
+    const BowFrameDev* kfs;                                    // host [n_kf]
+    BowFrameDev cur;
+    const uint8_t* bad;                                        // device [n_points], may be NULL
+    int* match_mp; int* match_slot; int* nmatches; int* status;   // device; match_slot may be NULL
+};
+cudaError_t launch_search_by_bow_device(const BowSearchDevArgs& a, cudaStream_t st);
+
 }  // namespace mcs

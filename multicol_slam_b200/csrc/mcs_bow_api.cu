@@ -1,6 +1,8 @@
 // mcs_bow_api.cu -- C ABI of the bag-of-words row (include/mcs_b200.h): vocabulary object, transform, score,
-// feature-vector guided SearchByBoW.  Tree descent and group distances run on the GPU (bow_kernels.cu); the
-// std::map bookkeeping of DBoW2 and the matcher's order-dependent greedy rule are replayed on the host.
+// feature-vector guided SearchByBoW.  Two routes.  Host arrays in, host arrays out: tree descent and group distances run on the
+// GPU (bow_kernels.cu), the std::map bookkeeping of DBoW2 and the matcher's order-dependent greedy rule are replayed on the host.
+// Packed feature buffers in, device arrays out (mcs_bow_vectors_device, mcs_search_by_bow_device): everything runs on the GPU
+// and nothing is read back.
 #include <algorithm>
 #include <cfloat>
 #include <climits>
@@ -14,6 +16,7 @@
 #include "api_check.h"
 #include "kernels.h"
 #include "dev_scratch.h"
+#include "packed_frame.h"
 
 using namespace mcs;
 
@@ -21,6 +24,7 @@ struct mcs_vocabulary {
     int k = 0, L = 0, scoring = 0, weighting = 0, n_nodes = 0, n_words = 0, device = 0;
     Dev child_off, child_ids, desc, word_of_node, weight;
     VocabularyDev view{};
+    std::vector<int> nodes_at, leaves_at;       // per depth (root = 0): nodes, and those of them that are leaves
 };
 
 extern "C" {
@@ -70,6 +74,16 @@ int mcs_vocabulary_create(int32_t k, int32_t L, int32_t scoring, int32_t weighti
     if (ndev == 0) return mcs_fail(MCS_ERR_NO_DEVICE, "no CUDA device");
     mcs_vocabulary* v = new mcs_vocabulary();
     v->k = k; v->L = L; v->scoring = scoring; v->weighting = weighting; v->n_nodes = n_nodes; v->n_words = n_words;
+    {   // depth of every node, parents before children: breadth first over the CSR children
+        std::vector<int> depth(n_nodes, 0), queue(1, 0);
+        for (size_t h = 0; h < queue.size(); ++h) {
+            const int nd = queue[h], d = depth[nd];
+            if ((int)v->nodes_at.size() <= d) { v->nodes_at.resize(d + 1, 0); v->leaves_at.resize(d + 1, 0); }
+            ++v->nodes_at[d];
+            if (cnt[nd + 1] == cnt[nd]) ++v->leaves_at[d];
+            for (int c = cnt[nd]; c < cnt[nd + 1]; ++c) { depth[ids[c]] = d + 1; queue.push_back(ids[c]); }
+        }
+    }
     cudaError_t e = cudaGetDevice(&v->device);
     if (e == cudaSuccess) e = v->child_off.upload(cnt.data(), (size_t)(n_nodes + 1) * 4);
     if (e == cudaSuccess) e = v->child_ids.upload(ids.data(), (size_t)(n_nodes - 1) * 4);
@@ -159,6 +173,84 @@ int mcs_bow_vectors(const mcs_vocabulary* voc, const uint8_t* desc, int32_t n, i
     }
     fv_offsets[nf] = (int)order.size();
     *n_fv = nf;
+    return MCS_OK;
+}
+
+int mcs_vocabulary_level_nodes(const mcs_vocabulary* voc, int32_t levelsup, int32_t* n_out) {
+    if (!voc || !n_out) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    // the descent records the node it stands on after L - levelsup steps (the root for <= 0) and the leaf when it ends earlier
+    const int level = std::max(voc->L - levelsup, 0), depths = (int)voc->nodes_at.size();
+    int n = level < depths ? voc->nodes_at[level] : 0;
+    for (int d = 0; d < std::min(level, depths); ++d) n += voc->leaves_at[d];
+    *n_out = n;
+    return MCS_OK;
+}
+
+int mcs_bow_vectors_device(const mcs_vocabulary* voc, const mcs_packed_frame* frame, int32_t n_cams, int32_t capacity, int32_t dim,
+                           int32_t levelsup, int32_t max_nodes, int32_t* word_dev, double* weight_dev, int32_t* node_dev,
+                           int32_t* fv_nodes_dev, int32_t* fv_offsets_dev, int32_t* n_fv_dev, int32_t* fv_features_dev,
+                           int32_t* bow_words_dev, double* bow_values_dev, int32_t* n_bow_dev, int32_t* status_dev, void* stream) {
+    if (!voc || !frame || !fv_nodes_dev || !fv_offsets_dev || !n_fv_dev || !fv_features_dev || !bow_words_dev || !bow_values_dev ||
+        !n_bow_dev || !status_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, frame, nullptr)) return rc;
+    if (dim != 32) return mcs_fail(MCS_ERR_UNSUPPORTED, "the vocabulary works on 32-byte descriptors (FORB::L)");
+    if (max_nodes < 1) return mcs_fail(MCS_ERR_INVALID, "max_nodes must be positive");
+    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    int cur = -1;
+    CUDA_CHECK(cudaGetDevice(&cur));
+    if (cur != voc->device) return mcs_fail(MCS_ERR_INVALID, "vocabulary was created on another CUDA device than the current one");
+    cudaStream_t st = (cudaStream_t)stream;
+    const std::vector<PsCamSlots> slots = packed_slots(*frame, n_cams, capacity, dim);
+    BowVectorsDevArgs a{};
+    a.n_cams = n_cams; a.capacity = capacity; a.levelsup = levelsup; a.max_nodes = max_nodes;
+    a.n_words = voc->n_words; a.scoring = voc->scoring; a.weighting = voc->weighting;
+    a.cams = slots.data();
+    a.word = word_dev; a.weight = weight_dev; a.node = node_dev;
+    a.fv_nodes = fv_nodes_dev; a.fv_offsets = fv_offsets_dev; a.n_fv = n_fv_dev; a.fv_features = fv_features_dev;
+    a.bow_words = bow_words_dev; a.bow_values = bow_values_dev; a.n_bow = n_bow_dev; a.status = status_dev;
+    CUDA_CHECK(launch_bow_vectors_device(voc->view, a, st));
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
+    return MCS_OK;
+}
+
+int mcs_search_by_bow_device(const mcs_bow_frame* kfs, int32_t n_kf, const mcs_bow_frame* cur, int32_t n_cams, int32_t capacity,
+                             int32_t dim, int32_t max_nodes, int32_t n_points, const uint8_t* bad_dev, int32_t th_low, double nnratio,
+                             int32_t having_masks, int32_t* match_mp_dev, int32_t* match_slot_dev, int32_t* nmatches_dev,
+                             int32_t* status_dev, void* stream) {
+    if (n_kf < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (n_kf == 0) return MCS_OK;
+    if (!kfs || !cur || !match_mp_dev || !nmatches_dev || !status_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, &cur->frame, nullptr)) return rc;
+    if (max_nodes < 1 || n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (!cur->fv_nodes_dev || !cur->fv_offsets_dev || !cur->n_fv_dev || !cur->fv_features_dev)
+        return mcs_fail(MCS_ERR_INVALID, "current frame: null feature vector");
+    for (int k = 0; k < n_kf; ++k) {
+        if (!packed_frame_ok(&kfs[k].frame, n_cams))
+            return mcs_fail(MCS_ERR_INVALID, "key frame " + std::to_string(k) + ": no buffer, or first_image + n_cams exceeds its images");
+        if (!kfs[k].fv_nodes_dev || !kfs[k].fv_offsets_dev || !kfs[k].n_fv_dev || !kfs[k].fv_features_dev || !kfs[k].mp_dev)
+            return mcs_fail(MCS_ERR_INVALID, "key frame " + std::to_string(k) + ": null feature vector or map-point array");
+    }
+    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_CHECK(keep_pool_memory());
+    std::vector<PsCamSlots> kslots;
+    std::vector<BowFrameDev> kdev(n_kf);
+    kslots.reserve((size_t)n_kf * n_cams);
+    for (int k = 0; k < n_kf; ++k) {
+        const std::vector<PsCamSlots> s = packed_slots(kfs[k].frame, n_cams, capacity, dim);
+        kslots.insert(kslots.end(), s.begin(), s.end());
+        kdev[k] = BowFrameDev{kfs[k].fv_nodes_dev, kfs[k].fv_offsets_dev, kfs[k].n_fv_dev, kfs[k].fv_features_dev, kfs[k].mp_dev};
+    }
+    const std::vector<PsCamSlots> cslots = packed_slots(cur->frame, n_cams, capacity, dim);
+    BowSearchDevArgs a{};
+    a.n_kf = n_kf; a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.max_nodes = max_nodes; a.n_points = n_points;
+    a.th_low = th_low; a.nnratio = nnratio; a.masked = having_masks != 0;
+    a.kf_cams = kslots.data(); a.cur_cams = cslots.data(); a.kfs = kdev.data();
+    a.cur = BowFrameDev{cur->fv_nodes_dev, cur->fv_offsets_dev, cur->n_fv_dev, cur->fv_features_dev, nullptr};
+    a.bad = bad_dev; a.match_mp = match_mp_dev; a.match_slot = match_slot_dev; a.nmatches = nmatches_dev; a.status = status_dev;
+    CUDA_CHECK(launch_search_by_bow_device(a, st));
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
     return MCS_OK;
 }
 

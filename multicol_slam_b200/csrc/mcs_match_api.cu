@@ -15,6 +15,7 @@
 #include "kernels.h"
 #include "dev_scratch.h"
 #include "mcs_common.cuh"
+#include "packed_frame.h"
 
 using namespace mcs;
 
@@ -594,43 +595,6 @@ int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const d
 }
 
 int mcs_search_by_projection_max_rounds(void) { return proj_search_max_rounds(); }
-
-}  // extern "C"
-
-namespace {
-// camera c of a packed frame = global image first_image + c = image (g mod part_images) of part g / part_images
-std::vector<PsCamSlots> packed_slots(const mcs_packed_frame& fr, int n_cams, int capacity, int dim) {
-    size_t off[4];
-    const size_t part_bytes = mcs_packed_layout(fr.part_images, capacity, dim, off);
-    std::vector<PsCamSlots> slots(n_cams);
-    for (int c = 0; c < n_cams; ++c) {
-        const int g = fr.first_image + c, p = g / fr.part_images, i = g - p * fr.part_images;
-        const uint8_t* b = (const uint8_t*)fr.packed_dev + (size_t)p * part_bytes;
-        slots[c] = PsCamSlots{(const int*)(b + off[0]) + i, (const mcs_keypoint*)(b + off[1]) + (size_t)i * capacity,
-                              b + off[2] + (size_t)i * capacity * dim, b + off[3] + (size_t)i * capacity * dim};
-    }
-    return slots;
-}
-
-bool packed_frame_ok(const mcs_packed_frame* fr, int n_cams) {
-    return fr->packed_dev && fr->n_parts >= 1 && fr->part_images >= 1 && fr->first_image >= 0 &&
-           (long long)fr->first_image + n_cams <= (long long)fr->n_parts * fr->part_images;
-}
-
-// the arguments of the frame the device searches search, and of the packed feature buffers the images of its cameras come from
-// (`last`: the searches between two frames only)
-int check_packed_frames(int n_cams, int capacity, int dim, const mcs_packed_frame* cur, const mcs_packed_frame* last) {
-    if (n_cams < 1) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
-    if (capacity < 1 || capacity > 65535) return mcs_fail(MCS_ERR_INVALID, "capacity must be 1..65535");
-    if (int rc = check_desc_dim(dim)) return rc;
-    if (!packed_frame_ok(cur, n_cams)) return mcs_fail(MCS_ERR_INVALID, "current frame: no buffer, or first_image + n_cams exceeds its images");
-    if (last && !packed_frame_ok(last, n_cams))
-        return mcs_fail(MCS_ERR_INVALID, "last frame: no buffer, or first_image + n_cams exceeds its images");
-    return MCS_OK;
-}
-}  // namespace
-
-extern "C" {
 
 int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int32_t part_images, int32_t first_image, int32_t n_cams,
                                     int32_t capacity, int32_t dim, const int32_t* cam_width, const int32_t* cam_height, int32_t n_levels,

@@ -1,0 +1,43 @@
+// packed_frame.h -- a frame in packed feature buffers (mcs_packed_frame), as the host entry points of the device searches
+// (mcs_match_api.cu) and of the device bag of words (mcs_bow_api.cu) read it: the per-camera section pointers, and the argument
+// checks the calls share.
+#pragma once
+#include <vector>
+#include "../../include/mcs_b200.h"
+#include "api_check.h"
+#include "kernels.h"
+
+namespace mcs {
+
+// camera c of a packed frame = global image first_image + c = image (g mod part_images) of part g / part_images
+inline std::vector<PsCamSlots> packed_slots(const mcs_packed_frame& fr, int n_cams, int capacity, int dim) {
+    size_t off[4];
+    const size_t part_bytes = mcs_packed_layout(fr.part_images, capacity, dim, off);
+    std::vector<PsCamSlots> slots(n_cams);
+    for (int c = 0; c < n_cams; ++c) {
+        const int g = fr.first_image + c, p = g / fr.part_images, i = g - p * fr.part_images;
+        const uint8_t* b = (const uint8_t*)fr.packed_dev + (size_t)p * part_bytes;
+        slots[c] = PsCamSlots{(const int*)(b + off[0]) + i, (const mcs_keypoint*)(b + off[1]) + (size_t)i * capacity,
+                              b + off[2] + (size_t)i * capacity * dim, b + off[3] + (size_t)i * capacity * dim};
+    }
+    return slots;
+}
+
+inline bool packed_frame_ok(const mcs_packed_frame* fr, int n_cams) {
+    return fr->packed_dev && fr->n_parts >= 1 && fr->part_images >= 1 && fr->first_image >= 0 &&
+           (long long)fr->first_image + n_cams <= (long long)fr->n_parts * fr->part_images;
+}
+
+// the arguments of the frame the device searches search, and of the packed feature buffers the images of its cameras come from
+// (`last`: the searches between two frames only)
+inline int check_packed_frames(int n_cams, int capacity, int dim, const mcs_packed_frame* cur, const mcs_packed_frame* last) {
+    if (n_cams < 1) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (capacity < 1 || capacity > 65535) return mcs_fail(MCS_ERR_INVALID, "capacity must be 1..65535");
+    if (int rc = check_desc_dim(dim)) return rc;
+    if (!packed_frame_ok(cur, n_cams)) return mcs_fail(MCS_ERR_INVALID, "current frame: no buffer, or first_image + n_cams exceeds its images");
+    if (last && !packed_frame_ok(last, n_cams))
+        return mcs_fail(MCS_ERR_INVALID, "last frame: no buffer, or first_image + n_cams exceeds its images");
+    return MCS_OK;
+}
+
+}  // namespace mcs

@@ -52,6 +52,13 @@ class PackedFrame(C.Structure):
     _fields_ = [("packed_dev", C.c_void_p), ("n_parts", C.c_int32), ("part_images", C.c_int32), ("first_image", C.c_int32)]
 
 
+class BowFrame(C.Structure):
+    """mcs_bow_frame: a frame in packed feature buffers with its FeatureVector (CSR, slots) and, for a key frame, its slot-indexed
+    map-point ids, all device pointers"""
+    _fields_ = [("frame", PackedFrame), ("fv_nodes_dev", C.c_void_p), ("fv_offsets_dev", C.c_void_p), ("n_fv_dev", C.c_void_p),
+                ("fv_features_dev", C.c_void_p), ("mp_dev", C.c_void_p)]
+
+
 def set_prototypes(lib):
     """argument types of the entry points whose many arguments are easiest to get wrong from Python"""
     P, I, D = C.c_void_p, C.c_int32, C.c_double
@@ -63,6 +70,15 @@ def set_prototypes(lib):
     f.restype = C.c_int
     f = lib.mcs_search_by_projection_frames_device
     f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, P, P, I, P, P, I, D, I, I, P, P, P, P, P]
+    f.restype = C.c_int
+    f = lib.mcs_vocabulary_level_nodes
+    f.argtypes = [P, I, C.POINTER(I)]
+    f.restype = C.c_int
+    f = lib.mcs_bow_vectors_device
+    f.argtypes = [P, C.POINTER(PackedFrame), I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P]
+    f.restype = C.c_int
+    f = lib.mcs_search_by_bow_device
+    f.argtypes = [C.POINTER(BowFrame), I, C.POINTER(BowFrame), I, I, I, I, I, P, I, D, I, P, P, P, P, P]
     f.restype = C.c_int
 
 

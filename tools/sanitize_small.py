@@ -17,4 +17,20 @@ idx, dist = api.hamming_topk(d, d[::-1].copy(), 2, m, m[::-1].copy())
 F = api.Frame.from_cameras([(k, d, m)], [(333, 211)], [ex.info.scale_factor[l] for l in range(4)])
 prev = np.stack([k["x"], k["y"]], 1).astype(np.float64)
 n, m12 = api.cORBmatcher(0.9, False, 32, True).SearchForInitialization(F, F, prev, 30)
-print("sanitize_small ok", len(k), n)
+# relocalisation's bag-of-words step on the device: the frame packed twice (key frame and current frame of one buffer), ComputeBoW
+# on each (the segment placement), then the search of the frame against itself (the taken flags inside a warp)
+import torch
+from multicol_slam_b200 import rig
+cap = len(k) + 3
+packed = torch.from_numpy(rig.pack([(k, d, m), (k, d, m)], cap, 32)).cuda()
+voc = api.ORBVocabulary(np.load(ROOT / "tests" / "golden" / "voc_small_9_6.npz"))
+bows = [voc.transform_device((packed, 1, 2, f), 1, cap) for f in range(2)]
+bw, bv, (fn, fo, ff) = bows[1].host()
+hw, hv, (hn, ho, hf) = voc.transform(d)
+assert np.array_equal(bw, hw) and np.array_equal(bv, hv) and np.array_equal(fn, hn) and np.array_equal(fo, ho) and np.array_equal(ff, hf)
+mp_t = torch.arange(cap, dtype=torch.int32, device="cuda")
+mt = api.cORBmatcher(0.9, False, 32, True)
+mmp, msl, nm, st = mt.SearchByBoWDevice([(bows[0], mp_t)], bows[1], cap)
+nh, mh = mt.SearchByBoWFrame(d, (hn, ho, hf), d, (hn, ho, hf), m, m)
+assert int(st.item()) == 0 and int(nm[0].item()) == nh and np.array_equal(msl[0, :len(k)].cpu().numpy(), mh)
+print("sanitize_small ok", len(k), n, nh)
