@@ -695,6 +695,24 @@ def _predict_level(scale_factors, ratio):
     return min(int(np.searchsorted(scale_factors, ratio, side="left")), len(scale_factors) - 1)
 
 
+def _packed_pair(cur, last):
+    """the mcs_packed_frame records, by reference, of cur / last = (packed uint8 cuda tensor, n_parts, part_images, first_image)"""
+    return [C.byref(PackedFrame(f[0].data_ptr(), *f[1:4])) for f in (cur, last)]
+
+
+def _search_outputs(out, diag, stream, dev):
+    """(nmatches [1], status [1], diag [4]) int32 cuda tensors, `out` or new, and the call's last four arguments (diag NULL unless asked)"""
+    if out is None:
+        import torch
+        out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
+    return out, (_dptr(out[0]), _dptr(out[1]), _dptr(out[2]) if diag else None, _stream_handle(stream, dev))
+
+
+def _search_result(out, frame_mp_t, diag):
+    """(nmatches, status, frame_mp_t), plus diag when it is asked for"""
+    return (out[0], out[1], frame_mp_t) + ((out[2],) if diag else ())
+
+
 class cORBmatcher:
     """ref include/cORBmatcher.h:55-178; thresholds as in src/cORBmatcher.cpp:46-64."""
 
@@ -723,20 +741,16 @@ class cORBmatcher:
         n_parts layouts of part_images images; camera c = image first_image + c) and the map points in a MapPointsDevice.  frame_mp_t:
         int32 cuda tensor [n_cams * capacity] indexed by slot, updated in place.  Asynchronous on `stream`.  Returns (nmatches [1],
         status [1], frame_mp_t), plus diag [4] when diag is set, as cuda tensors."""
-        import torch
-        dev = packed_t.device
         dim = mps_dev.desc.shape[1]
         cw = np.ascontiguousarray([s[0] for s in cam_sizes], np.int32)
         ch = np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
         sf = np.ascontiguousarray(scale_factors, np.float64)
-        if out is None:
-            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
+        out, tail = _search_outputs(out, diag, stream, packed_t.device)
         mv = mps_dev.view()
         _check(lib().mcs_search_by_projection_device(_dptr(packed_t), n_parts, part_images, first_image, n_cams, capacity, dim, _p(cw), _p(ch),
                                                      len(sf), _p(sf), C.byref(mv), C.c_double(th), C.c_double(self.mfNNratio), self.TH_HIGH_,
-                                                     int(self.havingMasks), _dptr(frame_mp_t), _dptr(out[0]), _dptr(out[1]),
-                                                     _dptr(out[2]) if diag else None, _stream_handle(stream, dev)))
-        return (out[0], out[1], frame_mp_t) + ((out[2],) if diag else ())
+                                                     int(self.havingMasks), _dptr(frame_mp_t), *tail))
+        return _search_result(out, frame_mp_t, diag)
 
     def SearchByProjectionLastDevice(self, cur, last, capacity, rig_cur, masks_t, scale_factors, last_mp_t, world_t, th, cur_mp_t,
                                      bad_t=None, last_outlier_t=None, stream=None, out=None, diag=False):
@@ -747,21 +761,16 @@ class cORBmatcher:
         slot (-1 none), cur_mp_t updated in place; world_t [n_points,3] f64 cuda; bad_t [n_points] / last_outlier_t [n_cams *
         capacity] u8 cuda or None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4] when
         diag is set, as cuda tensors."""
-        import torch
-        fc, fl = (PackedFrame(f[0].data_ptr(), *f[1:4]) for f in (cur, last))
-        dev = cur[0].device
         nc = len(rig_cur.cams)
         ocs = (Ocam * nc)(*[as_ocam(c) for c in rig_cur.cams])
         sf = np.ascontiguousarray(scale_factors, np.float64)
         mi = np.ascontiguousarray(rig_cur.MtMc_inv, np.float64)
-        if out is None:
-            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
-        _check(lib().mcs_search_by_projection_last_device(C.byref(fc), C.byref(fl), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t), len(sf),
+        out, tail = _search_outputs(out, diag, stream, cur[0].device)
+        _check(lib().mcs_search_by_projection_last_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t), len(sf),
                                                           _p(sf), _p(mi), _dptr(last_mp_t), _dptr(last_outlier_t), world_t.shape[0],
                                                           _dptr(world_t), _dptr(bad_t), th, self.TH_HIGH_, int(self.havingMasks),
-                                                          _dptr(cur_mp_t), _dptr(out[0]), _dptr(out[1]), _dptr(out[2]) if diag else None,
-                                                          _stream_handle(stream, dev)))
-        return (out[0], out[1], cur_mp_t) + ((out[2],) if diag else ())
+                                                          _dptr(cur_mp_t), *tail))
+        return _search_result(out, cur_mp_t, diag)
 
     def WindowSearchDevice(self, cur, last, capacity, cam_sizes, last_mp_t, window, cur_mp_t, min_level=0, max_level=2**31 - 1, bad_t=None,
                            stream=None, out=None, diag=False):
@@ -771,20 +780,15 @@ class cORBmatcher:
         overwritten (every slot below a camera's count starts at -1); bad_t [n_points] u8 cuda or None, n_points = len(bad_t) or
         every id when None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4] when diag is set,
         as cuda tensors."""
-        import torch
-        fc, fl = (PackedFrame(f[0].data_ptr(), *f[1:4]) for f in (cur, last))
-        dev = cur[0].device
         nc = len(cam_sizes)
         cw = np.ascontiguousarray([s[0] for s in cam_sizes], np.int32)
         ch = np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
         n_points = bad_t.shape[0] if bad_t is not None else 2**31 - 1
-        if out is None:
-            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
-        _check(lib().mcs_window_search_device(C.byref(fc), C.byref(fl), nc, capacity, self.mbFeatDim, _p(cw), _p(ch), _dptr(last_mp_t),
+        out, tail = _search_outputs(out, diag, stream, cur[0].device)
+        _check(lib().mcs_window_search_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, _p(cw), _p(ch), _dptr(last_mp_t),
                                               n_points, _dptr(bad_t), int(window), int(min_level), int(max_level), self.mfNNratio,
-                                              self.TH_HIGH_, int(self.havingMasks), _dptr(cur_mp_t), _dptr(out[0]), _dptr(out[1]),
-                                              _dptr(out[2]) if diag else None, _stream_handle(stream, dev)))
-        return (out[0], out[1], cur_mp_t) + ((out[2],) if diag else ())
+                                              self.TH_HIGH_, int(self.havingMasks), _dptr(cur_mp_t), *tail))
+        return _search_result(out, cur_mp_t, diag)
 
     def SearchByProjectionFramesDevice(self, cur, last, capacity, rig_cur, masks_t, last_mp_t, world_t, window, cur_mp_t, bad_t=None,
                                        stream=None, out=None, diag=False):
@@ -794,20 +798,15 @@ class cORBmatcher:
         map-point ids by slot (-1 none), cur_mp_t updated in place (its entries are "already found"); world_t [n_points,3] f64 cuda;
         bad_t [n_points] u8 cuda or None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4]
         when diag is set, as cuda tensors."""
-        import torch
-        fc, fl = (PackedFrame(f[0].data_ptr(), *f[1:4]) for f in (cur, last))
-        dev = cur[0].device
         nc = len(rig_cur.cams)
         ocs = (Ocam * nc)(*[as_ocam(c) for c in rig_cur.cams])
         mi = np.ascontiguousarray(rig_cur.MtMc_inv, np.float64)
-        if out is None:
-            out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 1, 4))
-        _check(lib().mcs_search_by_projection_frames_device(C.byref(fc), C.byref(fl), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t),
+        out, tail = _search_outputs(out, diag, stream, cur[0].device)
+        _check(lib().mcs_search_by_projection_frames_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t),
                                                             _p(mi), _dptr(last_mp_t), world_t.shape[0], _dptr(world_t), _dptr(bad_t),
                                                             int(window), self.mfNNratio, self.TH_HIGH_, int(self.havingMasks),
-                                                            _dptr(cur_mp_t), _dptr(out[0]), _dptr(out[1]), _dptr(out[2]) if diag else None,
-                                                            _stream_handle(stream, dev)))
-        return (out[0], out[1], cur_mp_t) + ((out[2],) if diag else ())
+                                                            _dptr(cur_mp_t), *tail))
+        return _search_result(out, cur_mp_t, diag)
 
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
         """ref :579-726.  vbPrevMatched [n1,2] float64 updated in place.  Returns (nmatches, vnMatches12)."""

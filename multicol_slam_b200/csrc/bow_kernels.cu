@@ -104,15 +104,13 @@ group_distance_kernel(const GroupQuery* __restrict__ queries, const int nq, cons
 cudaError_t launch_group_distance(const GroupQuery* queries, int nq, const uint8_t* desc1, const uint8_t* mask1, const uint8_t* desc2,
                                   const uint8_t* mask2, const int* cand, int dim, int* out, cudaStream_t st) {
     if (nq <= 0) return cudaSuccess;
+    if (dim != 16 && dim != 32 && dim != 64) return cudaErrorInvalidValue;
     const int blocks = (int)(((long long)nq * 32 + 255) / 256);
     const bool masked = mask1 && mask2;
-#define MCS_GD(W, M) group_distance_kernel<W, M><<<blocks, 256, 0, st>>>(queries, nq, (const uint32_t*)desc1, (const uint32_t*)mask1, \
-        (const uint32_t*)desc2, (const uint32_t*)mask2, cand, out)
-    if (dim == 16) { if (masked) MCS_GD(4, true); else MCS_GD(4, false); }
-    else if (dim == 32) { if (masked) MCS_GD(8, true); else MCS_GD(8, false); }
-    else if (dim == 64) { if (masked) MCS_GD(16, true); else MCS_GD(16, false); }
-    else return cudaErrorInvalidValue;
-#undef MCS_GD
+    with_desc_width(dim, masked, [&](auto W, auto M) {
+        group_distance_kernel<W, M><<<blocks, 256, 0, st>>>(queries, nq, (const uint32_t*)desc1, (const uint32_t*)mask1, (const uint32_t*)desc2,
+                                                            (const uint32_t*)mask2, cand, out);
+    });
     return cudaGetLastError();
 }
 
@@ -326,8 +324,6 @@ bv_normalize_kernel(double* __restrict__ vals, const int* __restrict__ n_bow, co
         for (int i = threadIdx.x; i < nb; i += blockDim.x) vals[i] /= nrm;
 }
 
-inline size_t bv_align(size_t b) { return (b + 255) & ~(size_t)255; }
-
 }  // namespace
 
 cudaError_t launch_bow_vectors_device(const VocabularyDev& v, const BowVectorsDevArgs& a, cudaStream_t st) {
@@ -336,22 +332,16 @@ cudaError_t launch_bow_vectors_device(const VocabularyDev& v, const BowVectorsDe
     const int tiles_n = (v.n_nodes + kBvTile - 1) / kBvTile, tiles_w = (a.n_words + kBvTile - 1) / kBvTile;
     const int max_tiles = tiles_n > tiles_w ? tiles_n : tiles_w;
     // the three cleared arrays first, in one block
-    const size_t sizes[] = {4ull * v.n_nodes, 4ull * a.n_words, 4ull * n_fill,                       // cnt_node cnt_word fill
-                            sizeof(PsCamSlots) * a.n_cams, 4ull * NS, 8ull * NS, 4ull * a.n_words,   // cams key_node wt word_rep
-                            4ull * NS, 4ull * NS, 16ull * max_tiles};                               // slot_rank unordered tile_sums
-    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
-    size_t off[nsz], total = 0;
-    for (int i = 0; i < nsz; ++i) { off[i] = total; total += bv_align(sizes[i]); }
-    cudaError_t e = keep_pool_memory();
+    StreamScratch sc;
+    cudaError_t e = sc.alloc({4ull * v.n_nodes, 4ull * a.n_words, 4ull * n_fill,                       // cnt_node cnt_word fill
+                              sizeof(PsCamSlots) * a.n_cams, 4ull * NS, 8ull * NS, 4ull * a.n_words,   // cams key_node wt word_rep
+                              4ull * NS, 4ull * NS, 16ull * max_tiles},                               // slot_rank unordered tile_sums
+                             st);
     if (e != cudaSuccess) return e;
-    uint8_t* base = nullptr;
-    e = cudaMallocAsync((void**)&base, total, st);
-    if (e != cudaSuccess) return e;
-    auto at = [&](int i) { return (void*)(base + off[i]); };
-    int* cnt_node = (int*)at(0); int* cnt_word = (int*)at(1); int* fill = (int*)at(2);
-    PsCamSlots* cams = (PsCamSlots*)at(3); int* key_node = (int*)at(4); double* wt = (double*)at(5); int* word_rep = (int*)at(6);
-    int* slot_rank = (int*)at(7); int* unordered = (int*)at(8); unsigned long long* tile_sums = (unsigned long long*)at(9);
-    e = cudaMemsetAsync(base, 0, off[3], st);
+    int* cnt_node = sc.at<int>(0); int* cnt_word = sc.at<int>(1); int* fill = sc.at<int>(2);
+    PsCamSlots* cams = sc.at<PsCamSlots>(3); int* key_node = sc.at<int>(4); double* wt = sc.at<double>(5); int* word_rep = sc.at<int>(6);
+    int* slot_rank = sc.at<int>(7); int* unordered = sc.at<int>(8); unsigned long long* tile_sums = sc.at<unsigned long long>(9);
+    e = cudaMemsetAsync(cnt_node, 0, sc.at<uint8_t>(3) - sc.at<uint8_t>(0), st);
     if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
     if (e == cudaSuccess) e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, cams, st);
     if (e == cudaSuccess) {
@@ -369,8 +359,7 @@ cudaError_t launch_bow_vectors_device(const VocabularyDev& v, const BowVectorsDe
         bv_normalize_kernel<<<1, 256, 0, st>>>(a.bow_values, a.n_bow, a.scoring, accumulate);
         e = cudaGetLastError();
     }
-    const cudaError_t ef = cudaFreeAsync(base, st);
-    return e != cudaSuccess ? e : ef;
+    return sc.release(e);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -510,36 +499,26 @@ __global__ void __launch_bounds__(256) bs_search_kernel(const BowSearchDev a) {
 
 cudaError_t launch_search_by_bow_device(const BowSearchDevArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
-    const size_t sizes[] = {sizeof(PsCamSlots) * a.n_cams * (size_t)a.n_kf, sizeof(PsCamSlots) * a.n_cams, sizeof(BowFrameDev) * a.n_kf};
-    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
-    size_t off[nsz], total = 0;
-    for (int i = 0; i < nsz; ++i) { off[i] = total; total += bv_align(sizes[i]); }
-    cudaError_t e = keep_pool_memory();
+    const size_t b_kf = sizeof(PsCamSlots) * a.n_cams * (size_t)a.n_kf, b_cur = sizeof(PsCamSlots) * a.n_cams, b_fv = sizeof(BowFrameDev) * a.n_kf;
+    StreamScratch sc;
+    cudaError_t e = sc.alloc({b_kf, b_cur, b_fv}, st);
     if (e != cudaSuccess) return e;
-    uint8_t* base = nullptr;
-    e = cudaMallocAsync((void**)&base, total, st);
-    if (e != cudaSuccess) return e;
-    BowSearchDev d{a.n_kf, a.n_cams, a.capacity, a.max_nodes, a.n_points, a.th_low, a.nnratio,
-                   (const PsCamSlots*)(base + off[0]), (const PsCamSlots*)(base + off[1]), (const BowFrameDev*)(base + off[2]), a.cur,
+    PsCamSlots* kf_cams = sc.at<PsCamSlots>(0); PsCamSlots* cur_cams = sc.at<PsCamSlots>(1); BowFrameDev* kfs = sc.at<BowFrameDev>(2);
+    BowSearchDev d{a.n_kf, a.n_cams, a.capacity, a.max_nodes, a.n_points, a.th_low, a.nnratio, kf_cams, cur_cams, kfs, a.cur,
                    a.bad, a.match_mp, a.match_slot, a.nmatches, a.status};
-    e = stage_to_device(a.kf_cams, sizes[0], base + off[0], st);
-    if (e == cudaSuccess) e = stage_to_device(a.cur_cams, sizes[1], base + off[1], st);
-    if (e == cudaSuccess) e = stage_to_device(a.kfs, sizes[2], base + off[2], st);
+    e = stage_to_device(a.kf_cams, b_kf, kf_cams, st);
+    if (e == cudaSuccess) e = stage_to_device(a.cur_cams, b_cur, cur_cams, st);
+    if (e == cudaSuccess) e = stage_to_device(a.kfs, b_fv, kfs, st);
     if (e == cudaSuccess) {
         const long long cells = (long long)a.n_kf * NS, items = (long long)a.n_kf * a.max_nodes;
         bs_clear_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(d);
         // a warp per (key frame, node) up to a grid that fills the device several times over; beyond it the warps stride
         const long long blocks = (items + 7) / 8;
         const unsigned grid = (unsigned)(blocks < 16384 ? blocks : 16384);
-#define MCS_BS(W, M) bs_search_kernel<W, M><<<grid, 256, 0, st>>>(d)
-        if (a.dim == 16) { if (a.masked) MCS_BS(4, true); else MCS_BS(4, false); }
-        else if (a.dim == 32) { if (a.masked) MCS_BS(8, true); else MCS_BS(8, false); }
-        else { if (a.masked) MCS_BS(16, true); else MCS_BS(16, false); }
-#undef MCS_BS
+        with_desc_width(a.dim, a.masked, [&](auto W, auto M) { bs_search_kernel<W, M><<<grid, 256, 0, st>>>(d); });
         e = cudaGetLastError();
     }
-    const cudaError_t ef = cudaFreeAsync(base, st);
-    return e != cudaSuccess ? e : ef;
+    return sc.release(e);
 }
 
 }  // namespace mcs

@@ -60,6 +60,33 @@ inline cudaError_t keep_pool_memory() {
     return e;
 }
 
+// One stream-ordered scratch block cut into pieces, each starting on a 256-byte boundary; a size of 0 gives a zero-length piece.
+class StreamScratch {
+public:
+    // keep_pool_memory(), then one cudaMallocAsync on `st` holding every piece
+    cudaError_t alloc(const std::vector<size_t>& sizes, cudaStream_t st) {
+        off_.assign(1, 0);
+        for (const size_t b : sizes) off_.push_back(off_.back() + ((b + 255) & ~(size_t)255));
+        cudaError_t e = keep_pool_memory();
+        if (e != cudaSuccess) return e;
+        st_ = st;
+        return cudaMallocAsync((void**)&base_, off_.back(), st);
+    }
+    template <class T> T* at(size_t i) const { return (T*)(base_ + off_[i]); }
+    // frees the block in stream order, if alloc made one; returns e, or the free's error when e is cudaSuccess
+    cudaError_t release(const cudaError_t e) {
+        if (!base_) return e;
+        const cudaError_t ef = cudaFreeAsync(base_, st_);
+        base_ = nullptr;
+        return e != cudaSuccess ? e : ef;
+    }
+
+private:
+    std::vector<size_t> off_;
+    uint8_t* base_ = nullptr;
+    cudaStream_t st_ = nullptr;
+};
+
 inline unsigned greedy_dist_bound(int th_low, double nnratio) {
     if (th_low <= 0) return 0u;                      // nothing can be accepted
     long b = th_low;
@@ -128,30 +155,27 @@ struct ProjSearchArgs : PsFrameArgs {   // SearchByProjection(F, vpMapPoints, th
     double th, nnratio;
 };
 cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st);
-struct ProjSearchLastArgs : PsFrameArgs {   // SearchByProjection(CurrentFrame, LastFrame, th): the frame searched is CurrentFrame
-    const PsCamSlots* last;                                  // host [n_cams]: LastFrame's image slots
-    const mcs_ocam* models; const double* mtmc_inv;          // host [n_cams], [n_cams * 16] (the current pose)
-    const uint8_t* masks;                                    // device [n_cams][h][w] level-0 mirror masks
+// The searches between two frames: the frame searched (PsFrameArgs) is the current one, the queries come from the last frame.
+struct PsTwoFrameArgs : PsFrameArgs {
+    const PsCamSlots* last;                                  // host [n_cams]: the last frame's image slots
     int n_points;
-    const int* last_mp; const uint8_t* last_outlier;         // device [n_cams * capacity], slot-indexed (outlier may be NULL)
-    const double* world_pos; const uint8_t* bad;             // device [n_points * 3], [n_points] (bad may be NULL)
+    const int* last_mp; const uint8_t* bad;                  // device, slot-indexed / [n_points] (bad may be NULL)
+    // the current pose, for the searches that project (NULL for WindowSearch)
+    const mcs_ocam* models; const double* mtmc_inv;          // host [n_cams], [n_cams * 16]
+    const uint8_t* masks;                                    // device [n_cams][h][w] level-0 mirror masks
+    const double* world_pos;                                 // device [n_points * 3]
+};
+struct ProjSearchLastArgs : PsTwoFrameArgs {   // SearchByProjection(CurrentFrame, LastFrame, th)
+    const uint8_t* last_outlier;                             // device, slot-indexed (may be NULL)
     double th;
 };
 cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaStream_t st);
 // TrackPreviousFrame's searches, F1 = the last frame, F2 = the frame searched.  Neither reads scale factors (n_levels = 0, sf NULL).
-struct WindowSearchDevArgs : PsFrameArgs {   // WindowSearch(F1, F2, window, ., min_level, max_level): frame_mp is an output
-    const PsCamSlots* last;                                  // host [n_cams]: F1's image slots
-    int n_points;
-    const int* last_mp; const uint8_t* bad;                  // device, slot-indexed / [n_points] (bad may be NULL)
+struct WindowSearchDevArgs : PsTwoFrameArgs {   // WindowSearch(F1, F2, window, ., min_level, max_level): frame_mp is an output
     double window, nnratio; int min_level, max_level;
 };
 cudaError_t launch_window_search_device(const WindowSearchDevArgs& a, cudaStream_t st);
-struct SearchFramesDevArgs : PsFrameArgs {   // SearchByProjection(F1, F2, window, .): frame_mp holds F2.mvpMapPoints on entry
-    const PsCamSlots* last;                                  // host [n_cams]: F1's image slots
-    const mcs_ocam* models; const double* mtmc_inv;          // host [n_cams], [n_cams * 16] (F2's pose)
-    const uint8_t* masks;                                    // device [n_cams][h][w] level-0 mirror masks
-    int n_points;
-    const int* last_mp; const double* world_pos; const uint8_t* bad;   // device (bad may be NULL)
+struct SearchFramesDevArgs : PsTwoFrameArgs {   // SearchByProjection(F1, F2, window, .): frame_mp holds F2.mvpMapPoints on entry
     double window, nnratio;
 };
 cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cudaStream_t st);

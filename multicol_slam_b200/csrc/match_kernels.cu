@@ -416,14 +416,14 @@ cudaError_t launch_hamming_topk(const uint8_t* q, const uint8_t* qmask, int nq, 
     if (e != cudaSuccess) return e;
     dim3 grid(qblocks, splits);
     const bool masked = qmask && dmask;
-#define MCS_TOPK2(W, M, KT) hamming_topk_kernel<W, M, KT><<<grid, kTopkThreads, 0, st>>>((const uint32_t*)q, (const uint32_t*)qmask, nq, \
-        (const uint32_t*)d, (const uint32_t*)dmask, nd, db_skip, K, chunk, bound, g_part)
-#define MCS_TOPK(W, M) { if (K <= 4) MCS_TOPK2(W, M, 4); else MCS_TOPK2(W, M, 8); }
-    if (dim == 16) { if (masked) MCS_TOPK(4, true) else MCS_TOPK(4, false) }
-    else if (dim == 32) { if (masked) MCS_TOPK(8, true) else MCS_TOPK(8, false) }
-    else { if (masked) MCS_TOPK(16, true) else MCS_TOPK(16, false) }
-#undef MCS_TOPK2
-#undef MCS_TOPK
+    with_desc_width(dim, masked, [&](auto W, auto M) {
+        const auto* q32 = (const uint32_t*)q;
+        const auto* qm32 = (const uint32_t*)qmask;
+        const auto* d32 = (const uint32_t*)d;
+        const auto* dm32 = (const uint32_t*)dmask;
+        if (K <= 4) hamming_topk_kernel<W, M, 4><<<grid, kTopkThreads, 0, st>>>(q32, qm32, nq, d32, dm32, nd, db_skip, K, chunk, bound, g_part);
+        else hamming_topk_kernel<W, M, 8><<<grid, kTopkThreads, 0, st>>>(q32, qm32, nq, d32, dm32, nd, db_skip, K, chunk, bound, g_part);
+    });
     topk_merge_kernel<<<(nq + 127) / 128, 128, 0, st>>>(g_part, splits, nq, K, topk_idx, topk_dist);
     e = cudaGetLastError();
     const cudaError_t ef = cudaFreeAsync(g_part, st);        // after the merge in stream order
@@ -473,14 +473,14 @@ cudaError_t launch_hamming_stream(const uint8_t* desc, const uint8_t* dmask, con
     if (img_count < 1) return cudaSuccess;
     dim3 grid((capacity + kTopkThreads - 1) / kTopkThreads, img_count);
     const bool masked = dmask != nullptr;
-#define MCS_HS2(W, M, KT) hamming_stream_kernel<W, M, KT><<<grid, kTopkThreads, 0, st>>>((const uint32_t*)desc, (const uint32_t*)dmask, counts, \
-        n_cams, capacity, K, img_lo, bound, out_idx, out_dist)
-#define MCS_HS(W, M) { if (K <= 4) MCS_HS2(W, M, 4); else MCS_HS2(W, M, 8); }
-    if (dim == 16) { if (masked) MCS_HS(4, true) else MCS_HS(4, false) }
-    else if (dim == 32) { if (masked) MCS_HS(8, true) else MCS_HS(8, false) }
-    else { if (masked) MCS_HS(16, true) else MCS_HS(16, false) }
-#undef MCS_HS
-#undef MCS_HS2
+    with_desc_width(dim, masked, [&](auto W, auto M) {
+        const auto* d32 = (const uint32_t*)desc;
+        const auto* m32 = (const uint32_t*)dmask;
+        if (K <= 4)
+            hamming_stream_kernel<W, M, 4><<<grid, kTopkThreads, 0, st>>>(d32, m32, counts, n_cams, capacity, K, img_lo, bound, out_idx, out_dist);
+        else
+            hamming_stream_kernel<W, M, 8><<<grid, kTopkThreads, 0, st>>>(d32, m32, counts, n_cams, capacity, K, img_lo, bound, out_idx, out_dist);
+    });
     return cudaGetLastError();
 }
 
@@ -819,24 +819,18 @@ cudaError_t launch_stream_replay(const int* list_idx, const int* list_dist, cons
     const size_t smem_db = smem + (size_t)capacity * dim * (masked ? 2 : 1) + 16;
     if (n_images <= sms && smem_db <= 200u * 1024u) {
         const void* fn = nullptr;
-#define MCS_SRS(W, M) fn = (const void*)stream_replay_smem_kernel<W, M>
-        if (dim == 16) { if (masked) MCS_SRS(4, true); else MCS_SRS(4, false); }
-        else if (dim == 32) { if (masked) MCS_SRS(8, true); else MCS_SRS(8, false); }
-        else { if (masked) MCS_SRS(16, true); else MCS_SRS(16, false); }
-#undef MCS_SRS
-        e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_db);     // per device, set every time
+        with_desc_width(dim, masked, [&](auto W, auto M) { fn = (const void*)stream_replay_smem_kernel<W, M>; });
+        e =cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_db);     // per device, set every time
         if (e != cudaSuccess) return e;
         const uint32_t *d32 = (const uint32_t*)desc, *m32 = (const uint32_t*)dmask;
         void* args[] = {(void*)&list_idx, (void*)&list_dist, (void*)&counts, (void*)&d32, (void*)&m32, (void*)&n_cams, (void*)&capacity, (void*)&K,
                         (void*)&img_lo, (void*)&th_low, (void*)&nnratio, (void*)&matches12, (void*)&nmatches, (void*)&redo};
         return cudaLaunchKernel(fn, dim3(n_images), dim3(kSmemReplayThreads), args, smem_db, st);
     }
-#define MCS_SR(W, M) stream_replay_kernel<W, M><<<n_images, kReplayThreads, smem, st>>>(list_idx, list_dist, counts, (const uint32_t*)desc, \
-        (const uint32_t*)dmask, n_cams, capacity, K, img_lo, th_low, nnratio, matches12, nmatches, redo)
-    if (dim == 16) { if (masked) MCS_SR(4, true); else MCS_SR(4, false); }
-    else if (dim == 32) { if (masked) MCS_SR(8, true); else MCS_SR(8, false); }
-    else { if (masked) MCS_SR(16, true); else MCS_SR(16, false); }
-#undef MCS_SR
+    with_desc_width(dim, masked, [&](auto W, auto M) {
+        stream_replay_kernel<W, M><<<n_images, kReplayThreads, smem, st>>>(list_idx, list_dist, counts, (const uint32_t*)desc, (const uint32_t*)dmask,
+                                                                         n_cams, capacity, K, img_lo, th_low, nnratio, matches12, nmatches, redo);
+    });
     return cudaGetLastError();
 }
 
@@ -897,11 +891,7 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&coop_ok, cudaDevAttrCooperativeLaunch, dev);
     if (e != cudaSuccess) return e;
     const void* fn = nullptr;
-#define MCS_BR(W, M) fn = (const void*)bruteforce_replay_kernel<W, M>
-    if (dim == 16) { if (masked) MCS_BR(4, true); else MCS_BR(4, false); }
-    else if (dim == 32) { if (masked) MCS_BR(8, true); else MCS_BR(8, false); }
-    else { if (masked) MCS_BR(16, true); else MCS_BR(16, false); }
-#undef MCS_BR
+    with_desc_width(dim, masked, [&](auto W, auto M) { fn = (const void*)bruteforce_replay_kernel<W, M>; });
     if (smem > 48 * 1024) {
         e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -1018,15 +1008,13 @@ cudaError_t launch_window_search(const WindowFrameDev& f, const mcs_window_query
                                  const uint8_t* qmask, int max_cand, int* cand_idx, int* cand_dist, int* cand_count,
                                  cudaStream_t st) {
     if (nq <= 0) return cudaSuccess;
+    if (f.dim != 16 && f.dim != 32 && f.dim != 64) return cudaErrorInvalidValue;
     const int blocks = (nq * 32 + 255) / 256;
     const bool masked = qmask && f.dmask;
-#define MCS_WS(W, M) window_search_kernel<W, M><<<blocks, 256, 0, st>>>(f, q, nq, (const uint32_t*)qdesc, (const uint32_t*)qmask, \
-        max_cand, cand_idx, cand_dist, cand_count)
-    if (f.dim == 16) { if (masked) MCS_WS(4, true); else MCS_WS(4, false); }
-    else if (f.dim == 32) { if (masked) MCS_WS(8, true); else MCS_WS(8, false); }
-    else if (f.dim == 64) { if (masked) MCS_WS(16, true); else MCS_WS(16, false); }
-    else return cudaErrorInvalidValue;
-#undef MCS_WS
+    with_desc_width(f.dim, masked, [&](auto W, auto M) {
+        window_search_kernel<W, M><<<blocks, 256, 0, st>>>(f, q, nq, (const uint32_t*)qdesc, (const uint32_t*)qmask, max_cand, cand_idx,
+                                                           cand_dist, cand_count);
+    });
     return cudaGetLastError();
 }
 

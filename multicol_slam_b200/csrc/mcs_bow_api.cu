@@ -196,7 +196,7 @@ int mcs_bow_vectors_device(const mcs_vocabulary* voc, const mcs_packed_frame* fr
     if (int rc = check_packed_frames(n_cams, capacity, dim, frame, nullptr)) return rc;
     if (dim != 32) return mcs_fail(MCS_ERR_UNSUPPORTED, "the vocabulary works on 32-byte descriptors (FORB::L)");
     if (max_nodes < 1) return mcs_fail(MCS_ERR_INVALID, "max_nodes must be positive");
-    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     int cur = -1;
     CUDA_CHECK(cudaGetDevice(&cur));
     if (cur != voc->device) return mcs_fail(MCS_ERR_INVALID, "vocabulary was created on another CUDA device than the current one");
@@ -210,8 +210,7 @@ int mcs_bow_vectors_device(const mcs_vocabulary* voc, const mcs_packed_frame* fr
     a.fv_nodes = fv_nodes_dev; a.fv_offsets = fv_offsets_dev; a.n_fv = n_fv_dev; a.fv_features = fv_features_dev;
     a.bow_words = bow_words_dev; a.bow_values = bow_values_dev; a.n_bow = n_bow_dev; a.status = status_dev;
     CUDA_CHECK(launch_bow_vectors_device(voc->view, a, st));
-    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
-    return MCS_OK;
+    return sync_if_null_stream(stream);
 }
 
 int mcs_search_by_bow_device(const mcs_bow_frame* kfs, int32_t n_kf, const mcs_bow_frame* cur, int32_t n_cams, int32_t capacity,
@@ -231,7 +230,7 @@ int mcs_search_by_bow_device(const mcs_bow_frame* kfs, int32_t n_kf, const mcs_b
         if (!kfs[k].fv_nodes_dev || !kfs[k].fv_offsets_dev || !kfs[k].n_fv_dev || !kfs[k].fv_features_dev || !kfs[k].mp_dev)
             return mcs_fail(MCS_ERR_INVALID, "key frame " + std::to_string(k) + ": null feature vector or map-point array");
     }
-    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_CHECK(keep_pool_memory());
     std::vector<PsCamSlots> kslots;
@@ -250,8 +249,7 @@ int mcs_search_by_bow_device(const mcs_bow_frame* kfs, int32_t n_kf, const mcs_b
     a.cur = BowFrameDev{cur->fv_nodes_dev, cur->fv_offsets_dev, cur->n_fv_dev, cur->fv_features_dev, nullptr};
     a.bad = bad_dev; a.match_mp = match_mp_dev; a.match_slot = match_slot_dev; a.nmatches = nmatches_dev; a.status = status_dev;
     CUDA_CHECK(launch_search_by_bow_device(a, st));
-    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
-    return MCS_OK;
+    return sync_if_null_stream(stream);
 }
 
 int mcs_bow_score(const mcs_vocabulary* voc, const int32_t* w1, const double* v1, int32_t n1, const int32_t* w2, const double* v2,

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "../../include/mcs_b200.h"
 
 namespace mcs {
@@ -67,6 +68,21 @@ __host__ __device__ inline int reflect101(int p, int n) {
     if (p < 0) p = -p;
     if (p >= n) p = 2 * (n - 1) - p;
     return p;
+}
+
+// The descriptor-width dispatch of the Hamming kernels: calls f(W, M) with W = std::integral_constant<int, dim / 4> (the 32-bit
+// words of a descriptor) and M = std::integral_constant<bool, masked>, so that `kern<W, M>` names one instantiation per width and
+// mask.  Any dim other than 16 and 32 takes the 64-byte path; callers that refuse other widths check dim first.
+template <class F>
+inline void with_desc_width(const int dim, const bool masked, F&& f) {
+    using std::integral_constant;
+    const auto with_mask = [&](auto W) {
+        if (masked) f(W, std::true_type{});
+        else f(W, std::false_type{});
+    };
+    if (dim == 16) with_mask(integral_constant<int, 4>{});
+    else if (dim == 32) with_mask(integral_constant<int, 8>{});
+    else with_mask(integral_constant<int, 16>{});
 }
 
 }  // namespace mcs

@@ -117,6 +117,24 @@ int window_search_compact(const FrameDev& fd, const mcs_window_query* qs, const 
     }
 }
 
+// The PsFrameArgs fields the four device searches fill alike: the frame searched (`cams`: its slots in the packed buffer), its
+// camera sizes, the acceptance threshold and the outputs.  n_levels and sf stay 0 / NULL for the searches that read no scale factor.
+void set_searched_frame(PsFrameArgs& a, const std::vector<PsCamSlots>& cams, int capacity, int dim, const int* cam_w, const int* cam_h,
+                        int th_high, int having_masks, int* frame_mp, int* nmatches, int* status, int* diag) {
+    a.n_cams = (int)cams.size(); a.capacity = capacity; a.dim = dim;
+    a.cams = cams.data(); a.cam_w = cam_w; a.cam_h = cam_h;
+    a.th_high = th_high; a.masked = having_masks != 0;
+    a.frame_mp = frame_mp; a.nmatches = nmatches; a.status = status; a.diag = diag;
+}
+
+// the image sizes of camera models, as the width and height arrays PsFrameArgs and check_cam_sizes read
+struct CamSizes {
+    std::vector<int> w, h;
+    CamSizes(const mcs_ocam* cams, int n) : w(n), h(n) {
+        for (int c = 0; c < n; ++c) { w[c] = cams[c].width; h[c] = cams[c].height; }
+    }
+};
+
 }  // namespace
 
 extern "C" {
@@ -590,8 +608,7 @@ int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const d
     const cudaError_t ef = cudaFreeAsync(d, st);
     CUDA_CHECK(e);
     CUDA_CHECK(ef);
-    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
-    return MCS_OK;
+    return sync_if_null_stream(stream);
 }
 
 int mcs_search_by_projection_max_rounds(void) { return proj_search_max_rounds(); }
@@ -610,23 +627,19 @@ int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int
     if (!mps->in_view || !mps->level || !mps->proj_x || !mps->proj_y || !mps->view_cos || !mps->desc)
         return mcs_fail(MCS_ERR_INVALID, "null map-point array");
     if (having_masks && !mps->dmask) return mcs_fail(MCS_ERR_INVALID, "masks requested but not supplied");
-    for (int c = 0; c < n_cams; ++c)
-        if (cam_width[c] < 1 || cam_height[c] < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
-    if ((long long)mps->n_points * n_cams >= (1LL << 24))
-        return mcs_fail(MCS_ERR_UNSUPPORTED, "more than 2^24 - 1 (map point, camera) entries in one call");
+    if (int rc = check_cam_sizes(n_cams, cam_width, cam_height, false)) return rc;
+    if (int rc = check_query_bound((long long)mps->n_points * n_cams, "more than 2^24 - 1 (map point, camera) entries in one call")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> slots = packed_slots(frame, n_cams, capacity, dim);
     ProjSearchArgs a{};
-    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.n_levels = n_levels; a.n_points = mps->n_points;
-    a.cams = slots.data(); a.cam_w = cam_width; a.cam_h = cam_height; a.sf = scale_factors;
+    set_searched_frame(a, slots, capacity, dim, cam_width, cam_height, th_high, having_masks, frame_mp_dev, nmatches_dev, status_dev, diag_dev);
+    a.n_levels = n_levels; a.sf = scale_factors; a.n_points = mps->n_points;
     a.bad = mps->bad; a.in_view = mps->in_view; a.level = mps->level; a.px = mps->proj_x; a.py = mps->proj_y; a.vcos = mps->view_cos;
     a.mp_desc = mps->desc; a.mp_dmask = having_masks ? mps->dmask : nullptr;
-    a.th = th; a.nnratio = nnratio; a.th_high = th_high; a.masked = having_masks != 0;
-    a.frame_mp = frame_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
+    a.th = th; a.nnratio = nnratio;
     CUDA_CHECK(launch_search_by_projection(a, st));
-    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
-    return MCS_OK;
+    return sync_if_null_stream(stream);
 }
 
 int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity,
@@ -641,28 +654,20 @@ int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_
     if (n_levels < 1 || n_levels > MCS_MAX_LEVELS) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
     if (int rc = check_packed_frames(n_cams, capacity, dim, cur, last)) return rc;
     if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
-    for (int c = 0; c < n_cams; ++c) {
-        if (cams[c].width < 1 || cams[c].height < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
-        if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
-            return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
-    }
-    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    const CamSizes cz(cams, n_cams);
+    if (int rc = check_cam_sizes(n_cams, cz.w.data(), cz.h.data(), true)) return rc;
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
-    std::vector<int> cw(n_cams), ch(n_cams);
-    for (int c = 0; c < n_cams; ++c) { cw[c] = cams[c].width; ch[c] = cams[c].height; }
     ProjSearchLastArgs a{};
-    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.n_levels = n_levels;
-    a.cams = cs.data(); a.cam_w = cw.data(); a.cam_h = ch.data(); a.sf = scale_factors;
-    a.th_high = th_high; a.masked = having_masks != 0;
-    a.frame_mp = cur_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
-    a.last = ls.data(); a.models = cams; a.mtmc_inv = mtmc_inv; a.masks = masks_dev;
-    a.n_points = n_points; a.last_mp = last_mp_dev; a.last_outlier = last_outlier_dev; a.world_pos = world_pos_dev; a.bad = bad_dev;
-    a.th = th;
+    set_searched_frame(a, cs, capacity, dim, cz.w.data(), cz.h.data(), th_high, having_masks, cur_mp_dev, nmatches_dev, status_dev, diag_dev);
+    a.n_levels = n_levels; a.sf = scale_factors;
+    a.last = ls.data(); a.n_points = n_points; a.last_mp = last_mp_dev; a.bad = bad_dev;
+    a.models = cams; a.mtmc_inv = mtmc_inv; a.masks = masks_dev; a.world_pos = world_pos_dev;
+    a.last_outlier = last_outlier_dev; a.th = th;
     CUDA_CHECK(launch_search_by_projection_last(a, st));
-    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
-    return MCS_OK;
+    return sync_if_null_stream(stream);
 }
 
 int mcs_window_search_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity, int32_t dim,
@@ -674,22 +679,17 @@ int mcs_window_search_device(const mcs_packed_frame* cur, const mcs_packed_frame
         return mcs_fail(MCS_ERR_INVALID, "null argument");
     if (int rc = check_packed_frames(n_cams, capacity, dim, cur, last)) return rc;
     if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
-    for (int c = 0; c < n_cams; ++c)
-        if (cam_width[c] < 1 || cam_height[c] < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
-    if ((long long)n_cams * capacity >= (1LL << 24)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity must stay below 2^24");
+    if (int rc = check_cam_sizes(n_cams, cam_width, cam_height, false)) return rc;
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
     WindowSearchDevArgs a{};
-    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim;
-    a.cams = cs.data(); a.cam_w = cam_width; a.cam_h = cam_height;
-    a.th_high = th_high; a.masked = having_masks != 0;
-    a.frame_mp = cur_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
+    set_searched_frame(a, cs, capacity, dim, cam_width, cam_height, th_high, having_masks, cur_mp_dev, nmatches_dev, status_dev, diag_dev);
     a.last = ls.data(); a.n_points = n_points; a.last_mp = last_mp_dev; a.bad = bad_dev;
     a.window = window; a.nnratio = nnratio; a.min_level = min_level; a.max_level = max_level;
     CUDA_CHECK(launch_window_search_device(a, st));
-    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
-    return MCS_OK;
+    return sync_if_null_stream(stream);
 }
 
 int mcs_search_by_projection_frames_device(const mcs_packed_frame* cur, const mcs_packed_frame* last, int32_t n_cams, int32_t capacity,
@@ -701,30 +701,20 @@ int mcs_search_by_projection_frames_device(const mcs_packed_frame* cur, const mc
         return mcs_fail(MCS_ERR_INVALID, "null argument");
     if (int rc = check_packed_frames(n_cams, capacity, dim, cur, last)) return rc;
     if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
-    for (int c = 0; c < n_cams; ++c) {
-        if (cams[c].width < 1 || cams[c].height < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
-        if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
-            return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
-    }
-    // one query per (last-frame slot, camera): the owner words hold a 24-bit query index
-    if ((long long)n_cams * n_cams * capacity >= (1LL << 24))
-        return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * n_cams * capacity must stay below 2^24");
+    const CamSizes cz(cams, n_cams);
+    if (int rc = check_cam_sizes(n_cams, cz.w.data(), cz.h.data(), true)) return rc;
+    // one query per (last-frame slot, camera)
+    if (int rc = check_query_bound((long long)n_cams * n_cams * capacity, "n_cams * n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
-    std::vector<int> cw(n_cams), ch(n_cams);
-    for (int c = 0; c < n_cams; ++c) { cw[c] = cams[c].width; ch[c] = cams[c].height; }
     SearchFramesDevArgs a{};
-    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim;
-    a.cams = cs.data(); a.cam_w = cw.data(); a.cam_h = ch.data();
-    a.th_high = th_high; a.masked = having_masks != 0;
-    a.frame_mp = cur_mp_dev; a.nmatches = nmatches_dev; a.status = status_dev; a.diag = diag_dev;
-    a.last = ls.data(); a.models = cams; a.mtmc_inv = mtmc_inv; a.masks = masks_dev;
-    a.n_points = n_points; a.last_mp = last_mp_dev; a.world_pos = world_pos_dev; a.bad = bad_dev;
+    set_searched_frame(a, cs, capacity, dim, cz.w.data(), cz.h.data(), th_high, having_masks, cur_mp_dev, nmatches_dev, status_dev, diag_dev);
+    a.last = ls.data(); a.n_points = n_points; a.last_mp = last_mp_dev; a.bad = bad_dev;
+    a.models = cams; a.mtmc_inv = mtmc_inv; a.masks = masks_dev; a.world_pos = world_pos_dev;
     a.window = window; a.nnratio = nnratio;
     CUDA_CHECK(launch_search_by_projection_frames(a, st));
-    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
-    return MCS_OK;
+    return sync_if_null_stream(stream);
 }
 
 int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view* f2, double* prev_matched, int32_t window_size,

@@ -40,4 +40,26 @@ inline int check_packed_frames(int n_cams, int capacity, int dim, const mcs_pack
     return MCS_OK;
 }
 
+// every camera's image size positive and, when `equal` (the searches that read the mirror masks as one [n_cams][h][w] array),
+// the same for all cameras
+inline int check_cam_sizes(int n_cams, const int* w, const int* h, bool equal) {
+    for (int c = 0; c < n_cams; ++c) {
+        if (w[c] < 1 || h[c] < 1) return mcs_fail(MCS_ERR_INVALID, "camera sizes must be positive");
+        if (equal && (w[c] != w[0] || h[c] != h[0])) return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
+    }
+    return MCS_OK;
+}
+
+// the device searches keep a query index in 24 bits (the owner words of the ordered acceptance); n is the call's bound on queries
+inline int check_query_bound(long long n, const char* msg) {
+    return n >= (1LL << 24) ? mcs_fail(MCS_ERR_UNSUPPORTED, msg) : MCS_OK;
+}
+
+// the end of an asynchronous entry point: a NULL stream (the legacy default stream) means the caller wants the results on return
+inline int sync_if_null_stream(void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!stream) CUDA_CHECK(cudaStreamSynchronize(st));
+    return MCS_OK;
+}
+
 }  // namespace mcs

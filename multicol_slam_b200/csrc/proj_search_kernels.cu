@@ -16,8 +16,8 @@
 //   ps_list_kernel      per query the K smallest (distance, visiting position) keys of its window and the true candidate count
 //   ps_round_kernel     one round of the fixpoint iteration of the ordered acceptance (DESIGN.md section 4)
 //   ps_walk_kernel      the sequential fallback past the round cap: one warp per camera walks the unsettled queries in order
-//   pl_round / pl_walk  the same two kernels under the motion model's acceptance rule (MCS_RULE_BEST)
-//   pr_round / pr_walk  the same two kernels under the previous-frame searches' ratio rule (MCS_RULE_RATIO)
+//                       Both are templates over (rule, width, mask): MCS_RULE_LEVEL_RATIO for the local map, MCS_RULE_BEST for
+//                       the motion model, MCS_RULE_RATIO for the previous-frame searches
 //
 // No kernel reads anything back to the host: every size that depends on the data (the number of queries, the rounds the
 // fixpoint needed, where the walk starts) lives in device memory and the kernels are launched for the upper bound.
@@ -470,8 +470,8 @@ __device__ __forceinline__ int* ps_chg(const PsState& p) { return p.ctl + 4; }
 // smaller index accepted it in round r - 1.  Queries below the first one whose decision changed in round r - 1 are final
 // (query p reads only decisions of queries < p) and only republish their keypoint.
 template <int RULE, int WORDS, bool MASKED>
-__device__ __forceinline__ void ps_round(const WindowFrameDev& f, const PsState& p, const int r, const uint32_t* __restrict__ qdesc,
-                                         const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
+__global__ void __launch_bounds__(256, 2) ps_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
+                                                          const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
     const int* chg = ps_chg(p);
     const int settled = r >= 2 ? chg[r - 1] : 0;
     if (settled == kNoChange) return;                         // converged in an earlier round
@@ -503,22 +503,6 @@ __device__ __forceinline__ void ps_round(const WindowFrameDev& f, const PsState&
         }
     }
 }
-// one kernel name per rule: MCS_RULE_LEVEL_RATIO (local map), MCS_RULE_BEST (motion model), MCS_RULE_RATIO (previous frame)
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(256, 2) ps_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
-                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
-    ps_round<MCS_RULE_LEVEL_RATIO, WORDS, MASKED>(f, p, r, qdesc, qmask, fmp_in);
-}
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(256, 2) pl_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
-                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
-    ps_round<MCS_RULE_BEST, WORDS, MASKED>(f, p, r, qdesc, qmask, fmp_in);
-}
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(256, 2) pr_round_kernel(const WindowFrameDev f, const PsState p, const int r, const uint32_t* __restrict__ qdesc,
-                                                       const uint32_t* __restrict__ qmask, const int* __restrict__ fmp_in) {
-    ps_round<MCS_RULE_RATIO, WORDS, MASKED>(f, p, r, qdesc, qmask, fmp_in);
-}
 
 // Writes the final decisions of the settled prefix into frame_mp and counts them; records where the walk has to start.
 __global__ void __launch_bounds__(256) ps_finalize_kernel(const PsState p, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
@@ -545,8 +529,8 @@ __global__ void __launch_bounds__(256) ps_finalize_kernel(const PsState p, int* 
 // Fallback past the round cap: one warp per camera walks its queries from the first unsettled one in order, with the camera's
 // taken keypoints as a bitmap in shared memory.
 template <int RULE, int WORDS, bool MASKED>
-__device__ __forceinline__ void ps_walk(const WindowFrameDev& f, const PsState& p, const uint32_t* __restrict__ qdesc,
-                                        const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
+__global__ void __launch_bounds__(32) ps_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
+                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
     extern __shared__ unsigned s_bits[];
     const int S = p.ctl[3];
     if (S < 0) return;
@@ -582,21 +566,6 @@ __device__ __forceinline__ void ps_walk(const WindowFrameDev& f, const PsState& 
     }
     if (lane == 0 && nm) atomicAdd(nmatches, nm);
 }
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(32) ps_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
-                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
-    ps_walk<MCS_RULE_LEVEL_RATIO, WORDS, MASKED>(f, p, qdesc, qmask, frame_mp, nmatches);
-}
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(32) pl_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
-                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
-    ps_walk<MCS_RULE_BEST, WORDS, MASKED>(f, p, qdesc, qmask, frame_mp, nmatches);
-}
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(32) pr_walk_kernel(const WindowFrameDev f, const PsState p, const uint32_t* __restrict__ qdesc,
-                                                     const uint32_t* __restrict__ qmask, int* __restrict__ frame_mp, int* __restrict__ nmatches) {
-    ps_walk<MCS_RULE_RATIO, WORDS, MASKED>(f, p, qdesc, qmask, frame_mp, nmatches);
-}
 
 __global__ void ps_diag_kernel(const int* __restrict__ ctl, int* __restrict__ diag) {
     diag[0] = ctl[1];        // fixpoint rounds run
@@ -604,8 +573,6 @@ __global__ void ps_diag_kernel(const int* __restrict__ ctl, int* __restrict__ di
     diag[2] = ctl[0];        // queries
     diag[3] = ctl[2];        // decisions that rescanned their window
 }
-
-size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 }  // namespace
 
@@ -624,34 +591,26 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
     const long long Q = qm.size();
     const int nb = (int)((Q + kQbTile - 1) / kQbTile);
     const size_t db = (size_t)NS * a.dim;
-    // one stream-ordered scratch block, carved below
-    const size_t sizes[] = {
-        sizeof(mcs_ocam) * a.n_cams, sizeof(double) * a.n_levels, sizeof(PsCamSlots) * a.n_cams,          // staged host inputs
-        sizeof(mcs_keypoint) * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, db, a.masked ? db : 0,     // keys key_cam kx ky koct desc dmask
-        4ull * NS, 4ull * ncell, 4ull * (ncell + 1), 4ull * NS, 8ull * a.n_cams, 8ull * a.n_cams,          // cell_of cursor start items winv hinv
-        4ull * (nb + 1), 4ull * (nb + 1), 4ull * (4 + kPsRounds),                                          // block counts / offsets, ctl
-        sizeof(mcs_window_query) * Q, 4ull * Q * kPsK, 4ull * Q * kPsK, 4ull * Q, 8ull * Q, 8ull * NS};    // qry lkey lslot lcnt dec owner
-    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
-    size_t off[nsz], total = 0;
-    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
-    cudaError_t e = keep_pool_memory();
-    if (e != cudaSuccess) return e;
     int dev = 0, sms = 132;
-    e = cudaGetDevice(&dev);
+    cudaError_t e = cudaGetDevice(&dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (e != cudaSuccess) return e;
-    uint8_t* base = nullptr;
-    e = cudaMallocAsync((void**)&base, total, st);
+    StreamScratch sc;
+    e = sc.alloc({sizeof(mcs_ocam) * a.n_cams, sizeof(double) * a.n_levels, sizeof(PsCamSlots) * a.n_cams,         // staged host inputs
+                  sizeof(mcs_keypoint) * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, db, a.masked ? db : 0,    // keys key_cam kx ky koct desc dmask
+                  4ull * NS, 4ull * ncell, 4ull * (ncell + 1), 4ull * NS, 8ull * a.n_cams, 8ull * a.n_cams,         // cell_of cursor start items winv hinv
+                  4ull * (nb + 1), 4ull * (nb + 1), 4ull * (4 + kPsRounds),                                         // block counts / offsets, ctl
+                  sizeof(mcs_window_query) * Q, 4ull * Q * kPsK, 4ull * Q * kPsK, 4ull * Q, 8ull * Q, 8ull * NS},   // qry lkey lslot lcnt dec owner
+                 st);
     if (e != cudaSuccess) return e;
-    auto at = [&](int i) { return (void*)(base + off[i]); };
-    mcs_ocam* cams = (mcs_ocam*)at(0); double* sf = (double*)at(1); PsCamSlots* slots = (PsCamSlots*)at(2);
-    mcs_keypoint* keys = (mcs_keypoint*)at(3); int* key_cam = (int*)at(4); float* kx = (float*)at(5); float* ky = (float*)at(6);
-    int* koct = (int*)at(7); uint8_t* desc = (uint8_t*)at(8); uint8_t* dmask = a.masked ? (uint8_t*)at(9) : nullptr;
-    int* cell_of = (int*)at(10); int* cursor = (int*)at(11); int* cell_start = (int*)at(12); int* cell_items = (int*)at(13);
-    double* winv = (double*)at(14); double* hinv = (double*)at(15);
-    int* bcount = (int*)at(16); int* boff = (int*)at(17); int* ctl = (int*)at(18);
-    mcs_window_query* qry = (mcs_window_query*)at(19); unsigned* lkey = (unsigned*)at(20); int* lslot = (int*)at(21); int* lcnt = (int*)at(22);
-    int* dec = (int*)at(23); unsigned* owner = (unsigned*)at(24);
+    mcs_ocam* cams = sc.at<mcs_ocam>(0); double* sf = sc.at<double>(1); PsCamSlots* slots = sc.at<PsCamSlots>(2);
+    mcs_keypoint* keys = sc.at<mcs_keypoint>(3); int* key_cam = sc.at<int>(4); float* kx = sc.at<float>(5); float* ky = sc.at<float>(6);
+    int* koct = sc.at<int>(7); uint8_t* desc = sc.at<uint8_t>(8); uint8_t* dmask = a.masked ? sc.at<uint8_t>(9) : nullptr;
+    int* cell_of = sc.at<int>(10); int* cursor = sc.at<int>(11); int* cell_start = sc.at<int>(12); int* cell_items = sc.at<int>(13);
+    double* winv = sc.at<double>(14); double* hinv = sc.at<double>(15);
+    int* bcount = sc.at<int>(16); int* boff = sc.at<int>(17); int* ctl = sc.at<int>(18);
+    mcs_window_query* qry = sc.at<mcs_window_query>(19); unsigned* lkey = sc.at<unsigned>(20); int* lslot = sc.at<int>(21);
+    int* lcnt = sc.at<int>(22); int* dec = sc.at<int>(23); unsigned* owner = sc.at<unsigned>(24);
 
     std::vector<mcs_ocam> hc(a.n_cams);
     std::memset(hc.data(), 0, sizeof(mcs_ocam) * a.n_cams);
@@ -662,7 +621,7 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl, 0, 16, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl + 4, 0x7F, 4 * kPsRounds, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(owner, 0xFF, 8ull * NS, st);
-    if (e != cudaSuccess) { cudaFreeAsync(base, st); return e; }
+    if (e != cudaSuccess) return sc.release(e);
 
     // frame view in slot order and its grid (the kernel the host entry points build their grid with)
     ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
@@ -683,34 +642,56 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
         const int wblocks = (int)std::min<long long>((Q + 7) / 8, (long long)sms * 16);
         const int fblocks = (int)std::min<long long>((Q + 255) / 256, (long long)sms * 4);
         const size_t walk_smem = 4ull * ((a.capacity + 31) / 32);
-#define MCS_PS(W, M)                                                                                                   \
-        {                                                                                                              \
-            ps_list_kernel<W, M><<<wblocks, 256, 0, st>>>(f, qry, ctl, qd, qk, lkey, lslot, lcnt);                     \
-            for (int r = 0; r < kPsRounds; ++r) {                                                                      \
-                if constexpr (RULE == MCS_RULE_BEST) pl_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp); \
-                else if constexpr (RULE == MCS_RULE_RATIO) pr_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp); \
-                else ps_round_kernel<W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp);                      \
-            }                                                                                                          \
-            ps_finalize_kernel<<<fblocks, 256, 0, st>>>(p, a.frame_mp, a.nmatches);                                    \
-            if constexpr (RULE == MCS_RULE_BEST) pl_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches); \
-            else if constexpr (RULE == MCS_RULE_RATIO) pr_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches); \
-            else ps_walk_kernel<W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches);          \
-        }
-        if (a.dim == 16) { if (a.masked) MCS_PS(4, true) else MCS_PS(4, false) }
-        else if (a.dim == 32) { if (a.masked) MCS_PS(8, true) else MCS_PS(8, false) }
-        else { if (a.masked) MCS_PS(16, true) else MCS_PS(16, false) }
-#undef MCS_PS
+        with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
+            ps_list_kernel<W, M><<<wblocks, 256, 0, st>>>(f, qry, ctl, qd, qk, lkey, lslot, lcnt);
+            for (int r = 0; r < kPsRounds; ++r) ps_round_kernel<RULE, W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp);
+            ps_finalize_kernel<<<fblocks, 256, 0, st>>>(p, a.frame_mp, a.nmatches);
+            ps_walk_kernel<RULE, W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches);
+        });
         e = cudaGetLastError();
     }
     if (e == cudaSuccess && a.diag) ps_diag_kernel<<<1, 1, 0, st>>>(ctl, a.diag);
     if (e == cudaSuccess) e = cudaGetLastError();
-    const cudaError_t ef = cudaFreeAsync(base, st);
-    return e != cudaSuccess ? e : ef;
+    return sc.release(e);
 }
 
 cudaError_t ps_zero_outputs(const PsFrameArgs& a, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(a.nmatches, 0, 4, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
+    return e;
+}
+
+// What the searches between two frames share, in the launcher's one stream-ordered scratch block: its own pieces (`own`, from
+// piece 0 on), then the staged slots of cur (when stage_cur) and of last, the staged camera models and mtmc_inv (when a.models is
+// set: the searches that project), and the last frame in slot order.  The caller releases `sc`, whatever the result.
+struct TwoFrameScratch {
+    StreamScratch sc;
+    PsCamSlots* cur; PsCamSlots* last; mcs_ocam* models; double* mtmc_inv;
+    mcs_keypoint* keys; uint8_t* desc; uint8_t* dmask;      // the last frame in slot order (dmask NULL unless masked)
+};
+
+// Allocates and stages those pieces, zeroes the outputs and gathers the last frame into slot order (without a grid).
+cudaError_t ps_open_two_frames(const PsTwoFrameArgs& a, const bool stage_cur, std::vector<size_t> own, TwoFrameScratch& t, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    const size_t db = (size_t)NS * a.dim, b_slots = sizeof(PsCamSlots) * a.n_cams;
+    const bool pose = a.models != nullptr;
+    const size_t k = own.size();
+    own.insert(own.end(), {stage_cur ? b_slots : 0, b_slots, pose ? sizeof(mcs_ocam) * a.n_cams : 0, pose ? 128ull * a.n_cams : 0,
+                           sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0});
+    cudaError_t e = t.sc.alloc(own, st);
+    if (e != cudaSuccess) return e;
+    t.cur = t.sc.at<PsCamSlots>(k); t.last = t.sc.at<PsCamSlots>(k + 1);
+    t.models = t.sc.at<mcs_ocam>(k + 2); t.mtmc_inv = t.sc.at<double>(k + 3);
+    t.keys = t.sc.at<mcs_keypoint>(k + 4); t.desc = t.sc.at<uint8_t>(k + 5); t.dmask = a.masked ? t.sc.at<uint8_t>(k + 6) : nullptr;
+    if (stage_cur) e = stage_to_device(a.cams, b_slots, t.cur, st);
+    if (e == cudaSuccess) e = stage_to_device(a.last, b_slots, t.last, st);
+    if (e == cudaSuccess && pose) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, t.models, st);
+    if (e == cudaSuccess && pose) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, t.mtmc_inv, st);
+    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
+    if (e == cudaSuccess) {
+        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(t.last, a.n_cams, a.capacity, a.dim, a.masked, t.keys, nullptr, t.desc, t.dmask);
+        e = cudaGetLastError();
+    }
     return e;
 }
 
@@ -723,122 +704,66 @@ cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st
     return ps_search<MCS_RULE_LEVEL_RATIO>(a, qm, a.nnratio, a.mp_desc, a.mp_dmask, nullptr, st);
 }
 
-// The last frame in slot order (gather without a grid) and its queries (pl_project_kernel), then the current frame searched under
-// MCS_RULE_BEST with the last frame's descriptors as the query rows and last_mp as the tags.
+// The last frame's queries (pl_project_kernel), then the current frame searched under MCS_RULE_BEST with the last frame's
+// descriptors as the query rows and last_mp as the tags.
 cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
-    const size_t db = (size_t)NS * a.dim;
-    const size_t sizes[] = {sizeof(PsCamSlots) * a.n_cams, sizeof(mcs_ocam) * a.n_cams, 128ull * a.n_cams,    // staged host inputs
-                            sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0, (size_t)NS, 8ull * NS, 8ull * NS}; // keys desc dmask ok u v
-    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
-    size_t off[nsz], total = 0;
-    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
-    cudaError_t e = keep_pool_memory();
-    if (e != cudaSuccess) return e;
-    uint8_t* base = nullptr;
-    e = cudaMallocAsync((void**)&base, total, st);
-    if (e != cudaSuccess) return e;
-    auto at = [&](int i) { return (void*)(base + off[i]); };
-    PsCamSlots* slots = (PsCamSlots*)at(0); mcs_ocam* models = (mcs_ocam*)at(1); double* mi = (double*)at(2);
-    mcs_keypoint* keys = (mcs_keypoint*)at(3); uint8_t* desc = (uint8_t*)at(4); uint8_t* dmask = a.masked ? (uint8_t*)at(5) : nullptr;
-    uint8_t* ok = (uint8_t*)at(6); double* u = (double*)at(7); double* v = (double*)at(8);
-    e = stage_to_device(a.last, sizeof(PsCamSlots) * a.n_cams, slots, st);
-    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
-    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, mi, st);
-    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
+    TwoFrameScratch t;
+    cudaError_t e = ps_open_two_frames(a, false, {(size_t)NS, 8ull * NS, 8ull * NS}, t, st);      // ok u v
+    if (e != cudaSuccess) return t.sc.release(e);
+    uint8_t* ok = t.sc.at<uint8_t>(0); double* u = t.sc.at<double>(1); double* v = t.sc.at<double>(2);
+    const LastProjArgs pa{t.last, a.n_cams, a.capacity, a.n_levels, a.n_points, t.keys, a.last_mp, a.last_outlier, a.bad, a.world_pos,
+                          t.models, t.mtmc_inv, a.masks};
+    pl_project_kernel<<<(NS + 255) / 256, 256, 0, st>>>(pa, ok, u, v, a.status);
+    e = cudaGetLastError();
     if (e == cudaSuccess) {
-        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, nullptr, desc, dmask);
-        const LastProjArgs pa{slots, a.n_cams, a.capacity, a.n_levels, a.n_points, keys, a.last_mp, a.last_outlier, a.bad, a.world_pos,
-                              models, mi, a.masks};
-        pl_project_kernel<<<(NS + 255) / 256, 256, 0, st>>>(pa, ok, u, v, a.status);
-        e = cudaGetLastError();
+        const LastFrameQueries qm{NS, a.capacity, ok, u, v, t.keys, nullptr, a.th};
+        e = ps_search<MCS_RULE_BEST>(a, qm, 0.0, t.desc, t.dmask, a.last_mp, st);
     }
-    if (e == cudaSuccess) {
-        const LastFrameQueries qm{NS, a.capacity, ok, u, v, keys, nullptr, a.th};
-        e = ps_search<MCS_RULE_BEST>(a, qm, 0.0, desc, dmask, a.last_mp, st);
-    }
-    const cudaError_t ef = cudaFreeAsync(base, st);
-    return e != cudaSuccess ? e : ef;
+    return t.sc.release(e);
 }
 
-// WindowSearch: cur_mp cleared below each camera's count, the last frame in slot order, then the current frame searched under
-// MCS_RULE_RATIO with one query per qualifying last-frame slot and last_mp as the tags.
+// WindowSearch: cur_mp cleared below each camera's count, then the current frame searched under MCS_RULE_RATIO with one query per
+// qualifying last-frame slot and last_mp as the tags.
 cudaError_t launch_window_search_device(const WindowSearchDevArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
-    const size_t db = (size_t)NS * a.dim;
-    const size_t sizes[] = {sizeof(PsCamSlots) * a.n_cams, sizeof(PsCamSlots) * a.n_cams,        // staged host inputs: cur, last
-                            sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0};                  // keys desc dmask
-    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
-    size_t off[nsz], total = 0;
-    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
-    cudaError_t e = keep_pool_memory();
-    if (e != cudaSuccess) return e;
-    uint8_t* base = nullptr;
-    e = cudaMallocAsync((void**)&base, total, st);
-    if (e != cudaSuccess) return e;
-    auto at = [&](int i) { return (void*)(base + off[i]); };
-    PsCamSlots* cur = (PsCamSlots*)at(0); PsCamSlots* last = (PsCamSlots*)at(1);
-    mcs_keypoint* keys = (mcs_keypoint*)at(2); uint8_t* desc = (uint8_t*)at(3); uint8_t* dmask = a.masked ? (uint8_t*)at(4) : nullptr;
-    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, cur, st);
-    if (e == cudaSuccess) e = stage_to_device(a.last, sizeof(PsCamSlots) * a.n_cams, last, st);
-    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
+    TwoFrameScratch t;
+    cudaError_t e = ps_open_two_frames(a, true, {}, t, st);
+    if (e != cudaSuccess) return t.sc.release(e);
+    pw_clear_kernel<<<(NS + 255) / 256, 256, 0, st>>>(t.cur, a.n_cams, a.capacity, a.frame_mp);
+    e = cudaGetLastError();
     if (e == cudaSuccess) {
-        pw_clear_kernel<<<(NS + 255) / 256, 256, 0, st>>>(cur, a.n_cams, a.capacity, a.frame_mp);
-        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(last, a.n_cams, a.capacity, a.dim, a.masked, keys, nullptr, desc, dmask);
-        e = cudaGetLastError();
+        const WindowQueries qm{NS, a.capacity, a.n_points, a.min_level, a.max_level, t.last, t.keys, a.last_mp, a.bad, nullptr, a.window};
+        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, t.desc, t.dmask, a.last_mp, st);
     }
-    if (e == cudaSuccess) {
-        const WindowQueries qm{NS, a.capacity, a.n_points, a.min_level, a.max_level, last, keys, a.last_mp, a.bad, nullptr, a.window};
-        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, desc, dmask, a.last_mp, st);
-    }
-    const cudaError_t ef = cudaFreeAsync(base, st);
-    return e != cudaSuccess ? e : ef;
+    return t.sc.release(e);
 }
 
-// SearchByProjection(F1 = last, F2 = cur): the skip flags (pf_flag_kernel), the last frame in slot order, the (slot, camera)
-// projections (pf_project_kernel), then the current frame searched under MCS_RULE_RATIO with last_mp as the tags.
+// SearchByProjection(F1 = last, F2 = cur): the skip flags (pf_flag_kernel), the (slot, camera) projections (pf_project_kernel),
+// then the current frame searched under MCS_RULE_RATIO with last_mp as the tags.
 cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     const size_t NK = (size_t)NS * a.n_cams;
-    const size_t db = (size_t)NS * a.dim;
-    const size_t sizes[] = {sizeof(PsCamSlots) * a.n_cams, sizeof(PsCamSlots) * a.n_cams, sizeof(mcs_ocam) * a.n_cams,  // staged: cur last
-                            128ull * a.n_cams,                                                                         // models mtmc_inv
-                            (size_t)a.n_points, 4ull * a.n_points,                                                     // found first
-                            sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0, NK, 8 * NK, 8 * NK};                    // keys desc dmask ok u v
-    constexpr int nsz = sizeof(sizes) / sizeof(sizes[0]);
-    size_t off[nsz], total = 0;
-    for (int i = 0; i < nsz; ++i) { off[i] = total; total += align256(sizes[i]); }
-    cudaError_t e = keep_pool_memory();
-    if (e != cudaSuccess) return e;
-    uint8_t* base = nullptr;
-    e = cudaMallocAsync((void**)&base, total, st);
-    if (e != cudaSuccess) return e;
-    auto at = [&](int i) { return (void*)(base + off[i]); };
-    PsCamSlots* cur = (PsCamSlots*)at(0); PsCamSlots* last = (PsCamSlots*)at(1); mcs_ocam* models = (mcs_ocam*)at(2); double* mi = (double*)at(3);
-    uint8_t* found = (uint8_t*)at(4); int* first = (int*)at(5);
-    mcs_keypoint* keys = (mcs_keypoint*)at(6); uint8_t* desc = (uint8_t*)at(7); uint8_t* dmask = a.masked ? (uint8_t*)at(8) : nullptr;
-    uint8_t* ok = (uint8_t*)at(9); double* u = (double*)at(10); double* v = (double*)at(11);
-    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, cur, st);
-    if (e == cudaSuccess) e = stage_to_device(a.last, sizeof(PsCamSlots) * a.n_cams, last, st);
-    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
-    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, mi, st);
-    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
-    if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(found, 0, a.n_points, st);
+    TwoFrameScratch t;
+    cudaError_t e = ps_open_two_frames(a, true, {(size_t)a.n_points, 4ull * a.n_points, NK, 8 * NK, 8 * NK}, t, st);   // found first ok u v
+    if (e != cudaSuccess) return t.sc.release(e);
+    uint8_t* found = t.sc.at<uint8_t>(0); int* first = t.sc.at<int>(1);
+    uint8_t* ok = t.sc.at<uint8_t>(2); double* u = t.sc.at<double>(3); double* v = t.sc.at<double>(4);
+    if (a.n_points > 0) e = cudaMemsetAsync(found, 0, a.n_points, st);
     if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(first, 0x7F, 4ull * a.n_points, st);     // above every slot
     if (e == cudaSuccess) {
-        pf_flag_kernel<<<(NS + 255) / 256, 256, 0, st>>>(cur, last, a.n_cams, a.capacity, a.n_points, a.frame_mp, a.last_mp, found, first,
+        pf_flag_kernel<<<(NS + 255) / 256, 256, 0, st>>>(t.cur, t.last, a.n_cams, a.capacity, a.n_points, a.frame_mp, a.last_mp, found, first,
                                                          a.status);
-        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(last, a.n_cams, a.capacity, a.dim, a.masked, keys, nullptr, desc, dmask);
-        const FramesProjArgs pa{last, a.n_cams, a.capacity, a.n_points, a.last_mp, a.bad, found, first, a.world_pos, models, mi, a.masks};
+        const FramesProjArgs pa{t.last, a.n_cams, a.capacity, a.n_points, a.last_mp, a.bad, found, first, a.world_pos, t.models, t.mtmc_inv,
+                                a.masks};
         pf_project_kernel<<<(unsigned)((NK + 255) / 256), 256, 0, st>>>(pa, ok, u, v);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) {
-        const FramesQueries qm{NS, a.n_cams, ok, u, v, keys, nullptr, a.window};
-        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, desc, dmask, a.last_mp, st);
+        const FramesQueries qm{NS, a.n_cams, ok, u, v, t.keys, nullptr, a.window};
+        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, t.desc, t.dmask, a.last_mp, st);
     }
-    const cudaError_t ef = cudaFreeAsync(base, st);
-    return e != cudaSuccess ? e : ef;
+    return t.sc.release(e);
 }
 
 }  // namespace mcs
