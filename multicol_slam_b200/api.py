@@ -55,6 +55,21 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def _dptr(t):
+    return C.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _stream_handle(stream, dev):
+    import torch
+    return C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _extract_inputs(masks, cams, cam_of_image=None):
+    """the host inputs of an extraction call: masks [n_cams,H,W] u8, the camera models as an mcs_ocam array, cam_of_image i32"""
+    coi = None if cam_of_image is None else np.ascontiguousarray(cam_of_image, np.int32)
+    return np.ascontiguousarray(masks, np.uint8), (Ocam * len(cams))(*[as_ocam(c) for c in cams]), coi
+
+
 def device_count():
     return lib().mcs_device_count()
 
@@ -151,11 +166,9 @@ class mdBRIEFextractorOct:
     def extract_batch(self, images, masks, cams, cam_of_image):
         """images [B,H,W] u8 host; masks [n_cams,H,W]; cams list; -> (kps [B,cap], desc [B,cap,ds], dmask, counts [B])"""
         images = np.ascontiguousarray(images, np.uint8)
-        masks = np.ascontiguousarray(masks, np.uint8)
-        coi = np.ascontiguousarray(cam_of_image, np.int32)
+        masks, ocs, coi = _extract_inputs(masks, cams, cam_of_image)
         B, H, W = images.shape
         cap, ds = self.info.capacity, self.info.desc_size
-        ocs = (Ocam * len(cams))(*[as_ocam(c) for c in cams])
         kps = np.zeros((B, cap), KEYPOINT_DTYPE)
         desc = np.zeros((B, cap, ds), np.uint8)
         dmask = np.zeros((B, cap, ds), np.uint8)
@@ -179,13 +192,10 @@ class mdBRIEFextractorOct:
                        desc=torch.empty((B, cap, ds), dtype=torch.uint8, device=dev),
                        dmask=torch.empty((B, cap, ds), dtype=torch.uint8, device=dev),
                        counts=torch.empty((B,), dtype=torch.int32, device=dev))
-        masks = np.ascontiguousarray(masks, np.uint8)
-        coi = np.ascontiguousarray(cam_of_image, np.int32)
-        ocs = (Ocam * len(cams))(*[as_ocam(c) for c in cams])
-        st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
-        _check(lib().mcs_extract_batch_device(self._h, B, C.c_void_p(images_t.data_ptr()), W, H, P, _p(masks), ocs, len(cams),
-                                              _p(coi), C.c_void_p(out["kps"].data_ptr()), C.c_void_p(out["desc"].data_ptr()),
-                                              C.c_void_p(out["dmask"].data_ptr()), C.c_void_p(out["counts"].data_ptr()), cap, st))
+        masks, ocs, coi = _extract_inputs(masks, cams, cam_of_image)
+        _check(lib().mcs_extract_batch_device(self._h, B, _dptr(images_t), W, H, P, _p(masks), ocs, len(cams), _p(coi), _dptr(out["kps"]),
+                                              _dptr(out["desc"]), _dptr(out["dmask"]), _dptr(out["counts"]), cap,
+                                              _stream_handle(stream, dev)))
         return out
 
     def packed_views(self, packed_t, n_images):
@@ -203,15 +213,11 @@ class mdBRIEFextractorOct:
     def extract_batch_packed_device(self, images_t, masks, cams, cam_of_image, packed_t, stream=None, width=None):
         """mcs_extract_batch_packed_device: K3 writes counts | keypoints | descriptors | masks straight into packed_t (uint8
         cuda tensor of rig.packed_layout(B, capacity, descSize)[1] bytes) -- the buffer mcs_allgather_features exchanges."""
-        import torch
         B, H, P = images_t.shape
         W = P if width is None else width
-        masks = np.ascontiguousarray(masks, np.uint8)
-        coi = np.ascontiguousarray(cam_of_image, np.int32)
-        ocs = (Ocam * len(cams))(*[as_ocam(c) for c in cams])
-        st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(images_t.device).cuda_stream)
-        _check(lib().mcs_extract_batch_packed_device(self._h, B, C.c_void_p(images_t.data_ptr()), W, H, P, _p(masks), ocs, len(cams),
-                                                     _p(coi), C.c_void_p(packed_t.data_ptr()), self.info.capacity, st))
+        masks, ocs, coi = _extract_inputs(masks, cams, cam_of_image)
+        _check(lib().mcs_extract_batch_packed_device(self._h, B, _dptr(images_t), W, H, P, _p(masks), ocs, len(cams), _p(coi),
+                                                     _dptr(packed_t), self.info.capacity, _stream_handle(stream, images_t.device)))
         return self.packed_views(packed_t, B)
 
     def extract_match_stream(self, images, masks, cams, K=2, out=None, packed_t=None, greedy=None):
@@ -219,10 +225,9 @@ class mdBRIEFextractorOct:
         against (frame-1,cam).  Returns dict(kps [F*C,cap], desc, dmask, counts, match_idx [F*C,cap,K], match_dist).
         `out` may hold preallocated (e.g. pinned) numpy arrays with the same keys."""
         images = np.ascontiguousarray(images, np.uint8)
-        masks = np.ascontiguousarray(masks, np.uint8)
+        masks, ocs, _ = _extract_inputs(masks, cams)
         F, Cn, H, W = images.shape
         cap, ds, B = self.info.capacity, self.info.desc_size, F * Cn
-        ocs = (Ocam * len(cams))(*[as_ocam(c) for c in cams])
         if out is None:
             out = dict(kps=np.zeros((B, cap), KEYPOINT_DTYPE), desc=np.zeros((B, cap, ds), np.uint8),
                        dmask=np.zeros((B, cap, ds), np.uint8), counts=np.zeros(B, np.int32),
@@ -238,7 +243,7 @@ class mdBRIEFextractorOct:
             _check(lib().mcs_extract_match_stream_packed(self._h, F, Cn, _p(images), W, H, W, _p(masks), ocs, _p(out["kps"]),
                                                          _p(out["desc"]), _p(out["dmask"]), _p(out["counts"]), cap, K,
                                                          _p(out["match_idx"]), _p(out["match_dist"]),
-                                                         C.c_void_p(packed_t.data_ptr()) if packed_t is not None else None, int(th),
+                                                         _dptr(packed_t), int(th),
                                                          C.c_double(ratio), _p(out.get("matches12")) if greedy is not None else None,
                                                          _p(out.get("nmatches")) if greedy is not None else None,
                                                          _p(out.get("redo")) if greedy is not None else None))
@@ -315,10 +320,9 @@ def hamming_topk_device(q_t, d_t, K=2, qmask_t=None, dmask_t=None, skip_t=None, 
     dev = q_t.device
     if out is None:
         out = (torch.empty((nq, K), dtype=torch.int32, device=dev), torch.empty((nq, K), dtype=torch.int32, device=dev))
-    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-    st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
-    _check(lib().mcs_hamming_topk_device(ptr(q_t), ptr(qmask_t), nq, ptr(d_t), ptr(dmask_t), d_t.shape[0], ptr(skip_t), dim, K,
-                                         ptr(out[0]), ptr(out[1]), st))
+    st = _stream_handle(stream, dev)
+    _check(lib().mcs_hamming_topk_device(_dptr(q_t), _dptr(qmask_t), nq, _dptr(d_t), _dptr(dmask_t), d_t.shape[0], _dptr(skip_t), dim, K,
+                                         _dptr(out[0]), _dptr(out[1]), st))
     return out
 
 
@@ -329,10 +333,9 @@ def match_stream_device(desc_t, dmask_t, counts_t, n_frames, n_cams, K=2, out=No
     dev = desc_t.device
     if out is None:
         out = (torch.empty((B, cap, K), dtype=torch.int32, device=dev), torch.empty((B, cap, K), dtype=torch.int32, device=dev))
-    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-    st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
-    _check(lib().mcs_match_stream_device(ptr(desc_t), ptr(dmask_t), ptr(counts_t), n_frames, n_cams, cap, dim, K, ptr(out[0]),
-                                         ptr(out[1]), st))
+    st = _stream_handle(stream, dev)
+    _check(lib().mcs_match_stream_device(_dptr(desc_t), _dptr(dmask_t), _dptr(counts_t), n_frames, n_cams, cap, dim, K, _dptr(out[0]),
+                                         _dptr(out[1]), st))
     return out
 
 
@@ -345,17 +348,15 @@ def match_stream_replay_device(idx_t, dist_t, counts_t, desc_t, dmask_t, n_frame
     if out is None:
         out = (torch.empty((B, cap), dtype=torch.int32, device=dev), torch.empty(B, dtype=torch.int32, device=dev),
                torch.empty(B, dtype=torch.int32, device=dev))
-    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-    st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
-    _check(lib().mcs_match_stream_replay_device(ptr(idx_t), ptr(dist_t), ptr(counts_t), ptr(desc_t), ptr(dmask_t), n_frames, n_cams, cap,
-                                                desc_t.shape[-1], K, int(th_low), C.c_double(nnratio), ptr(out[0]), ptr(out[1]), ptr(out[2]), st))
+    st = _stream_handle(stream, dev)
+    _check(lib().mcs_match_stream_replay_device(_dptr(idx_t), _dptr(dist_t), _dptr(counts_t), _dptr(desc_t), _dptr(dmask_t), n_frames, n_cams, cap,
+                                                desc_t.shape[-1], K, int(th_low), C.c_double(nnratio), _dptr(out[0]), _dptr(out[1]), _dptr(out[2]), st))
     return out
 
 
 def match_bruteforce_batch_device(q_t, qmask_t, valid1, seg_start, d_t, dmask_t, valid2, th_low, nnratio, stream=None):
     """mcs_match_bruteforce_batch_device: the query sets q_t[seg_start[s]:seg_start[s+1]] each matched against the database as a separate
     SearchByBoW(KF1, KF2) would, K-best lists of all sets from one launch.  Returns (nmatches [n_seg] numpy, matches12 numpy)."""
-    import torch
     nq, dim = q_t.shape
     nd = d_t.shape[0]
     seg = np.ascontiguousarray(seg_start, np.int32)
@@ -364,9 +365,8 @@ def match_bruteforce_batch_device(q_t, qmask_t, valid1, seg_start, d_t, dmask_t,
     v2 = None if valid2 is None else np.ascontiguousarray(valid2, np.uint8)
     m12 = np.zeros(nq, np.int32)
     nm = np.zeros(len(seg) - 1, np.int32)
-    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-    st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(q_t.device).cuda_stream)
-    _check(lib().mcs_match_bruteforce_batch_device(ptr(q_t), ptr(qmask_t), _p(v1), _p(seg), len(seg) - 1, ptr(d_t), ptr(dmask_t), _p(v2), nd, dim,
+    st = _stream_handle(stream, q_t.device)
+    _check(lib().mcs_match_bruteforce_batch_device(_dptr(q_t), _dptr(qmask_t), _p(v1), _p(seg), len(seg) - 1, _dptr(d_t), _dptr(dmask_t), _p(v2), nd, dim,
                                                    int(th_low), C.c_double(nnratio), _p(m12), _p(nm), st))
     return nm, m12
 
@@ -380,26 +380,23 @@ def match_stream_greedy_device(desc_t, dmask_t, counts_t, n_frames, n_cams, th_l
     dev = desc_t.device
     if out is None:
         out = (torch.empty((B, cap), dtype=torch.int32, device=dev), torch.empty(B, dtype=torch.int32, device=dev))
-    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-    st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
-    _check(lib().mcs_match_stream_greedy_device(ptr(desc_t), ptr(dmask_t), ptr(counts_t), n_frames, n_cams, cap, dim, int(th_low),
-                                                C.c_double(nnratio), ptr(out[0]), ptr(out[1]), st))
+    st = _stream_handle(stream, dev)
+    _check(lib().mcs_match_stream_greedy_device(_dptr(desc_t), _dptr(dmask_t), _dptr(counts_t), n_frames, n_cams, cap, dim, int(th_low),
+                                                C.c_double(nnratio), _dptr(out[0]), _dptr(out[1]), st))
     return out
 
 
 def match_bruteforce_device(q_t, qmask_t, valid1, d_t, dmask_t, valid2, th_low, nnratio, stream=None):
     """mcs_match_bruteforce_device: SearchByBoW(KF1, KF2) with descriptors resident on the GPU (torch uint8 [n, dim]);
     valid1 / valid2 host uint8 arrays or None.  Returns (nmatches, matches12 numpy)."""
-    import torch
     nq, dim = q_t.shape
     nd = d_t.shape[0]
     v1 = None if valid1 is None else np.ascontiguousarray(valid1, np.uint8)
     v2 = None if valid2 is None else np.ascontiguousarray(valid2, np.uint8)
     m12 = np.zeros(nq, np.int32)
     n = C.c_int32(0)
-    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None  # noqa: E731
-    st = C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(q_t.device).cuda_stream)
-    _check(lib().mcs_match_bruteforce_device(ptr(q_t), ptr(qmask_t), _p(v1), nq, ptr(d_t), ptr(dmask_t), _p(v2), nd, dim, int(th_low),
+    st = _stream_handle(stream, q_t.device)
+    _check(lib().mcs_match_bruteforce_device(_dptr(q_t), _dptr(qmask_t), _p(v1), nq, _dptr(d_t), _dptr(dmask_t), _p(v2), nd, dim, int(th_low),
                                              C.c_double(nnratio), _p(m12), C.byref(n), st))
     return n.value, m12
 
@@ -510,15 +507,6 @@ def project_mappoints(mtmc_inv, mtmc, cams, masks, world_pos, normal, min_dist, 
     _check(lib().mcs_project_mappoints(nc, _p(mi), _p(mm), ocs, _p(masks), n, _p(pos), _p(nrm), _p(dmin), _p(dmax), _p(sf), len(sf),
                                        _p(in_view), _p(level), _p(px), _p(py), _p(vc)))
     return in_view, level, px, py, vc
-
-
-def _dptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def _stream_handle(stream, dev):
-    import torch
-    return C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
 
 
 def project_mappoints_device(mtmc_inv, mtmc, cams, masks_t, world_t, normal_t, min_dist_t, max_dist_t, scale_factors, skip_t=None,

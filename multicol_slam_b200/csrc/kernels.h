@@ -1,4 +1,4 @@
-// kernels.h -- launchers exported by the .cu files to the C-ABI host layer (mcs_api.cu).
+// kernels.h -- launchers exported by the .cu files to the C-ABI host layer (mcs_api.cu, mcs_match_api.cu, mcs_bow_api.cu).
 #pragma once
 #include <vector>
 

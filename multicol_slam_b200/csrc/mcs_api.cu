@@ -1,9 +1,9 @@
-// mcs_api.cu -- C-ABI host layer of libmcs_b200.so (see include/mcs_b200.h).
+// mcs_api.cu -- C-ABI host layer of libmcs_b200.so (see include/mcs_b200.h): the error message, the camera-model helpers and
+// the extractor with its extract-and-match stream pipeline.
 //
 // Host responsibilities only: parameter tables of the extractor constructor (ref
-// src/mdBRIEFextractorOct.cpp:134-203), per-image-size geometry / look-up tables, device buffers,
-// kernel launches, and the order-dependent bookkeeping of the matchers (greedy assignment rules of
-// ref src/cORBmatcher.cpp:67-166, :579-726, :885-966) replayed over GPU-computed distances.
+// src/mdBRIEFextractorOct.cpp:134-203), per-image-size geometry / look-up tables, device buffers and
+// kernel launches.  The matcher entry points live in mcs_match_api.cu.
 // There is no CPU implementation of the image or distance arithmetic in this library: without a CUDA
 // device every compute entry point fails with MCS_ERR_NO_DEVICE.
 #include <algorithm>
@@ -19,6 +19,7 @@
 #include "cam_model.cuh"
 #include "kernels.h"
 #include "mcs_common.cuh"
+#include "packed_frame.h"
 
 using namespace mcs;
 
@@ -36,10 +37,15 @@ inline int cv_floor(double v) { int i = (int)v; return i - (i > v); }
 inline int cv_ceil(double v) { int i = (int)v; return i + (i < v); }
 inline short sat_short_round(float v) { int i = (int)lrintf(v); return (short)std::min(std::max(i, -32768), 32767); }
 
+// device memory owned by the extractor: freed with it (the caller makes the extractor's device current)
 template <typename T>
 struct DevBuf {
     T* p = nullptr;
     size_t n = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     cudaError_t ensure(size_t count) {
         if (count <= n) return cudaSuccess;
         if (p) cudaFree(p);
@@ -53,7 +59,6 @@ struct DevBuf {
         if (e != cudaSuccess) return e;
         return cudaDeviceSynchronize();
     }
-    void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
 
 }  // namespace
@@ -78,7 +83,7 @@ struct mcs_extractor {
     DevBuf<uint8_t> lvl[kMaxLevels], blur[kMaxLevels];
     DevBuf<uint8_t> masks;
     DevBuf<mcs_ocam> cams;
-    DevBuf<int> cam_of_image, coi_all;
+    DevBuf<int> cam_of_image;
     const int* coi_last = nullptr;      // camera-of-image table the last run used (device)
     DevBuf<uint32_t> raw;
     DevBuf<uint16_t> node_of;
@@ -270,7 +275,6 @@ int ensure_batch(mcs_extractor* ex, int B) {
         CUDA_CHECK(ex->lvl[l].ensure(G.lv[l].img_bytes * B + 256));
         CUDA_CHECK(ex->blur[l].ensure(G.lv[l].img_bytes * B + 256));
     }
-    CUDA_CHECK(ex->cam_of_image.ensure(B));
     CUDA_CHECK(ex->raw.ensure(G.raw_total * B));
     CUDA_CHECK(ex->node_of.ensure(G.raw_total * B));
     CUDA_CHECK(ex->raw_count.ensure((size_t)B * G.nlevels));
@@ -357,7 +361,7 @@ constexpr int kGraphMaxImages = 16;      // batches up to this size take the per
 // K1 (per level) -> K2 -> K3 on `st`: kernel launches and memsets only (no allocation, no host synchronisation, no pageable
 // copy), so the sequence can be stream-captured into a CUDA graph.
 int enqueue_kernels(mcs_extractor* ex, int n_images, const uint8_t* images_dev, int W, int H, int stride, const int* coi_d,
-                    mcs_keypoint* kps_dev, uint8_t* desc_dev, uint8_t* dmask_dev, int* counts_dev, int capacity, cudaStream_t st) {
+                    const FeatureView& out, int capacity, cudaStream_t st) {
     const PyramidGeom& G = ex->G;
     ex->coi_last = coi_d;
     CUDA_CHECK(cudaMemsetAsync(ex->raw_count.p, 0, sizeof(int) * n_images * G.nlevels, st));
@@ -380,53 +384,73 @@ int enqueue_kernels(mcs_extractor* ex, int n_images, const uint8_t* images_dev, 
     for (int l = 0; l < kMaxLevels; ++l) { a.lvl[l] = ex->lvl[l].p; a.blur[l] = ex->blur[l].p; }
     a.tier_stats = ex->tier_on ? ex->tier.p : nullptr;
     CUDA_CHECK(launch_describe(G, ex->G_dev.p, n_images, a, ex->cams.p, ex->luts.p, coi_d, ex->sel_xys.p, ex->sel_count.p,
-                               kps_dev, desc_dev, dmask_dev, counts_dev, capacity, st));
+                               out.kps, out.desc, out.dmask, out.counts, capacity, st));
     if (ex->profiling) CUDA_CHECK(cudaEventRecord(ex->ev[3], st));
     ex->last_n_images = n_images;
     return MCS_OK;
 }
 
 // Validation, geometry, buffer growth and the small host inputs of one call (everything that may allocate, synchronise or read
-// pageable host memory); *coi_d receives the device camera-of-image table the kernels should use.
-int prepare_inputs(mcs_extractor* ex, int n_images, int W, int H, int stride, const uint8_t* masks, const mcs_ocam* cams, int n_cams,
-                   const int* cam_of_image, cudaStream_t st, bool first_chunk, const int* coi_dev, const int** coi_d) {
+// pageable host memory).  `batch_images` sizes the per-launch buffers; the camera-of-image table (`n_coi` entries, one per image
+// of the call) goes to ex->cam_of_image, which every launch of the call reads from its first image on.
+int prepare_inputs(mcs_extractor* ex, int batch_images, int W, int H, int stride, const uint8_t* masks, const mcs_ocam* cams, int n_cams,
+                   const int* cam_of_image, int n_coi, cudaStream_t st) {
     if (n_cams < 1 || n_cams > 64) return mcs_fail(MCS_ERR_INVALID, "n_cams must be in [1,64]");
-    for (int i = 0; i < n_images; ++i)
+    for (int i = 0; i < n_coi; ++i)
         if (cam_of_image[i] < 0 || cam_of_image[i] >= n_cams) return mcs_fail(MCS_ERR_INVALID, "cam_of_image out of range");
     int rc = build_geometry(ex, W, H, stride);
     if (rc) return rc;
-    rc = ensure_batch(ex, n_images);
+    rc = ensure_batch(ex, batch_images);
     if (rc) return rc;
-    if (first_chunk) {
-        rc = upload_small_inputs(ex, W, H, masks, cams, n_cams, st);
-        if (rc) return rc;
-    }
-    *coi_d = coi_dev;
-    if (!coi_dev) {
-        CUDA_CHECK(cudaMemcpyAsync(ex->cam_of_image.p, cam_of_image, sizeof(int) * n_images, cudaMemcpyHostToDevice, st));
-        *coi_d = ex->cam_of_image.p;
-    }
+    CUDA_CHECK(ex->cam_of_image.ensure(n_coi));
+    rc = upload_small_inputs(ex, W, H, masks, cams, n_cams, st);
+    if (rc) return rc;
+    CUDA_CHECK(cudaMemcpyAsync(ex->cam_of_image.p, cam_of_image, sizeof(int) * n_coi, cudaMemcpyHostToDevice, st));
     ex->sf_valid = false;            // shared state (camera table, masks, tables) may now differ from what the cached graph assumes
     return MCS_OK;
 }
 
-int run_pipeline(mcs_extractor* ex, int n_images, const uint8_t* images_dev, int W, int H, int stride,
-                 const uint8_t* masks, const mcs_ocam* cams, int n_cams, const int* cam_of_image,
-                 mcs_keypoint* kps_dev, uint8_t* desc_dev, uint8_t* dmask_dev, int* counts_dev, int capacity,
-                 cudaStream_t st, bool first_chunk = true, const int* coi_dev = nullptr) {
-    const int* coi_d = nullptr;
-    int rc = prepare_inputs(ex, n_images, W, H, stride, masks, cams, n_cams, cam_of_image, st, first_chunk, coi_dev, &coi_d);
-    if (rc) return rc;
-    return enqueue_kernels(ex, n_images, images_dev, W, H, stride, coi_d, kps_dev, desc_dev, dmask_dev, counts_dev, capacity, st);
+// the overflow flags K1 / K2 leave in the status word
+int status_error(int s) {
+    if (s & 1) return mcs_fail(MCS_ERR_CAPACITY, "raw corner list overflow");
+    if (s & 2) return mcs_fail(MCS_ERR_CAPACITY, "octree node table overflow");
+    if (s & 4) return mcs_fail(MCS_ERR_CAPACITY, "selected keypoint slots overflow");
+    return MCS_OK;
 }
 
 int check_status(mcs_extractor* ex, cudaStream_t st) {
     int s = 0;
     CUDA_CHECK(cudaMemcpyAsync(&s, ex->status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
-    if (s & 1) return mcs_fail(MCS_ERR_CAPACITY, "raw corner list overflow");
-    if (s & 2) return mcs_fail(MCS_ERR_CAPACITY, "octree node table overflow");
-    if (s & 4) return mcs_fail(MCS_ERR_CAPACITY, "selected keypoint slots overflow");
+    return status_error(s);
+}
+
+// the checks every extract entry point makes after its own null-argument list (`count`: images, or frames of the stream calls)
+int check_extract_args(const mcs_extractor* ex, int count, int W, int H, int stride, int capacity, const void* dmask) {
+    if (count < 1 || W < 1 || H < 1 || stride < W) return mcs_fail(MCS_ERR_INVALID, "bad image geometry");
+    if (capacity < ex->capacity) return mcs_fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
+    if (ex->p.learn_masks && !dmask) return mcs_fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
+    return MCS_OK;
+}
+
+// the extractor's own feature buffers, grown to n images
+int own_features(mcs_extractor* ex, int n, int capacity, FeatureView* v) {
+    const size_t slots = (size_t)n * capacity, bytes = slots * ex->p.desc_size;
+    CUDA_CHECK(ex->kps.ensure(slots));
+    CUDA_CHECK(ex->desc.ensure(bytes));
+    CUDA_CHECK(ex->dmask.ensure(bytes));
+    CUDA_CHECK(ex->counts.ensure(n));
+    *v = FeatureView{ex->counts.p, ex->kps.p, ex->desc.p, ex->dmask.p};
+    return MCS_OK;
+}
+
+// device -> host copies of n images' counts, keypoints, descriptors and, when `with_dmask`, descriptor masks
+int copy_features(const FeatureView& dst, const FeatureView& src, int n, int capacity, int ds, bool with_dmask, cudaStream_t st) {
+    const size_t slots = (size_t)n * capacity;
+    CUDA_CHECK(cudaMemcpyAsync(dst.counts, src.counts, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(dst.kps, src.kps, sizeof(mcs_keypoint) * slots, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(dst.desc, src.desc, slots * ds, cudaMemcpyDeviceToHost, st));
+    if (with_dmask) CUDA_CHECK(cudaMemcpyAsync(dst.dmask, src.dmask, slots * ds, cudaMemcpyDeviceToHost, st));
     return MCS_OK;
 }
 
@@ -558,18 +582,11 @@ int mcs_extractor_create(const mcs_extractor_params* p, mcs_extractor** out) {
 
 void mcs_extractor_destroy(mcs_extractor* ex) {
     if (!ex) return;
-    cudaSetDevice(ex->device);
-    ex->lut_blob.release(); ex->G_dev.release(); ex->in_images.release();
-    for (int l = 0; l < kMaxLevels; ++l) { ex->lvl[l].release(); ex->blur[l].release(); }
-    ex->masks.release(); ex->cams.release(); ex->cam_of_image.release(); ex->coi_all.release(); ex->raw.release(); ex->node_of.release();
-    ex->raw_count.release(); ex->sel_count.release(); ex->status.release(); ex->counts.release(); ex->sel_xys.release();
-    ex->kps.release(); ex->desc.release(); ex->dmask.release();
+    cudaSetDevice(ex->device);      // the DevBuf members free their memory when `ex` is deleted, on this device
     if (ex->sf_exec) cudaGraphExecDestroy(ex->sf_exec);
     if (ex->pin_in) cudaFreeHost(ex->pin_in);
     if (ex->pin_out) cudaFreeHost(ex->pin_out);
-    ex->match_idx.release(); ex->match_dist.release(); ex->m12.release(); ex->nmat.release(); ex->redo.release(); ex->lut_coef.release(); ex->luts.release(); ex->tier.release(); ex->tile_flags.release();
     for (int i = 0; i < 4; ++i) if (ex->ev[i]) cudaEventDestroy(ex->ev[i]);
-    ex->in_tight.release();
     if (ex->s_copy) cudaStreamDestroy(ex->s_copy);
     if (ex->s_match) cudaStreamDestroy(ex->s_match);
     if (ex->s_out) cudaStreamDestroy(ex->s_out);
@@ -595,13 +612,13 @@ int mcs_extract_batch_device(mcs_extractor* ex, int32_t n_images, const uint8_t*
                              int32_t* counts_dev, int32_t capacity, void* stream) {
     if (!ex || !images_dev || !masks || !cams || !cam_of_image || !kps_dev || !desc_dev || !counts_dev)
         return mcs_fail(MCS_ERR_INVALID, "null argument");
-    if (n_images < 1 || width < 1 || height < 1 || stride < width) return mcs_fail(MCS_ERR_INVALID, "bad image geometry");
-    if (capacity < ex->capacity) return mcs_fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
-    if (ex->p.learn_masks && !dmask_dev) return mcs_fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
+    if (int rc = check_extract_args(ex, n_images, width, height, stride, capacity, dmask_dev)) return rc;
     CUDA_CHECK(cudaSetDevice(ex->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : ex->stream;
-    int rc = run_pipeline(ex, n_images, images_dev, width, height, stride, masks, cams, n_cams, cam_of_image, kps_dev, desc_dev,
-                          dmask_dev, counts_dev, capacity, st);
+    int rc = prepare_inputs(ex, n_images, width, height, stride, masks, cams, n_cams, cam_of_image, n_images, st);
+    if (rc == MCS_OK)
+        rc = enqueue_kernels(ex, n_images, images_dev, width, height, stride, ex->cam_of_image.p,
+                             FeatureView{counts_dev, kps_dev, desc_dev, dmask_dev}, capacity, st);
     if (rc) return rc;
     if (!stream) return check_status(ex, st);
     return MCS_OK;
@@ -618,32 +635,94 @@ int pin_ensure(uint8_t*& p, size_t& cap, size_t need, bool* moved) {
     return MCS_OK;
 }
 
-struct SmallOut { size_t status, counts, kps, desc, dmask, total; };
-SmallOut small_out_layout(int n, int capacity, int ds) {
-    SmallOut o;
-    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
-    o.status = 0; o.counts = 256;
-    o.kps = o.counts + up(sizeof(int) * n);
-    o.desc = o.kps + up(sizeof(mcs_keypoint) * n * capacity);
-    o.dmask = o.desc + up((size_t)n * capacity * ds);
-    o.total = o.dmask + up((size_t)n * capacity * ds);
-    return o;
-}
+constexpr size_t kStatusHeader = 256;    // pinned output staging: the status word, then the feature sections (mcs_packed_layout)
 
 // copy-in, re-pitch, K1..K3, copy-out of one small call between the extractor's pinned staging buffers: capturable
-int enqueue_small(mcs_extractor* ex, int n, int W, int H, int stride, int dpitch, const int* coi_d, int capacity, bool with_dmask, cudaStream_t st) {
+int enqueue_small(mcs_extractor* ex, int n, int W, int H, int stride, int dpitch, const FeatureView& own, int capacity, bool with_dmask,
+                  cudaStream_t st) {
     const int ds = ex->p.desc_size;
-    const SmallOut o = small_out_layout(n, capacity, ds);
     CUDA_CHECK(cudaMemcpyAsync(ex->in_tight.p, ex->pin_in, (size_t)stride * H * n, cudaMemcpyHostToDevice, st));
     launch_repitch(ex->in_tight.p, stride, ex->in_images.p, dpitch, W, (size_t)H * n, st);
     CUDA_CHECK(cudaMemsetAsync(ex->status.p, 0, sizeof(int), st));
-    int rc = enqueue_kernels(ex, n, ex->in_images.p, W, H, dpitch, coi_d, ex->kps.p, ex->desc.p, ex->dmask.p, ex->counts.p, capacity, st);
+    int rc = enqueue_kernels(ex, n, ex->in_images.p, W, H, dpitch, ex->cam_of_image.p, own, capacity, st);
     if (rc) return rc;
-    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.status, ex->status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.counts, ex->counts.p, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.kps, ex->kps.p, sizeof(mcs_keypoint) * n * capacity, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.desc, ex->desc.p, (size_t)n * capacity * ds, cudaMemcpyDeviceToHost, st));
-    if (with_dmask) CUDA_CHECK(cudaMemcpyAsync(ex->pin_out + o.dmask, ex->dmask.p, (size_t)n * capacity * ds, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(ex->pin_out, ex->status.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    return copy_features(packed_view(ex->pin_out + kStatusHeader, n, capacity, ds), own, n, capacity, ds, with_dmask, st);
+}
+
+// A call of at most kGraphMaxImages host images (what cMultiFrame's constructor issues per frame): pinned staging on both sides,
+// and the whole sequence as one graph launch once the inputs repeat.  `own`: the extractor's feature buffers, `out`: the caller's.
+int extract_small(mcs_extractor* ex, int n_images, const uint8_t* images, int width, int height, int stride, int dpitch,
+                  const uint8_t* masks, const mcs_ocam* cams, int n_cams, const int* cam_of_image, const FeatureView& own,
+                  const FeatureView& out, int capacity) {
+    cudaStream_t st = ex->stream;
+    const int ds = ex->p.desc_size;
+    const bool dm = out.dmask != nullptr;
+    const size_t in_bytes = (size_t)stride * height * n_images, mbytes = (size_t)n_cams * width * height;
+    bool moved = false;
+    int rc = pin_ensure(ex->pin_in, ex->pin_in_bytes, in_bytes, &moved);
+    if (rc) return rc;
+    rc = pin_ensure(ex->pin_out, ex->pin_out_bytes, kStatusHeader + mcs_packed_layout(n_images, capacity, ds, nullptr), &moved);
+    if (rc) return rc;
+    if (moved) ex->sf_valid = false;
+    // the caller's last row may hold only `width` valid bytes (a cv::Mat ROI with step > width at the end of its allocation)
+    std::memcpy(ex->pin_in, images, in_bytes - (size_t)(stride - width));
+    const mcs_extractor::SfKey& k = ex->sf_key;
+    bool hit = ex->sf_valid && ex->sf_exec && k.n == n_images && k.w == width && k.h == height && k.stride == stride &&
+               k.capacity == capacity && k.dm == dm && (int)k.cams.size() == n_cams &&
+               std::memcmp(k.coi.data(), cam_of_image, sizeof(int) * n_images) == 0 &&
+               std::memcmp(k.cams.data(), cams, sizeof(mcs_ocam) * n_cams) == 0 && ex->masks_host.size() == mbytes;
+    if (hit) {
+        // the graph goes first and the 1 MB mask comparison runs while the GPU works; if the masks did change the result
+        // is thrown away and the call starts over on the eager path (which uploads the new masks)
+        CUDA_CHECK(cudaGraphLaunch(ex->sf_exec, st));
+        if (std::memcmp(ex->masks_host.data(), masks, mbytes) != 0) {
+            CUDA_CHECK(cudaStreamSynchronize(st));
+            hit = false;
+        } else {
+            ++ex->sf_replays;
+        }
+    }
+    if (!hit) {
+        rc = prepare_inputs(ex, n_images, width, height, dpitch /* K1 reads the re-pitched copy */, masks, cams, n_cams, cam_of_image,
+                            n_images, st);
+        if (rc) return rc;
+        rc = enqueue_small(ex, n_images, width, height, stride, dpitch, own, capacity, dm, st);
+        if (rc) return rc;
+        // record the same sequence for the next call with these inputs (capture executes nothing)
+        if (ex->sf_exec) { cudaGraphExecDestroy(ex->sf_exec); ex->sf_exec = nullptr; }
+        cudaGraph_t graph = nullptr;
+        if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
+            const int crc = enqueue_small(ex, n_images, width, height, stride, dpitch, own, capacity, dm, st);
+            const cudaError_t ce = cudaStreamEndCapture(st, &graph);
+            if (crc == MCS_OK && ce == cudaSuccess && graph && cudaGraphInstantiate(&ex->sf_exec, graph, 0) == cudaSuccess) {
+                mcs_extractor::SfKey& nk = ex->sf_key;
+                nk.n = n_images; nk.w = width; nk.h = height; nk.stride = stride; nk.capacity = capacity;
+                nk.coi.assign(cam_of_image, cam_of_image + n_images);
+                nk.cams.assign(cams, cams + n_cams);
+                nk.dm = dm;
+                ex->sf_valid = true;
+            } else {
+                ex->sf_exec = nullptr;
+                cudaGetLastError();          // a failed capture only costs the shortcut
+            }
+            if (graph) cudaGraphDestroy(graph);
+        } else {
+            cudaGetLastError();
+        }
+    }
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    rc = status_error(*(const int*)ex->pin_out);
+    if (rc) return rc;
+    const FeatureView pin = packed_view(ex->pin_out + kStatusHeader, n_images, capacity, ds);
+    for (int i = 0; i < n_images; ++i) {
+        const size_t nused = (size_t)std::min(std::max(pin.counts[i], 0), capacity);
+        const FeatureView s = feature_at(pin, i, capacity, ds), d = feature_at(out, i, capacity, ds);
+        out.counts[i] = pin.counts[i];
+        std::memcpy(d.kps, s.kps, nused * sizeof(mcs_keypoint));
+        std::memcpy(d.desc, s.desc, nused * ds);
+        if (dm) std::memcpy(d.dmask, s.dmask, nused * ds);
+    }
     return MCS_OK;
 }
 
@@ -654,107 +733,31 @@ int mcs_extract_batch(mcs_extractor* ex, int32_t n_images, const uint8_t* images
                       mcs_keypoint* kps_out, uint8_t* desc_out, uint8_t* dmask_out, int32_t* counts_out, int32_t capacity) {
     if (!ex || !images || !masks || !cams || !cam_of_image || !kps_out || !desc_out || !counts_out)
         return mcs_fail(MCS_ERR_INVALID, "null argument");
-    if (n_images < 1 || width < 1 || height < 1 || stride < width) return mcs_fail(MCS_ERR_INVALID, "bad image geometry");
-    if (capacity < ex->capacity) return mcs_fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
-    if (ex->p.learn_masks && !dmask_out) return mcs_fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
+    if (int rc = check_extract_args(ex, n_images, width, height, stride, capacity, dmask_out)) return rc;
     CUDA_CHECK(cudaSetDevice(ex->device));
     cudaStream_t st = ex->stream;
-    const int ds = ex->p.desc_size;
     // device staging with a 64-byte-aligned pitch so that K1 can use 128-bit loads
     const int dpitch = (width + 63) & ~63;
     const size_t img_bytes = (size_t)dpitch * height;
     const void* before[6] = {ex->in_images.p, ex->kps.p, ex->desc.p, ex->dmask.p, ex->counts.p, ex->in_tight.p};
     CUDA_CHECK(ex->in_images.ensure(img_bytes * n_images + 256));
-    CUDA_CHECK(ex->kps.ensure((size_t)n_images * capacity));
-    CUDA_CHECK(ex->desc.ensure((size_t)n_images * capacity * ds));
-    CUDA_CHECK(ex->dmask.ensure((size_t)n_images * capacity * ds));
-    CUDA_CHECK(ex->counts.ensure(n_images));
+    FeatureView own;
+    int rc = own_features(ex, n_images, capacity, &own);
+    if (rc) return rc;
     // linear H2D + device re-pitch (a 2-D DMA of short rows is several times slower)
     CUDA_CHECK(ex->in_tight.ensure((size_t)stride * height * n_images + 256));
     const void* after[6] = {ex->in_images.p, ex->kps.p, ex->desc.p, ex->dmask.p, ex->counts.p, ex->in_tight.p};
-    bool moved = std::memcmp(before, after, sizeof(before)) != 0;
-
-    if (n_images <= kGraphMaxImages && !ex->profiling && !ex->tier_on) {
-        // ---- per-frame call: pinned staging + the whole sequence as one graph launch once the inputs repeat ----
-        if (n_cams < 1 || n_cams > 64) return mcs_fail(MCS_ERR_INVALID, "n_cams must be in [1,64]");
-        const size_t in_bytes = (size_t)stride * height * n_images, mbytes = (size_t)n_cams * width * height;
-        const SmallOut o = small_out_layout(n_images, capacity, ds);
-        int rc = pin_ensure(ex->pin_in, ex->pin_in_bytes, in_bytes, &moved);
-        if (rc) return rc;
-        rc = pin_ensure(ex->pin_out, ex->pin_out_bytes, o.total, &moved);
-        if (rc) return rc;
-        if (moved) ex->sf_valid = false;
-        // the caller's last row may hold only `width` valid bytes (a cv::Mat ROI with step > width at the end of its allocation)
-        std::memcpy(ex->pin_in, images, in_bytes - (size_t)(stride - width));
-        const mcs_extractor::SfKey& k = ex->sf_key;
-        bool hit = ex->sf_valid && ex->sf_exec && k.n == n_images && k.w == width && k.h == height && k.stride == stride &&
-                   k.capacity == capacity && k.dm == (dmask_out != nullptr) && (int)k.cams.size() == n_cams &&
-                   std::memcmp(k.coi.data(), cam_of_image, sizeof(int) * n_images) == 0 &&
-                   std::memcmp(k.cams.data(), cams, sizeof(mcs_ocam) * n_cams) == 0 && ex->masks_host.size() == mbytes;
-        if (hit) {
-            // the graph goes first and the 1 MB mask comparison runs while the GPU works; if the masks did change the result
-            // is thrown away and the call starts over on the eager path (which uploads the new masks)
-            CUDA_CHECK(cudaGraphLaunch(ex->sf_exec, st));
-            if (std::memcmp(ex->masks_host.data(), masks, mbytes) != 0) {
-                CUDA_CHECK(cudaStreamSynchronize(st));
-                hit = false;
-            } else {
-                ++ex->sf_replays;
-            }
-        }
-        if (!hit) {
-            const int* coi_d = nullptr;
-            rc = prepare_inputs(ex, n_images, width, height, dpitch /* K1 reads the re-pitched copy */, masks, cams, n_cams, cam_of_image, st, true, nullptr, &coi_d);
-            if (rc) return rc;
-            rc = enqueue_small(ex, n_images, width, height, stride, dpitch, coi_d, capacity, dmask_out != nullptr, st);
-            if (rc) return rc;
-            // record the same sequence for the next call with these inputs (capture executes nothing)
-            if (ex->sf_exec) { cudaGraphExecDestroy(ex->sf_exec); ex->sf_exec = nullptr; }
-            cudaGraph_t graph = nullptr;
-            if (cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
-                const int crc = enqueue_small(ex, n_images, width, height, stride, dpitch, coi_d, capacity, dmask_out != nullptr, st);
-                const cudaError_t ce = cudaStreamEndCapture(st, &graph);
-                if (crc == MCS_OK && ce == cudaSuccess && graph && cudaGraphInstantiate(&ex->sf_exec, graph, 0) == cudaSuccess) {
-                    mcs_extractor::SfKey& nk = ex->sf_key;
-                    nk.n = n_images; nk.w = width; nk.h = height; nk.stride = stride; nk.capacity = capacity;
-                    nk.coi.assign(cam_of_image, cam_of_image + n_images);
-                    nk.cams.assign(cams, cams + n_cams);
-                    nk.dm = dmask_out != nullptr;
-                    ex->sf_valid = true;
-                } else {
-                    ex->sf_exec = nullptr;
-                    cudaGetLastError();          // a failed capture only costs the shortcut
-                }
-                if (graph) cudaGraphDestroy(graph);
-            } else {
-                cudaGetLastError();
-            }
-        }
-        CUDA_CHECK(cudaStreamSynchronize(st));
-        const int status = *(const int*)(ex->pin_out + o.status);
-        if (status & 1) return mcs_fail(MCS_ERR_CAPACITY, "raw corner list overflow");
-        if (status & 2) return mcs_fail(MCS_ERR_CAPACITY, "octree node table overflow");
-        if (status & 4) return mcs_fail(MCS_ERR_CAPACITY, "selected keypoint slots overflow");
-        const int* cnt = (const int*)(ex->pin_out + o.counts);
-        for (int i = 0; i < n_images; ++i) {
-            const size_t nused = (size_t)std::min(std::max(cnt[i], 0), capacity), row = (size_t)i * capacity;
-            counts_out[i] = cnt[i];
-            std::memcpy(kps_out + row, ex->pin_out + o.kps + row * sizeof(mcs_keypoint), nused * sizeof(mcs_keypoint));
-            std::memcpy(desc_out + row * ds, ex->pin_out + o.desc + row * ds, nused * ds);
-            if (dmask_out) std::memcpy(dmask_out + row * ds, ex->pin_out + o.dmask + row * ds, nused * ds);
-        }
-        return MCS_OK;
-    }
+    if (std::memcmp(before, after, sizeof(before)) != 0) ex->sf_valid = false;     // the cached graph reads these buffers
+    const FeatureView out{counts_out, kps_out, desc_out, dmask_out};
+    if (n_images <= kGraphMaxImages && !ex->profiling && !ex->tier_on)
+        return extract_small(ex, n_images, images, width, height, stride, dpitch, masks, cams, n_cams, cam_of_image, own, out, capacity);
 
     CUDA_CHECK(cudaMemcpyAsync(ex->in_tight.p, images, (size_t)stride * height * n_images - (size_t)(stride - width), cudaMemcpyHostToDevice, st));
     launch_repitch(ex->in_tight.p, stride, ex->in_images.p, dpitch, width, (size_t)height * n_images, st);
-    int rc = run_pipeline(ex, n_images, ex->in_images.p, width, height, dpitch, masks, cams, n_cams, cam_of_image, ex->kps.p,
-                          ex->desc.p, ex->dmask.p, ex->counts.p, capacity, st);
+    rc = prepare_inputs(ex, n_images, width, height, dpitch, masks, cams, n_cams, cam_of_image, n_images, st);
+    if (rc == MCS_OK) rc = enqueue_kernels(ex, n_images, ex->in_images.p, width, height, dpitch, ex->cam_of_image.p, own, capacity, st);
+    if (rc == MCS_OK) rc = copy_features(out, own, n_images, capacity, ex->p.desc_size, dmask_out != nullptr, st);
     if (rc) return rc;
-    CUDA_CHECK(cudaMemcpyAsync(counts_out, ex->counts.p, sizeof(int) * n_images, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaMemcpyAsync(kps_out, ex->kps.p, sizeof(mcs_keypoint) * n_images * capacity, cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaMemcpyAsync(desc_out, ex->desc.p, (size_t)n_images * capacity * ds, cudaMemcpyDeviceToHost, st));
-    if (dmask_out) CUDA_CHECK(cudaMemcpyAsync(dmask_out, ex->dmask.p, (size_t)n_images * capacity * ds, cudaMemcpyDeviceToHost, st));
     return check_status(ex, st);
 }
 
@@ -887,56 +890,6 @@ int mcs_extractor_get_timings(mcs_extractor* ex, float* ms3) {
     return MCS_OK;
 }
 
-int mcs_match_stream_device(const uint8_t* desc_dev, const uint8_t* dmask_dev, const int32_t* counts_dev, int32_t n_frames,
-                            int32_t n_cams, int32_t capacity, int32_t dim, int32_t K, int32_t* match_idx_dev,
-                            int32_t* match_dist_dev, void* stream) {
-    if (!desc_dev || !counts_dev || !match_idx_dev || !match_dist_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || capacity < 1 || K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
-    if (int rc = check_desc_dim(dim)) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    CUDA_CHECK(launch_hamming_stream(desc_dev, dmask_dev, counts_dev, 0, n_frames * n_cams, n_cams, capacity, dim, K, 0xFFFFFFFFu, match_idx_dev, match_dist_dev, st));
-    return MCS_OK;
-}
-
-int mcs_match_stream_greedy_device(const uint8_t* desc_dev, const uint8_t* dmask_dev, const int32_t* counts_dev, int32_t n_frames,
-                                   int32_t n_cams, int32_t capacity, int32_t dim, int32_t th_low, double nnratio,
-                                   int32_t* matches12_dev, int32_t* nmatches_dev, void* stream) {
-    if (!desc_dev || !counts_dev || !matches12_dev || !nmatches_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535) return mcs_fail(MCS_ERR_INVALID, "bad sizes (capacity must be 1..65535)");
-    if (int rc = check_desc_dim(dim)) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    // K-best list length (the acceptance is exact for any K; K only sets how often the replay rescans).  H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs:
-    // K = 8 16.08 / 16.15 ms per 384-image step (47.9 Mfeatures/s) against 16.85 / 16.79 ms with K = 4.
-    constexpr int K = 8;
-    const size_t n = (size_t)n_frames * n_cams * capacity;
-    int *li = nullptr, *ld = nullptr, *redo = nullptr;
-    CUDA_CHECK(keep_pool_memory());
-    CUDA_CHECK(cudaMallocAsync((void**)&li, n * K * sizeof(int), st));
-    CUDA_CHECK(cudaMallocAsync((void**)&ld, n * K * sizeof(int), st));
-    CUDA_CHECK(cudaMallocAsync((void**)&redo, (size_t)n_frames * n_cams * sizeof(int), st));
-    cudaError_t e = launch_hamming_stream(desc_dev, dmask_dev, counts_dev, 0, n_frames * n_cams, n_cams, capacity, dim, K,
-                                          greedy_dist_bound(th_low, nnratio), li, ld, st);
-    if (e == cudaSuccess)
-        e = launch_stream_replay(li, ld, counts_dev, desc_dev, dmask_dev, dim, 0, n_frames * n_cams, n_cams, capacity, K, th_low, nnratio,
-                                 matches12_dev, nmatches_dev, redo, st);
-    cudaFreeAsync(li, st); cudaFreeAsync(ld, st); cudaFreeAsync(redo, st);
-    CUDA_CHECK(e);
-    return MCS_OK;
-}
-
-int mcs_match_stream_replay_device(const int32_t* match_idx_dev, const int32_t* match_dist_dev, const int32_t* counts_dev,
-                                   const uint8_t* desc_dev, const uint8_t* dmask_dev, int32_t n_frames, int32_t n_cams, int32_t capacity,
-                                   int32_t dim, int32_t K, int32_t th_low, double nnratio, int32_t* matches12_dev, int32_t* nmatches_dev,
-                                   int32_t* redo_dev, void* stream) {
-    if (!match_idx_dev || !match_dist_dev || !counts_dev || !desc_dev || !matches12_dev || !nmatches_dev || !redo_dev)
-        return mcs_fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535 || K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
-    if (int rc = check_desc_dim(dim)) return rc;
-    CUDA_CHECK(launch_stream_replay(match_idx_dev, match_dist_dev, counts_dev, desc_dev, dmask_dev, dim, 0, n_frames * n_cams, n_cams, capacity, K,
-                                    th_low, nnratio, matches12_dev, nmatches_dev, redo_dev, (cudaStream_t)stream));
-    return MCS_OK;
-}
-
 }  // extern "C"
 
 static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_t n_cams, const uint8_t* images, int32_t width,
@@ -946,10 +899,11 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
                              int32_t* matches12_out = nullptr, int32_t* nmatches_out = nullptr, int32_t* redo_out = nullptr) {
     if (!ex || !images || !masks || !cams || !kps_out || !desc_out || !counts_out || !match_idx_out || !match_dist_out)
         return mcs_fail(MCS_ERR_INVALID, "null argument");
-    if (n_frames < 1 || n_cams < 1 || width < 1 || height < 1 || stride < width) return mcs_fail(MCS_ERR_INVALID, "bad geometry");
-    if (capacity < ex->capacity) return mcs_fail(MCS_ERR_CAPACITY, "capacity below mcs_extractor_info.capacity");
-    if (ex->p.learn_masks && !dmask_out) return mcs_fail(MCS_ERR_INVALID, "dmask buffer required when learn_masks is set");
+    // both n_frames and n_cams must be positive
+    if (int rc = check_extract_args(ex, std::min(n_frames, n_cams), width, height, stride, capacity, dmask_out)) return rc;
     if (K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "K must be 1..8");
+    const bool replay = matches12_out != nullptr;
+    if (replay && (!nmatches_out || !redo_out)) return mcs_fail(MCS_ERR_INVALID, "the greedy acceptance needs all three outputs");
     CUDA_CHECK(cudaSetDevice(ex->device));
     cudaStream_t st = ex->stream;
     if (!ex->s_copy) CUDA_CHECK(cudaStreamCreateWithFlags(&ex->s_copy, cudaStreamNonBlocking));
@@ -976,27 +930,19 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
     const size_t tight_img = (size_t)stride * height, pitched_img = (size_t)dpitch * height;
     std::vector<int> coi(n_images);
     for (int i = 0; i < n_images; ++i) coi[i] = i % n_cams;
+    // validated before the stream's own buffers grow (a refused call leaves the cached per-frame graph usable), uploaded before
+    // the first image copy (see upload_small_inputs)
+    if (int rc = prepare_inputs(ex, ipc, width, height, dpitch, masks, cams, n_cams, coi.data(), n_images, st)) return rc;
     CUDA_CHECK(ex->in_tight.ensure(2 * tight_img * ipc + 256));
     CUDA_CHECK(ex->in_images.ensure(pitched_img * ipc + 256));
     // feature buffers: the extractor's own, or the caller's packed exchange buffer (mcs_packed_layout) when one is given
-    mcs_keypoint* kps_d; uint8_t* desc_d; uint8_t* dmask_d; int* counts_d;
-    if (packed_dev) {
-        size_t off[4];
-        mcs_packed_layout(n_images, capacity, ds, off);
-        uint8_t* base = (uint8_t*)packed_dev;
-        counts_d = (int*)(base + off[0]); kps_d = (mcs_keypoint*)(base + off[1]); desc_d = base + off[2]; dmask_d = base + off[3];
-    } else {
-        CUDA_CHECK(ex->kps.ensure((size_t)n_images * capacity));
-        CUDA_CHECK(ex->desc.ensure((size_t)n_images * capacity * ds));
-        CUDA_CHECK(ex->dmask.ensure((size_t)n_images * capacity * ds));
-        CUDA_CHECK(ex->counts.ensure(n_images));
-        kps_d = ex->kps.p; desc_d = ex->desc.p; dmask_d = ex->dmask.p; counts_d = ex->counts.p;
-    }
+    FeatureView feat;
+    if (packed_dev) feat = packed_view(packed_dev, n_images, capacity, ds);
+    else if (int rc = own_features(ex, n_images, capacity, &feat)) return rc;
+    const FeatureView host{counts_out, kps_out, desc_out, dmask_out};
     CUDA_CHECK(ex->match_idx.ensure((size_t)n_images * capacity * K));
     CUDA_CHECK(ex->match_dist.ensure((size_t)n_images * capacity * K));
-    const bool replay = matches12_out != nullptr;
     if (replay) {
-        if (!nmatches_out || !redo_out) return mcs_fail(MCS_ERR_INVALID, "the greedy acceptance needs all three outputs");
         CUDA_CHECK(ex->m12.ensure((size_t)n_images * capacity)); CUDA_CHECK(ex->nmat.ensure(n_images)); CUDA_CHECK(ex->redo.ensure(n_images));
     }
     struct Events {                       // destroyed on every path out of this function
@@ -1015,16 +961,11 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
         CUDA_CHECK(events.add(&ev_feat[c], cudaEventDisableTiming));
         CUDA_CHECK(events.add(&ev_done[c], cudaEventDisableTiming));
     }
-    // Everything asynchronous happens inside enqueue(); whatever it returns, the three streams are drained before this
-    // function returns, because the copies read caller memory and the local cam-of-image table.
+    // The chunks' copies and launches happen inside enqueue(); whatever it returns, the three streams are drained before this
+    // function returns, because the copies read and write caller memory.
     auto enqueue = [&]() -> int {
-    int rc = build_geometry(ex, width, height, dpitch);
-    if (rc == MCS_OK) rc = ensure_batch(ex, ipc);
-    if (rc == MCS_OK) rc = upload_small_inputs(ex, width, height, masks, cams, n_cams, st);     // before the first image copy, see there
-    if (rc) return rc;
-    CUDA_CHECK(ex->coi_all.ensure(n_images));
-    CUDA_CHECK(cudaMemcpyAsync(ex->coi_all.p, coi.data(), sizeof(int) * n_images, cudaMemcpyHostToDevice, st));
-    const uint8_t* dmask_for_match = ex->p.learn_masks ? dmask_d : nullptr;
+    int rc = MCS_OK;
+    const uint8_t* dmask_for_match = ex->p.learn_masks ? feat.dmask : nullptr;
     for (int c = 0; c < n_chunks && rc == MCS_OK; ++c) {
         const int img_lo = chunk_lo[c] * n_cams, nimg = (chunk_lo[c + 1] - chunk_lo[c]) * n_cams;
         if (nimg <= 0) continue;
@@ -1036,31 +977,24 @@ static int extract_match_stream_impl(mcs_extractor* ex, int32_t n_frames, int32_
         CUDA_CHECK(cudaStreamWaitEvent(st, ev_in[c], 0));
         launch_repitch(tight, stride, ex->in_images.p, dpitch, width, (size_t)height * nimg, st);
         CUDA_CHECK(cudaEventRecord(ev_free[c], st));
-        rc = run_pipeline(ex, nimg, ex->in_images.p, width, height, dpitch, masks, cams, n_cams, coi.data() + img_lo,
-                          kps_d + (size_t)img_lo * capacity, desc_d + (size_t)img_lo * capacity * ds,
-                          dmask_d + (size_t)img_lo * capacity * ds, counts_d + img_lo, capacity, st, false, ex->coi_all.p + img_lo);
+        const FeatureView chunk = feature_at(feat, img_lo, capacity, ds);
+        rc = enqueue_kernels(ex, nimg, ex->in_images.p, width, height, dpitch, ex->cam_of_image.p + img_lo, chunk, capacity, st);
         if (rc) break;
         CUDA_CHECK(cudaEventRecord(ev_feat[c], st));                              // features of the chunk are final: their D2H overlaps the matching
         // the matching of chunk c runs on its own stream, so that K1..K3 of chunk c+1 (on `st`) fill the SMs behind its tail;
         // it reads descriptors of this chunk and of the last frame of the previous one, both final at ev_feat[c]
         CUDA_CHECK(cudaStreamWaitEvent(ex->s_match, ev_feat[c], 0));
         // with the greedy acceptance on the device the lists only need the entries that can influence it (kernels.h: greedy_dist_bound)
-        CUDA_CHECK(launch_hamming_stream(desc_d, dmask_for_match, counts_d, img_lo, nimg, n_cams, capacity, ds, K,
+        CUDA_CHECK(launch_hamming_stream(feat.desc, dmask_for_match, feat.counts, img_lo, nimg, n_cams, capacity, ds, K,
                                          replay ? greedy_dist_bound(th_low, nnratio) : 0xFFFFFFFFu, ex->match_idx.p, ex->match_dist.p, ex->s_match));
         if (replay)     // greedy acceptance of SearchByBoW(KF1, KF2) over the lists of this chunk, still on the device
-            CUDA_CHECK(launch_stream_replay(ex->match_idx.p, ex->match_dist.p, counts_d, desc_d, dmask_for_match, ds, img_lo, nimg, n_cams, capacity, K,
-                                            th_low, nnratio, ex->m12.p, ex->nmat.p, ex->redo.p, ex->s_match));
+            CUDA_CHECK(launch_stream_replay(ex->match_idx.p, ex->match_dist.p, feat.counts, feat.desc, dmask_for_match, ds, img_lo, nimg, n_cams,
+                                            capacity, K, th_low, nnratio, ex->m12.p, ex->nmat.p, ex->redo.p, ex->s_match));
         CUDA_CHECK(cudaEventRecord(ev_done[c], ex->s_match));
         cudaStream_t so = ex->s_out;
         CUDA_CHECK(cudaStreamWaitEvent(so, ev_feat[c], 0));
-        CUDA_CHECK(cudaMemcpyAsync(counts_out + img_lo, counts_d + img_lo, sizeof(int) * nimg, cudaMemcpyDeviceToHost, so));
-        CUDA_CHECK(cudaMemcpyAsync(kps_out + (size_t)img_lo * capacity, kps_d + (size_t)img_lo * capacity,
-                                   sizeof(mcs_keypoint) * (size_t)nimg * capacity, cudaMemcpyDeviceToHost, so));
-        CUDA_CHECK(cudaMemcpyAsync(desc_out + (size_t)img_lo * capacity * ds, desc_d + (size_t)img_lo * capacity * ds,
-                                   (size_t)nimg * capacity * ds, cudaMemcpyDeviceToHost, so));
-        if (dmask_out)
-            CUDA_CHECK(cudaMemcpyAsync(dmask_out + (size_t)img_lo * capacity * ds, dmask_d + (size_t)img_lo * capacity * ds,
-                                       (size_t)nimg * capacity * ds, cudaMemcpyDeviceToHost, so));
+        rc = copy_features(feature_at(host, img_lo, capacity, ds), chunk, nimg, capacity, ds, dmask_out != nullptr, so);
+        if (rc) break;
         CUDA_CHECK(cudaStreamWaitEvent(so, ev_done[c], 0));
         CUDA_CHECK(cudaMemcpyAsync(match_idx_out + (size_t)img_lo * capacity * K, ex->match_idx.p + (size_t)img_lo * capacity * K,
                                    sizeof(int) * (size_t)nimg * capacity * K, cudaMemcpyDeviceToHost, so));
@@ -1108,11 +1042,9 @@ int mcs_extract_batch_packed_device(mcs_extractor* ex, int32_t n_images, const u
                                     int32_t stride, const uint8_t* masks, const mcs_ocam* cams, int32_t n_cams,
                                     const int32_t* cam_of_image, void* packed_dev, int32_t capacity, void* stream) {
     if (!ex || !packed_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
-    size_t off[4];
-    mcs_packed_layout(n_images, capacity, ex->p.desc_size, off);
-    uint8_t* base = (uint8_t*)packed_dev;
-    return mcs_extract_batch_device(ex, n_images, images_dev, width, height, stride, masks, cams, n_cams, cam_of_image,
-                                    (mcs_keypoint*)(base + off[1]), base + off[2], base + off[3], (int32_t*)(base + off[0]), capacity, stream);
+    const FeatureView v = packed_view(packed_dev, n_images, capacity, ex->p.desc_size);
+    return mcs_extract_batch_device(ex, n_images, images_dev, width, height, stride, masks, cams, n_cams, cam_of_image, v.kps, v.desc,
+                                    v.dmask, v.counts, capacity, stream);
 }
 
 }  // extern "C"

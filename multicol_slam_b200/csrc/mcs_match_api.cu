@@ -187,6 +187,54 @@ int mcs_hamming_topk(const uint8_t* q, const uint8_t* qmask, int32_t nq, const u
     return MCS_OK;
 }
 
+int mcs_match_stream_device(const uint8_t* desc_dev, const uint8_t* dmask_dev, const int32_t* counts_dev, int32_t n_frames,
+                            int32_t n_cams, int32_t capacity, int32_t dim, int32_t K, int32_t* match_idx_dev,
+                            int32_t* match_dist_dev, void* stream) {
+    if (!desc_dev || !counts_dev || !match_idx_dev || !match_dist_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_frames < 1 || n_cams < 1 || capacity < 1 || K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
+    if (int rc = check_desc_dim(dim)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_CHECK(launch_hamming_stream(desc_dev, dmask_dev, counts_dev, 0, n_frames * n_cams, n_cams, capacity, dim, K, 0xFFFFFFFFu, match_idx_dev, match_dist_dev, st));
+    return MCS_OK;
+}
+
+int mcs_match_stream_greedy_device(const uint8_t* desc_dev, const uint8_t* dmask_dev, const int32_t* counts_dev, int32_t n_frames,
+                                   int32_t n_cams, int32_t capacity, int32_t dim, int32_t th_low, double nnratio,
+                                   int32_t* matches12_dev, int32_t* nmatches_dev, void* stream) {
+    if (!desc_dev || !counts_dev || !matches12_dev || !nmatches_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535) return mcs_fail(MCS_ERR_INVALID, "bad sizes (capacity must be 1..65535)");
+    if (int rc = check_desc_dim(dim)) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    // K-best list length (the acceptance is exact for any K; K only sets how often the replay rescans).  H100 80GB HBM3, 400 W limit, bench.py config 2, 2 alternating runs:
+    // K = 8 16.08 / 16.15 ms per 384-image step (47.9 Mfeatures/s) against 16.85 / 16.79 ms with K = 4.
+    constexpr int K = 8;
+    const int n_images = n_frames * n_cams;
+    const size_t list_bytes = (size_t)n_images * capacity * K * sizeof(int);
+    StreamScratch sc;
+    cudaError_t e = sc.alloc({list_bytes, list_bytes, n_images * sizeof(int)}, st);      // list indices, list distances, redo
+    if (e == cudaSuccess)
+        e = launch_hamming_stream(desc_dev, dmask_dev, counts_dev, 0, n_images, n_cams, capacity, dim, K, greedy_dist_bound(th_low, nnratio),
+                                  sc.at<int>(0), sc.at<int>(1), st);
+    if (e == cudaSuccess)
+        e = launch_stream_replay(sc.at<int>(0), sc.at<int>(1), counts_dev, desc_dev, dmask_dev, dim, 0, n_images, n_cams, capacity, K, th_low,
+                                 nnratio, matches12_dev, nmatches_dev, sc.at<int>(2), st);
+    CUDA_CHECK(sc.release(e));
+    return MCS_OK;
+}
+
+int mcs_match_stream_replay_device(const int32_t* match_idx_dev, const int32_t* match_dist_dev, const int32_t* counts_dev,
+                                   const uint8_t* desc_dev, const uint8_t* dmask_dev, int32_t n_frames, int32_t n_cams, int32_t capacity,
+                                   int32_t dim, int32_t K, int32_t th_low, double nnratio, int32_t* matches12_dev, int32_t* nmatches_dev,
+                                   int32_t* redo_dev, void* stream) {
+    if (!match_idx_dev || !match_dist_dev || !counts_dev || !desc_dev || !matches12_dev || !nmatches_dev || !redo_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_frames < 1 || n_cams < 1 || capacity < 1 || capacity > 65535 || K < 1 || K > 8) return mcs_fail(MCS_ERR_INVALID, "bad sizes (K must be 1..8)");
+    if (int rc = check_desc_dim(dim)) return rc;
+    CUDA_CHECK(launch_stream_replay(match_idx_dev, match_dist_dev, counts_dev, desc_dev, dmask_dev, dim, 0, n_frames * n_cams, n_cams, capacity, K,
+                                    th_low, nnratio, matches12_dev, nmatches_dev, redo_dev, (cudaStream_t)stream));
+    return MCS_OK;
+}
+
 // SearchByBoW(KF1, KF2) (ref :885-966) with the descriptors already on the device: K best unmatched database entries per query
 // on the GPU, sequential greedy replay on the host, further rounds for queries whose list was used up by earlier matches
 static thread_local int g_bf_rounds = 0;

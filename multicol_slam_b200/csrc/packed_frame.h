@@ -1,6 +1,6 @@
-// packed_frame.h -- a frame in packed feature buffers (mcs_packed_frame), as the host entry points of the device searches
-// (mcs_match_api.cu) and of the device bag of words (mcs_bow_api.cu) read it: the per-camera section pointers, and the argument
-// checks the calls share.
+// packed_frame.h -- packed feature buffers (mcs_packed_layout) as the extractor (mcs_api.cu) writes them, and a frame in them
+// (mcs_packed_frame) as the host entry points of the device searches (mcs_match_api.cu) and of the device bag of words
+// (mcs_bow_api.cu) read it: the section pointers, and the argument checks the calls share.
 #pragma once
 #include <vector>
 #include "../../include/mcs_b200.h"
@@ -9,16 +9,34 @@
 
 namespace mcs {
 
+// the features of n images: counts [n], keypoints, descriptors and descriptor masks [n][capacity] (each image's slot row)
+struct FeatureView {
+    int* counts; mcs_keypoint* kps; uint8_t* desc; uint8_t* dmask;
+};
+
+// the four sections of a packed feature buffer of n_images images at `base`
+inline FeatureView packed_view(const void* base, int n_images, int capacity, int dim) {
+    size_t off[4];
+    mcs_packed_layout(n_images, capacity, dim, off);
+    uint8_t* b = (uint8_t*)base;
+    return FeatureView{(int*)(b + off[0]), (mcs_keypoint*)(b + off[1]), b + off[2], b + off[3]};
+}
+
+// `v` from image i on (a NULL dmask stays NULL)
+inline FeatureView feature_at(const FeatureView& v, size_t i, int capacity, int dim) {
+    const size_t slot = i * capacity;
+    return FeatureView{v.counts + i, v.kps + slot, v.desc + slot * dim, v.dmask ? v.dmask + slot * dim : nullptr};
+}
+
 // camera c of a packed frame = global image first_image + c = image (g mod part_images) of part g / part_images
 inline std::vector<PsCamSlots> packed_slots(const mcs_packed_frame& fr, int n_cams, int capacity, int dim) {
-    size_t off[4];
-    const size_t part_bytes = mcs_packed_layout(fr.part_images, capacity, dim, off);
+    const size_t part_bytes = mcs_packed_layout(fr.part_images, capacity, dim, nullptr);
     std::vector<PsCamSlots> slots(n_cams);
     for (int c = 0; c < n_cams; ++c) {
         const int g = fr.first_image + c, p = g / fr.part_images, i = g - p * fr.part_images;
-        const uint8_t* b = (const uint8_t*)fr.packed_dev + (size_t)p * part_bytes;
-        slots[c] = PsCamSlots{(const int*)(b + off[0]) + i, (const mcs_keypoint*)(b + off[1]) + (size_t)i * capacity,
-                              b + off[2] + (size_t)i * capacity * dim, b + off[3] + (size_t)i * capacity * dim};
+        const FeatureView v = feature_at(packed_view((const uint8_t*)fr.packed_dev + (size_t)p * part_bytes, fr.part_images, capacity, dim),
+                                         i, capacity, dim);
+        slots[c] = PsCamSlots{v.counts, v.kps, v.desc, v.dmask};
     }
     return slots;
 }
