@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <string>
 #include "../../include/mcs_b200.h"
+#include "mcs_common.cuh"
 
 // records `msg` for mcs_last_error() on the calling thread and returns `code` (mcs_api.cu)
 int mcs_fail(int code, const std::string& msg);
@@ -25,5 +26,5 @@ inline int mcs_cuda_fail(cudaError_t e, const std::string& what) {
 
 // descriptor widths (bytes) the matchers are built for: MCS_OK, or MCS_ERR_INVALID with the message set
 inline int check_desc_dim(int dim) {
-    return dim == 16 || dim == 32 || dim == 64 ? MCS_OK : mcs_fail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
+    return mcs::desc_width_ok(dim) ? MCS_OK : mcs_fail(MCS_ERR_INVALID, "dim must be 16, 32 or 64");
 }

@@ -104,7 +104,7 @@ group_distance_kernel(const GroupQuery* __restrict__ queries, const int nq, cons
 cudaError_t launch_group_distance(const GroupQuery* queries, int nq, const uint8_t* desc1, const uint8_t* mask1, const uint8_t* desc2,
                                   const uint8_t* mask2, const int* cand, int dim, int* out, cudaStream_t st) {
     if (nq <= 0) return cudaSuccess;
-    if (dim != 16 && dim != 32 && dim != 64) return cudaErrorInvalidValue;
+    if (!desc_width_ok(dim)) return cudaErrorInvalidValue;
     const int blocks = (int)(((long long)nq * 32 + 255) / 256);
     const bool masked = mask1 && mask2;
     with_desc_width(dim, masked, [&](auto W, auto M) {

@@ -60,6 +60,13 @@ inline cudaError_t keep_pool_memory() {
     return e;
 }
 
+// streaming multiprocessors of the current device
+inline cudaError_t sm_count(int& n) {
+    int dev = 0;
+    const cudaError_t e = cudaGetDevice(&dev);
+    return e != cudaSuccess ? e : cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+}
+
 // One stream-ordered scratch block cut into pieces, each starting on a 256-byte boundary; a size of 0 gives a zero-length piece.
 class StreamScratch {
 public:
@@ -96,12 +103,14 @@ inline unsigned greedy_dist_bound(int th_low, double nnratio) {
 cudaError_t launch_stream_replay(const int* list_idx, const int* list_dist, const int* counts, const uint8_t* desc, const uint8_t* dmask,
                                  int dim, int img_lo, int n_images, int n_cams, int capacity, int K, int th_low, double nnratio,
                                  int* matches12, int* nmatches, int* redo, cudaStream_t st);
+// Most dynamic shared memory an acceptance kernel is launched with: the stream matcher keeps the previous image resident only
+// below it, and the key-frame database is refused above it.
+constexpr size_t kReplaySmemMax = 200 * 1024;
 // Dynamic shared memory of bruteforce_replay_kernel: the [32][K] list chunk (indices and distances) and the leader's "already
-// matched" bitmap of the whole database.  The launcher refuses more than kBfReplaySmemMax, so the key-frame database holds at
+// matched" bitmap of the whole database.  The launcher refuses more than kReplaySmemMax, so the key-frame database holds at
 // most bruteforce_max_nd(K) entries.
-constexpr size_t kBfReplaySmemMax = 200 * 1024;
 inline size_t bruteforce_replay_smem(int K, int nd) { return (size_t)64 * K * 4 + (size_t)((nd + 31) / 32) * 4; }
-inline int bruteforce_max_nd(int K) { return (int)((kBfReplaySmemMax - bruteforce_replay_smem(K, 0)) / 4 * 32); }
+inline int bruteforce_max_nd(int K) { return (int)((kReplaySmemMax - bruteforce_replay_smem(K, 0)) / 4 * 32); }
 cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, int K, const uint8_t* q, const uint8_t* qm, const uint8_t* valid1,
                                      const int* seg, int n_seg, int nq_total, const uint8_t* d, const uint8_t* dm, const uint8_t* valid2, int nd, int dim,
                                      int th_low, double nnratio, int* matches12, int* nmatches, cudaStream_t st);

@@ -394,40 +394,34 @@ __global__ void topk_merge_kernel(const unsigned* __restrict__ part, const int s
 cudaError_t launch_hamming_topk(const uint8_t* q, const uint8_t* qmask, int nq, const uint8_t* d, const uint8_t* dmask,
                                 int nd, const uint8_t* db_skip, int dim, int K, unsigned bound, int* topk_idx, int* topk_dist,
                                 cudaStream_t st) {
-    if (K < 1 || K > kTopKMax || (dim != 16 && dim != 32 && dim != 64) || nd >= (1 << kTopkShift)) return cudaErrorInvalidValue;
+    if (K < 1 || K > kTopKMax || !desc_width_ok(dim) || nd >= (1 << kTopkShift)) return cudaErrorInvalidValue;
     if (nq <= 0) return cudaSuccess;
     const int qblocks = (nq + kTopkThreads - 1) / kTopkThreads;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int sms = 0;
+    cudaError_t e = sm_count(sms);
+    if (e != cudaSuccess) return e;
     // enough CTAs for ~4 waves; database chunks are multiples of the tile
     int splits = (4 * sms * 8 + qblocks - 1) / qblocks;
     const int tiles = (nd + kDbTile - 1) / kDbTile;
     splits = max(1, min(splits, tiles));
     const int chunk = ((tiles + splits - 1) / splits) * kDbTile;
     splits = max(1, (nd + chunk - 1) / chunk);
-    // partial top-K lists of the database splits: stream-ordered scratch owned by THIS call (cudaMallocAsync pool), so that
-    // concurrent callers -- the reference runs its matchers from three threads -- and different streams never share it
-    const size_t need = (size_t)splits * nq * kTopKMax * sizeof(unsigned);
-    unsigned* g_part = nullptr;
-    cudaError_t e = keep_pool_memory();
+    // partial top-K lists of the database splits: stream-ordered scratch owned by THIS call, so that concurrent callers -- the
+    // reference runs its matchers from three threads -- and different streams never share it
+    StreamScratch sc;
+    e = sc.alloc({(size_t)splits * nq * kTopKMax * sizeof(unsigned)}, st);
     if (e != cudaSuccess) return e;
-    e = cudaMallocAsync((void**)&g_part, need, st);
-    if (e != cudaSuccess) return e;
+    unsigned* part = sc.at<unsigned>(0);
     dim3 grid(qblocks, splits);
     const bool masked = qmask && dmask;
     with_desc_width(dim, masked, [&](auto W, auto M) {
-        const auto* q32 = (const uint32_t*)q;
-        const auto* qm32 = (const uint32_t*)qmask;
-        const auto* d32 = (const uint32_t*)d;
-        const auto* dm32 = (const uint32_t*)dmask;
-        if (K <= 4) hamming_topk_kernel<W, M, 4><<<grid, kTopkThreads, 0, st>>>(q32, qm32, nq, d32, dm32, nd, db_skip, K, chunk, bound, g_part);
-        else hamming_topk_kernel<W, M, 8><<<grid, kTopkThreads, 0, st>>>(q32, qm32, nq, d32, dm32, nd, db_skip, K, chunk, bound, g_part);
+        with_list_len(K, [&](auto KT) {
+            hamming_topk_kernel<W, M, KT><<<grid, kTopkThreads, 0, st>>>((const uint32_t*)q, (const uint32_t*)qmask, nq, (const uint32_t*)d,
+                                                                         (const uint32_t*)dmask, nd, db_skip, K, chunk, bound, part);
+        });
     });
-    topk_merge_kernel<<<(nq + 127) / 128, 128, 0, st>>>(g_part, splits, nq, K, topk_idx, topk_dist);
-    e = cudaGetLastError();
-    const cudaError_t ef = cudaFreeAsync(g_part, st);        // after the merge in stream order
-    return e != cudaSuccess ? e : ef;
+    topk_merge_kernel<<<(nq + 127) / 128, 128, 0, st>>>(part, splits, nq, K, topk_idx, topk_dist);
+    return sc.release(cudaGetLastError());                   // frees after the merge in stream order
 }
 
 // Stream matching: image i = (frame f, camera c) is matched against image i - n_cams = (f-1, c); both live in
@@ -469,17 +463,15 @@ hamming_stream_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restr
 
 cudaError_t launch_hamming_stream(const uint8_t* desc, const uint8_t* dmask, const int* counts, int img_lo, int img_count,
                                   int n_cams, int capacity, int dim, int K, unsigned bound, int* out_idx, int* out_dist, cudaStream_t st) {
-    if (K < 1 || K > kTopKMax || (dim != 16 && dim != 32 && dim != 64) || capacity > 65535) return cudaErrorInvalidValue;
+    if (K < 1 || K > kTopKMax || !desc_width_ok(dim) || capacity > 65535) return cudaErrorInvalidValue;
     if (img_count < 1) return cudaSuccess;
     dim3 grid((capacity + kTopkThreads - 1) / kTopkThreads, img_count);
     const bool masked = dmask != nullptr;
     with_desc_width(dim, masked, [&](auto W, auto M) {
-        const auto* d32 = (const uint32_t*)desc;
-        const auto* m32 = (const uint32_t*)dmask;
-        if (K <= 4)
-            hamming_stream_kernel<W, M, 4><<<grid, kTopkThreads, 0, st>>>(d32, m32, counts, n_cams, capacity, K, img_lo, bound, out_idx, out_dist);
-        else
-            hamming_stream_kernel<W, M, 8><<<grid, kTopkThreads, 0, st>>>(d32, m32, counts, n_cams, capacity, K, img_lo, bound, out_idx, out_dist);
+        with_list_len(K, [&](auto KT) {
+            hamming_stream_kernel<W, M, KT><<<grid, kTopkThreads, 0, st>>>((const uint32_t*)desc, (const uint32_t*)dmask, counts, n_cams,
+                                                                           capacity, K, img_lo, bound, out_idx, out_dist);
+        });
     });
     return cudaGetLastError();
 }
@@ -733,17 +725,19 @@ __device__ __forceinline__ void replay_helper(CoopSeg* cs, const int* log, const
     }
 }
 
-// Stream matcher: one CTA per image; queries = the image's slots, database = the same camera's image one frame earlier.
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(kReplayThreads)
-stream_replay_kernel(const int* __restrict__ list_idx, const int* __restrict__ list_dist, const int* __restrict__ counts,
-                     const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask,
-                     const int n_cams, const int capacity, const int K, const int img_lo, const int th_low, const double nnratio,
-                     int* __restrict__ matches12, int* __restrict__ nmatches, int* __restrict__ redo) {
-    extern __shared__ int s_mem[];
-    int* s_li = s_mem;                              // [32][K]
-    int* s_ld = s_mem + 32 * K;                     // [32][K]
-    unsigned* s_taken = (unsigned*)(s_mem + 64 * K);   // [(capacity + 31) / 32]
+// Stream matcher: one CTA per image; queries = the image's slots, database = the same camera's image one frame earlier.  The
+// shared memory `s_mem` holds, in order, the database (DB_SMEM: descriptors, then masks, [capacity][WORDS] each), the list chunk
+// ([32][K] indices, [32][K] distances) and the "already matched" bits ([(capacity + 31) / 32]).  Every thread of the CTA calls this.
+template <int WORDS, bool MASKED, bool DB_SMEM>
+__device__ __forceinline__ void stream_replay(const int* __restrict__ list_idx, const int* __restrict__ list_dist, const int* __restrict__ counts,
+                                              const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const int n_cams,
+                                              const int capacity, const int K, const int img_lo, const int th_low, const double nnratio,
+                                              int* __restrict__ matches12, int* __restrict__ nmatches, int* __restrict__ redo, int* s_mem) {
+    uint32_t* s_db = (uint32_t*)s_mem;
+    uint32_t* s_dbm = s_db + (DB_SMEM && MASKED ? (size_t)capacity * WORDS : 0);
+    int* s_li = DB_SMEM ? (int*)(s_dbm + (size_t)capacity * WORDS) : s_mem;
+    int* s_ld = s_li + 32 * K;
+    unsigned* s_taken = (unsigned*)(s_ld + 32 * K);
     __shared__ ReplayShared sh;
     __shared__ __align__(16) uint32_t s_qc[(MASKED ? 2 : 1) * 32 * WORDS];
     const int img = blockIdx.x + img_lo, tid = threadIdx.x;
@@ -753,12 +747,32 @@ stream_replay_kernel(const int* __restrict__ list_idx, const int* __restrict__ l
     const size_t q_row0 = (size_t)img * capacity, d_row0 = has_prev ? (size_t)(img - n_cams) * capacity : 0;
     for (int i = tid; i < (capacity + 31) / 32; i += kReplayThreads) s_taken[i] = 0u;
     for (int i = tid; i < capacity; i += kReplayThreads) matches12[q_row0 + i] = -1;
+    if (DB_SMEM && nq > 0) {
+        const uint4* src = (const uint4*)(desc + d_row0 * WORDS);
+        for (int i = tid; i < nd * WORDS / 4; i += kReplayThreads) ((uint4*)s_db)[i] = src[i];
+        if (MASKED) {
+            const uint4* msrc = (const uint4*)(dmask + d_row0 * WORDS);
+            for (int i = tid; i < nd * WORDS / 4; i += kReplayThreads) ((uint4*)s_dbm)[i] = msrc[i];
+        }
+    }
     __syncthreads();
+    const uint32_t* dd = DB_SMEM ? s_db : desc + d_row0 * WORDS;
+    const uint32_t* dm = MASKED ? (DB_SMEM ? s_dbm : dmask + d_row0 * WORDS) : nullptr;
     const int nm = replay_core<WORDS, MASKED, kReplayThreads>(list_idx + q_row0 * K, list_dist + q_row0 * K, K, nq, nullptr, desc + q_row0 * WORDS,
-                                                              MASKED ? dmask + q_row0 * WORDS : nullptr, desc + d_row0 * WORDS,
-                                                              MASKED ? dmask + d_row0 * WORDS : nullptr, nd, th_low, nnratio,
+                                                              MASKED ? dmask + q_row0 * WORDS : nullptr, dd, dm, nd, th_low, nnratio,
                                                               matches12 + q_row0, s_li, s_ld, s_taken, &sh, s_qc);
     if (tid == 0) { nmatches[img] = nm; redo[img] = 0; }
+}
+
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(kReplayThreads)
+stream_replay_kernel(const int* __restrict__ list_idx, const int* __restrict__ list_dist, const int* __restrict__ counts,
+                     const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask,
+                     const int n_cams, const int capacity, const int K, const int img_lo, const int th_low, const double nnratio,
+                     int* __restrict__ matches12, int* __restrict__ nmatches, int* __restrict__ redo) {
+    extern __shared__ int s_mem[];
+    stream_replay<WORDS, MASKED, false>(list_idx, list_dist, counts, desc, dmask, n_cams, capacity, K, img_lo, th_low, nnratio, matches12,
+                                        nmatches, redo, s_mem);
 }
 
 // The same walk with the previous image's descriptors (and masks) RESIDENT IN SHARED MEMORY: a rescan then reads its 8 x 64 bytes
@@ -767,71 +781,39 @@ stream_replay_kernel(const int* __restrict__ list_idx, const int* __restrict__ l
 // host-facing stream pipeline, whose last acceptance launch is the un-overlapped tail of the call; a full 384-image step keeps the
 // kernel above (2.6 CTAs per SM in flight hide each other's latency, and the extraction kernels of the next step share the SMs).
 // (256 threads as in the kernel above; 1024 -- more warps of its own for the CTA that is alone on its SM -- was no better)
-constexpr int kSmemReplayThreads = kReplayThreads;
 template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(kSmemReplayThreads, 1)
+__global__ void __launch_bounds__(kReplayThreads, 1)
 stream_replay_smem_kernel(const int* __restrict__ list_idx, const int* __restrict__ list_dist, const int* __restrict__ counts,
                           const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask,
                           const int n_cams, const int capacity, const int K, const int img_lo, const int th_low, const double nnratio,
                           int* __restrict__ matches12, int* __restrict__ nmatches, int* __restrict__ redo) {
     extern __shared__ __align__(16) int s_mem[];
-    uint32_t* s_db = (uint32_t*)s_mem;                                     // [capacity][WORDS]
-    uint32_t* s_dbm = s_db + (MASKED ? (size_t)capacity * WORDS : 0);      // [capacity][WORDS]
-    int* s_li = (int*)(s_dbm + (size_t)capacity * WORDS);                  // [32][K]
-    int* s_ld = s_li + 32 * K;                                             // [32][K]
-    unsigned* s_taken = (unsigned*)(s_ld + 32 * K);                        // [(capacity + 31) / 32]
-    __shared__ ReplayShared sh;
-    __shared__ __align__(16) uint32_t s_qc[(MASKED ? 2 : 1) * 32 * WORDS];
-    const int img = blockIdx.x + img_lo, tid = threadIdx.x;
-    const bool has_prev = img >= n_cams;
-    const int nq = has_prev ? min(counts[img], capacity) : 0;
-    const int nd = has_prev ? min(counts[img - n_cams], capacity) : 0;
-    const size_t q_row0 = (size_t)img * capacity, d_row0 = has_prev ? (size_t)(img - n_cams) * capacity : 0;
-    for (int i = tid; i < (capacity + 31) / 32; i += kSmemReplayThreads) s_taken[i] = 0u;
-    for (int i = tid; i < capacity; i += kSmemReplayThreads) matches12[q_row0 + i] = -1;
-    if (nq > 0) {
-        const uint4* src = (const uint4*)(desc + d_row0 * WORDS);
-        for (int i = tid; i < nd * WORDS / 4; i += kSmemReplayThreads) ((uint4*)s_db)[i] = src[i];
-        if (MASKED) {
-            const uint4* msrc = (const uint4*)(dmask + d_row0 * WORDS);
-            for (int i = tid; i < nd * WORDS / 4; i += kSmemReplayThreads) ((uint4*)s_dbm)[i] = msrc[i];
-        }
-    }
-    __syncthreads();
-    const int nm = replay_core<WORDS, MASKED, kSmemReplayThreads>(list_idx + q_row0 * K, list_dist + q_row0 * K, K, nq, nullptr, desc + q_row0 * WORDS,
-                                                              MASKED ? dmask + q_row0 * WORDS : nullptr, s_db, MASKED ? s_dbm : nullptr, nd, th_low,
-                                                              nnratio, matches12 + q_row0, s_li, s_ld, s_taken, &sh, s_qc);
-    if (tid == 0) { nmatches[img] = nm; redo[img] = 0; }
+    stream_replay<WORDS, MASKED, true>(list_idx, list_dist, counts, desc, dmask, n_cams, capacity, K, img_lo, th_low, nnratio, matches12,
+                                       nmatches, redo, s_mem);
 }
 
 cudaError_t launch_stream_replay(const int* list_idx, const int* list_dist, const int* counts, const uint8_t* desc, const uint8_t* dmask,
                                  int dim, int img_lo, int n_images, int n_cams, int capacity, int K, int th_low, double nnratio,
                                  int* matches12, int* nmatches, int* redo, cudaStream_t st) {
     if (n_images < 1) return cudaSuccess;
-    if (capacity > 65535 || (dim != 16 && dim != 32 && dim != 64)) return cudaErrorInvalidValue;
+    if (capacity > 65535 || !desc_width_ok(dim)) return cudaErrorInvalidValue;
     const size_t smem = (size_t)64 * K * 4 + (size_t)((capacity + 31) / 32) * 4;
     const bool masked = dmask != nullptr;
-    // one wave of images: the database of every image fits beside its walk (see stream_replay_smem_kernel)
-    int dev = 0, sms = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int sms = 0;
+    cudaError_t e = sm_count(sms);
     if (e != cudaSuccess) return e;
+    // one wave of images: the database of every image fits beside its walk (see stream_replay_smem_kernel)
     const size_t smem_db = smem + (size_t)capacity * dim * (masked ? 2 : 1) + 16;
-    if (n_images <= sms && smem_db <= 200u * 1024u) {
-        const void* fn = nullptr;
-        with_desc_width(dim, masked, [&](auto W, auto M) { fn = (const void*)stream_replay_smem_kernel<W, M>; });
-        e =cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_db);     // per device, set every time
-        if (e != cudaSuccess) return e;
-        const uint32_t *d32 = (const uint32_t*)desc, *m32 = (const uint32_t*)dmask;
-        void* args[] = {(void*)&list_idx, (void*)&list_dist, (void*)&counts, (void*)&d32, (void*)&m32, (void*)&n_cams, (void*)&capacity, (void*)&K,
-                        (void*)&img_lo, (void*)&th_low, (void*)&nnratio, (void*)&matches12, (void*)&nmatches, (void*)&redo};
-        return cudaLaunchKernel(fn, dim3(n_images), dim3(kSmemReplayThreads), args, smem_db, st);
-    }
+    const bool db_smem = n_images <= sms && smem_db <= kReplaySmemMax;
     with_desc_width(dim, masked, [&](auto W, auto M) {
-        stream_replay_kernel<W, M><<<n_images, kReplayThreads, smem, st>>>(list_idx, list_dist, counts, (const uint32_t*)desc, (const uint32_t*)dmask,
-                                                                         n_cams, capacity, K, img_lo, th_low, nnratio, matches12, nmatches, redo);
+        auto* kern = db_smem ? stream_replay_smem_kernel<W, M> : stream_replay_kernel<W, M>;
+        if (db_smem) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_db);   // per device, set every time
+        if (e == cudaSuccess)
+            kern<<<n_images, kReplayThreads, db_smem ? smem_db : smem, st>>>(list_idx, list_dist, counts, (const uint32_t*)desc,
+                                                                             (const uint32_t*)dmask, n_cams, capacity, K, img_lo, th_low,
+                                                                             nnratio, matches12, nmatches, redo);
     });
-    return cudaGetLastError();
+    return e != cudaSuccess ? e : cudaGetLastError();
 }
 
 // Key-frame database: one CTA per query set (seg[s] .. seg[s+1]) against the same nd database entries, each set with its own
@@ -881,13 +863,13 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
                                      const int* seg, int n_seg, int nq_total, const uint8_t* d, const uint8_t* dm, const uint8_t* valid2, int nd, int dim,
                                      int th_low, double nnratio, int* matches12, int* nmatches, cudaStream_t st) {
     if (n_seg < 1) return cudaSuccess;
-    if (nd >= (1 << kKeyShift) || (dim != 16 && dim != 32 && dim != 64)) return cudaErrorInvalidValue;
+    if (nd >= (1 << kKeyShift) || !desc_width_ok(dim)) return cudaErrorInvalidValue;
     const size_t smem = bruteforce_replay_smem(K, nd);
-    if (smem > kBfReplaySmemMax) return cudaErrorInvalidValue;
+    if (smem > kReplaySmemMax) return cudaErrorInvalidValue;
     const bool masked = qm && dm;
     int dev = 0, sms = 0, coop_ok = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaError_t e = sm_count(sms);
+    if (e == cudaSuccess) e = cudaGetDevice(&dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&coop_ok, cudaDevAttrCooperativeLaunch, dev);
     if (e != cudaSuccess) return e;
     const void* fn = nullptr;
@@ -902,13 +884,14 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kBfReplayThreads, smem);
     if (e != cudaSuccess) return e;
     if (coop_ok && nd >= 32768) helpers = std::max(0, std::min(kCoopMax, per_sm * sms / n_seg - 1));
+    StreamScratch sc;
     CoopSeg* cseg = nullptr; int* clog = nullptr;
     if (helpers) {
-        e = keep_pool_memory();
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&cseg, sizeof(CoopSeg) * n_seg, st);
-        if (e == cudaSuccess) e = cudaMallocAsync((void**)&clog, sizeof(int) * (size_t)std::max(nq_total, 1), st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(cseg, 0, sizeof(CoopSeg) * n_seg, st);
+        e = sc.alloc({sizeof(CoopSeg) * n_seg, sizeof(int) * (size_t)std::max(nq_total, 1)}, st);
         if (e != cudaSuccess) return e;
+        cseg = sc.at<CoopSeg>(0); clog = sc.at<int>(1);
+        e = cudaMemsetAsync(cseg, 0, sizeof(CoopSeg) * n_seg, st);
+        if (e != cudaSuccess) return sc.release(e);
     }
     const uint32_t *q32 = (const uint32_t*)q, *qm32 = (const uint32_t*)qm, *d32 = (const uint32_t*)d, *dm32 = (const uint32_t*)dm;
     void* args[] = {(void*)&list_idx, (void*)&list_dist, (void*)&K, (void*)&q32, (void*)&qm32, (void*)&valid1, (void*)&seg, (void*)&d32, (void*)&dm32,
@@ -917,8 +900,7 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
     const dim3 grid(n_seg * (helpers + 1)), block(kBfReplayThreads);
     if (helpers) e = cudaLaunchCooperativeKernel(fn, grid, block, args, smem, st);       // co-residency guaranteed or the launch fails
     else e = cudaLaunchKernel(fn, grid, block, args, smem, st);
-    if (helpers) { cudaFreeAsync(cseg, st); cudaFreeAsync(clog, st); }
-    return e != cudaSuccess ? e : cudaGetLastError();
+    return sc.release(e != cudaSuccess ? e : cudaGetLastError());
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1008,7 +990,7 @@ cudaError_t launch_window_search(const WindowFrameDev& f, const mcs_window_query
                                  const uint8_t* qmask, int max_cand, int* cand_idx, int* cand_dist, int* cand_count,
                                  cudaStream_t st) {
     if (nq <= 0) return cudaSuccess;
-    if (f.dim != 16 && f.dim != 32 && f.dim != 64) return cudaErrorInvalidValue;
+    if (!desc_width_ok(f.dim)) return cudaErrorInvalidValue;
     const int blocks = (nq * 32 + 255) / 256;
     const bool masked = qmask && f.dmask;
     with_desc_width(f.dim, masked, [&](auto W, auto M) {

@@ -232,7 +232,6 @@ int mcs_search_by_bow_device(const mcs_bow_frame* kfs, int32_t n_kf, const mcs_b
     }
     if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    CUDA_CHECK(keep_pool_memory());
     std::vector<PsCamSlots> kslots;
     std::vector<BowFrameDev> kdev(n_kf);
     kslots.reserve((size_t)n_kf * n_cams);

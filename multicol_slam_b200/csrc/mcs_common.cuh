@@ -70,9 +70,12 @@ __host__ __device__ inline int reflect101(int p, int n) {
     return p;
 }
 
+// descriptor widths (bytes) the Hamming kernels are built for
+inline bool desc_width_ok(const int dim) { return dim == 16 || dim == 32 || dim == 64; }
+
 // The descriptor-width dispatch of the Hamming kernels: calls f(W, M) with W = std::integral_constant<int, dim / 4> (the 32-bit
 // words of a descriptor) and M = std::integral_constant<bool, masked>, so that `kern<W, M>` names one instantiation per width and
-// mask.  Any dim other than 16 and 32 takes the 64-byte path; callers that refuse other widths check dim first.
+// mask.  Any dim other than 16 and 32 takes the 64-byte path; callers that refuse other widths test desc_width_ok first.
 template <class F>
 inline void with_desc_width(const int dim, const bool masked, F&& f) {
     using std::integral_constant;
@@ -83,6 +86,14 @@ inline void with_desc_width(const int dim, const bool masked, F&& f) {
     if (dim == 16) with_mask(integral_constant<int, 4>{});
     else if (dim == 32) with_mask(integral_constant<int, 8>{});
     else with_mask(integral_constant<int, 16>{});
+}
+
+// The list-length dispatch of the K-best kernels: calls f(KT) with KT = std::integral_constant<int, 4> for K <= 4 and
+// std::integral_constant<int, 8> otherwise, the compile-time length of the lists that hold K entries.
+template <class F>
+inline void with_list_len(const int K, F&& f) {
+    if (K <= 4) f(std::integral_constant<int, 4>{});
+    else f(std::integral_constant<int, 8>{});
 }
 
 }  // namespace mcs

@@ -637,25 +637,19 @@ int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const d
         if (cams[c].width != cams[0].width || cams[c].height != cams[0].height)
             return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
     cudaStream_t st = (cudaStream_t)stream;
-    CUDA_CHECK(keep_pool_memory());
-    if (n_points == 0) return MCS_OK;
     // poses, camera models and scale factors: one scratch block, staged in stream order
     const size_t b_pose = (size_t)n_cams * 128, b_cam = sizeof(mcs_ocam) * n_cams, b_sf = 8 * (size_t)n_levels;
-    std::vector<uint8_t> h(2 * b_pose + b_cam + b_sf);
-    std::memcpy(h.data(), mtmc_inv, b_pose);
-    std::memcpy(h.data() + b_pose, mtmc, b_pose);
-    std::memcpy(h.data() + 2 * b_pose, cams, b_cam);
-    std::memcpy(h.data() + 2 * b_pose + b_cam, scale_factors, b_sf);
-    uint8_t* d = nullptr;
-    CUDA_CHECK(cudaMallocAsync((void**)&d, h.size(), st));
-    cudaError_t e = stage_to_device(h.data(), h.size(), d, st);
+    StreamScratch sc;
+    CUDA_CHECK(sc.alloc({b_pose, b_pose, b_cam, b_sf}, st));
+    double* d_mtmc_inv = sc.at<double>(0); double* d_mtmc = sc.at<double>(1); mcs_ocam* d_cams = sc.at<mcs_ocam>(2); double* d_sf = sc.at<double>(3);
+    cudaError_t e = stage_to_device(mtmc_inv, b_pose, d_mtmc_inv, st);
+    if (e == cudaSuccess) e = stage_to_device(mtmc, b_pose, d_mtmc, st);
+    if (e == cudaSuccess) e = stage_to_device(cams, b_cam, d_cams, st);
+    if (e == cudaSuccess) e = stage_to_device(scale_factors, b_sf, d_sf, st);
     if (e == cudaSuccess)
-        e = launch_frustum(n_cams, (const double*)d, (const double*)(d + b_pose), (const mcs_ocam*)(d + 2 * b_pose), masks_dev, n_points,
-                           world_pos_dev, normal_dev, min_dist_dev, max_dist_dev, (const double*)(d + 2 * b_pose + b_cam), n_levels, in_view_dev,
-                           level_dev, proj_x_dev, proj_y_dev, view_cos_dev, skip_dev, st);
-    const cudaError_t ef = cudaFreeAsync(d, st);
-    CUDA_CHECK(e);
-    CUDA_CHECK(ef);
+        e = launch_frustum(n_cams, d_mtmc_inv, d_mtmc, d_cams, masks_dev, n_points, world_pos_dev, normal_dev, min_dist_dev, max_dist_dev, d_sf,
+                           n_levels, in_view_dev, level_dev, proj_x_dev, proj_y_dev, view_cos_dev, skip_dev, st);
+    CUDA_CHECK(sc.release(e));
     return sync_if_null_stream(stream);
 }
 
@@ -678,7 +672,6 @@ int mcs_search_by_projection_device(const void* packed_dev, int32_t n_parts, int
     if (int rc = check_cam_sizes(n_cams, cam_width, cam_height, false)) return rc;
     if (int rc = check_query_bound((long long)mps->n_points * n_cams, "more than 2^24 - 1 (map point, camera) entries in one call")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> slots = packed_slots(frame, n_cams, capacity, dim);
     ProjSearchArgs a{};
     set_searched_frame(a, slots, capacity, dim, cam_width, cam_height, th_high, having_masks, frame_mp_dev, nmatches_dev, status_dev, diag_dev);
@@ -706,7 +699,6 @@ int mcs_search_by_projection_last_device(const mcs_packed_frame* cur, const mcs_
     if (int rc = check_cam_sizes(n_cams, cz.w.data(), cz.h.data(), true)) return rc;
     if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
     ProjSearchLastArgs a{};
     set_searched_frame(a, cs, capacity, dim, cz.w.data(), cz.h.data(), th_high, having_masks, cur_mp_dev, nmatches_dev, status_dev, diag_dev);
@@ -730,7 +722,6 @@ int mcs_window_search_device(const mcs_packed_frame* cur, const mcs_packed_frame
     if (int rc = check_cam_sizes(n_cams, cam_width, cam_height, false)) return rc;
     if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
     WindowSearchDevArgs a{};
     set_searched_frame(a, cs, capacity, dim, cam_width, cam_height, th_high, having_masks, cur_mp_dev, nmatches_dev, status_dev, diag_dev);
@@ -754,7 +745,6 @@ int mcs_search_by_projection_frames_device(const mcs_packed_frame* cur, const mc
     // one query per (last-frame slot, camera)
     if (int rc = check_query_bound((long long)n_cams * n_cams * capacity, "n_cams * n_cams * capacity must stay below 2^24")) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    CUDA_CHECK(keep_pool_memory());
     const std::vector<PsCamSlots> cs = packed_slots(*cur, n_cams, capacity, dim), ls = packed_slots(*last, n_cams, capacity, dim);
     SearchFramesDevArgs a{};
     set_searched_frame(a, cs, capacity, dim, cz.w.data(), cz.h.data(), th_high, having_masks, cur_mp_dev, nmatches_dev, status_dev, diag_dev);

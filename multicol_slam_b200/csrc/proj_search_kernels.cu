@@ -591,9 +591,8 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
     const long long Q = qm.size();
     const int nb = (int)((Q + kQbTile - 1) / kQbTile);
     const size_t db = (size_t)NS * a.dim;
-    int dev = 0, sms = 132;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int sms = 0;
+    cudaError_t e = sm_count(sms);
     if (e != cudaSuccess) return e;
     StreamScratch sc;
     e = sc.alloc({sizeof(mcs_ocam) * a.n_cams, sizeof(double) * a.n_levels, sizeof(PsCamSlots) * a.n_cams,         // staged host inputs

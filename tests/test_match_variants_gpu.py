@@ -64,7 +64,7 @@ def bounded(idx, dist, bound):
 
 
 def replay_uses_smem(n_images, sms, capacity, dim, masked, K):
-    """launch_stream_replay's choice (multicol_slam_b200/csrc/match_kernels.cu:662-668): stream_replay_smem_kernel when the
+    """launch_stream_replay's choice (multicol_slam_b200/csrc/match_kernels.cu:800-807): stream_replay_smem_kernel when the
     launch holds no more images than the device has SMs and the previous image's descriptors (and masks) fit in 200 KB beside
     the walk, stream_replay_kernel otherwise"""
     smem = 64 * K * 4 + (capacity + 31) // 32 * 4
