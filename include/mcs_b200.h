@@ -82,7 +82,7 @@ typedef struct mcs_keypoint {
 
 typedef struct mcs_extractor_info {
     int32_t nlevels;
-    int32_t capacity;                       /* nfeatures + 2*nlevels: max keypoints per image */
+    int32_t capacity;                       /* sum over the levels of max(features_per_level + 2, 16): max keypoints per image */
     int32_t desc_size;
     int32_t features_per_level[MCS_MAX_LEVELS];
     double  scale_factor[MCS_MAX_LEVELS];
@@ -108,6 +108,14 @@ int  mcs_cam_mirror_mask(const mcs_ocam* cam, uint8_t* mask_out);
 int  mcs_extractor_create(const mcs_extractor_params* p, mcs_extractor** out);
 void mcs_extractor_destroy(mcs_extractor* ex);
 int  mcs_extractor_get_info(const mcs_extractor* ex, mcs_extractor_info* info);
+
+/* The octree sizes of width x height images, as the host plans them (no GPU needed).  DistributeOctTree's first pass divides
+ * each of its nIni = cvRound(level width / level height) roots whatever the level's quota, so a level returns up to
+ * max(4 nIni, quota + 2) keypoints.  Out: *node_table (K2's nodes per image and level), nodes_ini[l] and sel_cap[l] (selected
+ * keypoint slots) per level, *capacity (mcs_extractor_info.capacity).  Returns MCS_OK, or the refusal every extract call makes
+ * for that geometry before any launch: MCS_ERR_UNSUPPORTED where the levels' max(4 nIni, quota + 2) sum above the capacity. */
+int  mcs_extractor_octree_plan(const mcs_extractor_params* p, int32_t width, int32_t height, int32_t* node_table,
+                               int32_t* nodes_ini, int32_t* sel_cap, int32_t* capacity);
 
 /* operator() for one image.  Host buffers, synchronous.
  *   mask: h x w bytes, mandatory (the reference throws on an empty mask);

@@ -15,8 +15,8 @@ import pathlib
 
 import numpy as np
 
-from .ctypes_defs import (BowFrame, ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam, PackedFrame,
-                          WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
+from .ctypes_defs import (MAX_LEVELS, BowFrame, ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam,
+                          PackedFrame, WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
 
 _PKG = pathlib.Path(__file__).resolve().parent
 _LIB_PATH = _PKG / "libmcs_b200.so"
@@ -93,6 +93,16 @@ def distort_table(cam):
     out = np.zeros((n.value, row.value), np.float64)
     _check(lib().mcs_cam_distort_table(C.byref(oc), _p(out), n.value, C.byref(n), C.byref(row)))
     return out
+
+
+def octree_plan(width, height, **params):
+    """mcs_extractor_octree_plan (host only): -> (return code, node_table, nodes_ini [nlevels], sel_cap [nlevels], capacity) of
+    width x height images for an extractor made with make_params(**params)"""
+    p = make_params(**params)
+    nt, cap = C.c_int32(0), C.c_int32(0)
+    ni, sc = np.zeros(MAX_LEVELS, np.int32), np.zeros(MAX_LEVELS, np.int32)
+    rc = lib().mcs_extractor_octree_plan(C.byref(p), width, height, C.byref(nt), _p(ni), _p(sc), C.byref(cap))
+    return rc, nt.value, ni[:p.nlevels], sc[:p.nlevels], cap.value
 
 
 def world_to_img(cam, x, y, z):

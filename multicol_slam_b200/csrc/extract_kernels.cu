@@ -108,6 +108,8 @@ octree_kernel(const PyramidGeom* __restrict__ geom, const int cap /* node capaci
     const int minB = kEdge - 3;
     // ---- roots (ref :640-679) ----
     const int nIni = g.nodes_ini;
+    // s_child / s_rank hold one entry per root (the host sizes cap >= 4 nIni, what the first pass can create)
+    if (nIni > cap) { if (tid == 0) { sel_count[b * L + level] = 0; atomicOr(status, 2); } return; }
     for (int i = tid; i < nIni; i += kOctThreads) s_child[i][0] = 0;
     __syncthreads();
     for (int i = tid; i < n; i += kOctThreads) {
@@ -329,9 +331,7 @@ octree_kernel(const PyramidGeom* __restrict__ geom, const int cap /* node capaci
 cudaError_t launch_octree(const PyramidGeom& G, const PyramidGeom* G_dev, int n_images, const uint32_t* raw,
                           const int* raw_count, uint16_t* node_of, uint32_t* sel_xys, int* sel_count, int* status,
                           cudaStream_t st, int level_lo, int level_count) {
-    int cap = 0;
-    for (int l = 0; l < G.nlevels; ++l) cap = max(cap, G.lv[l].quota + 8);
-    cap = (cap + 31) & ~31;
+    const int cap = G.node_cap;
     if (cap > kMaxNodes) return cudaErrorInvalidValue;
     const size_t smem = octree_smem_bytes(cap);
     // the attribute is per device and there may be one extractor per device / thread: set it on every launch (a cheap

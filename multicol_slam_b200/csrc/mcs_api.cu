@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -119,9 +120,43 @@ struct mcs_extractor {
 
 namespace {
 
+// ---- extractor tables: everything that depends only on the params (ref :151-179) ----------------
+int init_tables(mcs_extractor* ex, const mcs_extractor_params* p) {
+    if (p->use_agast) return mcs_fail(MCS_ERR_UNSUPPORTED, "AGAST detector is not built (north star: FAST-9)");
+    if (p->fast_agast_type != 2) return mcs_fail(MCS_ERR_UNSUPPORTED, "only FastFeatureDetector::TYPE_9_16 (type 2) is built");
+    if (p->nlevels < 1 || p->nlevels > kMaxLevels) return mcs_fail(MCS_ERR_INVALID, "nlevels must be in [1,16]");
+    if (p->desc_size != 16 && p->desc_size != 32 && p->desc_size != 64) return mcs_fail(MCS_ERR_INVALID, "desc_size must be 16, 32 or 64");
+    if (p->nfeatures < 1 || !(p->scale_factor > 1.0f) || p->fast_threshold < 1 || p->fast_threshold > 254)
+        return mcs_fail(MCS_ERR_INVALID, "bad nfeatures / scale_factor / fast_threshold");
+    ex->p = *p;
+    const double sfd = (double)p->scale_factor;
+    ex->sf.resize(p->nlevels); ex->isf.resize(p->nlevels); ex->quota.resize(p->nlevels);
+    ex->sf[0] = 1; ex->isf[0] = 1;
+    for (int i = 1; i < p->nlevels; ++i) ex->sf[i] = ex->sf[i - 1] * sfd;
+    const double inv = 1.0 / sfd;
+    for (int i = 1; i < p->nlevels; ++i) ex->isf[i] = ex->isf[i - 1] * inv;
+    const double factor = 1.0 / sfd;
+    double nd = p->nfeatures * (1 - factor) / (1 - std::pow(factor, p->nlevels));
+    int sum = 0;
+    for (int l = 0; l < p->nlevels - 1; ++l) {
+        ex->quota[l] = cv_round(nd);
+        sum += ex->quota[l];
+        nd *= factor;
+    }
+    ex->quota[p->nlevels - 1] = std::max(p->nfeatures - sum, 0);
+    ex->capacity = 0;
+    for (int l = 0; l < p->nlevels; ++l) {
+        if (ex->quota[l] + 8 > kMaxNodes) return mcs_fail(MCS_ERR_UNSUPPORTED, "nfeatures too large for the octree node table");
+        ex->capacity += std::max(ex->quota[l] + 2, 16);
+    }
+    return MCS_OK;
+}
+
 // ---- geometry: everything that depends only on (width, height, params) ------------------------
-int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
-    if (ex->geom_w == W && ex->geom_h == H && ex->geom_stride == in_stride) return MCS_OK;
+struct LutOffsets { size_t xofs, xa0, xa1, yofs, yb0, yb1, cellx, celly, mx0, my0; };
+
+// ex->G without its table pointers, the tables (blob, off) and the refusals of a geometry: host only
+int plan_geometry(mcs_extractor* ex, int W, int H, int in_stride, std::vector<int16_t>& blob, LutOffsets* off) {
     PyramidGeom& G = ex->G;
     std::memset(&G, 0, sizeof(G));
     const int L = ex->p.nlevels;
@@ -130,8 +165,6 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
     G.do_dbrief = ex->p.do_dbrief; G.learn_masks = ex->p.learn_masks;
     if (W >= 4096 || H >= 4096) return mcs_fail(MCS_ERR_UNSUPPORTED, "images larger than 4095 px are not supported");
 
-    std::vector<int16_t> blob;     // all LUTs, int16
-    struct Off { size_t xofs, xa0, xa1, yofs, yb0, yb1, cellx, celly, mx0, my0; } off[kMaxLevels];
     std::vector<int16_t> pmx, pmy;
     size_t raw_off = 0;
     int sel_off = 0;
@@ -246,6 +279,32 @@ int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
     G.sel_total = sel_off; G.raw_total = raw_off; G.cap = ex->capacity;
     G.tiles_total = 0;
     for (int l = 0; l < L; ++l) { G.lv[l].tile_off = G.tiles_total; G.tiles_total += G.lv[l].tiles_x * G.lv[l].tiles_y; }
+    // DistributeOctTree (ref :640-854) divides every one of its nodes_ini roots in its first pass, whatever the quota N: up to
+    // 4 nodes_ini nodes.  Every later pass starts below N and adds at most 3 nodes per division, so it ends below N + 3.  K2's
+    // node table holds the larger of the two (quota + 8 as before); the output slots are fixed at mcs_extractor_create, before
+    // the image size is known, so a geometry whose worst case exceeds them is refused here, before any launch.
+    int nodes = 0, most = 0;
+    for (int l = 0; l < L; ++l) {
+        const LevelGeom& g = G.lv[l];
+        nodes = std::max(nodes, std::max(g.quota + 8, 4 * g.nodes_ini));
+        most += std::max(g.quota + 2, 4 * g.nodes_ini);
+    }
+    G.node_cap = (nodes + 31) & ~31;
+    if (G.node_cap > kMaxNodes) return mcs_fail(MCS_ERR_UNSUPPORTED, "octree roots exceed the node table");
+    if (most > ex->capacity)
+        return mcs_fail(MCS_ERR_UNSUPPORTED, "image too wide for nfeatures: the octree can return more keypoints than the capacity");
+    return MCS_OK;
+}
+
+int build_geometry(mcs_extractor* ex, int W, int H, int in_stride) {
+    if (ex->geom_w == W && ex->geom_h == H && ex->geom_stride == in_stride) return MCS_OK;
+    ex->geom_w = ex->geom_h = ex->geom_stride = 0;      // ex->G is rewritten: a refused size must not leave the previous key on it
+    std::vector<int16_t> blob;     // all LUTs, int16
+    LutOffsets off[kMaxLevels];
+    int rc = plan_geometry(ex, W, H, in_stride, blob, off);
+    if (rc) return rc;
+    PyramidGeom& G = ex->G;
+    const int L = G.nlevels;
     ex->tile_flags_valid = false;
     // kernels of an earlier *_device call on a caller-supplied stream may still read the tables about to be rewritten (a change of the
     // image size is rare: drain the device)
@@ -533,12 +592,8 @@ int mcs_cam_mirror_mask(const mcs_ocam* cam, uint8_t* out) {
 int mcs_extractor_create(const mcs_extractor_params* p, mcs_extractor** out) {
     if (!p || !out) return mcs_fail(MCS_ERR_INVALID, "null argument");
     *out = nullptr;
-    if (p->use_agast) return mcs_fail(MCS_ERR_UNSUPPORTED, "AGAST detector is not built (north star: FAST-9)");
-    if (p->fast_agast_type != 2) return mcs_fail(MCS_ERR_UNSUPPORTED, "only FastFeatureDetector::TYPE_9_16 (type 2) is built");
-    if (p->nlevels < 1 || p->nlevels > kMaxLevels) return mcs_fail(MCS_ERR_INVALID, "nlevels must be in [1,16]");
-    if (p->desc_size != 16 && p->desc_size != 32 && p->desc_size != 64) return mcs_fail(MCS_ERR_INVALID, "desc_size must be 16, 32 or 64");
-    if (p->nfeatures < 1 || !(p->scale_factor > 1.0f) || p->fast_threshold < 1 || p->fast_threshold > 254)
-        return mcs_fail(MCS_ERR_INVALID, "bad nfeatures / scale_factor / fast_threshold");
+    std::unique_ptr<mcs_extractor> ex(new mcs_extractor);
+    if (int rc = init_tables(ex.get(), p)) return rc;
     int dev = 0;
     {
         cudaError_t e = cudaGetDevice(&dev);
@@ -549,35 +604,25 @@ int mcs_extractor_create(const mcs_extractor_params* p, mcs_extractor** out) {
     }
     int rc = upload_consts_once(dev);
     if (rc) return rc;
-    mcs_extractor* ex = new mcs_extractor;
-    ex->p = *p; ex->device = dev;
-    // ref :151-179
-    const double sfd = (double)p->scale_factor;
-    ex->sf.resize(p->nlevels); ex->isf.resize(p->nlevels); ex->quota.resize(p->nlevels);
-    ex->sf[0] = 1; ex->isf[0] = 1;
-    for (int i = 1; i < p->nlevels; ++i) ex->sf[i] = ex->sf[i - 1] * sfd;
-    const double inv = 1.0 / sfd;
-    for (int i = 1; i < p->nlevels; ++i) ex->isf[i] = ex->isf[i - 1] * inv;
-    const double factor = 1.0 / sfd;
-    double nd = p->nfeatures * (1 - factor) / (1 - std::pow(factor, p->nlevels));
-    int sum = 0;
-    for (int l = 0; l < p->nlevels - 1; ++l) {
-        ex->quota[l] = cv_round(nd);
-        sum += ex->quota[l];
-        nd *= factor;
-    }
-    ex->quota[p->nlevels - 1] = std::max(p->nfeatures - sum, 0);
-    ex->capacity = 0;
-    for (int l = 0; l < p->nlevels; ++l) {
-        if (ex->quota[l] + 8 > kMaxNodes) { delete ex; return mcs_fail(MCS_ERR_UNSUPPORTED, "nfeatures too large for the octree node table"); }
-        ex->capacity += std::max(ex->quota[l] + 2, 16);
-    }
-    if (cudaStreamCreateWithFlags(&ex->stream, cudaStreamNonBlocking) != cudaSuccess) {
-        delete ex;
+    ex->device = dev;
+    if (cudaStreamCreateWithFlags(&ex->stream, cudaStreamNonBlocking) != cudaSuccess)
         return mcs_fail(MCS_ERR_CUDA, "cudaStreamCreate failed");
-    }
-    *out = ex;
+    *out = ex.release();
     return MCS_OK;
+}
+
+int mcs_extractor_octree_plan(const mcs_extractor_params* p, int32_t width, int32_t height, int32_t* node_table, int32_t* nodes_ini,
+                              int32_t* sel_cap, int32_t* capacity) {
+    if (!p || !node_table || !nodes_ini || !sel_cap || !capacity) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (width < 1 || height < 1) return mcs_fail(MCS_ERR_INVALID, "bad image geometry");
+    mcs_extractor ex;
+    if (int rc = init_tables(&ex, p)) return rc;
+    std::vector<int16_t> blob;
+    LutOffsets off[kMaxLevels];
+    const int rc = plan_geometry(&ex, width, height, width, blob, off);
+    *node_table = ex.G.node_cap; *capacity = ex.capacity;
+    for (int l = 0; l < p->nlevels; ++l) { nodes_ini[l] = ex.G.lv[l].nodes_ini; sel_cap[l] = ex.G.lv[l].sel_cap; }
+    return rc;
 }
 
 void mcs_extractor_destroy(mcs_extractor* ex) {

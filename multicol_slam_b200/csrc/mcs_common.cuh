@@ -16,7 +16,7 @@ constexpr int kTW = 64, kTH = 32, kHalo = 4;
 constexpr int kTileW = kTW + 2 * kHalo;     // 72
 constexpr int kTileH = kTH + 2 * kHalo;     // 40
 constexpr int kSrcH = 88;                   // staged source rows, enough for scale factors <= 2
-constexpr int kMaxNodes = 2048;             // octree nodes alive at once (>= max quota + 3)
+constexpr int kMaxNodes = 2048;             // octree nodes alive at once (>= max(quota + 8, 4 * nodes_ini) of every level)
 
 // Per-level geometry + look-up tables (device pointers into one blob built by the host).
 struct LevelGeom {
@@ -27,7 +27,7 @@ struct LevelGeom {
     int box_w, box_h;             // TMA box of the staged source region: bytes per row (multiple of 16) x rows, covers every tile
     int raw_cap;                  // capacity of the raw corner list of this level (per image)
     int quota;                    // mnFeaturesPerLevel[l]
-    int sel_cap;                  // quota + 3
+    int sel_cap;                  // max(quota + 3, 4 * nodes_ini): the most keypoints DistributeOctTree returns
     int sel_off;                  // offset of this level's selected-keypoint slots (per image)
     int n_cols, n_rows, w_cell, h_cell;   // FAST cell grid (ref :876-949)
     int nodes_ini;                // octree roots (ref :640)
@@ -53,6 +53,7 @@ struct PyramidGeom {
     int sel_total;                 // sum of sel_cap
     size_t raw_total;              // sum of raw_cap (elements per image)
     int tiles_total;               // sum of tiles_x * tiles_y
+    int node_cap;                  // K2's node table per (image, level): max(quota + 8, 4 * nodes_ini) over the levels, multiple of 32
     LevelGeom lv[kMaxLevels];
 };
 

@@ -635,6 +635,25 @@ void detect_level(Extractor& e, int level) {
     }
 }
 
+// Output slots per image: sum over the levels of max(N + 2, 16), fixed before the image size is known (the extractor's rule)
+int out_capacity(const Extractor& e) {
+    int cap = 0;
+    for (int l = 0; l < e.nlevels; ++l) cap += std::max(e.quota[l] + 2, 16);
+    return cap;
+}
+
+// The most keypoints DistributeOctTree returns for w x h images: its first pass divides every one of the nIni roots (:640)
+// whatever the quota N, and every later pass starts below N and adds at most 3 nodes per division (:693-854)
+int octree_bound(const Extractor& e, int w, int h) {
+    int most = 0;
+    for (int l = 0; l < e.nlevels; ++l) {
+        const int lw = cv_round((double)w * e.isf[l]), lh = cv_round((double)h * e.isf[l]);
+        const int nIni = cv_round((double)(lw - 2 * (EDGE - 3)) / (lh - 2 * (EDGE - 3)));
+        most += std::max(e.quota[l] + 2, 4 * nIni);
+    }
+    return most;
+}
+
 // operator()  :1244-1337
 int extract(Extractor& e, const Img& image, const Img& mask, const mcs_ocam& cam, mcs_keypoint* kps,
             uint8_t* desc, uint8_t* dmask, int capacity) {
@@ -785,7 +804,7 @@ int mcso_extractor_get_info(const mcso_extractor* h, mcs_extractor_info* info) {
     const Extractor& e = *h->e;
     std::memset(info, 0, sizeof(*info));
     info->nlevels = e.nlevels;
-    info->capacity = e.p.nfeatures + 2 * e.nlevels;
+    info->capacity = out_capacity(e);
     info->desc_size = e.p.desc_size;
     for (int l = 0; l < e.nlevels; ++l) {
         info->features_per_level[l] = e.quota[l];
@@ -802,6 +821,8 @@ int mcso_extractor_umax(const mcso_extractor* h, int* out17) {
 int mcso_extract(mcso_extractor* h, const uint8_t* image, int w, int hgt, int stride, const uint8_t* mask,
                  int mstride, const mcs_ocam* cam, mcs_keypoint* kps, uint8_t* desc, uint8_t* dmask, int capacity,
                  int* n_out) {
+    // the extractor refuses such images up front rather than drop keypoints
+    if (octree_bound(*h->e, w, hgt) > out_capacity(*h->e)) return MCS_ERR_UNSUPPORTED;
     Img im(w, hgt), mk(w, hgt);
     for (int y = 0; y < hgt; ++y) {
         std::memcpy(im.row(y), image + (size_t)y * stride, w);

@@ -61,7 +61,18 @@ class RefExtractor:
         self.params = make_params(**kw)
         self.h = C.c_void_p(lib().mcsref_extractor_create(C.byref(self.params)))
         self.nlevels, self.ds = self.params.nlevels, self.params.desc_size
-        self.capacity = self.params.nfeatures + 4 * self.params.nlevels + 64
+
+    def capacity(self, width, height):
+        """most keypoints DistributeOctTree can return for a width x height image: per level max(4 nIni, N + 2).  Its first pass
+        divides each of the nIni = cvRound((maxX - minX) / (maxY - minY)) roots into at most 4 nodes, whatever the quota N; every
+        later division adds at most 3 nodes and starts below N (src/mdBRIEFextractorOct.cpp:640, :693-854)."""
+        q, _, isf, _ = self.tables()
+        cap = 0
+        for l in range(self.nlevels):
+            w, h = lib().mcsref_cv_round(C.c_double(width * isf[l])), lib().mcsref_cv_round(C.c_double(height * isf[l]))
+            n_ini = lib().mcsref_cv_round(C.c_double((w - 44) / (h - 44)))       # maxX - minX = w - 2 * (EDGE_THRESHOLD - 3)
+            cap += max(4 * n_ini, int(q[l]) + 2)
+        return cap
 
     def __del__(self):
         if getattr(self, "h", None):
@@ -78,15 +89,16 @@ class RefExtractor:
         """operator() -> (kps structured array, desc [n,ds] u8, dmask [n,ds] u8)"""
         image = np.ascontiguousarray(image, np.uint8)
         mask = np.ascontiguousarray(mask, np.uint8)
-        cap, ds = self.capacity, self.ds
+        h, w = image.shape
+        cap, ds = self.capacity(w, h), self.ds
         kps = np.zeros(cap, KEYPOINT_DTYPE)
         desc = np.zeros((cap, ds), np.uint8)
         dmask = np.zeros((cap, ds), np.uint8)
         n = C.c_int(0)
         oc = _oc(cam)
-        h, w = image.shape
         st = lib().mcsref_extract(self.h, _p(image), w, h, image.strides[0], _p(mask), mask.strides[0], C.byref(oc),
                                   _p(kps), _p(desc), _p(dmask), cap, C.byref(n))
+        assert st != -4, f"the reference returned {n.value} keypoints, above the bound {cap}"   # MCS_ERR_CAPACITY: nothing copied
         if st != 0:
             raise RuntimeError(f"reference extract failed {st}")
         return kps[:n.value].copy(), desc[:n.value].copy(), dmask[:n.value].copy()

@@ -67,6 +67,27 @@ CASES = [
     ("syn_magnify130_dbrief300", "magnify130", 62, dict(nfeatures=300, **DBRIEF), True),
 ]
 
+# DistributeOctTree's edges, written as ref_octree_*.npz (tests/test_octree_bounds_cpu.py, tests/test_octree_edges_gpu.py): its first
+# pass divides every one of nIni = cvRound(width / height) roots whatever the level's quota, so wide images with small budgets
+# return up to 4 nIni keypoints per level; a zero quota leaves a level with the first pass alone; one-level pyramids at the node
+# table's limit make the ranked pass B run over ~2000 nodes.  Camera spec (index, width, height, "nomask"): rescaled, no mirror mask.
+OCTREE_CASES = [
+    ("wide_4095x600_orb100", (0, 4095, 600, "nomask"), 7, dict(nfeatures=100, **ORB), True),
+    ("wide_2000x250_orb50", (0, 2000, 250, "nomask"), 7, dict(nfeatures=50, **ORB), True),
+    ("wide_3000x400_orb200", (0, 3000, 400, "nomask"), 7, dict(nfeatures=200, **ORB), True),
+    ("wide_1500x200_l4_orb40", (0, 1500, 200, "nomask"), 7, dict(nfeatures=40, nlevels=4, **ORB), True),
+    ("wide_4095x244_l7_orb100", (0, 4095, 244, "nomask"), 71, dict(nfeatures=100, nlevels=7, **ORB), True),
+    ("wide_1920x640_orb50", (1, 1920, 640, "nomask"), 72, dict(nfeatures=50, **ORB), True),
+    ("wide_1920x640_mdbrief50", (2, 1920, 640), 73, dict(nfeatures=50, **MDBRIEF), True),
+    ("wide_3000x400_mdbrief100", (1, 3000, 400), 74, dict(nfeatures=100, **MDBRIEF), True),
+    ("zero_quota_orb8_cam0", 0, 75, dict(nfeatures=8, **ORB), True),
+    ("zero_quota_mdbrief1_cam1", 1, 76, dict(nfeatures=1, **MDBRIEF), True),
+    ("one_level_1280x720_orb2040", (0, 1280, 720, "nomask"), 77, dict(nfeatures=2040, nlevels=1, **ORB), False),
+    ("one_level_1920x1080_mdbrief2040", (1, 1920, 1080), 78, dict(nfeatures=2040, nlevels=1, **MDBRIEF), False),
+    ("one_level_1920x640_orb10", (2, 1920, 640, "nomask"), 79, dict(nfeatures=10, nlevels=1, **ORB), True),
+    ("one_level_4095x600_orb10", (0, 4095, 600, "nomask"), 80, dict(nfeatures=10, nlevels=1, **ORB), True),
+]
+
 
 def make_cam(spec):
     cams = synth.lafida_cams()
@@ -78,7 +99,10 @@ def make_cam(spec):
         c = dict(cams[spec[0]])
         c["mirror_mask"] = 0
         return c
-    return synth.scaled_cam(cams[spec[0]], spec[1], spec[2])
+    c = synth.scaled_cam(cams[spec[0]], spec[1], spec[2])
+    if spec[3:] == ("nomask",):
+        c["mirror_mask"] = 0
+    return c
 
 
 def crc(a):
@@ -86,8 +110,9 @@ def crc(a):
 
 
 def main(only=None):
-    for name, spec, seed, kw, full in CASES:
-        if only and not name.startswith(only):
+    cases = [(f"ref_extract_{name}", *rest) for name, *rest in CASES] + [(f"ref_octree_{name}", *rest) for name, *rest in OCTREE_CASES]
+    for name, spec, seed, kw, full in cases:
+        if only and only not in name:
             continue
         cam = make_cam(spec)
         img = synth.frame(cam, seed)
@@ -105,7 +130,7 @@ def main(only=None):
                    mask_level_crc=np.array([crc(ex.debug_read(l, 1)) for l in range(L)], np.int64))
         if full:
             out.update(kps=k, desc=d, dmask=m)
-        np.savez_compressed(GOLD / f"ref_extract_{name}.npz", **out)
+        np.savez_compressed(GOLD / f"{name}.npz", **out)
         print(f"{name}: {len(k)} keypoints, per level {out['per_level'].tolist()}")
 
 
