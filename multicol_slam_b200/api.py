@@ -59,15 +59,35 @@ def _dptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else None
 
 
+def _contig(a, dtype):
+    """np.ascontiguousarray(a, dtype), None passed through (an optional host array)"""
+    return None if a is None else np.ascontiguousarray(a, dtype)
+
+
 def _stream_handle(stream, dev):
     import torch
     return C.c_void_p(stream.cuda_stream if stream is not None else torch.cuda.current_stream(dev).cuda_stream)
 
 
+def _on_stream(stream, dev):
+    """the context that puts the fills of a call's new output tensors on the stream the call runs on: `stream`, or dev's current one"""
+    import torch
+    return torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(dev))
+
+
+def _ocams(cams):
+    """the camera models as an mcs_ocam array"""
+    return (Ocam * len(cams))(*[as_ocam(c) for c in cams])
+
+
+def _cam_wh(cam_sizes):
+    """[(w, h)] per camera -> (widths, heights) int32 arrays"""
+    return np.ascontiguousarray([s[0] for s in cam_sizes], np.int32), np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
+
+
 def _extract_inputs(masks, cams, cam_of_image=None):
     """the host inputs of an extraction call: masks [n_cams,H,W] u8, the camera models as an mcs_ocam array, cam_of_image i32"""
-    coi = None if cam_of_image is None else np.ascontiguousarray(cam_of_image, np.int32)
-    return np.ascontiguousarray(masks, np.uint8), (Ocam * len(cams))(*[as_ocam(c) for c in cams]), coi
+    return np.ascontiguousarray(masks, np.uint8), _ocams(cams), _contig(cam_of_image, np.int32)
 
 
 def device_count():
@@ -313,9 +333,7 @@ def DescriptorDistance64Masked(a, b, ma, mb, dim=32):
 def hamming_topk(q, d, K=2, qmask=None, dmask=None, db_skip=None):
     q = np.ascontiguousarray(q, np.uint8)
     d = np.ascontiguousarray(d, np.uint8)
-    qmask = None if qmask is None else np.ascontiguousarray(qmask, np.uint8)
-    dmask = None if dmask is None else np.ascontiguousarray(dmask, np.uint8)
-    db_skip = None if db_skip is None else np.ascontiguousarray(db_skip, np.uint8)
+    qmask, dmask, db_skip = (_contig(a, np.uint8) for a in (qmask, dmask, db_skip))
     nq, dim = q.shape
     idx = np.zeros((nq, K), np.int32)
     dist = np.zeros((nq, K), np.int32)
@@ -371,8 +389,7 @@ def match_bruteforce_batch_device(q_t, qmask_t, valid1, seg_start, d_t, dmask_t,
     nd = d_t.shape[0]
     seg = np.ascontiguousarray(seg_start, np.int32)
     assert seg[-1] == nq
-    v1 = None if valid1 is None else np.ascontiguousarray(valid1, np.uint8)
-    v2 = None if valid2 is None else np.ascontiguousarray(valid2, np.uint8)
+    v1, v2 = _contig(valid1, np.uint8), _contig(valid2, np.uint8)
     m12 = np.zeros(nq, np.int32)
     nm = np.zeros(len(seg) - 1, np.int32)
     st = _stream_handle(stream, q_t.device)
@@ -401,8 +418,7 @@ def match_bruteforce_device(q_t, qmask_t, valid1, d_t, dmask_t, valid2, th_low, 
     valid1 / valid2 host uint8 arrays or None.  Returns (nmatches, matches12 numpy)."""
     nq, dim = q_t.shape
     nd = d_t.shape[0]
-    v1 = None if valid1 is None else np.ascontiguousarray(valid1, np.uint8)
-    v2 = None if valid2 is None else np.ascontiguousarray(valid2, np.uint8)
+    v1, v2 = _contig(valid1, np.uint8), _contig(valid2, np.uint8)
     m12 = np.zeros(nq, np.int32)
     n = C.c_int32(0)
     st = _stream_handle(stream, q_t.device)
@@ -419,9 +435,8 @@ class Frame:
         self.keys = np.ascontiguousarray(keys, KEYPOINT_DTYPE)
         self.key_cam = np.ascontiguousarray(key_cam, np.int32)
         self.desc = np.ascontiguousarray(desc, np.uint8)
-        self.dmask = None if dmask is None else np.ascontiguousarray(dmask, np.uint8)
-        self.cam_w = np.ascontiguousarray([s[0] for s in cam_sizes], np.int32)
-        self.cam_h = np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
+        self.dmask = _contig(dmask, np.uint8)
+        self.cam_w, self.cam_h = _cam_wh(cam_sizes)
         self.scale_factors = np.ascontiguousarray(scale_factors, np.float64)
 
     @staticmethod
@@ -456,7 +471,7 @@ class MapPoints:
         self.proj_y = np.ascontiguousarray(proj_y, np.float64)
         self.view_cos = np.ascontiguousarray(view_cos, np.float64)
         self.desc = np.ascontiguousarray(desc, np.uint8)
-        self.dmask = None if dmask is None else np.ascontiguousarray(dmask, np.uint8)
+        self.dmask = _contig(dmask, np.uint8)
 
     def view(self):
         v = MapPointView()
@@ -471,7 +486,7 @@ class MapPoints:
 def window_search(frame, queries, qdesc, qmask=None, max_cand=64):
     queries = np.ascontiguousarray(queries, WINDOW_QUERY_DTYPE)
     qdesc = np.ascontiguousarray(qdesc, np.uint8)
-    qmask = None if qmask is None else np.ascontiguousarray(qmask, np.uint8)
+    qmask = _contig(qmask, np.uint8)
     nq = len(queries)
     idx = np.zeros((nq, max_cand), np.int32)
     dist = np.zeros((nq, max_cand), np.int32)
@@ -489,12 +504,11 @@ def frame_prepare(keys, key_cam, cams):
     keys = np.ascontiguousarray(keys, KEYPOINT_DTYPE)
     key_cam = np.ascontiguousarray(key_cam, np.int32)
     nc, n = len(cams), len(keys)
-    ocs = (Ocam * nc)(*[as_ocam(c) for c in cams])
     rays = np.zeros((n, 3))
     start = np.zeros(nc * 64 * 48 + 1, np.int32)
     items = np.zeros(max(n, 1), np.int32)
     ning = C.c_int32(0)
-    _check(lib().mcs_frame_prepare(_p(keys), _p(key_cam), n, ocs, nc, _p(rays), _p(start), _p(items), C.byref(ning)))
+    _check(lib().mcs_frame_prepare(_p(keys), _p(key_cam), n, _ocams(cams), nc, _p(rays), _p(start), _p(items), C.byref(ning)))
     return rays, start, items[:ning.value].copy()
 
 
@@ -510,12 +524,11 @@ def project_mappoints(mtmc_inv, mtmc, cams, masks, world_pos, normal, min_dist, 
     dmax = np.ascontiguousarray(max_dist, np.float64)
     sf = np.ascontiguousarray(scale_factors, np.float64)
     nc, n = len(cams), len(pos)
-    ocs = (Ocam * nc)(*[as_ocam(c) for c in cams])
     in_view = np.zeros((n, nc), np.uint8)
     level = np.zeros((n, nc), np.int32)
     px, py, vc = np.zeros((n, nc)), np.zeros((n, nc)), np.zeros((n, nc))
-    _check(lib().mcs_project_mappoints(nc, _p(mi), _p(mm), ocs, _p(masks), n, _p(pos), _p(nrm), _p(dmin), _p(dmax), _p(sf), len(sf),
-                                       _p(in_view), _p(level), _p(px), _p(py), _p(vc)))
+    _check(lib().mcs_project_mappoints(nc, _p(mi), _p(mm), _ocams(cams), _p(masks), n, _p(pos), _p(nrm), _p(dmin), _p(dmax), _p(sf),
+                                       len(sf), _p(in_view), _p(level), _p(px), _p(py), _p(vc)))
     return in_view, level, px, py, vc
 
 
@@ -530,13 +543,12 @@ def project_mappoints_device(mtmc_inv, mtmc, cams, masks_t, world_t, normal_t, m
     mm = np.ascontiguousarray(mtmc, np.float64)
     sf = np.ascontiguousarray(scale_factors, np.float64)
     nc, n, dev = len(cams), world_t.shape[0], world_t.device
-    ocs = (Ocam * nc)(*[as_ocam(c) for c in cams])
     if out is None:
         out = (torch.zeros((n, nc), dtype=torch.uint8, device=dev), torch.zeros((n, nc), dtype=torch.int32, device=dev),
                *(torch.zeros((n, nc), dtype=torch.float64, device=dev) for _ in range(3)))
-    _check(lib().mcs_project_mappoints_device(nc, _p(mi), _p(mm), ocs, _dptr(masks_t), n, _dptr(world_t), _dptr(normal_t), _dptr(min_dist_t),
-                                              _dptr(max_dist_t), _p(sf), len(sf), _dptr(skip_t), *(_dptr(t) for t in out),
-                                              _stream_handle(stream, dev)))
+    _check(lib().mcs_project_mappoints_device(nc, _p(mi), _p(mm), _ocams(cams), _dptr(masks_t), n, _dptr(world_t), _dptr(normal_t),
+                                              _dptr(min_dist_t), _dptr(max_dist_t), _p(sf), len(sf), _dptr(skip_t),
+                                              *(_dptr(t) for t in out), _stream_handle(stream, dev)))
     return out
 
 
@@ -589,7 +601,7 @@ def search_windows(frame, queries, qdesc, qmask, query_tag, rule, nnratio, thres
     """mcs_search_windows: generic projection-window search + greedy acceptance (see include/mcs_b200.h)."""
     queries = np.ascontiguousarray(queries, WINDOW_QUERY_DTYPE)
     qdesc = np.ascontiguousarray(qdesc, np.uint8)
-    qmask = None if qmask is None else np.ascontiguousarray(qmask, np.uint8)
+    qmask = _contig(qmask, np.uint8)
     tags = np.ascontiguousarray(query_tag, np.int32)
     assigned = np.ascontiguousarray(assigned, np.int32)
     n = C.c_int32(0)
@@ -693,6 +705,41 @@ def _predict_level(scale_factors, ratio):
     return min(int(np.searchsorted(scale_factors, ratio, side="left")), len(scale_factors) - 1)
 
 
+def _sim3_rig(rig, Scw):
+    """the rig with its pose replaced by the rigid part of the similarity Scw: camSys.Set_M_t(invMat(Rt2Hom(Rcw, tcw)))
+    (ref :1576-1584, :2279-2287)"""
+    S = np.asarray(Scw, np.float64)
+    sR = S[:3, :3]
+    inv_s = 1.0 / float(np.sqrt(sR[0, 0] * sR[0, 0] + sR[0, 1] * sR[0, 1] + sR[0, 2] * sR[0, 2]))
+    T = np.eye(4)
+    T[:3, :3], T[:3, 3] = inv_s * sR, inv_s * S[:3, 3]
+    return Rig(rig.cams, rig.M_c, inv_rigid(T))
+
+
+def _project(rig, scale_factors, world_pos, min_dist, max_dist, ids, cams, float_dist):
+    """projection front end of the Fuse overloads and SearchByProjection(KF, Scw) for map point ids[k] in camera cams[k, j] of rig:
+    WorldToCamHom_fast -> isPointInMirrorMask -> distance range -> predicted level (ref :1288-1318).
+    Returns uv [n, m, 2], ok [n, m] u8 (inside the mirror mask and the distance range), level [n, m] i32."""
+    world_pos = np.asarray(world_pos, np.float64)
+    Ow = rig.M_t[:3, 3].copy()
+    uv, ok, lvl = np.zeros(cams.shape + (2,)), np.zeros(cams.shape, np.uint8), np.zeros(cams.shape, np.int32)
+    for (k, j), c in np.ndenumerate(cams):
+        i, c = int(ids[k]), int(c)
+        p = world_pos[i]
+        u, v, _ = rig.world_to_cam(c, p)
+        if not rig.in_mirror_mask(c, u, v):
+            continue
+        po = p - Ow
+        d = float(np.sqrt(po[0] * po[0] + po[1] * po[1] + po[2] * po[2]))
+        if float_dist:
+            d = float(np.float32(d))                      # `const float dist3D = cv::norm(PO);` (ref :1301, :1472)
+        if d < min_dist[i] or d > max_dist[i]:
+            continue
+        uv[k, j] = (u, v); ok[k, j] = 1
+        lvl[k, j] = _predict_level(scale_factors, d / min_dist[i])
+    return uv, ok, lvl
+
+
 def _packed_pair(cur, last):
     """the mcs_packed_frame records, by reference, of cur / last = (packed uint8 cuda tensor, n_parts, part_images, first_image)"""
     return [C.byref(PackedFrame(f[0].data_ptr(), *f[1:4])) for f in (cur, last)]
@@ -740,8 +787,7 @@ class cORBmatcher:
         int32 cuda tensor [n_cams * capacity] indexed by slot, updated in place.  Asynchronous on `stream`.  Returns (nmatches [1],
         status [1], frame_mp_t), plus diag [4] when diag is set, as cuda tensors."""
         dim = mps_dev.desc.shape[1]
-        cw = np.ascontiguousarray([s[0] for s in cam_sizes], np.int32)
-        ch = np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
+        cw, ch = _cam_wh(cam_sizes)
         sf = np.ascontiguousarray(scale_factors, np.float64)
         out, tail = _search_outputs(out, diag, stream, packed_t.device)
         mv = mps_dev.view()
@@ -760,14 +806,13 @@ class cORBmatcher:
         capacity] u8 cuda or None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4] when
         diag is set, as cuda tensors."""
         nc = len(rig_cur.cams)
-        ocs = (Ocam * nc)(*[as_ocam(c) for c in rig_cur.cams])
         sf = np.ascontiguousarray(scale_factors, np.float64)
         mi = np.ascontiguousarray(rig_cur.MtMc_inv, np.float64)
         out, tail = _search_outputs(out, diag, stream, cur[0].device)
-        _check(lib().mcs_search_by_projection_last_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t), len(sf),
-                                                          _p(sf), _p(mi), _dptr(last_mp_t), _dptr(last_outlier_t), world_t.shape[0],
-                                                          _dptr(world_t), _dptr(bad_t), th, self.TH_HIGH_, int(self.havingMasks),
-                                                          _dptr(cur_mp_t), *tail))
+        _check(lib().mcs_search_by_projection_last_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, _ocams(rig_cur.cams),
+                                                          _dptr(masks_t), len(sf), _p(sf), _p(mi), _dptr(last_mp_t), _dptr(last_outlier_t),
+                                                          world_t.shape[0], _dptr(world_t), _dptr(bad_t), th, self.TH_HIGH_,
+                                                          int(self.havingMasks), _dptr(cur_mp_t), *tail))
         return _search_result(out, cur_mp_t, diag)
 
     def WindowSearchDevice(self, cur, last, capacity, cam_sizes, last_mp_t, window, cur_mp_t, min_level=0, max_level=2**31 - 1, bad_t=None,
@@ -779,8 +824,7 @@ class cORBmatcher:
         every id when None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4] when diag is set,
         as cuda tensors."""
         nc = len(cam_sizes)
-        cw = np.ascontiguousarray([s[0] for s in cam_sizes], np.int32)
-        ch = np.ascontiguousarray([s[1] for s in cam_sizes], np.int32)
+        cw, ch = _cam_wh(cam_sizes)
         n_points = bad_t.shape[0] if bad_t is not None else 2**31 - 1
         out, tail = _search_outputs(out, diag, stream, cur[0].device)
         _check(lib().mcs_window_search_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, _p(cw), _p(ch), _dptr(last_mp_t),
@@ -797,13 +841,12 @@ class cORBmatcher:
         bad_t [n_points] u8 cuda or None.  Asynchronous on `stream`.  Returns (nmatches [1], status [1], cur_mp_t), plus diag [4]
         when diag is set, as cuda tensors."""
         nc = len(rig_cur.cams)
-        ocs = (Ocam * nc)(*[as_ocam(c) for c in rig_cur.cams])
         mi = np.ascontiguousarray(rig_cur.MtMc_inv, np.float64)
         out, tail = _search_outputs(out, diag, stream, cur[0].device)
-        _check(lib().mcs_search_by_projection_frames_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, ocs, _dptr(masks_t),
-                                                            _p(mi), _dptr(last_mp_t), world_t.shape[0], _dptr(world_t), _dptr(bad_t),
-                                                            int(window), self.mfNNratio, self.TH_HIGH_, int(self.havingMasks),
-                                                            _dptr(cur_mp_t), *tail))
+        _check(lib().mcs_search_by_projection_frames_device(*_packed_pair(cur, last), nc, capacity, self.mbFeatDim, _ocams(rig_cur.cams),
+                                                            _dptr(masks_t), _p(mi), _dptr(last_mp_t), world_t.shape[0], _dptr(world_t),
+                                                            _dptr(bad_t), int(window), self.mfNNratio, self.TH_HIGH_,
+                                                            int(self.havingMasks), _dptr(cur_mp_t), *tail))
         return _search_result(out, cur_mp_t, diag)
 
     def SearchForInitialization(self, F1, F2, vbPrevMatched, windowSize=10):
@@ -818,6 +861,20 @@ class cORBmatcher:
             vbPrevMatched[...] = prev
         return n.value, m12
 
+    def _masks(self, *masks):
+        """the descriptor masks a search reads: each of `masks` as u8 when havingMasks and none of them is None, else None for
+        each; one mask in, one out"""
+        use = self.havingMasks and all(m is not None for m in masks)
+        masks = tuple(np.ascontiguousarray(m, np.uint8) if use else None for m in masks)
+        return masks if len(masks) > 1 else masks[0]
+
+    def _best_free(self, KF, q, qdesc, qmask, rule, threshold, _sw=None):
+        """RULE_BEST_FREE / RULE_FIRST_FREE on the queries q against KF -> the best keypoint of KF per query (-1 none).  These rules
+        ignore the tags and write each query's answer to assigned[query], so `assigned` has max(n_queries, n_keys) entries."""
+        _, res = (search_windows if _sw is None else _sw)(KF, q, qdesc, self._masks(qmask), np.zeros(len(q), np.int32), rule,
+                                                           self.mfNNratio, threshold, np.full(max(len(q), len(KF.keys)), -1, np.int32))
+        return res[:len(q)]
+
     def WindowSearch(self, F1, F2, windowSize, valid1, minScaleLevel=0, maxScaleLevel=2**31 - 1, _sw=None):
         """WindowSearch(F1, F2, windowSize, vpMapPointMatches2, minScaleLevel, maxScaleLevel) (ref :326-474).
         valid1[i1]: F1 keypoint i1 carries a non-bad map point.  Returns (nmatches, vnMatches21: F1 index per F2 keypoint)."""
@@ -826,87 +883,70 @@ class cORBmatcher:
                              ((maxScaleLevel >= 2**31 - 1) | (lv <= maxScaleLevel)))
         q = _queries(F1.key_cam[sel], F1.keys["x"][sel].astype(np.float64), F1.keys["y"][sel].astype(np.float64),
                      float(windowSize), -1, -1, sel)
-        return (search_windows if _sw is None else _sw)(F2, q, F1.desc, F1.dmask if self.havingMasks else None, sel, RULE_RATIO,
-                                                        self.mfNNratio, self.TH_HIGH_, np.full(len(F2.keys), -1, np.int32))
+        return (search_windows if _sw is None else _sw)(F2, q, F1.desc, self._masks(F1.dmask), sel, RULE_RATIO, self.mfNNratio,
+                                                        self.TH_HIGH_, np.full(len(F2.keys), -1, np.int32))
 
-    def SearchByProjectionFrames(self, F1, F2, windowSize, valid1, uv, in_mask, assigned2=None):
+    def SearchByProjectionFrames(self, F1, F2, windowSize, valid1, uv, in_mask, assigned2=None, mp1=None, _sw=None):
         """SearchByProjection(F1, F2, windowSize, vpMapPointMatches2) (ref :476-573).  valid1[i1]: keypoint i1 of F1 carries a
         map point that is not bad, not already found in F2 and not seen before in F1 (the caller's bookkeeping, :490-499);
         uv[i1, c] = projection of that map point into camera c of F2 (WorldToCamHom_fast), in_mask[i1, c] = isPointInMirrorMask.
-        assigned2 = F2.mvpMapPoints as indices (-1 = NULL).  Returns (nmatches, assigned2 with F1 indices for new matches)."""
-        n1, nc = len(F1.keys), len(F2.cam_w)
+        assigned2 = F2.mvpMapPoints as indices (-1 = NULL); mp1: map point id per F1 keypoint, when given a new match writes mp1[i1]
+        instead of i1.  Returns (nmatches, assigned2 with F1 indices (or mp1 ids) for new matches)."""
         if assigned2 is None:
             assigned2 = np.full(len(F2.keys), -1, np.int32)
         i1, c = np.nonzero((np.asarray(valid1) != 0)[:, None] & (np.asarray(in_mask) != 0))      # i1 outer, camera inner
         lv = F1.keys["octave"][i1]
         q = _queries(c, np.asarray(uv)[i1, c, 0], np.asarray(uv)[i1, c, 1], float(windowSize), lv, lv, i1)
-        return search_windows(F2, q, F1.desc, F1.dmask if self.havingMasks else None, i1, RULE_RATIO, self.mfNNratio,
-                              self.TH_HIGH_, assigned2)
+        return (search_windows if _sw is None else _sw)(F2, q, F1.desc, self._masks(F1.dmask), i1 if mp1 is None else np.asarray(mp1)[i1],
+                                                        RULE_RATIO, self.mfNNratio, self.TH_HIGH_, assigned2)
 
-    def SearchByProjectionLast(self, CurrentFrame, LastFrame, th, valid_last, uv, in_mask, assigned_cur=None):
+    def SearchByProjectionLast(self, CurrentFrame, LastFrame, th, valid_last, uv, in_mask, assigned_cur=None, last_mp=None, _sw=None):
         """SearchByProjection(CurrentFrame, LastFrame, th) (ref :1990-2118, motion model).  valid_last[i]: LastFrame keypoint i has a
         non-bad, non-outlier map point; uv[i] = its projection into its own camera of CurrentFrame, in_mask[i] = mirror-mask test.
-        Returns (nmatches, CurrentFrame.mvpMapPoints as LastFrame indices)."""
+        last_mp: map point id per LastFrame keypoint, when given a new match writes last_mp[i] instead of i.
+        Returns (nmatches, CurrentFrame.mvpMapPoints as LastFrame indices (or last_mp ids))."""
         if assigned_cur is None:
             assigned_cur = np.full(len(CurrentFrame.keys), -1, np.int32)
         sel = np.flatnonzero((np.asarray(valid_last) != 0) & (np.asarray(in_mask) != 0))
         lv = LastFrame.keys["octave"][sel]
         r = th * CurrentFrame.scale_factors[lv]
         q = _queries(LastFrame.key_cam[sel], np.asarray(uv)[sel, 0], np.asarray(uv)[sel, 1], r, lv - 1, lv + 1, sel)
-        return search_windows(CurrentFrame, q, LastFrame.desc, LastFrame.dmask if self.havingMasks else None, sel, RULE_BEST,
-                              self.mfNNratio, self.TH_HIGH_, assigned_cur)
+        return (search_windows if _sw is None else _sw)(CurrentFrame, q, LastFrame.desc, self._masks(LastFrame.dmask),
+                                                        sel if last_mp is None else np.asarray(last_mp)[sel], RULE_BEST, self.mfNNratio,
+                                                        self.TH_HIGH_, assigned_cur)
 
-    def FuseCandidates(self, KF, uv, in_mask, level, th, mp_desc, mp_dmask=None, first_wins=False):
+    def FuseCandidates(self, KF, uv, in_mask, level, th, mp_desc, mp_dmask=None, first_wins=False, points=None, _sw=None):
         """Matching core of Fuse(pKF, curKF, vpMapPoints, th) (ref :1265-1418) and Fuse(pKF, Scw, vpPoints, th) (:1570-1719): for map
         point i and camera c (in_mask[i,c]) the best keypoint of KF within th*scale[level] of uv[i,c] on levels {level-1, level},
         accepted when its distance <= TH_LOW_.  first_wins=True is Fuse(pKF, vpMapPoints, th) (:1420-1568) as the reference behaves:
-        the distance is discarded there, the first in-level candidate of the window wins (MCS_RULE_FIRST_FREE).
+        the distance is discarded there, the first in-level candidate of the window wins (MCS_RULE_FIRST_FREE).  points: map point
+        id per row i of uv, when given its queries read mp_desc[points[i]] instead of mp_desc[i].
         Returns best [n, n_cams] (keypoint index or -1); replacing / adding observations stays with the caller (host map bookkeeping)."""
         in_mask = np.asarray(in_mask) != 0
         i, c = np.nonzero(in_mask)
         lv = np.asarray(level)[i, c]
-        q = _queries(c, np.asarray(uv)[i, c, 0], np.asarray(uv)[i, c, 1], th * KF.scale_factors[lv], lv - 1, lv, i)
-        n, res = search_windows(KF, q, mp_desc, mp_dmask if self.havingMasks else None, np.zeros(len(q), np.int32),
-                                RULE_FIRST_FREE if first_wins else RULE_BEST_FREE,
-                                self.mfNNratio, self.TH_LOW_, np.full(max(len(q), len(KF.keys)), -1, np.int32))
+        q = _queries(c, np.asarray(uv)[i, c, 0], np.asarray(uv)[i, c, 1], th * KF.scale_factors[lv], lv - 1, lv,
+                     i if points is None else np.asarray(points, np.int64)[i])
         best = np.full(in_mask.shape, -1, np.int32)
-        best[i, c] = res[:len(q)]
+        best[i, c] = self._best_free(KF, q, mp_desc, mp_dmask, RULE_FIRST_FREE if first_wins else RULE_BEST_FREE, self.TH_LOW_, _sw)
         return best
 
-    def SearchByProjectionScw(self, KF, query_cam, uv, level, th, valid, mp_desc, mp_dmask=None, matched=None):
+    def SearchByProjectionScw(self, KF, query_cam, uv, level, th, valid, mp_desc, mp_dmask=None, matched=None, points=None, _sw=None):
         """Matching part of SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) (ref :2265-2392) as written there.  Entry i of
         vpPoints: valid[i] (not NULL / bad / already found, projected inside the mirror mask, distance in range), query_cam[i] =
         keypoint_to_cam[i] -- the reference looks the camera up with the POINT's list position (:2326) --, uv[i], level[i] the
-        predicted level.  matched = vpMatched as map point ids per keypoint (-1 = NULL), updated.  Candidate descriptors are read
-        the way the reference does (contiguous id as per-camera row; MCS_RULE_SCW) and keypoint 0 can never be matched (:2385)."""
+        predicted level.  matched = vpMatched as map point ids per keypoint (-1 = NULL), updated.  points: map point id per
+        entry i, when given its query reads mp_desc[points[i]] and a match writes points[i], instead of mp_desc[i] and i.  Candidate
+        descriptors are read the way the reference does (contiguous id as per-camera row; MCS_RULE_SCW) and keypoint 0 can never be
+        matched (:2385)."""
         if matched is None:
             matched = np.full(len(KF.keys), -1, np.int32)
         sel = np.flatnonzero(np.asarray(valid) != 0)
         lv = np.asarray(level)[sel]
-        q = _queries(np.asarray(query_cam)[sel], np.asarray(uv)[sel, 0], np.asarray(uv)[sel, 1], th * KF.scale_factors[lv], lv - 1, lv, sel)
-        return search_windows(KF, q, mp_desc, mp_dmask if self.havingMasks else None, sel, RULE_SCW, self.mfNNratio, self.TH_LOW_,
-                              matched)
-
-    def _project_for_fuse(self, KF, rig, Ow, world_pos, min_dist, max_dist, idx, float_dist):
-        """projection front-end shared by the Fuse overloads and SearchByProjection(KF, Scw): WorldToCamHom_fast ->
-        isPointInMirrorMask -> distance range -> predicted level (ref :1288-1318)"""
-        nc = len(rig.cams)
-        uv = np.zeros((len(idx), nc, 2)); ok = np.zeros((len(idx), nc), np.uint8); lvl = np.zeros((len(idx), nc), np.int32)
-        for k, i in enumerate(idx):
-            p = world_pos[i]
-            for c in range(nc):
-                u, v, _ = rig.world_to_cam(c, p)
-                if not rig.in_mirror_mask(c, u, v):
-                    continue
-                po = p - Ow
-                d = float(np.sqrt(po[0] * po[0] + po[1] * po[1] + po[2] * po[2]))
-                if float_dist:
-                    d = float(np.float32(d))                      # `const float dist3D = cv::norm(PO);` (ref :1301, :1472)
-                if d < min_dist[i] or d > max_dist[i]:
-                    continue
-                uv[k, c] = (u, v); ok[k, c] = 1
-                lvl[k, c] = _predict_level(KF.scale_factors, d / min_dist[i])
-        return uv, ok, lvl
+        ids = sel if points is None else np.asarray(points, np.int64)[sel]
+        q = _queries(np.asarray(query_cam)[sel], np.asarray(uv)[sel, 0], np.asarray(uv)[sel, 1], th * KF.scale_factors[lv], lv - 1, lv, ids)
+        return (search_windows if _sw is None else _sw)(KF, q, mp_desc, self._masks(mp_dmask), ids, RULE_SCW, self.mfNNratio, self.TH_LOW_,
+                                                        matched)
 
     def Fuse(self, KF, rig, kf_mp, points, world_pos, min_dist, max_dist, bad, in_kf, mp_desc, mp_dmask=None, th=2.5, variant=1,
              Scw=None, cur_rays=None, kf_rays=None, cur_rig=None, _sw=None):
@@ -919,36 +959,23 @@ class cORBmatcher:
         kf_mp [n_keys] map point id per keypoint (-1 none), updated like pKF->AddMapPoint does; points: candidate map point ids
         (-1 = NULL); bad / in_kf (IsInKeyFrame(pKF)) per map point.  Returns (nFused, ops) with ops rows (0, mp, keypoint) =
         AddObservation + AddMapPoint and (1, mp, other) = Replace(other), in the reference's call order."""
-        sw = search_windows if _sw is None else _sw
         kf_mp = np.ascontiguousarray(kf_mp, np.int32).copy()
-        world_pos = np.asarray(world_pos, np.float64)
         if variant == 2:
-            S = np.asarray(Scw, np.float64)
-            sR = S[:3, :3]
-            inv_s = 1.0 / float(np.sqrt(sR[0, 0] * sR[0, 0] + sR[0, 1] * sR[0, 1] + sR[0, 2] * sR[0, 2]))
-            T = np.eye(4)
-            T[:3, :3], T[:3, 3] = inv_s * sR, inv_s * S[:3, 3]
-            rig = Rig(rig.cams, rig.M_c, inv_rigid(T))            # camSys.Set_M_t(invMat(Rt2Hom(Rcw, tcw)))  (ref :1576-1584)
+            rig = _sim3_rig(rig, Scw)
             already = set(int(m) for m in kf_mp if m >= 0 and not bad[m])
             idx = [int(i) for i in points if not bad[i] and int(i) not in already]
         else:
             idx = [int(i) for i in points if i >= 0 and not bad[i] and not in_kf[i]]
-        Ow = rig.M_t[:3, 3].copy()
-        uv, ok, lvl = self._project_for_fuse(KF, rig, Ow, world_pos, min_dist, max_dist, idx, float_dist=(variant != 2))
-        k, c = np.nonzero(ok)
-        lv = lvl[k, c]
-        q = _queries(c, uv[k, c, 0], uv[k, c, 1], th * KF.scale_factors[lv], lv - 1, lv, np.asarray(idx, np.int64)[k])
-        n, res = sw(KF, q, mp_desc, mp_dmask if self.havingMasks else None, np.zeros(len(q), np.int32),
-                    RULE_FIRST_FREE if variant == 1 else RULE_BEST_FREE, self.mfNNratio, self.TH_LOW_,
-                    np.full(max(len(q), len(KF.keys)), -1, np.int32))
-        best = np.full(ok.shape, -1, np.int32)
-        best[k, c] = res[:len(q)]
+        nc = len(rig.cams)
+        uv, ok, lvl = _project(rig, KF.scale_factors, world_pos, min_dist, max_dist, idx, np.tile(np.arange(nc), (len(idx), 1)),
+                               float_dist=(variant != 2))
+        best = self.FuseCandidates(KF, uv, ok, lvl, th, mp_desc, mp_dmask, first_wins=(variant == 1), points=idx, _sw=_sw)
         ops, fused = [], 0
         pos_of = {}
         if variant == 0:
             pos_of = {int(i): j for j, i in enumerate(points) if i >= 0}     # keypoint of curKF that carries map point i
         for kk, i in enumerate(idx):
-            for cam in range(ok.shape[1]):
+            for cam in range(nc):
                 b = int(best[kk, cam])
                 if b < 0:
                     continue
@@ -971,90 +998,58 @@ class cORBmatcher:
         camera of entry iMP of vpPoints is keypoint_to_cam[iMP] (:2326), candidate descriptors are read with the contiguous id as
         per-camera row (:2367, :2372) and keypoint 0 is never matched (:2385).  points: map point ids (-1 = NULL), len <= n_keys;
         matched: vpMatched as map point ids per keypoint (-1 = NULL).  Returns (nmatches, vpMatched)."""
-        sw = search_windows if _sw is None else _sw
-        S = np.asarray(Scw, np.float64)
-        sR = S[:3, :3]
-        inv_s = 1.0 / float(np.sqrt(sR[0, 0] * sR[0, 0] + sR[0, 1] * sR[0, 1] + sR[0, 2] * sR[0, 2]))
-        T = np.eye(4)
-        T[:3, :3], T[:3, 3] = inv_s * sR, inv_s * S[:3, 3]
-        rig = Rig(rig.cams, rig.M_c, inv_rigid(T))
-        Ow = rig.M_t[:3, 3].copy()
         matched = np.ascontiguousarray(matched, np.int32).copy()
         found = set(int(m) for m in matched if m >= 0)
-        world_pos = np.asarray(world_pos, np.float64)
-        qc, quv, qlv, qi = [], [], [], []
-        for iMP, i in enumerate(points):
-            i = int(i)
-            if i < 0 or bad[i] or i in found:
-                continue
-            cam = int(KF.key_cam[iMP])
-            u, v, _ = rig.world_to_cam(cam, world_pos[i])
-            if not rig.in_mirror_mask(cam, u, v):
-                continue
-            po = world_pos[i] - Ow
-            d = float(np.sqrt(po[0] * po[0] + po[1] * po[1] + po[2] * po[2]))
-            if d < min_dist[i] or d > max_dist[i]:
-                continue
-            qc.append(cam); quv.append((u, v)); qlv.append(_predict_level(KF.scale_factors, d / min_dist[i])); qi.append(i)
-        if not qi:
+        entries = np.asarray([iMP for iMP, i in enumerate(points) if i >= 0 and not bad[i] and int(i) not in found], np.int64)
+        ids, cams = np.asarray(points, np.int64)[entries], KF.key_cam[entries]
+        uv, ok, lvl = _project(_sim3_rig(rig, Scw), KF.scale_factors, world_pos, min_dist, max_dist, ids, cams[:, None], float_dist=False)
+        if not ok.any():
             return 0, matched
-        lv = np.asarray(qlv)
-        quv = np.asarray(quv)
-        q = _queries(np.asarray(qc), quv[:, 0], quv[:, 1], float(int(th)) * KF.scale_factors[lv], lv - 1, lv, np.asarray(qi))
-        return sw(KF, q, mp_desc, mp_dmask if self.havingMasks else None, np.asarray(qi, np.int32), RULE_SCW, self.mfNNratio,
-                  self.TH_LOW_, matched)
+        return self.SearchByProjectionScw(KF, cams, uv[:, 0], lvl[:, 0], float(int(th)), ok[:, 0], mp_desc, mp_dmask, matched, ids, _sw)
 
     def SearchByProjectionFramesRig(self, F1, mp1, F2, rig2, mp2, world_pos, bad, windowSize, _sw=None):
         """SearchByProjection(F1, F2, windowSize, vpMapPointMatches2) (ref :476-577) as a whole entry point: every map point of F1
         (first occurrence only, not bad, not already in F2) is projected into EVERY camera of F2's rig and searched there on the level
         of its F1 keypoint; ratio test + TH_HIGH_, greedy.  mp1 / mp2: map point id per keypoint (-1 none).
         Returns (nmatches, vpMapPointMatches2 as map point ids)."""
-        sw = search_windows if _sw is None else _sw
         out = np.ascontiguousarray(mp2, np.int32).copy()
         already = set(int(x) for x in out)                   # spMapPointsAlreadyFound holds NULL as well: harmless
         world_pos = np.asarray(world_pos, np.float64)
+        n1, nc = len(F1.keys), len(rig2.cams)
+        valid1, uv, in_mask = np.zeros(n1, bool), np.zeros((n1, nc, 2)), np.zeros((n1, nc), bool)
         seen = set()
-        qc, quv, qlv, qi, tags = [], [], [], [], []
-        for i1 in range(len(F1.keys)):
+        for i1 in range(n1):
             p = int(mp1[i1])
             if p < 0 or bad[p] or p in already or p in seen:
                 continue
             seen.add(p)
-            for c in range(len(rig2.cams)):
+            valid1[i1] = True
+            for c in range(nc):
                 u, v, _ = rig2.world_to_cam(c, world_pos[p])
-                if rig2.in_mirror_mask(c, u, v):
-                    qc.append(c); quv.append((u, v)); qlv.append(int(F1.keys["octave"][i1])); qi.append(i1); tags.append(p)
-        if not qi:
+                uv[i1, c], in_mask[i1, c] = (u, v), rig2.in_mirror_mask(c, u, v)
+        if not in_mask.any():
             return 0, out
-        quv, lv = np.asarray(quv), np.asarray(qlv)
-        q = _queries(np.asarray(qc), quv[:, 0], quv[:, 1], float(int(windowSize)), lv, lv, np.asarray(qi))
-        return sw(F2, q, F1.desc, F1.dmask if self.havingMasks else None, np.asarray(tags, np.int32), RULE_RATIO, self.mfNNratio,
-                  self.TH_HIGH_, out)
+        return self.SearchByProjectionFrames(F1, F2, int(windowSize), valid1, uv, in_mask, out, mp1, _sw)
 
     def SearchByProjectionLastRig(self, CurrentFrame, rig_cur, cur_mp, LastFrame, last_mp, last_outlier, world_pos, bad, th, _sw=None):
         """SearchByProjection(CurrentFrame, LastFrame, th) (ref :1990-2118, motion model) as a whole entry point: the map point of
         every LastFrame keypoint (not bad, not an outlier) is projected into the SAME camera of the current rig pose and searched
         on levels octave-1 .. octave+1 within th*scale[octave]; best distance <= TH_HIGH_, greedy on CurrentFrame.mvpMapPoints.
         Returns (nmatches, CurrentFrame.mvpMapPoints as map point ids)."""
-        sw = search_windows if _sw is None else _sw
         out = np.ascontiguousarray(cur_mp, np.int32).copy()
         world_pos = np.asarray(world_pos, np.float64)
-        qc, quv, qlv, qi, tags = [], [], [], [], []
-        for i in range(len(LastFrame.keys)):
+        n = len(LastFrame.keys)
+        valid, uv, in_mask = np.zeros(n, bool), np.zeros((n, 2)), np.zeros(n, bool)
+        for i in range(n):
             p = int(last_mp[i])
             if p < 0 or bad[p] or (last_outlier is not None and last_outlier[i]):
                 continue
             cam = int(LastFrame.key_cam[i])
             u, v, _ = rig_cur.world_to_cam(cam, world_pos[p])
-            if not rig_cur.in_mirror_mask(cam, u, v):
-                continue
-            qc.append(cam); quv.append((u, v)); qlv.append(int(LastFrame.keys["octave"][i])); qi.append(i); tags.append(p)
-        if not qi:
+            valid[i], uv[i], in_mask[i] = True, (u, v), rig_cur.in_mirror_mask(cam, u, v)
+        if not in_mask.any():
             return 0, out
-        quv, lv = np.asarray(quv), np.asarray(qlv)
-        q = _queries(np.asarray(qc), quv[:, 0], quv[:, 1], th * CurrentFrame.scale_factors[lv], lv - 1, lv + 1, np.asarray(qi))
-        return sw(CurrentFrame, q, LastFrame.desc, LastFrame.dmask if self.havingMasks else None, np.asarray(tags, np.int32), RULE_BEST,
-                  self.mfNNratio, self.TH_HIGH_, out)
+        return self.SearchByProjectionLast(CurrentFrame, LastFrame, th, valid, uv, in_mask, out, last_mp, _sw)
 
     def SearchBySim3(self, KF1, rig1, mp1, KF2, rig2, mp2, world_pos, min_dist, max_dist, bad, mp_desc, mp_dmask, s12, R12, t12, th,
                      matches12=None, obs_idx2=None, _sw=None):
@@ -1063,7 +1058,6 @@ class cORBmatcher:
         (best distance <= TH_HIGH_), and only mutual agreements are kept.  mp1 / mp2: map point id per keypoint (-1 none);
         matches12 [n1]: already matched map point ids (-1 none) -- their keypoints are excluded, obs_idx2[id] = keypoint of KF2 that
         observes map point id (GetIndexInKeyFrame(pKF2)[0]).  Returns (nFound, vpMatches12 as map point ids)."""
-        sw = search_windows if _sw is None else _sw
         n1, n2 = len(KF1.keys), len(KF2.keys)
         m12 = np.full(n1, -1, np.int32) if matches12 is None else np.ascontiguousarray(matches12, np.int32).copy()
         world_pos = np.asarray(world_pos, np.float64)
@@ -1104,9 +1098,7 @@ class cORBmatcher:
             if qi:
                 lv, quv2 = np.asarray(qlv), np.asarray(quv)
                 q = _queries(np.asarray(qc), quv2[:, 0], quv2[:, 1], th * KFb.scale_factors[lv], lv - 1, lv, np.asarray(qd))
-                _, res = sw(KFb, q, mp_desc, mp_dmask if self.havingMasks else None, np.zeros(len(q), np.int32), RULE_BEST_FREE,
-                            self.mfNNratio, self.TH_HIGH_, np.full(max(len(q), len(KFb.keys)), -1, np.int32))
-                best[np.asarray(qi)] = res[:len(q)]
+                best[np.asarray(qi)] = self._best_free(KFb, q, mp_desc, mp_dmask, RULE_BEST_FREE, self.TH_HIGH_, _sw)
             return best
         b1 = one_way(KF1, mp1, T1, sR21, t21, KF2, rig2, done1)
         b2 = one_way(KF2, mp2, T2, sR12, t12, KF1, rig1, done2)
@@ -1123,7 +1115,6 @@ class cORBmatcher:
         map point is carried along its bearing ray into camera cam2 of the same rig (relative orientation of the two cameras),
         searched in a 40 px window (all levels, nothing skipped), and accepted when the best distance is <= 100 and the two rays
         satisfy the epipolar constraint.  Returns (nmatches, pairs [n,2] of contiguous keypoint ids)."""
-        sw = search_windows if _sw is None else _sw
         rel = _mm(inv_rigid(rig.M_c[cam1]), rig.M_c[cam2])
         E12 = compute_E_rel(rel)
         Rrel = rel[:3, :3].T.copy()
@@ -1142,8 +1133,7 @@ class cORBmatcher:
         if qi:
             quv = np.asarray(quv)
             q = _queries(np.full(len(qi), cam2), quv[:, 0], quv[:, 1], 40.0, -1, -1, np.asarray(qi))
-            _, res = sw(KF, q, KF.desc, KF.dmask if self.havingMasks else None, np.zeros(len(q), np.int32), RULE_BEST_FREE, self.mfNNratio,
-                        100, np.full(max(len(q), len(KF.keys)), -1, np.int32))
+            res = self._best_free(KF, q, KF.desc, KF.dmask, RULE_BEST_FREE, 100, _sw)
             for k, i in enumerate(qi):
                 b = int(res[k])
                 # the reference evaluates the epipolar test with the best candidate even when its distance fails (:1247-1249);
@@ -1156,9 +1146,7 @@ class cORBmatcher:
         """SearchForTriangulationRaw(KF1, KF2, ...) (ref :968-1156): free1/free2 flag keypoints WITHOUT a map point, rays = bearing
         vectors [n,3], E [n_cams,n_cams,3,3] from ComputeE.  Returns (nmatches, vMatches12)."""
         d1, d2 = np.ascontiguousarray(desc1, np.uint8), np.ascontiguousarray(desc2, np.uint8)
-        use = self.havingMasks and mask1 is not None and mask2 is not None
-        m1 = np.ascontiguousarray(mask1, np.uint8) if use else None
-        m2 = np.ascontiguousarray(mask2, np.uint8) if use else None
+        m1, m2 = self._masks(mask1, mask2)
         c1, c2 = np.ascontiguousarray(cam1, np.int32), np.ascontiguousarray(cam2, np.int32)
         f1, f2 = np.ascontiguousarray(free1, np.uint8), np.ascontiguousarray(free2, np.uint8)
         r1, r2 = np.ascontiguousarray(rays1, np.float64), np.ascontiguousarray(rays2, np.float64)
@@ -1174,11 +1162,8 @@ class cORBmatcher:
         map-point-bearing keypoints of two keyframes.  Returns (nmatches, matches12 indices into desc2)."""
         d1 = np.ascontiguousarray(desc1, np.uint8)
         d2 = np.ascontiguousarray(desc2, np.uint8)
-        use = self.havingMasks and mask1 is not None and mask2 is not None
-        m1 = np.ascontiguousarray(mask1, np.uint8) if use else None
-        m2 = np.ascontiguousarray(mask2, np.uint8) if use else None
-        v1 = None if valid1 is None else np.ascontiguousarray(valid1, np.uint8)
-        v2 = None if valid2 is None else np.ascontiguousarray(valid2, np.uint8)
+        m1, m2 = self._masks(mask1, mask2)
+        v1, v2 = _contig(valid1, np.uint8), _contig(valid2, np.uint8)
         m12 = np.zeros(len(d1), np.int32)
         n = C.c_int32(0)
         _check(lib().mcs_match_bruteforce(_p(d1), _p(m1), _p(v1), len(d1), _p(d2), _p(m2), _p(v2), len(d2), d1.shape[1],
@@ -1191,11 +1176,9 @@ class cORBmatcher:
         by ORBVocabulary.transform.  Returns (nmatches, match_of_f) with match_of_f[i] = key-frame keypoint or -1."""
         d1 = np.ascontiguousarray(desc_kf, np.uint8)
         d2 = np.ascontiguousarray(desc_f, np.uint8)
-        use = self.havingMasks and mask_kf is not None and mask_f is not None
-        m1 = np.ascontiguousarray(mask_kf, np.uint8) if use else None
-        m2 = np.ascontiguousarray(mask_f, np.uint8) if use else None
-        v1 = None if valid_kf is None else np.ascontiguousarray(valid_kf, np.uint8)
-        a = [np.ascontiguousarray(x, np.int32) for x in featvec_kf]
+        m1, m2 = self._masks(mask_kf, mask_f)
+        v1 = _contig(valid_kf, np.uint8)
+        a =[np.ascontiguousarray(x, np.int32) for x in featvec_kf]
         b = [np.ascontiguousarray(x, np.int32) for x in featvec_f]
         out = np.zeros(len(d2), np.int32)
         n = C.c_int32(0)
@@ -1218,8 +1201,8 @@ class cORBmatcher:
         if max_nodes is None:
             max_nodes = max([cur.max_nodes] + [b.max_nodes for b, _ in kfs])
         if out is None:
-            with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(dev)):     # the fills run on `stream` too
-                out = (torch.full((nk, ns), -1, dtype=torch.int32, device=dev), torch.full((nk, ns), -1, dtype=torch.int32, device=dev),
+            with _on_stream(stream, dev):
+                out =(torch.full((nk, ns), -1, dtype=torch.int32, device=dev), torch.full((nk, ns), -1, dtype=torch.int32, device=dev),
                        torch.zeros(nk, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev))
         frames = (BowFrame * max(nk, 1))(*[b.bow_frame(mp_t) for b, mp_t in kfs])
         fc = cur.bow_frame()
@@ -1275,8 +1258,7 @@ class ORBVocabulary:
         wt = np.ascontiguousarray(voc["weight"], np.float64)
         ds = np.ascontiguousarray(voc["desc"], np.uint8)
         wn = np.ascontiguousarray(voc["word_node"], np.int32)
-        order = voc["node_order"] if "node_order" in voc else None
-        order = None if order is None else np.ascontiguousarray(order, np.int32)
+        order = _contig(voc["node_order"] if "node_order" in voc else None, np.int32)
         if ds.shape != (len(par), 32) or len(wt) != len(par):
             raise ValueError("vocabulary arrays disagree in size")
         self._n_words = len(wn)
@@ -1367,8 +1349,8 @@ class ORBVocabulary:
             max_nodes = self.level_nodes(levelsup)
         i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=dev)  # noqa: E731
         f64 = lambda n: torch.zeros(n, dtype=torch.float64, device=dev)  # noqa: E731
-        with torch.cuda.stream(stream if stream is not None else torch.cuda.current_stream(dev)):         # the fills run on `stream` too
-            b = DeviceBoW(packed, n_cams, capacity, i32(max_nodes), i32(max_nodes + 1), i32(1), i32(ns), i32(ns), f64(ns), i32(1), i32(1),
+        with _on_stream(stream, dev):
+            b =DeviceBoW(packed, n_cams, capacity, i32(max_nodes), i32(max_nodes + 1), i32(1), i32(ns), i32(ns), f64(ns), i32(1), i32(1),
                           *((i32(ns), f64(ns), i32(ns)) if per_slot else ()))
         fr = PackedFrame(packed[0].data_ptr(), *packed[1:4])
         _check(lib().mcs_bow_vectors_device(self._h, C.byref(fr), n_cams, capacity, 32, levelsup, max_nodes, _dptr(b.word), _dptr(b.weight),
