@@ -557,6 +557,31 @@ int  mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_vie
                                    double nnratio, int32_t th_low, int32_t having_masks,
                                    int32_t* matches12, int32_t* nmatches);
 
+/* Map initialisation's search, cTracking::Initialize's SearchForInitialization(mInitialFrame, mCurrentFrame, mvbPrevMatched,
+ * mvIniMatches, windowSize) (ref src/cTracking.cpp:405-409, src/cORBmatcher.cpp:579-726), with both frames in packed feature
+ * buffers and its state on the device.  Conventions of mcs_window_search_device: asynchronous on `stream` (NULL synchronises),
+ * host validation before any launch, nothing read back, f1 / f2 in either packed layout and possibly one buffer.
+ *   Every F1 keypoint below its camera's count is a query, in contiguous order: GetFeaturesInArea(cam, prev.x, prev.y,
+ *   window_size, octave, octave) in the same camera of F2; candidates whose vMatchedDistance is <= their distance are skipped;
+ *   the best is accepted when best <= th_low and best < second * nnratio (second = INT_MAX without one), and takes its F2
+ *   keypoint from an earlier query.  checkOrientation is compile-time false (include/cORBmatcher.h:40).
+ *   cam_width / cam_height [n_cams] host.  prev_matched_dev [n_cams * capacity * 2] doubles, in/out, F1 slot-indexed (c * capacity +
+ *   j): the window centres, read before any is written; afterwards a surviving match's centre is its F2 keypoint's position.
+ *   matches12_dev [n_cams * capacity] out, F1 slot-indexed: the F2 SLOT matched, or -1; every F1 slot below a camera's count is
+ *   written.  Slots at or beyond a camera's count are neither read nor written, in any array or frame.  nmatches_dev [1]: the
+ *   reference's return value (F2 keypoints with an owner).  diag_dev (may be NULL): int32[2], the queries and the decisions that
+ *   rescanned their window.  No input is invalid in a data-dependent way (an octave outside the frame's levels finds no
+ *   candidate), so there is no status.
+ * capacity <= 65535 (visiting positions and walk state are 16-bit); n_cams * capacity < 2^24 (MCS_ERR_UNSUPPORTED beyond).
+ * mcs_search_for_initialization_seed_device: FirstInitialization's fill of mvbPrevMatched (ref src/cTracking.cpp:383-386):
+ *   prev_matched_dev[2 * slot .. +1] = (double) the keypoint's position, for every F1 slot below its camera's count. */
+int  mcs_search_for_initialization_device(const mcs_packed_frame* f1, const mcs_packed_frame* f2, int32_t n_cams, int32_t capacity,
+                                          int32_t dim, const int32_t* cam_width, const int32_t* cam_height, double* prev_matched_dev,
+                                          int32_t window_size, double nnratio, int32_t th_low, int32_t having_masks,
+                                          int32_t* matches12_dev, int32_t* nmatches_dev, int32_t* diag_dev, void* stream);
+int  mcs_search_for_initialization_seed_device(const mcs_packed_frame* f1, int32_t n_cams, int32_t capacity, int32_t dim,
+                                               double* prev_matched_dev, void* stream);
+
 /* ---- bag of words: ORBVocabulary::transform and the feature-vector guided search (SURVEY 8f, rank 4) ------- */
 /* The vocabulary tree of DBoW2::TemplatedVocabulary<FORB::TDescriptor, FORB> (ref include/cORBVocabulary.h:34,
  * ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h) as flat arrays.  Node 0 is the root; parent[0] is ignored.

@@ -758,6 +758,15 @@ def _search_result(out, frame_mp_t, diag):
     return (out[0], out[1], frame_mp_t) + ((out[2],) if diag else ())
 
 
+def _init_search_outputs(out, diag, stream, dev):
+    """_search_outputs for mcs_search_for_initialization_device, which has no status (none of its inputs can be invalid in a
+    data-dependent way) and a two-entry diag: (nmatches [1], diag [2]), `out` or new, and the call's last three arguments"""
+    if out is None:
+        import torch
+        out = tuple(torch.zeros(k, dtype=torch.int32, device=dev) for k in (1, 2))
+    return out, (_dptr(out[0]), _dptr(out[1]) if diag else None, _stream_handle(stream, dev))
+
+
 class cORBmatcher:
     """ref include/cORBmatcher.h:55-178; thresholds as in src/cORBmatcher.cpp:46-64."""
 
@@ -860,6 +869,27 @@ class cORBmatcher:
         if prev is not vbPrevMatched:
             vbPrevMatched[...] = prev
         return n.value, m12
+
+    def SearchForInitializationDevice(self, f1, f2, capacity, cam_sizes, prev_t, window, m12_t, stream=None, out=None, diag=False):
+        """mcs_search_for_initialization_device: SearchForInitialization(F1, F2, vbPrevMatched, vnMatches12, window) (ref :579-726)
+        with both frames in packed feature buffers.  f1 / f2: (packed uint8 cuda tensor, n_parts, part_images, first_image); cam_sizes
+        [(w, h)] per camera.  prev_t: float64 cuda [n_cams * capacity * 2] window centres by F1 slot, updated in place; m12_t: int32
+        cuda [n_cams * capacity], overwritten below each camera's count with the F2 slot matched or -1.  Asynchronous on `stream`.
+        Returns (nmatches [1], m12_t), plus diag [2] (queries, rescans) when diag is set, as cuda tensors."""
+        nc = len(cam_sizes)
+        cw, ch = _cam_wh(cam_sizes)
+        out, tail = _init_search_outputs(out, diag, stream, f1[0].device)
+        _check(lib().mcs_search_for_initialization_device(*_packed_pair(f1, f2), nc, capacity, self.mbFeatDim, _p(cw), _p(ch), _dptr(prev_t),
+                                                          int(window), self.mfNNratio, self.TH_LOW_, int(self.havingMasks), _dptr(m12_t),
+                                                          *tail))
+        return (out[0], m12_t) + ((out[1],) if diag else ())
+
+    def SearchForInitializationSeedDevice(self, f1, n_cams, capacity, prev_t, stream=None):
+        """mcs_search_for_initialization_seed_device: FirstInitialization's vbPrevMatched (ref src/cTracking.cpp:383-386) on the
+        device: prev_t [n_cams * capacity * 2] float64 cuda gets every F1 keypoint's position, by slot.  Returns prev_t."""
+        _check(lib().mcs_search_for_initialization_seed_device(C.byref(PackedFrame(f1[0].data_ptr(), *f1[1:4])), n_cams, capacity,
+                                                               self.mbFeatDim, _dptr(prev_t), _stream_handle(stream, f1[0].device)))
+        return prev_t
 
     def _masks(self, *masks):
         """the descriptor masks a search reads: each of `masks` as u8 when havingMasks and none of them is None, else None for

@@ -188,6 +188,16 @@ struct SearchFramesDevArgs : PsTwoFrameArgs {   // SearchByProjection(F1, F2, wi
     double window, nnratio;
 };
 cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cudaStream_t st);
+// SearchForInitialization(F1 = last, F2 = cur, vbPrevMatched, vnMatches12, window): th_high holds TH_LOW_; frame_mp, status,
+// last_mp, the map points and the pose are unused (NULL)
+struct InitSearchDevArgs : PsTwoFrameArgs {
+    double* prev;                                            // device [n_cams * capacity * 2], F1 slot-indexed, in/out
+    int* matches12;                                          // device [n_cams * capacity], F1 slot-indexed: the F2 slot or -1
+    int window; double nnratio;
+};
+cudaError_t launch_search_for_initialization(const InitSearchDevArgs& a, cudaStream_t st);
+// prev = the position of every F1 keypoint below its camera's count (f1: host [n_cams])
+cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_cams, int capacity, double* prev, cudaStream_t st);
 int proj_search_max_rounds();
 
 // ---- bag of words (bow_kernels.cu) ----

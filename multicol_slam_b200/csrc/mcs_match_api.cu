@@ -755,6 +755,36 @@ int mcs_search_by_projection_frames_device(const mcs_packed_frame* cur, const mc
     return sync_if_null_stream(stream);
 }
 
+int mcs_search_for_initialization_device(const mcs_packed_frame* f1, const mcs_packed_frame* f2, int32_t n_cams, int32_t capacity,
+                                         int32_t dim, const int32_t* cam_width, const int32_t* cam_height, double* prev_matched_dev,
+                                         int32_t window_size, double nnratio, int32_t th_low, int32_t having_masks,
+                                         int32_t* matches12_dev, int32_t* nmatches_dev, int32_t* diag_dev, void* stream) {
+    if (!f1 || !f2 || !cam_width || !cam_height || !prev_matched_dev || !matches12_dev || !nmatches_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, f2, f1)) return rc;
+    if (int rc = check_cam_sizes(n_cams, cam_width, cam_height, false)) return rc;
+    // the front end's query and slot indices (one query per F1 slot)
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const std::vector<PsCamSlots> s2 = packed_slots(*f2, n_cams, capacity, dim), s1 = packed_slots(*f1, n_cams, capacity, dim);
+    InitSearchDevArgs a{};
+    set_searched_frame(a, s2, capacity, dim, cam_width, cam_height, th_low, having_masks, nullptr, nmatches_dev, nullptr, diag_dev);
+    a.last = s1.data();
+    a.prev = prev_matched_dev; a.matches12 = matches12_dev; a.window = window_size; a.nnratio = nnratio;
+    CUDA_CHECK(launch_search_for_initialization(a, st));
+    return sync_if_null_stream(stream);
+}
+
+int mcs_search_for_initialization_seed_device(const mcs_packed_frame* f1, int32_t n_cams, int32_t capacity, int32_t dim,
+                                              double* prev_matched_dev, void* stream) {
+    if (!f1 || !prev_matched_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, f1, nullptr)) return rc;
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
+    const std::vector<PsCamSlots> s1 = packed_slots(*f1, n_cams, capacity, dim);
+    CUDA_CHECK(launch_search_for_initialization_seed(s1.data(), n_cams, capacity, prev_matched_dev, (cudaStream_t)stream));
+    return sync_if_null_stream(stream);
+}
+
 int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view* f2, double* prev_matched, int32_t window_size,
                                   double nnratio, int32_t th_low, int32_t having_masks, int32_t* matches12, int32_t* nmatches) {
     if (!f1 || !f2 || !prev_matched || !matches12 || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");

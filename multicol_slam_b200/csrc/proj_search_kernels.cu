@@ -18,12 +18,16 @@
 //   ps_walk_kernel      the sequential fallback past the round cap: one warp per camera walks the unsettled queries in order
 //                       Both are templates over (rule, width, mask): MCS_RULE_LEVEL_RATIO for the local map, MCS_RULE_BEST for
 //                       the motion model, MCS_RULE_RATIO for the previous-frame searches
+//   pi_walk_kernel      SearchForInitialization(F1, F2) (:579-726) only: its acceptance can take a keypoint back from an earlier
+//                       query, so it runs no rounds; one warp per camera walks the camera's queries in order (InitQueries: one per
+//                       F1 slot) and writes matches12 and the survivors' prev.  pi_seed_kernel: FirstInitialization's prev
 //
 // No kernel reads anything back to the host: every size that depends on the data (the number of queries, the rounds the
 // fixpoint needed, where the walk starts) lives in device memory and the kernels are launched for the upper bound.
 #include <algorithm>
 #include <climits>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "cam_model.cuh"
@@ -262,6 +266,24 @@ struct FramesQueries {           // SearchByProjection(F1 = last, F2 = cur, wind
     }
 };
 
+struct InitQueries {             // SearchForInitialization(F1, F2, vbPrevMatched, ., windowSize): entry k = F1 slot (ref :599-612)
+    int n_slots, capacity;
+    const PsCamSlots* f1; const mcs_keypoint* keys; const double* prev;   // keys: F1 in slot order; prev [n_slots * 2]
+    const double* sf; double window;                         // sf: unused, the octave is a level filter only
+    __host__ __device__ long long size() const { return n_slots; }
+    __device__ bool valid(long long k, int*) const {
+        if (k >= n_slots) return false;
+        const int c = (int)(k / capacity);
+        return (int)k - c * capacity < min(*f1[c].count, capacity);
+    }
+    __device__ mcs_window_query make(long long k) const {
+        mcs_window_query q;                          // GetFeaturesInArea(cam, prev.x, prev.y, windowSize, level1, level1)  (ref :609-612)
+        q.cam = (int)(k / capacity); q.min_level = keys[k].octave; q.max_level = q.min_level; q.desc_index = (int)k;
+        q.x = prev[2 * k]; q.y = prev[2 * k + 1]; q.r = window;
+        return q;
+    }
+};
+
 template <class QM>
 __global__ void __launch_bounds__(kQbThreads) ps_count_kernel(const QM a, int* __restrict__ block_count, int* __restrict__ status) {
     int total = 0;
@@ -317,11 +339,20 @@ __global__ void __launch_bounds__(kQbThreads) ps_fill_kernel(const QM a, const i
 // ---- window search keeping the KB smallest (distance << 16 | visiting position) keys of the candidates not taken ----
 // Mirrors window_search_kernel (GetFeaturesInArea, ref src/cMultiFrame.cpp:272-340): same cell range, visiting order, level filter
 // and distance.  Every lane ends with the same sorted list.  Returns the number of candidates in the window (taken ones included).
+// Taken is called as taken(id), or as taken(id, distance) when it takes a second argument: SearchForInitialization skips a
+// candidate by its distance (vMatchedDistance[i2] <= dist, ref :647-648), the other searches by the keypoint alone.
 struct NoneTaken { __device__ bool operator()(int) const { return false; } };
+template <class Taken> constexpr bool kTakenByDistance = std::is_invocable<const Taken&, int, unsigned>::value;
+
+template <class Taken> __device__ __forceinline__ bool is_taken(const Taken& taken, const int id, const unsigned dist) {
+    if constexpr (kTakenByDistance<Taken>) return taken(id, dist);
+    else return taken(id);
+}
 
 template <int WORDS, bool MASKED, int KB, class Taken>
 __device__ __forceinline__ int window_kbest(const WindowFrameDev& f, const mcs_window_query& qq, const uint32_t* __restrict__ qdesc,
                                             const uint32_t* __restrict__ qmask, const Taken& taken, unsigned (&key)[KB], int (&slot)[KB]) {
+    constexpr bool BY_DIST = kTakenByDistance<Taken>;
     const int lane = threadIdx.x & 31;
 #pragma unroll
     for (int k = 0; k < KB; ++k) { key[k] = kNoKey; slot[k] = -1; }
@@ -357,7 +388,7 @@ __device__ __forceinline__ int window_kbest(const WindowFrameDev& f, const mcs_w
                     if (ok) ok = !(fabs((double)f.kx[id] - x) > r || fabs((double)f.ky[id] - y) > r);
                 }
                 const unsigned m = __ballot_sync(0xffffffffu, ok);
-                const bool cand = ok && !taken(id);
+                const bool cand = ok && (BY_DIST || !is_taken(taken, id, 0u));
                 unsigned kk = kNoKey;
                 if (cand) {
                     const uint32_t* dd = (const uint32_t*)f.desc + (size_t)id * WORDS;
@@ -374,7 +405,7 @@ __device__ __forceinline__ int window_kbest(const WindowFrameDev& f, const mcs_w
 #pragma unroll
                         for (int k = 0; k < WORDS; ++k) dist += __popc(qw[k] ^ dd[k]);
                     }
-                    kk = (dist << 16) | (unsigned)(count + __popc(m & ((1u << lane) - 1u)));
+                    if (!BY_DIST || !is_taken(taken, id, dist)) kk = (dist << 16) | (unsigned)(count + __popc(m & ((1u << lane) - 1u)));
                 }
                 unsigned ins = __ballot_sync(0xffffffffu, cand && kk < key[KB - 1]);
                 while (ins) {
@@ -413,17 +444,20 @@ __global__ void __launch_bounds__(256) ps_list_kernel(const WindowFrameDev f, co
 // acceptance of :154-160.  MCS_RULE_BEST: the best free candidate alone (strict < over the visiting order, ref :2050-2068),
 // accepted when its distance is <= th_high (:2070).  MCS_RULE_RATIO: best / second best free candidate, accepted when
 // best <= second * nnratio and best <= th_high (WindowSearch :405-416, SearchByProjection(F1, F2) :553-566), in the double form of
-// the host replay.  The list decides when it holds as many free entries as the rule reads, or every candidate; otherwise the window
-// is scanned again with the predicate.
+// the host replay.  kRuleInit: best / second best candidate not skipped, accepted when best <= th_high and best < second * nnratio
+// (SearchForInitialization :662-677); its distance goes to *best_dist.  The list decides when it holds as many free entries as the
+// rule reads, or every candidate; otherwise the window is scanned again with the predicate.
+constexpr int kRuleInit = 100;               // not a public rule: SearchForInitialization's acceptance exists on the device only
 template <int RULE, int WORDS, bool MASKED, class Taken>
 __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_window_query& qq, const unsigned* lk, const int* ls, const int cnt,
                                          const uint32_t* qdesc, const uint32_t* qmask, const Taken& taken, const int th_high,
-                                         const double nnratio, int* rescans) {
-    static_assert(RULE == MCS_RULE_LEVEL_RATIO || RULE == MCS_RULE_BEST || RULE == MCS_RULE_RATIO, "device acceptance rules");
+                                         const double nnratio, int* rescans, int* best_dist = nullptr) {
+    static_assert(RULE == MCS_RULE_LEVEL_RATIO || RULE == MCS_RULE_BEST || RULE == MCS_RULE_RATIO || RULE == kRuleInit,
+                  "device acceptance rules");
     constexpr int NB = RULE == MCS_RULE_BEST ? 1 : 2;       // free keys the rule reads
     const int lane = threadIdx.x & 31;
     unsigned k = kNoKey; int s = -1; bool fr = false;
-    if (lane < kPsK) { k = lk[lane]; s = ls[lane]; fr = k != kNoKey && !taken(s); }
+    if (lane < kPsK) { k = lk[lane]; s = ls[lane]; fr = k != kNoKey && !is_taken(taken, s, k >> 16); }
     const unsigned fm = __ballot_sync(0xffffffffu, fr);
     unsigned k0 = kNoKey, k1 = kNoKey; int s0 = -1, s1 = -1;
     if (__popc(fm) >= NB || cnt <= kPsK) {
@@ -446,6 +480,11 @@ __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_wind
     if constexpr (RULE == MCS_RULE_RATIO) {
         const int d0 = (int)(k0 >> 16), d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX;
         return (double)d0 <= (double)d1 * nnratio && d0 <= th_high ? s0 : -1;
+    }
+    if constexpr (RULE == kRuleInit) {
+        const int d0 = (int)(k0 >> 16), d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX;
+        *best_dist = d0;
+        return d0 <= th_high && (double)d0 < (double)d1 * nnratio ? s0 : -1;
     }
     const int d0 = (int)(k0 >> 16), l0 = f.koct[s0];
     const int d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX, l1 = s1 >= 0 ? f.koct[s1] : -1;
@@ -574,18 +613,114 @@ __global__ void ps_diag_kernel(const int* __restrict__ ctl, int* __restrict__ di
     diag[3] = ctl[2];        // decisions that rescanned their window
 }
 
+// ---- SearchForInitialization: the ordered walk (DESIGN.md section 4) ----
+// A later query may take a keypoint away from an earlier one with a strictly smaller distance, so query p needs
+// MD(s) = min{ d_q : q < p accepted s } for every candidate s, which no per-keypoint owner word of a round answers.  Cameras are
+// independent (a query searches only its own camera of F2), so one warp per camera walks that camera's queries in order with MD
+// of the camera's F2 slots in shared memory (16 bits each, 0xFFFF = no acceptance yet: every distance is <= 512).
+struct InitWalk {
+    const mcs_window_query* qry;
+    const unsigned* lkey; const int* lslot; const int* lcnt;
+    int* ctl;                    // [0] nq  [2] rescans
+    const PsCamSlots* f1; const PsCamSlots* f2;              // device [n_cams]: the counts of both frames
+    const mcs_keypoint* keys2;   // F2 in slot order
+    int* dec;                    // [Q] the slot each query accepted, or -1
+    int* owner;                  // [n_slots] the last query that accepted an F2 slot, -1 on entry
+    int n_cams, capacity, th_low;
+    double nnratio;
+    int* matches12; double* prev; int* nmatches;             // device, F1 slot-indexed / [1]
+};
+
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(32) pi_walk_kernel(const WindowFrameDev f, const InitWalk w, const uint32_t* __restrict__ qdesc,
+                                                     const uint32_t* __restrict__ qmask) {
+    extern __shared__ unsigned short s_md[];
+    __shared__ unsigned s_key[32 * kPsK];
+    __shared__ int s_slot[32 * kPsK], s_cnt[32];
+    const int c = blockIdx.x, lane = threadIdx.x, cap = w.capacity, base_slot = c * cap;
+    int q0 = 0;                                              // the camera's queries are [q0, q0 + n1): one per F1 slot below the count
+    for (int k = 0; k < c; ++k) q0 += min(*w.f1[k].count, cap);
+    const int n1 = min(*w.f1[c].count, cap), n2 = min(*w.f2[c].count, cap);
+    for (int j = lane; j < n2; j += 32) s_md[j] = 0xFFFF;
+    __syncwarp();
+    auto skipped = [&](int s, unsigned d) { return s_md[s - base_slot] <= d; };   // vMatchedDistance[i2] <= dist (ref :647-648)
+    for (int b = 0; b < n1; b += 32) {
+        const int nb = min(32, n1 - b), qb = q0 + b;
+        for (int i = lane; i < nb * kPsK; i += 32) {         // the next 32 queries' lists in one coalesced pass
+            s_key[i] = w.lkey[(size_t)qb * kPsK + i];
+            s_slot[i] = w.lslot[(size_t)qb * kPsK + i];
+        }
+        if (lane < nb) s_cnt[lane] = w.lcnt[qb + lane];
+        __syncwarp();
+        for (int i = 0; i < nb; ++i) {
+            const int q = qb + i;
+            int d0 = 0;
+            const int s = ps_decide<kRuleInit, WORDS, MASKED>(f, w.qry[q], s_key + i * kPsK, s_slot + i * kPsK, s_cnt[i], qdesc, qmask,
+                                                              skipped, w.th_low, w.nnratio, w.ctl + 2, &d0);
+            if (lane == 0) {
+                w.dec[q] = s;
+                if (s >= 0) { s_md[s - base_slot] = (unsigned short)d0; w.owner[s] = q; }
+            }
+            __syncwarp();
+        }
+    }
+    // a query's match survives when no later query took its keypoint (ref :666-670); prev moves to the survivors' F2 keypoints
+    int nm = 0;
+    for (int j = lane; j < n1; j += 32) {
+        const int q = q0 + j, s = w.dec[q];
+        const bool keep = s >= 0 && w.owner[s] == q;
+        w.matches12[base_slot + j] = keep ? s : -1;
+        if (keep) {
+            const mcs_keypoint kp = w.keys2[s];
+            w.prev[2 * (size_t)(base_slot + j)] = (double)kp.x;
+            w.prev[2 * (size_t)(base_slot + j) + 1] = (double)kp.y;
+            ++nm;
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) nm += __shfl_xor_sync(0xffffffffu, nm, o);
+    if (lane == 0 && nm) atomicAdd(w.nmatches, nm);
+}
+
+__global__ void pi_diag_kernel(const int* __restrict__ ctl, int* __restrict__ diag) {
+    diag[0] = ctl[0];        // queries
+    diag[1] = ctl[2];        // decisions that rescanned their window
+}
+
+// FirstInitialization's fill (ref src/cTracking.cpp:383-386): prev = the keypoint position as doubles, for every slot below the count
+__global__ void pi_seed_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, double* __restrict__ prev) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_cams * capacity) return;
+    const int c = s / capacity, j = s - c * capacity;
+    if (j >= min(*cams[c].count, capacity)) return;
+    const mcs_keypoint kp = cams[c].kps[j];
+    prev[2 * (size_t)s] = (double)kp.x;
+    prev[2 * (size_t)s + 1] = (double)kp.y;
+}
+
 }  // namespace
 
 int proj_search_max_rounds() { return kPsRounds; }
 
 namespace {
 
-// Both searches from the query maker on: the frame view of `a` in slot order and its grid, the queries in the maker's order, the
-// lists, the rounds and the walk under RULE.  qdesc / qmask: the query descriptors, row desc_index; tag: see PsState.  The caller
-// has zeroed a.nmatches and a.status.
-template <int RULE, class QM>
-cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const uint8_t* qdesc, const uint8_t* qmask, const int* tag,
-                      cudaStream_t st) {
+// What the front end of the searches leaves for an acceptance stage, in one stream-ordered scratch block the caller releases: the
+// frame searched in slot order with its grid, the queries in the maker's order and their lists, and the acceptance scratch.
+struct PsFront {
+    StreamScratch sc;
+    WindowFrameDev f;
+    const PsCamSlots* slots;     // device [n_cams]: the searched frame's image slots
+    const mcs_keypoint* keys;    // the searched frame in slot order
+    const mcs_window_query* qry; const unsigned* lkey; const int* lslot; const int* lcnt;
+    int* ctl; int* dec; unsigned* owner;                     // PsState's; owner starts at 0xFFFFFFFF
+    const uint32_t* qd; const uint32_t* qk;                  // the query descriptors and masks (qk NULL unless masked)
+    long long Q;                                             // queries at most (the maker's size)
+    int sms, wblocks;
+};
+
+// The front end from the query maker on: the frame view of `a` in slot order and its grid, the queries in the maker's order and
+// their lists.  qdesc / qmask: the query descriptors, row desc_index.
+template <class QM>
+cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const uint8_t* qmask, PsFront& fr, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     const int ncell = a.n_cams * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
     const long long Q = qm.size();
@@ -594,7 +729,7 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
     int sms = 0;
     cudaError_t e = sm_count(sms);
     if (e != cudaSuccess) return e;
-    StreamScratch sc;
+    StreamScratch& sc = fr.sc;
     e = sc.alloc({sizeof(mcs_ocam) * a.n_cams, sizeof(double) * a.n_levels, sizeof(PsCamSlots) * a.n_cams,         // staged host inputs
                   sizeof(mcs_keypoint) * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, db, a.masked ? db : 0,    // keys key_cam kx ky koct desc dmask
                   4ull * NS, 4ull * ncell, 4ull * (ncell + 1), 4ull * NS, 8ull * a.n_cams, 8ull * a.n_cams,         // cell_of cursor start items winv hinv
@@ -620,7 +755,7 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl, 0, 16, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl + 4, 0x7F, 4 * kPsRounds, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(owner, 0xFF, 8ull * NS, st);
-    if (e != cudaSuccess) return sc.release(e);
+    if (e != cudaSuccess) return e;
 
     // frame view in slot order and its grid (the kernel the host entry points build their grid with)
     ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
@@ -633,30 +768,49 @@ cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const u
         ps_fill_kernel<<<nb, kQbThreads, 0, st>>>(qm, boff, qry);
         e = cudaGetLastError();
     }
+    fr.f = WindowFrameDev{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv};
+    fr.slots = slots; fr.keys = keys;
+    fr.qry = qry; fr.lkey = lkey; fr.lslot = lslot; fr.lcnt = lcnt; fr.ctl = ctl; fr.dec = dec; fr.owner = owner;
+    fr.qd = (const uint32_t*)qdesc; fr.qk = a.masked ? (const uint32_t*)qmask : nullptr;
+    fr.Q = Q; fr.sms = sms;
+    fr.wblocks = (int)std::min<long long>((Q + 7) / 8, (long long)sms * 16);
     if (e == cudaSuccess && Q > 0) {
-        const WindowFrameDev f{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv};
-        const PsState p{qry, lkey, lslot, lcnt, dec, owner, ctl, (int)Q, NS, a.capacity, a.th_high, nnratio, tag};
-        const uint32_t* qd = (const uint32_t*)qdesc;
-        const uint32_t* qk = a.masked ? (const uint32_t*)qmask : nullptr;
-        const int wblocks = (int)std::min<long long>((Q + 7) / 8, (long long)sms * 16);
-        const int fblocks = (int)std::min<long long>((Q + 255) / 256, (long long)sms * 4);
-        const size_t walk_smem = 4ull * ((a.capacity + 31) / 32);
         with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
-            ps_list_kernel<W, M><<<wblocks, 256, 0, st>>>(f, qry, ctl, qd, qk, lkey, lslot, lcnt);
-            for (int r = 0; r < kPsRounds; ++r) ps_round_kernel<RULE, W, M><<<wblocks, 256, 0, st>>>(f, p, r, qd, qk, a.frame_mp);
-            ps_finalize_kernel<<<fblocks, 256, 0, st>>>(p, a.frame_mp, a.nmatches);
-            ps_walk_kernel<RULE, W, M><<<a.n_cams, 32, walk_smem, st>>>(f, p, qd, qk, a.frame_mp, a.nmatches);
+            ps_list_kernel<W, M><<<fr.wblocks, 256, 0, st>>>(fr.f, qry, ctl, fr.qd, fr.qk, lkey, lslot, lcnt);
         });
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess && a.diag) ps_diag_kernel<<<1, 1, 0, st>>>(ctl, a.diag);
+    return e;
+}
+
+// Both searches from the query maker on: the front end, then the rounds and the walk under RULE.  tag: see PsState.  The caller
+// has zeroed a.nmatches and a.status.
+template <int RULE, class QM>
+cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const uint8_t* qdesc, const uint8_t* qmask, const int* tag,
+                      cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    PsFront fr;
+    cudaError_t e = ps_front(a, qm, qdesc, qmask, fr, st);
+    const long long Q = fr.Q;
+    if (e == cudaSuccess && Q > 0) {
+        const PsState p{fr.qry, fr.lkey, fr.lslot, fr.lcnt, fr.dec, fr.owner, fr.ctl, (int)Q, NS, a.capacity, a.th_high, nnratio, tag};
+        const int fblocks = (int)std::min<long long>((Q + 255) / 256, (long long)fr.sms * 4);
+        const size_t walk_smem = 4ull * ((a.capacity + 31) / 32);
+        with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
+            for (int r = 0; r < kPsRounds; ++r) ps_round_kernel<RULE, W, M><<<fr.wblocks, 256, 0, st>>>(fr.f, p, r, fr.qd, fr.qk, a.frame_mp);
+            ps_finalize_kernel<<<fblocks, 256, 0, st>>>(p, a.frame_mp, a.nmatches);
+            ps_walk_kernel<RULE, W, M><<<a.n_cams, 32, walk_smem, st>>>(fr.f, p, fr.qd, fr.qk, a.frame_mp, a.nmatches);
+        });
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && a.diag) ps_diag_kernel<<<1, 1, 0, st>>>(fr.ctl, a.diag);
     if (e == cudaSuccess) e = cudaGetLastError();
-    return sc.release(e);
+    return fr.sc.release(e);
 }
 
 cudaError_t ps_zero_outputs(const PsFrameArgs& a, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(a.nmatches, 0, 4, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
+    if (e == cudaSuccess && a.status) e = cudaMemsetAsync(a.status, 0, 4, st);     // NULL: a search whose input cannot be invalid
     return e;
 }
 
@@ -763,6 +917,47 @@ cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cud
         e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, t.desc, t.dmask, a.last_mp, st);
     }
     return t.sc.release(e);
+}
+
+// SearchForInitialization(F1 = last, F2 = cur): one query per F1 slot below its count, centred on prev, then the ordered walk
+// (pi_walk_kernel) instead of the rounds.
+cudaError_t launch_search_for_initialization(const InitSearchDevArgs& a, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    TwoFrameScratch t;
+    cudaError_t e = ps_open_two_frames(a, false, {}, t, st);
+    if (e != cudaSuccess) return t.sc.release(e);
+    const InitQueries qm{NS, a.capacity, t.last, t.keys, a.prev, nullptr, (double)a.window};
+    PsFront fr;
+    e = ps_front(a, qm, t.desc, t.dmask, fr, st);
+    if (e == cudaSuccess && fr.Q > 0) {
+        const InitWalk w{fr.qry, fr.lkey, fr.lslot, fr.lcnt, fr.ctl, t.last, fr.slots, fr.keys, fr.dec, (int*)fr.owner, a.n_cams, a.capacity,
+                         a.th_high, a.nnratio, a.matches12, a.prev, a.nmatches};
+        const size_t smem = 2ull * a.capacity;              // MD of one camera's F2 slots
+        with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
+            // The opt-in is set on every call: without it the static lists and MD together must fit in 48 KB, which capacities
+            // from 23 489 up do not (per device, so a set attribute cannot be remembered across devices either).
+            e = cudaFuncSetAttribute(pi_walk_kernel<W, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e == cudaSuccess) pi_walk_kernel<W, M><<<a.n_cams, 32, smem, st>>>(fr.f, w, fr.qd, fr.qk);
+        });
+        if (e == cudaSuccess) e = cudaGetLastError();
+    }
+    if (e == cudaSuccess && a.diag) pi_diag_kernel<<<1, 1, 0, st>>>(fr.ctl, a.diag);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return t.sc.release(fr.sc.release(e));
+}
+
+cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_cams, int capacity, double* prev, cudaStream_t st) {
+    const int NS = n_cams * capacity;
+    StreamScratch sc;
+    cudaError_t e = sc.alloc({sizeof(PsCamSlots) * n_cams}, st);
+    if (e != cudaSuccess) return e;
+    PsCamSlots* slots = sc.at<PsCamSlots>(0);
+    e = stage_to_device(f1, sizeof(PsCamSlots) * n_cams, slots, st);
+    if (e == cudaSuccess) {
+        pi_seed_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, n_cams, capacity, prev);
+        e = cudaGetLastError();
+    }
+    return sc.release(e);
 }
 
 }  // namespace mcs

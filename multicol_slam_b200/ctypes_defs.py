@@ -71,6 +71,12 @@ def set_prototypes(lib):
     f = lib.mcs_search_by_projection_frames_device
     f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, P, P, I, P, P, I, D, I, I, P, P, P, P, P]
     f.restype = C.c_int
+    f = lib.mcs_search_for_initialization_device
+    f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, P, I, D, I, I, P, P, P, P]
+    f.restype = C.c_int
+    f = lib.mcs_search_for_initialization_seed_device
+    f.argtypes = [C.POINTER(PackedFrame), I, I, I, P, P]
+    f.restype = C.c_int
     f = lib.mcs_vocabulary_level_nodes
     f.argtypes = [P, I, C.POINTER(I)]
     f.restype = C.c_int

@@ -33,4 +33,11 @@ mt = api.cORBmatcher(0.9, False, 32, True)
 mmp, msl, nm, st = mt.SearchByBoWDevice([(bows[0], mp_t)], bows[1], cap)
 nh, mh = mt.SearchByBoWFrame(d, (hn, ho, hf), d, (hn, ho, hf), m, m)
 assert int(st.item()) == 0 and int(nm[0].item()) == nh and np.array_equal(msl[0, :len(k)].cpu().numpy(), mh)
+# map initialisation's search on the device: the seed, then the frame against itself from the packed buffer (the walk's shared state)
+prev_t = torch.zeros(cap * 2, dtype=torch.float64, device="cuda")
+m12_t = torch.full((cap,), -1, dtype=torch.int32, device="cuda")
+mt.SearchForInitializationSeedDevice((packed, 1, 2, 0), 1, cap, prev_t)
+ni, _ = mt.SearchForInitializationDevice((packed, 1, 2, 0), (packed, 1, 2, 1), cap, [(333, 211)], prev_t, 30, m12_t)
+torch.cuda.synchronize()
+assert int(ni.item()) == n and np.array_equal(m12_t[:len(k)].cpu().numpy(), m12)
 print("sanitize_small ok", len(k), n, nh)
