@@ -582,6 +582,53 @@ int  mcs_search_for_initialization_device(const mcs_packed_frame* f1, const mcs_
 int  mcs_search_for_initialization_seed_device(const mcs_packed_frame* f1, int32_t n_cams, int32_t capacity, int32_t dim,
                                                double* prev_matched_dev, void* stream);
 
+/* The matching part of the three Fuse overloads (ref src/cORBmatcher.cpp:1265-1418, :1420-1567, :1570-1719) for n_kf target key
+ * frames in one call, with every target in packed feature buffers: cLocalMapping::SearchInNeighbors' Fuse(pKFi, curKF, .) per
+ * neighbour and its Fuse(curKF, candidates), cLoopClosing::SearchAndFuse's Fuse(pKF, Scw, ., 4) per corrected key frame.
+ * Conventions of mcs_search_by_projection_last_device: asynchronous on `stream` (NULL synchronises), host validation before any
+ * launch, nothing read back, stream-ordered scratch; the targets' frames in either packed layout, possibly sharing one buffer.
+ * The call decides which keypoint each (key frame, query, camera) hits; the map bookkeeping (Replace, AddObservation,
+ * AddMapPoint) stays with the caller, which replays the hits in row order over the live map.
+ *   kfs [n_kf] host: per target its frame, its slot-indexed map-point ids mp_dev [n_cams * capacity] (the frame_mp_dev format; NULL
+ *   = no "already in the key frame" pre-filter for it), mtmc_inv [n_cams * 16] host (row-major MtMc_inv of the pose to project
+ *   with) and ow, the centre the depth test measures from (GetCameraCenter, or the Sim3's rigid part for MCS_FUSE_SIM3).
+ *   cams [n_cams] host camera models (one image size for all), masks_dev [n_cams][height][width] their mirror masks,
+ *   scale_factors [n_levels] host.  query_mp_dev [n_q]: map-point ids, -1 = NULL (the array may be NULL when n_q is 0).  The map points: world_pos_dev [n_points * 3],
+ *   min_dist_dev / max_dist_dev [n_points] (GetMin/MaxDistanceInvariance), desc_dev / dmask_dev [n_points * dim] (dmask_dev only
+ *   read when having_masks), bad_dev [n_points] (may be NULL).
+ *   For every key frame k, query q, camera c, in that order: q is skipped when its id is -1, the point is bad, or a slot of
+ *   kfs[k].mp_dev below its camera's count holds it.  Otherwise the point is projected (WorldToCamHom_fast, mirror mask), its
+ *   distance to ow tested against [min, max] -- a float for MCS_FUSE_NEIGHBOUR / MCS_FUSE_FIRST, a double for MCS_FUSE_SIM3 --,
+ *   its level l predicted by lower_bound over the scale factors, and GetFeaturesInArea(c, u, v, th * scale_factors[l]) searched on
+ *   levels {l - 1, l}.  MCS_FUSE_NEIGHBOUR / MCS_FUSE_SIM3: the best candidate (strict < over the visiting order) hits when its
+ *   distance is <= th_low.  MCS_FUSE_FIRST: the first candidate in visiting order hits (the reference discards the distance).
+ *   The pre-filter relies on the caller's map: a point a key frame's slot holds is IsInKeyFrame of that key frame (the reference
+ *   always pairs AddMapPoint with AddObservation), and bad never reverts.  Skipping such a query changes no decision.
+ *   hits_dev [max_hits][3] out (may be NULL when max_hits is 0): (k, q, slot) rows in the order above, slot = c * capacity + j in key frame k.  n_hits_dev [1]: the
+ *   true number of hits.  status_dev [1]: MCS_ERR_CAPACITY when n_hits exceeds max_hits (only the first max_hits rows are written,
+ *   nothing past them), MCS_ERR_INVALID when a query id is >= n_points (that query is dropped, the others are unaffected; this
+ *   error is kept over MCS_ERR_CAPACITY), MCS_OK otherwise.
+ *   Scratch: 4 * n_points + n_kf * n_q bytes for the pre-filter, about 170 bytes per (k, q, c) entry, and the front end's
+ *   per-slot arrays for n_kf * n_cams images.
+ * capacity <= 65535; n_kf * n_cams * capacity < 2^24 and n_kf * n_q * n_cams < 2^24 (MCS_ERR_UNSUPPORTED beyond: split the
+ * batch); cameras of different sizes: MCS_ERR_UNSUPPORTED. */
+typedef struct mcs_fuse_target {
+    mcs_packed_frame frame;      /* the key frame's features */
+    const int32_t*   mp_dev;     /* [n_cams * capacity] slot-indexed map-point ids, or NULL */
+    const double*    mtmc_inv;   /* host [n_cams * 16] */
+    double           ow[3];
+} mcs_fuse_target;
+
+#define MCS_FUSE_NEIGHBOUR 0     /* Fuse(pKF, curKF, vpMapPoints, th)  :1265  float dist3D, best <= th_low          */
+#define MCS_FUSE_FIRST     1     /* Fuse(pKF, vpMapPoints, th)         :1420  float dist3D, first in-level candidate */
+#define MCS_FUSE_SIM3      2     /* Fuse(pKF, Scw, vpPoints, th)       :1570  double dist3D, best <= th_low         */
+
+int  mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, int32_t capacity, int32_t dim, const mcs_ocam* cams,
+                     const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, int32_t variant, const int32_t* query_mp_dev,
+                     int32_t n_q, int32_t n_points, const double* world_pos_dev, const double* min_dist_dev, const double* max_dist_dev,
+                     const uint8_t* desc_dev, const uint8_t* dmask_dev, const uint8_t* bad_dev, double th, int32_t th_low,
+                     int32_t having_masks, int32_t* hits_dev, int32_t max_hits, int32_t* n_hits_dev, int32_t* status_dev, void* stream);
+
 /* ---- bag of words: ORBVocabulary::transform and the feature-vector guided search (SURVEY 8f, rank 4) ------- */
 /* The vocabulary tree of DBoW2::TemplatedVocabulary<FORB::TDescriptor, FORB> (ref include/cORBVocabulary.h:34,
  * ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h) as flat arrays.  Node 0 is the root; parent[0] is ignored.

@@ -15,8 +15,8 @@ import pathlib
 
 import numpy as np
 
-from .ctypes_defs import (MAX_LEVELS, BowFrame, ExtractorInfo, ExtractorParams, FrameView, KEYPOINT_DTYPE, MapPointDevView, MapPointView, Ocam,
-                          PackedFrame, WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
+from .ctypes_defs import (MAX_LEVELS, BowFrame, ExtractorInfo, ExtractorParams, FrameView, FuseTarget, KEYPOINT_DTYPE, MapPointDevView,
+                          MapPointView, Ocam, PackedFrame, WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
 
 _PKG = pathlib.Path(__file__).resolve().parent
 _LIB_PATH = _PKG / "libmcs_b200.so"
@@ -767,6 +767,32 @@ def _init_search_outputs(out, diag, stream, dev):
     return out, (_dptr(out[0]), _dptr(out[1]) if diag else None, _stream_handle(stream, dev))
 
 
+def _fuse_replay(variant, rows, kf_mp, bad, rig, cur_rig=None, cur_rays=None, kf_rays=None):
+    """The map bookkeeping of the three Fuse overloads (ref :1377-1416, :1540-1565, :1692-1716) over their hits, in the
+    reference's order.  rows: (map point i, its keypoint in curKF for variant 0's ray, the hit keypoint of pKF per camera or -1),
+    query by query.  A hit on a keypoint with a non-bad occupant is a Replace (variant 0: only when CheckDistEpipolarLine holds,
+    with camera c's MtMc_inv of curKF and MtMc of pKF), a free keypoint gets AddObservation + AddMapPoint and kf_mp is updated in
+    place.  Returns (nFused, ops [k, 3]): rows (0, mp, keypoint) and (1, mp, other)."""
+    ops, fused = [], 0
+    for i, ray, hit in rows:
+        for cam, b in enumerate(hit):
+            b = int(b)
+            if b < 0:
+                continue
+            other = int(kf_mp[b])
+            if other >= 0:
+                good = not bad[other]
+                if variant == 0 and good:
+                    T1 = inv_rigid(cur_rig.MtMc[cam]) if cur_rig is not None else np.eye(4)
+                    E = compute_E_rel(_mm(T1, rig.MtMc[cam]))
+                    good = check_epipolar(cur_rays[ray], kf_rays[b], E, 1e-2)
+                if good:
+                    ops.append((1, i, other)); fused += 1
+            else:
+                ops.append((0, i, b)); kf_mp[b] = i
+    return fused, np.asarray(ops, np.int32).reshape(-1, 3)
+
+
 class cORBmatcher:
     """ref include/cORBmatcher.h:55-178; thresholds as in src/cORBmatcher.cpp:46-64."""
 
@@ -1000,27 +1026,83 @@ class cORBmatcher:
         uv, ok, lvl = _project(rig, KF.scale_factors, world_pos, min_dist, max_dist, idx, np.tile(np.arange(nc), (len(idx), 1)),
                                float_dist=(variant != 2))
         best = self.FuseCandidates(KF, uv, ok, lvl, th, mp_desc, mp_dmask, first_wins=(variant == 1), points=idx, _sw=_sw)
-        ops, fused = [], 0
         pos_of = {}
         if variant == 0:
             pos_of = {int(i): j for j, i in enumerate(points) if i >= 0}     # keypoint of curKF that carries map point i
-        for kk, i in enumerate(idx):
-            for cam in range(nc):
-                b = int(best[kk, cam])
-                if b < 0:
-                    continue
-                other = int(kf_mp[b])
-                if other >= 0:
-                    good = not bad[other]
-                    if variant == 0 and good:
-                        T1 = inv_rigid(cur_rig.MtMc[cam]) if cur_rig is not None else np.eye(4)
-                        E = compute_E_rel(_mm(T1, rig.MtMc[cam]))
-                        good = check_epipolar(cur_rays[pos_of[i]], kf_rays[b], E, 1e-2)
-                    if good:
-                        ops.append((1, i, other)); fused += 1
-                else:
-                    ops.append((0, i, b)); kf_mp[b] = i
-        return fused, np.asarray(ops, np.int32).reshape(-1, 3), kf_mp
+        rows = ((i, pos_of.get(i), best[kk]) for kk, i in enumerate(idx))
+        fused, ops = _fuse_replay(variant, rows, kf_mp, bad, rig, cur_rig, cur_rays, kf_rays)
+        return fused, ops, kf_mp
+
+    def FuseDevice(self, kfs, queries_t, capacity, cams, masks_t, scale_factors, world_t, min_dist_t, max_dist_t, desc_t, dmask_t=None,
+                   bad_t=None, variant=0, th=3.0, max_hits=None, stream=None, out=None):
+        """mcs_fuse_device: the matching part of the Fuse overloads for many key frames in one call (see include/mcs_b200.h).
+        kfs: per target key frame (frame, mp_t, MtMc_inv, ow) with frame = (packed uint8 cuda tensor, n_parts, part_images,
+        first_image), mp_t its int32 cuda [n_cams * capacity] map-point ids by slot or None, MtMc_inv [n_cams, 4, 4] of the pose
+        to project with and ow [3] the centre of the depth test.  queries_t: int32 cuda [n_q] map-point ids (-1 = NULL).  cams:
+        the rig's camera models, masks_t [n_cams,H,W] u8 cuda their mirror masks.  world_t [n_points,3] f64, min_dist_t /
+        max_dist_t [n_points] f64, desc_t / dmask_t [n_points, dim] u8, bad_t [n_points] u8 (or None): cuda tensors.  variant 0 =
+        Fuse(pKF, curKF, ., th) (:1265), 1 = Fuse(pKF, ., th) (:1420), 2 = Fuse(pKF, Scw, ., th) (:1570).  max_hits defaults to
+        n_kf * n_q * n_cams (every entry).  Asynchronous on `stream`.  Returns (hits [max_hits, 3] (k, q, slot) rows, n_hits [1],
+        status [1]) as cuda tensors."""
+        import torch
+        dev = queries_t.device
+        nc, n_q, n_kf = len(cams), int(queries_t.shape[0]), len(kfs)
+        if max_hits is None:
+            max_hits = max(n_kf * n_q * nc, 1)
+        if out is None:
+            out = (torch.zeros((max_hits, 3), dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev),
+                   torch.zeros(1, dtype=torch.int32, device=dev))
+        mi = [np.ascontiguousarray(k[2], np.float64).reshape(-1) for k in kfs]          # kept alive through the call
+        tg = (FuseTarget * n_kf)()
+        for t, (frame, mp_t, _, ow), m in zip(tg, kfs, mi):
+            t.frame = PackedFrame(frame[0].data_ptr(), *frame[1:4])
+            t.mp_dev, t.mtmc_inv = _dptr(mp_t), m.ctypes.data
+            t.ow[:] = [float(x) for x in ow]
+        sf = np.ascontiguousarray(scale_factors, np.float64)
+        _check(lib().mcs_fuse_device(tg, n_kf, nc, capacity, int(desc_t.shape[1]), _ocams(cams), _dptr(masks_t), len(sf), _p(sf), int(variant),
+                                     _dptr(queries_t), n_q, int(world_t.shape[0]), _dptr(world_t), _dptr(min_dist_t), _dptr(max_dist_t),
+                                     _dptr(desc_t), _dptr(dmask_t), _dptr(bad_t), float(th), self.TH_LOW_, int(self.havingMasks),
+                                     _dptr(out[0]), int(out[0].shape[0]), _dptr(out[1]), _dptr(out[2]), _stream_handle(stream, dev)))
+        return out
+
+    def FuseReplay(self, KF, rig, kf_mp, points, hits, capacity, world_pos, min_dist, max_dist, bad, in_kf, mp_desc, mp_dmask=None, th=2.5,
+                   variant=1, Scw=None, cur_rays=None, kf_rays=None, cur_rig=None, stale=(), _sw=None):
+        """Fuse on one target key frame from the hits FuseDevice computed for it: the same arguments and results as Fuse, plus
+        hits = that key frame's (q, slot) rows (q indexes `points`, slot = c * capacity + j) and `stale`, the map points whose
+        descriptor was rewritten since the device call (a Replace survivor's ComputeDistinctiveDescriptors).  The skip tests read
+        the live bad / in_kf / kf_mp given here; a stale query is searched again on the host (FuseCandidates) for variants 0 and 2,
+        whose decisions read the descriptor, and self.fuse_researched counts those queries.  KF's keypoints are in camera-major
+        order (cMultiFrame's, as Frame.from_cameras builds it), so that slot c * capacity + j is keypoint first[c] + j.  Variant
+        0 reads curKF's ray of query q at cur_rays[q] (the reference's GetKeyPointRay(i)).  Returns (nFused, ops, kf_mp), what
+        Fuse returns on the same state."""
+        kf_mp = np.ascontiguousarray(kf_mp, np.int32).copy()
+        nc = len(rig.cams)
+        if variant == 2:
+            rig = _sim3_rig(rig, Scw)
+            already = set(int(m) for m in kf_mp if m >= 0 and not bad[m])
+            live = [q for q, i in enumerate(points) if i >= 0 and not bad[i] and int(i) not in already]
+        else:
+            live = [q for q, i in enumerate(points) if i >= 0 and not bad[i] and not in_kf[i]]
+        counts = np.bincount(np.asarray(KF.key_cam, np.int64), minlength=nc)
+        first = np.concatenate([[0], np.cumsum(counts)])
+        best = {q: np.full(nc, -1, np.int32) for q in live}
+        for q, slot in np.asarray(hits, np.int64).reshape(-1, 2):
+            if int(q) in best:
+                c = int(slot) // capacity
+                best[int(q)][c] = first[c] + int(slot) - c * capacity
+        stale = set(int(i) for i in stale) if variant != 1 else set()
+        redo = [q for q in live if int(points[q]) in stale]
+        if redo:
+            ids = [int(points[q]) for q in redo]
+            uv, ok, lvl = _project(rig, KF.scale_factors, world_pos, min_dist, max_dist, ids, np.tile(np.arange(nc), (len(ids), 1)),
+                                   float_dist=(variant != 2))
+            again = self.FuseCandidates(KF, uv, ok, lvl, th, mp_desc, mp_dmask, first_wins=False, points=ids, _sw=_sw)
+            for q, row in zip(redo, again):
+                best[q] = row
+        self.fuse_researched = len(redo)
+        rows = ((int(points[q]), q, best[q]) for q in live)
+        fused, ops = _fuse_replay(variant, rows, kf_mp, bad, rig, cur_rig, cur_rays, kf_rays)
+        return fused, ops, kf_mp
 
     def SearchByProjectionKFScw(self, KF, rig, Scw, points, matched, world_pos, min_dist, max_dist, bad, mp_desc, mp_dmask=None, th=10,
                                 _sw=None):

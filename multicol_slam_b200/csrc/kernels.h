@@ -199,6 +199,20 @@ cudaError_t launch_search_for_initialization(const InitSearchDevArgs& a, cudaStr
 // prev = the position of every F1 keypoint below its camera's count (f1: host [n_cams])
 cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_cams, int capacity, double* prev, cudaStream_t st);
 int proj_search_max_rounds();
+// The Fuse overloads (mcs_fuse_device) for n_kf key frames in one call: the searched frame (PsFrameArgs) is the n_kf * n_cams
+// images of the targets, image k * n_cams + c = camera c of key frame k; th_high holds TH_LOW_; frame_mp and nmatches are unused.
+struct FuseDevArgs : PsFrameArgs {
+    int n_kf, n_kf_cams, variant, n_q, n_points;              // n_kf_cams: cameras per key frame
+    const int* const* kf_mp;                                 // host [n_kf]: each key frame's slot-indexed map-point ids (NULL entries)
+    const double* mtmc_inv; const double* ow;                // host [n_kf * n_kf_cams * 16], [n_kf * 3]
+    const mcs_ocam* models; const uint8_t* masks;            // host [n_kf_cams], device [n_kf_cams][h][w]
+    const int* query_mp;                                     // device [n_q], -1 = NULL
+    const double* world_pos; const double* min_dist; const double* max_dist;   // device map points
+    const uint8_t* desc; const uint8_t* dmask; const uint8_t* bad;
+    double th;
+    int* hits; int max_hits; int* n_hits;                    // device [max_hits * 3], [1]
+};
+cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st);
 
 // ---- bag of words (bow_kernels.cu) ----
 // vocabulary tree on the device: CSR children in the reference's order, 32-byte node descriptors as uint4 pairs

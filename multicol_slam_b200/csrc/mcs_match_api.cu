@@ -785,6 +785,53 @@ int mcs_search_for_initialization_seed_device(const mcs_packed_frame* f1, int32_
     return sync_if_null_stream(stream);
 }
 
+int mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, int32_t capacity, int32_t dim, const mcs_ocam* cams,
+                    const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, int32_t variant, const int32_t* query_mp_dev,
+                    int32_t n_q, int32_t n_points, const double* world_pos_dev, const double* min_dist_dev, const double* max_dist_dev,
+                    const uint8_t* desc_dev, const uint8_t* dmask_dev, const uint8_t* bad_dev, double th, int32_t th_low,
+                    int32_t having_masks, int32_t* hits_dev, int32_t max_hits, int32_t* n_hits_dev, int32_t* status_dev, void* stream) {
+    // query_mp_dev / hits_dev may be NULL only when they have no entry (an empty tensor has no address)
+    if (!kfs || !cams || !masks_dev || !scale_factors || (!query_mp_dev && n_q > 0) || !world_pos_dev || !min_dist_dev || !max_dist_dev ||
+        !desc_dev || (!hits_dev && max_hits > 0) || !n_hits_dev || !status_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (having_masks && !dmask_dev) return mcs_fail(MCS_ERR_INVALID, "masks requested but not supplied");
+    if (n_kf <= 0 || n_q < 0 || n_points < 0 || max_hits < 0 || n_levels < 1 || n_levels > MCS_MAX_LEVELS)
+        return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (variant < MCS_FUSE_NEIGHBOUR || variant > MCS_FUSE_SIM3) return mcs_fail(MCS_ERR_INVALID, "unknown Fuse variant");
+    for (int k = 0; k < n_kf; ++k) {
+        if (int rc = check_packed_frames(n_cams, capacity, dim, &kfs[k].frame, nullptr)) return rc;
+        if (!kfs[k].mtmc_inv) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    }
+    const CamSizes cz(cams, n_cams);
+    if (int rc = check_cam_sizes(n_cams, cz.w.data(), cz.h.data(), true)) return rc;
+    // the front end's slot and query indices: one image per (key frame, camera), one entry per (key frame, query, camera)
+    if (int rc = check_query_bound((long long)n_kf * n_cams * capacity, "n_kf * n_cams * capacity must stay below 2^24")) return rc;
+    if (int rc = check_query_bound((long long)n_kf * n_q * n_cams, "n_kf * n_q * n_cams must stay below 2^24")) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int NI = n_kf * n_cams;
+    std::vector<PsCamSlots> slots;
+    std::vector<const int*> kf_mp(n_kf);
+    std::vector<double> mtmc_inv(16 * (size_t)NI), ow(3 * (size_t)n_kf);
+    for (int k = 0; k < n_kf; ++k) {
+        const std::vector<PsCamSlots> s = packed_slots(kfs[k].frame, n_cams, capacity, dim);
+        slots.insert(slots.end(), s.begin(), s.end());
+        kf_mp[k] = kfs[k].mp_dev;
+        std::memcpy(&mtmc_inv[16 * (size_t)k * n_cams], kfs[k].mtmc_inv, 128ull * n_cams);
+        for (int i = 0; i < 3; ++i) ow[3 * k + i] = kfs[k].ow[i];
+    }
+    const std::vector<int> cw(NI, cz.w[0]), ch(NI, cz.h[0]);
+    FuseDevArgs a{};
+    set_searched_frame(a, slots, capacity, dim, cw.data(), ch.data(), th_low, having_masks, nullptr, nullptr, status_dev, nullptr);
+    a.n_levels = n_levels; a.sf = scale_factors;
+    a.n_kf = n_kf; a.n_kf_cams = n_cams; a.variant = variant; a.n_q = n_q; a.n_points = n_points;
+    a.kf_mp = kf_mp.data(); a.mtmc_inv = mtmc_inv.data(); a.ow = ow.data(); a.models = cams; a.masks = masks_dev;
+    a.query_mp = query_mp_dev; a.world_pos = world_pos_dev; a.min_dist = min_dist_dev; a.max_dist = max_dist_dev;
+    a.desc = desc_dev; a.dmask = having_masks ? dmask_dev : nullptr; a.bad = bad_dev;
+    a.th = th; a.hits = hits_dev; a.max_hits = max_hits; a.n_hits = n_hits_dev;
+    CUDA_CHECK(launch_fuse_device(a, st));
+    return sync_if_null_stream(stream);
+}
+
 int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view* f2, double* prev_matched, int32_t window_size,
                                   double nnratio, int32_t th_low, int32_t having_masks, int32_t* matches12, int32_t* nmatches) {
     if (!f1 || !f2 || !prev_matched || !matches12 || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");

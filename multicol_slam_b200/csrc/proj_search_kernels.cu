@@ -21,6 +21,9 @@
 //   pi_walk_kernel      SearchForInitialization(F1, F2) (:579-726) only: its acceptance can take a keypoint back from an earlier
 //                       query, so it runs no rounds; one warp per camera walks the camera's queries in order (InitQueries: one per
 //                       F1 slot) and writes matches12 and the survivors' prev.  pi_seed_kernel: FirstInitialization's prev
+//   fu_*                the Fuse overloads (:1265, :1420, :1570) for n_kf key frames searched as one frame of n_kf * n_cams
+//                       images: membership pre-filter, (key frame, query, camera) projections (FuseQueries), a stateless
+//                       decision per query (fu_best / fu_first) and the hit rows in the reference's order
 //
 // No kernel reads anything back to the host: every size that depends on the data (the number of queries, the rounds the
 // fixpoint needed, where the walk starts) lives in device memory and the kernels are launched for the upper bound.
@@ -317,6 +320,29 @@ __global__ void __launch_bounds__(1024) ps_scan_kernel(const int* __restrict__ b
     if (threadIdx.x == 0) *nq = carry;
 }
 
+// The fill of one block's kQbTile entries in the maker's order: emit(k, position) for every valid entry k, positions counted from
+// block_off[blockIdx.x] (ps_scan_kernel's exclusive scan of ps_count_kernel's counts).
+template <class QM, class Emit>
+__device__ __forceinline__ void ps_fill_tile(const QM& a, const int* __restrict__ block_off, const Emit& emit) {
+    __shared__ int s_w[kQbThreads / 32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    int run = block_off[blockIdx.x];
+    for (int i = 0; i < kQbPer; ++i) {
+        const long long k = (long long)blockIdx.x * kQbTile + i * kQbThreads + threadIdx.x;
+        const bool v = a.valid(k, nullptr);
+        const unsigned m = __ballot_sync(0xffffffffu, v);
+        if (lane == 0) s_w[w] = __popc(m);
+        __syncthreads();
+        int off = run, tot = 0;
+        for (int u = 0; u < kQbThreads / 32; ++u) { if (u < w) off += s_w[u]; tot += s_w[u]; }
+        if (v) emit(k, off + __popc(m & ((1u << lane) - 1u)));
+        run += tot;
+        __syncthreads();
+    }
+}
+
+// ps_fill_kernel keeps its own copy of the tile body: written through ps_fill_tile its SASS changes (the query pointer's load is
+// scheduled differently), and the existing searches keep their SASS.
 template <class QM>
 __global__ void __launch_bounds__(kQbThreads) ps_fill_kernel(const QM a, const int* __restrict__ block_off, mcs_window_query* __restrict__ qry) {
     __shared__ int s_w[kQbThreads / 32];
@@ -697,6 +723,171 @@ __global__ void pi_seed_kernel(const PsCamSlots* __restrict__ cams, const int n_
     prev[2 * (size_t)s + 1] = (double)kp.y;
 }
 
+// ---- Fuse (ref :1265-1418, :1420-1567, :1570-1719): n_kf target key frames searched as one frame of n_kf * n_cams images ----
+// A Fuse query takes nothing from another query (the "already occupied" test lives in the host bookkeeping), so there are no
+// rounds: every (key frame k, query q, camera c) entry projects, searches its window in image k * n_cams + c and decides alone.
+// qmap[p]: the first query position holding map point p (>= n_q: none); an id >= n_points drops its query and raises status.
+__global__ void fu_qmap_kernel(const int* __restrict__ query_mp, const int n_q, const int n_points, int* __restrict__ qmap,
+                               int* __restrict__ status) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= n_q) return;
+    const int p = query_mp[q];
+    if (p >= n_points) *status = MCS_ERR_INVALID;
+    else if (p >= 0) atomicMin(&qmap[p], q);
+}
+
+// The membership pre-filter: held[k * n_q + qmap[p]] = 1 for every point p a slot of key frame k's row holds (below the camera's
+// count).  Queries holding the same point share the flag of its first position.
+__global__ void fu_held_kernel(const PsCamSlots* __restrict__ slots, const int* const* __restrict__ kf_mp, const int n_kf, const int n_cams,
+                               const int capacity, const int n_q, const int n_points, const int* __restrict__ qmap, uint8_t* __restrict__ held) {
+    const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= (long long)n_kf * n_cams * capacity) return;
+    const int img = (int)(g / capacity), j = (int)(g - (long long)img * capacity), k = img / n_cams;
+    const int* mp = kf_mp[k];
+    if (!mp || j >= min(*slots[img].count, capacity)) return;
+    const int p = mp[(size_t)(img - k * n_cams) * capacity + j];
+    if (p < 0 || p >= n_points) return;
+    const int q = qmap[p];
+    if (q < n_q) held[(size_t)k * n_q + q] = 1;
+}
+
+// Entry e = (k * n_q + q) * n_cams + c: query q's point, when not NULL, not bad and not held by key frame k, projected with
+// k's MtMc_inv into camera c (WorldToCamHom_fast, mirror mask), its distance to k's centre in the range [min, max] and its
+// level predicted, in the operation order of the host projection (api._project): dist3D a float for :1265 / :1420, a double for
+// :1570 (ref :1301, :1472, :1624).  -fmad=false keeps the norm free of FMA contraction.
+struct FuseProjArgs {
+    int n_kf, n_cams, n_q, n_points, n_levels; bool float_dist;
+    const int* query_mp; const uint8_t* bad; const uint8_t* held; const int* qmap;
+    const double* pos; const double* dmin; const double* dmax;
+    const mcs_ocam* models; const double* mtmc_inv; const double* ow; const uint8_t* masks; const double* sf;
+};
+__global__ void __launch_bounds__(256) fu_project_kernel(const FuseProjArgs a, uint8_t* __restrict__ ok, double* __restrict__ u,
+                                                         double* __restrict__ v, int* __restrict__ level) {
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (long long)a.n_kf * a.n_q * a.n_cams) return;
+    const long long kq = e / a.n_cams;
+    const int c = (int)(e - kq * a.n_cams), k = (int)(kq / a.n_q), q = (int)(kq - (long long)k * a.n_q);
+    ok[e] = 0;
+    const int p = a.query_mp[q];
+    if (p < 0 || p >= a.n_points) return;
+    if ((a.bad && a.bad[p]) || a.held[(size_t)k * a.n_q + a.qmap[p]]) return;
+    const mcs_ocam cam = a.models[c];
+    const double P0 = a.pos[3 * p], P1 = a.pos[3 * p + 1], P2 = a.pos[3 * p + 2];
+    double x, y;
+    if (!cam_project_in_mask(a.mtmc_inv + 16 * ((size_t)k * a.n_cams + c), cam, a.masks + (size_t)c * cam.width * cam.height, P0, P1, P2, x, y))
+        return;
+    const double* O = a.ow + 3 * k;
+    const double o0 = P0 - O[0], o1 = P1 - O[1], o2 = P2 - O[2];
+    double d = sqrt((o0 * o0 + o1 * o1) + o2 * o2);
+    if (a.float_dist) d = (double)__double2float_rn(d);
+    if (d < a.dmin[p] || d > a.dmax[p]) return;
+    const double ratio = d / a.dmin[p];
+    int lv = 0;                                   // std::lower_bound(vfScaleFactors, ratio), clamped to the last level
+    while (lv < a.n_levels && a.sf[lv] < ratio) ++lv;
+    if (lv >= a.n_levels) lv = a.n_levels - 1;
+    ok[e] = 1; u[e] = x; v[e] = y; level[e] = lv;
+}
+
+struct FuseQueries {             // entry e as fu_project_kernel set it: GetFeaturesInArea(c, u, v, th * sf[l]) on levels {l - 1, l} of k
+    long long n_entries; int n_q, n_cams;
+    const uint8_t* ok; const double* u; const double* v; const int* level; const int* query_mp;
+    const double* sf; double th;
+    __host__ __device__ long long size() const { return n_entries; }
+    __device__ bool valid(long long e, int*) const { return e < n_entries && ok[e]; }
+    __device__ mcs_window_query make(long long e) const {
+        const long long kq = e / n_cams;
+        const int c = (int)(e - kq * n_cams), k = (int)(kq / n_q), lvl = level[e];
+        mcs_window_query qq;
+        qq.cam = k * n_cams + c; qq.min_level = lvl - 1; qq.max_level = lvl; qq.desc_index = query_mp[kq - (long long)k * n_q];
+        qq.x = u[e]; qq.y = v[e]; qq.r = th * sf[lvl];
+        return qq;
+    }
+};
+
+// entry[i] = the maker entry of query i: ps_fill_kernel's fill, writing the entry index instead of the query
+template <class QM>
+__global__ void __launch_bounds__(kQbThreads) fu_entry_kernel(const QM a, const int* __restrict__ block_off, int* __restrict__ entry) {
+    ps_fill_tile(a, block_off, [&](long long k, int o) { entry[o] = (int)k; });
+}
+
+// MCS_FUSE_NEIGHBOUR / MCS_FUSE_SIM3: the best candidate (strict < over the visiting order, ref :1345-1356) is the first key of
+// the query's list, which holds every candidate's key when nothing is taken; kept when its distance is <= th_low (:1359).
+__global__ void __launch_bounds__(256) fu_best_kernel(const int* __restrict__ nq_p, const unsigned* __restrict__ lkey,
+                                                      const int* __restrict__ lslot, const int th_low, int* __restrict__ dec) {
+    const int nq = *nq_p;
+    for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += gridDim.x * blockDim.x) {
+        const unsigned k0 = lkey[(size_t)q * kPsK];
+        dec[q] = k0 != kNoKey && (int)(k0 >> 16) <= th_low ? lslot[(size_t)q * kPsK] : -1;
+    }
+}
+
+// MCS_FUSE_FIRST: the distance is discarded (ref :1506-1514, `dist` stays 0), so the first candidate of the window in visiting
+// order that passes the level filter wins, whatever the distances the list sorted by.  One warp per query walks the window in
+// window_kbest's order and stops at the first candidate; a query whose list counted none is not walked.  The cell range, the
+// item order and the level / radius filter below must stay those of window_kbest (which keeps its own copy: its SASS is shared
+// by every device search); the MCS_FUSE_FIRST parity tests pin them against the host window search.
+__global__ void __launch_bounds__(256) fu_first_kernel(const WindowFrameDev f, const mcs_window_query* __restrict__ qry, const int* __restrict__ nq_p,
+                                                       const int* __restrict__ lcnt, const int th_low, int* __restrict__ dec) {
+    const int lane = threadIdx.x & 31, nq = *nq_p;
+    const int stride = gridDim.x * (blockDim.x >> 5);
+    for (int q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; q < nq; q += stride) {
+        int first = -1;
+        if (lcnt[q] > 0 && 0 <= th_low) {
+            const mcs_window_query qq = qry[q];
+            const int cam = qq.cam;
+            const double x = qq.x, y = qq.y, r = qq.r;
+            const double wi = f.winv[cam], hi = f.hinv[cam];
+            const int cx0 = max(0, (int)floor((x - 0 - r) * wi)), cx1 = min(MCS_FRAME_GRID_COLS - 1, (int)ceil((x - 0 + r) * wi));
+            const int cy0 = max(0, (int)floor((y - 0 - r) * hi)), cy1 = min(MCS_FRAME_GRID_ROWS - 1, (int)ceil((y - 0 + r) * hi));
+            const bool check = !(qq.min_level == -1 && qq.max_level == -1);
+            const bool same = check && qq.min_level == qq.max_level;
+            for (int ix = cx0; ix <= cx1 && first < 0; ++ix)
+                for (int iy = cy0; iy <= cy1 && first < 0; ++iy) {
+                    const int cell = (cam * MCS_FRAME_GRID_COLS + ix) * MCS_FRAME_GRID_ROWS + iy;
+                    const int s = f.cell_start[cell], e = f.cell_start[cell + 1];
+                    for (int base = s; base < e && first < 0; base += 32) {
+                        const int it = base + lane;
+                        bool ok = it < e;
+                        int id = 0;
+                        if (ok) {
+                            id = f.cell_items[it];
+                            const int oct = f.koct[id];
+                            if (check && !same) ok = !(oct < qq.min_level || oct > qq.max_level);
+                            else if (same) ok = (oct == qq.min_level);
+                            if (ok) ok = !(fabs((double)f.kx[id] - x) > r || fabs((double)f.ky[id] - y) > r);
+                        }
+                        const unsigned m = __ballot_sync(0xffffffffu, ok);
+                        if (m) first = __shfl_sync(0xffffffffu, id, __ffs(m) - 1);
+                    }
+                }
+        }
+        if (lane == 0) dec[q] = first;
+    }
+}
+
+struct FuseHitQueries {          // the queries with a hit, in query order (= the reference's (key frame, query, camera) order)
+    long long Q; const int* nq; const int* dec;
+    __host__ __device__ long long size() const { return Q; }
+    __device__ bool valid(long long i, int*) const { return i < Q && i < *nq && dec[i] >= 0; }
+};
+
+// The hit rows: row o = (k, q, slot in k) of the o-th query with a hit; rows past max_hits are counted (ps_scan_kernel writes the
+// true total) but not written, and raise MCS_ERR_CAPACITY unless status already holds an error.
+__global__ void __launch_bounds__(kQbThreads) fu_hits_kernel(const FuseHitQueries a, const int* __restrict__ block_off, const int* __restrict__ entry,
+                                                             const int n_q, const int n_cams, const int capacity, const int max_hits,
+                                                             int* __restrict__ hits, int* __restrict__ status) {
+    ps_fill_tile(a, block_off, [&](long long k, int o) {
+        if (o < max_hits) {
+            const int e = entry[k], kq = e / n_cams, kf = kq / n_q;
+            hits[3 * (size_t)o] = kf;
+            hits[3 * (size_t)o + 1] = kq - kf * n_q;
+            hits[3 * (size_t)o + 2] = a.dec[k] - kf * n_cams * capacity;
+        } else {
+            atomicCAS(status, MCS_OK, MCS_ERR_CAPACITY);
+        }
+    });
+}
+
 }  // namespace
 
 int proj_search_max_rounds() { return kPsRounds; }
@@ -711,6 +902,7 @@ struct PsFront {
     const PsCamSlots* slots;     // device [n_cams]: the searched frame's image slots
     const mcs_keypoint* keys;    // the searched frame in slot order
     const mcs_window_query* qry; const unsigned* lkey; const int* lslot; const int* lcnt;
+    const int* qoff;                                         // the query fill's block offsets (kQbTile entries of the maker per block)
     int* ctl; int* dec; unsigned* owner;                     // PsState's; owner starts at 0xFFFFFFFF
     const uint32_t* qd; const uint32_t* qk;                  // the query descriptors and masks (qk NULL unless masked)
     long long Q;                                             // queries at most (the maker's size)
@@ -718,9 +910,11 @@ struct PsFront {
 };
 
 // The front end from the query maker on: the frame view of `a` in slot order and its grid, the queries in the maker's order and
-// their lists.  qdesc / qmask: the query descriptors, row desc_index.
+// their lists.  qdesc / qmask: the query descriptors, row desc_index.  staged (may be NULL): a.cams already on the device, in
+// stream order, which the front end then reads instead of staging its own copy.
 template <class QM>
-cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const uint8_t* qmask, PsFront& fr, cudaStream_t st) {
+cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const uint8_t* qmask, PsFront& fr, cudaStream_t st,
+                     const PsCamSlots* staged = nullptr) {
     const int NS = a.n_cams * a.capacity;
     const int ncell = a.n_cams * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
     const long long Q = qm.size();
@@ -737,7 +931,8 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
                   sizeof(mcs_window_query) * Q, 4ull * Q * kPsK, 4ull * Q * kPsK, 4ull * Q, 8ull * Q, 8ull * NS},   // qry lkey lslot lcnt dec owner
                  st);
     if (e != cudaSuccess) return e;
-    mcs_ocam* cams = sc.at<mcs_ocam>(0); double* sf = sc.at<double>(1); PsCamSlots* slots = sc.at<PsCamSlots>(2);
+    mcs_ocam* cams = sc.at<mcs_ocam>(0); double* sf = sc.at<double>(1);
+    PsCamSlots* slots = staged ? const_cast<PsCamSlots*>(staged) : sc.at<PsCamSlots>(2);
     mcs_keypoint* keys = sc.at<mcs_keypoint>(3); int* key_cam = sc.at<int>(4); float* kx = sc.at<float>(5); float* ky = sc.at<float>(6);
     int* koct = sc.at<int>(7); uint8_t* desc = sc.at<uint8_t>(8); uint8_t* dmask = a.masked ? sc.at<uint8_t>(9) : nullptr;
     int* cell_of = sc.at<int>(10); int* cursor = sc.at<int>(11); int* cell_start = sc.at<int>(12); int* cell_items = sc.at<int>(13);
@@ -751,7 +946,7 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
     for (int c = 0; c < a.n_cams; ++c) { hc[c].width = a.cam_w[c]; hc[c].height = a.cam_h[c]; }
     if (e == cudaSuccess) e = stage_to_device(hc.data(), sizeof(mcs_ocam) * a.n_cams, cams, st);
     if (e == cudaSuccess) e = stage_to_device(a.sf, sizeof(double) * a.n_levels, sf, st);
-    if (e == cudaSuccess) e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, slots, st);
+    if (e == cudaSuccess && !staged) e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, slots, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl, 0, 16, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl + 4, 0x7F, 4 * kPsRounds, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(owner, 0xFF, 8ull * NS, st);
@@ -770,7 +965,7 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
     }
     fr.f = WindowFrameDev{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv};
     fr.slots = slots; fr.keys = keys;
-    fr.qry = qry; fr.lkey = lkey; fr.lslot = lslot; fr.lcnt = lcnt; fr.ctl = ctl; fr.dec = dec; fr.owner = owner;
+    fr.qry = qry; fr.lkey = lkey; fr.lslot = lslot; fr.lcnt = lcnt; fr.qoff = boff; fr.ctl = ctl; fr.dec = dec; fr.owner = owner;
     fr.qd = (const uint32_t*)qdesc; fr.qk = a.masked ? (const uint32_t*)qmask : nullptr;
     fr.Q = Q; fr.sms = sms;
     fr.wblocks = (int)std::min<long long>((Q + 7) / 8, (long long)sms * 16);
@@ -944,6 +1139,67 @@ cudaError_t launch_search_for_initialization(const InitSearchDevArgs& a, cudaStr
     if (e == cudaSuccess && a.diag) pi_diag_kernel<<<1, 1, 0, st>>>(fr.ctl, a.diag);
     if (e == cudaSuccess) e = cudaGetLastError();
     return t.sc.release(fr.sc.release(e));
+}
+
+// Fuse for n_kf key frames: membership pre-filter (fu_qmap / fu_held), the (k, q, c) projections (fu_project), the front end over
+// the n_kf * n_cams images with FuseQueries, the stateless decision (fu_best or fu_first), then a count / scan / fill of the hits
+// in query order.  Scratch beyond the front end's: 4 * n_points + n_kf * n_q bytes for the pre-filter and 33 bytes per entry.
+cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st) {
+    const int nk = a.n_kf, nc = a.n_kf_cams, NI = nk * nc;
+    const long long QE = (long long)nk * a.n_q * nc;
+    const int nb = (int)((QE + kQbTile - 1) / kQbTile);
+    cudaError_t e = cudaMemsetAsync(a.n_hits, 0, 4, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
+    if (e != cudaSuccess) return e;
+    StreamScratch sc;
+    e = sc.alloc({sizeof(PsCamSlots) * NI, sizeof(int*) * nk, 128ull * NI, 24ull * nk, sizeof(mcs_ocam) * nc, 8ull * a.n_levels,   // staged
+                  4ull * a.n_points, (size_t)nk * a.n_q,                                                                        // qmap held
+                  (size_t)QE, 8ull * QE, 8ull * QE, 4ull * QE, 4ull * QE, 4ull * QE, 4ull * (nb + 1), 4ull * (nb + 1)},         // ok u v level entry dec
+                 st);
+    if (e != cudaSuccess) return e;
+    PsCamSlots* slots = sc.at<PsCamSlots>(0); const int** kf_mp = sc.at<const int*>(1); double* mtmc_inv = sc.at<double>(2);
+    double* ow = sc.at<double>(3); mcs_ocam* models = sc.at<mcs_ocam>(4); double* sf = sc.at<double>(5);
+    int* qmap = sc.at<int>(6); uint8_t* held = sc.at<uint8_t>(7);
+    uint8_t* ok = sc.at<uint8_t>(8); double* u = sc.at<double>(9); double* v = sc.at<double>(10); int* level = sc.at<int>(11);
+    int* entry = sc.at<int>(12); int* dec = sc.at<int>(13); int* bcount = sc.at<int>(14); int* boff = sc.at<int>(15);
+    e = stage_to_device(a.cams, sizeof(PsCamSlots) * NI, slots, st);
+    if (e == cudaSuccess) e = stage_to_device(a.kf_mp, sizeof(int*) * nk, kf_mp, st);
+    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * NI, mtmc_inv, st);
+    if (e == cudaSuccess) e = stage_to_device(a.ow, 24ull * nk, ow, st);
+    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * nc, models, st);
+    if (e == cudaSuccess) e = stage_to_device(a.sf, 8ull * a.n_levels, sf, st);
+    if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(qmap, 0x7F, 4ull * a.n_points, st);     // above every query position
+    if (e == cudaSuccess && nk * a.n_q > 0) e = cudaMemsetAsync(held, 0, (size_t)nk * a.n_q, st);
+    if (e != cudaSuccess) return sc.release(e);
+    if (a.n_q > 0) {
+        fu_qmap_kernel<<<(a.n_q + 255) / 256, 256, 0, st>>>(a.query_mp, a.n_q, a.n_points, qmap, a.status);
+        const long long ns = (long long)NI * a.capacity;
+        fu_held_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, st>>>(slots, kf_mp, nk, nc, a.capacity, a.n_q, a.n_points, qmap, held);
+        const FuseProjArgs pa{nk, nc, a.n_q, a.n_points, a.n_levels, a.variant != MCS_FUSE_SIM3, a.query_mp, a.bad, held, qmap, a.world_pos,
+                              a.min_dist, a.max_dist, models, mtmc_inv, ow, a.masks, sf};
+        fu_project_kernel<<<(unsigned)((QE + 255) / 256), 256, 0, st>>>(pa, ok, u, v, level);
+        e = cudaGetLastError();
+    }
+    PsFront fr;
+    if (e == cudaSuccess) {
+        const FuseQueries qm{QE, a.n_q, nc, ok, u, v, level, a.query_mp, nullptr, a.th};
+        e = ps_front(a, qm, a.desc, a.dmask, fr, st, slots);      // the slot table the pre-filter already staged
+        if (e == cudaSuccess && nb > 0) {
+            fu_entry_kernel<<<nb, kQbThreads, 0, st>>>(qm, fr.qoff, entry);
+            if (a.variant == MCS_FUSE_FIRST) {
+                fu_first_kernel<<<fr.wblocks, 256, 0, st>>>(fr.f, fr.qry, fr.ctl, fr.lcnt, a.th_high, dec);
+            } else {
+                const int blocks = (int)std::min<long long>((QE + 255) / 256, (long long)fr.sms * 8);
+                fu_best_kernel<<<blocks, 256, 0, st>>>(fr.ctl, fr.lkey, fr.lslot, a.th_high, dec);
+            }
+            const FuseHitQueries hq{QE, fr.ctl, dec};
+            ps_count_kernel<<<nb, kQbThreads, 0, st>>>(hq, bcount, nullptr);
+            ps_scan_kernel<<<1, 1024, 0, st>>>(bcount, nb, boff, a.n_hits);
+            fu_hits_kernel<<<nb, kQbThreads, 0, st>>>(hq, boff, entry, a.n_q, nc, a.capacity, a.max_hits, a.hits, a.status);
+            e = cudaGetLastError();
+        }
+    }
+    return sc.release(fr.sc.release(e));
 }
 
 cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_cams, int capacity, double* prev, cudaStream_t st) {

@@ -59,6 +59,12 @@ class BowFrame(C.Structure):
                 ("fv_features_dev", C.c_void_p), ("mp_dev", C.c_void_p)]
 
 
+class FuseTarget(C.Structure):
+    """mcs_fuse_target: a Fuse target key frame in packed feature buffers, its slot-indexed map-point ids (device, or NULL), the
+    MtMc_inv of the pose to project with (host [n_cams * 16]) and the centre of the depth test"""
+    _fields_ = [("frame", PackedFrame), ("mp_dev", C.c_void_p), ("mtmc_inv", C.c_void_p), ("ow", C.c_double * 3)]
+
+
 def set_prototypes(lib):
     """argument types of the entry points whose many arguments are easiest to get wrong from Python"""
     P, I, D = C.c_void_p, C.c_int32, C.c_double
@@ -76,6 +82,9 @@ def set_prototypes(lib):
     f.restype = C.c_int
     f = lib.mcs_search_for_initialization_seed_device
     f.argtypes = [C.POINTER(PackedFrame), I, I, I, P, P]
+    f.restype = C.c_int
+    f = lib.mcs_fuse_device
+    f.argtypes = [C.POINTER(FuseTarget), I, I, I, I, P, P, I, P, I, P, I, I, P, P, P, P, P, P, D, I, I, P, I, P, P, P]
     f.restype = C.c_int
     f = lib.mcs_vocabulary_level_nodes
     f.argtypes = [P, I, C.POINTER(I)]

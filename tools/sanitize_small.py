@@ -40,4 +40,22 @@ mt.SearchForInitializationSeedDevice((packed, 1, 2, 0), 1, cap, prev_t)
 ni, _ = mt.SearchForInitializationDevice((packed, 1, 2, 0), (packed, 1, 2, 1), cap, [(333, 211)], prev_t, 30, m12_t)
 torch.cuda.synchronize()
 assert int(ni.item()) == n and np.array_equal(m12_t[:len(k)].cpu().numpy(), m12)
-print("sanitize_small ok", len(k), n, nh)
+# Fuse on the device: map points on the bearing rays of the frame's keypoints, the frame packed twice as two target key frames
+rg = api.Rig([cam])
+rays, _, _ = api.frame_prepare(k, np.zeros(len(k), np.int32), [cam])
+world = rays * np.linspace(2.0, 4.0, len(k))[:, None]
+lo, hi, pts = np.full(len(k), 1.0), np.full(len(k), 8.0), np.arange(len(k), dtype=np.int32)
+kf_mp = np.where(np.arange(len(k)) % 3 == 0, (np.arange(len(k)) + 1) % len(k), -1).astype(np.int32)
+fn, fops, _ = mt.Fuse(F, rg, kf_mp, pts, world, lo, hi, np.zeros(len(k), np.uint8), np.zeros(len(k), bool), d, m, th=2.5, variant=2,
+                      Scw=api.inv_rigid(rg.M_t))
+tt = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
+kft = [((packed, 1, 2, f), None, rg.MtMc_inv, rg.M_t[:3, 3]) for f in range(2)]
+hits, nh_t, st_t = mt.FuseDevice(kft, tt(pts), cap, [cam], tt(np.stack(rg.masks)), F.scale_factors, tt(world), tt(lo), tt(hi), tt(d), tt(m),
+                                 variant=2, th=2.5)
+torch.cuda.synchronize()
+h = hits[:int(nh_t.item())].cpu().numpy()
+gn, gops, _ = mt.FuseReplay(F, rg, kf_mp, pts, h[h[:, 0] == 0][:, 1:], cap, world, lo, hi, np.zeros(len(k), np.uint8), np.zeros(len(k), bool), d, m,
+                            th=2.5, variant=2, Scw=api.inv_rigid(rg.M_t))
+assert int(st_t.item()) == 0 and gn == fn and np.array_equal(gops, fops) and len(fops) > 0
+assert np.array_equal(h[h[:, 0] == 0][:, 1:], h[h[:, 0] == 1][:, 1:])
+print("sanitize_small ok", len(k), n, nh, len(fops))
