@@ -110,14 +110,14 @@ __device__ __forceinline__ unsigned hamming_words(const uint32_t (&qw)[WORDS], c
 // row's words permuted so that a lane's words of all half chunks are adjacent (one 32/64/128-bit load, the warp reads one
 // contiguous block: no bank conflicts).  b & m2 is formed in registers.
 // Epilogue: 3 integer instructions per pair (value, compare); one warp vote skips the rest when no lane has a pair below its
-// threshold.  Each lane keeps a partial K-best list for each of its 4 query rows over the 2 of every 8 columns it sees
-// (visited in increasing index order, so `<` keeps the earlier index on equal distance); the 4 lanes of a quad merge their lists
-// at the end.  Keys are unique (the index is part of the key), so the merge is exact.  Pairs below the threshold are appended to
-// the lane's candidate buffer and folded into the lists in batches, so that the warp runs as many insertions as its busiest lane
-// needs rather than one per (row, column) slot in which any lane has a candidate; the threshold is the tighter of the lane's own
-// K-th distance and the best K-th distance of its quad.  H100 80GB HBM3, 700 W limit, bench.py config 2, the greedy matcher's
-// list kernel (tools/m2_split.py): 3.92 ms with one insertion per slot and no quad bound, 3.90 / 3.63 ms with the quad bound
-// refreshed every 8 / 32 column steps, 1.76 ms with the candidate buffer (quad bound refreshed at each fold); 0.75-0.77 ms when
+// threshold.  The 4 lanes of a quad see the same 4 query rows over disjoint columns (2 of every 8), and together hold one sorted
+// K-best list per row, KT / 4 keys per lane (lane t positions t KT/4 ..).  A pair is a candidate iff its key is below the row's
+// K-th key kK (every lane of the quad knows it; for the columns still to come this is distance < dK, see bmma_klists); keys are
+// unique (the index is part of the key), so this is exact, and ties keep the earlier index.  Candidates are appended to the
+// lane's buffer in shared memory and folded in batches: per row, each lane sorts its buffer, a quad butterfly keeps the KT
+// smallest of the four, and they are merged with the list -- a fixed network per row, whatever the busiest lane buffered.  H100 80GB HBM3, 700 W limit, bench.py
+// config 2, the greedy matcher's list kernel (tools/m2_split.py): 3.92 ms with one insertion per slot into per-lane lists, 1.76 ms
+// with per-lane lists, the candidate buffer and a bound shared by the quad, 1.23-1.24 ms with one list per row; 0.65 ms when
 // nothing is listed (th_low = 0).
 // Keys are 32 bits: distance << SHIFT | index (SHIFT 16 for the stream matcher's slots, kTopkShift for the key-frame database).
 constexpr int kTopkShift = 21;
@@ -137,6 +137,27 @@ struct BmmaTile {                            // one staged database tile, rows p
     unsigned cd[kDbTile];                    // popc(b & m2) (masked) / popc(b), kColOff for a column that is not listed
     unsigned cand[kTopkThreads / 32][4][kCandDepth][32];    // [warp][row r][entry][lane]: the lanes' candidate buffers
 };
+
+__device__ __forceinline__ void cmp_swap(unsigned& a, unsigned& b) { const unsigned lo = min(a, b); b = max(a, b); a = lo; }
+// ascending sort of 8 keys, 19 compare-exchanges (Knuth, TAOCP 5.3.4)
+__device__ __forceinline__ void sort8(unsigned (&x)[8]) {
+    constexpr int kNet[19][2] = {{0, 2}, {1, 3}, {4, 6}, {5, 7}, {0, 4}, {1, 5}, {2, 6}, {3, 7}, {0, 1}, {2, 3},
+                                 {4, 5}, {6, 7}, {2, 4}, {3, 5}, {1, 4}, {3, 6}, {1, 2}, {3, 4}, {5, 6}};
+#pragma unroll
+    for (int i = 0; i < 19; ++i) cmp_swap(x[kNet[i][0]], x[kNet[i][1]]);
+}
+// x[0, N) <- the N smallest of x[0, N) and y[0, N), both ascending, in ascending order: min(x[i], y[N-1-i]) is a bitonic sequence
+// holding them, then a bitonic merge sorts it
+template <int N>
+__device__ __forceinline__ void merge_lowest(unsigned (&x)[8], const unsigned (&y)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) x[i] = min(x[i], y[N - 1 - i]);
+#pragma unroll
+    for (int j = N / 2; j > 0; j /= 2)
+#pragma unroll
+        for (int i = 0; i < N; ++i)
+            if (!(i & j)) cmp_swap(x[i], x[i + j]);
+}
 
 __device__ __forceinline__ void bmma_and_popc(int (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
     asm("mma.sync.aligned.m16n8k256.row.col.s32.b1.b1.s32.and.popc {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -183,7 +204,7 @@ __device__ __forceinline__ void bmma_stage(BmmaTile<WORDS, MASKED>& s, const uin
 
 // The K-best lists of the CTA's 128 queries (rows 0 .. nq_cta - 1 of q / qm; rows beyond are not listed) against database entries
 // [j0, j1) of d / dm that skip does not exclude, listing only distances below worst0.  Every thread of the CTA must call this.
-// emit(row, k, key) receives, from lane t == 0 of each quad, key k < KT of the CTA row (kNone past the list's end).
+// emit(row, k, key) receives, from the lane of the quad that holds it, key k < KT of the CTA row (kNone past the list's end).
 template <int WORDS, bool MASKED, int KT, int SHIFT, class Emit>
 __device__ __forceinline__ void bmma_klists(const uint32_t* __restrict__ q, const uint32_t* __restrict__ qm, const int nq_cta,
                                             const uint32_t* __restrict__ d, const uint32_t* __restrict__ dm, const uint8_t* __restrict__ skip,
@@ -217,39 +238,51 @@ __device__ __forceinline__ void bmma_klists(const uint32_t* __restrict__ q, cons
         cq[r] = c;
         thr[r] = act ? (MASKED ? 2 * worst0 : worst0) : 0u;
     }
-    unsigned best[4][KT];
+    constexpr int P = KT / 4;                                      // list positions per lane
+    static_assert(KT % 4 == 0 && KT <= 8 && kCandDepth <= 7, "a fold sorts one lane's buffer in 8 registers");
+    unsigned list[4][P];                                           // row r: positions t P .. t P + P - 1 of its list
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
-        for (int k = 0; k < KT; ++k) best[r][k] = kNone;
+        for (int p = 0; p < P; ++p) list[r][p] = kNone;
     unsigned* cand = &s.cand[warp][0][0][lane];                    // row r, entry i at cand[(r * kCandDepth + i) * 32]
     int cnt[4] = {0, 0, 0, 0};
-    // Fold the buffered candidates into the lists (the whole warp, every lane its own), then tighten each row's threshold to
-    //   own:  value < 2 dK (masked) / dK -- strict, dK this lane's K-th distance: within a lane columns arrive in index order, so a
-    //         later column at distance dK cannot displace an entry;
-    //   quad: value < 2 dq + 2 / dq + 1 -- inclusive, dq the smallest K-th distance of the quad's full lists (the 4 lanes list the
-    //         same rows over disjoint columns): a pair farther than dq has K smaller keys in that lane's list; one at dq is kept,
-    //         since across lanes the index order of the columns is not the order in which they are visited.
-    // The quad bound changes only when a list changes, i.e. here.
+    // Fold the quad's buffered keys of each row into its list: every lane sorts its own, two butterfly rounds leave the KT smallest
+    // of the quad's in every lane, and merging them with the list gives the new list in every lane; lane t keeps its positions.
+    // A pair is a candidate iff its key is below the row's K-th key kK.  Every column visited after a fold has a larger index than
+    // every column before it, kK's included, so for those columns key < kK is distance < dK, dK the distance of kK: the threshold
+    // on the value is exact and strict.  The list only improves, so a pair that was not buffered has K smaller keys in the list.
     auto fold = [&]() {
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
-            for (int i = 0; i < cnt[r]; ++i) {
-                unsigned key = cand[(r * kCandDepth + i) * 32];
+            if (!__any_sync(0xffffffffu, cnt[r] > 0)) continue;
+            unsigned x[8];
 #pragma unroll
-                for (int k = 0; k < KT; ++k) {
-                    if (k < K) { const unsigned lo = min(key, best[r][k]); key = max(key, best[r][k]); best[r][k] = lo; }
-                }
-            }
+            for (int i = 0; i < 8; ++i) x[i] = i < cnt[r] ? cand[(r * kCandDepth + i) * 32] : kNone;
             cnt[r] = 0;
-            unsigned w = best[r][0];
+            sort8(x);
 #pragma unroll
-            for (int k = 1; k < KT; ++k) if (k < K) w = best[r][k];
-            const unsigned own = w == kNone ? kNone : (MASKED ? 2 * (w >> SHIFT) : w >> SHIFT);
-            unsigned quad = w == kNone ? kNone : own + (MASKED ? 2 : 1);
-            quad = min(quad, __shfl_xor_sync(0xffffffffu, quad, 1));
-            quad = min(quad, __shfl_xor_sync(0xffffffffu, quad, 2));
-            thr[r] = min(thr[r], min(own, quad));
+            for (int m = 1; m <= 2; m <<= 1) {
+                unsigned y[KT];
+#pragma unroll
+                for (int i = 0; i < KT; ++i) y[i] = __shfl_xor_sync(0xffffffffu, x[i], m);
+                merge_lowest<KT>(x, y);
+            }
+            unsigned y[KT];
+#pragma unroll
+            for (int k = 0; k < KT; ++k) y[k] = __shfl_sync(0xffffffffu, list[r][k % P], (lane & ~3) | (k / P));
+            merge_lowest<KT>(x, y);
+#pragma unroll
+            for (int p = 0; p < P; ++p) {
+                unsigned v = x[p];
+#pragma unroll
+                for (int u = 1; u < 4; ++u) if (t == u) v = x[u * P + p];
+                list[r][p] = v;
+            }
+            unsigned w = x[0];
+#pragma unroll
+            for (int k = 1; k < KT; ++k) if (k < K) w = x[k];
+            if (w != kNone) thr[r] = min(thr[r], (w >> SHIFT) * (MASKED ? 2 : 1));
         }
     };
 
@@ -324,24 +357,13 @@ __device__ __forceinline__ void bmma_klists(const uint32_t* __restrict__ q, cons
         }
     }
     fold();
-    // quad merge: K rounds of "smallest head of the four lists", popped by the lane that holds it
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
         const int row = warp * 32 + (r >> 1) * 16 + (r & 1) * 8 + g;
 #pragma unroll
-        for (int k = 0; k < KT; ++k) {
-            unsigned m = kNone;
-            if (k < K) {
-                const unsigned h = best[r][0];
-                m = min(h, __shfl_xor_sync(0xffffffffu, h, 1));
-                m = min(m, __shfl_xor_sync(0xffffffffu, m, 2));
-                if (h == m) {
-#pragma unroll
-                    for (int j = 0; j + 1 < KT; ++j) best[r][j] = best[r][j + 1];
-                    best[r][KT - 1] = kNone;
-                }
-            }
-            if (t == 0) emit(row, k, m);
+        for (int p = 0; p < P; ++p) {
+            const int k = t * P + p;
+            emit(row, k, k < K ? list[r][p] : kNone);
         }
     }
 }
