@@ -5,6 +5,8 @@ contiguous conversion.  Integer work: bit-exact."""
 import numpy as np
 import pytest
 
+import acceptance_model as am
+
 pytestmark = pytest.mark.gpu
 
 FILL = 12345            # frame_mp value of the slots beyond a camera's count: must come back untouched
@@ -215,25 +217,6 @@ def _flip(rng, d, nbits):
     return out
 
 
-def _rounds_needed(dist, n_queries, taken0):
-    """rounds of the fixpoint iteration for n_queries identical queries over candidates with distinct distances `dist`"""
-    order = np.argsort(dist, kind="stable")
-    prev, r = None, 0
-    while True:
-        owner = {}
-        if prev is not None:
-            for q, d in enumerate(prev):
-                if d >= 0 and d not in owner:
-                    owner[d] = q
-        cur = []
-        for q in range(n_queries):
-            free = [k for k in order if not taken0[k] and not (k in owner and owner[k] < q)]
-            cur.append(free[0] if free else -1)
-        if prev is not None and cur == prev:
-            return r, cur
-        prev, r = cur, r + 1
-
-
 def test_long_dependency_chains_run_the_walk(api, oa):
     """Many map points share one window whose keypoints lie at strictly increasing distance with alternating octaves: every
     acceptance moves every later query to the next keypoint, so the chain is deeper than the round cap and the sequential walk
@@ -275,16 +258,16 @@ def test_long_dependency_chains_run_the_walk(api, oa):
     m = api.cORBmatcher(0.8, False, dim, False)
     pre = np.full(len(F.keys), -1, np.int32)
     pre[:nk][taken0] = 7
-    rounds, seq = _rounds_needed(dist, nmp, taken0)
-    cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
-    assert rounds > cap_rounds and all(s >= 0 for s in seq)
     n, fmp = m.SearchByProjection(F, mps, 3.0, pre.copy())
     on, ofmp = oa.search_by_projection(F, mps, 3.0, 0.8, m.TH_HIGH_, False, pre.copy())
     assert n == on and np.array_equal(fmp, ofmp) and n >= nmp
+    pn, pfmp, pdiag, _ = am.predict_local(api, oa, m, F, mps, 3.0, pre.copy())
+    cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
+    assert pn == n and np.array_equal(pfmp, fmp) and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts"):
         gn, gfmp, status, diag = _device_search(api, m, _per_cam(F), _sizes(F), sf, mps, 3.0, pre=pre.copy(), layout=layout)
         assert status == api.MCS_OK and gn == n and np.array_equal(gfmp, fmp)
-        assert diag[0] == cap_rounds and diag[1] >= 0 and diag[3] > 0      # the rounds hit the cap, the walk ran, windows were rescanned
+        assert diag.tolist() == pdiag          # rounds run, walk start, queries and rescans as the model of the rounds and walk has them
 
 
 def test_out_of_range_levels_are_flagged_and_skipped(api, oa, cams):

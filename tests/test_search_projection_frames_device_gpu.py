@@ -6,6 +6,7 @@ work: bit-exact."""
 import numpy as np
 import pytest
 
+import acceptance_model as am
 import test_ref_match_cpu as T
 from test_search_projection_device_gpu import FILL
 from test_search_projection_last_device_gpu import BIG_ID, _pack, _parity_scene
@@ -197,11 +198,15 @@ def test_long_dependency_chain_runs_the_walk(api, oa):
     hn, hout = m.SearchByProjectionFramesRig(Fl, mp_last, Fc, rig, free, world, bad, 40)
     on, oout = m.SearchByProjectionFramesRig(Fl, mp_last, Fc, rig, free, world, bad, 40, _sw=oa.search_windows)
     assert hn == on and np.array_equal(hout, oout) and hn == len(CHAIN_DISTS)
+    rec = am.Capture(oa)
+    m.SearchByProjectionFramesRig(Fl, mp_last, Fc, rig, free, world, bad, 40, _sw=rec)
+    pn, _, pdiag, _ = am.predict_windows(api, oa, rec.calls[0])
     cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
+    assert pn == hn and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts", "shared"):
         gn, gout, status, diag = _device_frames(api, m, Fc, Fl, rig, free, mp_last, world, bad, 40, layout=layout)
         assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
-        assert diag[0] == cap_rounds and diag[1] >= 0 and diag[3] > 0      # the rounds hit the cap, the walk ran, windows were rescanned
+        assert diag.tolist() == pdiag          # rounds run, walk start, queries and rescans as the model of the rounds and walk has them
 
 
 def test_invalid_ids(api, oa, frames, cams):

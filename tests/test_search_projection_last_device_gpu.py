@@ -6,6 +6,7 @@ Results are compared after the slot -> contiguous conversion.  Integer work: bit
 import numpy as np
 import pytest
 
+import acceptance_model as am
 import test_ref_match_cpu as T
 from test_search_projection_device_gpu import FILL, _flip, _per_cam
 
@@ -236,11 +237,15 @@ def test_long_dependency_chain_runs_the_walk(api, oa):
     on, oout = m.SearchByProjectionLastRig(Fc, rig, mp_cur, Fl, mp_last, None, world, bad, 50.0, _sw=oa.search_windows)
     assert hn == on and np.array_equal(hout, oout)
     assert (hout[:30] >= 0).sum() == 22                          # 20 acceptances along the chain + the 2 taken on entry
+    rec = am.Capture(oa)
+    m.SearchByProjectionLastRig(Fc, rig, mp_cur, Fl, mp_last, None, world, bad, 50.0, _sw=rec)
+    pn, _, pdiag, _ = am.predict_windows(api, oa, rec.calls[0])
     cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
+    assert pn == hn and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts", "shared"):
         gn, gout, status, diag = _device_last(api, m, Fc, Fl, rig, mp_cur, mp_last, None, world, bad, 50.0, layout=layout)
         assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
-        assert diag[0] == cap_rounds and diag[1] >= 0 and diag[3] > 0      # the rounds hit the cap, the walk ran, windows were rescanned
+        assert diag.tolist() == pdiag          # rounds run, walk start, queries and rescans as the model of the rounds and walk has them
 
 
 def test_invalid_ids_and_octaves_drop_only_their_query(api, oa, frames, cams):

@@ -6,6 +6,7 @@ bit-exact."""
 import numpy as np
 import pytest
 
+import acceptance_model as am
 import test_ref_match_cpu as T
 from test_search_projection_device_gpu import FILL, _flip
 from test_search_projection_last_device_gpu import BIG_ID, _pack, _parity_scene
@@ -176,12 +177,15 @@ def test_long_dependency_chain_runs_the_walk(api, oa):
     hn, hout = host_window_search(m, Fl, Fc, mp_last, bad, 50, 0, INT_MAX)
     on, oout = host_window_search(m, Fl, Fc, mp_last, bad, 50, 0, INT_MAX, sw=oa.search_windows)
     assert hn == on and np.array_equal(hout, oout) and hn == len(CHAIN_DISTS)
+    rec = am.Capture(oa)
+    host_window_search(m, Fl, Fc, mp_last, bad, 50, 0, INT_MAX, sw=rec)
+    pn, _, pdiag, _ = am.predict_windows(api, oa, rec.calls[0])
     cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
-    assert len(CHAIN_DISTS) > cap_rounds
+    assert len(CHAIN_DISTS) > cap_rounds and pn == hn and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts", "shared"):
         gn, gout, status, diag = _device_ws(api, m, Fc, Fl, mp_last, bad, 50, layout=layout)
         assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
-        assert diag[0] == cap_rounds and diag[1] >= 0 and diag[3] > 0      # the rounds hit the cap, the walk ran, windows were rescanned
+        assert diag.tolist() == pdiag          # rounds run, walk start, queries and rescans as the model of the rounds and walk has them
 
 
 def test_invalid_ids_drop_only_their_query(api, oa, frames, cams):

@@ -7,7 +7,9 @@ import re
 import numpy as np
 import pytest
 
-from test_search_projection_device_gpu import _device_search, _per_cam, _rounds_needed, _sizes
+import acceptance_model as am
+
+from test_search_projection_device_gpu import _device_search, _per_cam, _sizes
 from test_window_edges_cpu import EMPTY_CAM, SF, edge_scene, flip, projection_scene, second_frame
 
 pytestmark = pytest.mark.gpu
@@ -385,16 +387,16 @@ def test_device_long_dependency_chain(api, oa, dim):
     mps = api.MapPoints(np.zeros(nall, np.uint8), in_view, level, px, py, vc, desc, None)
     pre = np.full(len(F.keys), -1, np.int32)
     pre[:nk][taken0] = 7
-    rounds, seq = _rounds_needed(dist, nmp, taken0)
-    cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
-    assert rounds > cap_rounds and all(s >= 0 for s in seq)
     n, fmp = m.SearchByProjection(F, mps, 3.0, pre.copy())
     on, ofmp = oa.search_by_projection(F, mps, 3.0, 0.8, m.TH_HIGH_, False, pre.copy())
     assert n == on and np.array_equal(fmp, ofmp) and n >= nmp
+    pn, pfmp, pdiag, _ = am.predict_local(api, oa, m, F, mps, 3.0, pre.copy())
+    cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
+    assert pn == n and np.array_equal(pfmp, fmp) and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts"):
         gn, gfmp, status, diag = _device_search(api, m, _per_cam(F), _sizes(F), SF, mps, 3.0, pre=pre.copy(), layout=layout)
         assert status == api.MCS_OK and gn == n and np.array_equal(gfmp, fmp)
-        assert diag[0] == cap_rounds and diag[1] >= 0 and diag[3] > 0
+        assert diag.tolist() == pdiag
 
 
 @width
