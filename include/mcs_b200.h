@@ -629,6 +629,61 @@ int  mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, i
                      const uint8_t* desc_dev, const uint8_t* dmask_dev, const uint8_t* bad_dev, double th, int32_t th_low,
                      int32_t having_masks, int32_t* hits_dev, int32_t max_hits, int32_t* n_hits_dev, int32_t* status_dev, void* stream);
 
+/* Loop closing's two Sim3 searches (cLoopClosing::ComputeSim3, ref src/cLoopClosing.cpp:343 and :401) with the key frames in packed
+ * feature buffers.  Conventions of mcs_search_by_projection_last_device: asynchronous on `stream` (NULL synchronises), host
+ * validation before any launch, nothing read back, stream-ordered scratch; frames in either packed layout, possibly one buffer;
+ * map-point rows slot-indexed (c * capacity + j), slots at or beyond a camera's count neither read nor written.  cams [n_cams] host
+ * camera models (one image size for all, MCS_ERR_UNSUPPORTED otherwise), masks_dev [n_cams][height][width] their mirror masks,
+ * scale_factors [n_levels] host.  The map points: world_pos_dev [n_points * 3], min_dist_dev / max_dist_dev [n_points]
+ * (GetMin/MaxDistanceInvariance), desc_dev / dmask_dev [n_points * dim] (dmask_dev read only when having_masks), bad_dev
+ * [n_points] (may be NULL).  capacity <= 65535; n_cams * capacity < 2^24 (MCS_ERR_UNSUPPORTED beyond).
+ *
+ * mcs_search_by_sim3_device: SearchBySim3(pKF1, pKF2, vpMatches12, s12, R12, t12, th) (ref src/cORBmatcher.cpp:1721-1988).
+ *   kf1 / kf2 may be the same frame.  t1w / t2w host row-major 4x4, each key frame's GetPoseInverse(); mc_inv [n_cams * 16] host,
+ *   invMat(Get_M_c(c)) of the rig both key frames share; r12 [9] row-major, t12 [3], s12 != 0 (MCS_ERR_INVALID otherwise).  The
+ *   launcher forms sR12 = s12 * R12, sR21 = (1 / s12) * R12^T and t21 = -sR21 * t12 in cv::Matx order.
+ *   Direction 1: every KF1 slot in slot order whose id in mp1_dev exists, whose matches12_dev entry is -1 on entry (vbAlreadyMatched1)
+ *   and whose point is not bad: p3Dc1 = R1w * X + t1w, p3Dc2 = sR21 * p3Dc1 + t21, p4 = mc_inv[c] * (p3Dc2, 1) with c the keypoint's
+ *   camera; dropped when p3Dc2.z < 0 (the rig frame's z, not the camera's), when WorldToImg(p4) lies outside camera c's mirror mask,
+ *   or when |p4.xyz| (a double) lies outside [min, max]; else level l = lower_bound over the scale factors, clamped, and the best
+ *   candidate (strict < over the visiting order, nothing skipped) of GetFeaturesInArea(c, u, v, th * scale_factors[l]) of KF2 on
+ *   levels {l - 1, l} counts when its distance is <= th_high.  Direction 2 is the mirror image, KF2 into KF1 with sR12 and t12,
+ *   already2_dev (KF2 slot-indexed bytes, may be NULL: vbAlreadyMatched2, which the caller builds from GetIndexInKeyFrame(pKF2)[0])
+ *   as its skip list.  matches12_dev (KF1 slot-indexed map-point ids, in/out): matches12[s1] = mp2[s2] where direction 1 found s2
+ *   for s1 and direction 2 found s1 for s2.  nfound_dev [1]: those agreements.  status_dev: MCS_ERR_INVALID when an id in mp1_dev,
+ *   mp2_dev or matches12_dev is >= n_points (that slot is dropped, the others are unaffected), MCS_OK otherwise.
+ *
+ * mcs_search_by_projection_scw_device: SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) (ref :2265-2392) as written there.
+ *   mtmc_inv [n_cams * 16] host and ow [3] host: the rigid part of Scw (MtMc_inv and centre of the rig posed by
+ *   invMat(Rt2Hom(Rcw, tcw)), as mcs_fuse_target for MCS_FUSE_SIM3).  points_dev [n_q] map-point ids, -1 = NULL (may be NULL when
+ *   n_q is 0).  matched_dev: vpMatched, slot-indexed map-point ids, in/out; the points it holds on entry are spAlreadyFound for the
+ *   whole call, its slots holding an id are taken.  Entry i of points_dev in order, unless NULL, bad or already found: projected
+ *   (WorldToCamHom_fast, mirror mask) into the camera of CONTIGUOUS KEYPOINT i of the key frame (keypoint_to_cam.find(iMP), :2307),
+ *   its double distance to ow tested against [min, max], its level l predicted, and GetFeaturesInArea(cam, u, v, th *
+ *   scale_factors[l]) searched on levels {l - 1, l} without the taken keypoints.  Candidate j of camera c is compared through row
+ *   first(c) + j of camera c's descriptors (the reference indexes the camera's matrix with the contiguous id, :2367, :2372), and
+ *   dropped when that row is at or beyond camera c's count (the reference reads past the matrix there).  The best is accepted when
+ *   best <= th_low and it is not contiguous keypoint 0 (`bestIdx > 0`, :2385: the first slot of the first camera with keypoints),
+ *   greedily in entry order: matched_dev receives the point.  nmatches_dev [1]: the acceptances of this call (the reference's
+ *   return value; ComputeSim3's nTotalMatches counts every slot of matched_dev that holds a point).  status_dev: MCS_ERR_INVALID
+ *   when an id is >= n_points, or when an entry that reaches the camera look-up lies at or beyond the key frame's keypoint count
+ *   (the reference dereferences unordered_map::end() there: undefined); such an entry is dropped, the others are unaffected.
+ *   diag_dev (may be NULL): int32[4] as for mcs_search_by_projection_device.  n_q < 2^24 (MCS_ERR_UNSUPPORTED beyond). */
+int  mcs_search_by_sim3_device(const mcs_packed_frame* kf1, const mcs_packed_frame* kf2, int32_t n_cams, int32_t capacity, int32_t dim,
+                               const mcs_ocam* cams, const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, const double* t1w,
+                               const double* t2w, const double* mc_inv, double s12, const double* r12, const double* t12, double th,
+                               const int32_t* mp1_dev, const int32_t* mp2_dev, int32_t n_points, const double* world_pos_dev,
+                               const double* min_dist_dev, const double* max_dist_dev, const uint8_t* desc_dev, const uint8_t* dmask_dev,
+                               const uint8_t* bad_dev, const uint8_t* already2_dev, int32_t th_high, int32_t having_masks,
+                               int32_t* matches12_dev, int32_t* nfound_dev, int32_t* status_dev, void* stream);
+int  mcs_search_by_projection_scw_device(const mcs_packed_frame* kf, int32_t n_cams, int32_t capacity, int32_t dim, const mcs_ocam* cams,
+                                         const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, const double* mtmc_inv,
+                                         const double* ow, const int32_t* points_dev, int32_t n_q, int32_t n_points,
+                                         const double* world_pos_dev, const double* min_dist_dev, const double* max_dist_dev,
+                                         const uint8_t* desc_dev, const uint8_t* dmask_dev, const uint8_t* bad_dev, int32_t th, int32_t th_low,
+                                         int32_t having_masks, int32_t* matched_dev, int32_t* nmatches_dev, int32_t* status_dev,
+                                         int32_t* diag_dev, void* stream);
+
 /* ---- bag of words: ORBVocabulary::transform and the feature-vector guided search (SURVEY 8f, rank 4) ------- */
 /* The vocabulary tree of DBoW2::TemplatedVocabulary<FORB::TDescriptor, FORB> (ref include/cORBVocabulary.h:34,
  * ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h) as flat arrays.  Node 0 is the root; parent[0] is ignored.

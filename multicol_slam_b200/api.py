@@ -1222,6 +1222,44 @@ class cORBmatcher:
                 found += 1
         return found, m12
 
+    def SearchBySim3Device(self, kf1, kf2, capacity, rig1, rig2, masks_t, scale_factors, mp1_t, mp2_t, world_t, min_dist_t, max_dist_t,
+                           desc_t, dmask_t, s12, R12, t12, th, matches12_t, already2_t=None, bad_t=None, stream=None, out=None):
+        """mcs_search_by_sim3_device: SearchBySim3 (ref :1721-1988) with both key frames in packed feature buffers (see
+        include/mcs_b200.h).  kf1 / kf2: (packed uint8 cuda tensor, n_parts, part_images, first_image); rig1 / rig2: Rigs at the key
+        frames' poses (GetPoseInverse is inv_rigid(M_t); the camera offsets and models are rig2's, the rig both share).  mp1_t / mp2_t
+        int32 cuda [n_cams * capacity] map-point ids by slot; matches12_t likewise for KF1, updated in place (-1 = not matched yet);
+        already2_t u8 cuda by KF2 slot or None.  The map points as cuda tensors, as for FuseDevice.  Asynchronous on `stream`.
+        Returns (nfound [1], status [1], matches12_t) as cuda tensors."""
+        out, tail = _search_outputs(out, False, stream, mp1_t.device)
+        sf = np.ascontiguousarray(scale_factors, np.float64)
+        t1w, t2w = inv_rigid(rig1.M_t), inv_rigid(rig2.M_t)
+        mc_inv = np.ascontiguousarray(np.stack([inv_rigid(m) for m in rig2.M_c]), np.float64)
+        r12, v12 = np.ascontiguousarray(R12, np.float64), np.ascontiguousarray(t12, np.float64)
+        _check(lib().mcs_search_by_sim3_device(*_packed_pair(kf1, kf2), len(rig2.cams), capacity, int(desc_t.shape[1]), _ocams(rig2.cams),
+                                               _dptr(masks_t), len(sf), _p(sf), _p(t1w), _p(t2w), _p(mc_inv), float(s12), _p(r12), _p(v12),
+                                               float(th), _dptr(mp1_t), _dptr(mp2_t), int(world_t.shape[0]), _dptr(world_t), _dptr(min_dist_t),
+                                               _dptr(max_dist_t), _dptr(desc_t), _dptr(dmask_t), _dptr(bad_t), _dptr(already2_t), self.TH_HIGH_,
+                                               int(self.havingMasks), _dptr(matches12_t), tail[0], tail[1], tail[3]))
+        return out[0], out[1], matches12_t
+
+    def SearchByProjectionKFScwDevice(self, kf, capacity, rig, Scw, masks_t, scale_factors, points_t, world_t, min_dist_t, max_dist_t,
+                                      desc_t, dmask_t, th, matched_t, bad_t=None, stream=None, out=None, diag=False):
+        """mcs_search_by_projection_scw_device: SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) (ref :2265-2392) with the key
+        frame in packed feature buffers, quirks included (see include/mcs_b200.h).  kf: (packed uint8 cuda tensor, n_parts,
+        part_images, first_image); rig: the key frame's Rig, whose pose Scw's rigid part replaces (_sim3_rig).  points_t int32 cuda
+        [n_q] map-point ids (-1 = NULL); matched_t int32 cuda [n_cams * capacity], vpMatched by slot, updated in place.  Asynchronous
+        on `stream`.  Returns (nmatches [1], status [1], matched_t), plus diag [4] when diag is set, as cuda tensors."""
+        out, tail = _search_outputs(out, diag, stream, matched_t.device)
+        sf = np.ascontiguousarray(scale_factors, np.float64)
+        r = _sim3_rig(rig, Scw)
+        mi, ow = np.ascontiguousarray(r.MtMc_inv, np.float64), np.ascontiguousarray(r.M_t[:3, 3], np.float64)
+        _check(lib().mcs_search_by_projection_scw_device(C.byref(PackedFrame(kf[0].data_ptr(), *kf[1:4])), len(rig.cams), capacity,
+                                                         int(desc_t.shape[1]), _ocams(rig.cams), _dptr(masks_t), len(sf), _p(sf), _p(mi), _p(ow),
+                                                         _dptr(points_t), int(points_t.shape[0]), int(world_t.shape[0]), _dptr(world_t),
+                                                         _dptr(min_dist_t), _dptr(max_dist_t), _dptr(desc_t), _dptr(dmask_t), _dptr(bad_t),
+                                                         int(th), self.TH_LOW_, int(self.havingMasks), _dptr(matched_t), *tail))
+        return _search_result(out, matched_t, diag)
+
     def SearchForTriangulationBetweenCameras(self, KF, rig, kf_mp, rays, cam1, cam2, _sw=None):
         """SearchForTriangulationBetweenCameras(pKF1, cam1, cam2, ...) (ref :1158-1263): every keypoint of camera cam1 without a
         map point is carried along its bearing ray into camera cam2 of the same rig (relative orientation of the two cameras),

@@ -124,7 +124,9 @@ struct WindowFrameDev {
     const double* winv; const double* hinv;                 // [n_cams]
     // MCS_RULE_SCW only: [n_cams + 1] first contiguous keypoint id of every camera.  When set, candidate `id` of a query of
     // camera c is compared through descriptor row cam_first[c] + id -- the reference indexes camera c's matrix with the
-    // contiguous id (src/cORBmatcher.cpp:2367,2372) -- and dropped when that row lies beyond the camera's own rows.
+    // contiguous id (src/cORBmatcher.cpp:2367,2372) -- and dropped when that row lies beyond the camera's own rows.  The device
+    // search (launch_search_by_projection_scw) reads those rows in its frame view already and uses cam_first only to find
+    // contiguous keypoint 0.
     const int* cam_first = nullptr;
 };
 cudaError_t launch_window_search(const WindowFrameDev& f, const mcs_window_query* q, int nq, const uint8_t* qdesc,
@@ -213,6 +215,34 @@ struct FuseDevArgs : PsFrameArgs {
     int* hits; int max_hits; int* n_hits;                    // device [max_hits * 3], [1]
 };
 cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st);
+// SearchBySim3(KF1, KF2, .) (mcs_search_by_sim3_device): PsFrameArgs is KF2 (cams) with th_high = TH_HIGH_; nmatches is nFound;
+// frame_mp and diag are unused.
+struct Sim3SearchDevArgs : PsFrameArgs {
+    const PsCamSlots* kf1;                                   // host [n_cams]
+    const mcs_ocam* models; const uint8_t* masks;            // host [n_cams], device [n_cams][h][w]
+    const double* xf;                                        // host [48]: per direction R[9] t[3] sR[9] st[3] (direction 1, then 2)
+    const double* mc_inv;                                    // host [n_cams * 16]: invMat(Get_M_c(c))
+    double th;
+    int n_points;
+    const int* mp1; const int* mp2;                          // device, slot-indexed
+    const double* world_pos; const double* min_dist; const double* max_dist;
+    const uint8_t* desc; const uint8_t* dmask; const uint8_t* bad;
+    const uint8_t* already2;                                 // device, KF2 slot-indexed, may be NULL
+    int* matches12;                                          // device, KF1 slot-indexed, in/out
+};
+cudaError_t launch_search_by_sim3(const Sim3SearchDevArgs& a, cudaStream_t st);
+// SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) (mcs_search_by_projection_scw_device): PsFrameArgs is the key frame with
+// th_high = TH_LOW_ and frame_mp = vpMatched (slot-indexed, in/out).
+struct ScwSearchDevArgs : PsFrameArgs {
+    const mcs_ocam* models; const uint8_t* masks;            // host [n_cams], device [n_cams][h][w]
+    const double* mtmc_inv; const double* ow;                // host [n_cams * 16], [3]: the Sim3's rigid pose
+    int n_q, n_points;
+    const int* points;                                       // device [n_q], -1 = NULL
+    const double* world_pos; const double* min_dist; const double* max_dist;
+    const uint8_t* desc; const uint8_t* dmask; const uint8_t* bad;
+    int th;
+};
+cudaError_t launch_search_by_projection_scw(const ScwSearchDevArgs& a, cudaStream_t st);
 
 // ---- bag of words (bow_kernels.cu) ----
 // vocabulary tree on the device: CSR children in the reference's order, 32-byte node descriptors as uint4 pairs

@@ -832,6 +832,89 @@ int mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, in
     return sync_if_null_stream(stream);
 }
 
+int mcs_search_by_sim3_device(const mcs_packed_frame* kf1, const mcs_packed_frame* kf2, int32_t n_cams, int32_t capacity, int32_t dim,
+                              const mcs_ocam* cams, const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, const double* t1w,
+                              const double* t2w, const double* mc_inv, double s12, const double* r12, const double* t12, double th,
+                              const int32_t* mp1_dev, const int32_t* mp2_dev, int32_t n_points, const double* world_pos_dev,
+                              const double* min_dist_dev, const double* max_dist_dev, const uint8_t* desc_dev, const uint8_t* dmask_dev,
+                              const uint8_t* bad_dev, const uint8_t* already2_dev, int32_t th_high, int32_t having_masks,
+                              int32_t* matches12_dev, int32_t* nfound_dev, int32_t* status_dev, void* stream) {
+    if (!kf1 || !kf2 || !cams || !masks_dev || !scale_factors || !t1w || !t2w || !mc_inv || !r12 || !t12 || !mp1_dev || !mp2_dev ||
+        !world_pos_dev || !min_dist_dev || !max_dist_dev || !desc_dev || !matches12_dev || !nfound_dev || !status_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (having_masks && !dmask_dev) return mcs_fail(MCS_ERR_INVALID, "masks requested but not supplied");
+    if (n_levels < 1 || n_levels > MCS_MAX_LEVELS || n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (!(s12 != 0.0)) return mcs_fail(MCS_ERR_INVALID, "s12 must be non-zero");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, kf2, kf1)) return rc;
+    const CamSizes cz(cams, n_cams);
+    if (int rc = check_cam_sizes(n_cams, cz.w.data(), cz.h.data(), true)) return rc;
+    // one query per slot of the key frame carried over, in each direction
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
+    // sR12 = s12 * R12, sR21 = (1 / s12) * R12^T, t21 = -sR21 * t12 (ref :1741-1743), cv::Matx order: s = 0; s += a(i,k) * b(k) ...
+    double xf[48];
+    auto rig = [&](double* d, const double* T) {         // Hom2R / Hom2T of a row-major 4x4
+        for (int i = 0; i < 3; ++i) { for (int k = 0; k < 3; ++k) d[3 * i + k] = T[4 * i + k]; d[9 + i] = T[4 * i + 3]; }
+    };
+    rig(xf, t1w);
+    rig(xf + 24, t2w);
+    const double inv_s = 1.0 / s12;
+    for (int i = 0; i < 3; ++i)
+        for (int k = 0; k < 3; ++k) {
+            xf[12 + 3 * i + k] = inv_s * r12[3 * k + i];     // direction 1: sR21
+            xf[36 + 3 * i + k] = s12 * r12[3 * i + k];       // direction 2: sR12
+        }
+    for (int i = 0; i < 3; ++i) {
+        double acc = 0.0;
+        for (int k = 0; k < 3; ++k) acc += -xf[12 + 3 * i + k] * t12[k];
+        xf[21 + i] = acc;                                    // t21
+        xf[45 + i] = t12[i];
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const std::vector<PsCamSlots> s2 = packed_slots(*kf2, n_cams, capacity, dim), s1 = packed_slots(*kf1, n_cams, capacity, dim);
+    Sim3SearchDevArgs a{};
+    set_searched_frame(a, s2, capacity, dim, cz.w.data(), cz.h.data(), th_high, having_masks, nullptr, nfound_dev, status_dev, nullptr);
+    a.n_levels = n_levels; a.sf = scale_factors;
+    a.kf1 = s1.data(); a.models = cams; a.masks = masks_dev; a.xf = xf; a.mc_inv = mc_inv; a.th = th;
+    a.n_points = n_points; a.mp1 = mp1_dev; a.mp2 = mp2_dev;
+    a.world_pos = world_pos_dev; a.min_dist = min_dist_dev; a.max_dist = max_dist_dev;
+    a.desc = desc_dev; a.dmask = having_masks ? dmask_dev : nullptr; a.bad = bad_dev; a.already2 = already2_dev;
+    a.matches12 = matches12_dev;
+    CUDA_CHECK(launch_search_by_sim3(a, st));
+    return sync_if_null_stream(stream);
+}
+
+int mcs_search_by_projection_scw_device(const mcs_packed_frame* kf, int32_t n_cams, int32_t capacity, int32_t dim, const mcs_ocam* cams,
+                                        const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, const double* mtmc_inv,
+                                        const double* ow, const int32_t* points_dev, int32_t n_q, int32_t n_points,
+                                        const double* world_pos_dev, const double* min_dist_dev, const double* max_dist_dev,
+                                        const uint8_t* desc_dev, const uint8_t* dmask_dev, const uint8_t* bad_dev, int32_t th, int32_t th_low,
+                                        int32_t having_masks, int32_t* matched_dev, int32_t* nmatches_dev, int32_t* status_dev,
+                                        int32_t* diag_dev, void* stream) {
+    // points_dev may be NULL only when it has no entry (an empty tensor has no address)
+    if (!kf || !cams || !masks_dev || !scale_factors || !mtmc_inv || !ow || (!points_dev && n_q > 0) || !world_pos_dev || !min_dist_dev ||
+        !max_dist_dev || !desc_dev || !matched_dev || !nmatches_dev || !status_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (having_masks && !dmask_dev) return mcs_fail(MCS_ERR_INVALID, "masks requested but not supplied");
+    if (n_levels < 1 || n_levels > MCS_MAX_LEVELS || n_q < 0 || n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, kf, nullptr)) return rc;
+    const CamSizes cz(cams, n_cams);
+    if (int rc = check_cam_sizes(n_cams, cz.w.data(), cz.h.data(), true)) return rc;
+    // the front end's slot and query indices: one image per camera, one query per entry of vpPoints
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
+    if (int rc = check_query_bound(n_q, "n_q must stay below 2^24")) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    const std::vector<PsCamSlots> slots = packed_slots(*kf, n_cams, capacity, dim);
+    ScwSearchDevArgs a{};
+    set_searched_frame(a, slots, capacity, dim, cz.w.data(), cz.h.data(), th_low, having_masks, matched_dev, nmatches_dev, status_dev, diag_dev);
+    a.n_levels = n_levels; a.sf = scale_factors;
+    a.models = cams; a.masks = masks_dev; a.mtmc_inv = mtmc_inv; a.ow = ow;
+    a.n_q = n_q; a.n_points = n_points; a.points = points_dev;
+    a.world_pos = world_pos_dev; a.min_dist = min_dist_dev; a.max_dist = max_dist_dev;
+    a.desc = desc_dev; a.dmask = having_masks ? dmask_dev : nullptr; a.bad = bad_dev; a.th = th;
+    CUDA_CHECK(launch_search_by_projection_scw(a, st));
+    return sync_if_null_stream(stream);
+}
+
 int mcs_search_for_initialization(const mcs_frame_view* f1, const mcs_frame_view* f2, double* prev_matched, int32_t window_size,
                                   double nnratio, int32_t th_low, int32_t having_masks, int32_t* matches12, int32_t* nmatches) {
     if (!f1 || !f2 || !prev_matched || !matches12 || !nmatches) return mcs_fail(MCS_ERR_INVALID, "null argument");

@@ -471,16 +471,18 @@ __global__ void __launch_bounds__(256) ps_list_kernel(const WindowFrameDev f, co
 // accepted when its distance is <= th_high (:2070).  MCS_RULE_RATIO: best / second best free candidate, accepted when
 // best <= second * nnratio and best <= th_high (WindowSearch :405-416, SearchByProjection(F1, F2) :553-566), in the double form of
 // the host replay.  kRuleInit: best / second best candidate not skipped, accepted when best <= th_high and best < second * nnratio
-// (SearchForInitialization :662-677); its distance goes to *best_dist.  The list decides when it holds as many free entries as the
-// rule reads, or every candidate; otherwise the window is scanned again with the predicate.
+// (SearchForInitialization :662-677); its distance goes to *best_dist.  MCS_RULE_SCW: the best free candidate alone, accepted when
+// best <= th_high and it is not contiguous keypoint 0 (SearchByProjection(KF, Scw) :2385, `bestIdx > 0`): slot j = 0 of a camera
+// whose first contiguous id (f.cam_first) is 0.  The list decides when it holds as many free entries as the rule reads, or every
+// candidate; otherwise the window is scanned again with the predicate.
 constexpr int kRuleInit = 100;               // not a public rule: SearchForInitialization's acceptance exists on the device only
 template <int RULE, int WORDS, bool MASKED, class Taken>
 __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_window_query& qq, const unsigned* lk, const int* ls, const int cnt,
                                          const uint32_t* qdesc, const uint32_t* qmask, const Taken& taken, const int th_high,
                                          const double nnratio, int* rescans, int* best_dist = nullptr) {
-    static_assert(RULE == MCS_RULE_LEVEL_RATIO || RULE == MCS_RULE_BEST || RULE == MCS_RULE_RATIO || RULE == kRuleInit,
-                  "device acceptance rules");
-    constexpr int NB = RULE == MCS_RULE_BEST ? 1 : 2;       // free keys the rule reads
+    static_assert(RULE == MCS_RULE_LEVEL_RATIO || RULE == MCS_RULE_BEST || RULE == MCS_RULE_RATIO || RULE == kRuleInit ||
+                  RULE == MCS_RULE_SCW, "device acceptance rules");
+    constexpr int NB = RULE == MCS_RULE_BEST || RULE == MCS_RULE_SCW ? 1 : 2;       // free keys the rule reads
     const int lane = threadIdx.x & 31;
     unsigned k = kNoKey; int s = -1; bool fr = false;
     if (lane < kPsK) { k = lk[lane]; s = ls[lane]; fr = k != kNoKey && !is_taken(taken, s, k >> 16); }
@@ -503,6 +505,11 @@ __device__ __forceinline__ int ps_decide(const WindowFrameDev& f, const mcs_wind
     }
     if (s0 < 0) return -1;
     if constexpr (RULE == MCS_RULE_BEST) return (int)(k0 >> 16) <= th_high ? s0 : -1;
+    if constexpr (RULE == MCS_RULE_SCW) {
+        const int cap = f.n_keys / f.n_cams, c = s0 / cap;
+        const bool first = s0 == c * cap && f.cam_first[c] == 0;
+        return (int)(k0 >> 16) <= th_high && !first ? s0 : -1;
+    }
     if constexpr (RULE == MCS_RULE_RATIO) {
         const int d0 = (int)(k0 >> 16), d1 = s1 >= 0 ? (int)(k1 >> 16) : INT_MAX;
         return (double)d0 <= (double)d1 * nnratio && d0 <= th_high ? s0 : -1;
@@ -888,6 +895,211 @@ __global__ void __launch_bounds__(kQbThreads) fu_hits_kernel(const FuseHitQuerie
     });
 }
 
+// ---- SearchBySim3(KF1, KF2, vpMatches12, s12, R12, t12, th) (ref :1721-1988) ----
+// Nothing is skipped as taken in either direction, so each direction is Fuse's stateless decision (fu_best_kernel under th_high)
+// over one query per slot of the key frame whose points are carried over, and a mutual check joins the two.
+// The transforms of one direction: a's pose (R, t: GetPoseInverse's rotation and translation, row-major) and the similarity into
+// b's rig frame (sR, st), 24 doubles.
+struct Sim3Xf { double R[9], t[3], sR[9], st[3]; };
+
+// Slot s = c * capacity + j (j below camera c's count) of key frame a: its point p = mp[s] when p exists, s is not skipped (skip_mp:
+// matches12 on entry, >= 0 = already matched; skip: already2, non-zero = already matched), and p is not bad.  Then, in the order and
+// arithmetic of the reference (cv::Matx products, no FMA): pa = R * X + t, pb = sR * pa + st, p4 = mc_inv[c] * (pb, 1); the query is
+// dropped when pb.z < 0 (the RIG frame's z), when WorldToImg(p4) falls outside camera c's mirror mask, or when |p4| (a double) lies
+// outside [min, max]; else its level is lower_bound over the scale factors, clamped.  An id >= n_points in mp or skip_mp drops the
+// slot and raises status.
+struct Sim3ProjArgs {
+    const PsCamSlots* a; int n_cams, capacity, n_points, n_levels;
+    const int* mp; const int* skip_mp; const uint8_t* skip; const uint8_t* bad;
+    const double* pos; const double* dmin; const double* dmax;
+    const mcs_ocam* models; const Sim3Xf* xf; const double* mc_inv; const uint8_t* masks; const double* sf;
+};
+__global__ void __launch_bounds__(256) s3_project_kernel(const Sim3ProjArgs a, uint8_t* __restrict__ ok, double* __restrict__ u,
+                                                         double* __restrict__ v, int* __restrict__ level, int* __restrict__ status) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= a.n_cams * a.capacity) return;
+    const int c = s / a.capacity, j = s - c * a.capacity;
+    ok[s] = 0;
+    if (j >= min(*a.a[c].count, a.capacity)) return;
+    if (a.skip_mp) {                              // checked first: an invalid matches12 entry raises status whatever mp holds
+        const int m = a.skip_mp[s];
+        if (m >= a.n_points) { *status = MCS_ERR_INVALID; return; }
+        if (m >= 0) return;
+    }
+    const int p = a.mp[s];
+    if (p < 0) return;
+    if (p >= a.n_points) { *status = MCS_ERR_INVALID; return; }
+    if ((a.skip && a.skip[s]) || (a.bad && a.bad[p])) return;
+    const Sim3Xf x = *a.xf;
+    const double X0 = a.pos[3 * p], X1 = a.pos[3 * p + 1], X2 = a.pos[3 * p + 2];
+    double pa[3], pb[3], p4[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) pa[k] = ((x.R[3 * k] * X0 + x.R[3 * k + 1] * X1) + x.R[3 * k + 2] * X2) + x.t[k];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) pb[k] = ((x.sR[3 * k] * pa[0] + x.sR[3 * k + 1] * pa[1]) + x.sR[3 * k + 2] * pa[2]) + x.st[k];
+    const double* M = a.mc_inv + 16 * c;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) p4[k] = ((M[4 * k] * pb[0] + M[4 * k + 1] * pb[1]) + M[4 * k + 2] * pb[2]) + M[4 * k + 3] * 1.0;
+    if (pb[2] < 0.0) return;
+    const mcs_ocam cam = a.models[c];
+    double x_, y_;
+    cam_world_to_img(cam, p4[0], p4[1], p4[2], x_, y_);
+    const int ur = __double2int_rn(x_), vr = __double2int_rn(y_);
+    if (ur >= cam.width || ur <= 0 || vr >= cam.height || vr <= 0) return;
+    if (!a.masks[(size_t)c * cam.width * cam.height + (size_t)vr * cam.width + ur]) return;
+    const double d = sqrt((p4[0] * p4[0] + p4[1] * p4[1]) + p4[2] * p4[2]);
+    if (d < a.dmin[p] || d > a.dmax[p]) return;
+    const double ratio = d / a.dmin[p];
+    int lv = 0;                                   // std::lower_bound(vfScaleFactors, ratio), clamped to the last level
+    while (lv < a.n_levels && a.sf[lv] < ratio) ++lv;
+    if (lv >= a.n_levels) lv = a.n_levels - 1;
+    ok[s] = 1; u[s] = x_; v[s] = y_; level[s] = lv;
+}
+
+struct Sim3Queries {             // slot s of key frame a as s3_project_kernel set it: GetFeaturesInArea(c, u, v, th * sf[l]), levels {l - 1, l}
+    int n_slots, capacity;
+    const uint8_t* ok; const double* u; const double* v; const int* level; const int* mp;
+    const double* sf; double th;
+    __host__ __device__ long long size() const { return n_slots; }
+    __device__ bool valid(long long k, int*) const { return k < n_slots && ok[k]; }
+    __device__ mcs_window_query make(long long k) const {
+        const int lvl = level[k];
+        mcs_window_query q;
+        q.cam = (int)(k / capacity); q.min_level = lvl - 1; q.max_level = lvl; q.desc_index = mp[k];
+        q.x = u[k]; q.y = v[k]; q.r = th * sf[lvl];
+        return q;
+    }
+};
+
+// best[entry[q]] = dec[q]: a direction's decisions by slot of the key frame carried over (best starts at -1)
+__global__ void s3_scatter_kernel(const int* __restrict__ nq_p, const int* __restrict__ entry, const int* __restrict__ dec, int* __restrict__ best) {
+    const int nq = *nq_p;
+    for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += gridDim.x * blockDim.x) best[entry[q]] = dec[q];
+}
+
+// The agreement (ref :1964-1985): matches12[s1] = mp2[s2] where b1[s1] = s2 and b2[s2] = s1; nfound counts them.
+__global__ void __launch_bounds__(256) s3_mutual_kernel(const PsCamSlots* __restrict__ kf1, const int n_cams, const int capacity,
+                                                        const int* __restrict__ b1, const int* __restrict__ b2, const int* __restrict__ mp2,
+                                                        int* __restrict__ matches12, int* __restrict__ nfound) {
+    __shared__ int s_n;
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    if (s < n_cams * capacity) {
+        const int c = s / capacity, j = s - c * capacity;
+        const int s2 = j < min(*kf1[c].count, capacity) ? b1[s] : -1;
+        if (s2 >= 0 && b2[s2] == s) {
+            matches12[s] = mp2[s2];
+            atomicAdd(&s_n, 1);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && s_n) atomicAdd(nfound, s_n);
+}
+
+// ---- SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) (ref :2265-2392) ----
+// first[c]: the first contiguous keypoint id of camera c (the counts before it, each clamped to the capacity); first[n_cams]: the
+// key frame's keypoints.
+__global__ void scw_first_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, int* __restrict__ first) {
+    int acc = 0;
+    for (int c = 0; c < n_cams; ++c) { first[c] = acc; acc += min(*cams[c].count, capacity); }
+    first[n_cams] = acc;
+}
+
+// The frame view of the search: slot c * capacity + j carries keypoint j of camera c with the descriptor and mask of ROW first(c) + j
+// of camera c's matrix (the reference compares candidate idx through GetDescriptorRowPtr(camIdx, idx), idx the contiguous id,
+// :2367, :2372).  Where that row lies at or beyond the camera's count the reference reads past the matrix; the keypoint is then left
+// out, placed outside every image like an empty slot (ps_gather_kernel).
+__global__ void scw_gather_kernel(const PsCamSlots* __restrict__ cams, const int* __restrict__ first, const int n_cams, const int capacity,
+                                  const int dim, const bool masked, mcs_keypoint* __restrict__ keys, int* __restrict__ key_cam,
+                                  uint8_t* __restrict__ desc, uint8_t* __restrict__ dmask) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_cams * capacity) return;
+    const int c = s / capacity, j = s - c * capacity;
+    const PsCamSlots cs = cams[c];
+    const int n = min(*cs.count, capacity), row = first[c] + j;
+    key_cam[s] = c;
+    const int v4 = dim / 16;
+    if (j < n && row < n) {
+        keys[s] = cs.kps[j];
+        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = ((const uint4*)cs.desc)[(size_t)row * v4 + k];
+        if (masked)
+            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = ((const uint4*)cs.dmask)[(size_t)row * v4 + k];
+    } else {
+        mcs_keypoint e{};
+        e.x = e.y = -1.0e6f;                 // PosInGrid falls outside the image: never a candidate
+        keys[s] = e;
+        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = make_uint4(0, 0, 0, 0);
+        if (masked)
+            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = make_uint4(0, 0, 0, 0);
+    }
+}
+
+// found[p] = 1 for every point a slot of vpMatched holds on entry (spAlreadyFound).  Ids >= n_points mark their keypoint taken and
+// find no point.
+__global__ void scw_found_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, const int n_points,
+                                 const int* __restrict__ matched, uint8_t* __restrict__ found) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n_cams * capacity) return;
+    const int c = s / capacity, j = s - c * capacity;
+    if (j >= min(*cams[c].count, capacity)) return;
+    const int p = matched[s];
+    if (p >= 0 && p < n_points) found[p] = 1;
+}
+
+// Entry i of vpPoints: its point p, when not NULL, not bad and not already found, is projected into the camera of CONTIGUOUS
+// KEYPOINT i of the key frame (keypoint_to_cam.find(iMP), :2307) with the Sim3's rigid pose (WorldToCamHom_fast, mirror mask), its
+// double distance to ow tested against [min, max] and its level predicted, as fu_project_kernel does for MCS_FUSE_SIM3.  An entry
+// at or beyond the key frame's keypoints (where the reference dereferences end(): undefined) and an id >= n_points are dropped and
+// raise status.
+struct ScwProjArgs {
+    int n_q, n_cams, n_points, n_levels;
+    const int* points; const uint8_t* bad; const uint8_t* found; const int* first;
+    const double* pos; const double* dmin; const double* dmax;
+    const mcs_ocam* models; const double* mtmc_inv; const double* ow; const uint8_t* masks; const double* sf;
+};
+__global__ void __launch_bounds__(256) scw_project_kernel(const ScwProjArgs a, uint8_t* __restrict__ ok, double* __restrict__ u,
+                                                          double* __restrict__ v, int* __restrict__ level, int* __restrict__ qcam,
+                                                          int* __restrict__ status) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n_q) return;
+    ok[i] = 0;
+    const int p = a.points[i];
+    if (p < 0) return;
+    if (p >= a.n_points) { *status = MCS_ERR_INVALID; return; }
+    if ((a.bad && a.bad[p]) || a.found[p]) return;
+    if (i >= a.first[a.n_cams]) { *status = MCS_ERR_INVALID; return; }
+    int c = 0;
+    while (i >= a.first[c + 1]) ++c;
+    const mcs_ocam cam = a.models[c];
+    const double P0 = a.pos[3 * p], P1 = a.pos[3 * p + 1], P2 = a.pos[3 * p + 2];
+    double x, y;
+    if (!cam_project_in_mask(a.mtmc_inv + 16 * c, cam, a.masks + (size_t)c * cam.width * cam.height, P0, P1, P2, x, y)) return;
+    const double o0 = P0 - a.ow[0], o1 = P1 - a.ow[1], o2 = P2 - a.ow[2];
+    const double d = sqrt((o0 * o0 + o1 * o1) + o2 * o2);
+    if (d < a.dmin[p] || d > a.dmax[p]) return;
+    const double ratio = d / a.dmin[p];
+    int lv = 0;                                   // std::lower_bound(vfScaleFactors, ratio), clamped to the last level
+    while (lv < a.n_levels && a.sf[lv] < ratio) ++lv;
+    if (lv >= a.n_levels) lv = a.n_levels - 1;
+    ok[i] = 1; u[i] = x; v[i] = y; level[i] = lv; qcam[i] = c;
+}
+
+struct ScwQueries {              // entry i as scw_project_kernel set it: GetFeaturesInArea(cam, u, v, th * sf[l]) on levels {l - 1, l}
+    int n_q;
+    const uint8_t* ok; const double* u; const double* v; const int* level; const int* qcam; const int* points;
+    const double* sf; double th;
+    __host__ __device__ long long size() const { return n_q; }
+    __device__ bool valid(long long k, int*) const { return k < n_q && ok[k]; }
+    __device__ mcs_window_query make(long long k) const {
+        const int lvl = level[k];
+        mcs_window_query q;
+        q.cam = qcam[k]; q.min_level = lvl - 1; q.max_level = lvl; q.desc_index = points[k];
+        q.x = u[k]; q.y = v[k]; q.r = th * sf[lvl];
+        return q;
+    }
+};
+
 }  // namespace
 
 int proj_search_max_rounds() { return kPsRounds; }
@@ -911,10 +1123,12 @@ struct PsFront {
 
 // The front end from the query maker on: the frame view of `a` in slot order and its grid, the queries in the maker's order and
 // their lists.  qdesc / qmask: the query descriptors, row desc_index.  staged (may be NULL): a.cams already on the device, in
-// stream order, which the front end then reads instead of staging its own copy.
+// stream order, which the front end then reads instead of staging its own copy.  cam_first (may be NULL, needs staged): the device
+// [n_cams + 1] first contiguous ids of SearchByProjection(KF, Scw); the frame view is then scw_gather_kernel's, and the view's
+// cam_first is set for MCS_RULE_SCW's decision.
 template <class QM>
 cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const uint8_t* qmask, PsFront& fr, cudaStream_t st,
-                     const PsCamSlots* staged = nullptr) {
+                     const PsCamSlots* staged = nullptr, const int* cam_first = nullptr) {
     const int NS = a.n_cams * a.capacity;
     const int ncell = a.n_cams * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
     const long long Q = qm.size();
@@ -953,7 +1167,10 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
     if (e != cudaSuccess) return e;
 
     // frame view in slot order and its grid (the kernel the host entry points build their grid with)
-    ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
+    if (cam_first)
+        scw_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, cam_first, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
+    else
+        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
     e = launch_frame_prepare(keys, key_cam, NS, cams, a.n_cams, kx, ky, koct, nullptr, cell_of, cursor, cell_start, cell_items, winv, hinv, st);
     // queries in the reference's order
     qm.sf = sf;
@@ -963,7 +1180,7 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
         ps_fill_kernel<<<nb, kQbThreads, 0, st>>>(qm, boff, qry);
         e = cudaGetLastError();
     }
-    fr.f = WindowFrameDev{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv};
+    fr.f = WindowFrameDev{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv, cam_first};
     fr.slots = slots; fr.keys = keys;
     fr.qry = qry; fr.lkey = lkey; fr.lslot = lslot; fr.lcnt = lcnt; fr.qoff = boff; fr.ctl = ctl; fr.dec = dec; fr.owner = owner;
     fr.qd = (const uint32_t*)qdesc; fr.qk = a.masked ? (const uint32_t*)qmask : nullptr;
@@ -978,14 +1195,14 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
     return e;
 }
 
-// Both searches from the query maker on: the front end, then the rounds and the walk under RULE.  tag: see PsState.  The caller
-// has zeroed a.nmatches and a.status.
+// Both searches from the query maker on: the front end, then the rounds and the walk under RULE.  tag: see PsState.  staged,
+// cam_first: see ps_front.  The caller has zeroed a.nmatches and a.status.
 template <int RULE, class QM>
 cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const uint8_t* qdesc, const uint8_t* qmask, const int* tag,
-                      cudaStream_t st) {
+                      cudaStream_t st, const PsCamSlots* staged = nullptr, const int* cam_first = nullptr) {
     const int NS = a.n_cams * a.capacity;
     PsFront fr;
-    cudaError_t e = ps_front(a, qm, qdesc, qmask, fr, st);
+    cudaError_t e = ps_front(a, qm, qdesc, qmask, fr, st, staged, cam_first);
     const long long Q = fr.Q;
     if (e == cudaSuccess && Q > 0) {
         const PsState p{fr.qry, fr.lkey, fr.lslot, fr.lcnt, fr.dec, fr.owner, fr.ctl, (int)Q, NS, a.capacity, a.th_high, nnratio, tag};
@@ -1200,6 +1417,101 @@ cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st) {
         }
     }
     return sc.release(fr.sc.release(e));
+}
+
+// SearchBySim3: per direction the slot projections (s3_project_kernel), the front end over the other key frame with Sim3Queries,
+// Fuse's stateless decision under th_high and the scatter of the decisions to slots; then the mutual check.  The projection and
+// list scratch of direction 1 is reused by direction 2 in stream order.
+cudaError_t launch_search_by_sim3(const Sim3SearchDevArgs& a, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity, nb = (NS + kQbTile - 1) / kQbTile;
+    const size_t b_slots = sizeof(PsCamSlots) * a.n_cams;
+    static_assert(sizeof(Sim3Xf) == 24 * sizeof(double), "two directions of 24 doubles");
+    cudaError_t e = ps_zero_outputs(a, st);
+    if (e != cudaSuccess) return e;
+    StreamScratch sc;
+    e = sc.alloc({b_slots, b_slots, sizeof(mcs_ocam) * a.n_cams, 128ull * a.n_cams, 2 * sizeof(Sim3Xf), 8ull * a.n_levels,   // staged
+                  (size_t)NS, 8ull * NS, 8ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS},                     // ok u v level entry dec b1 b2
+                 st);
+    if (e != cudaSuccess) return e;
+    PsCamSlots* s1 = sc.at<PsCamSlots>(0); PsCamSlots* s2 = sc.at<PsCamSlots>(1); mcs_ocam* models = sc.at<mcs_ocam>(2);
+    double* mc_inv = sc.at<double>(3); Sim3Xf* xf = sc.at<Sim3Xf>(4); double* sf = sc.at<double>(5);
+    uint8_t* ok = sc.at<uint8_t>(6); double* u = sc.at<double>(7); double* v = sc.at<double>(8); int* level = sc.at<int>(9);
+    int* entry = sc.at<int>(10); int* dec = sc.at<int>(11); int* b1 = sc.at<int>(12); int* b2 = sc.at<int>(13);
+    e = stage_to_device(a.kf1, b_slots, s1, st);
+    if (e == cudaSuccess) e = stage_to_device(a.cams, b_slots, s2, st);
+    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
+    if (e == cudaSuccess) e = stage_to_device(a.mc_inv, 128ull * a.n_cams, mc_inv, st);
+    if (e == cudaSuccess) e = stage_to_device(a.xf, 2 * sizeof(Sim3Xf), xf, st);
+    if (e == cudaSuccess) e = stage_to_device(a.sf, 8ull * a.n_levels, sf, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(b1, 0xFF, 4ull * NS, st);        // no decision yet: -1
+    if (e == cudaSuccess) e = cudaMemsetAsync(b2, 0xFF, 4ull * NS, st);
+    int sms = 0;
+    if (e == cudaSuccess) e = sm_count(sms);
+    const int blocks = (int)std::min<long long>((NS + 255) / 256, (long long)sms * 8);
+    for (int dir = 0; dir < 2 && e == cudaSuccess; ++dir) {
+        const bool one = dir == 0;                           // direction 1: KF1's points into KF2; direction 2: KF2's into KF1
+        const int* mp = one ? a.mp1 : a.mp2;
+        const Sim3ProjArgs pa{one ? s1 : s2, a.n_cams, a.capacity, a.n_points, a.n_levels, mp, one ? a.matches12 : nullptr,
+                              one ? nullptr : a.already2, a.bad, a.world_pos, a.min_dist, a.max_dist, models, xf + dir, mc_inv, a.masks, sf};
+        s3_project_kernel<<<(NS + 255) / 256, 256, 0, st>>>(pa, ok, u, v, level, a.status);
+        e = cudaGetLastError();
+        PsFrameArgs fa = a;
+        fa.cams = one ? a.cams : a.kf1;
+        const Sim3Queries qm{NS, a.capacity, ok, u, v, level, mp, nullptr, a.th};
+        PsFront fr;
+        if (e == cudaSuccess) e = ps_front(fa, qm, a.desc, a.dmask, fr, st, one ? s2 : s1);
+        if (e == cudaSuccess) {
+            fu_entry_kernel<<<nb, kQbThreads, 0, st>>>(qm, fr.qoff, entry);
+            fu_best_kernel<<<blocks, 256, 0, st>>>(fr.ctl, fr.lkey, fr.lslot, a.th_high, dec);
+            s3_scatter_kernel<<<blocks, 256, 0, st>>>(fr.ctl, entry, dec, one ? b1 : b2);
+            e = cudaGetLastError();
+        }
+        e = fr.sc.release(e);
+    }
+    if (e == cudaSuccess) {
+        s3_mutual_kernel<<<(NS + 255) / 256, 256, 0, st>>>(s1, a.n_cams, a.capacity, b1, b2, a.mp2, a.matches12, a.nmatches);
+        e = cudaGetLastError();
+    }
+    return sc.release(e);
+}
+
+// SearchByProjection(KF, Scw): the first contiguous ids (scw_first_kernel), spAlreadyFound (scw_found_kernel), the entry projections
+// (scw_project_kernel), then the rounds and the walk under MCS_RULE_SCW over scw_gather_kernel's view, with the map-point ids as
+// the tags (desc_index).
+cudaError_t launch_search_by_projection_scw(const ScwSearchDevArgs& a, cudaStream_t st) {
+    const int NS = a.n_cams * a.capacity;
+    cudaError_t e = ps_zero_outputs(a, st);
+    if (e != cudaSuccess) return e;
+    StreamScratch sc;
+    e = sc.alloc({sizeof(PsCamSlots) * a.n_cams, sizeof(mcs_ocam) * a.n_cams, 128ull * a.n_cams, 24, 8ull * a.n_levels,   // staged
+                  4ull * (a.n_cams + 1), (size_t)a.n_points,                                                               // first found
+                  (size_t)a.n_q, 8ull * a.n_q, 8ull * a.n_q, 4ull * a.n_q, 4ull * a.n_q},                                  // ok u v level qcam
+                 st);
+    if (e != cudaSuccess) return e;
+    PsCamSlots* slots = sc.at<PsCamSlots>(0); mcs_ocam* models = sc.at<mcs_ocam>(1); double* mtmc_inv = sc.at<double>(2);
+    double* ow = sc.at<double>(3); double* sf = sc.at<double>(4); int* first = sc.at<int>(5); uint8_t* found = sc.at<uint8_t>(6);
+    uint8_t* ok = sc.at<uint8_t>(7); double* u = sc.at<double>(8); double* v = sc.at<double>(9); int* level = sc.at<int>(10);
+    int* qcam = sc.at<int>(11);
+    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, slots, st);
+    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
+    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, mtmc_inv, st);
+    if (e == cudaSuccess) e = stage_to_device(a.ow, 24, ow, st);
+    if (e == cudaSuccess) e = stage_to_device(a.sf, 8ull * a.n_levels, sf, st);
+    if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(found, 0, a.n_points, st);
+    if (e != cudaSuccess) return sc.release(e);
+    scw_first_kernel<<<1, 1, 0, st>>>(slots, a.n_cams, a.capacity, first);
+    scw_found_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.n_points, a.frame_mp, found);
+    if (a.n_q > 0) {
+        const ScwProjArgs pa{a.n_q, a.n_cams, a.n_points, a.n_levels, a.points, a.bad, found, first, a.world_pos, a.min_dist, a.max_dist,
+                             models, mtmc_inv, ow, a.masks, sf};
+        scw_project_kernel<<<(a.n_q + 255) / 256, 256, 0, st>>>(pa, ok, u, v, level, qcam, a.status);
+    }
+    e = cudaGetLastError();
+    if (e == cudaSuccess) {
+        const ScwQueries qm{a.n_q, ok, u, v, level, qcam, a.points, nullptr, (double)a.th};
+        e = ps_search<MCS_RULE_SCW>(a, qm, 0.0, a.desc, a.dmask, nullptr, st, slots, first);
+    }
+    return sc.release(e);
 }
 
 cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_cams, int capacity, double* prev, cudaStream_t st) {

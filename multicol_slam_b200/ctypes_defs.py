@@ -86,6 +86,13 @@ def set_prototypes(lib):
     f = lib.mcs_fuse_device
     f.argtypes = [C.POINTER(FuseTarget), I, I, I, I, P, P, I, P, I, P, I, I, P, P, P, P, P, P, D, I, I, P, I, P, P, P]
     f.restype = C.c_int
+    f = lib.mcs_search_by_sim3_device
+    f.argtypes = [C.POINTER(PackedFrame), C.POINTER(PackedFrame), I, I, I, P, P, I, P, P, P, P, D, P, P, D, P, P, I, P, P, P, P, P, P, P, I, I,
+                  P, P, P, P]
+    f.restype = C.c_int
+    f = lib.mcs_search_by_projection_scw_device
+    f.argtypes = [C.POINTER(PackedFrame), I, I, I, P, P, I, P, P, P, P, I, I, P, P, P, P, P, P, I, I, I, P, P, P, P, P]
+    f.restype = C.c_int
     f = lib.mcs_vocabulary_level_nodes
     f.argtypes = [P, I, C.POINTER(I)]
     f.restype = C.c_int
