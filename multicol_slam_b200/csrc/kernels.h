@@ -154,7 +154,7 @@ struct PsCamSlots {                     // camera c of the frame: its image slot
 struct PsFrameArgs {                    // both searches: the frame searched, the acceptance threshold, the outputs
     int n_cams, capacity, dim, n_levels;
     const PsCamSlots* cams;                                  // host [n_cams] (device pointers inside)
-    const int* cam_w; const int* cam_h; const double* sf;    // host
+    const int* cam_w; const int* cam_h; const double* sf;    // host; the sizes are read only by searches without camera models
     int th_high; bool masked;
     int* frame_mp; int* nmatches; int* status; int* diag;    // device
 };
@@ -201,16 +201,21 @@ cudaError_t launch_search_for_initialization(const InitSearchDevArgs& a, cudaStr
 // prev = the position of every F1 keypoint below its camera's count (f1: host [n_cams])
 cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_cams, int capacity, double* prev, cudaStream_t st);
 int proj_search_max_rounds();
+// The map points Fuse, SearchBySim3 and SearchByProjection(KF, Scw) project, and the cameras they are projected into.
+struct PsMapPoints {
+    int n_points;
+    const double* world_pos; const double* min_dist; const double* max_dist;   // device [n_points * 3], [n_points], [n_points]
+    const uint8_t* desc; const uint8_t* dmask; const uint8_t* bad;             // device (dmask NULL unless masked, bad may be NULL)
+    const mcs_ocam* models; const uint8_t* masks;                              // host [cameras], device [cameras][h][w]
+};
 // The Fuse overloads (mcs_fuse_device) for n_kf key frames in one call: the searched frame (PsFrameArgs) is the n_kf * n_cams
 // images of the targets, image k * n_cams + c = camera c of key frame k; th_high holds TH_LOW_; frame_mp and nmatches are unused.
 struct FuseDevArgs : PsFrameArgs {
-    int n_kf, n_kf_cams, variant, n_q, n_points;              // n_kf_cams: cameras per key frame
+    int n_kf, n_kf_cams, variant, n_q;                        // n_kf_cams: cameras per key frame, the models' count
     const int* const* kf_mp;                                 // host [n_kf]: each key frame's slot-indexed map-point ids (NULL entries)
     const double* mtmc_inv; const double* ow;                // host [n_kf * n_kf_cams * 16], [n_kf * 3]
-    const mcs_ocam* models; const uint8_t* masks;            // host [n_kf_cams], device [n_kf_cams][h][w]
     const int* query_mp;                                     // device [n_q], -1 = NULL
-    const double* world_pos; const double* min_dist; const double* max_dist;   // device map points
-    const uint8_t* desc; const uint8_t* dmask; const uint8_t* bad;
+    PsMapPoints pts;
     double th;
     int* hits; int max_hits; int* n_hits;                    // device [max_hits * 3], [1]
 };
@@ -219,14 +224,11 @@ cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st);
 // frame_mp and diag are unused.
 struct Sim3SearchDevArgs : PsFrameArgs {
     const PsCamSlots* kf1;                                   // host [n_cams]
-    const mcs_ocam* models; const uint8_t* masks;            // host [n_cams], device [n_cams][h][w]
     const double* xf;                                        // host [48]: per direction R[9] t[3] sR[9] st[3] (direction 1, then 2)
     const double* mc_inv;                                    // host [n_cams * 16]: invMat(Get_M_c(c))
     double th;
-    int n_points;
+    PsMapPoints pts;
     const int* mp1; const int* mp2;                          // device, slot-indexed
-    const double* world_pos; const double* min_dist; const double* max_dist;
-    const uint8_t* desc; const uint8_t* dmask; const uint8_t* bad;
     const uint8_t* already2;                                 // device, KF2 slot-indexed, may be NULL
     int* matches12;                                          // device, KF1 slot-indexed, in/out
 };
@@ -234,12 +236,10 @@ cudaError_t launch_search_by_sim3(const Sim3SearchDevArgs& a, cudaStream_t st);
 // SearchByProjection(pKF, Scw, vpPoints, vpMatched, th) (mcs_search_by_projection_scw_device): PsFrameArgs is the key frame with
 // th_high = TH_LOW_ and frame_mp = vpMatched (slot-indexed, in/out).
 struct ScwSearchDevArgs : PsFrameArgs {
-    const mcs_ocam* models; const uint8_t* masks;            // host [n_cams], device [n_cams][h][w]
     const double* mtmc_inv; const double* ow;                // host [n_cams * 16], [3]: the Sim3's rigid pose
-    int n_q, n_points;
+    int n_q;
     const int* points;                                       // device [n_q], -1 = NULL
-    const double* world_pos; const double* min_dist; const double* max_dist;
-    const uint8_t* desc; const uint8_t* dmask; const uint8_t* bad;
+    PsMapPoints pts;
     int th;
 };
 cudaError_t launch_search_by_projection_scw(const ScwSearchDevArgs& a, cudaStream_t st);

@@ -819,14 +819,12 @@ int mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, in
         std::memcpy(&mtmc_inv[16 * (size_t)k * n_cams], kfs[k].mtmc_inv, 128ull * n_cams);
         for (int i = 0; i < 3; ++i) ow[3 * k + i] = kfs[k].ow[i];
     }
-    const std::vector<int> cw(NI, cz.w[0]), ch(NI, cz.h[0]);
-    FuseDevArgs a{};
-    set_searched_frame(a, slots, capacity, dim, cw.data(), ch.data(), th_low, having_masks, nullptr, nullptr, status_dev, nullptr);
+    FuseDevArgs a{};                                     // the camera table is the models' (cam_w / cam_h unread)
+    set_searched_frame(a, slots, capacity, dim, nullptr, nullptr, th_low, having_masks, nullptr, nullptr, status_dev, nullptr);
     a.n_levels = n_levels; a.sf = scale_factors;
-    a.n_kf = n_kf; a.n_kf_cams = n_cams; a.variant = variant; a.n_q = n_q; a.n_points = n_points;
-    a.kf_mp = kf_mp.data(); a.mtmc_inv = mtmc_inv.data(); a.ow = ow.data(); a.models = cams; a.masks = masks_dev;
-    a.query_mp = query_mp_dev; a.world_pos = world_pos_dev; a.min_dist = min_dist_dev; a.max_dist = max_dist_dev;
-    a.desc = desc_dev; a.dmask = having_masks ? dmask_dev : nullptr; a.bad = bad_dev;
+    a.n_kf = n_kf; a.n_kf_cams = n_cams; a.variant = variant; a.n_q = n_q;
+    a.kf_mp = kf_mp.data(); a.mtmc_inv = mtmc_inv.data(); a.ow = ow.data(); a.query_mp = query_mp_dev;
+    a.pts = {n_points, world_pos_dev, min_dist_dev, max_dist_dev, desc_dev, having_masks ? dmask_dev : nullptr, bad_dev, cams, masks_dev};
     a.th = th; a.hits = hits_dev; a.max_hits = max_hits; a.n_hits = n_hits_dev;
     CUDA_CHECK(launch_fuse_device(a, st));
     return sync_if_null_stream(stream);
@@ -874,11 +872,9 @@ int mcs_search_by_sim3_device(const mcs_packed_frame* kf1, const mcs_packed_fram
     Sim3SearchDevArgs a{};
     set_searched_frame(a, s2, capacity, dim, cz.w.data(), cz.h.data(), th_high, having_masks, nullptr, nfound_dev, status_dev, nullptr);
     a.n_levels = n_levels; a.sf = scale_factors;
-    a.kf1 = s1.data(); a.models = cams; a.masks = masks_dev; a.xf = xf; a.mc_inv = mc_inv; a.th = th;
-    a.n_points = n_points; a.mp1 = mp1_dev; a.mp2 = mp2_dev;
-    a.world_pos = world_pos_dev; a.min_dist = min_dist_dev; a.max_dist = max_dist_dev;
-    a.desc = desc_dev; a.dmask = having_masks ? dmask_dev : nullptr; a.bad = bad_dev; a.already2 = already2_dev;
-    a.matches12 = matches12_dev;
+    a.kf1 = s1.data(); a.xf = xf; a.mc_inv = mc_inv; a.th = th;
+    a.pts = {n_points, world_pos_dev, min_dist_dev, max_dist_dev, desc_dev, having_masks ? dmask_dev : nullptr, bad_dev, cams, masks_dev};
+    a.mp1 = mp1_dev; a.mp2 = mp2_dev; a.already2 = already2_dev; a.matches12 = matches12_dev;
     CUDA_CHECK(launch_search_by_sim3(a, st));
     return sync_if_null_stream(stream);
 }
@@ -907,10 +903,9 @@ int mcs_search_by_projection_scw_device(const mcs_packed_frame* kf, int32_t n_ca
     ScwSearchDevArgs a{};
     set_searched_frame(a, slots, capacity, dim, cz.w.data(), cz.h.data(), th_low, having_masks, matched_dev, nmatches_dev, status_dev, diag_dev);
     a.n_levels = n_levels; a.sf = scale_factors;
-    a.models = cams; a.masks = masks_dev; a.mtmc_inv = mtmc_inv; a.ow = ow;
-    a.n_q = n_q; a.n_points = n_points; a.points = points_dev;
-    a.world_pos = world_pos_dev; a.min_dist = min_dist_dev; a.max_dist = max_dist_dev;
-    a.desc = desc_dev; a.dmask = having_masks ? dmask_dev : nullptr; a.bad = bad_dev; a.th = th;
+    a.mtmc_inv = mtmc_inv; a.ow = ow; a.n_q = n_q; a.points = points_dev;
+    a.pts = {n_points, world_pos_dev, min_dist_dev, max_dist_dev, desc_dev, having_masks ? dmask_dev : nullptr, bad_dev, cams, masks_dev};
+    a.th = th;
     CUDA_CHECK(launch_search_by_projection_scw(a, st));
     return sync_if_null_stream(stream);
 }

@@ -5,7 +5,8 @@
 // runs on the device.
 //
 //   ps_gather_kernel    a frame's keypoints / descriptors / masks in slot order (slot = cam * capacity + j); empty slots get a
-//                       position outside every image, so the unchanged frame_prepare_kernel leaves them out of the grid
+//                       position outside every image, so the unchanged frame_prepare_kernel leaves them out of the grid.
+//                       <true>: SearchByProjection(KF, Scw)'s descriptor rows, first[cam] + j
 //   pl_project_kernel   motion model only: per last-frame slot, its map point projected with the current pose into its camera
 //   pw_clear_kernel     WindowSearch only: the searched frame's assignments start free
 //   pf_flag / pf_project  SearchByProjection(F1, F2) only: "already found" and first-slot flags per map point, then per
@@ -22,7 +23,7 @@
 //                       query, so it runs no rounds; one warp per camera walks the camera's queries in order (InitQueries: one per
 //                       F1 slot) and writes matches12 and the survivors' prev.  pi_seed_kernel: FirstInitialization's prev
 //   fu_*                the Fuse overloads (:1265, :1420, :1570) for n_kf key frames searched as one frame of n_kf * n_cams
-//                       images: membership pre-filter, (key frame, query, camera) projections (FuseQueries), a stateless
+//                       images: membership pre-filter, (key frame, query, camera) projections (ProjectedQueries), a stateless
 //                       decision per query (fu_best / fu_first) and the hit rows in the reference's order
 //
 // No kernel reads anything back to the host: every size that depends on the data (the number of queries, the rounds the
@@ -69,22 +70,32 @@ constexpr int kNoChange = 0x7F7F7F7F;        // memset(0x7F): no decision change
 constexpr int kQbThreads = 256, kQbPer = 8, kQbTile = kQbThreads * kQbPer;
 static_assert(kPsRounds < 255, "round versions live in the top byte of the owner words");
 
+// slot s = c * capacity + j of a frame's slot table lies below camera c's count
+__device__ __forceinline__ bool ps_live(const PsCamSlots* cams, const int capacity, const int s) {
+    const int c = s / capacity;
+    return s - c * capacity < min(*cams[c].count, capacity);
+}
+
 // ---- frame view from the packed slots ----
-__global__ void ps_gather_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, const int dim,
-                                 const bool masked, mcs_keypoint* __restrict__ keys, int* __restrict__ key_cam,
+// Slot c * capacity + j carries keypoint j of camera c with the descriptor and mask of row j, or with SCW_ROWS those of row
+// first[c] + j (SearchByProjection(KF, Scw) compares candidate idx through GetDescriptorRowPtr(camIdx, idx), idx the contiguous
+// id, ref :2367, :2372); a keypoint whose row lies at or beyond the camera's count is left out like an empty slot.
+template <bool SCW_ROWS>
+__global__ void ps_gather_kernel(const PsCamSlots* __restrict__ cams, const int* __restrict__ first, const int n_cams, const int capacity,
+                                 const int dim, const bool masked, mcs_keypoint* __restrict__ keys, int* __restrict__ key_cam,
                                  uint8_t* __restrict__ desc, uint8_t* __restrict__ dmask) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_cams * capacity) return;
     const int c = s / capacity, j = s - c * capacity;
     const PsCamSlots cs = cams[c];
-    const int n = min(*cs.count, capacity);
+    const int n = min(*cs.count, capacity), row = SCW_ROWS ? first[c] + j : j;
     if (key_cam) key_cam[s] = c;          // NULL: a frame that is only read by slot, never through a grid
     const int v4 = dim / 16;
-    if (j < n) {
+    if (j < n && (!SCW_ROWS || row < n)) {
         keys[s] = cs.kps[j];
-        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = ((const uint4*)cs.desc)[(size_t)j * v4 + k];
+        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = ((const uint4*)cs.desc)[(size_t)row * v4 + k];
         if (masked)
-            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = ((const uint4*)cs.dmask)[(size_t)j * v4 + k];
+            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = ((const uint4*)cs.dmask)[(size_t)row * v4 + k];
     } else {
         mcs_keypoint e{};
         e.x = e.y = -1.0e6f;                 // PosInGrid falls outside the image: never a candidate
@@ -109,9 +120,9 @@ __global__ void __launch_bounds__(256) pl_project_kernel(const LastProjArgs a, u
                                                          double* __restrict__ v, int* __restrict__ status) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= a.n_cams * a.capacity) return;
-    const int c = s / a.capacity, j = s - c * a.capacity;
+    const int c = s / a.capacity;
     ok[s] = 0;
-    if (j >= min(*a.cams[c].count, a.capacity)) return;
+    if (!ps_live(a.cams, a.capacity, s)) return;
     const int i = a.last_mp[s];
     if (i < 0) return;
     if (i >= a.n_points) { *status = MCS_ERR_INVALID; return; }
@@ -130,8 +141,7 @@ __global__ void __launch_bounds__(256) pl_project_kernel(const LastProjArgs a, u
 __global__ void pw_clear_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, int* __restrict__ frame_mp) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_cams * capacity) return;
-    const int c = s / capacity, j = s - c * capacity;
-    if (j < min(*cams[c].count, capacity)) frame_mp[s] = -1;
+    if (ps_live(cams, capacity, s)) frame_mp[s] = -1;
 }
 
 // ---- previous frame: the skip rules of SearchByProjection(F1 = last, F2 = cur, window) (ref :481-500) ----
@@ -143,12 +153,11 @@ __global__ void pf_flag_kernel(const PsCamSlots* __restrict__ cur, const PsCamSl
                                int* __restrict__ first, int* __restrict__ status) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_cams * capacity) return;
-    const int c = s / capacity, j = s - c * capacity;
-    if (j < min(*cur[c].count, capacity)) {
+    if (ps_live(cur, capacity, s)) {
         const int p = cur_mp[s];
         if (p >= 0 && p < n_points) found[p] = 1;
     }
-    if (j < min(*last[c].count, capacity)) {
+    if (ps_live(last, capacity, s)) {
         const int p = last_mp[s];
         if (p >= n_points) *status = MCS_ERR_INVALID;
         else if (p >= 0) atomicMin(&first[p], s);
@@ -168,8 +177,7 @@ __global__ void __launch_bounds__(256) pf_project_kernel(const FramesProjArgs a,
     if (k >= (long long)a.n_cams * a.n_cams * a.capacity) return;
     const int s = (int)(k / a.n_cams), c = (int)(k - (long long)s * a.n_cams);
     ok[k] = 0;
-    const int cl = s / a.capacity;
-    if (s - cl * a.capacity >= min(*a.last[cl].count, a.capacity)) return;
+    if (!ps_live(a.last, a.capacity, s)) return;
     const int i = a.last_mp[s];
     if (i < 0 || i >= a.n_points) return;
     if ((a.bad && a.bad[i]) || a.found[i] || a.first[i] != s) return;
@@ -183,7 +191,7 @@ __global__ void __launch_bounds__(256) pf_project_kernel(const FramesProjArgs a,
 
 // ---- query build: a count / scan / fill over the entries of a query maker, in the maker's order ----
 // A maker has size() entries; valid(k) says whether entry k is a query (and may raise status), make(k) builds it.  sf is the
-// staged scale-factor table, set by ps_search.
+// launcher's staged scale-factor table.
 struct MapPointQueries {         // SearchByProjection(F, vpMapPoints): entry k = point * n_cams + cam, when not bad and in view
     int n_cams, n_points, n_levels;
     const uint8_t* bad; const uint8_t* in_view; const int* level;
@@ -758,6 +766,18 @@ __global__ void fu_held_kernel(const PsCamSlots* __restrict__ slots, const int* 
     if (q < n_q) held[(size_t)k * n_q + q] = 1;
 }
 
+// The range test and the predicted level of a projected point at distance d: false outside [dmin, dmax], else lv =
+// std::lower_bound(vfScaleFactors, d / dmin), clamped to the last level.
+__device__ __forceinline__ bool predict_level(const double d, const double dmin, const double dmax, const double* sf, const int n_levels,
+                                              int& lv) {
+    if (d < dmin || d > dmax) return false;
+    const double ratio = d / dmin;
+    lv = 0;
+    while (lv < n_levels && sf[lv] < ratio) ++lv;
+    if (lv >= n_levels) lv = n_levels - 1;
+    return true;
+}
+
 // Entry e = (k * n_q + q) * n_cams + c: query q's point, when not NULL, not bad and not held by key frame k, projected with
 // k's MtMc_inv into camera c (WorldToCamHom_fast, mirror mask), its distance to k's centre in the range [min, max] and its
 // level predicted, in the operation order of the host projection (api._project): dist3D a float for :1265 / :1420, a double for
@@ -787,28 +807,41 @@ __global__ void __launch_bounds__(256) fu_project_kernel(const FuseProjArgs a, u
     const double o0 = P0 - O[0], o1 = P1 - O[1], o2 = P2 - O[2];
     double d = sqrt((o0 * o0 + o1 * o1) + o2 * o2);
     if (a.float_dist) d = (double)__double2float_rn(d);
-    if (d < a.dmin[p] || d > a.dmax[p]) return;
-    const double ratio = d / a.dmin[p];
-    int lv = 0;                                   // std::lower_bound(vfScaleFactors, ratio), clamped to the last level
-    while (lv < a.n_levels && a.sf[lv] < ratio) ++lv;
-    if (lv >= a.n_levels) lv = a.n_levels - 1;
+    int lv;
+    if (!predict_level(d, a.dmin[p], a.dmax[p], a.sf, a.n_levels, lv)) return;
     ok[e] = 1; u[e] = x; v[e] = y; level[e] = lv;
 }
 
-struct FuseQueries {             // entry e as fu_project_kernel set it: GetFeaturesInArea(c, u, v, th * sf[l]) on levels {l - 1, l} of k
-    long long n_entries; int n_q, n_cams;
-    const uint8_t* ok; const double* u; const double* v; const int* level; const int* query_mp;
-    const double* sf; double th;
-    __host__ __device__ long long size() const { return n_entries; }
-    __device__ bool valid(long long e, int*) const { return e < n_entries && ok[e]; }
-    __device__ mcs_window_query make(long long e) const {
-        const long long kq = e / n_cams;
-        const int c = (int)(e - kq * n_cams), k = (int)(kq / n_q), lvl = level[e];
-        mcs_window_query qq;
-        qq.cam = k * n_cams + c; qq.min_level = lvl - 1; qq.max_level = lvl; qq.desc_index = query_mp[kq - (long long)k * n_q];
-        qq.x = u[e]; qq.y = v[e]; qq.r = th * sf[lvl];
-        return qq;
+// The query of entry k of a projection (fu_project / s3_project / scw_project_kernel set ok, u, v and level):
+// GetFeaturesInArea(cam, u, v, th * sf[l]) on levels {l - 1, l}.  `at` gives the entry's camera and descriptor row.
+template <class At> struct ProjectedQueries {
+    long long n; const uint8_t* ok; const double* u; const double* v; const int* level; const double* sf; double th;
+    At at;
+    __host__ __device__ long long size() const { return n; }
+    __device__ bool valid(long long k, int*) const { return k < n && ok[k]; }
+    __device__ mcs_window_query make(long long k) const {
+        const int lvl = level[k];
+        mcs_window_query q;
+        at(k, q.cam, q.desc_index);
+        q.min_level = lvl - 1; q.max_level = lvl; q.x = u[k]; q.y = v[k]; q.r = th * sf[lvl];
+        return q;
     }
+};
+struct FuseAt {                  // entry e = (k * n_q + q) * n_cams + c: image k * n_cams + c, the row of query q's map point
+    int n_q, n_cams; const int* query_mp;
+    __device__ void operator()(long long e, int& cam, int& row) const {
+        const long long kq = e / n_cams;
+        const int c = (int)(e - kq * n_cams), k = (int)(kq / n_q);
+        cam = k * n_cams + c; row = query_mp[kq - (long long)k * n_q];
+    }
+};
+struct Sim3At {                  // entry = slot s of key frame a: camera s / capacity, the row of the slot's map point
+    int capacity; const int* mp;
+    __device__ void operator()(long long s, int& cam, int& row) const { row = mp[s]; cam = (int)(s / capacity); }
+};
+struct ScwAt {                   // entry i of vpPoints: the camera scw_project_kernel found, the row of the entry's map point
+    const int* qcam; const int* points;
+    __device__ void operator()(long long i, int& cam, int& row) const { cam = qcam[i]; row = points[i]; }
 };
 
 // entry[i] = the maker entry of query i: ps_fill_kernel's fill, writing the entry index instead of the query
@@ -918,9 +951,9 @@ __global__ void __launch_bounds__(256) s3_project_kernel(const Sim3ProjArgs a, u
                                                          double* __restrict__ v, int* __restrict__ level, int* __restrict__ status) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= a.n_cams * a.capacity) return;
-    const int c = s / a.capacity, j = s - c * a.capacity;
+    const int c = s / a.capacity;
     ok[s] = 0;
-    if (j >= min(*a.a[c].count, a.capacity)) return;
+    if (!ps_live(a.a, a.capacity, s)) return;
     if (a.skip_mp) {                              // checked first: an invalid matches12 entry raises status whatever mp holds
         const int m = a.skip_mp[s];
         if (m >= a.n_points) { *status = MCS_ERR_INVALID; return; }
@@ -948,28 +981,10 @@ __global__ void __launch_bounds__(256) s3_project_kernel(const Sim3ProjArgs a, u
     if (ur >= cam.width || ur <= 0 || vr >= cam.height || vr <= 0) return;
     if (!a.masks[(size_t)c * cam.width * cam.height + (size_t)vr * cam.width + ur]) return;
     const double d = sqrt((p4[0] * p4[0] + p4[1] * p4[1]) + p4[2] * p4[2]);
-    if (d < a.dmin[p] || d > a.dmax[p]) return;
-    const double ratio = d / a.dmin[p];
-    int lv = 0;                                   // std::lower_bound(vfScaleFactors, ratio), clamped to the last level
-    while (lv < a.n_levels && a.sf[lv] < ratio) ++lv;
-    if (lv >= a.n_levels) lv = a.n_levels - 1;
+    int lv;
+    if (!predict_level(d, a.dmin[p], a.dmax[p], a.sf, a.n_levels, lv)) return;
     ok[s] = 1; u[s] = x_; v[s] = y_; level[s] = lv;
 }
-
-struct Sim3Queries {             // slot s of key frame a as s3_project_kernel set it: GetFeaturesInArea(c, u, v, th * sf[l]), levels {l - 1, l}
-    int n_slots, capacity;
-    const uint8_t* ok; const double* u; const double* v; const int* level; const int* mp;
-    const double* sf; double th;
-    __host__ __device__ long long size() const { return n_slots; }
-    __device__ bool valid(long long k, int*) const { return k < n_slots && ok[k]; }
-    __device__ mcs_window_query make(long long k) const {
-        const int lvl = level[k];
-        mcs_window_query q;
-        q.cam = (int)(k / capacity); q.min_level = lvl - 1; q.max_level = lvl; q.desc_index = mp[k];
-        q.x = u[k]; q.y = v[k]; q.r = th * sf[lvl];
-        return q;
-    }
-};
 
 // best[entry[q]] = dec[q]: a direction's decisions by slot of the key frame carried over (best starts at -1)
 __global__ void s3_scatter_kernel(const int* __restrict__ nq_p, const int* __restrict__ entry, const int* __restrict__ dec, int* __restrict__ best) {
@@ -986,8 +1001,7 @@ __global__ void __launch_bounds__(256) s3_mutual_kernel(const PsCamSlots* __rest
     if (threadIdx.x == 0) s_n = 0;
     __syncthreads();
     if (s < n_cams * capacity) {
-        const int c = s / capacity, j = s - c * capacity;
-        const int s2 = j < min(*kf1[c].count, capacity) ? b1[s] : -1;
+        const int s2 = ps_live(kf1, capacity, s) ? b1[s] : -1;
         if (s2 >= 0 && b2[s2] == s) {
             matches12[s] = mp2[s2];
             atomicAdd(&s_n, 1);
@@ -1006,43 +1020,13 @@ __global__ void scw_first_kernel(const PsCamSlots* __restrict__ cams, const int 
     first[n_cams] = acc;
 }
 
-// The frame view of the search: slot c * capacity + j carries keypoint j of camera c with the descriptor and mask of ROW first(c) + j
-// of camera c's matrix (the reference compares candidate idx through GetDescriptorRowPtr(camIdx, idx), idx the contiguous id,
-// :2367, :2372).  Where that row lies at or beyond the camera's count the reference reads past the matrix; the keypoint is then left
-// out, placed outside every image like an empty slot (ps_gather_kernel).
-__global__ void scw_gather_kernel(const PsCamSlots* __restrict__ cams, const int* __restrict__ first, const int n_cams, const int capacity,
-                                  const int dim, const bool masked, mcs_keypoint* __restrict__ keys, int* __restrict__ key_cam,
-                                  uint8_t* __restrict__ desc, uint8_t* __restrict__ dmask) {
-    const int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n_cams * capacity) return;
-    const int c = s / capacity, j = s - c * capacity;
-    const PsCamSlots cs = cams[c];
-    const int n = min(*cs.count, capacity), row = first[c] + j;
-    key_cam[s] = c;
-    const int v4 = dim / 16;
-    if (j < n && row < n) {
-        keys[s] = cs.kps[j];
-        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = ((const uint4*)cs.desc)[(size_t)row * v4 + k];
-        if (masked)
-            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = ((const uint4*)cs.dmask)[(size_t)row * v4 + k];
-    } else {
-        mcs_keypoint e{};
-        e.x = e.y = -1.0e6f;                 // PosInGrid falls outside the image: never a candidate
-        keys[s] = e;
-        for (int k = 0; k < v4; ++k) ((uint4*)desc)[(size_t)s * v4 + k] = make_uint4(0, 0, 0, 0);
-        if (masked)
-            for (int k = 0; k < v4; ++k) ((uint4*)dmask)[(size_t)s * v4 + k] = make_uint4(0, 0, 0, 0);
-    }
-}
-
 // found[p] = 1 for every point a slot of vpMatched holds on entry (spAlreadyFound).  Ids >= n_points mark their keypoint taken and
 // find no point.
 __global__ void scw_found_kernel(const PsCamSlots* __restrict__ cams, const int n_cams, const int capacity, const int n_points,
                                  const int* __restrict__ matched, uint8_t* __restrict__ found) {
     const int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n_cams * capacity) return;
-    const int c = s / capacity, j = s - c * capacity;
-    if (j >= min(*cams[c].count, capacity)) return;
+    if (!ps_live(cams, capacity, s)) return;
     const int p = matched[s];
     if (p >= 0 && p < n_points) found[p] = 1;
 }
@@ -1077,28 +1061,10 @@ __global__ void __launch_bounds__(256) scw_project_kernel(const ScwProjArgs a, u
     if (!cam_project_in_mask(a.mtmc_inv + 16 * c, cam, a.masks + (size_t)c * cam.width * cam.height, P0, P1, P2, x, y)) return;
     const double o0 = P0 - a.ow[0], o1 = P1 - a.ow[1], o2 = P2 - a.ow[2];
     const double d = sqrt((o0 * o0 + o1 * o1) + o2 * o2);
-    if (d < a.dmin[p] || d > a.dmax[p]) return;
-    const double ratio = d / a.dmin[p];
-    int lv = 0;                                   // std::lower_bound(vfScaleFactors, ratio), clamped to the last level
-    while (lv < a.n_levels && a.sf[lv] < ratio) ++lv;
-    if (lv >= a.n_levels) lv = a.n_levels - 1;
+    int lv;
+    if (!predict_level(d, a.dmin[p], a.dmax[p], a.sf, a.n_levels, lv)) return;
     ok[i] = 1; u[i] = x; v[i] = y; level[i] = lv; qcam[i] = c;
 }
-
-struct ScwQueries {              // entry i as scw_project_kernel set it: GetFeaturesInArea(cam, u, v, th * sf[l]) on levels {l - 1, l}
-    int n_q;
-    const uint8_t* ok; const double* u; const double* v; const int* level; const int* qcam; const int* points;
-    const double* sf; double th;
-    __host__ __device__ long long size() const { return n_q; }
-    __device__ bool valid(long long k, int*) const { return k < n_q && ok[k]; }
-    __device__ mcs_window_query make(long long k) const {
-        const int lvl = level[k];
-        mcs_window_query q;
-        q.cam = qcam[k]; q.min_level = lvl - 1; q.max_level = lvl; q.desc_index = points[k];
-        q.x = u[k]; q.y = v[k]; q.r = th * sf[lvl];
-        return q;
-    }
-};
 
 }  // namespace
 
@@ -1106,12 +1072,36 @@ int proj_search_max_rounds() { return kPsRounds; }
 
 namespace {
 
+// One small host input of a launcher: n elements at `host`, staged into the launcher's scratch; `dev` receives the device copy.
+template <class T> struct HostIn { const T*& dev; const T* host; size_t n; };
+template <class T> HostIn<T> host_in(const T*& dev, const T* host, size_t n) { return {dev, host, n}; }
+
+// A launcher's one stream-ordered scratch block: its own pieces first (own[i] is sc.at<T>(i)), then a device copy of every host
+// input, staged in stream order.  The caller releases sc, whatever the result.
+template <class... T>
+cudaError_t ps_open(StreamScratch& sc, std::vector<size_t> own, cudaStream_t st, const HostIn<T>&... in) {
+    size_t i = own.size();
+    (own.push_back(sizeof(T) * in.n), ...);
+    cudaError_t e = sc.alloc(own, st);
+    if (e != cudaSuccess) return e;
+    ((in.dev = sc.at<T>(i++)), ...);
+    ((e = e == cudaSuccess ? stage_to_device(in.host, sizeof(T) * in.n, (void*)in.dev, st) : e), ...);
+    return e;
+}
+
+// frame_prepare_kernel's camera table for a search without camera models: it reads only width and height (no rays)
+std::vector<mcs_ocam> cam_sizes(const PsFrameArgs& a) {
+    std::vector<mcs_ocam> hc(a.n_cams);
+    std::memset(hc.data(), 0, sizeof(mcs_ocam) * a.n_cams);
+    for (int c = 0; c < a.n_cams; ++c) { hc[c].width = a.cam_w[c]; hc[c].height = a.cam_h[c]; }
+    return hc;
+}
+
 // What the front end of the searches leaves for an acceptance stage, in one stream-ordered scratch block the caller releases: the
 // frame searched in slot order with its grid, the queries in the maker's order and their lists, and the acceptance scratch.
 struct PsFront {
     StreamScratch sc;
     WindowFrameDev f;
-    const PsCamSlots* slots;     // device [n_cams]: the searched frame's image slots
     const mcs_keypoint* keys;    // the searched frame in slot order
     const mcs_window_query* qry; const unsigned* lkey; const int* lslot; const int* lcnt;
     const int* qoff;                                         // the query fill's block offsets (kQbTile entries of the maker per block)
@@ -1122,13 +1112,12 @@ struct PsFront {
 };
 
 // The front end from the query maker on: the frame view of `a` in slot order and its grid, the queries in the maker's order and
-// their lists.  qdesc / qmask: the query descriptors, row desc_index.  staged (may be NULL): a.cams already on the device, in
-// stream order, which the front end then reads instead of staging its own copy.  cam_first (may be NULL, needs staged): the device
-// [n_cams + 1] first contiguous ids of SearchByProjection(KF, Scw); the frame view is then scw_gather_kernel's, and the view's
-// cam_first is set for MCS_RULE_SCW's decision.
+// their lists.  slots, cams: the searched frame's slot table and camera table [a.n_cams] on the device.  qdesc / qmask: the query
+// descriptors, row desc_index.  cam_first (may be NULL): the device [n_cams + 1] first contiguous ids of SearchByProjection(KF,
+// Scw); the frame view then carries the rows ps_gather_kernel<true> picks, and the view's cam_first is set for MCS_RULE_SCW.
 template <class QM>
-cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const uint8_t* qmask, PsFront& fr, cudaStream_t st,
-                     const PsCamSlots* staged = nullptr, const int* cam_first = nullptr) {
+cudaError_t ps_front(const PsFrameArgs& a, const QM& qm, const PsCamSlots* slots, const mcs_ocam* cams, const int* cam_first,
+                     const uint8_t* qdesc, const uint8_t* qmask, PsFront& fr, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     const int ncell = a.n_cams * MCS_FRAME_GRID_COLS * MCS_FRAME_GRID_ROWS;
     const long long Q = qm.size();
@@ -1138,42 +1127,32 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
     cudaError_t e = sm_count(sms);
     if (e != cudaSuccess) return e;
     StreamScratch& sc = fr.sc;
-    e = sc.alloc({sizeof(mcs_ocam) * a.n_cams, sizeof(double) * a.n_levels, sizeof(PsCamSlots) * a.n_cams,         // staged host inputs
-                  sizeof(mcs_keypoint) * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, db, a.masked ? db : 0,    // keys key_cam kx ky koct desc dmask
+    e = sc.alloc({sizeof(mcs_keypoint) * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, db, a.masked ? db : 0,    // keys key_cam kx ky koct desc dmask
                   4ull * NS, 4ull * ncell, 4ull * (ncell + 1), 4ull * NS, 8ull * a.n_cams, 8ull * a.n_cams,         // cell_of cursor start items winv hinv
                   4ull * (nb + 1), 4ull * (nb + 1), 4ull * (4 + kPsRounds),                                         // block counts / offsets, ctl
                   sizeof(mcs_window_query) * Q, 4ull * Q * kPsK, 4ull * Q * kPsK, 4ull * Q, 8ull * Q, 8ull * NS},   // qry lkey lslot lcnt dec owner
                  st);
     if (e != cudaSuccess) return e;
-    mcs_ocam* cams = sc.at<mcs_ocam>(0); double* sf = sc.at<double>(1);
-    PsCamSlots* slots = staged ? const_cast<PsCamSlots*>(staged) : sc.at<PsCamSlots>(2);
-    mcs_keypoint* keys = sc.at<mcs_keypoint>(3); int* key_cam = sc.at<int>(4); float* kx = sc.at<float>(5); float* ky = sc.at<float>(6);
-    int* koct = sc.at<int>(7); uint8_t* desc = sc.at<uint8_t>(8); uint8_t* dmask = a.masked ? sc.at<uint8_t>(9) : nullptr;
-    int* cell_of = sc.at<int>(10); int* cursor = sc.at<int>(11); int* cell_start = sc.at<int>(12); int* cell_items = sc.at<int>(13);
-    double* winv = sc.at<double>(14); double* hinv = sc.at<double>(15);
-    int* bcount = sc.at<int>(16); int* boff = sc.at<int>(17); int* ctl = sc.at<int>(18);
-    mcs_window_query* qry = sc.at<mcs_window_query>(19); unsigned* lkey = sc.at<unsigned>(20); int* lslot = sc.at<int>(21);
-    int* lcnt = sc.at<int>(22); int* dec = sc.at<int>(23); unsigned* owner = sc.at<unsigned>(24);
+    mcs_keypoint* keys = sc.at<mcs_keypoint>(0); int* key_cam = sc.at<int>(1); float* kx = sc.at<float>(2); float* ky = sc.at<float>(3);
+    int* koct = sc.at<int>(4); uint8_t* desc = sc.at<uint8_t>(5); uint8_t* dmask = a.masked ? sc.at<uint8_t>(6) : nullptr;
+    int* cell_of = sc.at<int>(7); int* cursor = sc.at<int>(8); int* cell_start = sc.at<int>(9); int* cell_items = sc.at<int>(10);
+    double* winv = sc.at<double>(11); double* hinv = sc.at<double>(12);
+    int* bcount = sc.at<int>(13); int* boff = sc.at<int>(14); int* ctl = sc.at<int>(15);
+    mcs_window_query* qry = sc.at<mcs_window_query>(16); unsigned* lkey = sc.at<unsigned>(17); int* lslot = sc.at<int>(18);
+    int* lcnt = sc.at<int>(19); int* dec = sc.at<int>(20); unsigned* owner = sc.at<unsigned>(21);
 
-    std::vector<mcs_ocam> hc(a.n_cams);
-    std::memset(hc.data(), 0, sizeof(mcs_ocam) * a.n_cams);
-    for (int c = 0; c < a.n_cams; ++c) { hc[c].width = a.cam_w[c]; hc[c].height = a.cam_h[c]; }
-    if (e == cudaSuccess) e = stage_to_device(hc.data(), sizeof(mcs_ocam) * a.n_cams, cams, st);
-    if (e == cudaSuccess) e = stage_to_device(a.sf, sizeof(double) * a.n_levels, sf, st);
-    if (e == cudaSuccess && !staged) e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, slots, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ctl, 0, 16, st);
+    e = cudaMemsetAsync(ctl, 0, 16, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctl + 4, 0x7F, 4 * kPsRounds, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(owner, 0xFF, 8ull * NS, st);
     if (e != cudaSuccess) return e;
 
     // frame view in slot order and its grid (the kernel the host entry points build their grid with)
     if (cam_first)
-        scw_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, cam_first, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
+        ps_gather_kernel<true><<<(NS + 255) / 256, 256, 0, st>>>(slots, cam_first, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
     else
-        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
+        ps_gather_kernel<false><<<(NS + 255) / 256, 256, 0, st>>>(slots, nullptr, a.n_cams, a.capacity, a.dim, a.masked, keys, key_cam, desc, dmask);
     e = launch_frame_prepare(keys, key_cam, NS, cams, a.n_cams, kx, ky, koct, nullptr, cell_of, cursor, cell_start, cell_items, winv, hinv, st);
     // queries in the reference's order
-    qm.sf = sf;
     if (e == cudaSuccess && nb > 0) {
         ps_count_kernel<<<nb, kQbThreads, 0, st>>>(qm, bcount, a.status);
         ps_scan_kernel<<<1, 1024, 0, st>>>(bcount, nb, boff, ctl);
@@ -1181,7 +1160,7 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
         e = cudaGetLastError();
     }
     fr.f = WindowFrameDev{a.n_cams, NS, a.dim, kx, ky, koct, desc, dmask, cell_start, cell_items, winv, hinv, cam_first};
-    fr.slots = slots; fr.keys = keys;
+    fr.keys = keys;
     fr.qry = qry; fr.lkey = lkey; fr.lslot = lslot; fr.lcnt = lcnt; fr.qoff = boff; fr.ctl = ctl; fr.dec = dec; fr.owner = owner;
     fr.qd = (const uint32_t*)qdesc; fr.qk = a.masked ? (const uint32_t*)qmask : nullptr;
     fr.Q = Q; fr.sms = sms;
@@ -1195,14 +1174,14 @@ cudaError_t ps_front(const PsFrameArgs& a, QM qm, const uint8_t* qdesc, const ui
     return e;
 }
 
-// Both searches from the query maker on: the front end, then the rounds and the walk under RULE.  tag: see PsState.  staged,
+// Both searches from the query maker on: the front end, then the rounds and the walk under RULE.  tag: see PsState.  slots, cams,
 // cam_first: see ps_front.  The caller has zeroed a.nmatches and a.status.
 template <int RULE, class QM>
-cudaError_t ps_search(const PsFrameArgs& a, QM qm, const double nnratio, const uint8_t* qdesc, const uint8_t* qmask, const int* tag,
-                      cudaStream_t st, const PsCamSlots* staged = nullptr, const int* cam_first = nullptr) {
+cudaError_t ps_search(const PsFrameArgs& a, const QM& qm, const double nnratio, const uint8_t* qdesc, const uint8_t* qmask, const int* tag,
+                      const PsCamSlots* slots, const mcs_ocam* cams, const int* cam_first, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     PsFront fr;
-    cudaError_t e = ps_front(a, qm, qdesc, qmask, fr, st, staged, cam_first);
+    cudaError_t e = ps_front(a, qm, slots, cams, cam_first, qdesc, qmask, fr, st);
     const long long Q = fr.Q;
     if (e == cudaSuccess && Q > 0) {
         const PsState p{fr.qry, fr.lkey, fr.lslot, fr.lcnt, fr.dec, fr.owner, fr.ctl, (int)Q, NS, a.capacity, a.th_high, nnratio, tag};
@@ -1227,34 +1206,31 @@ cudaError_t ps_zero_outputs(const PsFrameArgs& a, cudaStream_t st) {
 }
 
 // What the searches between two frames share, in the launcher's one stream-ordered scratch block: its own pieces (`own`, from
-// piece 0 on), then the staged slots of cur (when stage_cur) and of last, the staged camera models and mtmc_inv (when a.models is
-// set: the searches that project), and the last frame in slot order.  The caller releases `sc`, whatever the result.
+// piece 0 on), the last frame in slot order, and the staged slot tables of cur and last, camera table (the models when the search
+// projects, else the image sizes), mtmc_inv (searches that project) and scale factors.  The caller releases `sc`, whatever the
+// result.
 struct TwoFrameScratch {
     StreamScratch sc;
-    PsCamSlots* cur; PsCamSlots* last; mcs_ocam* models; double* mtmc_inv;
+    const PsCamSlots* cur; const PsCamSlots* last; const mcs_ocam* cams; const double* mtmc_inv; const double* sf;
     mcs_keypoint* keys; uint8_t* desc; uint8_t* dmask;      // the last frame in slot order (dmask NULL unless masked)
 };
 
 // Allocates and stages those pieces, zeroes the outputs and gathers the last frame into slot order (without a grid).
-cudaError_t ps_open_two_frames(const PsTwoFrameArgs& a, const bool stage_cur, std::vector<size_t> own, TwoFrameScratch& t, cudaStream_t st) {
+cudaError_t ps_open_two_frames(const PsTwoFrameArgs& a, std::vector<size_t> own, TwoFrameScratch& t, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
-    const size_t db = (size_t)NS * a.dim, b_slots = sizeof(PsCamSlots) * a.n_cams;
+    const size_t db = (size_t)NS * a.dim, k = own.size();
+    own.insert(own.end(), {sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0});
     const bool pose = a.models != nullptr;
-    const size_t k = own.size();
-    own.insert(own.end(), {stage_cur ? b_slots : 0, b_slots, pose ? sizeof(mcs_ocam) * a.n_cams : 0, pose ? 128ull * a.n_cams : 0,
-                           sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0});
-    cudaError_t e = t.sc.alloc(own, st);
+    const std::vector<mcs_ocam> sizes = pose ? std::vector<mcs_ocam>() : cam_sizes(a);
+    cudaError_t e = ps_open(t.sc, own, st, host_in(t.cur, a.cams, a.n_cams), host_in(t.last, a.last, a.n_cams),
+                            host_in(t.cams, pose ? a.models : sizes.data(), a.n_cams), host_in(t.mtmc_inv, a.mtmc_inv, pose ? 16 * a.n_cams : 0),
+                            host_in(t.sf, a.sf, a.n_levels));
     if (e != cudaSuccess) return e;
-    t.cur = t.sc.at<PsCamSlots>(k); t.last = t.sc.at<PsCamSlots>(k + 1);
-    t.models = t.sc.at<mcs_ocam>(k + 2); t.mtmc_inv = t.sc.at<double>(k + 3);
-    t.keys = t.sc.at<mcs_keypoint>(k + 4); t.desc = t.sc.at<uint8_t>(k + 5); t.dmask = a.masked ? t.sc.at<uint8_t>(k + 6) : nullptr;
-    if (stage_cur) e = stage_to_device(a.cams, b_slots, t.cur, st);
-    if (e == cudaSuccess) e = stage_to_device(a.last, b_slots, t.last, st);
-    if (e == cudaSuccess && pose) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, t.models, st);
-    if (e == cudaSuccess && pose) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, t.mtmc_inv, st);
-    if (e == cudaSuccess) e = ps_zero_outputs(a, st);
+    t.keys = t.sc.at<mcs_keypoint>(k); t.desc = t.sc.at<uint8_t>(k + 1); t.dmask = a.masked ? t.sc.at<uint8_t>(k + 2) : nullptr;
+    e = ps_zero_outputs(a, st);
     if (e == cudaSuccess) {
-        ps_gather_kernel<<<(NS + 255) / 256, 256, 0, st>>>(t.last, a.n_cams, a.capacity, a.dim, a.masked, t.keys, nullptr, t.desc, t.dmask);
+        ps_gather_kernel<false><<<(NS + 255) / 256, 256, 0, st>>>(t.last, nullptr, a.n_cams, a.capacity, a.dim, a.masked, t.keys, nullptr, t.desc,
+                                                                  t.dmask);
         e = cudaGetLastError();
     }
     return e;
@@ -1263,10 +1239,17 @@ cudaError_t ps_open_two_frames(const PsTwoFrameArgs& a, const bool stage_cur, st
 }  // namespace
 
 cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st) {
-    const cudaError_t e = ps_zero_outputs(a, st);
+    cudaError_t e = ps_zero_outputs(a, st);
     if (e != cudaSuccess) return e;
-    const MapPointQueries qm{a.n_cams, a.n_points, a.n_levels, a.bad, a.in_view, a.level, a.px, a.py, a.vcos, nullptr, a.th};
-    return ps_search<MCS_RULE_LEVEL_RATIO>(a, qm, a.nnratio, a.mp_desc, a.mp_dmask, nullptr, st);
+    const std::vector<mcs_ocam> sizes = cam_sizes(a);
+    const PsCamSlots* slots; const mcs_ocam* cams; const double* sf;
+    StreamScratch sc;
+    e = ps_open(sc, {}, st, host_in(slots, a.cams, a.n_cams), host_in(cams, sizes.data(), a.n_cams), host_in(sf, a.sf, a.n_levels));
+    if (e == cudaSuccess) {
+        const MapPointQueries qm{a.n_cams, a.n_points, a.n_levels, a.bad, a.in_view, a.level, a.px, a.py, a.vcos, sf, a.th};
+        e = ps_search<MCS_RULE_LEVEL_RATIO>(a, qm, a.nnratio, a.mp_desc, a.mp_dmask, nullptr, slots, cams, nullptr, st);
+    }
+    return sc.release(e);
 }
 
 // The last frame's queries (pl_project_kernel), then the current frame searched under MCS_RULE_BEST with the last frame's
@@ -1274,16 +1257,16 @@ cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st
 cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     TwoFrameScratch t;
-    cudaError_t e = ps_open_two_frames(a, false, {(size_t)NS, 8ull * NS, 8ull * NS}, t, st);      // ok u v
+    cudaError_t e = ps_open_two_frames(a, {(size_t)NS, 8ull * NS, 8ull * NS}, t, st);      // ok u v
     if (e != cudaSuccess) return t.sc.release(e);
     uint8_t* ok = t.sc.at<uint8_t>(0); double* u = t.sc.at<double>(1); double* v = t.sc.at<double>(2);
     const LastProjArgs pa{t.last, a.n_cams, a.capacity, a.n_levels, a.n_points, t.keys, a.last_mp, a.last_outlier, a.bad, a.world_pos,
-                          t.models, t.mtmc_inv, a.masks};
+                          t.cams, t.mtmc_inv, a.masks};
     pl_project_kernel<<<(NS + 255) / 256, 256, 0, st>>>(pa, ok, u, v, a.status);
     e = cudaGetLastError();
     if (e == cudaSuccess) {
-        const LastFrameQueries qm{NS, a.capacity, ok, u, v, t.keys, nullptr, a.th};
-        e = ps_search<MCS_RULE_BEST>(a, qm, 0.0, t.desc, t.dmask, a.last_mp, st);
+        const LastFrameQueries qm{NS, a.capacity, ok, u, v, t.keys, t.sf, a.th};
+        e = ps_search<MCS_RULE_BEST>(a, qm, 0.0, t.desc, t.dmask, a.last_mp, t.cur, t.cams, nullptr, st);
     }
     return t.sc.release(e);
 }
@@ -1293,13 +1276,13 @@ cudaError_t launch_search_by_projection_last(const ProjSearchLastArgs& a, cudaSt
 cudaError_t launch_window_search_device(const WindowSearchDevArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     TwoFrameScratch t;
-    cudaError_t e = ps_open_two_frames(a, true, {}, t, st);
+    cudaError_t e = ps_open_two_frames(a, {}, t, st);
     if (e != cudaSuccess) return t.sc.release(e);
     pw_clear_kernel<<<(NS + 255) / 256, 256, 0, st>>>(t.cur, a.n_cams, a.capacity, a.frame_mp);
     e = cudaGetLastError();
     if (e == cudaSuccess) {
         const WindowQueries qm{NS, a.capacity, a.n_points, a.min_level, a.max_level, t.last, t.keys, a.last_mp, a.bad, nullptr, a.window};
-        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, t.desc, t.dmask, a.last_mp, st);
+        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, t.desc, t.dmask, a.last_mp, t.cur, t.cams, nullptr, st);
     }
     return t.sc.release(e);
 }
@@ -1310,7 +1293,7 @@ cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cud
     const int NS = a.n_cams * a.capacity;
     const size_t NK = (size_t)NS * a.n_cams;
     TwoFrameScratch t;
-    cudaError_t e = ps_open_two_frames(a, true, {(size_t)a.n_points, 4ull * a.n_points, NK, 8 * NK, 8 * NK}, t, st);   // found first ok u v
+    cudaError_t e = ps_open_two_frames(a, {(size_t)a.n_points, 4ull * a.n_points, NK, 8 * NK, 8 * NK}, t, st);   // found first ok u v
     if (e != cudaSuccess) return t.sc.release(e);
     uint8_t* found = t.sc.at<uint8_t>(0); int* first = t.sc.at<int>(1);
     uint8_t* ok = t.sc.at<uint8_t>(2); double* u = t.sc.at<double>(3); double* v = t.sc.at<double>(4);
@@ -1319,14 +1302,14 @@ cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cud
     if (e == cudaSuccess) {
         pf_flag_kernel<<<(NS + 255) / 256, 256, 0, st>>>(t.cur, t.last, a.n_cams, a.capacity, a.n_points, a.frame_mp, a.last_mp, found, first,
                                                          a.status);
-        const FramesProjArgs pa{t.last, a.n_cams, a.capacity, a.n_points, a.last_mp, a.bad, found, first, a.world_pos, t.models, t.mtmc_inv,
+        const FramesProjArgs pa{t.last, a.n_cams, a.capacity, a.n_points, a.last_mp, a.bad, found, first, a.world_pos, t.cams, t.mtmc_inv,
                                 a.masks};
         pf_project_kernel<<<(unsigned)((NK + 255) / 256), 256, 0, st>>>(pa, ok, u, v);
         e = cudaGetLastError();
     }
     if (e == cudaSuccess) {
         const FramesQueries qm{NS, a.n_cams, ok, u, v, t.keys, nullptr, a.window};
-        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, t.desc, t.dmask, a.last_mp, st);
+        e = ps_search<MCS_RULE_RATIO>(a, qm, a.nnratio, t.desc, t.dmask, a.last_mp, t.cur, t.cams, nullptr, st);
     }
     return t.sc.release(e);
 }
@@ -1334,15 +1317,14 @@ cudaError_t launch_search_by_projection_frames(const SearchFramesDevArgs& a, cud
 // SearchForInitialization(F1 = last, F2 = cur): one query per F1 slot below its count, centred on prev, then the ordered walk
 // (pi_walk_kernel) instead of the rounds.
 cudaError_t launch_search_for_initialization(const InitSearchDevArgs& a, cudaStream_t st) {
-    const int NS = a.n_cams * a.capacity;
     TwoFrameScratch t;
-    cudaError_t e = ps_open_two_frames(a, false, {}, t, st);
+    cudaError_t e = ps_open_two_frames(a, {}, t, st);
     if (e != cudaSuccess) return t.sc.release(e);
-    const InitQueries qm{NS, a.capacity, t.last, t.keys, a.prev, nullptr, (double)a.window};
+    const InitQueries qm{a.n_cams * a.capacity, a.capacity, t.last, t.keys, a.prev, nullptr, (double)a.window};
     PsFront fr;
-    e = ps_front(a, qm, t.desc, t.dmask, fr, st);
+    e = ps_front(a, qm, t.cur, t.cams, nullptr, t.desc, t.dmask, fr, st);
     if (e == cudaSuccess && fr.Q > 0) {
-        const InitWalk w{fr.qry, fr.lkey, fr.lslot, fr.lcnt, fr.ctl, t.last, fr.slots, fr.keys, fr.dec, (int*)fr.owner, a.n_cams, a.capacity,
+        const InitWalk w{fr.qry, fr.lkey, fr.lslot, fr.lcnt, fr.ctl, t.last, t.cur, fr.keys, fr.dec, (int*)fr.owner, a.n_cams, a.capacity,
                          a.th_high, a.nnratio, a.matches12, a.prev, a.nmatches};
         const size_t smem = 2ull * a.capacity;              // MD of one camera's F2 slots
         with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
@@ -1359,8 +1341,9 @@ cudaError_t launch_search_for_initialization(const InitSearchDevArgs& a, cudaStr
 }
 
 // Fuse for n_kf key frames: membership pre-filter (fu_qmap / fu_held), the (k, q, c) projections (fu_project), the front end over
-// the n_kf * n_cams images with FuseQueries, the stateless decision (fu_best or fu_first), then a count / scan / fill of the hits
-// in query order.  Scratch beyond the front end's: 4 * n_points + n_kf * n_q bytes for the pre-filter and 33 bytes per entry.
+// the n_kf * n_cams images with the projected queries, the stateless decision (fu_best or fu_first), then a count / scan / fill of
+// the hits in query order.  Scratch beyond the front end's: 4 * n_points + n_kf * n_q bytes for the pre-filter and 33 bytes per
+// entry.
 cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st) {
     const int nk = a.n_kf, nc = a.n_kf_cams, NI = nk * nc;
     const long long QE = (long long)nk * a.n_q * nc;
@@ -1368,39 +1351,34 @@ cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(a.n_hits, 0, 4, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
     if (e != cudaSuccess) return e;
+    std::vector<mcs_ocam> models;            // the camera table of the searched frame's NI images; fu_project reads the first nc
+    for (int k = 0; k < nk; ++k) models.insert(models.end(), a.pts.models, a.pts.models + nc);
+    const PsCamSlots* slots; const int* const* kf_mp; const double* mtmc_inv; const double* ow; const mcs_ocam* cams; const double* sf;
     StreamScratch sc;
-    e = sc.alloc({sizeof(PsCamSlots) * NI, sizeof(int*) * nk, 128ull * NI, 24ull * nk, sizeof(mcs_ocam) * nc, 8ull * a.n_levels,   // staged
-                  4ull * a.n_points, (size_t)nk * a.n_q,                                                                        // qmap held
-                  (size_t)QE, 8ull * QE, 8ull * QE, 4ull * QE, 4ull * QE, 4ull * QE, 4ull * (nb + 1), 4ull * (nb + 1)},         // ok u v level entry dec
-                 st);
-    if (e != cudaSuccess) return e;
-    PsCamSlots* slots = sc.at<PsCamSlots>(0); const int** kf_mp = sc.at<const int*>(1); double* mtmc_inv = sc.at<double>(2);
-    double* ow = sc.at<double>(3); mcs_ocam* models = sc.at<mcs_ocam>(4); double* sf = sc.at<double>(5);
-    int* qmap = sc.at<int>(6); uint8_t* held = sc.at<uint8_t>(7);
-    uint8_t* ok = sc.at<uint8_t>(8); double* u = sc.at<double>(9); double* v = sc.at<double>(10); int* level = sc.at<int>(11);
-    int* entry = sc.at<int>(12); int* dec = sc.at<int>(13); int* bcount = sc.at<int>(14); int* boff = sc.at<int>(15);
-    e = stage_to_device(a.cams, sizeof(PsCamSlots) * NI, slots, st);
-    if (e == cudaSuccess) e = stage_to_device(a.kf_mp, sizeof(int*) * nk, kf_mp, st);
-    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * NI, mtmc_inv, st);
-    if (e == cudaSuccess) e = stage_to_device(a.ow, 24ull * nk, ow, st);
-    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * nc, models, st);
-    if (e == cudaSuccess) e = stage_to_device(a.sf, 8ull * a.n_levels, sf, st);
-    if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(qmap, 0x7F, 4ull * a.n_points, st);     // above every query position
+    e = ps_open(sc, {4ull * a.pts.n_points, (size_t)nk * a.n_q,                                                                    // qmap held
+                     (size_t)QE, 8ull * QE, 8ull * QE, 4ull * QE, 4ull * QE, 4ull * QE, 4ull * (nb + 1), 4ull * (nb + 1)},          // ok u v level entry dec
+                st, host_in(slots, a.cams, NI), host_in(kf_mp, a.kf_mp, nk), host_in(mtmc_inv, a.mtmc_inv, 16 * NI), host_in(ow, a.ow, 3 * nk),
+                host_in(cams, models.data(), NI), host_in(sf, a.sf, a.n_levels));
+    if (e != cudaSuccess) return sc.release(e);
+    int* qmap = sc.at<int>(0); uint8_t* held = sc.at<uint8_t>(1);
+    uint8_t* ok = sc.at<uint8_t>(2); double* u = sc.at<double>(3); double* v = sc.at<double>(4); int* level = sc.at<int>(5);
+    int* entry = sc.at<int>(6); int* dec = sc.at<int>(7); int* bcount = sc.at<int>(8); int* boff = sc.at<int>(9);
+    if (a.pts.n_points > 0) e = cudaMemsetAsync(qmap, 0x7F, 4ull * a.pts.n_points, st);     // above every query position
     if (e == cudaSuccess && nk * a.n_q > 0) e = cudaMemsetAsync(held, 0, (size_t)nk * a.n_q, st);
     if (e != cudaSuccess) return sc.release(e);
     if (a.n_q > 0) {
-        fu_qmap_kernel<<<(a.n_q + 255) / 256, 256, 0, st>>>(a.query_mp, a.n_q, a.n_points, qmap, a.status);
+        fu_qmap_kernel<<<(a.n_q + 255) / 256, 256, 0, st>>>(a.query_mp, a.n_q, a.pts.n_points, qmap, a.status);
         const long long ns = (long long)NI * a.capacity;
-        fu_held_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, st>>>(slots, kf_mp, nk, nc, a.capacity, a.n_q, a.n_points, qmap, held);
-        const FuseProjArgs pa{nk, nc, a.n_q, a.n_points, a.n_levels, a.variant != MCS_FUSE_SIM3, a.query_mp, a.bad, held, qmap, a.world_pos,
-                              a.min_dist, a.max_dist, models, mtmc_inv, ow, a.masks, sf};
+        fu_held_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, st>>>(slots, kf_mp, nk, nc, a.capacity, a.n_q, a.pts.n_points, qmap, held);
+        const FuseProjArgs pa{nk, nc, a.n_q, a.pts.n_points, a.n_levels, a.variant != MCS_FUSE_SIM3, a.query_mp, a.pts.bad, held, qmap,
+                              a.pts.world_pos, a.pts.min_dist, a.pts.max_dist, cams, mtmc_inv, ow, a.pts.masks, sf};
         fu_project_kernel<<<(unsigned)((QE + 255) / 256), 256, 0, st>>>(pa, ok, u, v, level);
         e = cudaGetLastError();
     }
     PsFront fr;
     if (e == cudaSuccess) {
-        const FuseQueries qm{QE, a.n_q, nc, ok, u, v, level, a.query_mp, nullptr, a.th};
-        e = ps_front(a, qm, a.desc, a.dmask, fr, st, slots);      // the slot table the pre-filter already staged
+        const ProjectedQueries<FuseAt> qm{QE, ok, u, v, level, sf, a.th, {a.n_q, nc, a.query_mp}};
+        e = ps_front(a, qm, slots, cams, nullptr, a.pts.desc, a.pts.dmask, fr, st);
         if (e == cudaSuccess && nb > 0) {
             fu_entry_kernel<<<nb, kQbThreads, 0, st>>>(qm, fr.qoff, entry);
             if (a.variant == MCS_FUSE_FIRST) {
@@ -1419,31 +1397,23 @@ cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st) {
     return sc.release(fr.sc.release(e));
 }
 
-// SearchBySim3: per direction the slot projections (s3_project_kernel), the front end over the other key frame with Sim3Queries,
-// Fuse's stateless decision under th_high and the scatter of the decisions to slots; then the mutual check.  The projection and
-// list scratch of direction 1 is reused by direction 2 in stream order.
+// SearchBySim3: per direction the slot projections (s3_project_kernel), the front end over the other key frame with the projected
+// queries, Fuse's stateless decision under th_high and the scatter of the decisions to slots; then the mutual check.  The
+// projection and list scratch of direction 1 is reused by direction 2 in stream order.
 cudaError_t launch_search_by_sim3(const Sim3SearchDevArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity, nb = (NS + kQbTile - 1) / kQbTile;
-    const size_t b_slots = sizeof(PsCamSlots) * a.n_cams;
     static_assert(sizeof(Sim3Xf) == 24 * sizeof(double), "two directions of 24 doubles");
     cudaError_t e = ps_zero_outputs(a, st);
     if (e != cudaSuccess) return e;
+    const PsCamSlots* s1; const PsCamSlots* s2; const mcs_ocam* models; const double* mc_inv; const Sim3Xf* xf; const double* sf;
     StreamScratch sc;
-    e = sc.alloc({b_slots, b_slots, sizeof(mcs_ocam) * a.n_cams, 128ull * a.n_cams, 2 * sizeof(Sim3Xf), 8ull * a.n_levels,   // staged
-                  (size_t)NS, 8ull * NS, 8ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS},                     // ok u v level entry dec b1 b2
-                 st);
-    if (e != cudaSuccess) return e;
-    PsCamSlots* s1 = sc.at<PsCamSlots>(0); PsCamSlots* s2 = sc.at<PsCamSlots>(1); mcs_ocam* models = sc.at<mcs_ocam>(2);
-    double* mc_inv = sc.at<double>(3); Sim3Xf* xf = sc.at<Sim3Xf>(4); double* sf = sc.at<double>(5);
-    uint8_t* ok = sc.at<uint8_t>(6); double* u = sc.at<double>(7); double* v = sc.at<double>(8); int* level = sc.at<int>(9);
-    int* entry = sc.at<int>(10); int* dec = sc.at<int>(11); int* b1 = sc.at<int>(12); int* b2 = sc.at<int>(13);
-    e = stage_to_device(a.kf1, b_slots, s1, st);
-    if (e == cudaSuccess) e = stage_to_device(a.cams, b_slots, s2, st);
-    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
-    if (e == cudaSuccess) e = stage_to_device(a.mc_inv, 128ull * a.n_cams, mc_inv, st);
-    if (e == cudaSuccess) e = stage_to_device(a.xf, 2 * sizeof(Sim3Xf), xf, st);
-    if (e == cudaSuccess) e = stage_to_device(a.sf, 8ull * a.n_levels, sf, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(b1, 0xFF, 4ull * NS, st);        // no decision yet: -1
+    e = ps_open(sc, {(size_t)NS, 8ull * NS, 8ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS}, st,        // ok u v level entry dec b1 b2
+                host_in(s1, a.kf1, a.n_cams), host_in(s2, a.cams, a.n_cams), host_in(models, a.pts.models, a.n_cams),
+                host_in(mc_inv, a.mc_inv, 16 * a.n_cams), host_in(xf, (const Sim3Xf*)a.xf, 2), host_in(sf, a.sf, a.n_levels));
+    if (e != cudaSuccess) return sc.release(e);
+    uint8_t* ok = sc.at<uint8_t>(0); double* u = sc.at<double>(1); double* v = sc.at<double>(2); int* level = sc.at<int>(3);
+    int* entry = sc.at<int>(4); int* dec = sc.at<int>(5); int* b1 = sc.at<int>(6); int* b2 = sc.at<int>(7);
+    e = cudaMemsetAsync(b1, 0xFF, 4ull * NS, st);        // no decision yet: -1
     if (e == cudaSuccess) e = cudaMemsetAsync(b2, 0xFF, 4ull * NS, st);
     int sms = 0;
     if (e == cudaSuccess) e = sm_count(sms);
@@ -1451,15 +1421,14 @@ cudaError_t launch_search_by_sim3(const Sim3SearchDevArgs& a, cudaStream_t st) {
     for (int dir = 0; dir < 2 && e == cudaSuccess; ++dir) {
         const bool one = dir == 0;                           // direction 1: KF1's points into KF2; direction 2: KF2's into KF1
         const int* mp = one ? a.mp1 : a.mp2;
-        const Sim3ProjArgs pa{one ? s1 : s2, a.n_cams, a.capacity, a.n_points, a.n_levels, mp, one ? a.matches12 : nullptr,
-                              one ? nullptr : a.already2, a.bad, a.world_pos, a.min_dist, a.max_dist, models, xf + dir, mc_inv, a.masks, sf};
+        const Sim3ProjArgs pa{one ? s1 : s2, a.n_cams, a.capacity, a.pts.n_points, a.n_levels, mp, one ? a.matches12 : nullptr,
+                              one ? nullptr : a.already2, a.pts.bad, a.pts.world_pos, a.pts.min_dist, a.pts.max_dist, models, xf + dir, mc_inv,
+                              a.pts.masks, sf};
         s3_project_kernel<<<(NS + 255) / 256, 256, 0, st>>>(pa, ok, u, v, level, a.status);
         e = cudaGetLastError();
-        PsFrameArgs fa = a;
-        fa.cams = one ? a.cams : a.kf1;
-        const Sim3Queries qm{NS, a.capacity, ok, u, v, level, mp, nullptr, a.th};
+        const ProjectedQueries<Sim3At> qm{NS, ok, u, v, level, sf, a.th, {a.capacity, mp}};
         PsFront fr;
-        if (e == cudaSuccess) e = ps_front(fa, qm, a.desc, a.dmask, fr, st, one ? s2 : s1);
+        if (e == cudaSuccess) e = ps_front(a, qm, one ? s2 : s1, models, nullptr, a.pts.desc, a.pts.dmask, fr, st);
         if (e == cudaSuccess) {
             fu_entry_kernel<<<nb, kQbThreads, 0, st>>>(qm, fr.qoff, entry);
             fu_best_kernel<<<blocks, 256, 0, st>>>(fr.ctl, fr.lkey, fr.lslot, a.th_high, dec);
@@ -1476,51 +1445,44 @@ cudaError_t launch_search_by_sim3(const Sim3SearchDevArgs& a, cudaStream_t st) {
 }
 
 // SearchByProjection(KF, Scw): the first contiguous ids (scw_first_kernel), spAlreadyFound (scw_found_kernel), the entry projections
-// (scw_project_kernel), then the rounds and the walk under MCS_RULE_SCW over scw_gather_kernel's view, with the map-point ids as
-// the tags (desc_index).
+// (scw_project_kernel), then the rounds and the walk under MCS_RULE_SCW over ps_gather_kernel<true>'s view, with the map-point ids
+// as the tags (desc_index).
 cudaError_t launch_search_by_projection_scw(const ScwSearchDevArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
     cudaError_t e = ps_zero_outputs(a, st);
     if (e != cudaSuccess) return e;
+    const PsCamSlots* slots; const mcs_ocam* models; const double* mtmc_inv; const double* ow; const double* sf;
     StreamScratch sc;
-    e = sc.alloc({sizeof(PsCamSlots) * a.n_cams, sizeof(mcs_ocam) * a.n_cams, 128ull * a.n_cams, 24, 8ull * a.n_levels,   // staged
-                  4ull * (a.n_cams + 1), (size_t)a.n_points,                                                               // first found
-                  (size_t)a.n_q, 8ull * a.n_q, 8ull * a.n_q, 4ull * a.n_q, 4ull * a.n_q},                                  // ok u v level qcam
-                 st);
-    if (e != cudaSuccess) return e;
-    PsCamSlots* slots = sc.at<PsCamSlots>(0); mcs_ocam* models = sc.at<mcs_ocam>(1); double* mtmc_inv = sc.at<double>(2);
-    double* ow = sc.at<double>(3); double* sf = sc.at<double>(4); int* first = sc.at<int>(5); uint8_t* found = sc.at<uint8_t>(6);
-    uint8_t* ok = sc.at<uint8_t>(7); double* u = sc.at<double>(8); double* v = sc.at<double>(9); int* level = sc.at<int>(10);
-    int* qcam = sc.at<int>(11);
-    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, slots, st);
-    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * a.n_cams, models, st);
-    if (e == cudaSuccess) e = stage_to_device(a.mtmc_inv, 128ull * a.n_cams, mtmc_inv, st);
-    if (e == cudaSuccess) e = stage_to_device(a.ow, 24, ow, st);
-    if (e == cudaSuccess) e = stage_to_device(a.sf, 8ull * a.n_levels, sf, st);
-    if (e == cudaSuccess && a.n_points > 0) e = cudaMemsetAsync(found, 0, a.n_points, st);
+    e = ps_open(sc, {4ull * (a.n_cams + 1), (size_t)a.pts.n_points,                                                   // first found
+                     (size_t)a.n_q, 8ull * a.n_q, 8ull * a.n_q, 4ull * a.n_q, 4ull * a.n_q},                          // ok u v level qcam
+                st, host_in(slots, a.cams, a.n_cams), host_in(models, a.pts.models, a.n_cams), host_in(mtmc_inv, a.mtmc_inv, 16 * a.n_cams),
+                host_in(ow, a.ow, 3), host_in(sf, a.sf, a.n_levels));
+    if (e != cudaSuccess) return sc.release(e);
+    int* first = sc.at<int>(0); uint8_t* found = sc.at<uint8_t>(1);
+    uint8_t* ok = sc.at<uint8_t>(2); double* u = sc.at<double>(3); double* v = sc.at<double>(4); int* level = sc.at<int>(5);
+    int* qcam = sc.at<int>(6);
+    if (a.pts.n_points > 0) e = cudaMemsetAsync(found, 0, a.pts.n_points, st);
     if (e != cudaSuccess) return sc.release(e);
     scw_first_kernel<<<1, 1, 0, st>>>(slots, a.n_cams, a.capacity, first);
-    scw_found_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.n_points, a.frame_mp, found);
+    scw_found_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, a.n_cams, a.capacity, a.pts.n_points, a.frame_mp, found);
     if (a.n_q > 0) {
-        const ScwProjArgs pa{a.n_q, a.n_cams, a.n_points, a.n_levels, a.points, a.bad, found, first, a.world_pos, a.min_dist, a.max_dist,
-                             models, mtmc_inv, ow, a.masks, sf};
+        const ScwProjArgs pa{a.n_q, a.n_cams, a.pts.n_points, a.n_levels, a.points, a.pts.bad, found, first, a.pts.world_pos, a.pts.min_dist,
+                             a.pts.max_dist, models, mtmc_inv, ow, a.pts.masks, sf};
         scw_project_kernel<<<(a.n_q + 255) / 256, 256, 0, st>>>(pa, ok, u, v, level, qcam, a.status);
     }
     e = cudaGetLastError();
     if (e == cudaSuccess) {
-        const ScwQueries qm{a.n_q, ok, u, v, level, qcam, a.points, nullptr, (double)a.th};
-        e = ps_search<MCS_RULE_SCW>(a, qm, 0.0, a.desc, a.dmask, nullptr, st, slots, first);
+        const ProjectedQueries<ScwAt> qm{a.n_q, ok, u, v, level, sf, (double)a.th, {qcam, a.points}};
+        e = ps_search<MCS_RULE_SCW>(a, qm, 0.0, a.pts.desc, a.pts.dmask, nullptr, slots, models, first, st);
     }
     return sc.release(e);
 }
 
 cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_cams, int capacity, double* prev, cudaStream_t st) {
     const int NS = n_cams * capacity;
+    const PsCamSlots* slots;
     StreamScratch sc;
-    cudaError_t e = sc.alloc({sizeof(PsCamSlots) * n_cams}, st);
-    if (e != cudaSuccess) return e;
-    PsCamSlots* slots = sc.at<PsCamSlots>(0);
-    e = stage_to_device(f1, sizeof(PsCamSlots) * n_cams, slots, st);
+    cudaError_t e = ps_open(sc, {}, st, host_in(slots, f1, n_cams));
     if (e == cudaSuccess) {
         pi_seed_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, n_cams, capacity, prev);
         e = cudaGetLastError();
