@@ -684,6 +684,50 @@ int  mcs_search_by_projection_scw_device(const mcs_packed_frame* kf, int32_t n_c
                                          int32_t having_masks, int32_t* matched_dev, int32_t* nmatches_dev, int32_t* status_dev,
                                          int32_t* diag_dev, void* stream);
 
+/* ---- map-point tables on the device: cMapPoint::ComputeDistinctiveDescriptors and UpdateNormalAndDepth ------------------------ */
+/* The producer of the map-point tables the device searches read (desc_dev / dmask_dev, normal_dev, min_dist_dev / max_dist_dev):
+ * for every listed point, the reference's methods over its observations, with the key frames in packed feature buffers.
+ * Conventions of the device searches: asynchronous on `stream` (NULL synchronises), every argument checked on the host before any
+ * launch, small host tables staged in stream order, stream-ordered scratch, status on the device, nothing read back.
+ *   kfs [n_kf] host: the key frames the observations name.  frame: either packed layout, several key frames may share a buffer;
+ *   ow: GetCameraCenter(); bad: isBad() (its rows are no descriptor candidates, it still adds its term to the normal).
+ *   scale_factors [n_levels] host (mvScaleFactors).  point_ids_dev [n_upd]: the points to update, repeats allowed (every point
+ *   depends only on its own inputs, so a repeated id writes the same bytes).
+ *   Observations, a CSR indexed by map-point id: obs_offsets_dev [n_points + 1], and per entry obs_kf_dev (index into kfs) and
+ *   obs_slot_dev (c * capacity + j in that key frame).  Entries come in mObservations order -- a std::map keyed by key-frame
+ *   address, so the caller lists the order it wants -- with each key frame's slots adjacent, in AddObservation order.
+ *   ref_kf_dev [n_points] (index into kfs: mpRefKF), bad_dev [n_points] (may be NULL: no point is bad; a bad point is left
+ *   untouched), world_pos_dev [n_points * 3].
+ *   what = MCS_MP_DESCRIPTOR: ComputeDistinctiveDescriptors(having_masks) (ref src/cMapPoint.cpp:294-388).  The rows of the
+ *   non-bad key frames' observations in list order; none: nothing changes; N <= 2: row 0; else the row i < N - 1 whose median
+ *   of its upper part {D(i, j) : j > i} (the element of rank floor((N - 1 - i) / 2)) is strictly smallest, the first on ties.
+ *   D is DescriptorDistance64, or DescriptorDistance64Masked when having_masks.  desc_dev [n_points * dim] receives the row,
+ *   dmask_dev [n_points * dim] its mask only when having_masks (otherwise dmask_dev is neither read nor written).
+ *   what = MCS_MP_NORMAL_DEPTH: UpdateNormalAndDepth() (:449-492).  normal_dev [n_points * 3] = the mean over the listed KEY
+ *   FRAMES (bad ones included) of (X - Ow) / |X - Ow|, with OpenCV's Vec / scalar = multiplication by the rounded reciprocal;
+ *   NaN for a point without observations (0 * (1. / 0)).  level = octave of the ref key frame's first observation, 1 when it
+ *   has none; s = scale_factors[level], dist = |X - Ow_ref|; min_dist_dev = 0.8 * (((1 / s) * dist) / s) and max_dist_dev =
+ *   1.2 * ((s * dist) * scale_factors[n_levels - 1 - level]): GetMin/MaxDistanceInvariance, the values the searches take.
+ *   Only the listed rows of the arrays `what` selects are written; the arrays it does not select may be NULL.
+ *   status_dev [1]: MCS_ERR_INVALID when a listed id is outside [0, n_points), an obs_kf or (MCS_MP_NORMAL_DEPTH) ref_kf index
+ *   is outside [0, n_kf), a slot lies at or beyond its camera's count, a key frame's observations are not adjacent, or the level
+ *   read lies outside [0, n_levels) -- that point is left untouched, the others are unaffected --, MCS_OK otherwise.
+ * capacity <= 65535, dim 16 / 32 / 64. */
+typedef struct mcs_mp_keyframe {
+    mcs_packed_frame frame;   /* the key frame's features, either packed layout */
+    double ow[3];             /* GetCameraCenter() */
+    int32_t bad;              /* isBad(): no descriptor rows, still counted in the normal */
+} mcs_mp_keyframe;
+#define MCS_MP_DESCRIPTOR   1 /* ComputeDistinctiveDescriptors */
+#define MCS_MP_NORMAL_DEPTH 2 /* UpdateNormalAndDepth */
+int  mcs_update_mappoints_device(const mcs_mp_keyframe* kfs, int32_t n_kf, int32_t n_cams, int32_t capacity, int32_t dim,
+                                 int32_t n_levels, const double* scale_factors, int32_t what, int32_t having_masks,
+                                 const int32_t* point_ids_dev, int32_t n_upd, int32_t n_points,
+                                 const int32_t* obs_offsets_dev, const int32_t* obs_kf_dev, const int32_t* obs_slot_dev,
+                                 const int32_t* ref_kf_dev, const uint8_t* bad_dev, const double* world_pos_dev,
+                                 uint8_t* desc_dev, uint8_t* dmask_dev, double* normal_dev, double* min_dist_dev, double* max_dist_dev,
+                                 int32_t* status_dev, void* stream);
+
 /* ---- bag of words: ORBVocabulary::transform and the feature-vector guided search (SURVEY 8f, rank 4) ------- */
 /* The vocabulary tree of DBoW2::TemplatedVocabulary<FORB::TDescriptor, FORB> (ref include/cORBVocabulary.h:34,
  * ThirdParty/DBoW2/DBoW2/TemplatedVocabulary.h) as flat arrays.  Node 0 is the root; parent[0] is ignored.

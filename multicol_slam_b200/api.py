@@ -16,7 +16,7 @@ import pathlib
 import numpy as np
 
 from .ctypes_defs import (MAX_LEVELS, BowFrame, ExtractorInfo, ExtractorParams, FrameView, FuseTarget, KEYPOINT_DTYPE, MapPointDevView,
-                          MapPointView, Ocam, PackedFrame, WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
+                          MapPointView, MpKeyFrame, Ocam, PackedFrame, WINDOW_QUERY_DTYPE, make_ocam, make_params, set_prototypes)
 
 _PKG = pathlib.Path(__file__).resolve().parent
 _LIB_PATH = _PKG / "libmcs_b200.so"
@@ -611,6 +611,159 @@ def search_windows(frame, queries, qdesc, qmask, query_tag, rule, nnratio, thres
     _check(lib().mcs_search_windows(C.byref(fv), _p(queries), len(queries), _p(qdesc), _p(qmask), _p(tags), rule,
                                     C.c_double(nnratio), threshold, _p(assigned), C.byref(n)))
     return n.value, assigned
+
+
+MCS_MP_DESCRIPTOR, MCS_MP_NORMAL_DEPTH = 1, 2
+
+
+def _dist64(a, b, ma=None, mb=None):
+    """DescriptorDistance64 (ma is None) or DescriptorDistance64Masked over two descriptor rows"""
+    x = np.bitwise_xor(a, b)
+    if ma is None:
+        return int(np.unpackbits(x).sum())
+    return (int(np.unpackbits(x & ma).sum()) + int(np.unpackbits(x & mb).sum())) // 2
+
+
+def ComputeDistinctiveDescriptors(obs, kf_desc, kf_bad, having_masks=False, kf_dmask=None, bad=False):
+    """cMapPoint::ComputeDistinctiveDescriptors(havingMasks) (ref src/cMapPoint.cpp:294-388) on one point.  obs: its observations
+    as (k, slot) pairs in mObservations order (each key frame's slots adjacent, in AddObservation order); kf_desc[k] / kf_dmask[k]:
+    key frame k's descriptor rows [n_cams * capacity, dim] u8 by slot (c * capacity + j); kf_bad[k]: isBad().  Returns the
+    position in obs of the row that becomes mDescriptor (and, with having_masks, mDescriptorMask), or None when nothing changes
+    (a bad point, or no row of a non-bad key frame)."""
+    if bad:
+        return None
+    rows = [i for i, (k, _) in enumerate(obs) if not kf_bad[k]]
+    if not rows:
+        return None
+    N = len(rows)
+    if N <= 2:
+        return rows[0]
+
+    def row(i):
+        k, s = obs[rows[i]]
+        return kf_desc[k][s], (kf_dmask[k][s] if having_masks else None)
+    best_median, best = 2**31 - 1, 0
+    for i in range(N - 1):
+        di, mi = row(i)
+        d = sorted(_dist64(di, dj, mi, mj) for dj, mj in (row(j) for j in range(i + 1, N)))
+        median = d[len(d) // 2]                           # misc.h:96-104: nth_element at size / 2
+        if median < best_median:
+            best_median, best = median, i
+    return rows[best]
+
+
+def UpdateNormalAndDepth(obs, kf_ow, ref_kf, world_pos, kf_octave, scale_factors, bad=False):
+    """cMapPoint::UpdateNormalAndDepth() (ref src/cMapPoint.cpp:449-492) followed by GetMin/MaxDistanceInvariance (:494-504) on one
+    point.  obs as for ComputeDistinctiveDescriptors; kf_ow[k]: GetCameraCenter() of key frame k; ref_kf: mpRefKF as an index of
+    the key frames; kf_octave[k][slot]: the keypoint octaves by slot.  Returns (normal [3], 0.8 * mfMinDistance, 1.2 *
+    mfMaxDistance), or None for a bad point.  The arithmetic is the reference's in its order, with OpenCV's Vec / scalar being
+    Vec * (1. / scalar) (core/matx.hpp, Matx_ScaleOp); a point without observations gets the NaN normal 0 * (1. / 0)."""
+    if bad:
+        return None
+    X = [float(v) for v in world_pos]
+    normal, n, prev = [0.0, 0.0, 0.0], 0, None
+    for k, _ in obs:                                      # one term per key frame, bad ones included
+        if k == prev:
+            continue
+        prev = k
+        d = [X[i] - float(kf_ow[k][i]) for i in range(3)]
+        nr = math.sqrt((d[0] * d[0] + d[1] * d[1]) + d[2] * d[2])
+        inv = 1.0 / nr if nr else math.inf
+        normal = [normal[i] + d[i] * inv for i in range(3)]
+        n += 1
+    p = [X[i] - float(kf_ow[ref_kf][i]) for i in range(3)]
+    dist = math.sqrt((p[0] * p[0] + p[1] * p[1]) + p[2] * p[2])
+    level = next((int(kf_octave[k][s]) for k, s in obs if k == ref_kf), 1)
+    sf, nl = [float(v) for v in scale_factors], len(scale_factors)
+    s = sf[level]
+    mn = ((1.0 / s) * dist) / s
+    mx = (s * dist) * sf[nl - 1 - level]
+    inv_n = 1.0 / n if n else math.inf
+    return np.array([v * inv_n for v in normal]), 0.8 * mn, 1.2 * mx
+
+
+def mappoint_obs_csr(obs_lists):
+    """the observation CSR of update_mappoints_device from per-point lists of (k, slot): (offsets [n + 1], obs_kf, obs_slot) int32"""
+    off = np.zeros(len(obs_lists) + 1, np.int32)
+    off[1:] = np.cumsum([len(o) for o in obs_lists])
+    flat = [e for o in obs_lists for e in o]
+    kf = np.array([k for k, _ in flat], np.int32)
+    slot = np.array([s for _, s in flat], np.int32)
+    return off, kf, slot
+
+
+def update_mappoints_host(kf_desc, kf_dmask, kf_octave, kf_ow, kf_bad, n_cams, capacity, kf_counts, scale_factors, point_ids, obs_offsets,
+                          obs_kf, obs_slot, ref_kf, bad, world_pos, desc, dmask, normal, min_dist, max_dist, what=3, having_masks=False):
+    """update_mappoints_device on the host, through ComputeDistinctiveDescriptors / UpdateNormalAndDepth: the same checks, and the
+    same rows of the same numpy arrays written in place.  kf_desc / kf_dmask / kf_octave / kf_ow / kf_bad / kf_counts [n_kf]:
+    each key frame's slot-indexed descriptor rows, masks and octaves, its centre, isBad() and per-camera keypoint counts.
+    Returns the status (MCS_OK or MCS_ERR_INVALID)."""
+    status, n_kf, n_points, nl = MCS_OK, len(kf_ow), len(obs_offsets) - 1, len(scale_factors)
+    for pid in (int(i) for i in point_ids):
+        if not 0 <= pid < n_points:
+            status = MCS_ERR_INVALID
+            continue
+        if bad is not None and bad[pid]:
+            continue
+        o0, o1 = int(obs_offsets[pid]), int(obs_offsets[pid + 1])
+        obs = [(int(obs_kf[e]), int(obs_slot[e])) for e in range(o0, o1)] if 0 <= o0 <= o1 else None
+        ok = obs is not None
+        for e, (k, s) in enumerate(obs or []):
+            ok = ok and 0 <= k < n_kf and 0 <= s < n_cams * capacity and s % capacity < kf_counts[k][s // capacity]
+            ok = ok and not (e > 0 and obs[e - 1][0] != k and any(kk == k for kk, _ in obs[:e - 1]))
+        if ok and what & MCS_MP_NORMAL_DEPTH:
+            ok = 0 <= int(ref_kf[pid]) < n_kf
+            if ok:
+                lv = next((int(kf_octave[k][s]) for k, s in obs if k == int(ref_kf[pid])), 1)
+                ok = 0 <= lv < nl
+        if not ok:
+            status = MCS_ERR_INVALID
+            continue
+        if what & MCS_MP_DESCRIPTOR:
+            b = ComputeDistinctiveDescriptors(obs, kf_desc, kf_bad, having_masks, kf_dmask)
+            if b is not None:
+                k, s = obs[b]
+                desc[pid] = kf_desc[k][s]
+                if having_masks:
+                    dmask[pid] = kf_dmask[k][s]
+        if what & MCS_MP_NORMAL_DEPTH:
+            normal[pid], min_dist[pid], max_dist[pid] = UpdateNormalAndDepth(obs, kf_ow, int(ref_kf[pid]), world_pos[pid], kf_octave,
+                                                                             scale_factors)
+    return status
+
+
+def update_mappoints_device(kfs, n_cams, capacity, scale_factors, point_ids_t, obs_offsets_t, obs_kf_t, obs_slot_t, what=3,
+                            having_masks=False, desc_t=None, dmask_t=None, normal_t=None, min_dist_t=None, max_dist_t=None, ref_kf_t=None,
+                            world_t=None, bad_t=None, dim=None, status=None, stream=None):
+    """mcs_update_mappoints_device: ComputeDistinctiveDescriptors (what & 1) and UpdateNormalAndDepth (what & 2) for the map points
+    point_ids_t lists, writing their rows of the device tables the searches read (see include/mcs_b200.h).  kfs: per key frame
+    (frame, ow, bad) with frame = (packed uint8 cuda tensor, n_parts, part_images, first_image), ow its GetCameraCenter() and bad
+    its isBad().  Cuda tensors: point_ids_t int32 [n_upd]; the observation CSR obs_offsets_t [n_points + 1], obs_kf_t, obs_slot_t
+    int32 (mappoint_obs_csr); desc_t / dmask_t [n_points, dim] u8, normal_t [n_points, 3], min_dist_t / max_dist_t [n_points],
+    world_t [n_points, 3] f64, ref_kf_t int32 and bad_t u8 [n_points] (bad_t may be None).  Asynchronous on `stream`.  Returns the
+    status tensor [1] int32."""
+    import torch
+    dev = point_ids_t.device
+    if status is None:
+        with _on_stream(stream, dev):
+            status = torch.zeros(1, dtype=torch.int32, device=dev)
+    if dim is None:
+        dim = int((desc_t if desc_t is not None else dmask_t).shape[1])
+    # the observation arrays must have an address even when no point has an observation
+    obs_kf_t = obs_kf_t if obs_kf_t.numel() else torch.zeros(1, dtype=torch.int32, device=dev)
+    obs_slot_t = obs_slot_t if obs_slot_t.numel() else torch.zeros(1, dtype=torch.int32, device=dev)
+    ks = (MpKeyFrame * len(kfs))()
+    for t, (frame, ow, bad) in zip(ks, kfs):
+        t.frame = PackedFrame(frame[0].data_ptr(), *frame[1:4])
+        t.ow[:] = [float(x) for x in ow]
+        t.bad = int(bool(bad))
+    sf = np.ascontiguousarray(scale_factors, np.float64)
+    _check(lib().mcs_update_mappoints_device(ks, len(kfs), n_cams, capacity, dim, len(sf), _p(sf), int(what), int(bool(having_masks)),
+                                             _dptr(point_ids_t) if point_ids_t.numel() else None, int(point_ids_t.numel()),
+                                             int(obs_offsets_t.numel()) - 1, _dptr(obs_offsets_t), _dptr(obs_kf_t), _dptr(obs_slot_t),
+                                             _dptr(ref_kf_t), _dptr(bad_t), _dptr(world_t), _dptr(desc_t), _dptr(dmask_t), _dptr(normal_t),
+                                             _dptr(min_dist_t), _dptr(max_dist_t), _dptr(status), _stream_handle(stream, dev)))
+    return status
 
 
 def _queries(cam, x, y, r, min_level, max_level, desc_index):

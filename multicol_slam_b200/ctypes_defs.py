@@ -65,6 +65,11 @@ class FuseTarget(C.Structure):
     _fields_ = [("frame", PackedFrame), ("mp_dev", C.c_void_p), ("mtmc_inv", C.c_void_p), ("ow", C.c_double * 3)]
 
 
+class MpKeyFrame(C.Structure):
+    """mcs_mp_keyframe: a key frame in packed feature buffers, its GetCameraCenter() and isBad()"""
+    _fields_ = [("frame", PackedFrame), ("ow", C.c_double * 3), ("bad", C.c_int32)]
+
+
 def set_prototypes(lib):
     """argument types of the entry points whose many arguments are easiest to get wrong from Python"""
     P, I, D = C.c_void_p, C.c_int32, C.c_double
@@ -92,6 +97,9 @@ def set_prototypes(lib):
     f.restype = C.c_int
     f = lib.mcs_search_by_projection_scw_device
     f.argtypes = [C.POINTER(PackedFrame), I, I, I, P, P, I, P, P, P, P, I, I, P, P, P, P, P, P, I, I, I, P, P, P, P, P]
+    f.restype = C.c_int
+    f = lib.mcs_update_mappoints_device
+    f.argtypes = [C.POINTER(MpKeyFrame), I, I, I, I, I, P, I, I, P, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P]
     f.restype = C.c_int
     f = lib.mcs_vocabulary_level_nodes
     f.argtypes = [P, I, C.POINTER(I)]
