@@ -28,7 +28,11 @@ class RefVocabulary:
         if not self.h:
             raise RuntimeError("reference vocabulary did not load")
         if scoring is not None or weighting is not None:
-            self.lib.refbow_set_types(self.h, int(scoring), int(weighting))
+            self.set_types(scoring, weighting)
+
+    def set_types(self, scoring, weighting):
+        """the scoring and weighting types, without loading the tree again"""
+        self.lib.refbow_set_types(self.h, int(scoring), int(weighting))
 
     def __del__(self):
         if getattr(self, "h", None):

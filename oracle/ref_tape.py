@@ -88,6 +88,8 @@ def _args_key(what, args, kwargs):
             h.update(digest(v).hexdigest.encode())
         elif isinstance(v, _Proxy):
             h.update(v._path.encode())
+        elif isinstance(v, os.PathLike):          # a file's name, not where it lies: recorded in one place, replayed in another
+            h.update(pathlib.PurePath(v).name.encode())
         elif v is None or isinstance(v, (bool, int, float, str, np.integer, np.floating)):
             h.update(repr(v).encode())
         elif isinstance(v, dict):
