@@ -669,6 +669,38 @@ int  mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, i
  *   when an id is >= n_points, or when an entry that reaches the camera look-up lies at or beyond the key frame's keypoint count
  *   (the reference dereferences unordered_map::end() there: undefined); such an entry is dropped, the others are unaffected.
  *   diag_dev (may be NULL): int32[4] as for mcs_search_by_projection_device.  n_q < 2^24 (MCS_ERR_UNSUPPORTED beyond). */
+/* Loop closing's first matcher call, SearchByBoW(mpCurrentKF, pKF, vvpMapPointMatches[i]) (cLoopClosing::ComputeSim3, ref
+ * src/cLoopClosing.cpp:281; src/cORBmatcher.cpp:885-966), for n_kf candidate key frames in one call.  Per candidate k,
+ * independently of the others (n_kf candidates in one call give what n_kf calls with one candidate give):
+ *   Queries: the KF1 slots below each camera's count, in slot order (the reference's contiguous order), whose mp1_dev id is >= 0
+ *   and whose point is not bad.  Database: the slots of kfs[k] below each camera's count whose mp_dev[k] id is >= 0 and not bad.
+ *   Each query takes the best and second-best distance (strict <, in slot order) over the database slots this candidate has not
+ *   yet taken; accepted when best < th_low and (double)best < nnratio * (double)second (second = INT_MAX without one), and the
+ *   slot is then taken for the rest of the candidate's walk.  Distances are DescriptorDistance64 / DescriptorDistance64Masked
+ *   (having_masks) between the packed descriptor rows, dim 16 / 32 / 64.
+ *   matches12_dev [n_kf][n_cams * capacity]: per KF1 slot the map-point id of the candidate slot it matched (vpMapPoints2[bestIdx2]),
+ *   or -1: the matches12_dev row mcs_search_by_sim3_device takes, once the caller's RANSAC has cleared the outliers.
+ *   match_slot_dev (same shape, may be NULL): the candidate slot matched, or -1.  Both are set below each camera's count of KF1;
+ *   slots at or beyond a count are neither read nor written, in any frame.  nmatches_dev [n_kf]: the reference's return value.
+ *   status_dev [1]: MCS_ERR_INVALID when a map-point id is >= n_points -- that slot is dropped, the others are unaffected --,
+ *   MCS_OK otherwise.  bad_dev [n_points] may be NULL.
+ * Conventions of mcs_search_by_bow_device: asynchronous on `stream` (NULL synchronises), every argument checked on the host before
+ * any launch, stream-ordered scratch, nothing read back.  Each frame in either packed layout; KF1 and the candidates may share
+ * buffers, and KF1 may be one of its own candidates.  n_kf = 0 is a successful no-op.
+ * Limits (MCS_ERR_UNSUPPORTED beyond, before any launch): n_cams * capacity <= 1 622 016, the "taken" bits of one candidate's
+ * database held in the shared memory of one acceptance CTA (and below the lists' 21-bit index); n_cams * capacity < 2^24 (the
+ * query bound of the device searches); n_kf * n_cams * capacity < 2^31.  capacity <= 65535.
+ * Scratch, one stream-ordered block: per slot of each of the 1 + n_kf frames, dim bytes of compact descriptors (2 * dim with
+ * having_masks) and 4 of slot map; per (candidate, slot), 32 * splits bytes of partial K-best lists, 64 of merged lists and 4 of
+ * compact matches, with NS = n_cams * capacity and splits <= min(ceil(NS / 256), max(1, ceil(32 * SMs / (ceil(NS / 128) * n_kf))))
+ * database chunks: on a 132-SM device and a config-3 frame (NS = 8 000), 32 chunks (about 1.1 KB per row) for one candidate, 5
+ * for 16.  The limits above bound indices, not memory: near n_kf * NS = 2^31 the scratch would be about 200 GB, and the call
+ * then fails with MCS_ERR_CUDA from the scratch allocation, before any kernel is launched. */
+int  mcs_search_by_bow_keyframes_device(const mcs_packed_frame* kf1, const int32_t* mp1_dev, const mcs_packed_frame* kfs,
+                                        const int32_t* const* mp_dev, int32_t n_kf, int32_t n_cams, int32_t capacity, int32_t dim,
+                                        int32_t n_points, const uint8_t* bad_dev, int32_t th_low, double nnratio, int32_t having_masks,
+                                        int32_t* matches12_dev, int32_t* match_slot_dev, int32_t* nmatches_dev, int32_t* status_dev,
+                                        void* stream);
 int  mcs_search_by_sim3_device(const mcs_packed_frame* kf1, const mcs_packed_frame* kf2, int32_t n_cams, int32_t capacity, int32_t dim,
                                const mcs_ocam* cams, const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, const double* t1w,
                                const double* t2w, const double* mc_inv, double s12, const double* r12, const double* t12, double th,

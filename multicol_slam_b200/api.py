@@ -1473,6 +1473,72 @@ class cORBmatcher:
                                           self.TH_LOW_, C.c_double(self.mfNNratio), _p(m12), C.byref(n)))
         return n.value, m12
 
+    def SearchByBoWKeyFramesDevice(self, kf1, mp1_t, kfs, n_cams, capacity, n_points, bad_t=None, stream=None, out=None):
+        """mcs_search_by_bow_keyframes_device: SearchByBoW(KF1, KF_k, vpMatches12) (ref :885-966) for every loop candidate of
+        ComputeSim3 in one call (see include/mcs_b200.h).  kf1: (packed uint8 cuda tensor, n_parts, part_images, first_image); mp1_t
+        int32 cuda [n_cams * capacity] its map-point ids by slot (-1 none); kfs: [(packed frame, mp_t)] per candidate.  bad_t
+        [n_points] u8 cuda or None.  Asynchronous on `stream`.  Returns (matches12 [n_kf, n_cams * capacity], match_slot (same
+        shape), nmatches [n_kf], status [1]) as int32 cuda tensors: per KF1 slot the candidate's map-point id matched and its slot,
+        -1 = none; slots at or beyond a camera's count are not written."""
+        import torch
+        dev = mp1_t.device
+        nk, ns = len(kfs), n_cams * capacity
+        if out is None:
+            with _on_stream(stream, dev):
+                out = (torch.full((nk, ns), -1, dtype=torch.int32, device=dev), torch.full((nk, ns), -1, dtype=torch.int32, device=dev),
+                       torch.zeros(nk, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev))
+        frames = (PackedFrame * max(nk, 1))(*[PackedFrame(f[0].data_ptr(), *f[1:4]) for f, _ in kfs])
+        mps = (C.c_void_p * max(nk, 1))(*[mp_t.data_ptr() for _, mp_t in kfs])
+        _check(lib().mcs_search_by_bow_keyframes_device(C.byref(PackedFrame(kf1[0].data_ptr(), *kf1[1:4])), _dptr(mp1_t), frames, mps, nk,
+                                                        n_cams, capacity, self.mbFeatDim, n_points, _dptr(bad_t), self.TH_LOW_,
+                                                        C.c_double(self.mfNNratio), int(self.havingMasks), _dptr(out[0]), _dptr(out[1]),
+                                                        _dptr(out[2]), _dptr(out[3]), _stream_handle(stream, dev)))
+        return out
+
+    def SearchByBoWKeyFramesHost(self, kf1, mp1_t, kfs, n_cams, capacity, n_points, bad_t=None, _bf=None):
+        """The host route of SearchByBoWKeyFramesDevice, what a caller does without it: read the frames and map-point rows back,
+        put them in contiguous order (slots_to_contiguous) and call SearchByBoW (mcs_match_bruteforce) once per candidate.  Same
+        arguments; returns (matches12, match_slot, nmatches, status) as numpy arrays of the device call's shapes, with -1 at every
+        slot at or beyond a camera's count.  A map-point id >= n_points makes its keypoint no query / database entry and sets
+        status to MCS_ERR_INVALID.  _bf: another brute-force matcher with oracle_api.match_bruteforce's arguments (the tests'
+        oracle route); the frames may then be CPU tensors."""
+        from . import rig
+        dim, ns = self.mbFeatDim, n_cams * capacity
+        bad = None if bad_t is None else bad_t.cpu().numpy()
+        status = [MCS_OK]
+
+        def frame(f, mp_t):
+            buf = f[0].cpu().numpy()
+            part = rig.packed_layout(f[2], capacity, dim)[1]
+            cams = []
+            for c in range(n_cams):
+                g = f[3] + c
+                cams.append(rig.unpack(buf[(g // f[2]) * part:(g // f[2] + 1) * part], f[2], capacity, dim)[g % f[2]])
+            counts = [len(k) for k, _, _ in cams]
+            mp = slots_to_contiguous(mp_t.cpu().numpy(), counts, capacity)
+            if (mp >= n_points).any():
+                status[0] = MCS_ERR_INVALID
+            ok = (mp >= 0) & (mp < n_points)
+            if bad is not None:
+                ok[ok] = bad[mp[ok]] == 0
+            slots = slots_to_contiguous(np.arange(ns, dtype=np.int32), counts, capacity)
+            return np.concatenate([d for _, d, _ in cams]), np.concatenate([m for _, _, m in cams]), ok.astype(np.uint8), mp, slots, counts
+
+        d1, m1, v1, _, s1, counts1 = frame(kf1, mp1_t)
+        m12 = np.full((len(kfs), ns), -1, np.int32)
+        slot12 = np.full((len(kfs), ns), -1, np.int32)
+        nm = np.zeros(len(kfs), np.int32)
+        for k, (f, mp_t) in enumerate(kfs):
+            d2, m2, v2, mp2, s2, _ = frame(f, mp_t)
+            if _bf is None:
+                nm[k], b = self.SearchByBoW(d1, d2, m1, m2, v1, v2)
+            else:
+                nm[k], b = _bf(d1, d2, self.TH_LOW_, self.mfNNratio, *((m1, m2) if self.havingMasks else (None, None)), v1, v2)
+            hit = b >= 0
+            m12[k, s1[hit]] = mp2[b[hit]]
+            slot12[k, s1[hit]] = s2[b[hit]]
+        return m12, slot12, nm, np.asarray(status, np.int32)
+
     def SearchByBoWFrame(self, desc_kf, featvec_kf, desc_f, featvec_f, mask_kf=None, mask_f=None, valid_kf=None):
         """SearchByBoW(cMultiKeyFrame* pKF, cMultiFrame& F, vpMapPointMatches) (ref src/cORBmatcher.cpp:179-324): matching
         restricted to keypoints that fall into the same vocabulary node.  featvec_* = (nodes, offsets, features) as returned

@@ -288,4 +288,16 @@ struct BowSearchDevArgs {
 };
 cudaError_t launch_search_by_bow_device(const BowSearchDevArgs& a, cudaStream_t st);
 
+// SearchByBoW(KF1, KF_k) for n_kf candidate key frames (mcs_search_by_bow_keyframes_device, match_kernels.cu).  The launcher refuses
+// nothing: the host entry point has checked n_cams * capacity <= bruteforce_max_nd(kTopKMax) and n_kf * n_cams * capacity < 2^31.
+struct BowKfSearchDevArgs {
+    int n_kf, n_cams, capacity, dim, n_points, th_low;
+    double nnratio; bool masked;
+    const PsCamSlots* cams;                                    // host [(1 + n_kf) * n_cams]: KF1's cameras, then each candidate's
+    const int* const* mp;                                      // host [1 + n_kf]: the frames' slot-indexed map-point ids (device)
+    const uint8_t* bad;                                        // device [n_points], may be NULL
+    int* matches12; int* match_slot; int* nmatches; int* status;   // device; match_slot may be NULL
+};
+cudaError_t launch_search_by_bow_keyframes(const BowKfSearchDevArgs& a, cudaStream_t st);
+
 }  // namespace mcs

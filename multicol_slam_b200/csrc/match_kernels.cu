@@ -926,6 +926,174 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
 }
 
 // ------------------------------------------------------------------------------------------------
+// SearchByBoW(KF1, KF_k) for n_kf candidates (ref src/cORBmatcher.cpp:885-966, mcs_search_by_bow_keyframes_device)
+// ------------------------------------------------------------------------------------------------
+// Frame 0 is KF1, frame 1 + k candidate k, NS = n_cams * capacity slots each.  The number of valid slots is known only on the
+// device, so every grid is sized from NS and the kernels read the real counts (nvalid) there.
+//   kk_gather_kernel  one CTA per frame: the valid slots (below the camera's count, map-point id >= 0 and not bad) in slot order,
+//                     compacted into descriptor / mask rows [f][NS] with their slots (c2s) and the number of them (nvalid[f]).
+//   kk_lists_kernel   the K-best lists of every (candidate, KF1 query) pair on the binary tensor cores (bmma_klists), one CTA per
+//                     (candidate, 128 queries, database chunk); topk_merge_kernel merges the chunks' partial lists.
+//   kk_replay_kernel  one CTA per candidate: the reference's ordered walk (replay_core) with the candidate's own "taken" bits, then
+//                     compact indices back to slots and map-point ids.
+// Compaction keeps slot order, so a compact index is the reference's contiguous order among the valid keypoints: ties broken by
+// index in the lists and the rescans are the reference's strict `<` scan order.
+__global__ void __launch_bounds__(1024)
+kk_gather_kernel(const PsCamSlots* __restrict__ cams, const int* const* __restrict__ mp, const int n_cams, const int capacity, const int dim,
+                 const bool masked, const int n_points, const uint8_t* __restrict__ bad, uint8_t* __restrict__ desc, uint8_t* __restrict__ dmask,
+                 int* __restrict__ c2s, int* __restrict__ nvalid, int* __restrict__ status) {
+    __shared__ int s_warp[32];
+    const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int NS = n_cams * capacity, n16 = dim / 16;
+    const PsCamSlots* fc = cams + (size_t)f * n_cams;
+    const int* m = mp[f];
+    const size_t row0 = (size_t)f * NS;
+    int base = 0;
+    for (int s0 = 0; s0 < NS; s0 += 1024) {
+        const int s = s0 + tid, c = s / capacity, j = s - c * capacity;
+        bool ok = false;
+        if (s < NS && j < min(*fc[c].count, capacity)) {
+            const int id = m[s];
+            if (id >= n_points) *status = MCS_ERR_INVALID;            // dropped; the other slots are unaffected
+            else ok = id >= 0 && !(bad && bad[id]);
+        }
+        const unsigned bal = __ballot_sync(0xffffffffu, ok);
+        if (lane == 0) s_warp[warp] = __popc(bal);
+        __syncthreads();
+        int before = 0, total = 0;
+        for (int w = 0; w < 32; ++w) { const int v = s_warp[w]; before += w < warp ? v : 0; total += v; }
+        if (ok) {
+            const size_t r = row0 + base + before + __popc(bal & ((1u << lane) - 1u));
+            c2s[r] = s;
+            const uint4* src = reinterpret_cast<const uint4*>(fc[c].desc + (size_t)j * dim);
+            for (int h = 0; h < n16; ++h) reinterpret_cast<uint4*>(desc + r * dim)[h] = src[h];
+            if (masked) {
+                const uint4* msrc = reinterpret_cast<const uint4*>(fc[c].dmask + (size_t)j * dim);
+                for (int h = 0; h < n16; ++h) reinterpret_cast<uint4*>(dmask + r * dim)[h] = msrc[h];
+            }
+        }
+        base += total;
+        __syncthreads();                                               // s_warp is rewritten by the next chunk
+    }
+    if (tid == 0) nvalid[f] = base;
+}
+
+// CTA x = (candidate k, query block), y = database chunk; part [chunks][n_kf * NS][kTopKMax].  A CTA with no query or no database
+// entry below the device-side counts writes empty partial lists, so that the merge reads defined keys for every row.
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(kTopkThreads, kListMinBlocks<WORDS, MASKED>)
+kk_lists_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const int* __restrict__ nvalid, const int NS,
+                const int qblocks, const int n_rows, const int chunk, const unsigned bound, unsigned* __restrict__ part) {
+    __shared__ __align__(16) BmmaTile<WORDS, MASKED> s;
+    const int k = blockIdx.x / qblocks, qb = (blockIdx.x - k * qblocks) * kTopkThreads;
+    const int nq = nvalid[0], nd = nvalid[1 + k];
+    const int j0 = blockIdx.y * chunk, j1 = min(j0 + chunk, nd);
+    unsigned* o = part + ((size_t)blockIdx.y * n_rows + (size_t)k * NS + qb) * kTopKMax;
+    if (qb >= nq || j0 >= j1) {
+        for (int i = threadIdx.x; i < min(kTopkThreads, NS - qb) * kTopKMax; i += kTopkThreads) o[i] = 0xFFFFFFFFu;
+        return;
+    }
+    const size_t d_row0 = (size_t)(1 + k) * NS;
+    bmma_klists<WORDS, MASKED, kTopKMax, kTopkShift>(desc + (size_t)qb * WORDS, MASKED ? dmask + (size_t)qb * WORDS : nullptr, nq - qb,
+                                                     desc + d_row0 * WORDS, MASKED ? dmask + d_row0 * WORDS : nullptr, nullptr, j0, j1,
+                                                     kTopKMax, min(bound, 0x7FFu), s, [=](int row, int kk, unsigned key) {
+        if (qb + row < NS) o[(size_t)row * kTopKMax + kk] = key;
+    });
+}
+
+// Threads of the acceptance CTA: 512 leaves 128 registers per thread, where replay_core at 1024 spills with 64 (the masked
+// 32- and 64-byte instances); a rescan of a key frame's few thousand valid slots is still a handful of entries per thread.
+constexpr int kKfReplayThreads = 512;
+
+// One CTA per candidate k: its ordered walk over the merged lists [n_kf][NS][kTopKMax] into m12c (compact database indices), then the
+// outputs: -1 for every KF1 slot below its camera's count, the candidate's map-point id and slot for the accepted ones.
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(kKfReplayThreads, 1)
+kk_replay_kernel(const int* __restrict__ list_idx, const int* __restrict__ list_dist, const uint32_t* __restrict__ desc,
+                 const uint32_t* __restrict__ dmask, const int* __restrict__ nvalid, const int* __restrict__ c2s,
+                 const PsCamSlots* __restrict__ kf1, const int* const* __restrict__ mp, const int n_cams, const int capacity,
+                 const int th_low, const double nnratio, int* __restrict__ m12c, int* __restrict__ matches12, int* __restrict__ match_slot,
+                 int* __restrict__ nmatches) {
+    constexpr int K = kTopKMax;
+    extern __shared__ int s_mem[];
+    int* s_li = s_mem;
+    int* s_ld = s_mem + 32 * K;
+    unsigned* s_taken = (unsigned*)(s_mem + 64 * K);
+    __shared__ ReplayShared sh;
+    __shared__ __align__(16) uint32_t s_qc[(MASKED ? 2 : 1) * 32 * WORDS];
+    const int k = blockIdx.x, tid = threadIdx.x, NS = n_cams * capacity;
+    const int nq = nvalid[0], nd = nvalid[1 + k];
+    const size_t o0 = (size_t)k * NS, d_row0 = (size_t)(1 + k) * NS;
+    for (int w = tid; w < (nd + 31) / 32; w += kKfReplayThreads) s_taken[w] = 0u;
+    for (int i = tid; i < nq; i += kKfReplayThreads) m12c[o0 + i] = -1;
+    __syncthreads();
+    const int nm = replay_core<WORDS, MASKED, kKfReplayThreads>(list_idx + o0 * K, list_dist + o0 * K, K, nq, nullptr, desc,
+                                                                MASKED ? dmask : nullptr, desc + d_row0 * WORDS,
+                                                                MASKED ? dmask + d_row0 * WORDS : nullptr, nd, th_low, nnratio, m12c + o0,
+                                                                s_li, s_ld, s_taken, &sh, s_qc);
+    if (tid == 0) nmatches[k] = nm;
+    for (int s = tid; s < NS; s += kKfReplayThreads) {
+        const int c = s / capacity;
+        if (s - c * capacity < min(*kf1[c].count, capacity)) {
+            matches12[o0 + s] = -1;
+            if (match_slot) match_slot[o0 + s] = -1;
+        }
+    }
+    __syncthreads();
+    const int* mpk = mp[1 + k];
+    for (int q = tid; q < nq; q += kKfReplayThreads) {
+        const int b = m12c[o0 + q];
+        if (b < 0) continue;
+        const int s1 = c2s[q], s2 = c2s[d_row0 + b];
+        matches12[o0 + s1] = mpk[s2];
+        if (match_slot) match_slot[o0 + s1] = s2;
+    }
+}
+
+cudaError_t launch_search_by_bow_keyframes(const BowKfSearchDevArgs& a, cudaStream_t st) {
+    constexpr int K = kTopKMax;
+    const int n_fr = a.n_kf + 1, NS = a.n_cams * a.capacity, n_rows = a.n_kf * NS;
+    int sms = 0;
+    cudaError_t e = sm_count(sms);
+    if (e != cudaSuccess) return e;
+    // chunks of the database as launch_hamming_topk cuts them, from the upper bound NS on every frame's valid slots
+    const int qblocks = (NS + kTopkThreads - 1) / kTopkThreads, tiles = (NS + kDbTile - 1) / kDbTile;
+    const long long cta_q = (long long)qblocks * a.n_kf;
+    int splits = (int)std::max(1LL, std::min((long long)tiles, (4LL * sms * 8 + cta_q - 1) / cta_q));
+    const int chunk = ((tiles + splits - 1) / splits) * kDbTile;
+    splits = (NS + chunk - 1) / chunk;
+    const size_t rows = (size_t)n_fr * NS, lists = (size_t)n_rows * K;
+    StreamScratch sc;
+    e = sc.alloc({sizeof(PsCamSlots) * a.n_cams * n_fr, sizeof(int*) * n_fr, rows * a.dim, a.masked ? rows * a.dim : 0, rows * 4,
+                  (size_t)n_fr * 4, (size_t)splits * lists * 4, lists * 4, lists * 4, (size_t)n_rows * 4}, st);
+    if (e != cudaSuccess) return e;
+    PsCamSlots* cams = sc.at<PsCamSlots>(0);
+    const int* const* mp = sc.at<const int*>(1);
+    uint8_t* desc = sc.at<uint8_t>(2); uint8_t* dmask = a.masked ? sc.at<uint8_t>(3) : nullptr;
+    int* c2s = sc.at<int>(4); int* nvalid = sc.at<int>(5);
+    unsigned* part = sc.at<unsigned>(6); int* lidx = sc.at<int>(7); int* ldist = sc.at<int>(8); int* m12c = sc.at<int>(9);
+    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams * n_fr, cams, st);
+    if (e == cudaSuccess) e = stage_to_device(a.mp, sizeof(int*) * n_fr, (void*)mp, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, sizeof(int), st);                  // MCS_OK
+    if (e != cudaSuccess) return sc.release(e);
+    kk_gather_kernel<<<n_fr, 1024, 0, st>>>(cams, mp, a.n_cams, a.capacity, a.dim, a.masked, a.n_points, a.bad, desc, dmask, c2s, nvalid,
+                                            a.status);
+    const size_t smem = bruteforce_replay_smem(K, NS);
+    with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
+        const uint32_t *d32 = (const uint32_t*)desc, *m32 = (const uint32_t*)dmask;
+        kk_lists_kernel<W, M><<<dim3((unsigned)cta_q, splits), kTopkThreads, 0, st>>>(d32, m32, nvalid, NS, qblocks, n_rows, chunk,
+                                                                                      greedy_dist_bound(a.th_low, a.nnratio), part);
+        topk_merge_kernel<<<(n_rows + 127) / 128, 128, 0, st>>>(part, splits, n_rows, K, lidx, ldist);
+        auto* kern = kk_replay_kernel<W, M>;
+        if (smem > 48 * 1024) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e == cudaSuccess)
+            kern<<<a.n_kf, kKfReplayThreads, smem, st>>>(lidx, ldist, d32, m32, nvalid, c2s, cams, mp, a.n_cams, a.capacity, a.th_low, a.nnratio,
+                                                         m12c, a.matches12, a.match_slot, a.nmatches);
+    });
+    return sc.release(e != cudaSuccess ? e : cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------------
 // window search
 // ------------------------------------------------------------------------------------------------
 template <int WORDS, bool MASKED>

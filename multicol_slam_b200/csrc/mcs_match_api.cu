@@ -830,6 +830,42 @@ int mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, in
     return sync_if_null_stream(stream);
 }
 
+int mcs_search_by_bow_keyframes_device(const mcs_packed_frame* kf1, const int32_t* mp1_dev, const mcs_packed_frame* kfs,
+                                       const int32_t* const* mp_dev, int32_t n_kf, int32_t n_cams, int32_t capacity, int32_t dim,
+                                       int32_t n_points, const uint8_t* bad_dev, int32_t th_low, double nnratio, int32_t having_masks,
+                                       int32_t* matches12_dev, int32_t* match_slot_dev, int32_t* nmatches_dev, int32_t* status_dev,
+                                       void* stream) {
+    if (n_kf < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (n_kf == 0) return MCS_OK;
+    if (!kf1 || !mp1_dev || !kfs || !mp_dev || !matches12_dev || !nmatches_dev || !status_dev) return mcs_fail(MCS_ERR_INVALID, "null argument");
+    if (n_points < 0) return mcs_fail(MCS_ERR_INVALID, "bad sizes");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, kf1, nullptr)) return rc;
+    for (int k = 0; k < n_kf; ++k) {
+        if (!packed_frame_ok(&kfs[k], n_cams))
+            return mcs_fail(MCS_ERR_INVALID, "candidate " + std::to_string(k) + ": no buffer, or first_image + n_cams exceeds its images");
+        if (!mp_dev[k]) return mcs_fail(MCS_ERR_INVALID, "candidate " + std::to_string(k) + ": null map-point array");
+    }
+    // one "taken" bit per database slot in the acceptance CTA's shared memory (K-best lists of 8), compact indices in 21 bits
+    const long long ns = (long long)n_cams * capacity;
+    if (ns > bruteforce_max_nd(8)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_cams * capacity above " + std::to_string(bruteforce_max_nd(8)));
+    if (int rc = check_query_bound(ns, "n_cams * capacity must stay below 2^24")) return rc;
+    if (ns * n_kf >= (1LL << 31)) return mcs_fail(MCS_ERR_UNSUPPORTED, "n_kf * n_cams * capacity must stay below 2^31 (split the candidates)");
+    std::vector<PsCamSlots> cams = packed_slots(*kf1, n_cams, capacity, dim);
+    std::vector<const int*> mp(1, mp1_dev);
+    for (int k = 0; k < n_kf; ++k) {
+        const std::vector<PsCamSlots> s = packed_slots(kfs[k], n_cams, capacity, dim);
+        cams.insert(cams.end(), s.begin(), s.end());
+        mp.push_back(mp_dev[k]);
+    }
+    BowKfSearchDevArgs a{};
+    a.n_kf = n_kf; a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.n_points = n_points; a.th_low = th_low;
+    a.nnratio = nnratio; a.masked = having_masks != 0;
+    a.cams = cams.data(); a.mp = mp.data(); a.bad = bad_dev;
+    a.matches12 = matches12_dev; a.match_slot = match_slot_dev; a.nmatches = nmatches_dev; a.status = status_dev;
+    CUDA_CHECK(launch_search_by_bow_keyframes(a, (cudaStream_t)stream));
+    return sync_if_null_stream(stream);
+}
+
 int mcs_search_by_sim3_device(const mcs_packed_frame* kf1, const mcs_packed_frame* kf2, int32_t n_cams, int32_t capacity, int32_t dim,
                               const mcs_ocam* cams, const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, const double* t1w,
                               const double* t2w, const double* mc_inv, double s12, const double* r12, const double* t12, double th,
