@@ -701,6 +701,33 @@ int  mcs_search_by_bow_keyframes_device(const mcs_packed_frame* kf1, const int32
                                         int32_t n_points, const uint8_t* bad_dev, int32_t th_low, double nnratio, int32_t having_masks,
                                         int32_t* matches12_dev, int32_t* match_slot_dev, int32_t* nmatches_dev, int32_t* status_dev,
                                         void* stream);
+/* Local mapping's search, SearchForTriangulationRaw(mpCurrentMultiKeyFrame, pKF2, ...) (cLocalMapping::CreateNewMapPoints, ref
+ * src/cLocalMapping.cpp:226-380; src/cORBmatcher.cpp:968-1107, no rotation check), for ONE neighbour key frame per call:
+ *   Queries: the KF1 slots below each camera's count whose mp1_dev id is -1 (free; any other id is taken, bad or not), in slot order
+ *   (the reference's contiguous order).  Candidates of a query: the free KF2 slots of the SAME camera, below its count, not taken
+ *   by an earlier query of this call, at distance <= th_low (DescriptorDistance64 / DescriptorDistance64Masked with having_masks,
+ *   dim 16 / 32 / 64).  With best the smallest candidate distance, the candidates are walked in (distance, slot) order while
+ *   distance <= 2 * best and the first with CheckDistEpipolarLine(ray1, ray2, E[c][c], epi_thresh) (ref src/misc.cpp:53-69) is
+ *   matched and taken.  Rays are mvKeysRays: cam_img_to_world of the keypoint's float position under cams[c].
+ *   cams [n_cams] and E [n_cams * n_cams * 9] (row-major 3x3 blocks E[c1][c2], the layout of mcs_search_for_triangulation and of
+ *   the settings' essential matrices; only the blocks E[c][c] are read) are host memory.  Cameras may differ in size.
+ *   mp1_dev / mp2_dev: slot-indexed map-point ids [n_cams * capacity].  matches12_dev [n_cams * capacity]: per KF1 slot the KF2
+ *   slot matched, or -1, for every slot below its camera's count; no slot at or beyond a count is read or written, in either frame.
+ *   nmatches_dev [1]: the reference's return value.  diag_dev (may be NULL): int32[2], the queries and the decisions that rescanned
+ *   a camera's database because the K-best lists could not decide them.
+ * The reference's CreateNewMapPoints adds the points it triangulates to KF1 before it searches the next neighbour, which removes
+ * their keypoints from the next call's queries: call once per neighbour and write the new ids into mp1_dev / mp2_dev in between.
+ * Conventions of mcs_search_for_initialization_device: asynchronous on `stream` (NULL synchronises), every argument checked on the
+ * host before any launch, stream-ordered scratch, nothing read back.  Each frame in either packed layout; KF1 and KF2 may share
+ * buffers or be the same frame.
+ * Limits (MCS_ERR_UNSUPPORTED beyond, before any launch): capacity <= 65535 (a camera's rows and "taken" bits in one CTA);
+ * n_cams * capacity < 2^24.  Scratch, one stream-ordered block: per slot of each frame dim bytes of compact descriptors (2 * dim
+ * with having_masks), 24 of ray and 4 of slot map; per KF1 slot 32 * splits + 72 bytes of K-best lists and flags, splits <=
+ * ceil(capacity / 256) database chunks. */
+int  mcs_search_for_triangulation_device(const mcs_packed_frame* kf1, const int32_t* mp1_dev, const mcs_packed_frame* kf2,
+                                         const int32_t* mp2_dev, int32_t n_cams, int32_t capacity, int32_t dim, const mcs_ocam* cams,
+                                         const double* E, double epi_thresh, int32_t th_low, int32_t having_masks,
+                                         int32_t* matches12_dev, int32_t* nmatches_dev, int32_t* diag_dev, void* stream);
 int  mcs_search_by_sim3_device(const mcs_packed_frame* kf1, const mcs_packed_frame* kf2, int32_t n_cams, int32_t capacity, int32_t dim,
                                const mcs_ocam* cams, const uint8_t* masks_dev, int32_t n_levels, const double* scale_factors, const double* t1w,
                                const double* t2w, const double* mc_inv, double s12, const double* r12, const double* t12, double th,

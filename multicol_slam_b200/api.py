@@ -898,6 +898,19 @@ def _packed_pair(cur, last):
     return [C.byref(PackedFrame(f[0].data_ptr(), *f[1:4])) for f in (cur, last)]
 
 
+def _unpack_frame(f, n_cams, capacity, dim):
+    """the (keypoints, descriptors, masks) of each camera of packed frame f = (packed uint8 tensor, n_parts, part_images,
+    first_image), read back to the host"""
+    from . import rig
+    buf = f[0].cpu().numpy()
+    part = rig.packed_layout(f[2], capacity, dim)[1]
+    out = []
+    for c in range(n_cams):
+        g = f[3] + c
+        out.append(rig.unpack(buf[(g // f[2]) * part:(g // f[2] + 1) * part], f[2], capacity, dim)[g % f[2]])
+    return out
+
+
 def _search_outputs(out, diag, stream, dev):
     """(nmatches [1], status [1], diag [4]) int32 cuda tensors, `out` or new, and the call's last four arguments (diag NULL unless asked)"""
     if out is None:
@@ -1460,6 +1473,62 @@ class cORBmatcher:
                                                   len(d2), d1.shape[1], self.TH_LOW_, _p(Em), Em.shape[0], C.c_double(epi_thresh), _p(m12), C.byref(n)))
         return n.value, m12
 
+    def SearchForTriangulationRawDevice(self, kf1, mp1_t, kf2, mp2_t, cams, capacity, E, epi_thresh=1e-2, stream=None, out=None,
+                                        diag=False):
+        """mcs_search_for_triangulation_device: SearchForTriangulationRaw(KF1, KF2, ...) (ref :968-1107) for one neighbour key frame,
+        both frames in packed feature buffers (see include/mcs_b200.h).  kf1 / kf2: (packed uint8 cuda tensor, n_parts, part_images,
+        first_image); mp1_t / mp2_t: int32 cuda [n_cams * capacity] map-point ids by slot, -1 = free; cams: the camera models; E
+        [n_cams, n_cams, 3, 3] host (ComputeE, or the settings' essential matrices).  Asynchronous on `stream`.  Returns (nmatches
+        [1], matches12 [n_cams * capacity]: per KF1 slot the KF2 slot matched or -1, slots at or beyond a count not written), plus
+        diag [2] (queries, rescans) when diag is set, as int32 cuda tensors."""
+        import torch
+        dev = mp1_t.device
+        nc = len(cams)
+        Em = np.ascontiguousarray(E, np.float64)
+        if Em.shape != (nc, nc, 3, 3):
+            raise ValueError(f"E must be [{nc}, {nc}, 3, 3], not {list(Em.shape)}")
+        if out is None:
+            with _on_stream(stream, dev):
+                out = (torch.zeros(1, dtype=torch.int32, device=dev), torch.full((nc * capacity,), -1, dtype=torch.int32, device=dev),
+                       torch.zeros(2, dtype=torch.int32, device=dev))
+        p1, p2 = _packed_pair(kf1, kf2)
+        _check(lib().mcs_search_for_triangulation_device(p1, _dptr(mp1_t), p2, _dptr(mp2_t), nc, capacity, self.mbFeatDim, _ocams(cams),
+                                                         _p(Em), C.c_double(epi_thresh), self.TH_LOW_, int(self.havingMasks),
+                                                         _dptr(out[1]), _dptr(out[0]), _dptr(out[2]) if diag else None,
+                                                         _stream_handle(stream, dev)))
+        return (out[0], out[1]) + ((out[2],) if diag else ())
+
+    def SearchForTriangulationRawHost(self, kf1, mp1_t, kf2, mp2_t, cams, capacity, E, epi_thresh=1e-2, _st=None):
+        """The host route of SearchForTriangulationRawDevice, what a caller does without it: read both frames and map-point rows
+        back, put them in contiguous order (slots_to_contiguous), compute the rays on the host (img_to_world of each keypoint) and
+        call SearchForTriangulationRaw (mcs_search_for_triangulation).  Same arguments; returns (nmatches, matches12) with matches12
+        int32 [n_cams * capacity] as the device call's: the KF2 slot or -1, and -1 at every slot at or beyond a camera's count.
+        _st: another search with oracle_api.search_for_triangulation's arguments (the tests' oracle route); the frames may then be
+        CPU tensors."""
+        nc = len(cams)
+
+        def frame(f, mp_t):
+            per = _unpack_frame(f, nc, capacity, self.mbFeatDim)
+            counts = [len(k) for k, _, _ in per]
+            keys = np.concatenate([k for k, _, _ in per])
+            cam = np.concatenate([np.full(n, c, np.int32) for c, n in enumerate(counts)])
+            rays = np.array([img_to_world(cams[cam[i]], float(k["x"]), float(k["y"])) for i, k in enumerate(keys)], np.float64).reshape(-1, 3)
+            free = (slots_to_contiguous(mp_t.cpu().numpy(), counts, capacity) == -1).astype(np.uint8)
+            slots = slots_to_contiguous(np.arange(nc * capacity, dtype=np.int32), counts, capacity)
+            return (np.concatenate([d for _, d, _ in per]), np.concatenate([m for _, _, m in per]), cam, free, rays), slots
+
+        a1, s1 = frame(kf1, mp1_t)
+        a2, s2 = frame(kf2, mp2_t)
+        if _st is None:
+            n, b = self.SearchForTriangulationRaw(*a1, *a2, E, epi_thresh)
+        else:
+            masks = (lambda m: m) if self.havingMasks else (lambda m: None)
+            n, b = _st(a1[0], masks(a1[1]), *a1[2:], a2[0], masks(a2[1]), *a2[2:], E, self.TH_LOW_, epi_thresh)
+        m12 = np.full(nc * capacity, -1, np.int32)
+        hit = b >= 0
+        m12[s1[hit]] = s2[b[hit]]
+        return int(n), m12
+
     def SearchByBoW(self, desc1, desc2, mask1=None, mask2=None, valid1=None, valid2=None):
         """SearchByBoW(cMultiKeyFrame*, cMultiKeyFrame*, vpMatches12) (ref :885-966): all-pairs scan over the
         map-point-bearing keypoints of two keyframes.  Returns (nmatches, matches12 indices into desc2)."""
@@ -1502,18 +1571,12 @@ class cORBmatcher:
         slot at or beyond a camera's count.  A map-point id >= n_points makes its keypoint no query / database entry and sets
         status to MCS_ERR_INVALID.  _bf: another brute-force matcher with oracle_api.match_bruteforce's arguments (the tests'
         oracle route); the frames may then be CPU tensors."""
-        from . import rig
         dim, ns = self.mbFeatDim, n_cams * capacity
         bad = None if bad_t is None else bad_t.cpu().numpy()
         status = [MCS_OK]
 
         def frame(f, mp_t):
-            buf = f[0].cpu().numpy()
-            part = rig.packed_layout(f[2], capacity, dim)[1]
-            cams = []
-            for c in range(n_cams):
-                g = f[3] + c
-                cams.append(rig.unpack(buf[(g // f[2]) * part:(g // f[2] + 1) * part], f[2], capacity, dim)[g % f[2]])
+            cams = _unpack_frame(f, n_cams, capacity, dim)
             counts = [len(k) for k, _, _ in cams]
             mp = slots_to_contiguous(mp_t.cpu().numpy(), counts, capacity)
             if (mp >= n_points).any():

@@ -65,4 +65,18 @@ MCS_HD void cam_undistort(const mcs_ocam& cam, double px, double py, double s, d
     oy = -y / z * s;
 }
 
+// CheckDistEpipolarLine(ray1, ray2, E12, thresh) (ref src/misc.cpp:53-69).  The cv::Matx products accumulate s = 0; s += a * b in
+// index order; the host search (mcs_search_for_triangulation) and the device one (tr_epi_kernel, tr_walk_kernel) both call this.
+MCS_HD bool cam_epipolar_ok(const double* r1, const double* r2, const double* E, double thresh) {
+    double t[3];                                       // ray2^T * E  (1x3)
+    for (int j = 0; j < 3; ++j) { double s = 0; for (int i = 0; i < 3; ++i) s += r2[i] * E[3 * i + j]; t[j] = s; }
+    double nom = 0; for (int j = 0; j < 3; ++j) nom += t[j] * r1[j];
+    double ex1[3], etx2[3];
+    for (int i = 0; i < 3; ++i) { double s = 0; for (int k = 0; k < 3; ++k) s += E[3 * i + k] * r1[k]; ex1[i] = s; }
+    for (int i = 0; i < 3; ++i) { double s = 0; for (int k = 0; k < 3; ++k) s += E[3 * k + i] * r2[k]; etx2[i] = s; }
+    const double den = ex1[0] * ex1[0] + ex1[1] * ex1[1] + ex1[2] * ex1[2] + etx2[0] * etx2[0] + etx2[1] * etx2[1] + etx2[2] * etx2[2];
+    if (den == 0.0) return false;
+    return (nom * nom) / den < thresh;
+}
+
 }  // namespace mcs

@@ -300,4 +300,17 @@ struct BowKfSearchDevArgs {
 };
 cudaError_t launch_search_by_bow_keyframes(const BowKfSearchDevArgs& a, cudaStream_t st);
 
+// SearchForTriangulationRaw(KF1, KF2) (mcs_search_for_triangulation_device, match_kernels.cu).  The launcher refuses nothing: the host
+// entry point has checked capacity <= 65535 and n_cams * capacity < 2^24.
+struct TriSearchDevArgs {
+    int n_cams, capacity, dim, th_low;
+    bool masked; double epi_thresh;
+    const PsCamSlots* cams;                                    // host [2 * n_cams]: KF1's cameras, then KF2's
+    const int* mp[2];                                          // device, slot-indexed map-point ids of KF1 / KF2 (-1 = free)
+    const mcs_ocam* models;                                    // host [n_cams]
+    const double* E;                                           // host [n_cams][9]: the diagonal blocks E[c][c]
+    int* matches12; int* nmatches; int* diag;                  // device; diag may be NULL
+};
+cudaError_t launch_search_for_triangulation(const TriSearchDevArgs& a, cudaStream_t st);
+
 }  // namespace mcs

@@ -938,10 +938,15 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
 //                     compact indices back to slots and map-point ids.
 // Compaction keeps slot order, so a compact index is the reference's contiguous order among the valid keypoints: ties broken by
 // index in the lists and the rescans are the reference's strict `<` scan order.
+// FREE_ROWS selects the rows of SearchForTriangulationRaw instead (tr_* below): the slots whose map-point id is -1, each row with
+// its bearing ray ([f][NS][3], cam_img_to_world of the keypoint, models [n_cams]), and each camera's first row (seg [f][n_cams + 1],
+// the last entry = nvalid[f]); n_points, bad and status are then unused.
+template <bool FREE_ROWS>
 __global__ void __launch_bounds__(1024)
 kk_gather_kernel(const PsCamSlots* __restrict__ cams, const int* const* __restrict__ mp, const int n_cams, const int capacity, const int dim,
                  const bool masked, const int n_points, const uint8_t* __restrict__ bad, uint8_t* __restrict__ desc, uint8_t* __restrict__ dmask,
-                 int* __restrict__ c2s, int* __restrict__ nvalid, int* __restrict__ status) {
+                 int* __restrict__ c2s, int* __restrict__ nvalid, int* __restrict__ status, const mcs_ocam* __restrict__ models,
+                 double* __restrict__ rays, int* __restrict__ seg) {
     __shared__ int s_warp[32];
     const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int NS = n_cams * capacity, n16 = dim / 16;
@@ -954,7 +959,8 @@ kk_gather_kernel(const PsCamSlots* __restrict__ cams, const int* const* __restri
         bool ok = false;
         if (s < NS && j < min(*fc[c].count, capacity)) {
             const int id = m[s];
-            if (id >= n_points) *status = MCS_ERR_INVALID;            // dropped; the other slots are unaffected
+            if constexpr (FREE_ROWS) ok = id == -1;
+            else if (id >= n_points) *status = MCS_ERR_INVALID;            // dropped; the other slots are unaffected
             else ok = id >= 0 && !(bad && bad[id]);
         }
         const unsigned bal = __ballot_sync(0xffffffffu, ok);
@@ -962,6 +968,9 @@ kk_gather_kernel(const PsCamSlots* __restrict__ cams, const int* const* __restri
         __syncthreads();
         int before = 0, total = 0;
         for (int w = 0; w < 32; ++w) { const int v = s_warp[w]; before += w < warp ? v : 0; total += v; }
+        if constexpr (FREE_ROWS) {
+            if (s < NS && j == 0) seg[(size_t)f * (n_cams + 1) + c] = base + before + __popc(bal & ((1u << lane) - 1u));
+        }
         if (ok) {
             const size_t r = row0 + base + before + __popc(bal & ((1u << lane) - 1u));
             c2s[r] = s;
@@ -971,11 +980,20 @@ kk_gather_kernel(const PsCamSlots* __restrict__ cams, const int* const* __restri
                 const uint4* msrc = reinterpret_cast<const uint4*>(fc[c].dmask + (size_t)j * dim);
                 for (int h = 0; h < n16; ++h) reinterpret_cast<uint4*>(dmask + r * dim)[h] = msrc[h];
             }
+            if constexpr (FREE_ROWS) {                                 // mvKeysRays (ref src/cMultiFrame.cpp:145-151)
+                const mcs_keypoint k = fc[c].kps[j];
+                double x, y, z;
+                cam_img_to_world(models[c], (double)k.x, (double)k.y, x, y, z);
+                rays[3 * r] = x; rays[3 * r + 1] = y; rays[3 * r + 2] = z;
+            }
         }
         base += total;
         __syncthreads();                                               // s_warp is rewritten by the next chunk
     }
-    if (tid == 0) nvalid[f] = base;
+    if (tid == 0) {
+        nvalid[f] = base;
+        if constexpr (FREE_ROWS) seg[(size_t)f * (n_cams + 1) + n_cams] = base;
+    }
 }
 
 // CTA x = (candidate k, query block), y = database chunk; part [chunks][n_kf * NS][kTopKMax].  A CTA with no query or no database
@@ -1076,8 +1094,8 @@ cudaError_t launch_search_by_bow_keyframes(const BowKfSearchDevArgs& a, cudaStre
     if (e == cudaSuccess) e = stage_to_device(a.mp, sizeof(int*) * n_fr, (void*)mp, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, sizeof(int), st);                  // MCS_OK
     if (e != cudaSuccess) return sc.release(e);
-    kk_gather_kernel<<<n_fr, 1024, 0, st>>>(cams, mp, a.n_cams, a.capacity, a.dim, a.masked, a.n_points, a.bad, desc, dmask, c2s, nvalid,
-                                            a.status);
+    kk_gather_kernel<false><<<n_fr, 1024, 0, st>>>(cams, mp, a.n_cams, a.capacity, a.dim, a.masked, a.n_points, a.bad, desc, dmask, c2s,
+                                                   nvalid, a.status, nullptr, nullptr, nullptr);
     const size_t smem = bruteforce_replay_smem(K, NS);
     with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
         const uint32_t *d32 = (const uint32_t*)desc, *m32 = (const uint32_t*)dmask;
@@ -1091,6 +1109,256 @@ cudaError_t launch_search_by_bow_keyframes(const BowKfSearchDevArgs& a, cudaStre
                                                          m12c, a.matches12, a.match_slot, a.nmatches);
     });
     return sc.release(e != cudaSuccess ? e : cudaGetLastError());
+}
+
+// ------------------------------------------------------------------------------------------------
+// SearchForTriangulationRaw(KF1, KF2) (ref src/cORBmatcher.cpp:968-1107, mcs_search_for_triangulation_device)
+// ------------------------------------------------------------------------------------------------
+// Frame 0 is KF1, frame 1 KF2, NS = n_cams * capacity slots each.  A query only sees the keypoints of its own camera, so past the
+// gather everything runs on camera segments: seg[f][c] .. seg[f][c + 1] are camera c's rows of frame f, and a database index is
+// relative to its segment (< capacity <= 65535, inside the lists' and the rescans' 21-bit index).
+//   kk_gather_kernel<true>  one CTA per frame: the free slots (map-point id -1) in slot order, their rays and the segments.
+//   tr_lists_kernel         the K-best (distance, index) lists, distance <= th_low, of every KF1 row against the KF2 rows of its
+//                           camera (bmma_klists), one CTA per (camera, 128 queries, database chunk); topk_merge_kernel merges.
+//   tr_epi_kernel           CheckDistEpipolarLine of every list entry, one thread per (row, entry).
+//   tr_walk_kernel          one CTA per camera: the reference's ordered walk over the camera's queries with the camera's "taken"
+//                           bits, then the KF2 slot of each match into matches12.
+// The reference walks a query's candidates (distance <= th_low, not taken) in (distance, index) order while distance <= 2 * best
+// and takes the first that passes the epipolar test: the winner is the smallest (distance, index) candidate that passes, accepted
+// iff its distance <= 2 * best.  From a list made before any query took anything: best = its first open (untaken) entry, since every
+// entry before it is taken and every key after it or not listed is larger; the winner = its first open entry that passes.  Without
+// one, a list with a -1 entry holds every candidate, so there is none; a full list bounds every key not listed by its last
+// distance dK, so there is none within 2 * best when dK > 2 * best.  Otherwise (a full list with no open entry, or with no open
+// entry that passes and dK <= 2 * best) the query is undecided from its list, and the whole CTA rescans the camera's segment.
+// Compaction keeps slot order, so (distance, index) order inside a camera is the reference's (distance, contiguous index) order.
+constexpr int kTrWalkThreads = 256;          // a camera segment is <= 65535 rows: a rescan is <= 293 rows per scanning thread
+
+struct TriWalkShared {
+    int cmd;                                  // 0 while the walk runs, -1 once it is over
+    int bq;                                   // the rescan's chunk-relative query
+    unsigned k1[kTrWalkThreads / 32], k2[kTrWalkThreads / 32];     // per scanning warp (1 ..): smallest open key, smallest that passes
+};
+
+// CTA x = (camera c, query block), y = database chunk; part [chunks][NS][kTopKMax] by KF1 row.  Each row of a camera's queries is
+// written by every chunk's CTA of its block, as an empty list where the chunk lies beyond the camera's database.
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(kTopkThreads, kListMinBlocks<WORDS, MASKED>)
+tr_lists_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const int* __restrict__ seg, const int n_cams,
+                const int NS, const int qblocks, const int chunk, const unsigned bound, unsigned* __restrict__ part) {
+    __shared__ __align__(16) BmmaTile<WORDS, MASKED> s;
+    const int c = blockIdx.x / qblocks, qb = (blockIdx.x - c * qblocks) * kTopkThreads;
+    const int q_lo = seg[c], nq = seg[c + 1] - q_lo, d_lo = seg[n_cams + 1 + c], nd = seg[n_cams + 2 + c] - d_lo;
+    if (qb >= nq) return;
+    const int j0 = blockIdx.y * chunk, j1 = min(j0 + chunk, nd);
+    unsigned* o = part + ((size_t)blockIdx.y * NS + q_lo + qb) * kTopKMax;
+    if (j0 >= j1) {
+        for (int i = threadIdx.x; i < min(kTopkThreads, nq - qb) * kTopKMax; i += kTopkThreads) o[i] = 0xFFFFFFFFu;
+        return;
+    }
+    const size_t q_row = (size_t)q_lo + qb, d_row = (size_t)NS + d_lo;
+    bmma_klists<WORDS, MASKED, kTopKMax, kTopkShift>(desc + q_row * WORDS, MASKED ? dmask + q_row * WORDS : nullptr, nq - qb,
+                                                     desc + d_row * WORDS, MASKED ? dmask + d_row * WORDS : nullptr, nullptr, j0, j1,
+                                                     kTopKMax, bound, s, [=](int row, int kk, unsigned key) {
+        if (qb + row < nq) o[(size_t)row * kTopKMax + kk] = key;               // the rows past nq are the next camera's
+    });
+}
+
+// flag [NS][kTopKMax]: CheckDistEpipolarLine(ray1, ray2, E[c][c], epi) of KF1 row `row` and its list entry (0 for an empty entry)
+__global__ void tr_epi_kernel(const int* __restrict__ list_idx, const double* __restrict__ rays, const int* __restrict__ seg,
+                              const int* __restrict__ c2s, const int* __restrict__ nvalid, const double* __restrict__ E, const int n_cams,
+                              const int capacity, const double epi, uint8_t* __restrict__ flag) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x, row = i / kTopKMax, NS = n_cams * capacity;
+    if (row >= nvalid[0]) return;
+    const int id = list_idx[i];
+    if (id < 0) { flag[i] = 0; return; }
+    const int c = c2s[row] / capacity;
+    flag[i] = cam_epipolar_ok(rays + (size_t)row * 3, rays + ((size_t)NS + seg[n_cams + 1 + c] + id) * 3, E + 9 * c, epi) ? 1 : 0;
+}
+
+// One pass over this thread's share of the camera's database rows [0, nd) (dd / dm / r2 start at the segment; the scanning warps
+// are warps 1 .. of the CTA) for the query descriptor qd (qm) and ray r1: the smallest key (distance << kKeyShift | index) over the
+// rows not taken with distance <= th_low (k1), and over those that also pass the epipolar test (k2), each reduced over the warp.
+// The test runs only for a key below k2.
+template <int WORDS, bool MASKED>
+__device__ __forceinline__ void tr_scan(const uint32_t* qd, const uint32_t* qmk, const double* r1, const uint32_t* __restrict__ dd,
+                                        const uint32_t* __restrict__ dm, const double* __restrict__ r2, const int nd, const unsigned* s_taken,
+                                        const double* E, const double epi, const int th_low, unsigned& k1, unsigned& k2) {
+    uint32_t qw[WORDS], qm[MASKED ? WORDS : 1];
+#pragma unroll
+    for (int k = 0; k < WORDS; ++k) { qw[k] = qd[k]; if (MASKED) qm[k] = qmk[k]; }
+    const double ray1[3] = {r1[0], r1[1], r1[2]};
+    k1 = 0xFFFFFFFFu; k2 = 0xFFFFFFFFu;
+    for (int id = threadIdx.x - 32; id < nd; id += kTrWalkThreads - 32) {
+        if (s_taken[id >> 5] >> (id & 31) & 1u) continue;
+        const uint4* dp = reinterpret_cast<const uint4*>(dd + (size_t)id * WORDS);
+        const uint4* mp = MASKED ? reinterpret_cast<const uint4*>(dm + (size_t)id * WORDS) : nullptr;
+        uint32_t dw[WORDS], mw[MASKED ? WORDS : 1];
+#pragma unroll
+        for (int k = 0; k < WORDS / 4; ++k) {
+            const uint4 t = dp[k]; dw[4 * k] = t.x; dw[4 * k + 1] = t.y; dw[4 * k + 2] = t.z; dw[4 * k + 3] = t.w;
+            if (MASKED) { const uint4 u = mp[k]; mw[4 * k] = u.x; mw[4 * k + 1] = u.y; mw[4 * k + 2] = u.z; mw[4 * k + 3] = u.w; }
+        }
+        const unsigned dist = hamming_words<WORDS, MASKED>(qw, qm, dw, mw);
+        if ((int)dist > th_low) continue;
+        const unsigned key = (dist << kKeyShift) | (unsigned)id;
+        k1 = min(k1, key);
+        if (key < k2 && cam_epipolar_ok(ray1, r2 + 3 * (size_t)id, E, epi)) k2 = key;
+    }
+    k1 = __reduce_min_sync(0xffffffffu, k1);
+    k2 = __reduce_min_sync(0xffffffffu, k2);
+}
+
+// One CTA per camera c.  Warp 0 walks the camera's queries in order and decides from the lists with the whole warp (lane k holds
+// entry k; ballots give the open and the open passing entries); the other warps sleep on a named barrier and wake only for a
+// rescan, which they alone run: the walk then holds no call of the double division's slow path, whose calling convention would
+// make ptxas spill the walk's state.  Every KF1 slot of the camera below its count gets -1 or the KF2 slot it matched.
+template <int WORDS, bool MASKED>
+__global__ void __launch_bounds__(kTrWalkThreads)
+tr_walk_kernel(const int* __restrict__ list_idx, const int* __restrict__ list_dist, const uint8_t* __restrict__ list_epi,
+               const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const double* __restrict__ rays,
+               const int* __restrict__ seg, const int* __restrict__ c2s, const PsCamSlots* __restrict__ kf1, const double* __restrict__ E,
+               const int n_cams, const int capacity, const int th_low, const double epi, int* __restrict__ matches12,
+               int* __restrict__ nmatches, int* __restrict__ diag) {
+    constexpr int K = kTopKMax, THREADS = kTrWalkThreads;
+    extern __shared__ unsigned s_taken[];                              // [(capacity + 31) / 32]: bit = segment index of KF2
+    __shared__ int s_li[32 * K], s_ld[32 * K];
+    __shared__ uint8_t s_fl[32 * K];
+    __shared__ __align__(16) uint32_t s_qc[(MASKED ? 2 : 1) * 32 * WORDS];   // the chunk's query descriptors (and masks)
+    __shared__ double s_qr[32 * 3], s_E[9];
+    __shared__ TriWalkShared sh;
+    const int c = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, NS = n_cams * capacity;
+    const int q_lo = seg[c], nq = seg[c + 1] - q_lo, d_lo = seg[n_cams + 1 + c], nd = seg[n_cams + 2 + c] - d_lo;
+    const int n1 = min(*kf1[c].count, capacity);
+    for (int j = tid; j < n1; j += THREADS) matches12[(size_t)c * capacity + j] = -1;
+    for (int w = tid; w < (nd + 31) / 32; w += THREADS) s_taken[w] = 0u;
+    if (tid < 9) s_E[tid] = E[9 * c + tid];
+    __syncthreads();
+    const uint32_t* dd = desc + ((size_t)NS + d_lo) * WORDS;
+    const uint32_t* dm = MASKED ? dmask + ((size_t)NS + d_lo) * WORDS : nullptr;
+    const double* r2 = rays + ((size_t)NS + d_lo) * 3;
+    const uint32_t* s_qm = s_qc + (MASKED ? 32 * WORDS : 0);
+    if (warp != 0) {
+        for (;;) {
+            named_bar<THREADS>(1);
+            if (*(volatile int*)&sh.cmd < 0) return;
+            const int b = sh.bq;
+            unsigned k1, k2;
+            tr_scan<WORDS, MASKED>(s_qc + b * WORDS, s_qm + b * WORDS, s_qr + 3 * b, dd, dm, r2, nd, s_taken, s_E, epi, th_low, k1, k2);
+            if (lane == 0) { sh.k1[warp] = k1; sh.k2[warp] = k2; }
+            named_bar<THREADS>(2);
+        }
+    }
+    int nm = 0, rescans = 0;
+    if (lane == 0) sh.cmd = 0;
+    const unsigned kmask = (1u << K) - 1u;
+    for (int q0 = 0; q0 < nq; q0 += 32) {
+        const int nchunk = min(32, nq - q0);
+        const size_t r0 = (size_t)q_lo + q0;
+        for (int i = lane; i < nchunk * K; i += 32) {
+            s_li[i] = list_idx[r0 * K + i];
+            s_ld[i] = list_dist[r0 * K + i];
+            s_fl[i] = list_epi[r0 * K + i];
+        }
+        for (int i = lane; i < nchunk * (WORDS / 4); i += 32) {
+            reinterpret_cast<uint4*>(s_qc)[i] = reinterpret_cast<const uint4*>(desc + r0 * WORDS)[i];
+            if (MASKED) reinterpret_cast<uint4*>(s_qc + 32 * WORDS)[i] = reinterpret_cast<const uint4*>(dmask + r0 * WORDS)[i];
+        }
+        for (int i = lane; i < nchunk * 3; i += 32) s_qr[i] = rays[r0 * 3 + i];
+        __syncwarp();
+        for (int t = 0; t < nchunk; ++t) {
+            //   code 0 no match, 1 match `win`, 2 undecided from the list
+            int code, win;
+            {
+                const int id = lane < K ? s_li[t * K + lane] : -1;
+                const int dl = lane < K ? s_ld[t * K + lane] : 0x7FFFFFFF;
+                const bool open = id >= 0 && !(s_taken[id >> 5] >> (id & 31) & 1u);
+                const unsigned m_valid = __ballot_sync(0xffffffffu, id >= 0);
+                const unsigned m_open = __ballot_sync(0xffffffffu, open);
+                const unsigned m_pass = __ballot_sync(0xffffffffu, open && s_fl[t * K + lane] != 0);
+                const int best = __shfl_sync(0xffffffffu, dl, m_open ? __ffs(m_open) - 1 : 0);
+                const int wl = m_pass ? __ffs(m_pass) - 1 : 0;
+                const int wd = __shfl_sync(0xffffffffu, dl, wl), dK = __shfl_sync(0xffffffffu, dl, K - 1);
+                win = __shfl_sync(0xffffffffu, id, wl);
+                if (m_pass) code = wd <= 2 * best ? 1 : 0;
+                else if (m_valid != kmask) code = 0;                   // the list holds every candidate
+                else if (!m_open) code = 2;
+                else code = dK <= 2 * best ? 2 : 0;
+            }
+            if (code == 2) {
+                // exact rescan of the camera's database: the smallest open key, and the smallest open key that passes
+                if (lane == 0) sh.bq = t;
+                named_bar<THREADS>(1);
+                named_bar<THREADS>(2);
+                const bool w = lane >= 1 && lane < THREADS / 32;
+                const unsigned B = __reduce_min_sync(0xffffffffu, w ? sh.k1[lane] : 0xFFFFFFFFu);
+                const unsigned W = __reduce_min_sync(0xffffffffu, w ? sh.k2[lane] : 0xFFFFFFFFu);
+                code = W != 0xFFFFFFFFu && (W >> kKeyShift) <= 2 * (B >> kKeyShift) ? 1 : 0;
+                win = (int)(W & ((1u << kKeyShift) - 1u));
+                ++rescans;
+            }
+            if (code == 1) {
+                if (lane == 0) {
+                    matches12[c2s[r0 + t]] = c2s[(size_t)NS + d_lo + win];
+                    s_taken[win >> 5] |= 1u << (win & 31);
+                }
+                ++nm;
+            }
+            __syncwarp();
+        }
+    }
+    if (lane == 0) sh.cmd = -1;
+    named_bar<THREADS>(1);
+    if (lane == 0) {
+        atomicAdd(nmatches, nm);
+        if (diag) { atomicAdd(diag, nq); atomicAdd(diag + 1, rescans); }
+    }
+}
+
+cudaError_t launch_search_for_triangulation(const TriSearchDevArgs& a, cudaStream_t st) {
+    constexpr int K = kTopKMax;
+    const int nc = a.n_cams, NS = nc * a.capacity;
+    int sms = 0;
+    cudaError_t e = sm_count(sms);
+    if (e != cudaSuccess) return e;
+    // chunks of a camera's database as launch_hamming_topk cuts them, from the upper bound `capacity` on its free rows
+    const int qblocks = (a.capacity + kTopkThreads - 1) / kTopkThreads, tiles = (a.capacity + kDbTile - 1) / kDbTile;
+    const long long cta_q = (long long)qblocks * nc;
+    int splits = (int)std::max(1LL, std::min((long long)tiles, (4LL * sms * 8 + cta_q - 1) / cta_q));
+    const int chunk = ((tiles + splits - 1) / splits) * kDbTile;
+    splits = (a.capacity + chunk - 1) / chunk;
+    const size_t rows = (size_t)2 * NS, lists = (size_t)NS * K;
+    StreamScratch sc;
+    e = sc.alloc({sizeof(PsCamSlots) * 2 * nc, sizeof(int*) * 2, sizeof(mcs_ocam) * nc, sizeof(double) * 9 * nc, rows * a.dim,
+                  a.masked ? rows * a.dim : 0, rows * 4, 2 * 4, (size_t)2 * (nc + 1) * 4, rows * 24, (size_t)splits * lists * 4, lists * 4,
+                  lists * 4, lists}, st);
+    if (e != cudaSuccess) return e;
+    PsCamSlots* cams = sc.at<PsCamSlots>(0);
+    const int* const* mp = sc.at<const int*>(1);
+    mcs_ocam* models = sc.at<mcs_ocam>(2); double* E = sc.at<double>(3);
+    uint8_t* desc = sc.at<uint8_t>(4); uint8_t* dmask = a.masked ? sc.at<uint8_t>(5) : nullptr;
+    int* c2s = sc.at<int>(6); int* nvalid = sc.at<int>(7); int* seg = sc.at<int>(8); double* rays = sc.at<double>(9);
+    unsigned* part = sc.at<unsigned>(10); int* lidx = sc.at<int>(11); int* ldist = sc.at<int>(12); uint8_t* flag = sc.at<uint8_t>(13);
+    e = stage_to_device(a.cams, sizeof(PsCamSlots) * 2 * nc, cams, st);
+    if (e == cudaSuccess) e = stage_to_device(a.mp, sizeof(int*) * 2, (void*)mp, st);
+    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * nc, models, st);
+    if (e == cudaSuccess) e = stage_to_device(a.E, sizeof(double) * 9 * nc, E, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a.nmatches, 0, sizeof(int), st);
+    if (e == cudaSuccess && a.diag) e = cudaMemsetAsync(a.diag, 0, 2 * sizeof(int), st);
+    if (e != cudaSuccess) return sc.release(e);
+    kk_gather_kernel<true><<<2, 1024, 0, st>>>(cams, mp, nc, a.capacity, a.dim, a.masked, 0, nullptr, desc, dmask, c2s, nvalid, nullptr,
+                                               models, rays, seg);
+    // distances <= th_low are listed (bmma_klists lists those below its bound)
+    const unsigned bound = a.th_low < 0 ? 0u : (unsigned)std::min(a.th_low + 1LL, 0x7FFLL);
+    const size_t smem = (size_t)((a.capacity + 31) / 32) * 4;
+    with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
+        const uint32_t *d32 = (const uint32_t*)desc, *m32 = (const uint32_t*)dmask;
+        tr_lists_kernel<W, M><<<dim3((unsigned)cta_q, splits), kTopkThreads, 0, st>>>(d32, m32, seg, nc, NS, qblocks, chunk, bound, part);
+        topk_merge_kernel<<<(NS + 127) / 128, 128, 0, st>>>(part, splits, NS, K, lidx, ldist);
+        tr_epi_kernel<<<(unsigned)((lists + 255) / 256), 256, 0, st>>>(lidx, rays, seg, c2s, nvalid, E, nc, a.capacity, a.epi_thresh, flag);
+        tr_walk_kernel<W, M><<<nc, kTrWalkThreads, smem, st>>>(lidx, ldist, flag, d32, m32, rays, seg, c2s, cams, E, nc, a.capacity, a.th_low,
+                                                               a.epi_thresh, a.matches12, a.nmatches, a.diag);
+    });
+    return sc.release(cudaGetLastError());
 }
 
 // ------------------------------------------------------------------------------------------------

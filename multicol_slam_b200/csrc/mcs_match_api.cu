@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "api_check.h"
+#include "cam_model.cuh"
 #include "kernels.h"
 #include "dev_scratch.h"
 #include "mcs_common.cuh"
@@ -329,19 +330,6 @@ int mcs_match_bruteforce(const uint8_t* q, const uint8_t* qmask, const uint8_t* 
                            masked ? ddm.as<uint8_t>() : nullptr, valid2, nd, dim, th_low, nnratio, matches12, nmatches, nullptr);
 }
 
-// CheckDistEpipolarLine (ref src/misc.cpp:53-69): cv::Matx products accumulate s = 0; s += a*b in index order
-static bool epipolar_ok(const double* r1, const double* r2, const double* E, double thresh) {
-    double t[3];                                       // ray2^T * E  (1x3)
-    for (int j = 0; j < 3; ++j) { double s = 0; for (int i = 0; i < 3; ++i) s += r2[i] * E[3 * i + j]; t[j] = s; }
-    double nom = 0; for (int j = 0; j < 3; ++j) nom += t[j] * r1[j];
-    double ex1[3], etx2[3];
-    for (int i = 0; i < 3; ++i) { double s = 0; for (int k = 0; k < 3; ++k) s += E[3 * i + k] * r1[k]; ex1[i] = s; }
-    for (int i = 0; i < 3; ++i) { double s = 0; for (int k = 0; k < 3; ++k) s += E[3 * k + i] * r2[k]; etx2[i] = s; }
-    const double den = ex1[0] * ex1[0] + ex1[1] * ex1[1] + ex1[2] * ex1[2] + etx2[0] * etx2[0] + etx2[1] * etx2[1] + etx2[2] * etx2[2];
-    if (den == 0.0) return false;
-    return (nom * nom) / den < thresh;
-}
-
 int mcs_search_for_triangulation(const uint8_t* desc1, const uint8_t* mask1, const int32_t* cam1, const uint8_t* free1,
                                  const double* rays1, int32_t n1, const uint8_t* desc2, const uint8_t* mask2, const int32_t* cam2,
                                  const uint8_t* free2, const double* rays2, int32_t n2, int32_t dim, int32_t th_low, const double* E,
@@ -395,7 +383,7 @@ int mcs_search_for_triangulation(const uint8_t* desc1, const uint8_t* mask1, con
                     if (matched2[idx[e]]) continue;                                       // taken by an earlier query of this pass
                     if (best < 0) { best = dst[e]; dist_th = (int)lrint(2.0 * best); }
                     if (dst[e] > dist_th) { done = true; return false; }
-                    if (epipolar_ok(r1, rays2 + 3 * (size_t)idx[e], Ecc, epi_thresh)) { found = idx[e]; done = true; return false; }
+                    if (cam_epipolar_ok(r1, rays2 + 3 * (size_t)idx[e], Ecc, epi_thresh)) { found = idx[e]; done = true; return false; }
                     skip[idx[e]] = 2; marked.push_back(idx[e]);                           // examined by this query (paging only)
                 }
                 return true;
@@ -863,6 +851,30 @@ int mcs_search_by_bow_keyframes_device(const mcs_packed_frame* kf1, const int32_
     a.cams = cams.data(); a.mp = mp.data(); a.bad = bad_dev;
     a.matches12 = matches12_dev; a.match_slot = match_slot_dev; a.nmatches = nmatches_dev; a.status = status_dev;
     CUDA_CHECK(launch_search_by_bow_keyframes(a, (cudaStream_t)stream));
+    return sync_if_null_stream(stream);
+}
+
+int mcs_search_for_triangulation_device(const mcs_packed_frame* kf1, const int32_t* mp1_dev, const mcs_packed_frame* kf2,
+                                        const int32_t* mp2_dev, int32_t n_cams, int32_t capacity, int32_t dim, const mcs_ocam* cams,
+                                        const double* E, double epi_thresh, int32_t th_low, int32_t having_masks,
+                                        int32_t* matches12_dev, int32_t* nmatches_dev, int32_t* diag_dev, void* stream) {
+    if (!kf1 || !mp1_dev || !kf2 || !mp2_dev || !cams || !E || !matches12_dev || !nmatches_dev)
+        return mcs_fail(MCS_ERR_INVALID, "null argument");
+    // a camera's rows, and the index of a list entry or rescan key inside its segment, fit 16 bits
+    if (capacity > 65535) return mcs_fail(MCS_ERR_UNSUPPORTED, "capacity above 65535");
+    if (int rc = check_packed_frames(n_cams, capacity, dim, kf1, kf2)) return rc;
+    if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
+    std::vector<PsCamSlots> slots = packed_slots(*kf1, n_cams, capacity, dim);
+    const std::vector<PsCamSlots> s2 = packed_slots(*kf2, n_cams, capacity, dim);
+    slots.insert(slots.end(), s2.begin(), s2.end());
+    std::vector<double> e_diag((size_t)n_cams * 9);                  // only E[c][c] is read: a query sees its own camera only
+    for (int c = 0; c < n_cams; ++c) std::memcpy(&e_diag[(size_t)c * 9], E + ((size_t)c * n_cams + c) * 9, 9 * sizeof(double));
+    TriSearchDevArgs a{};
+    a.n_cams = n_cams; a.capacity = capacity; a.dim = dim; a.th_low = th_low;
+    a.masked = having_masks != 0; a.epi_thresh = epi_thresh;
+    a.cams = slots.data(); a.mp[0] = mp1_dev; a.mp[1] = mp2_dev; a.models = cams; a.E = e_diag.data();
+    a.matches12 = matches12_dev; a.nmatches = nmatches_dev; a.diag = diag_dev;
+    CUDA_CHECK(launch_search_for_triangulation(a, (cudaStream_t)stream));
     return sync_if_null_stream(stream);
 }
 

@@ -98,6 +98,9 @@ def set_prototypes(lib):
     f = lib.mcs_search_by_bow_keyframes_device
     f.argtypes = [C.POINTER(PackedFrame), P, C.POINTER(PackedFrame), P, I, I, I, I, I, P, I, D, I, P, P, P, P, P]
     f.restype = C.c_int
+    f = lib.mcs_search_for_triangulation_device
+    f.argtypes = [C.POINTER(PackedFrame), P, C.POINTER(PackedFrame), P, I, I, I, P, P, D, I, I, P, P, P, P]
+    f.restype = C.c_int
     f = lib.mcs_search_by_projection_scw_device
     f.argtypes = [C.POINTER(PackedFrame), I, I, I, P, P, I, P, P, P, P, I, I, P, P, P, P, P, P, I, I, I, P, P, P, P, P]
     f.restype = C.c_int
