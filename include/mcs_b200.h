@@ -261,7 +261,8 @@ int  mcs_descriptor_distance64_masked(const uint64_t* a, const uint64_t* b,
 /* For every query q: the K smallest (distance, index) pairs over the nd database descriptors that
  * are not flagged in db_skip (nd bytes, may be NULL), ordered by (distance, index) ascending.
  * Distances are the reference's bit-level popcounts (masked form when qmask/dmask != NULL).
- * Output: topk_idx[nq*K] (-1 = none), topk_dist[nq*K].  Host buffers.  nd < 2^21 per call (MCS_ERR_UNSUPPORTED beyond: split the database). */
+ * Output: topk_idx[nq*K] (-1 = none), topk_dist[nq*K] (0x7FFFFFFF = none).  Host buffers.  nd < 2^21 per call (MCS_ERR_UNSUPPORTED
+ * beyond: split the database).  nd may be 0 (d must still be a valid address): every query then gets K "none" entries. */
 int  mcs_hamming_topk(const uint8_t* q, const uint8_t* qmask, int32_t nq,
                       const uint8_t* d, const uint8_t* dmask, int32_t nd,
                       const uint8_t* db_skip, int32_t dim, int32_t K,

@@ -911,6 +911,18 @@ def _unpack_frame(f, n_cams, capacity, dim):
     return out
 
 
+def _contiguous_frame(f, mp_t, n_cams, capacity, dim):
+    """packed frame f (see _unpack_frame) read back in the contiguous keypoint order of Frame / cMultiFrame: (keys, descriptors,
+    masks, the camera of each keypoint, the counts per camera, the slot-indexed int32 tensor mp_t in contiguous order, the slot of
+    each contiguous index)"""
+    per = _unpack_frame(f, n_cams, capacity, dim)
+    counts = [len(k) for k, _, _ in per]
+    cam = np.concatenate([np.full(n, c, np.int32) for c, n in enumerate(counts)])
+    return (np.concatenate([k for k, _, _ in per]), np.concatenate([d for _, d, _ in per]), np.concatenate([m for _, _, m in per]), cam,
+            counts, slots_to_contiguous(mp_t.cpu().numpy(), counts, capacity),
+            slots_to_contiguous(np.arange(n_cams * capacity, dtype=np.int32), counts, capacity))
+
+
 def _search_outputs(out, diag, stream, dev):
     """(nmatches [1], status [1], diag [4]) int32 cuda tensors, `out` or new, and the call's last four arguments (diag NULL unless asked)"""
     if out is None:
@@ -1508,14 +1520,9 @@ class cORBmatcher:
         nc = len(cams)
 
         def frame(f, mp_t):
-            per = _unpack_frame(f, nc, capacity, self.mbFeatDim)
-            counts = [len(k) for k, _, _ in per]
-            keys = np.concatenate([k for k, _, _ in per])
-            cam = np.concatenate([np.full(n, c, np.int32) for c, n in enumerate(counts)])
+            keys, d, m, cam, _, mp, slots = _contiguous_frame(f, mp_t, nc, capacity, self.mbFeatDim)
             rays = np.array([img_to_world(cams[cam[i]], float(k["x"]), float(k["y"])) for i, k in enumerate(keys)], np.float64).reshape(-1, 3)
-            free = (slots_to_contiguous(mp_t.cpu().numpy(), counts, capacity) == -1).astype(np.uint8)
-            slots = slots_to_contiguous(np.arange(nc * capacity, dtype=np.int32), counts, capacity)
-            return (np.concatenate([d for _, d, _ in per]), np.concatenate([m for _, _, m in per]), cam, free, rays), slots
+            return (d, m, cam, (mp == -1).astype(np.uint8), rays), slots
 
         a1, s1 = frame(kf1, mp1_t)
         a2, s2 = frame(kf2, mp2_t)
@@ -1576,23 +1583,20 @@ class cORBmatcher:
         status = [MCS_OK]
 
         def frame(f, mp_t):
-            cams = _unpack_frame(f, n_cams, capacity, dim)
-            counts = [len(k) for k, _, _ in cams]
-            mp = slots_to_contiguous(mp_t.cpu().numpy(), counts, capacity)
+            _, d, m, _, _, mp, slots = _contiguous_frame(f, mp_t, n_cams, capacity, dim)
             if (mp >= n_points).any():
                 status[0] = MCS_ERR_INVALID
             ok = (mp >= 0) & (mp < n_points)
             if bad is not None:
                 ok[ok] = bad[mp[ok]] == 0
-            slots = slots_to_contiguous(np.arange(ns, dtype=np.int32), counts, capacity)
-            return np.concatenate([d for _, d, _ in cams]), np.concatenate([m for _, _, m in cams]), ok.astype(np.uint8), mp, slots, counts
+            return d, m, ok.astype(np.uint8), mp, slots
 
-        d1, m1, v1, _, s1, counts1 = frame(kf1, mp1_t)
+        d1, m1, v1, _, s1 = frame(kf1, mp1_t)
         m12 = np.full((len(kfs), ns), -1, np.int32)
         slot12 = np.full((len(kfs), ns), -1, np.int32)
         nm = np.zeros(len(kfs), np.int32)
         for k, (f, mp_t) in enumerate(kfs):
-            d2, m2, v2, mp2, s2, _ = frame(f, mp_t)
+            d2, m2, v2, mp2, s2 = frame(f, mp_t)
             if _bf is None:
                 nm[k], b = self.SearchByBoW(d1, d2, m1, m2, v1, v2)
             else:

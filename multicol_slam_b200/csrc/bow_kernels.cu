@@ -333,17 +333,17 @@ cudaError_t launch_bow_vectors_device(const VocabularyDev& v, const BowVectorsDe
     const int max_tiles = tiles_n > tiles_w ? tiles_n : tiles_w;
     // the three cleared arrays first, in one block
     StreamScratch sc;
-    cudaError_t e = sc.alloc({4ull * v.n_nodes, 4ull * a.n_words, 4ull * n_fill,                       // cnt_node cnt_word fill
-                              sizeof(PsCamSlots) * a.n_cams, 4ull * NS, 8ull * NS, 4ull * a.n_words,   // cams key_node wt word_rep
-                              4ull * NS, 4ull * NS, 16ull * max_tiles},                               // slot_rank unordered tile_sums
-                             st);
-    if (e != cudaSuccess) return e;
+    const PsCamSlots* cams;
+    cudaError_t e = open_scratch(sc, {4ull * v.n_nodes, 4ull * a.n_words, 4ull * n_fill,            // cnt_node cnt_word fill
+                                      4ull * NS, 8ull * NS, 4ull * a.n_words,                     // key_node wt word_rep
+                                      4ull * NS, 4ull * NS, 16ull * max_tiles},                   // slot_rank unordered tile_sums
+                                 st, host_in(cams, a.cams, a.n_cams));
+    if (e != cudaSuccess) return sc.release(e);
     int* cnt_node = sc.at<int>(0); int* cnt_word = sc.at<int>(1); int* fill = sc.at<int>(2);
-    PsCamSlots* cams = sc.at<PsCamSlots>(3); int* key_node = sc.at<int>(4); double* wt = sc.at<double>(5); int* word_rep = sc.at<int>(6);
-    int* slot_rank = sc.at<int>(7); int* unordered = sc.at<int>(8); unsigned long long* tile_sums = sc.at<unsigned long long>(9);
+    int* key_node = sc.at<int>(3); double* wt = sc.at<double>(4); int* word_rep = sc.at<int>(5);
+    int* slot_rank = sc.at<int>(6); int* unordered = sc.at<int>(7); unsigned long long* tile_sums = sc.at<unsigned long long>(8);
     e = cudaMemsetAsync(cnt_node, 0, sc.at<uint8_t>(3) - sc.at<uint8_t>(0), st);
     if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, 4, st);
-    if (e == cudaSuccess) e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams, cams, st);
     if (e == cudaSuccess) {
         const BvKeys nodes{cnt_node, v.n_nodes, a.fv_nodes, a.fv_offsets, a.n_fv, a.max_nodes};
         const BvKeys words{cnt_word, a.n_words, a.bow_words, nullptr, a.n_bow, NS};
@@ -499,16 +499,11 @@ __global__ void __launch_bounds__(256) bs_search_kernel(const BowSearchDev a) {
 
 cudaError_t launch_search_by_bow_device(const BowSearchDevArgs& a, cudaStream_t st) {
     const int NS = a.n_cams * a.capacity;
-    const size_t b_kf = sizeof(PsCamSlots) * a.n_cams * (size_t)a.n_kf, b_cur = sizeof(PsCamSlots) * a.n_cams, b_fv = sizeof(BowFrameDev) * a.n_kf;
-    StreamScratch sc;
-    cudaError_t e = sc.alloc({b_kf, b_cur, b_fv}, st);
-    if (e != cudaSuccess) return e;
-    PsCamSlots* kf_cams = sc.at<PsCamSlots>(0); PsCamSlots* cur_cams = sc.at<PsCamSlots>(1); BowFrameDev* kfs = sc.at<BowFrameDev>(2);
-    BowSearchDev d{a.n_kf, a.n_cams, a.capacity, a.max_nodes, a.n_points, a.th_low, a.nnratio, kf_cams, cur_cams, kfs, a.cur,
+    BowSearchDev d{a.n_kf, a.n_cams, a.capacity, a.max_nodes, a.n_points, a.th_low, a.nnratio, nullptr, nullptr, nullptr, a.cur,
                    a.bad, a.match_mp, a.match_slot, a.nmatches, a.status};
-    e = stage_to_device(a.kf_cams, b_kf, kf_cams, st);
-    if (e == cudaSuccess) e = stage_to_device(a.cur_cams, b_cur, cur_cams, st);
-    if (e == cudaSuccess) e = stage_to_device(a.kfs, b_fv, kfs, st);
+    StreamScratch sc;
+    cudaError_t e = open_scratch(sc, {}, st, host_in(d.kf_cams, a.kf_cams, (size_t)a.n_cams * a.n_kf), host_in(d.cur_cams, a.cur_cams, a.n_cams),
+                                 host_in(d.kfs, a.kfs, a.n_kf));
     if (e == cudaSuccess) {
         const long long cells = (long long)a.n_kf * NS, items = (long long)a.n_kf * a.max_nodes;
         bs_clear_kernel<<<(unsigned)((cells + 255) / 256), 256, 0, st>>>(d);

@@ -94,6 +94,27 @@ private:
     cudaStream_t st_ = nullptr;
 };
 
+// Copies small host data into device memory in stream order through kernel parameters, so that the calling thread never waits
+// for the stream (a cudaMemcpyAsync from pageable memory may).  Defined in proj_search_kernels.cu.
+cudaError_t stage_to_device(const void* host, size_t bytes, void* dev, cudaStream_t st);
+
+// One small host input of a launcher: n elements at `host`, staged into the launcher's scratch; `dev` receives the device copy.
+template <class T> struct HostIn { const T*& dev; const T* host; size_t n; };
+template <class T> HostIn<T> host_in(const T*& dev, const T* host, size_t n) { return {dev, host, n}; }
+
+// A launcher's one stream-ordered scratch block: its own pieces first (own[i] is sc.at<T>(i)), then a device copy of every host
+// input, staged in stream order.  The caller releases sc, whatever the result.
+template <class... T>
+cudaError_t open_scratch(StreamScratch& sc, std::vector<size_t> own, cudaStream_t st, const HostIn<T>&... in) {
+    size_t i = own.size();
+    (own.push_back(sizeof(T) * in.n), ...);
+    cudaError_t e = sc.alloc(own, st);
+    if (e != cudaSuccess) return e;
+    ((in.dev = sc.at<T>(i++)), ...);
+    ((e = e == cudaSuccess ? stage_to_device(in.host, sizeof(T) * in.n, (void*)in.dev, st) : e), ...);
+    return e;
+}
+
 inline unsigned greedy_dist_bound(int th_low, double nnratio) {
     if (th_low <= 0) return 0u;                      // nothing can be accepted
     long b = th_low;
@@ -145,9 +166,6 @@ cudaError_t launch_frustum(int n_cams, const double* mtmc_inv, const double* mtm
                            cudaStream_t st);
 
 // device-resident SearchByProjection (proj_search_kernels.cu)
-// Copies small host data into device memory in stream order through kernel parameters, so that the calling thread never waits
-// for the stream (a cudaMemcpyAsync from pageable memory may).
-cudaError_t stage_to_device(const void* host, size_t bytes, void* dev, cudaStream_t st);
 struct PsCamSlots {                     // camera c of the frame: its image slot inside the packed feature buffer
     const int* count; const mcs_keypoint* kps; const uint8_t* desc; const uint8_t* dmask;
 };

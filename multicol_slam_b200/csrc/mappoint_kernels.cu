@@ -222,18 +222,12 @@ __global__ void __launch_bounds__(32 * kMpWarps) mp_update_kernel(const MpDev a)
 cudaError_t launch_update_mappoints(const MpUpdateArgs& a, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(a.status, 0, 4, st);
     if (e != cudaSuccess || a.n_upd == 0) return e;
-    const size_t NI = (size_t)a.n_kf * a.n_cams;
-    const size_t b_slots = sizeof(PsCamSlots) * NI, b_bad = 4ull * a.n_kf, b_ow = 24ull * a.n_kf, b_sf = 8ull * a.n_levels;
-    StreamScratch sc;
-    e = sc.alloc({b_slots, b_bad, b_ow, b_sf}, st);
-    if (e != cudaSuccess) return sc.release(e);
-    MpDev d{a.n_kf, a.n_cams, a.capacity, a.n_levels, a.what, sc.at<PsCamSlots>(0), sc.at<int>(1), sc.at<double>(2), sc.at<double>(3),
+    MpDev d{a.n_kf, a.n_cams, a.capacity, a.n_levels, a.what, nullptr, nullptr, nullptr, nullptr,
             a.ids, a.n_upd, a.n_points, a.obs_off, a.obs_kf, a.obs_slot, a.ref_kf, a.bad, a.world_pos,
             a.desc, a.dmask, a.normal, a.min_dist, a.max_dist, a.status};
-    e = stage_to_device(a.slots, b_slots, (void*)d.slots, st);
-    if (e == cudaSuccess) e = stage_to_device(a.kf_bad, b_bad, (void*)d.kf_bad, st);
-    if (e == cudaSuccess) e = stage_to_device(a.kf_ow, b_ow, (void*)d.kf_ow, st);
-    if (e == cudaSuccess) e = stage_to_device(a.sf, b_sf, (void*)d.sf, st);
+    StreamScratch sc;
+    e = open_scratch(sc, {}, st, host_in(d.slots, a.slots, (size_t)a.n_kf * a.n_cams), host_in(d.kf_bad, a.kf_bad, a.n_kf),
+                     host_in(d.kf_ow, a.kf_ow, 3 * (size_t)a.n_kf), host_in(d.sf, a.sf, a.n_levels));
     if (e == cudaSuccess) {
         const unsigned blocks = (unsigned)((a.n_upd + kMpWarps - 1) / kMpWarps);
         with_desc_width(a.dim, a.masked, [&](auto W, auto M) {

@@ -413,6 +413,16 @@ __global__ void topk_merge_kernel(const unsigned* __restrict__ part, const int s
     }
 }
 
+// The database chunks of the K-best list kernels for cta_q CTAs of queries and a database of at most n_db entries: enough CTAs for
+// ~4 waves, chunks a multiple of the tile, and `splits` chunks cover n_db.  An empty database is one empty chunk.
+struct ListPlan { int chunk, splits; };
+ListPlan list_plan(const int sms, const long long cta_q, const int n_db) {
+    const int tiles = (n_db + kDbTile - 1) / kDbTile;
+    const int splits = (int)std::max(1LL, std::min((long long)tiles, (4LL * sms * 8 + cta_q - 1) / cta_q));
+    const int chunk = std::max(1, (tiles + splits - 1) / splits) * kDbTile;
+    return {chunk, std::max(1, (n_db + chunk - 1) / chunk)};
+}
+
 cudaError_t launch_hamming_topk(const uint8_t* q, const uint8_t* qmask, int nq, const uint8_t* d, const uint8_t* dmask,
                                 int nd, const uint8_t* db_skip, int dim, int K, unsigned bound, int* topk_idx, int* topk_dist,
                                 cudaStream_t st) {
@@ -422,27 +432,22 @@ cudaError_t launch_hamming_topk(const uint8_t* q, const uint8_t* qmask, int nq, 
     int sms = 0;
     cudaError_t e = sm_count(sms);
     if (e != cudaSuccess) return e;
-    // enough CTAs for ~4 waves; database chunks are multiples of the tile
-    int splits = (4 * sms * 8 + qblocks - 1) / qblocks;
-    const int tiles = (nd + kDbTile - 1) / kDbTile;
-    splits = max(1, min(splits, tiles));
-    const int chunk = ((tiles + splits - 1) / splits) * kDbTile;
-    splits = max(1, (nd + chunk - 1) / chunk);
+    const ListPlan pl = list_plan(sms, qblocks, nd);
     // partial top-K lists of the database splits: stream-ordered scratch owned by THIS call, so that concurrent callers -- the
     // reference runs its matchers from three threads -- and different streams never share it
     StreamScratch sc;
-    e = sc.alloc({(size_t)splits * nq * kTopKMax * sizeof(unsigned)}, st);
+    e = sc.alloc({(size_t)pl.splits * nq * kTopKMax * sizeof(unsigned)}, st);
     if (e != cudaSuccess) return e;
     unsigned* part = sc.at<unsigned>(0);
-    dim3 grid(qblocks, splits);
+    dim3 grid(qblocks, pl.splits);
     const bool masked = qmask && dmask;
     with_desc_width(dim, masked, [&](auto W, auto M) {
         with_list_len(K, [&](auto KT) {
             hamming_topk_kernel<W, M, KT><<<grid, kTopkThreads, 0, st>>>((const uint32_t*)q, (const uint32_t*)qmask, nq, (const uint32_t*)d,
-                                                                         (const uint32_t*)dmask, nd, db_skip, K, chunk, bound, part);
+                                                                         (const uint32_t*)dmask, nd, db_skip, K, pl.chunk, bound, part);
         });
     });
-    topk_merge_kernel<<<(nq + 127) / 128, 128, 0, st>>>(part, splits, nq, K, topk_idx, topk_dist);
+    topk_merge_kernel<<<(nq + 127) / 128, 128, 0, st>>>(part, pl.splits, nq, K, topk_idx, topk_dist);
     return sc.release(cudaGetLastError());                   // frees after the merge in stream order
 }
 
@@ -932,8 +937,8 @@ cudaError_t launch_bruteforce_replay(const int* list_idx, const int* list_dist, 
 // device, so every grid is sized from NS and the kernels read the real counts (nvalid) there.
 //   kk_gather_kernel  one CTA per frame: the valid slots (below the camera's count, map-point id >= 0 and not bad) in slot order,
 //                     compacted into descriptor / mask rows [f][NS] with their slots (c2s) and the number of them (nvalid[f]).
-//   kk_lists_kernel   the K-best lists of every (candidate, KF1 query) pair on the binary tensor cores (bmma_klists), one CTA per
-//                     (candidate, 128 queries, database chunk); topk_merge_kernel merges the chunks' partial lists.
+//   seg_lists_kernel<KfSegs>  the K-best lists of every (candidate, KF1 query) pair on the binary tensor cores (bmma_klists), one
+//                     CTA per (candidate, 128 queries, database chunk); topk_merge_kernel merges the chunks' partial lists.
 //   kk_replay_kernel  one CTA per candidate: the reference's ordered walk (replay_core) with the candidate's own "taken" bits, then
 //                     compact indices back to slots and map-point ids.
 // Compaction keeps slot order, so a compact index is the reference's contiguous order among the valid keypoints: ties broken by
@@ -996,28 +1001,44 @@ kk_gather_kernel(const PsCamSlots* __restrict__ cams, const int* const* __restri
     }
 }
 
-// CTA x = (candidate k, query block), y = database chunk; part [chunks][n_kf * NS][kTopKMax].  A CTA with no query or no database
-// entry below the device-side counts writes empty partial lists, so that the merge reads defined keys for every row.
-template <int WORDS, bool MASKED>
+// The rows segment g of a segmented list kernel reads and writes: queries q_row .. q_row + nq - 1 and database entries
+// d_row .. d_row + nd - 1 of the gathered descriptors, partial-list rows o_row .. o_row + n_out - 1 (n_out >= nq): rows past nq
+// get empty lists.  Row numbers fit an int: the entry points keep every search's gathered rows below 2^31.
+struct SegRows { int q_row, nq, d_row, nd, o_row, n_out; };
+
+// CTA x = (segment g, query block), y = database chunk; part [chunks][part_rows][kTopKMax].  Seg maps g to its SegRows on the device.
+// Every chunk's CTA of a block writes the block's rows below n_out, as empty lists where it has no query or no database entry, so that
+// the merge reads defined keys for every such row.  Distances are listed below `bound`, clamped to the keys' 11-bit distance field.
+template <class Seg, int WORDS, bool MASKED>
 __global__ void __launch_bounds__(kTopkThreads, kListMinBlocks<WORDS, MASKED>)
-kk_lists_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const int* __restrict__ nvalid, const int NS,
-                const int qblocks, const int n_rows, const int chunk, const unsigned bound, unsigned* __restrict__ part) {
+seg_lists_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const Seg seg, const int qblocks,
+                 const size_t part_rows, const int chunk, const unsigned bound, unsigned* __restrict__ part) {
     __shared__ __align__(16) BmmaTile<WORDS, MASKED> s;
-    const int k = blockIdx.x / qblocks, qb = (blockIdx.x - k * qblocks) * kTopkThreads;
-    const int nq = nvalid[0], nd = nvalid[1 + k];
-    const int j0 = blockIdx.y * chunk, j1 = min(j0 + chunk, nd);
-    unsigned* o = part + ((size_t)blockIdx.y * n_rows + (size_t)k * NS + qb) * kTopKMax;
-    if (qb >= nq || j0 >= j1) {
-        for (int i = threadIdx.x; i < min(kTopkThreads, NS - qb) * kTopKMax; i += kTopkThreads) o[i] = 0xFFFFFFFFu;
+    const int g = blockIdx.x / qblocks, qb = (blockIdx.x - g * qblocks) * kTopkThreads;
+    const SegRows r = seg(g);
+    if (qb >= r.n_out) return;
+    const int j0 = blockIdx.y * chunk, j1 = min(j0 + chunk, r.nd);
+    unsigned* o = part + (blockIdx.y * part_rows + (size_t)r.o_row + qb) * kTopKMax;
+    if (qb >= r.nq || j0 >= j1) {
+        for (int i = threadIdx.x; i < min(kTopkThreads, r.n_out - qb) * kTopKMax; i += kTopkThreads) o[i] = 0xFFFFFFFFu;
         return;
     }
-    const size_t d_row0 = (size_t)(1 + k) * NS;
-    bmma_klists<WORDS, MASKED, kTopKMax, kTopkShift>(desc + (size_t)qb * WORDS, MASKED ? dmask + (size_t)qb * WORDS : nullptr, nq - qb,
-                                                     desc + d_row0 * WORDS, MASKED ? dmask + d_row0 * WORDS : nullptr, nullptr, j0, j1,
+    const size_t q_row = (size_t)r.q_row + qb, d_row = r.d_row;
+    bmma_klists<WORDS, MASKED, kTopKMax, kTopkShift>(desc + q_row * WORDS, MASKED ? dmask + q_row * WORDS : nullptr, r.nq - qb,
+                                                     desc + d_row * WORDS, MASKED ? dmask + d_row * WORDS : nullptr, nullptr, j0, j1,
                                                      kTopKMax, min(bound, 0x7FFu), s, [=](int row, int kk, unsigned key) {
-        if (qb + row < NS) o[(size_t)row * kTopKMax + kk] = key;
+        if (qb + row < r.n_out) o[(size_t)row * kTopKMax + kk] = key;
     });
 }
+
+// SearchByBoW(KF1, KF_k): segment k lists frame 0's valid rows against frame 1 + k's (counts nvalid), into rows k * NS .. of part;
+// every one of the NS rows is written.
+struct KfSegs {
+    const int* nvalid; int NS;
+    __device__ SegRows operator()(const int k) const {
+        return {0, nvalid[0], (1 + k) * NS, nvalid[1 + k], k * NS, NS};
+    }
+};
 
 // Threads of the acceptance CTA: 512 leaves 128 registers per thread, where replay_core at 1024 spills with 64 (the masked
 // 32- and 64-byte instances); a rescan of a key frame's few thousand valid slots is still a handful of entries per thread.
@@ -1074,34 +1095,30 @@ cudaError_t launch_search_by_bow_keyframes(const BowKfSearchDevArgs& a, cudaStre
     int sms = 0;
     cudaError_t e = sm_count(sms);
     if (e != cudaSuccess) return e;
-    // chunks of the database as launch_hamming_topk cuts them, from the upper bound NS on every frame's valid slots
-    const int qblocks = (NS + kTopkThreads - 1) / kTopkThreads, tiles = (NS + kDbTile - 1) / kDbTile;
+    // chunks of the database from the upper bound NS on every frame's valid slots
+    const int qblocks = (NS + kTopkThreads - 1) / kTopkThreads;
     const long long cta_q = (long long)qblocks * a.n_kf;
-    int splits = (int)std::max(1LL, std::min((long long)tiles, (4LL * sms * 8 + cta_q - 1) / cta_q));
-    const int chunk = ((tiles + splits - 1) / splits) * kDbTile;
-    splits = (NS + chunk - 1) / chunk;
+    const ListPlan pl = list_plan(sms, cta_q, NS);
     const size_t rows = (size_t)n_fr * NS, lists = (size_t)n_rows * K;
     StreamScratch sc;
-    e = sc.alloc({sizeof(PsCamSlots) * a.n_cams * n_fr, sizeof(int*) * n_fr, rows * a.dim, a.masked ? rows * a.dim : 0, rows * 4,
-                  (size_t)n_fr * 4, (size_t)splits * lists * 4, lists * 4, lists * 4, (size_t)n_rows * 4}, st);
-    if (e != cudaSuccess) return e;
-    PsCamSlots* cams = sc.at<PsCamSlots>(0);
-    const int* const* mp = sc.at<const int*>(1);
-    uint8_t* desc = sc.at<uint8_t>(2); uint8_t* dmask = a.masked ? sc.at<uint8_t>(3) : nullptr;
-    int* c2s = sc.at<int>(4); int* nvalid = sc.at<int>(5);
-    unsigned* part = sc.at<unsigned>(6); int* lidx = sc.at<int>(7); int* ldist = sc.at<int>(8); int* m12c = sc.at<int>(9);
-    e = stage_to_device(a.cams, sizeof(PsCamSlots) * a.n_cams * n_fr, cams, st);
-    if (e == cudaSuccess) e = stage_to_device(a.mp, sizeof(int*) * n_fr, (void*)mp, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a.status, 0, sizeof(int), st);                  // MCS_OK
+    const PsCamSlots* cams;
+    const int* const* mp;
+    e = open_scratch(sc, {rows * a.dim, a.masked ? rows * a.dim : 0, rows * 4, (size_t)n_fr * 4, (size_t)pl.splits * lists * 4, lists * 4,
+                          lists * 4, (size_t)n_rows * 4}, st, host_in(cams, a.cams, (size_t)a.n_cams * n_fr), host_in(mp, a.mp, n_fr));
+    if (e != cudaSuccess) return sc.release(e);
+    uint8_t* desc = sc.at<uint8_t>(0); uint8_t* dmask = a.masked ? sc.at<uint8_t>(1) : nullptr;
+    int* c2s = sc.at<int>(2); int* nvalid = sc.at<int>(3);
+    unsigned* part = sc.at<unsigned>(4); int* lidx = sc.at<int>(5); int* ldist = sc.at<int>(6); int* m12c = sc.at<int>(7);
+    e = cudaMemsetAsync(a.status, 0, sizeof(int), st);                                      // MCS_OK
     if (e != cudaSuccess) return sc.release(e);
     kk_gather_kernel<false><<<n_fr, 1024, 0, st>>>(cams, mp, a.n_cams, a.capacity, a.dim, a.masked, a.n_points, a.bad, desc, dmask, c2s,
                                                    nvalid, a.status, nullptr, nullptr, nullptr);
     const size_t smem = bruteforce_replay_smem(K, NS);
     with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
         const uint32_t *d32 = (const uint32_t*)desc, *m32 = (const uint32_t*)dmask;
-        kk_lists_kernel<W, M><<<dim3((unsigned)cta_q, splits), kTopkThreads, 0, st>>>(d32, m32, nvalid, NS, qblocks, n_rows, chunk,
-                                                                                      greedy_dist_bound(a.th_low, a.nnratio), part);
-        topk_merge_kernel<<<(n_rows + 127) / 128, 128, 0, st>>>(part, splits, n_rows, K, lidx, ldist);
+        seg_lists_kernel<KfSegs, W, M><<<dim3((unsigned)cta_q, pl.splits), kTopkThreads, 0, st>>>(
+            d32, m32, KfSegs{nvalid, NS}, qblocks, (size_t)n_rows, pl.chunk, greedy_dist_bound(a.th_low, a.nnratio), part);
+        topk_merge_kernel<<<(n_rows + 127) / 128, 128, 0, st>>>(part, pl.splits, n_rows, K, lidx, ldist);
         auto* kern = kk_replay_kernel<W, M>;
         if (smem > 48 * 1024) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e == cudaSuccess)
@@ -1118,8 +1135,8 @@ cudaError_t launch_search_by_bow_keyframes(const BowKfSearchDevArgs& a, cudaStre
 // gather everything runs on camera segments: seg[f][c] .. seg[f][c + 1] are camera c's rows of frame f, and a database index is
 // relative to its segment (< capacity <= 65535, inside the lists' and the rescans' 21-bit index).
 //   kk_gather_kernel<true>  one CTA per frame: the free slots (map-point id -1) in slot order, their rays and the segments.
-//   tr_lists_kernel         the K-best (distance, index) lists, distance <= th_low, of every KF1 row against the KF2 rows of its
-//                           camera (bmma_klists), one CTA per (camera, 128 queries, database chunk); topk_merge_kernel merges.
+//   seg_lists_kernel<CamSegs>  the K-best (distance, index) lists, distance <= th_low, of every KF1 row against the KF2 rows of
+//                           its camera (bmma_klists), one CTA per (camera, 128 queries, database chunk); topk_merge_kernel merges.
 //   tr_epi_kernel           CheckDistEpipolarLine of every list entry, one thread per (row, entry).
 //   tr_walk_kernel          one CTA per camera: the reference's ordered walk over the camera's queries with the camera's "taken"
 //                           bits, then the KF2 slot of each match into matches12.
@@ -1139,29 +1156,15 @@ struct TriWalkShared {
     unsigned k1[kTrWalkThreads / 32], k2[kTrWalkThreads / 32];     // per scanning warp (1 ..): smallest open key, smallest that passes
 };
 
-// CTA x = (camera c, query block), y = database chunk; part [chunks][NS][kTopKMax] by KF1 row.  Each row of a camera's queries is
-// written by every chunk's CTA of its block, as an empty list where the chunk lies beyond the camera's database.
-template <int WORDS, bool MASKED>
-__global__ void __launch_bounds__(kTopkThreads, kListMinBlocks<WORDS, MASKED>)
-tr_lists_kernel(const uint32_t* __restrict__ desc, const uint32_t* __restrict__ dmask, const int* __restrict__ seg, const int n_cams,
-                const int NS, const int qblocks, const int chunk, const unsigned bound, unsigned* __restrict__ part) {
-    __shared__ __align__(16) BmmaTile<WORDS, MASKED> s;
-    const int c = blockIdx.x / qblocks, qb = (blockIdx.x - c * qblocks) * kTopkThreads;
-    const int q_lo = seg[c], nq = seg[c + 1] - q_lo, d_lo = seg[n_cams + 1 + c], nd = seg[n_cams + 2 + c] - d_lo;
-    if (qb >= nq) return;
-    const int j0 = blockIdx.y * chunk, j1 = min(j0 + chunk, nd);
-    unsigned* o = part + ((size_t)blockIdx.y * NS + q_lo + qb) * kTopKMax;
-    if (j0 >= j1) {
-        for (int i = threadIdx.x; i < min(kTopkThreads, nq - qb) * kTopKMax; i += kTopkThreads) o[i] = 0xFFFFFFFFu;
-        return;
+// Camera segment c lists KF1's rows of camera c against KF2's, into the same rows of part [chunks][NS][kTopKMax]; the rows past
+// its queries are the next camera's, so n_out = nq.
+struct CamSegs {
+    const int* seg; int n_cams, NS;
+    __device__ SegRows operator()(const int c) const {
+        const int q_lo = seg[c], nq = seg[c + 1] - q_lo, d_lo = seg[n_cams + 1 + c];
+        return {q_lo, nq, NS + d_lo, seg[n_cams + 2 + c] - d_lo, q_lo, nq};
     }
-    const size_t q_row = (size_t)q_lo + qb, d_row = (size_t)NS + d_lo;
-    bmma_klists<WORDS, MASKED, kTopKMax, kTopkShift>(desc + q_row * WORDS, MASKED ? dmask + q_row * WORDS : nullptr, nq - qb,
-                                                     desc + d_row * WORDS, MASKED ? dmask + d_row * WORDS : nullptr, nullptr, j0, j1,
-                                                     kTopKMax, bound, s, [=](int row, int kk, unsigned key) {
-        if (qb + row < nq) o[(size_t)row * kTopKMax + kk] = key;               // the rows past nq are the next camera's
-    });
-}
+};
 
 // flag [NS][kTopKMax]: CheckDistEpipolarLine(ray1, ray2, E[c][c], epi) of KF1 row `row` and its list entry (0 for an empty entry)
 __global__ void tr_epi_kernel(const int* __restrict__ list_idx, const double* __restrict__ rays, const int* __restrict__ seg,
@@ -1320,40 +1323,36 @@ cudaError_t launch_search_for_triangulation(const TriSearchDevArgs& a, cudaStrea
     int sms = 0;
     cudaError_t e = sm_count(sms);
     if (e != cudaSuccess) return e;
-    // chunks of a camera's database as launch_hamming_topk cuts them, from the upper bound `capacity` on its free rows
-    const int qblocks = (a.capacity + kTopkThreads - 1) / kTopkThreads, tiles = (a.capacity + kDbTile - 1) / kDbTile;
+    // chunks of a camera's database from the upper bound `capacity` on its free rows
+    const int qblocks = (a.capacity + kTopkThreads - 1) / kTopkThreads;
     const long long cta_q = (long long)qblocks * nc;
-    int splits = (int)std::max(1LL, std::min((long long)tiles, (4LL * sms * 8 + cta_q - 1) / cta_q));
-    const int chunk = ((tiles + splits - 1) / splits) * kDbTile;
-    splits = (a.capacity + chunk - 1) / chunk;
+    const ListPlan pl = list_plan(sms, cta_q, a.capacity);
     const size_t rows = (size_t)2 * NS, lists = (size_t)NS * K;
     StreamScratch sc;
-    e = sc.alloc({sizeof(PsCamSlots) * 2 * nc, sizeof(int*) * 2, sizeof(mcs_ocam) * nc, sizeof(double) * 9 * nc, rows * a.dim,
-                  a.masked ? rows * a.dim : 0, rows * 4, 2 * 4, (size_t)2 * (nc + 1) * 4, rows * 24, (size_t)splits * lists * 4, lists * 4,
-                  lists * 4, lists}, st);
-    if (e != cudaSuccess) return e;
-    PsCamSlots* cams = sc.at<PsCamSlots>(0);
-    const int* const* mp = sc.at<const int*>(1);
-    mcs_ocam* models = sc.at<mcs_ocam>(2); double* E = sc.at<double>(3);
-    uint8_t* desc = sc.at<uint8_t>(4); uint8_t* dmask = a.masked ? sc.at<uint8_t>(5) : nullptr;
-    int* c2s = sc.at<int>(6); int* nvalid = sc.at<int>(7); int* seg = sc.at<int>(8); double* rays = sc.at<double>(9);
-    unsigned* part = sc.at<unsigned>(10); int* lidx = sc.at<int>(11); int* ldist = sc.at<int>(12); uint8_t* flag = sc.at<uint8_t>(13);
-    e = stage_to_device(a.cams, sizeof(PsCamSlots) * 2 * nc, cams, st);
-    if (e == cudaSuccess) e = stage_to_device(a.mp, sizeof(int*) * 2, (void*)mp, st);
-    if (e == cudaSuccess) e = stage_to_device(a.models, sizeof(mcs_ocam) * nc, models, st);
-    if (e == cudaSuccess) e = stage_to_device(a.E, sizeof(double) * 9 * nc, E, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a.nmatches, 0, sizeof(int), st);
+    const PsCamSlots* cams;
+    const int* const* mp;
+    const mcs_ocam* models;
+    const double* E;
+    e = open_scratch(sc, {rows * a.dim, a.masked ? rows * a.dim : 0, rows * 4, 2 * 4, (size_t)2 * (nc + 1) * 4, rows * 24,
+                          (size_t)pl.splits * lists * 4, lists * 4, lists * 4, lists},
+                     st, host_in(cams, a.cams, 2 * (size_t)nc), host_in(mp, a.mp, 2), host_in(models, a.models, nc), host_in(E, a.E, 9 * (size_t)nc));
+    if (e != cudaSuccess) return sc.release(e);
+    uint8_t* desc = sc.at<uint8_t>(0); uint8_t* dmask = a.masked ? sc.at<uint8_t>(1) : nullptr;
+    int* c2s = sc.at<int>(2); int* nvalid = sc.at<int>(3); int* seg = sc.at<int>(4); double* rays = sc.at<double>(5);
+    unsigned* part = sc.at<unsigned>(6); int* lidx = sc.at<int>(7); int* ldist = sc.at<int>(8); uint8_t* flag = sc.at<uint8_t>(9);
+    e = cudaMemsetAsync(a.nmatches, 0, sizeof(int), st);
     if (e == cudaSuccess && a.diag) e = cudaMemsetAsync(a.diag, 0, 2 * sizeof(int), st);
     if (e != cudaSuccess) return sc.release(e);
     kk_gather_kernel<true><<<2, 1024, 0, st>>>(cams, mp, nc, a.capacity, a.dim, a.masked, 0, nullptr, desc, dmask, c2s, nvalid, nullptr,
                                                models, rays, seg);
     // distances <= th_low are listed (bmma_klists lists those below its bound)
-    const unsigned bound = a.th_low < 0 ? 0u : (unsigned)std::min(a.th_low + 1LL, 0x7FFLL);
+    const unsigned bound = a.th_low < 0 ? 0u : (unsigned)(a.th_low + 1LL);
     const size_t smem = (size_t)((a.capacity + 31) / 32) * 4;
     with_desc_width(a.dim, a.masked, [&](auto W, auto M) {
         const uint32_t *d32 = (const uint32_t*)desc, *m32 = (const uint32_t*)dmask;
-        tr_lists_kernel<W, M><<<dim3((unsigned)cta_q, splits), kTopkThreads, 0, st>>>(d32, m32, seg, nc, NS, qblocks, chunk, bound, part);
-        topk_merge_kernel<<<(NS + 127) / 128, 128, 0, st>>>(part, splits, NS, K, lidx, ldist);
+        seg_lists_kernel<CamSegs, W, M><<<dim3((unsigned)cta_q, pl.splits), kTopkThreads, 0, st>>>(d32, m32, CamSegs{seg, nc, NS}, qblocks,
+                                                                                                   (size_t)NS, pl.chunk, bound, part);
+        topk_merge_kernel<<<(NS + 127) / 128, 128, 0, st>>>(part, pl.splits, NS, K, lidx, ldist);
         tr_epi_kernel<<<(unsigned)((lists + 255) / 256), 256, 0, st>>>(lidx, rays, seg, c2s, nvalid, E, nc, a.capacity, a.epi_thresh, flag);
         tr_walk_kernel<W, M><<<nc, kTrWalkThreads, smem, st>>>(lidx, ldist, flag, d32, m32, rays, seg, c2s, cams, E, nc, a.capacity, a.th_low,
                                                                a.epi_thresh, a.matches12, a.nmatches, a.diag);

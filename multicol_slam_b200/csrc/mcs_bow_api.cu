@@ -236,8 +236,7 @@ int mcs_search_by_bow_device(const mcs_bow_frame* kfs, int32_t n_kf, const mcs_b
     std::vector<BowFrameDev> kdev(n_kf);
     kslots.reserve((size_t)n_kf * n_cams);
     for (int k = 0; k < n_kf; ++k) {
-        const std::vector<PsCamSlots> s = packed_slots(kfs[k].frame, n_cams, capacity, dim);
-        kslots.insert(kslots.end(), s.begin(), s.end());
+        append_slots(kslots, kfs[k].frame, n_cams, capacity, dim);
         kdev[k] = BowFrameDev{kfs[k].fv_nodes_dev, kfs[k].fv_offsets_dev, kfs[k].n_fv_dev, kfs[k].fv_features_dev, kfs[k].mp_dev};
     }
     const std::vector<PsCamSlots> cslots = packed_slots(cur->frame, n_cams, capacity, dim);

@@ -32,8 +32,7 @@ int mcs_update_mappoints_device(const mcs_mp_keyframe* kfs, int32_t n_kf, int32_
     std::vector<int> kf_bad(n_kf);
     std::vector<double> kf_ow(3 * (size_t)n_kf);
     for (int k = 0; k < n_kf; ++k) {
-        const std::vector<PsCamSlots> s = packed_slots(kfs[k].frame, n_cams, capacity, dim);
-        slots.insert(slots.end(), s.begin(), s.end());
+        append_slots(slots, kfs[k].frame, n_cams, capacity, dim);
         kf_bad[k] = kfs[k].bad != 0;
         for (int i = 0; i < 3; ++i) kf_ow[3 * k + i] = kfs[k].ow[i];
     }

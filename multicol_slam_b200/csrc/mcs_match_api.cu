@@ -626,14 +626,11 @@ int mcs_project_mappoints_device(int32_t n_cams, const double* mtmc_inv, const d
             return mcs_fail(MCS_ERR_UNSUPPORTED, "cameras of different image sizes");
     cudaStream_t st = (cudaStream_t)stream;
     // poses, camera models and scale factors: one scratch block, staged in stream order
-    const size_t b_pose = (size_t)n_cams * 128, b_cam = sizeof(mcs_ocam) * n_cams, b_sf = 8 * (size_t)n_levels;
     StreamScratch sc;
-    CUDA_CHECK(sc.alloc({b_pose, b_pose, b_cam, b_sf}, st));
-    double* d_mtmc_inv = sc.at<double>(0); double* d_mtmc = sc.at<double>(1); mcs_ocam* d_cams = sc.at<mcs_ocam>(2); double* d_sf = sc.at<double>(3);
-    cudaError_t e = stage_to_device(mtmc_inv, b_pose, d_mtmc_inv, st);
-    if (e == cudaSuccess) e = stage_to_device(mtmc, b_pose, d_mtmc, st);
-    if (e == cudaSuccess) e = stage_to_device(cams, b_cam, d_cams, st);
-    if (e == cudaSuccess) e = stage_to_device(scale_factors, b_sf, d_sf, st);
+    const double *d_mtmc_inv, *d_mtmc, *d_sf;
+    const mcs_ocam* d_cams;
+    cudaError_t e = open_scratch(sc, {}, st, host_in(d_mtmc_inv, mtmc_inv, 16 * (size_t)n_cams), host_in(d_mtmc, mtmc, 16 * (size_t)n_cams),
+                                 host_in(d_cams, cams, n_cams), host_in(d_sf, scale_factors, n_levels));
     if (e == cudaSuccess)
         e = launch_frustum(n_cams, d_mtmc_inv, d_mtmc, d_cams, masks_dev, n_points, world_pos_dev, normal_dev, min_dist_dev, max_dist_dev, d_sf,
                            n_levels, in_view_dev, level_dev, proj_x_dev, proj_y_dev, view_cos_dev, skip_dev, st);
@@ -801,8 +798,7 @@ int mcs_fuse_device(const mcs_fuse_target* kfs, int32_t n_kf, int32_t n_cams, in
     std::vector<const int*> kf_mp(n_kf);
     std::vector<double> mtmc_inv(16 * (size_t)NI), ow(3 * (size_t)n_kf);
     for (int k = 0; k < n_kf; ++k) {
-        const std::vector<PsCamSlots> s = packed_slots(kfs[k].frame, n_cams, capacity, dim);
-        slots.insert(slots.end(), s.begin(), s.end());
+        append_slots(slots, kfs[k].frame, n_cams, capacity, dim);
         kf_mp[k] = kfs[k].mp_dev;
         std::memcpy(&mtmc_inv[16 * (size_t)k * n_cams], kfs[k].mtmc_inv, 128ull * n_cams);
         for (int i = 0; i < 3; ++i) ow[3 * k + i] = kfs[k].ow[i];
@@ -841,8 +837,7 @@ int mcs_search_by_bow_keyframes_device(const mcs_packed_frame* kf1, const int32_
     std::vector<PsCamSlots> cams = packed_slots(*kf1, n_cams, capacity, dim);
     std::vector<const int*> mp(1, mp1_dev);
     for (int k = 0; k < n_kf; ++k) {
-        const std::vector<PsCamSlots> s = packed_slots(kfs[k], n_cams, capacity, dim);
-        cams.insert(cams.end(), s.begin(), s.end());
+        append_slots(cams, kfs[k], n_cams, capacity, dim);
         mp.push_back(mp_dev[k]);
     }
     BowKfSearchDevArgs a{};
@@ -865,8 +860,7 @@ int mcs_search_for_triangulation_device(const mcs_packed_frame* kf1, const int32
     if (int rc = check_packed_frames(n_cams, capacity, dim, kf1, kf2)) return rc;
     if (int rc = check_query_bound((long long)n_cams * capacity, "n_cams * capacity must stay below 2^24")) return rc;
     std::vector<PsCamSlots> slots = packed_slots(*kf1, n_cams, capacity, dim);
-    const std::vector<PsCamSlots> s2 = packed_slots(*kf2, n_cams, capacity, dim);
-    slots.insert(slots.end(), s2.begin(), s2.end());
+    append_slots(slots, *kf2, n_cams, capacity, dim);
     std::vector<double> e_diag((size_t)n_cams * 9);                  // only E[c][c] is read: a query sees its own camera only
     for (int c = 0; c < n_cams; ++c) std::memcpy(&e_diag[(size_t)c * 9], E + ((size_t)c * n_cams + c) * 9, 9 * sizeof(double));
     TriSearchDevArgs a{};

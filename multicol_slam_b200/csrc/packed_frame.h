@@ -28,16 +28,22 @@ inline FeatureView feature_at(const FeatureView& v, size_t i, int capacity, int 
     return FeatureView{v.counts + i, v.kps + slot, v.desc + slot * dim, v.dmask ? v.dmask + slot * dim : nullptr};
 }
 
-// camera c of a packed frame = global image first_image + c = image (g mod part_images) of part g / part_images
-inline std::vector<PsCamSlots> packed_slots(const mcs_packed_frame& fr, int n_cams, int capacity, int dim) {
+// appends the slots of cameras 0 .. n_cams - 1 of a packed frame to `slots`, so that the tables of several frames follow each other:
+// camera c = global image first_image + c = image (g mod part_images) of part g / part_images
+inline void append_slots(std::vector<PsCamSlots>& slots, const mcs_packed_frame& fr, int n_cams, int capacity, int dim) {
     const size_t part_bytes = mcs_packed_layout(fr.part_images, capacity, dim, nullptr);
-    std::vector<PsCamSlots> slots(n_cams);
     for (int c = 0; c < n_cams; ++c) {
         const int g = fr.first_image + c, p = g / fr.part_images, i = g - p * fr.part_images;
         const FeatureView v = feature_at(packed_view((const uint8_t*)fr.packed_dev + (size_t)p * part_bytes, fr.part_images, capacity, dim),
                                          i, capacity, dim);
-        slots[c] = PsCamSlots{v.counts, v.kps, v.desc, v.dmask};
+        slots.push_back(PsCamSlots{v.counts, v.kps, v.desc, v.dmask});
     }
+}
+
+// the slot table of one packed frame
+inline std::vector<PsCamSlots> packed_slots(const mcs_packed_frame& fr, int n_cams, int capacity, int dim) {
+    std::vector<PsCamSlots> slots;
+    append_slots(slots, fr, n_cams, capacity, dim);
     return slots;
 }
 

@@ -1072,23 +1072,6 @@ int proj_search_max_rounds() { return kPsRounds; }
 
 namespace {
 
-// One small host input of a launcher: n elements at `host`, staged into the launcher's scratch; `dev` receives the device copy.
-template <class T> struct HostIn { const T*& dev; const T* host; size_t n; };
-template <class T> HostIn<T> host_in(const T*& dev, const T* host, size_t n) { return {dev, host, n}; }
-
-// A launcher's one stream-ordered scratch block: its own pieces first (own[i] is sc.at<T>(i)), then a device copy of every host
-// input, staged in stream order.  The caller releases sc, whatever the result.
-template <class... T>
-cudaError_t ps_open(StreamScratch& sc, std::vector<size_t> own, cudaStream_t st, const HostIn<T>&... in) {
-    size_t i = own.size();
-    (own.push_back(sizeof(T) * in.n), ...);
-    cudaError_t e = sc.alloc(own, st);
-    if (e != cudaSuccess) return e;
-    ((in.dev = sc.at<T>(i++)), ...);
-    ((e = e == cudaSuccess ? stage_to_device(in.host, sizeof(T) * in.n, (void*)in.dev, st) : e), ...);
-    return e;
-}
-
 // frame_prepare_kernel's camera table for a search without camera models: it reads only width and height (no rays)
 std::vector<mcs_ocam> cam_sizes(const PsFrameArgs& a) {
     std::vector<mcs_ocam> hc(a.n_cams);
@@ -1222,9 +1205,9 @@ cudaError_t ps_open_two_frames(const PsTwoFrameArgs& a, std::vector<size_t> own,
     own.insert(own.end(), {sizeof(mcs_keypoint) * NS, db, a.masked ? db : 0});
     const bool pose = a.models != nullptr;
     const std::vector<mcs_ocam> sizes = pose ? std::vector<mcs_ocam>() : cam_sizes(a);
-    cudaError_t e = ps_open(t.sc, own, st, host_in(t.cur, a.cams, a.n_cams), host_in(t.last, a.last, a.n_cams),
-                            host_in(t.cams, pose ? a.models : sizes.data(), a.n_cams), host_in(t.mtmc_inv, a.mtmc_inv, pose ? 16 * a.n_cams : 0),
-                            host_in(t.sf, a.sf, a.n_levels));
+    cudaError_t e = open_scratch(t.sc, own, st, host_in(t.cur, a.cams, a.n_cams), host_in(t.last, a.last, a.n_cams),
+                                 host_in(t.cams, pose ? a.models : sizes.data(), a.n_cams), host_in(t.mtmc_inv, a.mtmc_inv, pose ? 16 * a.n_cams : 0),
+                                 host_in(t.sf, a.sf, a.n_levels));
     if (e != cudaSuccess) return e;
     t.keys = t.sc.at<mcs_keypoint>(k); t.desc = t.sc.at<uint8_t>(k + 1); t.dmask = a.masked ? t.sc.at<uint8_t>(k + 2) : nullptr;
     e = ps_zero_outputs(a, st);
@@ -1244,7 +1227,7 @@ cudaError_t launch_search_by_projection(const ProjSearchArgs& a, cudaStream_t st
     const std::vector<mcs_ocam> sizes = cam_sizes(a);
     const PsCamSlots* slots; const mcs_ocam* cams; const double* sf;
     StreamScratch sc;
-    e = ps_open(sc, {}, st, host_in(slots, a.cams, a.n_cams), host_in(cams, sizes.data(), a.n_cams), host_in(sf, a.sf, a.n_levels));
+    e = open_scratch(sc, {}, st, host_in(slots, a.cams, a.n_cams), host_in(cams, sizes.data(), a.n_cams), host_in(sf, a.sf, a.n_levels));
     if (e == cudaSuccess) {
         const MapPointQueries qm{a.n_cams, a.n_points, a.n_levels, a.bad, a.in_view, a.level, a.px, a.py, a.vcos, sf, a.th};
         e = ps_search<MCS_RULE_LEVEL_RATIO>(a, qm, a.nnratio, a.mp_desc, a.mp_dmask, nullptr, slots, cams, nullptr, st);
@@ -1355,10 +1338,10 @@ cudaError_t launch_fuse_device(const FuseDevArgs& a, cudaStream_t st) {
     for (int k = 0; k < nk; ++k) models.insert(models.end(), a.pts.models, a.pts.models + nc);
     const PsCamSlots* slots; const int* const* kf_mp; const double* mtmc_inv; const double* ow; const mcs_ocam* cams; const double* sf;
     StreamScratch sc;
-    e = ps_open(sc, {4ull * a.pts.n_points, (size_t)nk * a.n_q,                                                                    // qmap held
-                     (size_t)QE, 8ull * QE, 8ull * QE, 4ull * QE, 4ull * QE, 4ull * QE, 4ull * (nb + 1), 4ull * (nb + 1)},          // ok u v level entry dec
-                st, host_in(slots, a.cams, NI), host_in(kf_mp, a.kf_mp, nk), host_in(mtmc_inv, a.mtmc_inv, 16 * NI), host_in(ow, a.ow, 3 * nk),
-                host_in(cams, models.data(), NI), host_in(sf, a.sf, a.n_levels));
+    e = open_scratch(sc, {4ull * a.pts.n_points, (size_t)nk * a.n_q,                                                                    // qmap held
+                          (size_t)QE, 8ull * QE, 8ull * QE, 4ull * QE, 4ull * QE, 4ull * QE, 4ull * (nb + 1), 4ull * (nb + 1)},          // ok u v level entry dec
+                     st, host_in(slots, a.cams, NI), host_in(kf_mp, a.kf_mp, nk), host_in(mtmc_inv, a.mtmc_inv, 16 * NI), host_in(ow, a.ow, 3 * nk),
+                     host_in(cams, models.data(), NI), host_in(sf, a.sf, a.n_levels));
     if (e != cudaSuccess) return sc.release(e);
     int* qmap = sc.at<int>(0); uint8_t* held = sc.at<uint8_t>(1);
     uint8_t* ok = sc.at<uint8_t>(2); double* u = sc.at<double>(3); double* v = sc.at<double>(4); int* level = sc.at<int>(5);
@@ -1407,9 +1390,9 @@ cudaError_t launch_search_by_sim3(const Sim3SearchDevArgs& a, cudaStream_t st) {
     if (e != cudaSuccess) return e;
     const PsCamSlots* s1; const PsCamSlots* s2; const mcs_ocam* models; const double* mc_inv; const Sim3Xf* xf; const double* sf;
     StreamScratch sc;
-    e = ps_open(sc, {(size_t)NS, 8ull * NS, 8ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS}, st,        // ok u v level entry dec b1 b2
-                host_in(s1, a.kf1, a.n_cams), host_in(s2, a.cams, a.n_cams), host_in(models, a.pts.models, a.n_cams),
-                host_in(mc_inv, a.mc_inv, 16 * a.n_cams), host_in(xf, (const Sim3Xf*)a.xf, 2), host_in(sf, a.sf, a.n_levels));
+    e = open_scratch(sc, {(size_t)NS, 8ull * NS, 8ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS, 4ull * NS}, st,        // ok u v level entry dec b1 b2
+                     host_in(s1, a.kf1, a.n_cams), host_in(s2, a.cams, a.n_cams), host_in(models, a.pts.models, a.n_cams),
+                     host_in(mc_inv, a.mc_inv, 16 * a.n_cams), host_in(xf, (const Sim3Xf*)a.xf, 2), host_in(sf, a.sf, a.n_levels));
     if (e != cudaSuccess) return sc.release(e);
     uint8_t* ok = sc.at<uint8_t>(0); double* u = sc.at<double>(1); double* v = sc.at<double>(2); int* level = sc.at<int>(3);
     int* entry = sc.at<int>(4); int* dec = sc.at<int>(5); int* b1 = sc.at<int>(6); int* b2 = sc.at<int>(7);
@@ -1453,10 +1436,10 @@ cudaError_t launch_search_by_projection_scw(const ScwSearchDevArgs& a, cudaStrea
     if (e != cudaSuccess) return e;
     const PsCamSlots* slots; const mcs_ocam* models; const double* mtmc_inv; const double* ow; const double* sf;
     StreamScratch sc;
-    e = ps_open(sc, {4ull * (a.n_cams + 1), (size_t)a.pts.n_points,                                                   // first found
-                     (size_t)a.n_q, 8ull * a.n_q, 8ull * a.n_q, 4ull * a.n_q, 4ull * a.n_q},                          // ok u v level qcam
-                st, host_in(slots, a.cams, a.n_cams), host_in(models, a.pts.models, a.n_cams), host_in(mtmc_inv, a.mtmc_inv, 16 * a.n_cams),
-                host_in(ow, a.ow, 3), host_in(sf, a.sf, a.n_levels));
+    e = open_scratch(sc, {4ull * (a.n_cams + 1), (size_t)a.pts.n_points,                                                   // first found
+                          (size_t)a.n_q, 8ull * a.n_q, 8ull * a.n_q, 4ull * a.n_q, 4ull * a.n_q},                          // ok u v level qcam
+                     st, host_in(slots, a.cams, a.n_cams), host_in(models, a.pts.models, a.n_cams), host_in(mtmc_inv, a.mtmc_inv, 16 * a.n_cams),
+                     host_in(ow, a.ow, 3), host_in(sf, a.sf, a.n_levels));
     if (e != cudaSuccess) return sc.release(e);
     int* first = sc.at<int>(0); uint8_t* found = sc.at<uint8_t>(1);
     uint8_t* ok = sc.at<uint8_t>(2); double* u = sc.at<double>(3); double* v = sc.at<double>(4); int* level = sc.at<int>(5);
@@ -1482,7 +1465,7 @@ cudaError_t launch_search_for_initialization_seed(const PsCamSlots* f1, int n_ca
     const int NS = n_cams * capacity;
     const PsCamSlots* slots;
     StreamScratch sc;
-    cudaError_t e = ps_open(sc, {}, st, host_in(slots, f1, n_cams));
+    cudaError_t e = open_scratch(sc, {}, st, host_in(slots, f1, n_cams));
     if (e == cudaSuccess) {
         pi_seed_kernel<<<(NS + 255) / 256, 256, 0, st>>>(slots, n_cams, capacity, prev);
         e = cudaGetLastError();

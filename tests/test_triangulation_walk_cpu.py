@@ -117,7 +117,7 @@ def test_th_low_edge(api, oa, cams):
 
 
 def test_ties_across_chunks_and_scan_warps(api, oa, cams):
-    """equal-distance candidates straddle a database chunk boundary of tr_lists_kernel and are taken in index order; equal-distance
+    """equal-distance candidates straddle a database chunk boundary of seg_lists_kernel and are taken in index order; equal-distance
     candidates held by different scanning warps of a rescan are taken in index order"""
     (spec, s, p), = _runs(api, oa, cams, "ties")
     chunk, splits = tm.chunk_of(s["cap"], 3)

@@ -2,8 +2,8 @@
 multicol_slam_b200/csrc/match_kernels.cu, DESIGN.md "Local mapping's triangulation search on the device") and a seeded catalogue
 of planted scenes that put its walk on each of its decision edges.
 
-The model restates the kernels one for one: lists() is tr_lists_kernel with topk_merge_kernel, flags() is tr_epi_kernel and walk()
-is tr_walk_kernel with its exact rescan (tr_scan).  Its output is what the device writes -- matches12 by slot, nmatches and
+The model restates the kernels one for one: lists() is seg_lists_kernel<CamSegs> with topk_merge_kernel, flags() is tr_epi_kernel
+and walk() is tr_walk_kernel with its exact rescan (tr_scan).  Its output is what the device writes -- matches12 by slot, nmatches and
 diag = [queries, rescans] -- plus a record of the rule that decided each query, which the scene classes assert on.  `mutant`
 switches one rule to a plausible wrong one; the tests show that some scene tells each of them from the sequential loop.
 
@@ -51,8 +51,8 @@ def segments(F, free):
 
 
 def lists(dist, th_low, mutant=None):
-    """tr_lists_kernel + topk_merge_kernel for one camera: per query row, the K smallest (distance, segment index) keys with
-    distance <= th_low, as (index, distance) lists padded with (-1, INT_MAX)"""
+    """seg_lists_kernel<CamSegs> + topk_merge_kernel for one camera: per query row, the K smallest (distance, segment index) keys
+    with distance <= th_low, as (index, distance) lists padded with (-1, INT_MAX)"""
     out = []
     for row in dist:
         ok = row < th_low if mutant == "list_th_low_lt" else row <= th_low
@@ -169,7 +169,8 @@ def counts(F):
 
 
 def chunk_of(capacity, n_cams, sms=H100_SMS):
-    """launch_search_for_triangulation's database chunk of tr_lists_kernel (a multiple of kDbTile) and the number of chunks"""
+    """launch_search_for_triangulation's database chunk of seg_lists_kernel<CamSegs> (a multiple of kDbTile) and the number of
+    chunks: list_plan(sms, ceil(capacity / 128) * n_cams, capacity) in match_kernels.cu, the one plan of the K-best list kernels"""
     qblocks, tiles = -(-capacity // TOPK_THREADS), -(-capacity // DB_TILE)
     cta_q = qblocks * n_cams
     splits = max(1, min(tiles, -(-(4 * sms * 8) // cta_q)))
@@ -417,7 +418,7 @@ def _th_low(api, oa, cams, P, rig1, rig2, E, var):
 
 
 def _ties(api, oa, cams, P, rig1, rig2, E, var):
-    """class 5: ten equal-distance passing candidates on both sides of a database chunk boundary of tr_lists_kernel (camera 0), taken
+    """class 5: ten equal-distance passing candidates on both sides of a database chunk boundary of seg_lists_kernel (camera 0), taken
     by a chain of identical queries in index order; camera 1: equal-distance passing candidates that different scanning warps of a
     rescan hold, taken by a chain of rescanning queries in index order"""
     b = P.base()
