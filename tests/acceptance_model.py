@@ -8,6 +8,8 @@ window_search), plus the keypoints taken on entry.  Its output is what the devic
 walk start, queries, rescans), so the tests can tell a correct acceptance from one that only ends at the right answer."""
 import numpy as np
 
+from device_frames import flip
+
 K = 8                       # kPsK in proj_search_kernels.cu: list length per query
 INT_MAX = 2**31 - 1
 RULE_RATIO, RULE_BEST, RULE_LEVEL_RATIO = 0, 1, 2          # MCS_RULE_* (include/mcs_b200.h)
@@ -259,14 +261,6 @@ def predict_init(oa, m, F1, F2, prev, window):
 # ------------------------------------------------------------------------------------------------------------------------------
 # the scene generator
 # ------------------------------------------------------------------------------------------------------------------------------
-def flip(rng, d, nbits):
-    """d with nbits distinct bits flipped: Hamming distance nbits"""
-    out = d.copy()
-    for b in rng.choice(8 * len(d), nbits, replace=False):
-        out[b // 8] ^= 1 << (b % 8)
-    return out
-
-
 class Abstract:
     """a search-independent scene: keypoints of the searched frame per camera, queries in the order the search makes them, the
     searched keypoints taken on entry, and the descriptor masks (None: unmasked)"""

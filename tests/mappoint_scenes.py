@@ -8,8 +8,8 @@ points whose observations are lists of (key frame, slot), each key frame's slots
 reference key frames that do not observe their point."""
 import numpy as np
 
+from device_frames import pack_frames
 from multicol_slam_b200.ctypes_defs import KEYPOINT_DTYPE
-from multicol_slam_b200 import rig
 
 EDGE_COUNTS = (0, 1, 2, 3, 6, 7, 32, 33, 300)
 
@@ -56,7 +56,7 @@ def scene(seed, dim=32, n_cams=3, capacity=16, n_kf=160, n_levels=8, scale=1.2, 
 
 
 def slot_rows(sc, k):
-    """(kps, desc, dmask) per camera of key frame k, for rig.pack"""
+    """(kps, desc, dmask) per camera of key frame k, the images of a packed frame"""
     cap, out = sc["capacity"], []
     for c in range(sc["n_cams"]):
         n = int(sc["kf_counts"][k, c])
@@ -67,17 +67,22 @@ def slot_rows(sc, k):
     return out
 
 
-def packed_frames(sc, layout):
-    """the key frames as packed buffers: "one" = every image in one layout, "parts" = one image per layout of one buffer,
-    "separate" = one buffer per key frame.  Returns (list of uint8 numpy buffers, per key frame (buffer index, n_parts,
-    part_images, first_image))."""
-    n_kf, nc, cap, dim = len(sc["ow"]), sc["n_cams"], sc["capacity"], sc["dim"]
-    images = [im for k in range(n_kf) for im in slot_rows(sc, k)]
-    if layout == "one":
-        return [rig.pack(images, cap, dim)], [(0, 1, n_kf * nc, k * nc) for k in range(n_kf)]
-    if layout == "parts":
-        return [np.concatenate([rig.pack([im], cap, dim) for im in images])], [(0, n_kf * nc, 1, k * nc) for k in range(n_kf)]
-    return [rig.pack(images[k * nc:(k + 1) * nc], cap, dim) for k in range(n_kf)], [(k, 1, nc, 0) for k in range(n_kf)]
+def packed_frames(sc, layout, device="cuda"):
+    """the key frames as packed-frame records (buffer, n_parts, part_images, first_image): "one" = every image in one layout,
+    "parts" = one image per layout of one buffer, "separate" = one buffer per key frame; device None gives numpy buffers"""
+    kw = {"one": dict(layout="joint"), "parts": dict(layout="parts"), "separate": dict(layout="single", first_image=0, after=0)}[layout]
+    return pack_frames([slot_rows(sc, k) for k in range(len(sc["ow"]))], sc["capacity"], sc["dim"], device=device, **kw)
+
+
+SCENES = {"d32": dict(seed=1), "d32_masks": dict(seed=2, masks=True), "d16_masks": dict(seed=3, dim=16, masks=True),
+          "d64": dict(seed=4, dim=64), "ties": dict(seed=5, pool=2, flips=1, masks=True), "equal": dict(seed=6, pool=1, flips=0)}
+
+
+def named_scene(name):
+    """the scene SCENES[name] and whether it runs with masks"""
+    kw = dict(SCENES[name])
+    masks = kw.pop("masks", False)
+    return scene(**kw), masks
 
 
 def host_update(api, sc, ids, what, having_masks, obs=None, tables=None):

@@ -6,11 +6,8 @@ import numpy as np
 import pytest
 
 import acceptance_model as am
-from test_search_for_initialization_device_gpu import device_init, host_init
-from test_search_projection_device_gpu import _device_search, _per_cam, _sizes
-from test_search_projection_frames_device_gpu import _device_frames
-from test_search_projection_last_device_gpu import _device_last
-from test_window_search_device_gpu import _device_ws
+from device_frames import per_cam, sizes
+from device_searches import device_init, device_last, device_projection, device_search_frames, device_ws, host_init
 
 pytestmark = pytest.mark.gpu
 
@@ -26,12 +23,12 @@ SPECS = am.catalogue(_cap())
 def _device(api, m, s, layout):
     k = s["kind"]
     if k == "local":
-        return _device_search(api, m, _per_cam(s["F"]), _sizes(s["F"]), s["F"].scale_factors, s["mps"], s["th"], pre=s["pre"].copy(), layout=layout)
+        return device_projection(api, m, per_cam(s["F"]), sizes(s["F"]), s["F"].scale_factors, s["mps"], s["th"], pre=s["pre"].copy(), layout=layout)
     if k == "last":
-        return _device_last(api, m, s["F"], s["Fl"], s["rig"], s["mp_cur"], s["mp_last"], None, s["world"], s["bad"], s["th"], layout=layout)
+        return device_last(api, m, s["F"], s["Fl"], s["rig"], s["mp_cur"], s["mp_last"], None, s["world"], s["bad"], s["th"], layout=layout)
     if k == "frames":
-        return _device_frames(api, m, s["F"], s["Fl"], s["rig"], s["mp_cur"], s["mp_last"], s["world"], s["bad"], s["th"], layout=layout)
-    return _device_ws(api, m, s["F"], s["Fl"], s["mp_last"], s["bad"], s["th"], layout=layout)
+        return device_search_frames(api, m, s["F"], s["Fl"], s["rig"], s["mp_cur"], s["mp_last"], s["world"], s["bad"], s["th"], layout=layout)
+    return device_ws(api, m, s["F"], s["Fl"], s["mp_last"], s["bad"], s["th"], layout=layout)
 
 
 @pytest.mark.parametrize("spec", SPECS, ids=[am.spec_id(s) for s in SPECS])

@@ -14,12 +14,11 @@ import numpy as np
 import pytest
 
 import bow_scale
-from test_bow_vectors_device_gpu import FILL, GUARD, call, check, pack_frames, split, to_contiguous
-from test_search_by_bow_device_gpu import device_search, frame_of, host_search, same
+from bow_device import TAIL_WORDS, VEC_FILL, call, check, device_bow_search, frame_of, host_bow_search, pack_bow_frames, same, split
+from device_frames import SIZES, on_device, rm, slot_to_contiguous_index, to_slots  # noqa: F401  (rm: a fixture)
 
 pytestmark = pytest.mark.gpu
 TILE, NORM_CHUNK, GRID_WARPS = 2048, 2048, 16384 * 256 // 32
-SIZES = [(754, 480)] * 3
 
 
 @pytest.fixture(scope="module")
@@ -36,12 +35,6 @@ def v(api, voc):
 @pytest.fixture(scope="module")
 def o(oa, voc):
     return oa.OracleVocabulary(voc)
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
 
 
 def tiles(n):
@@ -77,7 +70,7 @@ def test_device_vectors_at_every_levelsup(api, v, o, voc, n_cams, cap, layout):
     counts = [cap - 7 * c for c in range(n_cams)]
     desc = bow_scale.spread(voc, sum(counts), 10 + n_cams)
     other = split(bow_scale.clustered(voc, 100 * n_cams, 3), [100] * n_cams)         # frame 0 of the shared buffer
-    packed = pack_frames([other, split(desc, counts)], cap, 32, layout)[1]
+    packed = pack_bow_frames([other, split(desc, counts)], cap, 32, layout)[1]
     seen = dict(nb=0, node=0, word=0)
     for levelsup in range(8):
         H = call(api, v, packed, counts, cap, levelsup)
@@ -94,7 +87,7 @@ def test_device_vectors_at_every_levelsup(api, v, o, voc, n_cams, cap, layout):
 def test_device_vectors_every_scoring_and_weighting(api, oa, voc, scoring):
     counts = [2048, 2040, 2030, 2020]
     desc = bow_scale.spread(voc, sum(counts), 30 + scoring)
-    packed = pack_frames([split(desc, counts)], 2048, 32, "parts")[0]
+    packed = pack_bow_frames([split(desc, counts)], 2048, 32, "parts")[0]
     for weighting in range(4):
         vs, os_ = api.ORBVocabulary(voc, scoring, weighting), oa.OracleVocabulary(voc, scoring, weighting)
         for levelsup in (0, 4):
@@ -106,7 +99,7 @@ def test_device_vectors_every_scoring_and_weighting(api, oa, voc, scoring):
 def test_device_vectors_clustered_and_stopped(api, v, o, voc):
     counts = [1500, 1200, 1400]
     for desc in (bow_scale.clustered(voc, sum(counts), 40), bow_scale.stopped(voc, sum(counts), 41)):
-        packed = pack_frames([split(desc, counts)], 1500, 32, "single")[0]
+        packed = pack_bow_frames([split(desc, counts)], 1500, 32, "single")[0]
         for levelsup in (0, 2, 4):
             check(api, call(api, v, packed, counts, 1500, levelsup), v, desc, counts, 1500, levelsup, o)
 
@@ -115,15 +108,15 @@ def test_device_vectors_clustered_and_stopped(api, v, o, voc):
 def test_max_nodes_one_short_at_full_size(api, v, voc, levelsup):
     counts = [2048, 2048, 2048]
     desc = bow_scale.spread(voc, sum(counts), 50)
-    packed = pack_frames([split(desc, counts)], 2048, 32, "single")[0]
+    packed = pack_bow_frames([split(desc, counts)], 2048, 32, "single")[0]
     bw, bv, (fn, fo, ff) = v.transform(desc, levelsup)
     short = len(fn) - 1
     assert fn[-1] >= (2**20 if levelsup == 0 else 100000)
     H = call(api, v, packed, counts, 2048, levelsup, max_nodes=short)                # the guard words are checked inside
     assert H["status"][0] == api.MCS_ERR_CAPACITY and H["n_fv"][0] == short
     assert np.array_equal(H["fv_nodes"][:short], fn[:short]) and np.array_equal(H["fv_offsets"][:short + 1], fo[:short + 1])
-    assert np.array_equal(to_contiguous(H["fv_features"][:fo[short]], counts, 2048), ff[:fo[short]])
-    assert np.all(H["fv_features"][fo[short]:3 * 2048] == FILL)
+    assert np.array_equal(slot_to_contiguous_index(H["fv_features"][:fo[short]], counts, 2048), ff[:fo[short]])
+    assert np.all(H["fv_features"][fo[short]:3 * 2048] == VEC_FILL)
     assert np.array_equal(H["bow_words"][:len(bw)], bw) and np.array_equal(H["bow_values"][:len(bw)], bv)
 
 
@@ -133,14 +126,14 @@ def test_other_widths_are_refused(api, v, voc, dim):
     from multicol_slam_b200.ctypes_defs import PackedFrame
     counts = [500, 400, 300]
     d = bow_scale.other_width(voc, sum(counts), 60, dim)
-    packed = pack_frames([split(d, counts)], 512, dim, "single")[0]
-    out = [torch.full((3 * 512 + GUARD,), FILL, dtype=torch.float64 if k == 5 else torch.int32, device="cuda") for k in range(8)]
+    packed = pack_bow_frames([split(d, counts)], 512, dim, "single")[0]
+    out = [torch.full((3 * 512 + TAIL_WORDS,), VEC_FILL, dtype=torch.float64 if k == 5 else torch.int32, device="cuda") for k in range(8)]
     fr = PackedFrame(packed[0].data_ptr(), *packed[1:4])
     rc = api.lib().mcs_bow_vectors_device(v._h, C.byref(fr), 3, 512, dim, 4, 200, None, None, None,
                                           *(C.c_void_p(t.data_ptr()) for t in out), None)
     assert rc == api.MCS_ERR_UNSUPPORTED
     torch.cuda.synchronize()
-    assert all(bool((t == FILL).all()) for t in out)
+    assert all(bool((t == VEC_FILL).all()) for t in out)
     with pytest.raises(ValueError):
         v.transform(d, 4)
 
@@ -173,7 +166,7 @@ def reloc(voc):
     cur = frame(6000, 300, False)
     kfs = [frame(int(rng.integers(4500, 6200)), int(rng.integers(200, 1500)), True) for _ in range(N_KF)]
     half = N_KF // 2
-    packed = pack_frames([p for p, _ in kfs[:half]], CAP, 32, "single") + pack_frames([p for p, _ in kfs[half:]] + [cur[0]], CAP, 32, "shared")
+    packed = pack_bow_frames([p for p, _ in kfs[:half]], CAP, 32, "single") + pack_bow_frames([p for p, _ in kfs[half:]] + [cur[0]], CAP, 32, "shared")
     assert packed[half][0].data_ptr() == packed[-1][0].data_ptr() != packed[0][0].data_ptr()
     return dict(kfs=kfs, cur=cur, packed=packed, n_points=n_points, bad=bad)
 
@@ -189,7 +182,7 @@ def test_search_many_key_frames(api, oa, rm, cams, v, reloc, levelsup, masks):
         bw, bv, fv = v.transform(desc, levelsup)
         db = b.host()
         assert int(b.status.item()) == 0 and np.array_equal(db[0], bw) and np.array_equal(db[1], bv) and np.array_equal(db[2][0], fv[0])
-        assert np.array_equal(db[2][1], fv[1]) and np.array_equal(to_contiguous(db[2][2], [len(p[0]) for p in per], CAP), fv[2])
+        assert np.array_equal(db[2][1], fv[1]) and np.array_equal(slot_to_contiguous_index(db[2][2], [len(p[0]) for p in per], CAP), fv[2])
         hosts.append(fv)
     kfs = [frame_of(per, fv, mp) for (per, mp), fv in zip(reloc["kfs"], hosts)]
     cur = frame_of(reloc["cur"][0], hosts[-1])
@@ -200,15 +193,15 @@ def test_search_many_key_frames(api, oa, rm, cams, v, reloc, levelsup, masks):
         assert items > GRID_WARPS
     m = api.cORBmatcher(0.9, False, 32, masks)
     n_points, bad = reloc["n_points"], reloc["bad"]
-    res, status = device_search(api, m, kfs, cur, n_points, bad, cap=CAP, bows=bows)
+    res, status = device_bow_search(api, m, kfs, cur, n_points, bad, cap=CAP, bows=bows)
     assert status == api.MCS_OK
     total = 0
     for k, (kf, r) in enumerate(zip(kfs, res)):
-        h = host_search(api, m, kf, cur, n_points, bad)
+        h = host_bow_search(api, m, kf, cur, n_points, bad)
         assert same(r, h), k
         total += r[0]
         if k % 11 == 0:
-            assert same(h, host_search(api, m, kf, cur, n_points, bad, oa.search_by_bow)), k
+            assert same(h, host_bow_search(api, m, kf, cur, n_points, bad, oa.search_by_bow)), k
         if rm and k % 11 == 0 and levelsup == 4:
             sf = [1.2 ** lv for lv in range(8)]
             F1, F2 = (api.Frame.from_cameras(f["per"], SIZES, sf) for f in (kf, cur))
@@ -235,7 +228,7 @@ def test_full_chain_on_a_config3_rig(api, v, masks):
     imgs = bench.make_stream(cams, list(range(nc)), 2, 1000)
     pitch = (W + 63) // 64 * 64
     dev_images = torch.zeros((2 * nc, H, pitch), dtype=torch.uint8, device="cuda")
-    dev_images[:, :, :W] = torch.from_numpy(imgs.reshape(2 * nc, H, W)).cuda()
+    dev_images[:, :, :W] = on_device(imgs.reshape(2 * nc, H, W))
     from multicol_slam_b200 import synth
     packed = torch.zeros(rig.packed_layout(2 * nc, cap, 32)[1], dtype=torch.uint8, device="cuda")
     views = ex.extract_batch_packed_device(dev_images, np.stack([synth.mirror_mask(c) for c in cams]), cams, list(range(nc)) * 2, packed, width=W)
@@ -245,7 +238,7 @@ def test_full_chain_on_a_config3_rig(api, v, masks):
     M = [np.concatenate([views["dmask"][nc * f + c, :counts[nc * f + c]].cpu().numpy() for c in range(nc)]) for f in range(2)]
     rng = np.random.default_rng(3)
     mp = np.where(rng.random(len(D[0])) < 0.7, np.arange(len(D[0])), -1).astype(np.int32)
-    mp_t = torch.from_numpy(api.contiguous_to_slots(mp, counts[:nc], cap)).cuda()
+    mp_t = to_slots(api, counts[:nc], mp, cap, -1)
     mt = api.cORBmatcher(0.9, False, 32, masks)
     for levelsup in (4, 0):
         bows = [v.transform_device((packed, 1, 2 * nc, nc * f), nc, cap, levelsup) for f in range(2)]
@@ -255,10 +248,10 @@ def test_full_chain_on_a_config3_rig(api, v, masks):
         n_h, m_h = mt.SearchByBoWFrame(D[0], fv[0], D[1], fv[1], M[0] if masks else None, M[1] if masks else None, (mp >= 0).astype(np.uint8))
         assert int(st.item()) == api.MCS_OK and int(nm[0].item()) == n_h and n_h > 100, (levelsup, n_h)
         sl = api.slots_to_contiguous(msl[0].cpu().numpy(), counts[nc:], cap)
-        assert np.array_equal(np.where(sl >= 0, to_contiguous(np.maximum(sl, 0), counts[:nc], cap), -1), m_h)
+        assert np.array_equal(np.where(sl >= 0, slot_to_contiguous_index(np.maximum(sl, 0), counts[:nc], cap), -1), m_h)
         assert np.array_equal(api.slots_to_contiguous(mmp[0].cpu().numpy(), counts[nc:], cap), np.where(m_h >= 0, mp[np.maximum(m_h, 0)], -1))
         for f in range(2):
             bw, bv, (fn, fo, ff) = bows[f].host()
             hw, hv, _ = v.transform(D[f], levelsup)
             assert np.array_equal(bw, hw) and np.array_equal(bv, hv) and np.array_equal(fn, fv[f][0]) and np.array_equal(fo, fv[f][1])
-            assert np.array_equal(to_contiguous(ff, counts[nc * f:nc * f + nc], cap), fv[f][2])
+            assert np.array_equal(slot_to_contiguous_index(ff, counts[nc * f:nc * f + nc], cap), fv[f][2])

@@ -3,18 +3,16 @@ mcs_bow_transform on the concatenated host copy of the same descriptors, the CPU
 reference's own DBoW2.  Ids and feature lists bit-exact, weights and values == (same double operation order).  Feature indices of
 the device call are slots c * capacity + j; they are compared after the slot -> contiguous conversion."""
 import ctypes as C
-import pathlib
 import sys
 
 import numpy as np
 import pytest
 
+from bow_device import GOLD, LAYOUTS, VEC_FILL, call, check, pack_bow_frames, split
+from device_frames import slot_to_contiguous_index
+
 pytestmark = pytest.mark.gpu
-ROOT = pathlib.Path(__file__).resolve().parents[1]
-GOLD = ROOT / "tests" / "golden"
 sys.path.insert(0, str(GOLD))
-GUARD, FILL = 8, -77
-LAYOUTS = ["single", "parts", "shared"]
 
 
 @pytest.fixture(scope="module")
@@ -47,87 +45,6 @@ def numpy_level_nodes(v, levelsup):
     return int((depth == level).sum() + (leaf & (depth < level)).sum())
 
 
-def split(desc, counts):
-    """descriptors -> per-camera (kps, desc, mask) with the given counts"""
-    from multicol_slam_b200.ctypes_defs import KEYPOINT_DTYPE
-    o, per = 0, []
-    for n in counts:
-        per.append((np.zeros(n, KEYPOINT_DTYPE), np.ascontiguousarray(desc[o:o + n]), np.full((n, desc.shape[1]), 255, np.uint8)))
-        o += n
-    assert o == len(desc)
-    return per
-
-
-def pack_frames(frames, cap, dim, layout):
-    """frames: list of per-camera [(kps, desc, mask)] -> list of (uint8 cuda tensor, n_parts, part_images, first_image)"""
-    import torch
-    from multicol_slam_b200 import rig
-    t = lambda b: torch.from_numpy(b).cuda()  # noqa: E731
-    nc = len(frames[0])
-    k, d, m = max(frames[0], key=lambda p: len(p[0]))
-    decoy = (k[::-1].copy(), d[::-1].copy(), m[::-1].copy())
-    if layout == "single":        # one buffer per frame, a decoy image before and after its cameras
-        return [(t(rig.pack([decoy] + per + [decoy], cap, dim)), 1, nc + 2, 1) for per in frames]
-    if layout == "parts":         # n_cams one-image buffers back to back, as the allgather leaves them
-        return [(t(np.concatenate([rig.pack([p], cap, dim) for p in per])), nc, 1, 0) for per in frames]
-    b = t(rig.pack([p for per in frames for p in per], cap, dim))         # "shared": consecutive images of one buffer
-    return [(b, 1, len(frames) * nc, f * nc) for f in range(len(frames))]
-
-
-def to_contiguous(slots, counts, cap):
-    first = np.concatenate([[0], np.cumsum(counts)])
-    slots = np.asarray(slots)
-    c, j = slots // cap, slots % cap
-    assert np.all(j < np.asarray(counts)[c])
-    return (first[c] + j).astype(np.int32)
-
-
-def call(api, v, packed, counts, cap, levelsup, max_nodes=None, stream=None):
-    """mcs_bow_vectors_device with every output FILLed first and GUARD words behind it -> dict of host arrays"""
-    import torch
-    nc, ns = len(counts), len(counts) * cap
-    max_nodes = v.level_nodes(levelsup) if max_nodes is None else max_nodes
-    sizes = dict(word=ns, weight=ns, node=ns, fv_nodes=max_nodes, fv_offsets=max_nodes + 1, n_fv=1, fv_features=ns, bow_words=ns,
-                 bow_values=ns, n_bow=1, status=1)
-    T = {k: torch.full((n + GUARD,), FILL, dtype=torch.float64 if k in ("weight", "bow_values") else torch.int32, device="cuda")
-         for k, n in sizes.items()}
-    from multicol_slam_b200.ctypes_defs import PackedFrame
-    fr = PackedFrame(packed[0].data_ptr(), *packed[1:4])
-    h = C.c_void_p(stream.cuda_stream) if stream is not None else None
-    torch.cuda.current_stream().synchronize()                    # the fills above; `stream` keeps whatever it is busy with
-    rc =api.lib().mcs_bow_vectors_device(v._h, C.byref(fr), nc, cap, 32, levelsup, max_nodes, *(C.c_void_p(T[k].data_ptr()) for k in sizes), h)
-    assert rc == 0, api.lib().mcs_last_error()
-    torch.cuda.synchronize()
-    H = {k: a.cpu().numpy() for k, a in T.items()}
-    for k, n in sizes.items():
-        assert np.all(H[k][n:] == FILL), f"{k}: written beyond the array"
-    H["sizes"] = sizes
-    return H
-
-
-def check(api, H, v, desc, counts, cap, levelsup, oracle=None):
-    """the device outputs H against mcs_bow_vectors / mcs_bow_transform on the concatenated descriptors (and the oracle)"""
-    bw, bv, (fn, fo, ff) = v.transform(desc, levelsup)
-    assert H["status"][0] == 0
-    nb, nf = int(H["n_bow"][0]), int(H["n_fv"][0])
-    assert nb == len(bw) and np.array_equal(H["bow_words"][:nb], bw) and np.array_equal(H["bow_values"][:nb], bv)
-    assert nf == len(fn) and np.array_equal(H["fv_nodes"][:nf], fn) and np.array_equal(H["fv_offsets"][:nf + 1], fo)
-    assert np.array_equal(to_contiguous(H["fv_features"][:fo[nf]], counts, cap), ff)
-    ns = len(counts) * cap
-    assert np.all(H["bow_words"][nb:ns] == FILL) and np.all(H["fv_features"][fo[nf]:ns] == FILL)
-    w, wt, nd = v.transform_features(desc, levelsup) if len(desc) else (np.zeros(0, np.int32), np.zeros(0), np.zeros(0, np.int32))
-    live = np.zeros(ns, bool)
-    for c, n in enumerate(counts):
-        live[c * cap:c * cap + n] = True
-    for k, ref in (("word", w), ("weight", wt), ("node", nd)):
-        assert np.array_equal(H[k][:ns][live], ref), k
-        assert np.all(H[k][:ns][~live] == FILL), k                 # untouched at or beyond a camera's count
-    if oracle is not None:
-        obw, obv, ofn, ofo, off = oracle.transform(desc, levelsup)
-        assert np.array_equal(bw, obw) and np.array_equal(bv, obv) and np.array_equal(fn, ofn) and np.array_equal(fo, ofo) and np.array_equal(ff, off)
-    return nb, nf
-
-
 @pytest.fixture(scope="module")
 def extracted(api, cams):
     """a 3-camera frame from the device extractor"""
@@ -158,7 +75,7 @@ def test_extracted_frame_in_every_buffer_shape(api, oa, voc, extracted, layout):
     desc = np.concatenate([p[1] for p in extracted])
     assert len(desc) > 2500
     other = [(k[: len(k) // 2], d[: len(k) // 2], m[: len(k) // 2]) for k, d, m in extracted]       # frame 0 of the shared buffer
-    packed = pack_frames([other, extracted], cap, 32, layout)[1]
+    packed = pack_bow_frames([other, extracted], cap, 32, layout)[1]
     assert layout != "shared" or packed[3] == 3
     v, o = api.ORBVocabulary(voc), oa.OracleVocabulary(voc)
     for levelsup in (4, 0):
@@ -169,7 +86,7 @@ def test_extracted_frame_in_every_buffer_shape(api, oa, voc, extracted, layout):
     bw, bv, (fn, fo, ff) = b.host()
     hw, hv, (hn, ho, hf) = v.transform(desc, 4)
     assert np.array_equal(bw, hw) and np.array_equal(bv, hv) and np.array_equal(fn, hn) and np.array_equal(fo, ho)
-    assert np.array_equal(to_contiguous(ff, counts, cap), hf) and int(b.status.item()) == 0
+    assert np.array_equal(slot_to_contiguous_index(ff, counts, cap), hf) and int(b.status.item()) == 0
     assert b.max_nodes == v.level_nodes(4) and b.node is not None
 
 
@@ -179,7 +96,7 @@ def test_scoring_and_weighting(api, oa, voc, scoring, weighting):
     v, o = api.ORBVocabulary(voc, scoring, weighting), oa.OracleVocabulary(voc, scoring, weighting)
     desc = descriptors(voc, 3000, 40 + scoring)
     counts = [1100, 900, 1000]
-    packed = pack_frames([split(desc, counts)], 1101, 32, "single")[0]
+    packed = pack_bow_frames([split(desc, counts)], 1101, 32, "single")[0]
     for levelsup in (4, 1, 0, 6, 8):
         check(api, call(api, v, packed, counts, 1101, levelsup), v, desc, counts, 1101, levelsup, o)
 
@@ -192,7 +109,7 @@ def test_empty_camera_empty_frame_one_keypoint(api, oa, voc):
         for counts, d in (([400, 0, 300], desc), ([0, 0, 0], desc[:0]), ([0, 1, 0], desc[5:6]), ([0, 0, 700], desc)):
             per = split(d, counts)
             full = split(desc, [300, 200, 200])                          # the neighbour frame of the shared buffer is not empty
-            packed = pack_frames([full, per], 420 if counts[2] != 700 else 700, 32, layout)[1]
+            packed = pack_bow_frames([full, per], 420 if counts[2] != 700 else 700, 32, layout)[1]
             cap = 420 if counts[2] != 700 else 700
             H = call(api, v, packed, counts, cap, 4)
             nb, nf = check(api, H, v, d, counts, cap, 4, o if len(d) else None)
@@ -211,22 +128,22 @@ def test_identical_descriptors_and_stopped_words(api, oa, voc, scoring, weightin
     one = descriptors(voc, 1, 11)
     desc = np.repeat(one, 2500, axis=0)
     counts = [1000, 700, 800]
-    packed = pack_frames([split(desc, counts)], 1000, 32, "parts")[0]
+    packed = pack_bow_frames([split(desc, counts)], 1000, 32, "parts")[0]
     for levelsup in (4, 0):
         H = call(api, v, packed, counts, 1000, levelsup)
         assert check(api, H, v, desc, counts, 1000, levelsup, o) == (1, 1)
-        assert np.array_equal(to_contiguous(H["fv_features"][:2500], counts, 1000), np.arange(2500))
+        assert np.array_equal(slot_to_contiguous_index(H["fv_features"][:2500], counts, 1000), np.arange(2500))
     stopped = {k: voc[k].copy() for k in voc.files}
     wn = stopped["word_node"]
     stopped["weight"][wn[::2]] = 0.0
     vs, os_ = api.ORBVocabulary(stopped, scoring, weighting), oa.OracleVocabulary(stopped, scoring, weighting)
     desc = descriptors(voc, 2500, 12)
-    packed = pack_frames([split(desc, counts)], 1000, 32, "single")[0]
+    packed = pack_bow_frames([split(desc, counts)], 1000, 32, "single")[0]
     for levelsup in (4, 0):
         H = call(api, vs, packed, counts, 1000, levelsup)
         check(api, H, vs, desc, counts, 1000, levelsup, os_)
         n_live = int(H["fv_offsets"][H["n_fv"][0]])
-        assert 500 < n_live < 2000 and np.all(H["weight"][:3000][H["weight"][:3000] != FILL] >= 0)
+        assert 500 < n_live < 2000 and np.all(H["weight"][:3000][H["weight"][:3000] != VEC_FILL] >= 0)
 
 
 def test_wide_toy_tree(api, oa):
@@ -236,7 +153,7 @@ def test_wide_toy_tree(api, oa):
     n = len(toy["parent"])
     q = np.concatenate([toy["desc"][rng.integers(1, n, 300)], rng.integers(0, 256, (300, 32), dtype=np.uint8)]).astype(np.uint8)
     counts = [250, 150, 200]
-    packed = pack_frames([split(q, counts)], 256, 32, "single")[0]
+    packed = pack_bow_frames([split(q, counts)], 256, 32, "single")[0]
     for levelsup in (1, 0, 2):
         check(api, call(api, tv, packed, counts, 256, levelsup), tv, q, counts, 256, levelsup, to)
 
@@ -246,15 +163,15 @@ def test_max_nodes_too_small(api, voc):
     v = api.ORBVocabulary(voc)
     desc = descriptors(voc, 3000, 21)
     counts = [1000, 1000, 1000]
-    packed = pack_frames([split(desc, counts)], 1024, 32, "single")[0]
+    packed = pack_bow_frames([split(desc, counts)], 1024, 32, "single")[0]
     bw, bv, (fn, fo, ff) = v.transform(desc, 4)
     for short in (len(fn) - 1, 1):
         H = call(api, v, packed, counts, 1024, 4, max_nodes=short)              # the guard words are checked inside
         assert H["status"][0] == api.MCS_ERR_CAPACITY and H["n_fv"][0] == short
         # the nodes that fit are complete; the BowVector does not depend on max_nodes
         assert np.array_equal(H["fv_nodes"][:short], fn[:short]) and np.array_equal(H["fv_offsets"][:short + 1], fo[:short + 1])
-        assert np.array_equal(to_contiguous(H["fv_features"][:fo[short]], counts, 1024), ff[:fo[short]])
-        assert np.all(H["fv_features"][fo[short]:3 * 1024] == FILL)
+        assert np.array_equal(slot_to_contiguous_index(H["fv_features"][:fo[short]], counts, 1024), ff[:fo[short]])
+        assert np.all(H["fv_features"][fo[short]:3 * 1024] == VEC_FILL)
         assert np.array_equal(H["bow_words"][:len(bw)], bw) and np.array_equal(H["bow_values"][:len(bw)], bv)
     H = call(api, v, packed, counts, 1024, 4, max_nodes=len(fn))
     assert H["status"][0] == 0 and H["n_fv"][0] == len(fn)
@@ -266,7 +183,7 @@ def test_busy_stream(api, voc, extracted):
     counts = [len(p[0]) for p in extracted]
     cap = max(counts)
     desc = np.concatenate([p[1] for p in extracted])
-    packed = pack_frames([extracted], cap, 32, "single")[0]
+    packed = pack_bow_frames([extracted], cap, 32, "single")[0]
     v = api.ORBVocabulary(voc)
     s = torch.cuda.Stream()
     a = torch.randn(4096, 4096, device="cuda")
@@ -285,11 +202,11 @@ def test_reference_golden_through_the_packed_buffer(api, voc):
         d = g[f"c{ci}_desc"]
         counts = [n // 3, n - n // 3 - n // 4, n // 4]
         cap = max(counts) + 3
-        H = call(api, v, pack_frames([split(d, counts)], cap, 32, "parts")[0], counts, cap, levelsup)
+        H = call(api, v, pack_bow_frames([split(d, counts)], cap, 32, "parts")[0], counts, cap, levelsup)
         nb, nf = int(H["n_bow"][0]), int(H["n_fv"][0])
         assert np.array_equal(H["bow_words"][:nb], g[f"c{ci}_bow_words"]) and np.array_equal(H["bow_values"][:nb], g[f"c{ci}_bow_values"])
         assert np.array_equal(H["fv_nodes"][:nf], g[f"c{ci}_fv_nodes"]) and np.array_equal(H["fv_offsets"][:nf + 1], g[f"c{ci}_fv_off"])
-        assert np.array_equal(to_contiguous(H["fv_features"][:H["fv_offsets"][nf]], counts, cap), g[f"c{ci}_fv_feat"])
+        assert np.array_equal(slot_to_contiguous_index(H["fv_features"][:H["fv_offsets"][nf]], counts, cap), g[f"c{ci}_fv_feat"])
         live = np.concatenate([np.arange(c * cap, c * cap + k) for c, k in enumerate(counts)])
         assert np.array_equal(H["word"][live], g[f"c{ci}_word"]) and np.array_equal(H["weight"][live], g[f"c{ci}_weight"])
 
@@ -297,7 +214,7 @@ def test_reference_golden_through_the_packed_buffer(api, voc):
 def test_refusals_that_need_a_vocabulary(api, voc, extracted):
     counts = [len(p[0]) for p in extracted]
     cap = max(counts)
-    packed = pack_frames([extracted], cap, 32, "single")[0]
+    packed = pack_bow_frames([extracted], cap, 32, "single")[0]
     v = api.ORBVocabulary(voc)
     with pytest.raises(api.McsError) as e:
         v.transform_device((packed[0], 1, 5, 3), 3, cap)                   # first_image + n_cams beyond the buffer's images

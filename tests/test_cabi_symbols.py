@@ -1,19 +1,11 @@
 """CPU: libmcs_b200.so loads, exports every function include/mcs_b200.h declares, validates arguments,
 and refuses to compute without a GPU (no CPU fallback)."""
 import ctypes as C
-import pathlib
-import re
 
 import numpy as np
 import pytest
 
-ROOT = pathlib.Path(__file__).resolve().parents[1]
-
-
-def declared_symbols():
-    txt = (ROOT / "include" / "mcs_b200.h").read_text()
-    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
-    return sorted(set(re.findall(r"\b(mcs_[a-z0-9_]+)\s*\(", txt)))
+from device_frames import declared_symbols
 
 
 def test_exports_every_declared_symbol(api):

@@ -5,28 +5,9 @@ oracle."""
 import numpy as np
 import pytest
 
+from extract_cases import extract_and_compare
+
 pytestmark = pytest.mark.gpu
-MODES = {"orb": dict(do_dbrief=False, learn_masks=False), "dbrief": dict(do_dbrief=True, learn_masks=False),
-         "mdbrief": dict(do_dbrief=True, learn_masks=True)}
-
-
-def extract_and_compare(api, oa, imgs, masks, cams, coi, nf, mode="mdbrief", ex=None, **kw):
-    """extract_batch of imgs (camera coi[i] of cams / masks) against the oracle per image; returns the per-image counts"""
-    m = MODES[mode]
-    ex = ex or api.mdBRIEFextractorOct(nfeatures=nf, do_dBrief=m["do_dbrief"], learnMasks=m["learn_masks"], **kw)
-    okw = {"nlevels": kw["nlevels"]} if "nlevels" in kw else {}
-    if "descSize" in kw:
-        okw["desc_size"] = kw["descSize"]
-    oe = oa.OracleExtractor(nfeatures=nf, **m, **okw)
-    kps, desc, dmask, counts = ex.extract_batch(np.stack(imgs), np.stack(masks), cams, coi)
-    for i, img in enumerate(imgs):
-        ok, od, om = oe.extract(img, masks[coi[i]], cams[coi[i]])
-        n = counts[i]
-        assert n == len(ok), f"image {i}: {n} keypoints, oracle {len(ok)}"
-        assert kps[i, :n].tobytes() == ok.tobytes(), f"image {i}: keypoints"
-        assert np.array_equal(desc[i, :n], od), f"image {i}: descriptors"
-        assert np.array_equal(dmask[i, :n], om), f"image {i}: descriptor masks"
-    return counts
 
 
 # (nlevels, nfeatures, mask, keypoints of the first image): 0 on a flat image, 1 through a 6 x 6 mask window, and 31 / 32 / 33

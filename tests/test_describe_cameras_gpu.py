@@ -8,7 +8,9 @@ import pathlib
 
 import numpy as np
 import pytest
-from test_describe_batch_gpu import extract_and_compare
+
+from device_frames import on_device
+from extract_cases import extract_and_compare
 
 pytestmark = pytest.mark.gpu
 SYNTHETIC = {c["name"]: c for c in json.loads((pathlib.Path(__file__).resolve().parent / "golden" / "synthetic_cams.json").read_text())}
@@ -69,7 +71,7 @@ def test_packed_device_buffer(api, oa):
     imgs, masks = frames(cam, [730, 731])
     ex = api.mdBRIEFextractorOct(nfeatures=2000, do_dBrief=True, learnMasks=True)
     packed = torch.zeros(rig.packed_layout(2, ex.capacity, 32)[1], dtype=torch.uint8, device="cuda")
-    v = ex.extract_batch_packed_device(torch.from_numpy(np.stack(imgs)).cuda(), np.stack(masks), [cam], [0, 0], packed)
+    v = ex.extract_batch_packed_device(on_device(np.stack(imgs)), np.stack(masks), [cam], [0, 0], packed)
     torch.cuda.synchronize()
     counts = v["counts"].cpu().numpy()
     kps = v["kps"].cpu().numpy().view(api.KEYPOINT_DTYPE).reshape(2, ex.capacity)

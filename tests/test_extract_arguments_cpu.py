@@ -2,11 +2,11 @@
 tests/test_extract_arguments_gpu.py."""
 import ctypes as C
 
-FAKE = C.c_void_p(0x10000)      # stands for a buffer: never dereferenced by the host
+from device_frames import FAKE
 
 
 def test_null_extractor_refused(api):
-    L, F = api.lib(), FAKE
+    L, F = api.lib(), C.c_void_p(FAKE)         # stands for a buffer: never dereferenced by the host
     calls = {
         "mcs_extract": lambda: L.mcs_extract(None, F, 64, 64, 64, F, 64, F, F, F, F, 100, F),
         "mcs_extract_batch": lambda: L.mcs_extract_batch(None, 1, F, 64, 64, 64, F, F, 1, F, F, F, F, F, 100),

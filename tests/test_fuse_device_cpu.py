@@ -4,17 +4,10 @@ device route, still reproduces the reference's recorded map mutations, for all t
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
+from device_frames import FAKE, frames, taped_rm  # noqa: F401  (frames: a fixture)
+from search_scenes import fuse_scene, host_fuse, reference_ops
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
-frames = T.frames
-
-
-@pytest.fixture(scope="module")
-def rm():
-    """the reference's own matcher, live while recording and replayed from tests/golden/ref_tape_fuse_device_cpu.* otherwise"""
-    import ref_tape
-    return ref_tape.module("ref_match_api", "fuse_device_cpu", T.TAPE_LIMIT)
+rm = taped_rm("fuse_device_cpu")
 
 
 def _fuse(api, cams, n_kf=2, n_cams=3, capacity=2000, dim=32, frame=None, frames_=None, mtmc=True, n_levels=8, sf="ok", variant=0, q=FAKE,
@@ -70,64 +63,6 @@ def test_symbol_is_declared_and_exported(api):
     assert "int  mcs_fuse_device(" in hdr and "typedef struct mcs_fuse_target" in hdr
     assert hasattr(api.lib(), "mcs_fuse_device")
     assert callable(api.cORBmatcher.FuseDevice) and callable(api.cORBmatcher.FuseReplay)
-
-
-def fuse_scene(api, oa, cams, KF, variant, seed=5):
-    """the scene of test_ref_match_cpu.py::test_fuse_equals_reference; variant 0 adds a current key frame: a second rig pose a few
-    centimetres away whose keypoints carry the query points (their rays are the bearing rays of the points seen from it)"""
-    sc = T.make_scene(api, oa, cams, KF, 11 + variant)
-    rng = np.random.default_rng(seed)
-    n = len(sc["world"])
-    kf_mp = np.full(len(KF.keys), -1, np.int32)
-    occupied = rng.choice(len(KF.keys), len(KF.keys) // 3, replace=False)
-    extra_bad = (rng.random(len(occupied)) < 0.1).astype(np.uint8)
-    kf_mp[occupied] = n + np.arange(len(occupied))
-    bad = np.concatenate([sc["bad"], extra_bad])
-    in_kf = np.concatenate([(rng.random(n) < 0.1), np.ones(len(occupied), bool)])
-    pad = lambda a, fill=0.0: np.concatenate([a, np.full((len(occupied),) + a.shape[1:], fill, a.dtype)])  # noqa: E731
-    s = dict(sc=sc, n=n, kf_mp=kf_mp, occupied=occupied, bad=bad, in_kf=in_kf, points=np.arange(n, dtype=np.int32),
-             world=pad(sc["world"]), min_d=pad(sc["min_d"], 1.0), max_d=pad(sc["max_d"], 2.0), desc=pad(sc["desc"]), dmask=pad(sc["dmask"]),
-             Scw=None, cur=None)
-    if variant == 2:
-        Scw = api.inv_rigid(sc["M_t"]).copy()
-        Scw[:3, :3] *= 1.3
-        Scw[:3, 3] *= 1.3
-        s["Scw"] = Scw
-    if variant == 0:
-        # curKF: the same keypoints on a rig moved by a few cm; keypoint j of curKF carries points[j] (one key frame of map points
-        # per keypoint, as vpMapPointMatches of curKF).  Rays: the point's bearing from the moved rig, jittered so that the
-        # epipolar check both passes and fails among the occupied hits.
-        M_t2 = sc["M_t"].copy()
-        M_t2[:3, 3] += [0.03, -0.01, 0.02]
-        cur_rig = api.Rig(cams, sc["M_c"], M_t2)
-        rays = np.zeros((n, 3))
-        for j in range(n):
-            c = int(KF.key_cam[sc["src"][j]])
-            pc = api._mm(cur_rig.MtMc_inv[c], np.append(sc["world"][j], 1.0))[:3]
-            r = pc / np.linalg.norm(pc) + rng.normal(0, 0.08 if j % 2 else 0.0005, 3)
-            rays[j] = r / np.linalg.norm(r)
-        key_cam = np.asarray(KF.key_cam[sc["src"]], np.int32)
-        s["cur"] = dict(rig=cur_rig, M_t=M_t2, rays=rays, key_cam=key_cam)
-    return s
-
-
-def reference_ops(api, rm, cams, KF, s, variant, masks):
-    sc = s["sc"]
-    table = rm.MPTable(3, s["desc"], dmask=s["dmask"], bad=s["bad"], world_pos=s["world"], min_dist=s["min_d"], max_dist=s["max_d"],
-                       obs_kf=np.where(s["in_kf"], 0, -1).astype(np.int32), obs_idx=np.zeros(len(s["bad"]), np.int32))
-    kfr = rm.KF(KF, cams, M_c=sc["M_c"], M_t=sc["M_t"], mp=s["kf_mp"], rays=sc["rays"])
-    cur = None
-    if variant == 0:
-        Fc = api.Frame(KF.keys[sc["src"]], s["cur"]["key_cam"], KF.desc[sc["src"]], KF.dmask[sc["src"]], T.SIZES, KF.scale_factors)
-        cur = rm.KF(Fc, cams, M_c=sc["M_c"], M_t=s["cur"]["M_t"], mp=s["points"], rays=s["cur"]["rays"])
-    return rm.fuse(variant, kfr, table, s["points"], 2.5, 0.6, masks, CurK=cur, Scw=s["Scw"])
-
-
-def host_fuse(api, m, KF, s, variant, _sw=None, **kw):
-    sc = s["sc"]
-    cur = s["cur"] or {}
-    return m.Fuse(KF, sc["rig"], s["kf_mp"], s["points"], s["world"], s["min_d"], s["max_d"], s["bad"], s["in_kf"], s["desc"], s["dmask"],
-                  th=2.5, variant=variant, Scw=s["Scw"], cur_rays=cur.get("rays"), kf_rays=sc["rays"], cur_rig=cur.get("rig"), _sw=_sw, **kw)
 
 
 @pytest.mark.parametrize("masks", [False, True])

@@ -5,96 +5,20 @@ buffer.  Everything compared is integer: bit for bit."""
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
-from test_fuse_device_cpu import fuse_scene, host_fuse
-from test_search_projection_device_gpu import _per_cam
+from device_frames import BIG_ID, GUARD, SIZES, counts, keep_cameras, on_device, pack_frames, to_slots, widen, widener
+from device_frames import frames, rm  # noqa: F401  (fixtures)
+from device_searches import dev_map, fuse_device, fuse_pose, fuse_replay, fuse_targets
+from search_scenes import fuse_scene, host_fuse, reference_ops
 
 pytestmark = pytest.mark.gpu
-frames = T.frames
-BIG_ID = 1 << 30            # map-point id of the mp rows' slots beyond a camera's count: must never be read
-GUARD = -999
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
-
-
-def _counts(F):
-    return [int((F.key_cam == c).sum()) for c in range(len(F.cam_w))]
-
-
-def _pack_kfs(KFs, cap, layout):
-    """-> one packed-frame descriptor (tensor, n_parts, part_images, first_image) per key frame"""
-    import torch
-    from multicol_slam_b200 import rig
-    dim = KFs[0].desc.shape[1]
-    t = lambda b: torch.from_numpy(b).cuda()  # noqa: E731
-    per = [_per_cam(F) for F in KFs]
-    nc = len(per[0])
-    if layout == "single":          # each key frame alone in its buffer, a decoy image before and after its cameras
-        out = []
-        for p in per:
-            k, d, m = p[0]
-            decoy = (k[::-1].copy(), d[::-1].copy(), None if m is None else m[::-1].copy())
-            out.append((t(rig.pack([decoy] + p + [decoy], cap, dim)), 1, nc + 2, 1))
-        return out
-    # "parts": every key frame's cameras are one-image parts of one buffer, as the allgather leaves a batch of frames
-    b = t(np.concatenate([rig.pack([c], cap, dim) for p in per for c in p]))
-    return [(b, nc * len(per), 1, nc * i) for i in range(len(per))]
-
-
-def _mp_slots(api, F, kf_mp, cap):
-    import torch
-    return torch.from_numpy(api.contiguous_to_slots(np.asarray(kf_mp, np.int32), _counts(F), cap, fill=BIG_ID)).cuda()
-
-
-def _dev_map(s, bad=None, desc=None):
-    import torch
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    return dict(world_t=t(np.asarray(s["world"], np.float64)), min_t=t(np.asarray(s["min_d"], np.float64)),
-                max_t=t(np.asarray(s["max_d"], np.float64)), desc_t=t(s["desc"] if desc is None else desc), dmask_t=t(s["dmask"]),
-                bad_t=None if bad is None else t(np.asarray(bad, np.uint8)))
-
-
-def _pose(rig, variant, Scw):
-    """(MtMc_inv, ow) of the pose a variant projects with"""
-    from multicol_slam_b200.api import _sim3_rig
-    r = rig if variant != 2 else _sim3_rig(rig, Scw)
-    return r.MtMc_inv, r.M_t[:3, 3].copy()
-
-
-def _device(api, m, KFs, rigs, mps, points, dm, cap, layout, variant, Scw=None, th=2.5, max_hits=None, stream=None, sf=None):
-    """FuseDevice over the key frames -> (hits [n, 3] numpy, n_hits, status, out tensors)"""
-    import torch
-    packed = _pack_kfs(KFs, cap, layout)
-    kfs = [(packed[k], mps[k]) + _pose(rigs[k], variant, Scw) for k in range(len(KFs))]
-    q_t = torch.from_numpy(np.ascontiguousarray(points, np.int32)).cuda()
-    masks_t = torch.from_numpy(np.stack(rigs[0].masks)).cuda()
-    out = m.FuseDevice(kfs, q_t, cap, rigs[0].cams, masks_t, KFs[0].scale_factors if sf is None else sf, dm["world_t"], dm["min_t"], dm["max_t"],
-                       dm["desc_t"], dm["dmask_t"], bad_t=dm["bad_t"], variant=variant, th=th, max_hits=max_hits, stream=stream)
-    torch.cuda.synchronize()
-    n = int(out[1].item())
-    return out[0].cpu().numpy()[:n], n, int(out[2].item()), out
-
-
-def _replay(m, KF, s, variant, hits, cap, k=0, **kw):
-    sc, cur = s["sc"], s["cur"] or {}
-    rows = hits[hits[:, 0] == k][:, 1:]
-    return m.FuseReplay(KF, sc["rig"], s["kf_mp"], s["points"], rows, cap, s["world"], s["min_d"], s["max_d"], s["bad"], s["in_kf"], s["desc"],
-                        s["dmask"], th=2.5, variant=variant, Scw=s["Scw"], cur_rays=cur.get("rays"), kf_rays=sc["rays"], cur_rig=cur.get("rig"),
-                        **kw)
 
 
 def _with_dim(api, KF, s, dim):
     """the key frame and scene at descriptor width dim: 16 = the first half of every row, 64 = the row and its complement"""
     if dim == 32:
         return KF, s
-    w = (lambda d: np.ascontiguousarray(d[:, :16])) if dim == 16 else (lambda d: np.ascontiguousarray(np.concatenate([d, d ^ 0x5A], 1)))
-    K2 = api.Frame(KF.keys, KF.key_cam, w(KF.desc), w(KF.dmask), list(zip(KF.cam_w, KF.cam_h)), KF.scale_factors)
-    s2 = dict(s, desc=w(s["desc"]), dmask=w(s["dmask"]))
-    return K2, s2
+    w = widener(dim)
+    return widen(api, KF, dim), dict(s, desc=w(s["desc"]), dmask=w(s["dmask"]))
 
 
 @pytest.mark.parametrize("layout", ["single", "parts"])
@@ -109,14 +33,13 @@ def test_per_key_frame_parity(api, oa, rm, frames, cams, variant, masks, dim, la
     KF, s = _with_dim(api, KF0, s0, dim)
     m = api.cORBmatcher(0.6, False, dim, masks)
     hn, hops, hmp = host_fuse(api, m, KF, s, variant)
-    cap = max(_counts(KF)) + 7
-    hits, n, status, _ = _device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], _dev_map(s), cap, layout, variant, Scw=s["Scw"])
+    cap = max(counts(KF)) + 7
+    hits, n, status, _ = fuse_device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], dev_map(s), cap, layout, variant, Scw=s["Scw"])
     assert status == api.MCS_OK and n == len(hits) > 50
-    dn, dops, dmp = _replay(m, KF, s, variant, hits, cap)
+    dn, dops, dmp = fuse_replay(m, KF, s, variant, hits, cap)
     assert dn == hn and np.array_equal(dops, hops) and np.array_equal(dmp, hmp)
     assert (hops[:, 0] == 0).sum() > 10 and (hops[:, 0] == 1).sum() > 10
     if rm:
-        from test_fuse_device_cpu import reference_ops
         rn, rops = reference_ops(api, rm, cams, KF, s, variant, masks)
     else:
         rn, rops, _ = host_fuse(api, m, KF, s, variant, _sw=oa.search_windows)
@@ -124,19 +47,8 @@ def test_per_key_frame_parity(api, oa, rm, frames, cams, variant, masks, dim, la
     if variant == 0:
         # the device route's replay rejected occupied hits on the epipolar check: with a check that always holds it fuses more
         monkeypatch.setattr(api, "check_epipolar", lambda *a: True)
-        an, _, _ = _replay(m, KF, s, variant, hits, cap)
+        an, _, _ = fuse_replay(m, KF, s, variant, hits, cap)
         assert 10 < dn < an
-
-
-def _targets(api, cams, sc, n_kf, seed):
-    """n_kf poses of the key frame's rig around the scene's, a few centimetres apart"""
-    rng = np.random.default_rng(seed)
-    rigs = []
-    for _ in range(n_kf):
-        M_t = sc["M_t"].copy()
-        M_t[:3, 3] += rng.normal(0, 0.02, 3)
-        rigs.append(api.Rig(cams, sc["M_c"], M_t))
-    return rigs
 
 
 @pytest.mark.parametrize("variant", [0, 1, 2])
@@ -146,15 +58,15 @@ def test_batch_equals_separate_calls(api, oa, frames, cams, variant):
     KF = frames[0]
     s = fuse_scene(api, oa, cams, KF, variant)
     m = api.cORBmatcher(0.6, False, 32, True)
-    rigs = _targets(api, cams, s["sc"], 22, 3)
-    cap = max(_counts(KF)) + 3
-    dm = _dev_map(s)
-    mps = [None if k % 3 else _mp_slots(api, KF, s["kf_mp"], cap) for k in range(22)]
-    batch, n, status, _ = _device(api, m, [KF] * 22, rigs, mps, s["points"], dm, cap, "parts", variant, Scw=s["Scw"])
+    rigs = fuse_targets(api, cams, s["sc"], 22, 3)
+    cap = max(counts(KF)) + 3
+    dm = dev_map(s)
+    mps = [None if k % 3 else to_slots(api, KF, s["kf_mp"], cap, BIG_ID) for k in range(22)]
+    batch, n, status, _ = fuse_device(api, m, [KF] * 22, rigs, mps, s["points"], dm, cap, "parts", variant, Scw=s["Scw"])
     assert status == api.MCS_OK
     sep = []
     for k in range(22):
-        h, _, st, _ = _device(api, m, [KF], [rigs[k]], [mps[k]], s["points"], dm, cap, "single", variant, Scw=s["Scw"])
+        h, _, st, _ = fuse_device(api, m, [KF], [rigs[k]], [mps[k]], s["points"], dm, cap, "single", variant, Scw=s["Scw"])
         assert st == api.MCS_OK
         h = h.copy()
         h[:, 0] = k
@@ -172,17 +84,17 @@ def test_prefilter_is_exact(api, oa, frames, cams, variant):
     s["in_kf"] = s["in_kf"].copy()
     s["in_kf"][s["kf_mp"][s["kf_mp"] >= 0]] = True
     m = api.cORBmatcher(0.6, False, 32, False)
-    cap = max(_counts(KF)) + 3
+    cap = max(counts(KF)) + 3
     # map points held by the key frame among the queries too, so that the row filters some queries out
     extra = np.flatnonzero(s["kf_mp"] >= 0)[:40]
     s["points"] = np.concatenate([s["points"], s["kf_mp"][extra]]).astype(np.int32)
-    full, _, st0, _ = _device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], _dev_map(s), cap, "single", variant, Scw=s["Scw"])
-    filt, _, st1, _ = _device(api, m, [KF], [s["sc"]["rig"]], [_mp_slots(api, KF, s["kf_mp"], cap)], s["points"], _dev_map(s, bad=s["bad"]),
+    full, _, st0, _ = fuse_device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], dev_map(s), cap, "single", variant, Scw=s["Scw"])
+    filt, _, st1, _ = fuse_device(api, m, [KF], [s["sc"]["rig"]], [to_slots(api, KF, s["kf_mp"], cap, BIG_ID)], s["points"], dev_map(s, bad=s["bad"]),
                               cap, "single", variant, Scw=s["Scw"])
     assert st0 == st1 == api.MCS_OK and len(filt) < len(full)
     fs = set(map(tuple, full.tolist()))
     assert all(tuple(r) in fs for r in filt.tolist())
-    a, b = _replay(m, KF, s, variant, full, cap), _replay(m, KF, s, variant, filt, cap)
+    a, b = fuse_replay(m, KF, s, variant, full, cap), fuse_replay(m, KF, s, variant, filt, cap)
     assert a[0] == b[0] and np.array_equal(a[1], b[1]) and np.array_equal(a[2], b[2]) and len(a[1]) > 50
 
 
@@ -229,9 +141,9 @@ def test_search_in_neighbors_sequence(api, oa, frames, cams):
     s = fuse_scene(api, oa, cams, KF, 0)
     sc, n = s["sc"], s["n"]
     m = api.cORBmatcher(0.6, False, 32, True)
-    cap = max(_counts(KF)) + 3
+    cap = max(counts(KF)) + 3
     n_kf = 6
-    rigs = [sc["rig"]] + _targets(api, cams, sc, n_kf - 1, 8)
+    rigs = [sc["rig"]] + fuse_targets(api, cams, sc, n_kf - 1, 8)
     # target 0's occupied slots hold query points (points it observes), so its Replace survivors are queries of the later targets
     rng = np.random.default_rng(4)
     rows0 = s["kf_mp"].copy()
@@ -245,9 +157,9 @@ def test_search_in_neighbors_sequence(api, oa, frames, cams):
         mp = _Map(base.bad, base.desc, base.rows)
         ops_all, researched = [], 0
         if device:
-            dm = _dev_map(s, bad=mp.bad, desc=mp.desc)
-            mps = [_mp_slots(api, KF, mp.rows[k], cap) for k in range(n_kf)]
-            hits, _, st, _ = _device(api, m, [KF] * n_kf, rigs, mps, s["points"], dm, cap, "parts", 0)
+            dm = dev_map(s, bad=mp.bad, desc=mp.desc)
+            mps = [to_slots(api, KF, mp.rows[k], cap, BIG_ID) for k in range(n_kf)]
+            hits, _, st, _ = fuse_device(api, m, [KF] * n_kf, rigs, mps, s["points"], dm, cap, "parts", 0)
             assert st == api.MCS_OK
         for k in range(n_kf):
             args = (KF, rigs[k], mp.rows[k], s["points"])
@@ -266,15 +178,15 @@ def test_search_in_neighbors_sequence(api, oa, frames, cams):
         # curKF as a frame: its keypoints in camera-major order (cMultiFrame's), keypoint j carrying point order[j]
         order = np.argsort(s["cur"]["key_cam"], kind="stable")
         src = sc["src"][order]
-        Fc = api.Frame(KF.keys[src], KF.key_cam[src], KF.desc[src], KF.dmask[src], T.SIZES, KF.scale_factors)
+        Fc = api.Frame(KF.keys[src], KF.key_cam[src], KF.desc[src], KF.dmask[src], SIZES, KF.scale_factors)
         cur_row = s["points"][order].copy()
         cur_row[1::2] = -1                          # half of curKF's keypoints free: the candidates both replace and add
         cur_in = np.zeros(len(mp.bad), bool)
         cur_in[cur_row[cur_row >= 0]] = True
         if device:
-            cc = max(_counts(Fc)) + 3
-            dm = _dev_map(s, bad=mp.bad, desc=mp.desc)
-            h2, _, st, _ = _device(api, m, [Fc], [s["cur"]["rig"]], [_mp_slots(api, Fc, cur_row, cc)], cand, dm, cc, "single", 1)
+            cc = max(counts(Fc)) + 3
+            dm = dev_map(s, bad=mp.bad, desc=mp.desc)
+            h2, _, st, _ = fuse_device(api, m, [Fc], [s["cur"]["rig"]], [to_slots(api, Fc, cur_row, cc, BIG_ID)], cand, dm, cc, "single", 1)
             assert st == api.MCS_OK
             _, ops, _ = m.FuseReplay(Fc, s["cur"]["rig"], cur_row, cand, h2[:, 1:], cc, s["world"], s["min_d"], s["max_d"], mp.bad, cur_in,
                                      mp.desc, s["dmask"], th=2.5, variant=1)
@@ -299,17 +211,17 @@ def test_capacity_and_edges(api, oa, frames, cams):
     KF = frames[0]
     s = fuse_scene(api, oa, cams, KF, 2)
     m = api.cORBmatcher(0.6, False, 32, False)
-    cap = max(_counts(KF)) + 3
-    dm = _dev_map(s)
+    cap = max(counts(KF)) + 3
+    dm = dev_map(s)
     rig = s["sc"]["rig"]
-    full, n, st, _ = _device(api, m, [KF], [rig], [None], s["points"], dm, cap, "single", 2, Scw=s["Scw"])
+    full, n, st, _ = fuse_device(api, m, [KF], [rig], [None], s["points"], dm, cap, "single", 2, Scw=s["Scw"])
     assert st == api.MCS_OK and n > 100
     # max_hits below the total: the true total, the first rows, and nothing written past max_hits
     k = n // 3
-    packed = _pack_kfs([KF], cap, "single")
-    mi, ow = _pose(rig, 2, s["Scw"])
-    q_t = torch.from_numpy(s["points"]).cuda()
-    masks_t = torch.from_numpy(np.stack(rig.masks)).cuda()
+    packed = pack_frames([KF], cap, layout="single")
+    mi, ow = fuse_pose(rig, 2, s["Scw"])
+    q_t = on_device(s["points"])
+    masks_t = on_device(np.stack(rig.masks))
     out = (torch.full((k + 5, 3), GUARD, dtype=torch.int32, device="cuda"), torch.zeros(1, dtype=torch.int32, device="cuda"),
            torch.zeros(1, dtype=torch.int32, device="cuda"))
     m.FuseDevice([(packed[0], None, mi, ow)], q_t, cap, rig.cams, masks_t, KF.scale_factors, dm["world_t"], dm["min_t"], dm["max_t"], dm["desc_t"],
@@ -320,23 +232,22 @@ def test_capacity_and_edges(api, oa, frames, cams):
     assert np.array_equal(h[:k], full[:k]) and np.all(h[k:] == GUARD)
     # n_q = 0, every query NULL
     for pts in (np.zeros(0, np.int32), np.full(50, -1, np.int32)):
-        h, n0, st0, _ = _device(api, m, [KF], [rig], [None], pts, dm, cap, "single", 2, Scw=s["Scw"])
+        h, n0, st0, _ = fuse_device(api, m, [KF], [rig], [None], pts, dm, cap, "single", 2, Scw=s["Scw"])
         assert st0 == api.MCS_OK and n0 == 0
     # ids >= n_points: MCS_ERR_INVALID, those queries dropped, the others' hits unchanged
     bad_ids = s["points"].copy()
     bad_ids[::50] = len(s["world"]) + 7
-    h, nb, stb, _ = _device(api, m, [KF], [rig], [None], bad_ids, dm, cap, "single", 2, Scw=s["Scw"])
+    h, nb, stb, _ = fuse_device(api, m, [KF], [rig], [None], bad_ids, dm, cap, "single", 2, Scw=s["Scw"])
     keep = full[full[:, 1] % 50 != 0]
     assert stb == api.MCS_ERR_INVALID and np.array_equal(h, keep)
     # counts at capacity: the key frame's fullest camera fills its slots exactly
-    h, nc_, stc, _ = _device(api, m, [KF], [rig], [None], s["points"], dm, max(_counts(KF)), "parts", 2, Scw=s["Scw"])
+    h, nc_, stc, _ = fuse_device(api, m, [KF], [rig], [None], s["points"], dm, max(counts(KF)), "parts", 2, Scw=s["Scw"])
     c_full = full.copy()
-    c_full[:, 2] = (full[:, 2] // cap) * max(_counts(KF)) + full[:, 2] % cap
+    c_full[:, 2] = (full[:, 2] // cap) * max(counts(KF)) + full[:, 2] % cap
     assert stc == api.MCS_OK and np.array_equal(h, c_full)
     # a camera without keypoints: its hits vanish, the other cameras' stay
-    keep_cam = KF.key_cam != 1
-    K2 = api.Frame(KF.keys[keep_cam], KF.key_cam[keep_cam], KF.desc[keep_cam], KF.dmask[keep_cam], list(zip(KF.cam_w, KF.cam_h)), KF.scale_factors)
-    h, _, ste, _ = _device(api, m, [K2], [rig], [None], s["points"], dm, cap, "single", 2, Scw=s["Scw"])
+    K2, _ = keep_cameras(api, KF, [0, 2])
+    h, _, ste, _ = fuse_device(api, m, [K2], [rig], [None], s["points"], dm, cap, "single", 2, Scw=s["Scw"])
     assert ste == api.MCS_OK and np.array_equal(h, full[full[:, 2] // cap != 1])
     # a busy stream: the call queues behind the stream's work and returns the same hits
     st_ = torch.cuda.Stream()
@@ -345,7 +256,7 @@ def test_capacity_and_edges(api, oa, frames, cams):
         for _ in range(20):
             a = a @ a
             a = a / a.norm()
-        hb, nbz, stz, _ = _device(api, m, [KF], [rig], [None], s["points"], dm, cap, "single", 2, Scw=s["Scw"], stream=st_)
+        hb, nbz, stz, _ = fuse_device(api, m, [KF], [rig], [None], s["points"], dm, cap, "single", 2, Scw=s["Scw"], stream=st_)
     assert stz == api.MCS_OK and np.array_equal(hb, full)
 
 
@@ -440,17 +351,16 @@ def test_projection_edges(api, oa, rm, frames, cams, variant, monkeypatch):
     assert all(lvl[i][cam_of[i]] == KF.keys["octave"][s["sc"]["src"][i]] + 1 for i in ties)
     # the device, hit for hit on the queries Fuse does not skip (without the key frame's row on the device, the call also searches
     # the points already in the key frame; the replay skips them)
-    cap = max(_counts(KF)) + 5
-    dhits, n, status, _ = _device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], _dev_map(s), cap, "single", variant, Scw=s["Scw"])
-    first = np.concatenate([[0], np.cumsum(_counts(KF))])
+    cap = max(counts(KF)) + 5
+    dhits, n, status, _ = fuse_device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], dev_map(s), cap, "single", variant, Scw=s["Scw"])
+    first = np.concatenate([[0], np.cumsum(counts(KF))])
     dh = [(int(q), int(sl) // cap, int(first[sl // cap] + sl % cap)) for _, q, sl in dhits if int(q) in live]
     assert status == api.MCS_OK and dh == hh and len(hh) > 100
     # and the replayed ops
     hn, hops, _ = host_fuse(api, m, KF, s, variant)
-    dn, dops, _ = _replay(m, KF, s, variant, dhits, cap)
+    dn, dops, _ = fuse_replay(m, KF, s, variant, dhits, cap)
     assert dn == hn and np.array_equal(dops, hops)
     if rm:
-        from test_fuse_device_cpu import reference_ops
         rn, rops = reference_ops(api, rm, cams, KF, s, variant, False)
         assert rn == dn and np.array_equal(rops, dops)
     # the edges discriminate: the other precision, or lower_bound replaced by an upper bound, gives other hits

@@ -8,7 +8,7 @@ tile matter: corners everywhere, saturated margins, and maxima on both sides of 
 import numpy as np
 import pytest
 
-from test_extract_adversarial_gpu import boundary_lattice, cams_for, run_batch
+from extract_cases import boundary_lattice, cams_for, run_batch
 
 pytestmark = pytest.mark.gpu
 

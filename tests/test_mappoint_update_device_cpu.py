@@ -9,15 +9,10 @@ import numpy as np
 import pytest
 
 import mappoint_scenes as S
+from device_frames import FAKE, taped_rm
+from mappoint_scenes import SCENES, named_scene
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
-
-
-@pytest.fixture(scope="module")
-def rm():
-    """the reference's own cMapPoint, live while recording and replayed from tests/golden/ref_tape_mappoint_update_device_cpu.*"""
-    import ref_tape
-    return ref_tape.module("ref_mappoint_api", "mappoint_update_device_cpu")
+rm = taped_rm("mappoint_update_device_cpu", "ref_mappoint_api", 256)
 
 
 def test_exported_symbol_and_layout(api):
@@ -58,16 +53,6 @@ def test_refusals_before_any_launch(api):
             assert _call(api, **kw) == api.MCS_ERR_NO_DEVICE, kw
 
 
-SCENES = {"d32": dict(seed=1), "d32_masks": dict(seed=2, masks=True), "d16_masks": dict(seed=3, dim=16, masks=True),
-          "d64": dict(seed=4, dim=64), "ties": dict(seed=5, pool=2, flips=1, masks=True), "equal": dict(seed=6, pool=1, flips=0)}
-
-
-def _scene(name):
-    kw = dict(SCENES[name])
-    masks = kw.pop("masks", False)
-    return S.scene(**kw), masks
-
-
 def _ref_order(obs, order):
     """obs regrouped into the key-frame order mObservations iterated in (each key frame's slots keep their order)"""
     return [e for k in order for e in obs if e[0] == k]
@@ -87,7 +72,7 @@ def _reference(rm, sc, masks):
 
 @pytest.mark.parametrize("name", sorted(SCENES))
 def test_mirrors_equal_reference(api, rm, name):
-    sc, masks = _scene(name)
+    sc, masks = named_scene(name)
     for p, (obs, ds, ms, d, m, nd) in enumerate(_reference(rm, sc, masks)):
         b = api.ComputeDistinctiveDescriptors(obs, sc["desc"], sc["kf_bad"], masks, sc["dmask"], bad=bool(sc["bad"][p]))
         assert (b is not None) == ds, (name, p)
@@ -109,7 +94,7 @@ def test_scenes_reach_their_edges(api):
     ref key frames that do not observe their point"""
     upper_only = ties = division = nan = level1 = 0
     for name in sorted(SCENES):
-        sc, masks = _scene(name)
+        sc, masks = named_scene(name)
         for p, obs in enumerate(sc["obs"]):
             if sc["bad"][p]:
                 continue

@@ -6,25 +6,19 @@ import numpy as np
 import pytest
 
 import mappoint_scenes as S
-from test_mappoint_update_device_cpu import SCENES, _scene
+from device_frames import on_device
+from mappoint_scenes import SCENES, named_scene
 
 pytestmark = pytest.mark.gpu
 
 
-def _t(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
 def _device(api, sc, layout, ids, what, masks, obs=None, ref=None, stream=None, busy=False):
     import torch
-    bufs, frames = S.packed_frames(sc, layout)
-    tb = [_t(b) for b in bufs]
-    kfs = [((tb[bi], n_parts, part_images, first), sc["ow"][k], sc["kf_bad"][k]) for k, (bi, n_parts, part_images, first) in enumerate(frames)]
+    kfs = [(fr, sc["ow"][k], sc["kf_bad"][k]) for k, fr in enumerate(S.packed_frames(sc, layout))]
     off, okf, oslot = api.mappoint_obs_csr(sc["obs"] if obs is None else obs)
-    tables = [_t(t) for t in S.fill_tables(len(off) - 1, sc["dim"])]
-    args = [_t(np.asarray(ids, np.int32)), _t(off), _t(okf), _t(oslot)]
-    ref_t, world_t, bad_t = _t(sc["ref"] if ref is None else ref), _t(sc["X"]), _t(sc["bad"])
+    tables = [on_device(t) for t in S.fill_tables(len(off) - 1, sc["dim"])]
+    args = [on_device(np.asarray(ids, np.int32)), on_device(off), on_device(okf), on_device(oslot)]
+    ref_t, world_t, bad_t = on_device(sc["ref"] if ref is None else ref), on_device(sc["X"]), on_device(sc["bad"])
     torch.cuda.synchronize()
     if busy:
         with torch.cuda.stream(stream):
@@ -48,7 +42,7 @@ def _all_ids(n, seed=0):
 @pytest.mark.parametrize("layout", ["one", "parts", "separate"])
 @pytest.mark.parametrize("name", sorted(SCENES))
 def test_device_equals_mirror(api, name, layout):
-    sc, masks = _scene(name)
+    sc, masks = named_scene(name)
     ids = _all_ids(len(sc["obs"]))
     st_h, t_h = S.host_update(api, sc, ids, 3, masks)
     st_d, t_d = _device(api, sc, layout, ids, 3, masks)
@@ -60,7 +54,7 @@ def test_device_equals_mirror(api, name, layout):
 @pytest.mark.parametrize("what", [1, 2, 3])
 def test_what_selects_the_arrays(api, what, masks):
     """each `what` writes only its arrays, dmask only with masks; a subset of the points, the others keep their rows"""
-    sc, _ = _scene("d32_masks")
+    sc, _ = named_scene("d32_masks")
     ids = np.arange(0, len(sc["obs"]), 2)
     st_h, t_h = S.host_update(api, sc, ids, what, masks)
     st_d, t_d = _device(api, sc, "one", ids, what, masks)
@@ -74,7 +68,7 @@ def test_what_selects_the_arrays(api, what, masks):
 
 
 def test_invalid_points_are_left_untouched(api):
-    sc, masks = _scene("d32_masks")
+    sc, masks = named_scene("d32_masks")
     n = len(sc["obs"])
     obs = [list(o) for o in sc["obs"]]
     cand = [i for i in range(n) if len({k for k, _ in obs[i]}) >= 2 and not sc["bad"][i] and sc["ref"][i] in {k for k, _ in obs[i]}]
@@ -112,7 +106,7 @@ def test_invalid_points_are_left_untouched(api):
 
 def test_busy_stream_and_empty_call(api):
     import torch
-    sc, masks = _scene("ties")
+    sc, masks = named_scene("ties")
     ids = _all_ids(len(sc["obs"]), 1)
     s = torch.cuda.Stream()
     st_h, t_h = S.host_update(api, sc, ids, 3, masks)
@@ -125,17 +119,17 @@ def test_busy_stream_and_empty_call(api):
 def test_tables_feed_the_projection(api, cams):
     """mcs_project_mappoints_device gives the same outputs from the device-written normal / min / max tables as from the host's"""
     import torch
-    sc, masks = _scene("d32")
+    sc, masks = named_scene("d32")
     ids = np.arange(len(sc["obs"]))
     keep = ~sc["bad"].astype(bool) & np.array([len(o) > 0 for o in sc["obs"]])      # rows the update writes with finite normals
     _, t_h = S.host_update(api, sc, ids, 3, masks)
     _, t_d = _device(api, sc, "one", ids, 3, masks)
-    masks_t = _t(np.stack([api.mirror_mask(c) for c in cams[:3]]))
+    masks_t = on_device(np.stack([api.mirror_mask(c) for c in cams[:3]]))
     mi = np.tile(np.eye(4), (3, 1, 1))
     outs = []
     for t in (t_h, t_d):
-        X = _t(sc["X"][keep])
-        outs.append(api.project_mappoints_device(mi, mi, cams[:3], masks_t, X, _t(t[2][keep]), _t(t[3][keep]), _t(t[4][keep]), sc["sf"]))
+        X = on_device(sc["X"][keep])
+        outs.append(api.project_mappoints_device(mi, mi, cams[:3], masks_t, X, on_device(t[2][keep]), on_device(t[3][keep]), on_device(t[4][keep]), sc["sf"]))
     torch.cuda.synchronize()
     for a, b in zip(*outs):
         assert a.cpu().numpy().tobytes() == b.cpu().numpy().tobytes()

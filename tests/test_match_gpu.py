@@ -3,6 +3,8 @@ SearchByProjection / SearchForInitialization replays (M1, M3) vs the CPU oracle.
 import numpy as np
 import pytest
 
+from match_scenes import make_frames, random_rig
+
 pytestmark = pytest.mark.gpu
 
 
@@ -74,16 +76,6 @@ def test_bruteforce_search_by_bow(api, oa, masked):
     on, om12 = oa.match_bruteforce(q, d, matcher.TH_LOW_, 0.9, qm, dm, v1, v2)
     assert n == on and np.array_equal(m12, om12)
     assert n > 20
-
-
-def make_frames(api, oa, cams, seeds, nf=600, masks=True):
-    from multicol_slam_b200 import synth
-    ex = api.mdBRIEFextractorOct(nfeatures=nf, do_dBrief=True, learnMasks=masks)
-    per = []
-    for c, s in enumerate(seeds):
-        per.append(ex(synth.frame(cams[c], s), synth.mirror_mask(cams[c]), cams[c]))
-    sf = [ex.info.scale_factor[l] for l in range(8)]
-    return api.Frame.from_cameras(per, [(754, 480)] * len(seeds), sf)
 
 
 def test_window_search_candidates(api, oa, cams):
@@ -346,26 +338,13 @@ def test_m4_window_searches(api, oa, cams, masks):
     assert n4 == on4 and np.array_equal(f4, of4)
 
 
-def _random_rig(rng, n_cams):
-    """MtMc[c] = [R t; 0 1] with random rotations looking roughly outwards, and the rigid inverse (cConverter::invMat)."""
-    mtmc, inv = np.zeros((n_cams, 4, 4)), np.zeros((n_cams, 4, 4))
-    for c in range(n_cams):
-        q, _ = np.linalg.qr(rng.normal(size=(3, 3)))
-        if np.linalg.det(q) < 0:
-            q[:, 0] = -q[:, 0]
-        t = rng.normal(0, 0.2, 3)
-        mtmc[c, :3, :3], mtmc[c, :3, 3], mtmc[c, 3, 3] = q, t, 1.0
-        inv[c, :3, :3], inv[c, :3, 3], inv[c, 3, 3] = q.T, -(q.T @ t), 1.0
-    return mtmc, inv
-
-
 def test_project_mappoints_and_search(api, oa, cams):
     """Projection front-end (isInFrustum batched, SURVEY 8f row 2) vs the oracle, then the full chain
     projection -> SearchByProjection on the GPU against the oracle's chain."""
     from multicol_slam_b200 import synth
     rng = np.random.default_rng(12)
     nc, n = 3, 20000
-    mtmc, inv = _random_rig(rng, nc)
+    mtmc, inv = random_rig(rng, nc)
     masks = np.stack([synth.mirror_mask(c) for c in cams])
     pos = rng.normal(size=(n, 3)); pos *= (rng.uniform(1.5, 12.0, n) / np.linalg.norm(pos, axis=1))[:, None]
     nrm = rng.normal(size=(n, 3)); nrm /= np.linalg.norm(nrm, axis=1)[:, None]

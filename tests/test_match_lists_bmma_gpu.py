@@ -5,37 +5,12 @@ equals a database row whose mask is all zero (masked distance 0 from both masks'
 import numpy as np
 import pytest
 
-from test_match_variants_gpu import INT_MAX, pair_dist, ref_lists
+from device_frames import INT_MAX
+from match_lists import check_stream, pair_dist, ref_lists, stream_lists
 
 pytestmark = pytest.mark.gpu
 
 EDGE_COUNTS = (1, 2, 3, 4, 5, 6, 7, 8, 9, 15, 16, 17, 255, 256, 257)
-
-
-def stream_lists(api, desc, dmask, counts, n_frames, n_cams, K):
-    import torch
-    dev = torch.device("cuda", 0)
-    idx, dist = api.match_stream_device(torch.from_numpy(desc).to(dev), None if dmask is None else torch.from_numpy(dmask).to(dev),
-                                        torch.from_numpy(counts).to(dev), n_frames, n_cams, K=K)
-    torch.cuda.synchronize()
-    return idx.cpu().numpy(), dist.cpu().numpy()
-
-
-def check_stream(desc, dmask, counts, n_cams, idx, dist, K):
-    cap = desc.shape[1]
-    for b in range(len(counts)):
-        if b < n_cams or counts[b] == 0:
-            assert (idx[b] == -1).all() and (dist[b] == INT_MAX).all(), b
-            continue
-        nq, nd = counts[b], counts[b - n_cams]
-        if nd == 0:
-            ri, rd = np.full((nq, K), -1, np.int32), np.full((nq, K), INT_MAX, np.int32)
-        else:
-            qm = None if dmask is None else dmask[b, :nq]
-            dm = None if dmask is None else dmask[b - n_cams, :nd]
-            ri, rd = ref_lists(pair_dist(desc[b, :nq], desc[b - n_cams, :nd], qm, dm), K)
-        assert np.array_equal(idx[b, :nq], ri) and np.array_equal(dist[b, :nq], rd), (b, nq, nd)
-        assert (idx[b, nq:cap] == -1).all() and (dist[b, nq:cap] == INT_MAX).all(), b
 
 
 @pytest.mark.parametrize("dim", [16, 32, 64])

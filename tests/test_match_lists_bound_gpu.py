@@ -7,8 +7,8 @@ matchers consume, through their matches against the oracle's SearchByBoW.  Integ
 import numpy as np
 import pytest
 
-from test_match_lists_bmma_gpu import check_stream, stream_lists
-from test_match_variants_gpu import INT_MAX, pair_dist, ref_lists
+from device_frames import INT_MAX
+from match_lists import check_stream, greedy_dist_bound, pair_dist, ref_lists, stream_lists
 
 pytestmark = pytest.mark.gpu
 
@@ -121,7 +121,6 @@ def test_bounded_lists_ties_at_bound(api, oa, dim, masked):
     match_bruteforce_device) against the oracle, with the planted ties one below, at and one above the relevance bound of
     (TH_LOW_, 0.9) and (TH_LOW_, 1.0)"""
     import torch
-    from test_match_variants_gpu import greedy_dist_bound
     dev = torch.device("cuda", 0)
     t = lambda a: None if a is None else torch.from_numpy(a).to(dev)  # noqa: E731
     matcher = api.cORBmatcher(0.9, False, dim, masked)

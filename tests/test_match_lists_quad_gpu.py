@@ -7,8 +7,7 @@ lane; and bursts of 36 near copies inside one 256-column tile, each closer than 
 import numpy as np
 import pytest
 
-from test_match_lists_bmma_gpu import check_stream, stream_lists
-from test_match_variants_gpu import pair_dist, ref_lists
+from match_lists import check_stream, pair_dist, ref_lists, stream_lists
 
 pytestmark = pytest.mark.gpu
 

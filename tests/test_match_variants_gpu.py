@@ -16,45 +16,10 @@ import re
 import numpy as np
 import pytest
 
+from device_frames import INT_MAX
+from match_lists import greedy_dist_bound, pair_dist, ref_lists
+
 pytestmark = pytest.mark.gpu
-
-INT_MAX = 0x7FFFFFFF
-
-
-def pair_dist(q, d, qm=None, dm=None):
-    """[nq, nd] distances: popcount of q ^ d, or the masked form (popc(x & qm) + popc(x & dm)) // 2 summed over the descriptor"""
-    q64 = np.ascontiguousarray(q).view(np.uint64)
-    d64 = np.ascontiguousarray(d).view(np.uint64)
-    out = np.zeros((len(q), len(d)), np.int64)
-    for r0 in range(0, len(q), 256):
-        x = q64[r0:r0 + 256, None, :] ^ d64[None, :, :]
-        if qm is None:
-            out[r0:r0 + 256] = np.bitwise_count(x).sum(axis=2, dtype=np.int64)
-        else:
-            a = np.bitwise_count(x & np.ascontiguousarray(qm).view(np.uint64)[r0:r0 + 256, None, :]).sum(axis=2, dtype=np.int64)
-            b = np.bitwise_count(x & np.ascontiguousarray(dm).view(np.uint64)[None, :, :]).sum(axis=2, dtype=np.int64)
-            out[r0:r0 + 256] = (a + b) // 2
-    return out
-
-
-def ref_lists(dist, K):
-    """the K best (index, distance) of every row ordered by (distance, index), padded with (-1, INT_MAX)"""
-    order = np.argsort(dist, axis=1, kind="stable")[:, :K]
-    idx = np.full((dist.shape[0], K), -1, np.int32)
-    dd = np.full((dist.shape[0], K), INT_MAX, np.int32)
-    idx[:, :order.shape[1]] = order
-    dd[:, :order.shape[1]] = np.take_along_axis(dist, order, axis=1)
-    return idx, dd
-
-
-def greedy_dist_bound(th_low, nnratio):
-    """mirror of greedy_dist_bound (multicol_slam_b200/csrc/kernels.h): lists of the greedy matchers stop below this distance"""
-    if th_low <= 0:
-        return 0
-    b = th_low
-    while b < (1 << 20) and not (th_low - 1 < nnratio * b):
-        b += 1
-    return b
 
 
 def bounded(idx, dist, bound):

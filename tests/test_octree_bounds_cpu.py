@@ -8,8 +8,6 @@ nodes and returns that many keypoints; on wide images with small budgets the fir
 every geometry the extractor accepts (mcs_extractor_octree_plan, host only) and compare the sizes with those bounds, check the
 bounds against the reference's own per-level counts, and check the oracle restatement against the reference fixtures of those
 edges, including the geometries the extractor refuses."""
-import glob
-import json
 import math
 import pathlib
 import re
@@ -17,21 +15,10 @@ import re
 import numpy as np
 import pytest
 
-GOLD = pathlib.Path(__file__).resolve().parent / "golden"
+from octree_fixtures import FIXTURES, REFUSED, TOO_WIDE, load, zlib_crc
+
 CSRC = pathlib.Path(__file__).resolve().parents[1] / "multicol_slam_b200" / "csrc"
-FIXTURES = sorted(glob.glob(str(GOLD / "ref_octree_*.npz")))
 EDGE = 25
-TOO_WIDE = "image too wide for nfeatures: the octree can return more keypoints than the capacity"
-# what the extractor says about each fixture's geometry before any launch; every other fixture is extracted
-REFUSED = {
-    "wide_4095x600_orb100": TOO_WIDE,
-    "wide_3000x400_orb200": TOO_WIDE,
-    "wide_3000x400_mdbrief100": TOO_WIDE,
-    "wide_1500x200_l4_orb40": TOO_WIDE,
-    "wide_4095x244_l7_orb100": TOO_WIDE,
-    "one_level_4095x600_orb10": TOO_WIDE,
-    "wide_2000x250_orb50": "level too small for the 30 px cell grid",     # level 7 is 70 px high: no row of 30 px cells
-}
 # the extractor's refusals of a geometry for reasons other than the octree
 OTHER_REFUSALS = {"pyramid level smaller than 58 px", "level too small for the 30 px cell grid", "FAST cells narrower than 30 px",
                   "portrait images narrower than half their height"}
@@ -134,21 +121,6 @@ def test_plan_of_the_benchmark_geometries_is_unchanged(api):
         assert rc == api.MCS_OK and max(n_ini) <= 2
         assert node_table == (max(q) + 8 + 31) // 32 * 32 and cap == sum(q) + 16
         assert sel_cap.tolist() == [a + 3 for a in q]
-
-
-def load(path):
-    from multicol_slam_b200 import synth
-    g = np.load(path)
-    cam = json.loads(bytes(g["cam_json"]).decode())
-    kw = json.loads(bytes(g["params_json"]).decode())
-    img = synth.frame(cam, int(g["seed"]))
-    assert zlib_crc(img) == int(g["image_crc"]), "synthetic image generator changed"
-    return pathlib.Path(path).stem[len("ref_octree_"):], g, cam, kw, img
-
-
-def zlib_crc(a):
-    import zlib
-    return zlib.crc32(np.ascontiguousarray(a).tobytes())
 
 
 def test_fixture_set_covers_the_edges():

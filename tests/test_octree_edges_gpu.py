@@ -6,7 +6,8 @@ and mcs_extract_batch_packed_device, in a multi-camera batch next to another cam
 refused fixture is checked as that refusal, made before any kernel writes an output."""
 import numpy as np
 import pytest
-from test_octree_bounds_cpu import FIXTURES, REFUSED, load, zlib_crc
+
+from octree_fixtures import FIXTURES, REFUSED, load, zlib_crc
 
 pytestmark = pytest.mark.gpu
 KW = {"nfeatures": "nfeatures", "scale_factor": "scaleFactor", "nlevels": "nlevels", "fast_threshold": "fastThreshold",

@@ -17,7 +17,10 @@ import pathlib
 import numpy as np
 import pytest
 
-import test_projection_edges_cpu as E
+import projection_edge_scenes as E
+from device_frames import flip, on_device
+from device_searches import device_last
+from window_edge_scenes import f32_boundary
 
 pytestmark = pytest.mark.gpu
 GOLD = pathlib.Path(__file__).resolve().parent / "golden"
@@ -45,9 +48,9 @@ def near_tie(x):
 def _device(api, sc, skip=None, out=None, dmax=None):
     import torch
     pos, nrm, dmin, dmx = sc.arrays()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    d = api.project_mappoints_device(sc.inv, sc.mtmc, sc.cams, t(sc.masks), t(pos), t(nrm), t(dmin), t(dmx if dmax is None else dmax),
-                                     sc.sf, skip_t=None if skip is None else t(skip), out=out)
+    d = api.project_mappoints_device(sc.inv, sc.mtmc, sc.cams, on_device(sc.masks), on_device(pos), on_device(nrm), on_device(dmin),
+                                     on_device(dmx if dmax is None else dmax),
+                                     sc.sf, skip_t=None if skip is None else on_device(skip), out=out)
     torch.cuda.synchronize()
     return d
 
@@ -152,7 +155,6 @@ def _motion_scene(api, rng, th):
     edge scenes; one last-frame keypoint per map point (its camera, a random octave), and per point eight current keypoints on the
     float32 extremes of its window (th * sf[octave] about the host projection) and one float beyond: the ones beyond carry the
     closer descriptors, so a window that takes one in changes the match"""
-    from test_window_edges_cpu import _f32_boundary
     scs = [E.scenes()["lafida0/identity"], E.scenes()["lafida0_open/identity"]]
     cams = [scs[0].cams[0], scs[1].cams[0]]
     rig = api.Rig(cams)
@@ -173,10 +175,10 @@ def _motion_scene(api, rng, th):
             last[c].append((p, oct_, base))
             r = th * float(E.SF12[oct_])
             for sign in (-1, 1):
-                ix, ox = _f32_boundary(u, r, sign)
-                iy, oy = _f32_boundary(v, r, sign)
+                ix, ox = f32_boundary(u, r, sign)
+                iy, oy = f32_boundary(v, r, sign)
                 for (kx, ky), dist in (((ix, v), 20), ((u, iy), 22), ((ox, v), 4), ((u, oy), 6)):
-                    cur[c].append((float(kx), float(ky), oct_, _flip(rng, base, dist + int(rng.integers(0, 2)))))
+                    cur[c].append((float(kx), float(ky), oct_, flip(rng, base, dist + int(rng.integers(0, 2)))))
     sf = E.SF12
 
     def frame(rows, key):
@@ -198,16 +200,8 @@ def _motion_scene(api, rng, th):
     return rig, Fl, Fc, np.array(world), mp_last
 
 
-def _flip(rng, d, nbits):
-    out = d.copy()
-    for b in rng.choice(8 * len(d), nbits, replace=False):
-        out[b // 8] ^= 1 << (b % 8)
-    return out
-
-
 @pytest.mark.parametrize("th", [1.0, 3.0])
 def test_motion_model_search_at_the_edges(api, oa, th):
-    from test_search_projection_last_device_gpu import _device_last
     rng = np.random.default_rng(int(th * 10))
     rig, Fl, Fc, world, mp_last = _motion_scene(api, rng, th)
     m = api.cORBmatcher(0.8, False, 32, False)
@@ -228,7 +222,7 @@ def test_motion_model_search_at_the_edges(api, oa, th):
             host_in = rig.in_mirror_mask(c, u, v)
             if bool(g[0][j, 0]) != host_in or (host_in and (g[2][j, 0] != u or g[3][j, 0] != v)):
                 div.add(int(p))
-    gn, gout, status, _ = _device_last(api, m, Fc, Fl, rig, mp_cur, mp_last, None, world, bad, th)
+    gn, gout, status, _ = device_last(api, m, Fc, Fl, rig, mp_cur, mp_last, None, world, bad, th)
     assert status == api.MCS_OK
     keep = ~np.isin(hout, list(div)) & ~np.isin(gout, list(div))
     print(f"\nth {th}: {n} map points, {len(Fc.keys)} current keypoints, {hn} host matches, {gn} device matches, "

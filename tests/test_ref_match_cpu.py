@@ -8,47 +8,18 @@ import sys
 import numpy as np
 import pytest
 
+from device_frames import SIZES, TAPE_LIMIT, flip_bits, frames, taped_rm  # noqa: F401  (frames: a fixture)
+from search_scenes import make_scene
+
 ROOT = pathlib.Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT / "oracle"))
-SIZES = [(754, 480)] * 3
-
-
-TAPE_LIMIT = 1 << 20       # results stored whole: the tests compute on them
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_tape
-    return ref_tape.module("ref_match_api", "ref_match_cpu", TAPE_LIMIT)
+rm = taped_rm("ref_match_cpu")
 
 
 @pytest.fixture(scope="module")
 def api():
     import multicol_slam_b200.api as a            # holders and host-side compositions only; no device call is made in this file
     return a
-
-
-@pytest.fixture(scope="module")
-def frames(oa, cams):
-    """two consecutive 3-camera frames of the sliding-texture stream, extracted by the CPU oracle"""
-    import multicol_slam_b200.api as api            # plain array holders only; no device call is made in this file
-    from multicol_slam_b200 import synth
-    ex = oa.OracleExtractor(nfeatures=350, do_dbrief=True, learn_masks=True)
-    sf = [float(ex.info.scale_factor[l]) for l in range(8)]
-    out = []
-    streams = [synth.texture_stream(cams[c], 2, seed=60 + c) for c in range(3)]
-    for t in range(2):
-        per = [ex.extract(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)]
-        out.append(api.Frame.from_cameras(per, SIZES, sf))
-    return out
-
-
-def flip_bits(rng, desc, kmax):
-    d = desc.copy()
-    for i in range(len(d)):
-        for b in rng.choice(8 * d.shape[1], rng.integers(0, kmax + 1), replace=False):
-            d[i, b // 8] ^= 1 << (b % 8)
-    return d
 
 
 def test_thresholds_and_distances(oa, rm):
@@ -156,34 +127,6 @@ def test_check_orientation_constant():
     """every call site passes the compile-time constant checkOrientation == false (include/cORBmatcher.h:40): the wrapper does too"""
     txt = (ROOT / "oracle" / "ref_mcs" / "wrap_match.cpp").read_text()
     assert txt.count("checkOrientation") >= 10
-
-
-# ---- scenes with 3-D map points for the projection-based searches ---------------------------------------------------------------
-def make_scene(api, oa, cams, frame, seed, npts=500, pose_noise=0.0):
-    """A key frame = `frame` on a 3-camera rig, and map points that really project near its keypoints: each point sits on the
-    bearing ray of a keypoint at a random depth; descriptor = that keypoint's with a few flipped bits."""
-    rng = np.random.default_rng(seed)
-    nc = 3
-    M_c = np.tile(np.eye(4), (nc, 1, 1))
-    for c in range(nc):                                            # cameras looking 120 degrees apart, 10 cm off the rig centre
-        a = 2 * np.pi * c / nc
-        M_c[c, :3, :3] = np.array([[np.cos(a), 0, np.sin(a)], [0, 1, 0], [-np.sin(a), 0, np.cos(a)]])
-        M_c[c, :3, 3] = [0.1 * np.sin(a), 0.0, 0.1 * np.cos(a)]
-    M_t = np.eye(4)
-    M_t[:3, 3] = [0.3, -0.2, 0.1]
-    rig = api.Rig(cams, M_c, M_t)
-    rays, _, _ = oa.frame_prepare(frame.keys, frame.key_cam, cams)
-    src = rng.choice(len(frame.keys), npts, replace=False)
-    depth = rng.uniform(2.0, 6.0, npts)
-    world = np.zeros((npts, 3))
-    for i, k in enumerate(src):
-        pc = np.append(rays[k] * depth[i], 1.0)
-        world[i] = api._mm(rig.MtMc[int(frame.key_cam[k])], pc)[:3] + rng.normal(0, pose_noise, 3)
-    desc = flip_bits(rng, frame.desc[src], 30)
-    dmask = frame.dmask[src].copy()
-    bad = (rng.random(npts) < 0.05).astype(np.uint8)
-    min_d, max_d = depth * rng.uniform(0.5, 0.9, npts), depth * rng.uniform(1.2, 3.0, npts)
-    return dict(rig=rig, M_c=M_c, M_t=M_t, rays=rays, src=src, world=world, desc=desc, dmask=dmask, bad=bad, min_d=min_d, max_d=max_d)
 
 
 @pytest.mark.parametrize("masks", [False, True])

@@ -4,16 +4,10 @@ library did not travel to this box the same comparisons run against the oracle r
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
+from device_frames import flip_bits, frames, rm  # noqa: F401  (frames, rm: fixtures)
+from search_scenes import make_scene
 
 pytestmark = pytest.mark.gpu
-frames = T.frames
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
 
 
 @pytest.mark.parametrize("masks", [False, True])
@@ -50,7 +44,7 @@ def test_core_searches_gpu_vs_reference(api, oa, rm, frames, cams, masks):
 @pytest.mark.parametrize("variant", [1, 2])
 def test_fuse_gpu_vs_reference(api, oa, rm, frames, cams, masks, variant):
     KF = frames[0]
-    sc = T.make_scene(api, oa, cams, KF, 11 + variant)
+    sc = make_scene(api, oa, cams, KF, 11 + variant)
     rng = np.random.default_rng(5)
     n = len(sc["world"])
     kf_mp = np.full(len(KF.keys), -1, np.int32)
@@ -85,7 +79,7 @@ def test_scw_rule_gpu_vs_oracle_multicamera(api, oa, frames, cams, masks):
     """MCS_RULE_SCW on a 3-camera key frame: contiguous id used as the per-camera descriptor row, rows beyond the camera's own
     dropped, keypoint 0 never matched, taken keypoints skipped -- kernel + replay vs the oracle restatement of the same rule"""
     KF = frames[0]
-    sc = T.make_scene(api, oa, cams, KF, 41)
+    sc = make_scene(api, oa, cams, KF, 41)
     n = len(sc["world"])
     points = np.arange(n, dtype=np.int32)
     matched = np.full(len(KF.keys), -1, np.int32)
@@ -121,10 +115,10 @@ def test_sim3_and_between_cameras_gpu(api, oa, rm, frames, cams, masks):
         rn, rp = m.SearchForTriangulationBetweenCameras(KF, rig, kf_mp, rays, 0, 1, _sw=oa.search_windows)
     assert gn == rn and np.array_equal(gp, rp) and gn > 50
     # Sim3
-    sc1 = T.make_scene(api, oa, cams, KF, 51, npts=300)
+    sc1 = make_scene(api, oa, cams, KF, 51, npts=300)
     rng2 = np.random.default_rng(52)
     w2 = sc1["world"] + rng2.normal(0, 0.003, sc1["world"].shape)
-    d2 = T.flip_bits(rng2, KF.desc[sc1["src"]], 30)
+    d2 = flip_bits(rng2, KF.desc[sc1["src"]], 30)
     world = np.concatenate([sc1["world"], w2]); desc = np.concatenate([sc1["desc"], d2]); dmask = np.concatenate([sc1["dmask"], sc1["dmask"]])
     bad = np.concatenate([sc1["bad"], np.roll(sc1["bad"], 7)])
     min_d = np.concatenate([sc1["min_d"], sc1["min_d"]]) * 0.5; max_d = np.concatenate([sc1["max_d"], sc1["max_d"]]) * 2.0

@@ -3,7 +3,7 @@ before any launch, and without a device the calls fail with MCS_ERR_NO_DEVICE.  
 needs one (mcs_vocabulary_level_nodes' counts, the other-device refusal) is in tests/test_bow_vectors_device_gpu.py."""
 import ctypes as C
 
-FAKE = 0x10000      # stands for a device pointer (or a vocabulary that is never looked into): never dereferenced by the host
+from device_frames import FAKE, declared_symbols    # FAKE also stands for a vocabulary that is never looked into
 
 
 def _vectors(api, voc=FAKE, frame=(FAKE, 1, 4, 0), n_cams=4, capacity=2016, dim=32, levelsup=4, max_nodes=81, null=()):
@@ -81,7 +81,6 @@ def test_level_nodes_refuses_null(api):
 
 def test_symbols_are_declared_exported_and_mirrored(api):
     from multicol_slam_b200 import ctypes_defs
-    from test_cabi_symbols import declared_symbols
     for s in ("mcs_vocabulary_level_nodes", "mcs_bow_vectors_device", "mcs_search_by_bow_device"):
         assert s in declared_symbols() and hasattr(api.lib(), s)
     assert hasattr(api.ORBVocabulary, "transform_device") and hasattr(api.ORBVocabulary, "level_nodes")

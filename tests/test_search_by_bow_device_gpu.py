@@ -1,112 +1,18 @@
 """GPU: SearchByBoW(KF_i, F) for a batch of key frames on the device (mcs_search_by_bow_device), against mcs_search_by_bow run per
 key frame on the host copies, the CPU oracle and, where oracle/_ref travelled, the reference's own SearchByBoW(KF, F).  Every frame
 comes from a packed feature buffer; slots are compared after the slot -> contiguous conversion.  Integer work: bit-exact."""
-import pathlib
-
 import numpy as np
 import pytest
 
-from test_bow_vectors_device_gpu import GOLD, LAYOUTS, pack_frames, split, to_contiguous
+from bow_device import GOLD, LAYOUTS, device_bow_search, frame_of, host_bow_search, same, split
+from device_frames import SIZES, on_device, rm, slot_to_contiguous_index, to_slots  # noqa: F401  (rm: a fixture)
 
 pytestmark = pytest.mark.gpu
-ROOT = pathlib.Path(__file__).resolve().parents[1]
-SIZES = [(754, 480)] * 3
-FILL = -55
 
 
 @pytest.fixture(scope="module")
 def voc():
     return np.load(GOLD / "voc_small_9_6.npz")
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
-
-
-def counts_of(per):
-    return [len(p[0]) for p in per]
-
-
-def frame_of(per, fv, mp=None):
-    """a frame on the host: per-camera (kps, desc, mask), its FeatureVector over contiguous keypoint ids, a key frame's map points"""
-    return dict(per=per, fv=tuple(np.asarray(x, np.int32) for x in fv), mp=None if mp is None else np.asarray(mp, np.int32),
-                desc=np.concatenate([p[1] for p in per]), mask=np.concatenate([p[2] for p in per]))
-
-
-def to_slots(idx, counts, cap):
-    first = np.concatenate([[0], np.cumsum(counts)])
-    idx = np.asarray(idx, np.int64)
-    c = np.searchsorted(first, idx, side="right") - 1
-    return (c * cap + idx - first[c]).astype(np.int32)
-
-
-def device_bow(api, packed, fr, cap, max_nodes):
-    """DeviceBoW from a host FeatureVector: CSR tensors padded to max_nodes, features as slots"""
-    import torch
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.int32)).cuda()  # noqa: E731
-    nodes, off, feat = fr["fv"]
-    counts = counts_of(fr["per"])
-    pn = np.full(max_nodes, FILL, np.int32); pn[:len(nodes)] = nodes
-    po = np.full(max_nodes + 1, FILL, np.int32); po[:len(off)] = off
-    ns = len(counts) * cap
-    pf = np.full(max(ns, len(feat)), FILL, np.int32); pf[:len(feat)] = to_slots(feat, counts, cap) if len(feat) else feat
-    return api.DeviceBoW(packed, len(counts), cap, t(pn), t(po), t([len(nodes)]), t(pf))
-
-
-def mp_slots(api, fr, cap):
-    import torch
-    return torch.from_numpy(api.contiguous_to_slots(fr["mp"], counts_of(fr["per"]), cap, fill=2**30)).cuda()
-
-
-def device_search(api, m, kfs, cur, n_points, bad, layout="single", cap=None, stream=None, bows=None):
-    """-> ([(nmatches, match_of_f, match_mp)] per key frame in contiguous keypoint ids, status)"""
-    import torch
-    frames = kfs + [cur]
-    dim = cur["desc"].shape[1]
-    cap = cap or max(max(counts_of(f["per"])) for f in frames) + 3
-    packed = pack_frames([f["per"] for f in frames], cap, dim, layout)
-    max_nodes = max(len(f["fv"][0]) for f in frames) + 2
-    if bows is None:
-        bows = [device_bow(api, p, f, cap, max_nodes) for p, f in zip(packed, frames)]
-    ns = len(cur["per"]) * cap
-    out = (torch.full((len(kfs), ns), FILL, dtype=torch.int32, device="cuda"), torch.full((len(kfs), ns), FILL, dtype=torch.int32, device="cuda"),
-           torch.full((len(kfs),), FILL, dtype=torch.int32, device="cuda"), torch.full((1,), FILL, dtype=torch.int32, device="cuda"))
-    bad_t = None if bad is None else torch.from_numpy(np.ascontiguousarray(bad, np.uint8)).cuda()
-    torch.cuda.current_stream().synchronize()
-    m.SearchByBoWDevice([(b, mp_slots(api, f, cap)) for b, f in zip(bows[:-1], kfs)], bows[-1], n_points, bad_t, stream=stream, out=out)
-    torch.cuda.synchronize()
-    mmp, msl, nm, st = (x.cpu().numpy() for x in out)
-    cc = counts_of(cur["per"])
-    res = []
-    for k, kf in enumerate(kfs):
-        beyond = np.concatenate([np.arange(c * cap + n, (c + 1) * cap) for c, n in enumerate(cc)])
-        assert np.all(mmp[k][beyond] == FILL) and np.all(msl[k][beyond] == FILL)           # slots beyond a count are not written
-        sl, mp = api.slots_to_contiguous(msl[k], cc, cap), api.slots_to_contiguous(mmp[k], cc, cap)
-        idx = np.where(sl >= 0, to_contiguous(np.maximum(sl, 0), counts_of(kf["per"]), cap), -1).astype(np.int32)
-        res.append((int(nm[k]), idx, mp))
-    return res, int(st[0])
-
-
-def host_search(api, m, kf, cur, n_points, bad, search=None):
-    """mcs_search_by_bow (or the oracle) on the host copies -> (nmatches, match_of_f, match_mp)"""
-    mp = kf["mp"]
-    valid = (mp >= 0) & (mp < n_points)
-    if bad is not None:
-        valid &= np.asarray(bad)[np.clip(mp, 0, n_points - 1)] == 0
-    use = m.havingMasks
-    if search is None:
-        n, out = m.SearchByBoWFrame(kf["desc"], kf["fv"], cur["desc"], cur["fv"], kf["mask"] if use else None, cur["mask"] if use else None,
-                                    valid.astype(np.uint8))
-    else:
-        n, out = search(kf["desc"], kf["mask"] if use else None, valid.astype(np.uint8), kf["fv"], cur["desc"], cur["mask"] if use else None,
-                        cur["fv"], m.TH_LOW_, m.mfNNratio)
-    return n, out, np.where(out >= 0, mp[np.maximum(out, 0)], -1).astype(np.int32)
-
-
-def same(a, b):
-    return a[0] == b[0] and np.array_equal(a[1], b[1]) and np.array_equal(a[2], b[2])
 
 
 @pytest.fixture(scope="module")
@@ -136,11 +42,11 @@ def test_parity_with_host_oracle_and_reference(api, oa, rm, cams, scene, masks, 
     fr, n_points, bad = scene["frames"], scene["n_points"], scene["bad"]
     m = api.cORBmatcher(0.9, False, 32, masks)
     kfs, cur = [fr[0], fr[2]], fr[1]
-    res, status = device_search(api, m, kfs, cur, n_points, bad, layout)
+    res, status = device_bow_search(api, m, kfs, cur, n_points, bad, layout)
     assert status == api.MCS_OK
     for kf, r in zip(kfs, res):
-        h = host_search(api, m, kf, cur, n_points, bad)
-        assert same(r, h) and same(h, host_search(api, m, kf, cur, n_points, bad, oa.search_by_bow))
+        h = host_bow_search(api, m, kf, cur, n_points, bad)
+        assert same(r, h) and same(h, host_bow_search(api, m, kf, cur, n_points, bad, oa.search_by_bow))
         assert r[0] > 60 and (r[1] >= 0).sum() == r[0] and np.all(kf["mp"][r[1][r[1] >= 0]] >= 0)
         if rm:
             F1, F2 = (api.Frame.from_cameras(f["per"], SIZES, scene["sf"]) for f in (kf, cur))
@@ -155,11 +61,11 @@ def test_batches_equal_single_calls_and_no_state_leaks(api, scene):
     cur = fr[1]
     eight = [fr[0], fr[2], fr[3], fr[0], fr[2], fr[1], fr[3], fr[0]]          # repeated key frames, and the current frame itself
     for kfs in (eight[:1], eight[:2], eight):
-        res, status = device_search(api, m, kfs, cur, n_points, None, "shared" if len(kfs) == 2 else "single")
+        res, status = device_bow_search(api, m, kfs, cur, n_points, None, "shared" if len(kfs) == 2 else "single")
         assert status == api.MCS_OK
         for k, kf in enumerate(kfs):
-            one, st1 = device_search(api, m, [kf], cur, n_points, None)
-            assert st1 == api.MCS_OK and same(res[k], one[0]) and same(res[k], host_search(api, m, kf, cur, n_points, None))
+            one, st1 = device_bow_search(api, m, [kf], cur, n_points, None)
+            assert st1 == api.MCS_OK and same(res[k], one[0]) and same(res[k], host_bow_search(api, m, kf, cur, n_points, None))
     assert same(res[0], res[3]) and same(res[0], res[7]) and same(res[1], res[4]) and same(res[2], res[6])
     assert res[5][0] > 0.6 * (cur["mp"] >= 0).sum()                            # the frame against itself
     # n_kf = 0 is a successful no-op
@@ -170,18 +76,18 @@ def test_map_point_ids_bad_points_and_status(api, scene):
     fr, n_points, bad = scene["frames"], scene["n_points"], scene["bad"]
     m = api.cORBmatcher(0.9, False, 32, False)
     kf, cur = dict(fr[3]), fr[2]
-    with_bad, st = device_search(api, m, [kf], cur, n_points, bad)
-    without, st2 = device_search(api, m, [kf], cur, n_points, None)
+    with_bad, st = device_bow_search(api, m, [kf], cur, n_points, bad)
+    without, st2 = device_bow_search(api, m, [kf], cur, n_points, None)
     assert st == st2 == api.MCS_OK
-    assert same(with_bad[0], host_search(api, m, kf, cur, n_points, bad)) and same(without[0], host_search(api, m, kf, cur, n_points, None))
+    assert same(with_bad[0], host_bow_search(api, m, kf, cur, n_points, bad)) and same(without[0], host_bow_search(api, m, kf, cur, n_points, None))
     assert without[0][0] > with_bad[0][0] and np.all(bad[with_bad[0][2][with_bad[0][2] >= 0]] == 0)
     # an id beyond the table: status raised, only that keypoint dropped
     good = without[0][1][without[0][1] >= 0]
     kf["mp"] = kf["mp"].copy()
     kf["mp"][good[3]] = n_points + 5
-    res, st = device_search(api, m, [fr[0], kf], cur, n_points, None)
+    res, st = device_bow_search(api, m, [fr[0], kf], cur, n_points, None)
     assert st == api.MCS_ERR_INVALID and good[3] not in res[1][1]
-    assert same(res[1], host_search(api, m, kf, cur, n_points, None)) and same(res[0], host_search(api, m, fr[0], cur, n_points, None))
+    assert same(res[1], host_bow_search(api, m, kf, cur, n_points, None)) and same(res[0], host_bow_search(api, m, fr[0], cur, n_points, None))
 
 
 def built(rng, dim, n_kf_pts, n_cur_pts, nodes_kf, nodes_cur, flips):
@@ -220,9 +126,9 @@ def test_descriptor_widths_with_hand_built_feature_vectors(api, oa, dim, masks):
     assert 7 not in cur["fv"][0] and 9 not in kf["fv"][0]
     m = api.cORBmatcher(0.8, False, dim, masks)
     for layout in ("single", "parts"):
-        res, st = device_search(api, m, [kf, kf], cur, 900, None, layout)
-        h = host_search(api, m, kf, cur, 900, None)
-        assert st == api.MCS_OK and same(res[0], h) and same(res[1], h) and same(h, host_search(api, m, kf, cur, 900, None, oa.search_by_bow))
+        res, st = device_bow_search(api, m, [kf, kf], cur, 900, None, layout)
+        h = host_bow_search(api, m, kf, cur, 900, None)
+        assert st == api.MCS_OK and same(res[0], h) and same(res[1], h) and same(h, host_bow_search(api, m, kf, cur, 900, None, oa.search_by_bow))
         assert h[0] > 100
 
 
@@ -239,8 +145,8 @@ def edge_case(api, m, q_descs, c_descs, expect):
     per = lambda ds: [(np.zeros(len(ds), KEYPOINT_DTYPE), np.stack(ds), np.full((len(ds), 32), 255, np.uint8))]  # noqa: E731
     kf = frame_of(per(q_descs), ([4], [0, len(q_descs)], np.arange(len(q_descs))), np.arange(len(q_descs)) + 10)
     cur = frame_of(per(c_descs), ([4], [0, len(c_descs)], np.arange(len(c_descs))))
-    res, st = device_search(api, m, [kf], cur, 100, None)
-    assert st == api.MCS_OK and same(res[0], host_search(api, m, kf, cur, 100, None))
+    res, st = device_bow_search(api, m, [kf], cur, 100, None)
+    assert st == api.MCS_OK and same(res[0], host_bow_search(api, m, kf, cur, 100, None))
     assert list(res[0][1]) == expect, (list(res[0][1]), expect)
 
 
@@ -278,12 +184,12 @@ def test_one_big_node_and_disjoint_vectors(api, oa):
     kf = frame_of(split(d1, [1700, 1700]), ([17], [0, n], np.arange(n)), np.arange(n))
     cur = frame_of(split(d2, [3000, 400]), ([3, 17], [0, 0, n], rng.permutation(n)))
     m = api.cORBmatcher(0.8, False, 32, False)
-    res, st = device_search(api, m, [kf], cur, n, None)
-    h = host_search(api, m, kf, cur, n, None)
-    assert st == api.MCS_OK and same(res[0], h) and same(h, host_search(api, m, kf, cur, n, None, oa.search_by_bow)) and h[0] > 3000
+    res, st = device_bow_search(api, m, [kf], cur, n, None)
+    h = host_bow_search(api, m, kf, cur, n, None)
+    assert st == api.MCS_OK and same(res[0], h) and same(h, host_bow_search(api, m, kf, cur, n, None, oa.search_by_bow)) and h[0] > 3000
     # disjoint vectors: no match, both outputs all -1
     other = frame_of(cur["per"], ([3, 18], [0, 0, n], cur["fv"][2]))
-    res, st = device_search(api, m, [kf], other, n, None)
+    res, st = device_bow_search(api, m, [kf], other, n, None)
     assert st == api.MCS_OK and res[0][0] == 0 and np.all(res[0][1] == -1) and np.all(res[0][2] == -1)
     assert KEYPOINT_DTYPE.itemsize == 28
 
@@ -300,7 +206,7 @@ def test_full_chain_from_the_device_extractor(api, voc, cams, masks):
     H, W = imgs.shape[2:]
     pitch = (W + 63) // 64 * 64
     dev_images = torch.zeros((6, H, pitch), dtype=torch.uint8, device="cuda")
-    dev_images[:, :, :W] = torch.from_numpy(imgs.reshape(6, H, W)).cuda()
+    dev_images[:, :, :W] = on_device(imgs.reshape(6, H, W))
     masks_np = np.stack([synth.mirror_mask(c) for c in cams[:3]])
     packed = torch.zeros(rig.packed_layout(6, cap, 32)[1], dtype=torch.uint8, device="cuda")
     views = ex.extract_batch_packed_device(dev_images, masks_np, cams[:3], [0, 1, 2] * 2, packed, width=W)
@@ -318,7 +224,7 @@ def test_full_chain_from_the_device_extractor(api, voc, cams, masks):
     D = [np.concatenate([views["desc"][3 * f + c, :counts[3 * f + c]].cpu().numpy() for c in range(3)]) for f in range(2)]
     M = [np.concatenate([views["dmask"][3 * f + c, :counts[3 * f + c]].cpu().numpy() for c in range(3)]) for f in range(2)]
     mp = np.where(rng.random(len(D[0])) < 0.7, np.arange(len(D[0])), -1).astype(np.int32)
-    mp_t = torch.from_numpy(api.contiguous_to_slots(mp, counts[:3], cap)).cuda()
+    mp_t = to_slots(api, counts[:3], mp, cap, -1)
     mt = api.cORBmatcher(0.9, False, 32, masks)
     torch.cuda.current_stream().synchronize()
     mmp, msl, nm, st = mt.SearchByBoWDevice([(bows[0], mp_t)], bows[1], len(D[0]), stream=s)
@@ -327,10 +233,10 @@ def test_full_chain_from_the_device_extractor(api, voc, cams, masks):
     n_h, m_h = mt.SearchByBoWFrame(D[0], fv[0], D[1], fv[1], M[0] if masks else None, M[1] if masks else None, (mp >= 0).astype(np.uint8))
     assert int(st.item()) == api.MCS_OK and int(nm[0].item()) == n_h and n_h > 100
     sl = api.slots_to_contiguous(msl[0].cpu().numpy(), counts[3:], cap)
-    assert np.array_equal(np.where(sl >= 0, to_contiguous(np.maximum(sl, 0), counts[:3], cap), -1), m_h)
+    assert np.array_equal(np.where(sl >= 0, slot_to_contiguous_index(np.maximum(sl, 0), counts[:3], cap), -1), m_h)
     assert np.array_equal(api.slots_to_contiguous(mmp[0].cpu().numpy(), counts[3:], cap), np.where(m_h >= 0, mp[np.maximum(m_h, 0)], -1))
     for f in range(2):
         bw, bv, (fn, fo, ff) = bows[f].host()
         hw, hv, _ = v.transform(D[f])
         assert np.array_equal(bw, hw) and np.array_equal(bv, hv) and np.array_equal(fn, fv[f][0]) and np.array_equal(fo, fv[f][1])
-        assert np.array_equal(to_contiguous(ff, counts[3 * f:3 * f + 3], cap), fv[f][2])
+        assert np.array_equal(slot_to_contiguous_index(ff, counts[3 * f:3 * f + 3], cap), fv[f][2])

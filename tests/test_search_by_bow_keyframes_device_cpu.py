@@ -8,18 +8,10 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
+from device_frames import FAKE, counts, declared_symbols, frames, taped_rm  # noqa: F401  (frames: a fixture)
+from search_scenes import bow_kf_scene, host_bow_kf, max_count, reference_bow_kf
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
-BIG_ID = 1 << 30    # map-point id of the slots at or beyond a camera's count: reading one would raise the status
-frames = T.frames
-
-
-@pytest.fixture(scope="module")
-def rm():
-    """the reference's own matcher, live while recording and replayed from tests/golden/ref_tape_search_by_bow_keyframes_device_cpu.*"""
-    import ref_tape
-    return ref_tape.module("ref_match_api", "search_by_bow_keyframes_device_cpu", T.TAPE_LIMIT)
+rm = taped_rm("search_by_bow_keyframes_device_cpu")
 
 
 def _call(api, kf1=(FAKE, 1, 4, 0), mp1=FAKE, kfs=((FAKE, 1, 4, 0),), mps=None, n_kf=None, n_cams=4, capacity=2000, dim=32, n_points=500,
@@ -66,92 +58,8 @@ def test_validation(api):
 
 
 def test_symbol_is_declared_and_exported(api):
-    from test_cabi_symbols import declared_symbols
     assert "mcs_search_by_bow_keyframes_device" in declared_symbols() and hasattr(api.lib(), "mcs_search_by_bow_keyframes_device")
     assert callable(api.cORBmatcher.SearchByBoWKeyFramesDevice) and callable(api.cORBmatcher.SearchByBoWKeyFramesHost)
-
-
-# ---- the scenes ------------------------------------------------------------------------------------------------------------------
-def counts(F):
-    return [int((F.key_cam == c).sum()) for c in range(len(F.cam_w))]
-
-
-def max_count(s):
-    """the most keypoints a camera of the scene's frames holds"""
-    return max(max(counts(F)) for F in [s["KF1"]] + s["cands"])
-
-
-def widen(api, F, dim):
-    """F with 16- or 64-byte rows made from its 32-byte ones (first half / row and its bitwise complement-ish variant)"""
-    if dim == 32:
-        return F
-    w = (lambda d: np.ascontiguousarray(d[:, :16])) if dim == 16 else (lambda d: np.ascontiguousarray(np.concatenate([d, d ^ 0x5A], 1)))
-    return api.Frame(F.keys, F.key_cam, w(F.desc), w(F.dmask), list(zip(F.cam_w, F.cam_h)), F.scale_factors)
-
-
-def bow_kf_scene(api, frames, n_kf, seed=5, dim=32):
-    """KF1 = the first frame, about 60 % of its keypoints carrying map points 0 ..; candidate k a variant of either frame (a few bits
-    flipped per descriptor, more for later candidates) carrying points of its own; about 5 % of all points bad."""
-    F1, F2 = frames
-    rng = np.random.default_rng(seed)
-    KF1 = widen(api, F1, dim)
-    n1 = len(F1.keys)
-    mp1 = np.where(rng.random(n1) < 0.6, np.arange(n1), -1).astype(np.int32)
-    cands, mps, off = [], [], n1
-    for k in range(n_kf):
-        B = F2 if k % 2 else F1
-        F = api.Frame(B.keys, B.key_cam, T.flip_bits(rng, B.desc, 2 + k % 6), B.dmask, list(zip(B.cam_w, B.cam_h)), B.scale_factors)
-        cands.append(widen(api, F, dim))
-        n = len(B.keys)
-        mps.append(np.where(rng.random(n) < 0.6, off + np.arange(n), -1).astype(np.int32))
-        off += n
-    bad = (rng.random(off) < 0.05).astype(np.uint8)
-    return dict(KF1=KF1, mp1=mp1, cands=cands, mps=mps, bad=bad, n_points=off)
-
-
-def pack_frames(KFs, cap, layout, device="cpu"):
-    """one (packed uint8 tensor, n_parts, part_images, first_image) per frame.  single: each frame alone in its buffer with a decoy
-    image before and after its cameras; parts: every camera a one-image part of one buffer (an allgather); joint: all frames' cameras
-    as images of one single-part buffer."""
-    import torch
-    from multicol_slam_b200 import rig
-    dim = KFs[0].desc.shape[1]
-    t = lambda b: torch.from_numpy(b).to(device)  # noqa: E731
-    per = [[(F.keys[F.key_cam == c], F.desc[F.key_cam == c], F.dmask[F.key_cam == c]) for c in range(len(F.cam_w))] for F in KFs]
-    nc = len(per[0])
-    if layout == "single":
-        out = []
-        for p in per:
-            k, d, m = p[0]
-            decoy = (k[::-1].copy(), d[::-1].copy(), m[::-1].copy())
-            out.append((t(rig.pack([decoy] + p + [decoy], cap, dim)), 1, nc + 2, 1))
-        return out
-    if layout == "parts":
-        b = t(np.concatenate([rig.pack([c], cap, dim) for p in per for c in p]))
-        return [(b, nc * len(per), 1, nc * i) for i in range(len(per))]
-    b = t(rig.pack([c for p in per for c in p], cap, dim))
-    return [(b, 1, nc * len(per), nc * i) for i in range(len(per))]
-
-
-def slot_row(api, F, mp, cap, fill=BIG_ID, device="cpu"):
-    import torch
-    return torch.from_numpy(api.contiguous_to_slots(np.asarray(mp, np.int32), counts(F), cap, fill=fill)).to(device)
-
-
-def host_route(api, m, s, cap, layout="single", device="cpu", _bf=None, cands=None):
-    """SearchByBoWKeyFramesHost on the scene -> (matches12, match_slot, nmatches, status)"""
-    import torch
-    idx = range(len(s["cands"])) if cands is None else cands
-    packs = pack_frames([s["KF1"]] + [s["cands"][k] for k in idx], cap, layout, device)
-    kfs = [(packs[1 + i], slot_row(api, s["cands"][k], s["mps"][k], cap, device=device)) for i, k in enumerate(idx)]
-    return m.SearchByBoWKeyFramesHost(packs[0], slot_row(api, s["KF1"], s["mp1"], cap, device=device), kfs, len(s["KF1"].cam_w), cap,
-                                      s["n_points"], torch.from_numpy(s["bad"]).to(device), _bf=_bf)
-
-
-def reference_bow_kf(rm, cams, s, k, nnratio, masks):
-    """the reference's SearchByBoW(KF1, KF_k): (nmatches, map-point id per KF1 keypoint in contiguous order)"""
-    table = rm.MPTable(3, np.zeros((s["n_points"], 32), np.uint8), bad=s["bad"])
-    return rm.search_by_bow_kfkf(rm.KF(s["KF1"], cams, mp=s["mp1"]), rm.KF(s["cands"][k], cams, mp=s["mps"][k]), table, nnratio, masks)
 
 
 @pytest.mark.parametrize("masks", [False, True])
@@ -162,7 +70,7 @@ def test_host_route_equals_reference(oa, rm, api, frames, cams, masks):
     s["cands"].append(s["KF1"]); s["mps"].append(s["mp1"])
     m = api.cORBmatcher(0.75, False, 32, masks)
     cap = max_count(s) + 3
-    m12, slot12, nm, st = host_route(api, m, s, cap, _bf=oa.match_bruteforce)
+    m12, slot12, nm, st = host_bow_kf(api, m, s, cap, _bf=oa.match_bruteforce)
     assert st[0] == api.MCS_OK
     for k in range(len(s["cands"])):
         rn, rout = reference_bow_kf(rm, cams, s, k, 0.75, masks)

@@ -5,18 +5,10 @@ is integer: bit for bit, matches12, match_slot, nmatches and status."""
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
-from test_search_by_bow_keyframes_device_cpu import bow_kf_scene, counts, max_count, host_route, pack_frames, reference_bow_kf, slot_row
+from device_frames import BIG_ID, GUARD, SIZES, counts, frames, from_slots, on_device, pack_frames, rm, to_slots  # noqa: F401  (frames, rm: fixtures)
+from search_scenes import bow_kf_scene, host_bow_kf, host_sim3, max_count, reference_bow_kf, sim3_scene
 
 pytestmark = pytest.mark.gpu
-frames = T.frames
-GUARD = -999
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
 
 
 def device_route(api, m, s, cap, layout="single", cands=None, stream=None, bad=True, mp1=None, mps=None, guard=True):
@@ -25,27 +17,25 @@ def device_route(api, m, s, cap, layout="single", cands=None, stream=None, bad=T
     import torch
     idx = list(range(len(s["cands"]))) if cands is None else cands
     mps = s["mps"] if mps is None else mps
-    packs = pack_frames([s["KF1"]] + [s["cands"][k] for k in idx], cap, layout, "cuda")
-    kfs = [(packs[1 + i], slot_row(api, s["cands"][k], mps[k], cap, device="cuda")) for i, k in enumerate(idx)]
+    packs = pack_frames([s["KF1"]] + [s["cands"][k] for k in idx], cap, layout=layout)
+    kfs = [(packs[1 + i], to_slots(api, s["cands"][k], mps[k], cap, BIG_ID)) for i, k in enumerate(idx)]
     nc, ns = len(s["KF1"].cam_w), len(s["KF1"].cam_w) * cap
     out = None
     if guard:
         out = (torch.full((len(idx), ns), GUARD, dtype=torch.int32, device="cuda"), torch.full((len(idx), ns), GUARD, dtype=torch.int32, device="cuda"),
                torch.full((len(idx),), GUARD, dtype=torch.int32, device="cuda"), torch.full((1,), GUARD, dtype=torch.int32, device="cuda"))
-    bad_t = torch.from_numpy(s["bad"]).cuda() if bad else None
-    r = m.SearchByBoWKeyFramesDevice(packs[0], slot_row(api, s["KF1"], s["mp1"] if mp1 is None else mp1, cap, device="cuda"), kfs, nc, cap,
+    bad_t = on_device(s["bad"]) if bad else None
+    r = m.SearchByBoWKeyFramesDevice(packs[0], to_slots(api, s["KF1"], s["mp1"] if mp1 is None else mp1, cap, BIG_ID), kfs, nc, cap,
                                      s["n_points"], bad_t, stream=stream, out=out)
     torch.cuda.synchronize()
     m12, sl, nm, st = (t.cpu().numpy() for t in r)
-    live = np.zeros((nc, cap), bool)
-    for c, n in enumerate(counts(s["KF1"])):
-        live[c, :n] = True
-    live = live.reshape(-1)
-    if guard:
-        assert (m12[:, ~live] == GUARD).all() and (sl[:, ~live] == GUARD).all()
-    m12[:, ~live] = -1
-    sl[:, ~live] = -1
-    return m12, sl, nm, st
+    cc = counts(s["KF1"])
+
+    def live(rows):
+        """-1 at and beyond each count, after checking those slots still hold GUARD"""
+        back = [from_slots(api, row, cc, cap, GUARD) if guard else api.slots_to_contiguous(row, cc, cap) for row in rows]
+        return np.array([api.contiguous_to_slots(b, cc, cap) for b in back], np.int32).reshape(rows.shape)
+    return live(m12), live(sl), nm, st
 
 
 def _same(a, b):
@@ -62,12 +52,12 @@ def test_parity(api, oa, rm, frames, cams, masks, dim, layout):
     m = api.cORBmatcher(0.75, False, dim, masks)
     cap = max_count(s) + 3
     d = device_route(api, m, s, cap, layout)
-    h = host_route(api, m, s, cap, layout, "cuda")
-    o = host_route(api, m, s, cap, _bf=oa.match_bruteforce)
+    h = host_bow_kf(api, m, s, cap, layout, "cuda")
+    o = host_bow_kf(api, m, s, cap, _bf=oa.match_bruteforce)
     assert _same(d, h) and _same(d, o) and d[3][0] == api.MCS_OK and (d[2] > 20).all()
     # match_slot names a candidate slot holding the id in matches12
     for k, F in enumerate(s["cands"]):
-        row = slot_row(api, F, s["mps"][k], cap).numpy()
+        row = to_slots(api, F, s["mps"][k], cap, BIG_ID, "cpu").numpy()
         hit = d[1][k] >= 0
         assert np.array_equal(row[d[1][k][hit]], d[0][k][hit])
     if rm and dim == 32:
@@ -85,7 +75,7 @@ def test_batch_equals_single_calls(api, frames):
     for k in range(16):
         one = device_route(api, m, s, cap, "single", cands=[k])
         assert all(np.array_equal(a[k], b[0]) for a, b in zip(d[:3], one[:3])), k
-    assert _same(d, host_route(api, m, s, cap, "parts", "cuda"))
+    assert _same(d, host_bow_kf(api, m, s, cap, "parts", "cuda"))
 
 
 def _frame(api, per_cam_desc, dim):
@@ -96,7 +86,7 @@ def _frame(api, per_cam_desc, dim):
         k["x"] = np.arange(len(d)) % 700 + 10; k["y"] = np.arange(len(d)) // 700 + 10
         keys.append(k); cam += [c] * len(d); desc.append(np.asarray(d, np.uint8).reshape(-1, dim))
     D = np.concatenate(desc)
-    return api.Frame(np.concatenate(keys), np.asarray(cam, np.int32), D, np.full_like(D, 0xFF), T.SIZES, [1.2 ** i for i in range(8)])
+    return api.Frame(np.concatenate(keys), np.asarray(cam, np.int32), D, np.full_like(D, 0xFF), SIZES, [1.2 ** i for i in range(8)])
 
 
 def _flip(base, bits):
@@ -137,7 +127,7 @@ def test_contention_rescans(api, oa):
     m = api.cORBmatcher(0.9, False, 32, False)
     cap = 48
     d = device_route(api, m, s, cap)
-    assert _same(d, host_route(api, m, s, cap, "single", "cuda")) and _same(d, host_route(api, m, s, cap, _bf=oa.match_bruteforce))
+    assert _same(d, host_bow_kf(api, m, s, cap, "single", "cuda")) and _same(d, host_bow_kf(api, m, s, cap, _bf=oa.match_bruteforce))
     for k, F in enumerate(s["cands"]):
         row = api.slots_to_contiguous(d[1][k], counts(s["KF1"]), cap)[15:35]      # KF1's cluster queries (camera 0): candidate slots
         desc_of = dict(zip(api.slots_to_contiguous(np.arange(3 * cap, dtype=np.int32), counts(F), cap).tolist(), F.desc))
@@ -167,7 +157,7 @@ def test_decision_edges(api, oa, nnratio):
              bad=np.zeros(21, np.uint8), n_points=21)
     cap = 9                                                                       # camera 0 of the candidate at capacity
     d = device_route(api, m, s, cap)
-    assert _same(d, host_route(api, m, s, cap, "single", "cuda")) and _same(d, host_route(api, m, s, cap, _bf=oa.match_bruteforce))
+    assert _same(d, host_bow_kf(api, m, s, cap, "single", "cuda")) and _same(d, host_bow_kf(api, m, s, cap, _bf=oa.match_bruteforce))
     row = api.slots_to_contiguous(d[1][0], counts(KF1), cap)
     if nnratio < 1:
         assert row.tolist() == [0, -1, -1, -1, cap, -1, -1] and d[2][0] == 2
@@ -188,20 +178,20 @@ def test_invalid_ids_bad_and_empty_camera(api, frames):
     i1, i2 = int(np.flatnonzero(mp1 >= 0)[4]), int(np.flatnonzero(mps[1] >= 0)[9])
     mp1[i1], mps[1][i2] = s["n_points"] + 4, s["n_points"] + 7
     d = device_route(api, m, s, cap, mp1=mp1, mps=mps)
-    h = host_route(api, m, dict(s, mp1=mp1, mps=mps), cap, "single", "cuda")
+    h = host_bow_kf(api, m, dict(s, mp1=mp1, mps=mps), cap, "single", "cuda")
     assert d[3][0] == h[3][0] == api.MCS_ERR_INVALID and _same(d[:3], h[:3])
     clean1, cleans = mp1.copy(), [r.copy() for r in mps]
     clean1[i1], cleans[1][i2] = -1, -1
-    assert _same(d[:3], host_route(api, m, dict(s, mp1=clean1, mps=cleans), cap, "single", "cuda")[:3])
+    assert _same(d[:3], host_bow_kf(api, m, dict(s, mp1=clean1, mps=cleans), cap, "single", "cuda")[:3])
     # bad_dev NULL is "no point is bad"
     d = device_route(api, m, s, cap, bad=False)
-    assert d[3][0] == api.MCS_OK and _same(d, host_route(api, m, dict(s, bad=np.zeros_like(s["bad"])), cap, "single", "cuda"))
+    assert d[3][0] == api.MCS_OK and _same(d, host_bow_kf(api, m, dict(s, bad=np.zeros_like(s["bad"])), cap, "single", "cuda"))
     # a candidate whose camera 1 holds no keypoint
     F = s["cands"][0]
     keep = F.key_cam != 1
-    s2 = dict(s, cands=[api.Frame(F.keys[keep], F.key_cam[keep], F.desc[keep], F.dmask[keep], T.SIZES, F.scale_factors)] + s["cands"][1:],
+    s2 = dict(s, cands=[api.Frame(F.keys[keep], F.key_cam[keep], F.desc[keep], F.dmask[keep], SIZES, F.scale_factors)] + s["cands"][1:],
               mps=[s["mps"][0][keep]] + s["mps"][1:])
-    assert _same(device_route(api, m, s2, cap, "joint"), host_route(api, m, s2, cap, "joint", "cuda"))
+    assert _same(device_route(api, m, s2, cap, "joint"), host_bow_kf(api, m, s2, cap, "joint", "cuda"))
     # a busy stream: the call waits for the work queued before it
     st_ = torch.cuda.Stream()
     with torch.cuda.stream(st_):
@@ -210,34 +200,32 @@ def test_invalid_ids_bad_and_empty_camera(api, frames):
             big = big @ big
             big /= big.norm()
         d = device_route(api, m, s, cap, "parts", stream=st_)
-    assert _same(d, host_route(api, m, s, cap, "parts", "cuda"))
+    assert _same(d, host_bow_kf(api, m, s, cap, "parts", "cuda"))
 
 
 def test_feeds_search_by_sim3(api, oa, frames, cams):
     """ComputeSim3's first two steps on the device: a candidate's matches12_dev row goes as it is into mcs_search_by_sim3_device
     (every match an inlier), and gives what the host composition gives"""
     import torch
-    from test_sim3_searches_device_cpu import host_sim3, sim3_scene
     s3 = sim3_scene(api, oa, cams, frames[0])
     m = api.cORBmatcher(0.75, False, 32, True)
     s = dict(KF1=s3["KF1"], mp1=s3["mp1"], cands=[s3["KF2"]], mps=[s3["mp2"]], bad=s3["bad"], n_points=len(s3["world"]))
     cap = max(counts(s3["KF1"])) + 2
-    packs = pack_frames([s3["KF1"], s3["KF2"]], cap, "parts", "cuda")
-    mp1_t, mp2_t = slot_row(api, s3["KF1"], s3["mp1"], cap, device="cuda"), slot_row(api, s3["KF2"], s3["mp2"], cap, device="cuda")
-    bad_t = torch.from_numpy(s3["bad"]).cuda()
+    packs = pack_frames([s3["KF1"], s3["KF2"]], cap, layout="parts")
+    mp1_t, mp2_t = to_slots(api, s3["KF1"], s3["mp1"], cap, BIG_ID), to_slots(api, s3["KF2"], s3["mp2"], cap, BIG_ID)
+    bad_t = on_device(s3["bad"])
     m12_t, slot_t, nm_t, st_t = m.SearchByBoWKeyFramesDevice(packs[0], mp1_t, [(packs[1], mp2_t)], 3, cap, s["n_points"], bad_t)
-    hm12, hslot, hnm, _ = host_route(api, m, s, cap, "parts", "cuda")
+    hm12, hslot, hnm, _ = host_bow_kf(api, m, s, cap, "parts", "cuda")
     assert np.array_equal(m12_t.cpu().numpy()[0], hm12[0]) and int(nm_t[0]) == hnm[0] > 30 and int(st_t[0]) == api.MCS_OK
     pre = api.slots_to_contiguous(hm12[0], counts(s3["KF1"]), cap)
     a2 = np.zeros(cap * 3, np.uint8)                                # vbAlreadyMatched2: the KF2 slots the BoW matches hold
     a2[hslot[0][hslot[0] >= 0]] = 1
     row = m12_t[0].clone()
-    dn, dst, out = m.SearchBySim3Device(packs[0], packs[1], cap, s3["rig1"], s3["rig2"], torch.from_numpy(np.stack(s3["rig1"].masks)).cuda(),
-                                        s3["KF1"].scale_factors, mp1_t, mp2_t, torch.from_numpy(np.asarray(s3["world"], np.float64)).cuda(),
-                                        torch.from_numpy(np.asarray(s3["min_d"], np.float64)).cuda(),
-                                        torch.from_numpy(np.asarray(s3["max_d"], np.float64)).cuda(), torch.from_numpy(s3["desc"]).cuda(),
-                                        torch.from_numpy(s3["dmask"]).cuda(), s3["s12"], s3["R12"], s3["t12"], 10.0, row,
-                                        already2_t=torch.from_numpy(a2).cuda(), bad_t=bad_t)
+    dn, dst, out = m.SearchBySim3Device(packs[0], packs[1], cap, s3["rig1"], s3["rig2"], on_device(np.stack(s3["rig1"].masks)),
+                                        s3["KF1"].scale_factors, mp1_t, mp2_t, on_device(np.asarray(s3["world"], np.float64)),
+                                        on_device(np.asarray(s3["min_d"], np.float64)), on_device(np.asarray(s3["max_d"], np.float64)),
+                                        on_device(s3["desc"]), on_device(s3["dmask"]), s3["s12"], s3["R12"], s3["t12"], 10.0, row,
+                                        already2_t=on_device(a2), bad_t=bad_t)
     torch.cuda.synchronize()
     hn, h12 = host_sim3(m, s3, 10.0, pre=pre)
     assert int(dst[0]) == api.MCS_OK and int(dn[0]) == hn and np.array_equal(api.slots_to_contiguous(out.cpu().numpy(), counts(s3["KF1"]), cap), h12)

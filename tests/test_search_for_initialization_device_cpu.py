@@ -3,7 +3,7 @@
 with MCS_ERR_NO_DEVICE."""
 import numpy as np
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
+from device_frames import FAKE, declared_symbols
 
 
 def _search(api, f1=(FAKE, 1, 4, 0), f2=(FAKE, 1, 4, 0), n_cams=4, capacity=4000, dim=32, sizes=None, prev=FAKE, m12=FAKE, nm=FAKE,
@@ -61,7 +61,6 @@ def test_seed_validation(api):
 
 
 def test_symbols_are_declared_and_exported(api):
-    from test_cabi_symbols import declared_symbols
     for name in ("mcs_search_for_initialization_device", "mcs_search_for_initialization_seed_device"):
         assert name in declared_symbols()
         assert hasattr(api.lib(), name)

@@ -6,22 +6,10 @@ conversion and prev are compared bit for bit; the slots beyond each camera's cou
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
-from test_search_projection_device_gpu import FILL, _flip
-from test_search_projection_last_device_gpu import _pack
+from device_frames import PREV_FILL, SIZES, flip, keep_cameras, rm  # noqa: F401  (rm: a fixture)
+from device_searches import collect_init, device_init, host_init, init_inputs, launch_init
 
 pytestmark = pytest.mark.gpu
-PREV_FILL = -7777.25        # prev value of the slots beyond a camera's count
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
-
-
-def _counts(F):
-    return [int((F.key_cam == c).sum()) for c in range(len(F.cam_w))]
 
 
 def init_frames(api, cams, masks, n=2, nfeatures=800):
@@ -30,63 +18,8 @@ def init_frames(api, cams, masks, n=2, nfeatures=800):
     ex = api.mdBRIEFextractorOct(nfeatures=nfeatures, fastThreshold=5, do_dBrief=True, learnMasks=masks)
     sf = [ex.info.scale_factor[l] for l in range(8)]
     streams = [synth.texture_stream(cams[c], n, seed=40 + c) for c in range(3)]
-    return [api.Frame.from_cameras([ex(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], T.SIZES, sf)
+    return [api.Frame.from_cameras([ex(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], SIZES, sf)
             for t in range(n)]
-
-
-def _prev_slots(prev, counts, cap):
-    out = np.full((len(counts), cap, 2), PREV_FILL)
-    o = 0
-    for c, n in enumerate(counts):
-        out[c, :n] = prev[o:o + n]
-        o += n
-    return out.reshape(-1)
-
-
-def _prepare(api, F1, F2, prev, layout="single", cap=None, seed=3):
-    import torch
-    c1, c2 = _counts(F1), _counts(F2)
-    cap = cap or max(c1 + c2) + 5
-    f2, f1 = _pack(F2, F1, layout, cap, F1.desc.shape[1])
-    junk = np.random.default_rng(seed).integers(-1, 600, len(F1.keys)).astype(np.int32)
-    return dict(f1=f1, f2=f2, cap=cap, c1=c1, c2=c2, sizes=list(zip(F1.cam_w.tolist(), F1.cam_h.tolist())),
-                prev_t=torch.from_numpy(_prev_slots(np.asarray(prev, np.float64), c1, cap)).cuda(),
-                m12_t=torch.from_numpy(api.contiguous_to_slots(junk, c1, cap, fill=FILL)).cuda())
-
-
-def _launch(m, d, window, stream=None):
-    return m.SearchForInitializationDevice(d["f1"], d["f2"], d["cap"], d["sizes"], d["prev_t"], window, d["m12_t"], stream=stream, diag=True)
-
-
-def _collect(api, d, n_t, m12_t, diag_t):
-    """-> (nmatches, contiguous matches12 as contiguous F2 indices, contiguous prev [n1, 2], diag), checking the untouched slots"""
-    cap, c1, c2 = d["cap"], d["c1"], d["c2"]
-    m = m12_t.cpu().numpy()
-    p = d["prev_t"].cpu().numpy().reshape(len(c1), cap, 2)
-    for c in range(len(c1)):
-        assert np.all(m[c * cap + c1[c]:(c + 1) * cap] == FILL) and np.all(p[c, c1[c]:] == PREV_FILL)
-    m = api.slots_to_contiguous(m, c1, cap)
-    off2 = np.concatenate([[0], np.cumsum(c2)])
-    s = np.maximum(m, 0)
-    cam, j = s // cap, s % cap
-    assert np.all(j[m >= 0] < np.asarray(c2)[cam[m >= 0]])
-    m12 = np.where(m >= 0, off2[cam] + j, -1).astype(np.int32)
-    prev = np.concatenate([p[c, :c1[c]] for c in range(len(c1))])
-    return int(n_t.item()), m12, prev, diag_t.cpu().numpy()
-
-
-def device_init(api, m, F1, F2, prev, window, layout="single", cap=None):
-    import torch
-    d = _prepare(api, F1, F2, prev, layout, cap)
-    res = _launch(m, d, window)
-    torch.cuda.synchronize()
-    return _collect(api, d, *res)
-
-
-def host_init(m, F1, F2, prev, window):
-    p = np.array(prev, np.float64, copy=True)
-    n, m12 = m.SearchForInitialization(F1, F2, p, window)
-    return n, m12, p
 
 
 def _same(a, b):
@@ -118,7 +51,7 @@ def test_seed_and_chained_frames(api, cams):
     fr = init_frames(api, cams, True, n=5)
     F1 = fr[0]
     m = api.cORBmatcher(0.9, False, 32, True)
-    d = _prepare(api, F1, fr[1], np.zeros((len(F1.keys), 2)))
+    d = init_inputs(api, F1, fr[1], np.zeros((len(F1.keys), 2)))
     m.SearchForInitializationSeedDevice(d["f1"], 3, d["cap"], d["prev_t"])
     torch.cuda.synchronize()
     p = d["prev_t"].cpu().numpy().reshape(3, d["cap"], 2)
@@ -129,11 +62,11 @@ def test_seed_and_chained_frames(api, cams):
         h = host_init(m, F1, F2, hp, 50)
         hp = h[2]
         # the same packed F1 and prev tensor every call; F2 packed anew
-        d2 = _prepare(api, F1, F2, np.zeros((len(F1.keys), 2)), cap=d["cap"])
+        d2 = init_inputs(api, F1, F2, np.zeros((len(F1.keys), 2)), cap=d["cap"])
         d2["f1"], d2["prev_t"] = d["f1"], d["prev_t"]
-        res = _launch(m, d2, 50)
+        res = launch_init(m, d2, 50)
         torch.cuda.synchronize()
-        g = _collect(api, d2, *res)
+        g = collect_init(api, d2, *res)
         assert _same(h, g[:3]) and h[0] > 100
 
 
@@ -144,7 +77,7 @@ def test_descriptor_sizes(api, oa, cams, dim, masks):
     ex = oa.OracleExtractor(nfeatures=400, fast_threshold=5, do_dbrief=True, learn_masks=True, desc_size=dim)
     streams = [synth.texture_stream(cams[c], 2, seed=60 + c) for c in range(3)]
     sf = [float(ex.info.scale_factor[l]) for l in range(8)]
-    F1, F2 = [api.Frame.from_cameras([ex.extract(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], T.SIZES, sf)
+    F1, F2 = [api.Frame.from_cameras([ex.extract(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], SIZES, sf)
               for t in range(2)]
     assert F1.desc.shape[1] == dim
     m = api.cORBmatcher(0.9, False, dim, masks)
@@ -159,7 +92,7 @@ def _frame(api, per_cam0, dim=32):
     """camera 0 holds (kps, desc); cameras 1 and 2 are empty"""
     e = np.zeros(0, api.KEYPOINT_DTYPE), np.zeros((0, dim), np.uint8), None
     k, dsc = per_cam0
-    return api.Frame.from_cameras([(k, dsc, None), e, e], T.SIZES, np.cumprod([1.0] + [1.2000000476837158] * 7))
+    return api.Frame.from_cameras([(k, dsc, None), e, e], SIZES, np.cumprod([1.0] + [1.2000000476837158] * 7))
 
 
 def _kps(api, xy):
@@ -185,27 +118,27 @@ def displacement_scene(api, rng, dim=32):
     t0 = target((100.0, 100.0), base)
     chain = [62, 58, 51, 47, 40, 33, 29, 22, 17, 11, 6, 2]
     for i, d in enumerate(chain):
-        query((100.0 + 0.5 * i, 100.0), _flip(rng, base, d), t0 if i == len(chain) - 1 else -1)
-    query((101.0, 101.0), _flip(rng, base, 2), -1)
-    query((101.0, 100.5), _flip(rng, base, 3), -1)
-    query((101.0, 99.0), _flip(rng, base, 1), t0)         # ... and one below it takes it again
+        query((100.0 + 0.5 * i, 100.0), flip(rng, base, d), t0 if i == len(chain) - 1 else -1)
+    query((101.0, 101.0), flip(rng, base, 2), -1)
+    query((101.0, 100.5), flip(rng, base, 3), -1)
+    query((101.0, 99.0), flip(rng, base, 1), t0)         # ... and one below it takes it again
     expect[len(chain) - 1] = -1
     # d0 == th_low accepted, th_low + 1 rejected (one candidate each: second = INT_MAX)
     b1, b2 = (rng.integers(0, 256, dim).astype(np.uint8) for _ in range(2))
     t1 = target((200.0, 100.0), b1)
-    query((200.0, 100.0), _flip(rng, b1, 2 * dim), t1)
+    query((200.0, 100.0), flip(rng, b1, 2 * dim), t1)
     target((300.0, 100.0), b2)
-    query((300.0, 100.0), _flip(rng, b2, 2 * dim + 1), -1)
+    query((300.0, 100.0), flip(rng, b2, 2 * dim + 1), -1)
     # an exact ratio tie: 9 against 10 at 0.9 (9 < 9.0 fails)
     b3 = rng.integers(0, 256, dim).astype(np.uint8)
-    q3 = _flip(rng, b3, 0)
-    target((400.0, 100.0), _flip(rng, b3, 9)); target((402.0, 101.0), _flip(rng, b3, 10))
+    q3 = flip(rng, b3, 0)
+    target((400.0, 100.0), flip(rng, b3, 9)); target((402.0, 101.0), flip(rng, b3, 10))
     query((401.0, 100.0), q3, -1)
     assert 9 >= 10 * 0.9
     # rescans: ten candidates at distances 1..10 from a query; seven earlier queries take the seven best with distance 0, so the
     # query's list of 8 holds one free entry and its window is scanned again: 8 against 9 passes (8 < 8.1)
     b4 = rng.integers(0, 256, dim).astype(np.uint8)
-    cands = [_flip(rng, b4, d) for d in range(1, 11)]
+    cands = [flip(rng, b4, d) for d in range(1, 11)]
     ids = [target((500.0 + 1.5 * (i % 5), 100.0 + 2.0 * (i // 5)), cands[i]) for i in range(10)]
     for i in range(7):
         query((503.0, 101.0), cands[i], ids[i])
@@ -252,7 +185,7 @@ def test_equal_distances_earlier_visit_wins(api, oa):
     grid cell to the left of keypoint 0's"""
     rng = np.random.default_rng(5)
     base = rng.integers(0, 256, 32).astype(np.uint8)
-    F2 = _frame(api, (_kps(api, [(318.0, 200.0), (290.0, 200.0)]), np.stack([_flip(rng, base, 5), _flip(rng, base, 5)])))
+    F2 = _frame(api, (_kps(api, [(318.0, 200.0), (290.0, 200.0)]), np.stack([flip(rng, base, 5), flip(rng, base, 5)])))
     F1 = _frame(api, (_kps(api, [(304.0, 200.0)]), base[None, :].copy()))
     m = api.cORBmatcher(1.2, False, 32, False)
     prev = _kp_prev(F1)
@@ -264,10 +197,7 @@ def test_equal_distances_earlier_visit_wins(api, oa):
 def test_shapes(api, oa, cams):
     F1, F2 = init_frames(api, cams, True)
     m = api.cORBmatcher(0.9, False, 32, True)
-
-    def sub(F, keep):
-        i = np.flatnonzero(np.isin(F.key_cam, keep))
-        return api.Frame(F.keys[i], F.key_cam[i], F.desc[i], F.dmask[i], list(zip(F.cam_w, F.cam_h)), F.scale_factors)
+    sub = lambda F, keep: keep_cameras(api, F, keep)[0]  # noqa: E731
     # empty cameras in either frame
     for A, B in ((sub(F1, [0, 2]), F2), (F1, sub(F2, [1])), (sub(F1, [1]), sub(F2, [0, 1]))):
         prev = _kp_prev(A)
@@ -298,13 +228,13 @@ def test_call_does_not_wait_for_the_stream(api, cams):
     m = api.cORBmatcher(0.9, False, 32, True)
     prev = _kp_prev(F1)
     h = host_init(m, F1, F2, prev, 50)
-    d = _prepare(api, F1, F2, prev)
+    d = init_inputs(api, F1, F2, prev)
     torch.cuda.synchronize()
     st = torch.cuda.Stream()
     with torch.cuda.stream(st):
         torch.cuda._sleep(400_000_000)                  # a few hundred milliseconds of work ahead of the call
-        res = _launch(m, d, 50, stream=st)
+        res = launch_init(m, d, 50, stream=st)
         busy = st.query()
     assert busy is False
     st.synchronize()
-    assert _same(h, _collect(api, d, *res)[:3])
+    assert _same(h, collect_init(api, d, *res)[:3])

@@ -9,18 +9,10 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
-from test_search_by_bow_keyframes_device_cpu import counts, pack_frames, slot_row, widen
+from device_frames import BIG_ID, FAKE, counts, declared_symbols, frames, pack_frames, taped_rm, to_slots  # noqa: F401  (frames: a fixture)
+from search_scenes import essential, rays_of, reference_tri, rig_of, tri_scene
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
-frames = T.frames
-
-
-@pytest.fixture(scope="module")
-def rm():
-    """the reference's own matcher, live while recording and replayed from tests/golden/ref_tape_search_for_triangulation_device_cpu.*"""
-    import ref_tape
-    return ref_tape.module("ref_match_api", "search_for_triangulation_device_cpu", T.TAPE_LIMIT)
+rm = taped_rm("search_for_triangulation_device_cpu")
 
 
 def _call(api, kf1=(FAKE, 1, 4, 0), mp1=FAKE, kf2=(FAKE, 1, 4, 0), mp2=FAKE, n_cams=4, capacity=2000, dim=32, cams=True, E=True,
@@ -57,62 +49,16 @@ def test_validation(api):
 
 
 def test_symbol_is_declared_and_exported(api):
-    from test_cabi_symbols import declared_symbols
     assert "mcs_search_for_triangulation_device" in declared_symbols() and hasattr(api.lib(), "mcs_search_for_triangulation_device")
     assert callable(api.cORBmatcher.SearchForTriangulationRawDevice) and callable(api.cORBmatcher.SearchForTriangulationRawHost)
 
 
-# ---- the scenes ------------------------------------------------------------------------------------------------------------------
-def rig_of(api, cams, shift):
-    """make_scene's 3-camera rig (cameras 120 degrees apart) at a pose moved by `shift` metres"""
-    nc = 3
-    M_c = np.tile(np.eye(4), (nc, 1, 1))
-    for c in range(nc):
-        a = 2 * np.pi * c / nc
-        M_c[c, :3, :3] = np.array([[np.cos(a), 0, np.sin(a)], [0, 1, 0], [-np.sin(a), 0, np.cos(a)]])
-        M_c[c, :3, 3] = [0.1 * np.sin(a), 0.0, 0.1 * np.cos(a)]
-    M_t = np.eye(4)
-    M_t[:3, 3] = np.array([0.3, -0.2, 0.1]) + np.asarray(shift)
-    return api.Rig(cams, M_c, M_t)
-
-
-def essential(rig1, rig2):
-    """Es[i][j] = ComputeE(KF1.Get_MtMc_inv(i), KF2.Get_MtMc(j)) (ref :988-1001)"""
-    from multicol_slam_b200 import settings
-    return settings.essential_matrices(rig1.MtMc_inv, rig2.MtMc)
-
-
-def rays_of(api, F, cams):
-    """mvKeysRays: ImgToWorld of each keypoint's float position"""
-    return np.array([api.img_to_world(cams[int(F.key_cam[i])], float(k["x"]), float(k["y"])) for i, k in enumerate(F.keys)]).reshape(-1, 3)
-
-
-def tri_scene(api, frames, cams, n_nb, seed=3, dim=32, free=0.5):
-    """KF1 = the first frame with about `free` of its keypoints free (id -1) and the others carrying map points; neighbour k a
-    variant of either frame (a few bits flipped per descriptor, more for later neighbours) at a pose a few centimetres from KF1's,
-    with its own points.  Poses as rigs, for the reference and for E."""
-    F1, F2 = frames
-    rng = np.random.default_rng(seed)
-    n1 = len(F1.keys)
-    mp1 = np.where(rng.random(n1) < free, -1, np.arange(n1)).astype(np.int32)
-    nbs, mps, rigs, off = [], [], [], n1
-    for k in range(n_nb):
-        B = F2 if k % 2 else F1
-        F = api.Frame(B.keys, B.key_cam, T.flip_bits(rng, B.desc, 2 + k % 5), B.dmask, list(zip(B.cam_w, B.cam_h)), B.scale_factors)
-        nbs.append(widen(api, F, dim))
-        n = len(B.keys)
-        mps.append(np.where(rng.random(n) < free, -1, off + np.arange(n)).astype(np.int32))
-        rigs.append(rig_of(api, cams, rng.uniform(-0.04, 0.04, 3)))
-        off += n
-    return dict(KF1=widen(api, F1, dim), mp1=mp1, nbs=nbs, mps=mps, rig1=rig_of(api, cams, [0, 0, 0]), rigs=rigs, next_id=off)
-
-
 def host_route(api, m, s, k, cams, cap, mp1, mp2, layout="single", device="cpu", _st=None, epi=1e-2):
     """SearchForTriangulationRawHost(KF1, neighbour k) with the given contiguous map-point rows -> (nmatches, matches12 by slot)"""
-    packs = pack_frames([s["KF1"], s["nbs"][k]], cap, layout, device)
+    packs = pack_frames([s["KF1"], s["nbs"][k]], cap, layout=layout, device=device)
     E = essential(s["rig1"], s["rigs"][k])
-    return m.SearchForTriangulationRawHost(packs[0], slot_row(api, s["KF1"], mp1, cap, device=device), packs[1],
-                                           slot_row(api, s["nbs"][k], mp2, cap, device=device), cams, cap, E, epi, _st=_st)
+    return m.SearchForTriangulationRawHost(packs[0], to_slots(api, s["KF1"], mp1, cap, BIG_ID, device), packs[1],
+                                           to_slots(api, s["nbs"][k], mp2, cap, BIG_ID, device), cams, cap, E, epi, _st=_st)
 
 
 def pairs_of(api, s, k, m12, cap):
@@ -121,14 +67,6 @@ def pairs_of(api, s, k, m12, cap):
     s2 = api.slots_to_contiguous(np.arange(len(m12), dtype=np.int32), counts(s["nbs"][k]), cap)
     inv = {int(v): i for i, v in enumerate(s2)}
     return np.array([(i, inv[int(b)]) for i, b in enumerate(c1) if b >= 0], np.int32).reshape(-1, 2)
-
-
-def reference_tri(rm, api, s, k, cams, mp1, mp2, masks):
-    """the reference's SearchForTriangulationRaw(KF1, KF_k): (nmatches, vMatchedPairs)"""
-    r1, r2 = s["rig1"], s["rigs"][k]
-    k1 = rm.KF(s["KF1"], cams, M_c=r1.M_c, M_t=r1.M_t, mp=np.where(mp1 == -1, -1, 0).astype(np.int32), rays=rays_of(api, s["KF1"], cams))
-    k2 = rm.KF(s["nbs"][k], cams, M_c=r2.M_c, M_t=r2.M_t, mp=np.where(mp2 == -1, -1, 0).astype(np.int32), rays=rays_of(api, s["nbs"][k], cams))
-    return rm.search_for_triangulation_raw(k1, k2, rm.MPTable(3, np.zeros((1, 32), np.uint8)), 0.6, masks)
 
 
 def triangulate_stand_in(rng, s, k, m12, cap, mp1_slots, mp2_slots):

@@ -9,61 +9,22 @@ test's arithmetic: the threshold equal to a pair's residual rejects it on both r
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
-from test_search_by_bow_keyframes_device_cpu import counts, pack_frames, slot_row
-from test_search_for_triangulation_device_cpu import essential, rig_of, tri_scene
+from device_frames import counts, flip_bits, frames, keep_cameras, pack_frames, to_slots  # noqa: F401  (frames: a fixture)
+from device_searches import assert_same_tri, device_tri, host_tri, tri_inputs
+from search_scenes import epipolar_residual, essential, rig_of, tri_scene
 
 pytestmark = pytest.mark.gpu
-
-POISON = 7777       # matches12 at or beyond a camera's count: must survive the call
-frames = T.frames
-
-
-def device_inputs(api, KF1, KF2, mp1, mp2, cams, cap, layout="single", same=False):
-    """freshly packed frames, map-point rows with -1 (free) past the counts and poisoned outputs, all on the device:
-    (kf1, mp1_t, kf2, mp2_t, out)"""
-    import torch
-    packs = pack_frames([KF1] if same else [KF1, KF2], cap, layout, "cuda")
-    mp1_t = slot_row(api, KF1, mp1, cap, fill=-1, device="cuda")
-    mp2_t = mp1_t if same else slot_row(api, KF2, mp2, cap, fill=-1, device="cuda")
-    out = (torch.full((1,), -3, dtype=torch.int32, device="cuda"), torch.full((len(cams) * cap,), POISON, dtype=torch.int32, device="cuda"),
-           torch.full((2,), -3, dtype=torch.int32, device="cuda"))
-    torch.cuda.synchronize()
-    return packs[0], mp1_t, packs[0 if same else 1], mp2_t, out
-
-
-def device_call(api, m, KF1, KF2, mp1, mp2, cams, cap, E, layout="single", epi=1e-2, same=False):
-    """-> (nmatches, matches12, diag) of the device call, on the host"""
-    p1, mp1_t, p2, mp2_t, out = device_inputs(api, KF1, KF2, mp1, mp2, cams, cap, layout, same)
-    r = m.SearchForTriangulationRawDevice(p1, mp1_t, p2, mp2_t, cams, cap, E, epi, out=out, diag=True)
-    return int(r[0].item()), r[1].cpu().numpy(), r[2].cpu().numpy()
-
-
-def host_call(api, m, KF1, KF2, mp1, mp2, cams, cap, E, epi=1e-2, oa=None):
-    packs = pack_frames([KF1, KF2], cap, "single", "cpu")
-    return m.SearchForTriangulationRawHost(packs[0], slot_row(api, KF1, mp1, cap), packs[1], slot_row(api, KF2, mp2, cap), cams, cap, E, epi,
-                                           _st=None if oa is None else oa.search_for_triangulation)
-
-
-def assert_same(api, KF1, dev, host, cap):
-    """nmatches and every slot below KF1's counts equal; every slot at or beyond a count still poisoned"""
-    n, m12, _ = dev
-    hn, hm12 = host
-    assert n == hn
-    live = api.contiguous_to_slots(np.ones(len(KF1.keys), np.int32), counts(KF1), cap, fill=0).astype(bool)
-    assert np.array_equal(m12[live], hm12[live])
-    assert (m12[~live] == POISON).all()
 
 
 def compare(api, m, s, k, cams, cap, mp1=None, mp2=None, layout="single", epi=1e-2, oa=None):
     mp1 = s["mp1"] if mp1 is None else mp1
     mp2 = s["mps"][k] if mp2 is None else mp2
     E = essential(s["rig1"], s["rigs"][k])
-    dev = device_call(api, m, s["KF1"], s["nbs"][k], mp1, mp2, cams, cap, E, layout, epi)
-    host = host_call(api, m, s["KF1"], s["nbs"][k], mp1, mp2, cams, cap, E, epi)
-    assert_same(api, s["KF1"], dev, host, cap)
+    dev = device_tri(api, m, s["KF1"], s["nbs"][k], mp1, mp2, cams, cap, E, layout, epi)
+    host = host_tri(api, m, s["KF1"], s["nbs"][k], mp1, mp2, cams, cap, E, epi)
+    assert_same_tri(api, s["KF1"], dev, host, cap)
     if oa is not None:
-        ho = host_call(api, m, s["KF1"], s["nbs"][k], mp1, mp2, cams, cap, E, epi, oa)
+        ho = host_tri(api, m, s["KF1"], s["nbs"][k], mp1, mp2, cams, cap, E, epi, oa)
         assert host[0] == ho[0] and np.array_equal(host[1], ho[1])
     free1 = int((np.asarray(mp1) == -1).sum())
     assert dev[2][0] == free1                                          # diag: the queries
@@ -127,17 +88,13 @@ def test_rescans(api, frames, cams, dim, masked):
     rng = np.random.default_rng(dim)
     KF1 = sparse["KF1"]                                                 # (neighbour 0 has KF1's keypoints)
     d1 = rng.integers(0, 256, KF1.desc.shape, dtype=np.uint8)           # random rows: unrelated pairs lie far beyond th_low
-    d2 = T.flip_bits(rng, d1, 2)                                        # the neighbour: each row a near copy of KF1's
+    d2 = flip_bits(rng, d1, 2)                                        # the neighbour: each row a near copy of KF1's
     full = np.full(KF1.desc.shape, 255, np.uint8)
     sizes = list(zip(KF1.cam_w, KF1.cam_h))
     sparse["KF1"] = api.Frame(KF1.keys, KF1.key_cam, d1, full, sizes, KF1.scale_factors)
     sparse["nbs"][0] = api.Frame(KF1.keys, KF1.key_cam, d2, full, sizes, KF1.scale_factors)
     n, _, diag = compare(api, m, sparse, 0, cams, cap_of(sparse) + 1, epi=1e300)
     assert n > 50 and diag[1] == 0
-
-
-def _subset(api, F, keep):
-    return api.Frame(F.keys[keep], F.key_cam[keep], F.desc[keep], F.dmask[keep], list(zip(F.cam_w, F.cam_h)), F.scale_factors)
 
 
 def test_edges(api, frames, cams):
@@ -148,8 +105,8 @@ def test_edges(api, frames, cams):
     assert counts(s["nbs"][0]) == counts(s["KF1"])
     compare(api, m, s, 0, cams, cap)
     # camera 1 of KF1 empty, camera 2 of the neighbour empty
-    k1, k2 = s["KF1"].key_cam != 1, s["nbs"][0].key_cam != 2
-    e = dict(s, KF1=_subset(api, s["KF1"], k1), mp1=s["mp1"][k1], nbs=[_subset(api, s["nbs"][0], k2)], mps=[s["mps"][0][k2]])
+    (K1, k1), (K2, k2) = keep_cameras(api, s["KF1"], [0, 2]), keep_cameras(api, s["nbs"][0], [0, 1])
+    e = dict(s, KF1=K1, mp1=s["mp1"][k1], nbs=[K2], mps=[s["mps"][0][k2]])
     assert counts(e["KF1"])[1] == 0 and counts(e["nbs"][0])[2] == 0
     assert compare(api, m, e, 0, cams, cap)[0] > 10
     # no free query in camera 0
@@ -168,9 +125,9 @@ def test_kf1_is_kf2(api, frames, cams):
     s = tri_scene(api, frames, cams, 1, seed=60)
     cap = cap_of(s) + 4
     E = essential(s["rig1"], rig_of(api, cams, [0.03, 0.0, 0.01]))
-    dev = device_call(api, m, s["KF1"], s["KF1"], s["mp1"], s["mp1"], cams, cap, E, same=True)
-    host = host_call(api, m, s["KF1"], s["KF1"], s["mp1"], s["mp1"], cams, cap, E)
-    assert_same(api, s["KF1"], dev, host, cap)
+    dev = device_tri(api, m, s["KF1"], s["KF1"], s["mp1"], s["mp1"], cams, cap, E, same=True)
+    host = host_tri(api, m, s["KF1"], s["KF1"], s["mp1"], s["mp1"], cams, cap, E)
+    assert_same_tri(api, s["KF1"], dev, host, cap)
     assert dev[0] > 50
 
 
@@ -182,8 +139,8 @@ def test_busy_and_null_stream(api, frames, cams):
     cap = cap_of(s) + 3
     E = essential(s["rig1"], s["rigs"][0])
     args = (s["KF1"], s["nbs"][0], s["mp1"], s["mps"][0], cams, cap)
-    host = host_call(api, m, *args, E)
-    p1, mp1_t, p2, mp2_t, out = device_inputs(api, *args)
+    host = host_tri(api, m, *args, E)
+    p1, mp1_t, p2, mp2_t, out = tri_inputs(api, *args)
     side = torch.cuda.Stream()
     a = torch.randn(8192, 8192, device="cuda")
     torch.cuda.synchronize()
@@ -192,11 +149,11 @@ def test_busy_and_null_stream(api, frames, cams):
             a = a @ a * 1e-4
     n_t, m12_t, d_t = m.SearchForTriangulationRawDevice(p1, mp1_t, p2, mp2_t, cams, cap, E, stream=side, out=out, diag=True)
     side.synchronize()
-    assert_same(api, s["KF1"], (int(n_t.item()), m12_t.cpu().numpy(), d_t.cpu().numpy()), host, cap)
+    assert_same_tri(api, s["KF1"], (int(n_t.item()), m12_t.cpu().numpy(), d_t.cpu().numpy()), host, cap)
     assert torch.cuda.current_stream().cuda_stream == 0                  # stream=None passes the NULL stream
-    p1, mp1_t, p2, mp2_t, out = device_inputs(api, *args)
+    p1, mp1_t, p2, mp2_t, out = tri_inputs(api, *args)
     n_t, m12_t = m.SearchForTriangulationRawDevice(p1, mp1_t, p2, mp2_t, cams, cap, E, out=out)
-    assert_same(api, s["KF1"], (int(n_t.item()), m12_t.cpu().numpy(), None), host, cap)
+    assert_same_tri(api, s["KF1"], (int(n_t.item()), m12_t.cpu().numpy(), None), host, cap)
 
 
 @pytest.mark.parametrize("masked", [False, True])
@@ -207,20 +164,20 @@ def test_neighbour_sequence_on_device(api, frames, cams, masked):
     s = tri_scene(api, frames, cams, 5, seed=11)
     m = api.cORBmatcher(0.6, False, 32, masked)
     cap = cap_of(s) + 3
-    packs = pack_frames([s["KF1"]] + s["nbs"], cap, "joint", "cuda")
-    mp1_t = slot_row(api, s["KF1"], s["mp1"], cap, fill=-1, device="cuda")
+    packs = pack_frames([s["KF1"]] + s["nbs"], cap, layout="joint")
+    mp1_t = to_slots(api, s["KF1"], s["mp1"], cap, -1)
     gen = torch.Generator(device="cuda").manual_seed(5)
     next_id = s["next_id"]
     for k in range(5):
-        mp2_t = slot_row(api, s["nbs"][k], s["mps"][k], cap, fill=-1, device="cuda")
+        mp2_t = to_slots(api, s["nbs"][k], s["mps"][k], cap, -1)
         E = essential(s["rig1"], s["rigs"][k])
         mp1_now = api.slots_to_contiguous(mp1_t.cpu().numpy(), counts(s["KF1"]), cap)
-        host = host_call(api, m, s["KF1"], s["nbs"][k], mp1_now, s["mps"][k], cams, cap, E)
+        host = host_tri(api, m, s["KF1"], s["nbs"][k], mp1_now, s["mps"][k], cams, cap, E)
         n_t, m12_t = m.SearchForTriangulationRawDevice(packs[0], mp1_t, packs[1 + k], mp2_t, cams, cap, E)
         m12 = m12_t.cpu().numpy()
         assert int(n_t.item()) == host[0] > 10
-        live = api.contiguous_to_slots(np.ones(len(s["KF1"].keys), np.int32), counts(s["KF1"]), cap, fill=0).astype(bool)
-        assert np.array_equal(m12[live], host[1][live]), k
+        n1 = counts(s["KF1"])
+        assert np.array_equal(api.slots_to_contiguous(m12, n1, cap), api.slots_to_contiguous(host[1], n1, cap)), k
         # the stand-in, on the device: about 70 % of the pairs become points with new ids
         keep = (m12_t >= 0) & (torch.rand(m12_t.shape, generator=gen, device="cuda") < 0.7)
         ids = next_id + torch.cumsum(keep.to(torch.int32), 0, dtype=torch.int32) - 1
@@ -228,16 +185,7 @@ def test_neighbour_sequence_on_device(api, frames, cams, masked):
         mp2_t[m12_t[keep].long()] = ids[keep]
         next_id += int(keep.sum().item())
     # KF1's row went from searches to the next: later searches see fewer queries than the entry state has
-    assert int((mp1_t.cpu().numpy() == -1).sum()) < int((slot_row(api, s["KF1"], s["mp1"], cap, fill=0).numpy() == -1).sum())
-
-
-def residual(api, r1, r2, E):
-    """(nom * nom) / den of CheckDistEpipolarLine (ref src/misc.cpp:53-69), cv::Matx order"""
-    nom = float(api._mm(api._mm(r2.reshape(1, 3), E), r1.reshape(3, 1))[0, 0])
-    ex1 = api._mm(E, r1.reshape(3, 1)).ravel()
-    etx2 = api._mm(E.T.copy(), r2.reshape(3, 1)).ravel()
-    den = float(ex1[0] * ex1[0] + ex1[1] * ex1[1] + ex1[2] * ex1[2] + etx2[0] * etx2[0] + etx2[1] * etx2[1] + etx2[2] * etx2[2])
-    return (nom * nom) / den
+    assert int((mp1_t.cpu().numpy() == -1).sum()) < int((to_slots(api, s["KF1"], s["mp1"], cap, 0, "cpu").numpy() == -1).sum())
 
 
 def test_epipolar_threshold_edge(api, cams):
@@ -254,12 +202,12 @@ def test_epipolar_threshold_edge(api, cams):
     E = essential(rig_of(api, cams, [0, 0, 0]), rig_of(api, cams, [0.03, -0.01, 0.02]))
     r1 = np.array(api.img_to_world(cams[0], float(keys["x"][0]), float(keys["y"][0])))
     r2 = np.array(api.img_to_world(cams[0], float(keys["x"][1]), float(keys["y"][1])))
-    res = residual(api, r1, r2, E[0, 0])
+    res = epipolar_residual(api, r1, r2, E[0, 0])
     assert res > 0
     m = api.cORBmatcher(0.6, False, 32, True)
     mp = np.array([-1], np.int32)
     for thr, want in ((res, 0), (float(np.nextafter(res, np.inf)), 1)):
-        host = host_call(api, m, KF1, KF2, mp, mp, cams, 4, E, thr)
-        dev = device_call(api, m, KF1, KF2, mp, mp, cams, 4, E, epi=thr)
+        host = host_tri(api, m, KF1, KF2, mp, mp, cams, 4, E, thr)
+        dev = device_tri(api, m, KF1, KF2, mp, mp, cams, 4, E, epi=thr)
         assert host[0] == want and dev[0] == want, (thr, host[0], dev[0])
-        assert_same(api, KF1, dev, host, 4)
+        assert_same_tri(api, KF1, dev, host, 4)

@@ -5,7 +5,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-FAKE = C.c_void_p(0x10000)      # stands for a device pointer: never dereferenced by the host
+from device_frames import FAKE
+
+PTR = C.c_void_p(FAKE)      # FAKE as a pointer argument
 
 
 def _mps(n_points=10, **null):
@@ -13,19 +15,19 @@ def _mps(n_points=10, **null):
     v = MapPointDevView()
     v.n_points = n_points
     for k in ("bad", "in_view", "level", "proj_x", "proj_y", "view_cos", "desc", "dmask"):
-        setattr(v, k, None if null.get(k) else FAKE.value)
+        setattr(v, k, None if null.get(k) else FAKE)
     return v
 
 
-def _search(api, mps=None, packed=FAKE, n_parts=1, part_images=4, first_image=0, n_cams=4, capacity=2016, dim=32, masks=1,
-            frame_mp=FAKE, cam_w=None, n_levels=8):
+def _search(api, mps=None, packed=PTR, n_parts=1, part_images=4, first_image=0, n_cams=4, capacity=2016, dim=32, masks=1,
+            frame_mp=PTR, cam_w=None, n_levels=8):
     cw = np.full(max(n_cams, 1), 1280, np.int32) if cam_w is None else np.ascontiguousarray(cam_w, np.int32)
     ch = np.full(max(n_cams, 1), 720, np.int32)
     sf = np.ones(max(n_levels, 1))
     mv = _mps() if mps is None else mps
     return api.lib().mcs_search_by_projection_device(packed, n_parts, part_images, first_image, n_cams, capacity, dim, api._p(cw), api._p(ch),
                                                      n_levels, api._p(sf), C.byref(mv), C.c_double(3.0), C.c_double(0.8), 48, masks,
-                                                     frame_mp, FAKE, FAKE, None, None)
+                                                     frame_mp, PTR, PTR, None, None)
 
 
 def test_search_by_projection_device_validation(api):
@@ -52,9 +54,9 @@ def test_project_mappoints_device_validation(api, cams):
     sf = np.ones(8)
     ocs = (Ocam * 3)(*[api.as_ocam(c) for c in cams])
 
-    def call(n_cams=3, mi=poses, masks=FAKE, n_points=100, n_levels=8, cams_=ocs, out=FAKE):
-        return lib.mcs_project_mappoints_device(n_cams, api._p(mi) if mi is not None else None, api._p(poses), cams_, masks, n_points, FAKE,
-                                                FAKE, FAKE, FAKE, api._p(sf), n_levels, None, out, FAKE, FAKE, FAKE, FAKE, None)
+    def call(n_cams=3, mi=poses, masks=PTR, n_points=100, n_levels=8, cams_=ocs, out=PTR):
+        return lib.mcs_project_mappoints_device(n_cams, api._p(mi) if mi is not None else None, api._p(poses), cams_, masks, n_points, PTR,
+                                                PTR, PTR, PTR, api._p(sf), n_levels, None, out, PTR, PTR, PTR, PTR, None)
     for kw in (dict(mi=None), dict(masks=None), dict(out=None), dict(n_cams=0), dict(n_points=-1), dict(n_levels=0)):
         assert call(**kw) == api.MCS_ERR_INVALID, kw
     big = api.as_ocam(cams[0])

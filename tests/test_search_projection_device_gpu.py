@@ -6,65 +6,15 @@ import numpy as np
 import pytest
 
 import acceptance_model as am
+from device_frames import flip, on_device, per_cam, sizes
+from device_searches import collect, device_projection, launch_projection, projection_inputs
+from match_scenes import make_frames, random_rig
 
 pytestmark = pytest.mark.gpu
-
-FILL = 12345            # frame_mp value of the slots beyond a camera's count: must come back untouched
-
-
-def _prepare(api, per_cam, mps, pre=None, layout="single", first_image=2, cap=None):
-    """per_cam [(kps, desc, dmask)] -> the device inputs of mcs_search_by_projection_device, frame_mp in slot order"""
-    import torch
-    from multicol_slam_b200 import rig
-    counts = [len(p[0]) for p in per_cam]
-    nc, dim = len(per_cam), per_cam[0][1].shape[1]
-    cap = cap or max(counts) + 5
-    if layout == "single":         # decoys before and after the frame's cameras
-        decoy = (per_cam[0][0][::-1].copy(), per_cam[0][1][::-1].copy(), None if per_cam[0][2] is None else per_cam[0][2][::-1].copy())
-        imgs = [decoy] * first_image + list(per_cam) + [decoy]
-        buf, n_parts, part_images, first = rig.pack(imgs, cap, dim), 1, len(imgs), first_image
-    else:                          # n_cams one-image buffers back to back
-        buf, n_parts, part_images, first = np.concatenate([rig.pack([p], cap, dim) for p in per_cam]), nc, 1, 0
-    packed = torch.from_numpy(buf).cuda()
-    fm = api.contiguous_to_slots(np.full(sum(counts), -1, np.int32) if pre is None else pre, counts, cap, fill=FILL)
-    mdev = api.MapPointsDevice.from_host(mps, packed.device) if isinstance(mps, api.MapPoints) else mps
-    return dict(packed=packed, n_parts=n_parts, part_images=part_images, first=first, nc=nc, cap=cap, counts=counts,
-                fm_t=torch.from_numpy(fm).cuda(), mdev=mdev)
-
-
-def _launch(matcher, d, sizes, sf, th, stream=None):
-    return matcher.SearchByProjectionDevice(d["packed"], d["n_parts"], d["part_images"], d["first"], d["nc"], d["cap"], sizes, sf, d["mdev"],
-                                            th, d["fm_t"], stream=stream, diag=True)
-
-
-def _device_search(api, matcher, per_cam, sizes, sf, mps, th, pre=None, layout="single", first_image=2, cap=None):
-    """-> (nmatches, contiguous frame_mp, status, diag) of mcs_search_by_projection_device"""
-    import torch
-    d = _prepare(api, per_cam, mps, pre, layout, first_image, cap)
-    n_t, st_t, fm_t, diag_t = _launch(matcher, d, sizes, sf, th)
-    torch.cuda.synchronize()
-    return _collect(api, d, n_t, st_t, fm_t) + (diag_t.cpu().numpy(),)
-
-
-def _collect(api, d, n_t, st_t, fm_t):
-    out, cap, counts = fm_t.cpu().numpy(), d["cap"], d["counts"]
-    empty = np.concatenate([out[c * cap + counts[c]:(c + 1) * cap] for c in range(d["nc"])])
-    assert np.all(empty == FILL)
-    return int(n_t.item()), api.slots_to_contiguous(out, counts, cap), int(st_t.item())
-
-
-def _per_cam(F):
-    return [(F.keys[F.key_cam == c], F.desc[F.key_cam == c], None if F.dmask is None else F.dmask[F.key_cam == c])
-            for c in range(len(F.cam_w))]
-
-
-def _sizes(F):
-    return list(zip(F.cam_w.tolist(), F.cam_h.tolist()))
 
 
 def _projection_scene(api, cams, masks, seed=2, nmp=4000):
     """the inputs of test_match_gpu.py::test_search_by_projection"""
-    from test_match_gpu import make_frames
     F = make_frames(api, None, cams, [4, 5, 6], masks=masks)
     rng = np.random.default_rng(seed)
     nc = 3
@@ -99,7 +49,7 @@ def test_search_by_projection_device_matches_host(api, oa, cams, masks, layout):
     m = api.cORBmatcher(0.8, False, 32, masks)
     n, fmp = m.SearchByProjection(F, mps, 3.0)
     on, ofmp = oa.search_by_projection(F, mps, 3.0, 0.8, m.TH_HIGH_, masks)
-    gn, gfmp, status, diag = _device_search(api, m, _per_cam(F), _sizes(F), F.scale_factors, mps, 3.0, layout=layout)
+    gn, gfmp, status, diag = device_projection(api, m, per_cam(F), sizes(F), F.scale_factors, mps, 3.0, layout=layout)
     assert status == api.MCS_OK and n == on == gn and np.array_equal(fmp, ofmp) and np.array_equal(gfmp, fmp)
     assert gn > 500 and diag[2] == int(((mps.in_view != 0) & (mps.bad[:, None] == 0)).sum())
     # pre-assigned keypoints are skipped (ref :121), th = 1 keeps the radius unscaled
@@ -107,7 +57,7 @@ def test_search_by_projection_device_matches_host(api, oa, cams, masks, layout):
     pre[::3] = 0
     n2, fmp2 = m.SearchByProjection(F, mps, 1.0, pre.copy())
     on2, ofmp2 = oa.search_by_projection(F, mps, 1.0, 0.8, m.TH_HIGH_, masks, pre.copy())
-    gn2, gfmp2, status2, _ = _device_search(api, m, _per_cam(F), _sizes(F), F.scale_factors, mps, 1.0, pre=pre.copy(), layout=layout,
+    gn2, gfmp2, status2, _ = device_projection(api, m, per_cam(F), sizes(F), F.scale_factors, mps, 1.0, pre=pre.copy(), layout=layout,
                                             first_image=1)
     assert status2 == api.MCS_OK and n2 == on2 == gn2 and np.array_equal(fmp2, ofmp2) and np.array_equal(gfmp2, fmp2)
 
@@ -119,7 +69,7 @@ def test_config3_size_from_the_extractor(api, oa, cams):
     from multicol_slam_b200 import synth
     cam4 = [synth.scaled_cam(cams[i % 3], 1280, 720) for i in range(4)]
     ex = api.mdBRIEFextractorOct(nfeatures=2000, do_dBrief=True, learnMasks=True)
-    imgs = torch.from_numpy(np.stack([synth.frame(cam4[c], 300 + c) for c in range(4)])).cuda()
+    imgs = on_device(np.stack([synth.frame(cam4[c], 300 + c) for c in range(4)]))
     mk = np.stack([synth.mirror_mask(c) for c in cam4])
     from multicol_slam_b200 import rig
     cap = ex.capacity
@@ -166,18 +116,16 @@ def test_project_device_then_search_device(api, oa, cams):
     and skip_dev leaving the flagged points' entries untouched"""
     import torch
     from multicol_slam_b200 import synth
-    from test_match_gpu import _random_rig
     rng = np.random.default_rng(12)
     nc, n = 3, 20000
-    mtmc, inv = _random_rig(rng, nc)
+    mtmc, inv = random_rig(rng, nc)
     masks = np.stack([synth.mirror_mask(c) for c in cams])
     pos = rng.normal(size=(n, 3)); pos *= (rng.uniform(1.5, 12.0, n) / np.linalg.norm(pos, axis=1))[:, None]
     nrm = rng.normal(size=(n, 3)); nrm /= np.linalg.norm(nrm, axis=1)[:, None]
     dmin = rng.uniform(0.5, 4.0, n); dmax = dmin * rng.uniform(1.5, 6.0, n)
     sf = np.cumprod([1.0] + [1.2000000476837158] * 7)
     g = api.project_mappoints(inv, mtmc, cams, masks, pos, nrm, dmin, dmax, sf)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    masks_t, pos_t, nrm_t, dmin_t, dmax_t = t(masks), t(pos), t(nrm), t(dmin), t(dmax)
+    masks_t, pos_t, nrm_t, dmin_t, dmax_t = on_device(masks), on_device(pos), on_device(nrm), on_device(dmin), on_device(dmax)
     d = api.project_mappoints_device(inv, mtmc, cams, masks_t, pos_t, nrm_t, dmin_t, dmax_t, sf)
     torch.cuda.synchronize()
     for a, b in zip(g, d):
@@ -185,8 +133,8 @@ def test_project_device_then_search_device(api, oa, cams):
     # skip: flagged points keep what the output arrays held before the call
     skip = (rng.random(n) < 0.3).astype(np.uint8)
     before = [x.clone() for x in d]
-    mt2, inv2 = _random_rig(rng, nc)
-    d2 = api.project_mappoints_device(inv2, mt2, cams, masks_t, pos_t, nrm_t, dmin_t, dmax_t, sf, skip_t=t(skip), out=d)
+    mt2, inv2 = random_rig(rng, nc)
+    d2 = api.project_mappoints_device(inv2, mt2, cams, masks_t, pos_t, nrm_t, dmin_t, dmax_t, sf, skip_t=on_device(skip), out=d)
     g2 = api.project_mappoints(inv2, mt2, cams, masks, pos, nrm, dmin, dmax, sf)
     torch.cuda.synchronize()
     for a, b, o in zip(g2, d2, before):
@@ -201,20 +149,13 @@ def test_project_device_then_search_device(api, oa, cams):
     mps_h = api.MapPoints(np.zeros(n, np.uint8), g[0], g[1], g[2], g[3], g[4], desc, dmask)
     m = api.cORBmatcher(0.8, False, 32, True)
     ng, fg = m.SearchByProjection(F, mps_h, 3.0)
-    mdev = api.MapPointsDevice(None, *d_fresh(api, inv, mtmc, cams, masks_t, pos_t, nrm_t, dmin_t, dmax_t, sf), t(desc), t(dmask))
-    gn, gf, status, _ = _device_search(api, m, _per_cam(F), _sizes(F), F.scale_factors, mdev, 3.0)
+    mdev = api.MapPointsDevice(None, *d_fresh(api, inv, mtmc, cams, masks_t, pos_t, nrm_t, dmin_t, dmax_t, sf), on_device(desc), on_device(dmask))
+    gn, gf, status, _ = device_projection(api, m, per_cam(F), sizes(F), F.scale_factors, mdev, 3.0)
     assert status == api.MCS_OK and gn == ng and np.array_equal(gf, fg) and ng > 100
 
 
 def d_fresh(api, inv, mtmc, cams, masks_t, pos_t, nrm_t, dmin_t, dmax_t, sf):
     return api.project_mappoints_device(inv, mtmc, cams, masks_t, pos_t, nrm_t, dmin_t, dmax_t, sf)
-
-
-def _flip(rng, d, nbits):
-    out = d.copy()
-    for b in rng.choice(8 * len(d), nbits, replace=False):
-        out[b // 8] ^= 1 << (b % 8)
-    return out
 
 
 def test_long_dependency_chains_run_the_walk(api, oa):
@@ -227,7 +168,7 @@ def test_long_dependency_chains_run_the_walk(api, oa):
     keys = np.zeros(nk, api.KEYPOINT_DTYPE)
     keys["x"] = rng.uniform(92, 108, nk)                 # spread over several grid cells: visiting order != index order
     keys["y"] = rng.uniform(93, 107, nk)
-    kd = np.stack([_flip(rng, base, k + 1) for k in rng.permutation(nk)])       # distance to `base` = k + 1, in shuffled order
+    kd = np.stack([flip(rng, base, k + 1) for k in rng.permutation(nk)])       # distance to `base` = k + 1, in shuffled order
     dist = np.array([int(np.unpackbits(base ^ kd[k]).sum()) for k in range(nk)])
     taken0 = np.zeros(nk, bool)
     taken0[rng.choice(nk, 14, replace=False)] = True     # keypoints of the chain taken on entry
@@ -253,7 +194,7 @@ def test_long_dependency_chains_run_the_walk(api, oa):
     src = rng.integers(0, 200, n2)
     in_view[other, 1] = 1; level[other, 1] = keys2["octave"][src]
     px[other, 1] = keys2["x"][src] + rng.normal(0, 1, n2); py[other, 1] = keys2["y"][src] + rng.normal(0, 1, n2)
-    desc[other] = np.stack([_flip(rng, kd2[s], int(rng.integers(0, 20))) for s in src])
+    desc[other] = np.stack([flip(rng, kd2[s], int(rng.integers(0, 20))) for s in src])
     mps = api.MapPoints(np.zeros(nall, np.uint8), in_view, level, px, py, vc, desc, None)
     m = api.cORBmatcher(0.8, False, dim, False)
     pre = np.full(len(F.keys), -1, np.int32)
@@ -265,7 +206,7 @@ def test_long_dependency_chains_run_the_walk(api, oa):
     cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
     assert pn == n and np.array_equal(pfmp, fmp) and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts"):
-        gn, gfmp, status, diag = _device_search(api, m, _per_cam(F), _sizes(F), sf, mps, 3.0, pre=pre.copy(), layout=layout)
+        gn, gfmp, status, diag = device_projection(api, m, per_cam(F), sizes(F), sf, mps, 3.0, pre=pre.copy(), layout=layout)
         assert status == api.MCS_OK and gn == n and np.array_equal(gfmp, fmp)
         assert diag.tolist() == pdiag          # rounds run, walk start, queries and rescans as the model of the rounds and walk has them
 
@@ -282,7 +223,7 @@ def test_out_of_range_levels_are_flagged_and_skipped(api, oa, cams):
     m = api.cORBmatcher(0.8, False, 32, True)
     with pytest.raises(api.McsError):                   # the host call refuses such input
         m.SearchByProjection(F, broken, 3.0)
-    gn, gfmp, status, _ = _device_search(api, m, _per_cam(F), _sizes(F), F.scale_factors, broken, 3.0)
+    gn, gfmp, status, _ = device_projection(api, m, per_cam(F), sizes(F), F.scale_factors, broken, 3.0)
     assert status == api.MCS_ERR_INVALID
     iv2 = mps.in_view.copy()
     iv2[pick[:, 0], pick[:, 1]] = 0
@@ -298,28 +239,26 @@ def test_calls_do_not_wait_for_the_stream(api, oa, cams):
     n, fmp = m.SearchByProjection(F, mps, 3.0)
     rng = np.random.default_rng(1)
     nc, npt = 3, 5000
-    from test_match_gpu import _random_rig
     from multicol_slam_b200 import synth
-    mtmc, inv = _random_rig(rng, nc)
+    mtmc, inv = random_rig(rng, nc)
     masks = np.stack([synth.mirror_mask(c) for c in cams])
     pos = rng.normal(size=(npt, 3)) * 4.0
     nrm = rng.normal(size=(npt, 3)); nrm /= np.linalg.norm(nrm, axis=1)[:, None]
     dmin = rng.uniform(0.5, 2.0, npt); dmax = dmin * 8.0
     sf = F.scale_factors
     g = api.project_mappoints(inv, mtmc, cams, masks, pos, nrm, dmin, dmax, sf)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    args = (t(masks), t(pos), t(nrm), t(dmin), t(dmax))
-    prep = _prepare(api, _per_cam(F), mps)
+    args = (on_device(masks), on_device(pos), on_device(nrm), on_device(dmin), on_device(dmax))
+    prep = projection_inputs(api, per_cam(F), mps)
     torch.cuda.synchronize()
     s = torch.cuda.Stream()
     with torch.cuda.stream(s):
         torch.cuda._sleep(400_000_000)                  # a few hundred milliseconds of work ahead of both calls
         d = api.project_mappoints_device(inv, mtmc, cams, *args, sf, stream=s)
-        n_t, st_t, fm_t, _ = _launch(m, prep, _sizes(F), sf, 3.0, stream=s)
+        n_t, st_t, fm_t, _ = launch_projection(m, prep, sizes(F), sf, 3.0, stream=s)
         busy = s.query()
     assert busy is False
     s.synchronize()
     for a, b in zip(g, d):
         assert np.array_equal(a, b.cpu().numpy())
-    gn, gfmp, status = _collect(api, prep, n_t, st_t, fm_t)
+    gn, gfmp, status = collect(api, prep, n_t, st_t, fm_t)
     assert gn == n and status == api.MCS_OK and np.array_equal(gfmp, fmp)

@@ -7,50 +7,11 @@ import numpy as np
 import pytest
 
 import acceptance_model as am
-import test_ref_match_cpu as T
-from test_search_projection_device_gpu import FILL
-from test_search_projection_last_device_gpu import BIG_ID, _pack, _parity_scene
-from test_window_search_device_gpu import CHAIN_DISTS, INT_MAX, _counts, host_window_search, ratio_chain_scene
+from device_frames import INT_MAX, SIZES, frames, keep_cameras, on_device, rm  # noqa: F401  (frames, rm: fixtures)
+from device_searches import collect, device_search_frames, launch_frames
+from search_scenes import CHAIN_DISTS, host_window_search, make_scene, parity_scene, ratio_chain_scene
 
 pytestmark = pytest.mark.gpu
-frames = T.frames
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
-
-
-def _device_frames(api, m, Fc, Fl, rig_cur, mp_cur, mp_last, world, bad, window, layout="single", cap=None, stream=None, last_keys=None,
-                   run=True):
-    """mcs_search_by_projection_frames_device on host arrays -> (nmatches, contiguous cur_mp, status, diag)"""
-    import torch
-    cc, cl = _counts(Fc), _counts(Fl)
-    cap = cap or max(cc + cl) + 5
-    if last_keys is not None:
-        Fl = api.Frame(last_keys, Fl.key_cam, Fl.desc, Fl.dmask, list(zip(Fl.cam_w, Fl.cam_h)), Fl.scale_factors)
-    cur, last = _pack(Fc, Fl, layout, cap, Fc.desc.shape[1])
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    d = dict(cur=cur, last=last, cap=cap, cc=cc, rig=rig_cur, window=window, masks_t=t(np.stack(rig_cur.masks)),
-             last_mp_t=t(api.contiguous_to_slots(mp_last, cl, cap, fill=BIG_ID)), world_t=t(np.asarray(world, np.float64).reshape(-1, 3)),
-             bad_t=None if bad is None else t(np.asarray(bad, np.uint8)), cur_mp_t=t(api.contiguous_to_slots(mp_cur, cc, cap, fill=FILL)))
-    if not run:
-        return d
-    res = _launch(m, d, stream)
-    torch.cuda.synchronize()
-    return _collect(api, d, *res)
-
-
-def _launch(m, d, stream=None):
-    return m.SearchByProjectionFramesDevice(d["cur"], d["last"], d["cap"], d["rig"], d["masks_t"], d["last_mp_t"], d["world_t"], d["window"],
-                                            d["cur_mp_t"], bad_t=d["bad_t"], stream=stream, diag=True)
-
-
-def _collect(api, d, n_t, st_t, fm_t, diag_t):
-    out, cap, cc = fm_t.cpu().numpy(), d["cap"], d["cc"]
-    assert np.all(np.concatenate([out[c * cap + cc[c]:(c + 1) * cap] for c in range(len(cc))]) == FILL)
-    return int(n_t.item()), api.slots_to_contiguous(out, cc, cap), int(st_t.item()), diag_t.cpu().numpy()
 
 
 def _host(m, s, window=40, oa=None, mp1=None, mp2=None, F1=None, world=None):
@@ -61,13 +22,13 @@ def _host(m, s, window=40, oa=None, mp1=None, mp2=None, F1=None, world=None):
 
 def _dev(api, m, s, window=40, **kw):
     kw.setdefault("mp_cur", s["mp2"]); kw.setdefault("mp_last", s["mp1"]); kw.setdefault("world", s["sc"]["world"])
-    return _device_frames(api, m, s["F2"], s["F1"], s["rig2"], bad=s["sc"]["bad"], window=window, **kw)
+    return device_search_frames(api, m, s["F2"], s["F1"], s["rig2"], bad=s["sc"]["bad"], window=window, **kw)
 
 
 @pytest.mark.parametrize("layout", ["single", "parts", "shared"])
 @pytest.mark.parametrize("masks", [False, True])
 def test_parity_with_host_oracle_and_reference(api, oa, rm, frames, cams, masks, layout):
-    s = _parity_scene(api, oa, cams, frames)
+    s = parity_scene(api, oa, cams, frames)
     m = api.cORBmatcher(0.8, False, 32, masks)
     hn, hout = _host(m, s)
     on, oout = _host(m, s, oa=oa)
@@ -90,7 +51,7 @@ def test_parity_with_host_oracle_and_reference(api, oa, rm, frames, cams, masks,
 def test_first_occurrence_and_every_camera(api, oa, frames, cams):
     """the map point on two last-frame keypoints is searched once, from its first keypoint; a point may be accepted in several
     cameras of the current frame"""
-    s = _parity_scene(api, oa, cams, frames)
+    s = parity_scene(api, oa, cams, frames)
     m = api.cORBmatcher(0.8, False, 32, True)
     src = s["sc"]["src"]
     p = int(s["mp1"][src[4]])
@@ -116,7 +77,7 @@ def test_first_occurrence_and_every_camera(api, oa, frames, cams):
     bad = np.zeros(len(world), np.uint8)
     free = np.full(len(both.keys), -1, np.int32)
     hn, hout = m2.SearchByProjectionFramesRig(Fl, mp_last, both, rig, free, world, bad, 50)
-    gn, gout, status, diag = _device_frames(api, m2, both, Fl, rig, free, mp_last, world, bad, 50)
+    gn, gout, status, diag = device_search_frames(api, m2, both, Fl, rig, free, mp_last, world, bad, 50)
     assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
     acc = gout[gout >= 0]
     assert len(acc) > len(np.unique(acc))                      # some point accepted in both cameras
@@ -124,13 +85,9 @@ def test_first_occurrence_and_every_camera(api, oa, frames, cams):
 
 def test_empty_cameras_and_untouched_slots(api, oa, frames, cams):
     """camera 1 has no keypoints in either frame, camera 2 none in the last frame; slots beyond each count stay as they were"""
-    s = _parity_scene(api, oa, cams, frames)
-
-    def sub(F, keep):
-        i = np.flatnonzero(np.isin(F.key_cam, keep))
-        return api.Frame(F.keys[i], F.key_cam[i], F.desc[i], F.dmask[i], list(zip(F.cam_w, F.cam_h)), F.scale_factors), i
-    F1, i1 = sub(s["F1"], [0])
-    F2, i2 = sub(s["F2"], [0, 2])
+    s = parity_scene(api, oa, cams, frames)
+    F1, i1 = keep_cameras(api, s["F1"], [0])
+    F2, i2 = keep_cameras(api, s["F2"], [0, 2])
     s.update(F1=F1, F2=F2, mp1=s["mp1"][i1], mp2=s["mp2"][i2])
     m = api.cORBmatcher(0.8, False, 32, True)
     hn, hout = _host(m, s)
@@ -142,7 +99,7 @@ def test_empty_cameras_and_untouched_slots(api, oa, frames, cams):
 def test_edge_queries(api, oa, frames, cams):
     """last-frame octaves -1 (no level filter) and n_levels (no candidate); map points behind the rig, outside every mask, at
     non-finite positions and at the rig centre; windows without candidates"""
-    s = _parity_scene(api, oa, cams, frames, seed=62)
+    s = parity_scene(api, oa, cams, frames, seed=62)
     rng = np.random.default_rng(23)
     F1 = s["F1"]
     keys = F1.keys.copy()
@@ -176,9 +133,9 @@ def test_descriptor_sizes(api, oa, cams, dim, masks):
     ex = oa.OracleExtractor(nfeatures=350, do_dbrief=True, learn_masks=True, desc_size=dim)
     streams = [synth.texture_stream(cams[c], 2, seed=60 + c) for c in range(3)]
     sf = [float(ex.info.scale_factor[l]) for l in range(8)]
-    fr = [api.Frame.from_cameras([ex.extract(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], T.SIZES, sf)
+    fr = [api.Frame.from_cameras([ex.extract(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], SIZES, sf)
           for t in range(2)]
-    s = _parity_scene(api, oa, cams, fr, seed=63 + dim)
+    s = parity_scene(api, oa, cams, fr, seed=63 + dim)
     m = api.cORBmatcher(0.8, False, dim, masks)
     hn, hout = _host(m, s)
     on, oout = _host(m, s, oa=oa)
@@ -204,14 +161,14 @@ def test_long_dependency_chain_runs_the_walk(api, oa):
     cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
     assert pn == hn and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts", "shared"):
-        gn, gout, status, diag = _device_frames(api, m, Fc, Fl, rig, free, mp_last, world, bad, 40, layout=layout)
+        gn, gout, status, diag = device_search_frames(api, m, Fc, Fl, rig, free, mp_last, world, bad, 40, layout=layout)
         assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
         assert diag.tolist() == pdiag          # rounds run, walk start, queries and rescans as the model of the rounds and walk has them
 
 
 def test_invalid_ids(api, oa, frames, cams):
     """last-frame ids >= n_points drop their keypoint and raise status; current-frame ids >= n_points only mark their keypoint taken"""
-    s = _parity_scene(api, oa, cams, frames)
+    s = parity_scene(api, oa, cams, frames)
     m = api.cORBmatcher(0.8, False, 32, True)
     rng = np.random.default_rng(3)
     ids = rng.choice(np.flatnonzero(s["mp1"] >= 0), 8, replace=False)
@@ -244,7 +201,7 @@ def test_track_previous_frame_chain_from_the_extractor(api, oa, cams):
     imgs = torch.zeros((6, H, pitch), dtype=torch.uint8, device="cuda")
     for t in range(2):
         for c in range(3):
-            imgs[3 * t + c, :, :W] = torch.from_numpy(np.ascontiguousarray(streams[c][t]).reshape(H, W)).cuda()
+            imgs[3 * t + c, :, :W] = on_device(np.ascontiguousarray(streams[c][t]).reshape(H, W))
     masks = np.stack([synth.mirror_mask(c) for c in cams])
     cap = ex.capacity
     packed = torch.zeros(rigmod.packed_layout(6, cap, 32)[1], dtype=torch.uint8, device="cuda")
@@ -254,19 +211,18 @@ def test_track_previous_frame_chain_from_the_extractor(api, oa, cams):
     kps = v["kps"].cpu().numpy().view(api.KEYPOINT_DTYPE).reshape(6, cap)
     sf = [float(ex.info.scale_factor[l]) for l in range(8)]
     Fs = [api.Frame.from_cameras([(kps[i, :counts[i]], v["desc"][i, :counts[i]].cpu().numpy(), v["dmask"][i, :counts[i]].cpu().numpy())
-                                  for i in range(3 * t, 3 * t + 3)], T.SIZES, sf) for t in range(2)]
+                                  for i in range(3 * t, 3 * t + 3)], SIZES, sf) for t in range(2)]
     Fl, Fc = Fs
-    sc = T.make_scene(api, oa, cams, Fl, 71, npts=min(700, len(Fl.keys)))
+    sc = make_scene(api, oa, cams, Fl, 71, npts=min(700, len(Fl.keys)))
     rig1 = sc["rig"]
     world, n = sc["world"], len(sc["world"])
     nrm = world - rig1.M_t[:3, 3]
     nrm /= np.linalg.norm(nrm, axis=1)[:, None]
     m = api.cORBmatcher(0.8, False, 32, True)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    masks_t, world_t, nrm_t, dmin_t, dmax_t = t(masks), t(world), t(nrm), t(sc["min_d"]), t(sc["max_d"])
-    desc_t, dmask_t = t(sc["desc"]), t(sc["dmask"])
+    masks_t, world_t, nrm_t, dmin_t, dmax_t = on_device(masks), on_device(world), on_device(nrm), on_device(sc["min_d"]), on_device(sc["max_d"])
+    desc_t, dmask_t = on_device(sc["desc"]), on_device(sc["dmask"])
     zeros = np.zeros(n, np.uint8)
-    zeros_t = t(zeros)
+    zeros_t = on_device(zeros)
     cur, last = (packed, 1, 6, 3), (packed, 1, 6, 0)
     as_contig = lambda x, k: api.slots_to_contiguous(x.cpu().numpy(), counts[3 * k:3 * k + 3], cap)  # noqa: E731
     # 1. the last frame's map points: local-map search at the last pose
@@ -274,7 +230,7 @@ def test_track_previous_frame_chain_from_the_extractor(api, oa, cams):
     n1, fmp_last = m.SearchByProjection(Fl, api.MapPoints(zeros, *g, sc["desc"], sc["dmask"]), 3.0)
     proj = api.project_mappoints_device(rig1.MtMc_inv, rig1.MtMc, cams, masks_t, world_t, nrm_t, dmin_t, dmax_t, sf)
     fm_last_t = torch.full((3 * cap,), -1, dtype=torch.int32, device="cuda")
-    gn1, st1, _ = m.SearchByProjectionDevice(packed, 1, 6, 0, 3, cap, T.SIZES, sf, api.MapPointsDevice(None, *proj, desc_t, dmask_t), 3.0,
+    gn1, st1, _ = m.SearchByProjectionDevice(packed, 1, 6, 0, 3, cap, SIZES, sf, api.MapPointsDevice(None, *proj, desc_t, dmask_t), 3.0,
                                              fm_last_t)
     torch.cuda.synchronize()
     assert int(st1.item()) == api.MCS_OK and int(gn1.item()) == n1 and n1 > 100
@@ -282,7 +238,7 @@ def test_track_previous_frame_chain_from_the_extractor(api, oa, cams):
     # 2. WindowSearch(LastFrame, CurrentFrame, 60, ., 1): the device frame_mp of the last frame is last_mp as it stands
     n2, mp_cur = host_window_search(m, Fl, Fc, fmp_last, zeros, 60, 1, INT_MAX)
     cur_mp_t = torch.full((3 * cap,), -1, dtype=torch.int32, device="cuda")
-    gn2, st2, _ = m.WindowSearchDevice(cur, last, cap, T.SIZES, fm_last_t, 60, cur_mp_t, min_level=1, bad_t=zeros_t)
+    gn2, st2, _ = m.WindowSearchDevice(cur, last, cap, SIZES, fm_last_t, 60, cur_mp_t, min_level=1, bad_t=zeros_t)
     torch.cuda.synchronize()
     assert int(st2.item()) == api.MCS_OK and int(gn2.item()) == n2 and n2 > 50
     assert np.array_equal(as_contig(cur_mp_t, 1), mp_cur)
@@ -290,7 +246,7 @@ def test_track_previous_frame_chain_from_the_extractor(api, oa, cams):
     acc = np.flatnonzero(mp_cur >= 0)[::5]
     mp_cur[acc] = -1
     slot = np.concatenate([c * cap + np.arange(counts[3 + c]) for c in range(3)])[acc]
-    cur_mp_t[t(slot.astype(np.int64))] = -1
+    cur_mp_t[on_device(slot.astype(np.int64))] = -1
     M_t2 = sc["M_t"].copy()
     M_t2[:3, 3] += [0.003, 0.002, -0.004]
     rig2 = api.Rig(cams, sc["M_c"], M_t2)
@@ -304,7 +260,7 @@ def test_track_previous_frame_chain_from_the_extractor(api, oa, cams):
     g2 = api.project_mappoints(rig2.MtMc_inv, rig2.MtMc, cams, masks, world, nrm, sc["min_d"], sc["max_d"], sf)
     n5, fmp_cur = m.SearchByProjection(Fc, api.MapPoints(zeros, *g2, sc["desc"], sc["dmask"]), 3.0, mp_cur4.copy())
     proj2 = api.project_mappoints_device(rig2.MtMc_inv, rig2.MtMc, cams, masks_t, world_t, nrm_t, dmin_t, dmax_t, sf)
-    gn5, st5, _ = m.SearchByProjectionDevice(packed, 1, 6, 3, 3, cap, T.SIZES, sf, api.MapPointsDevice(None, *proj2, desc_t, dmask_t), 3.0,
+    gn5, st5, _ = m.SearchByProjectionDevice(packed, 1, 6, 3, 3, cap, SIZES, sf, api.MapPointsDevice(None, *proj2, desc_t, dmask_t), 3.0,
                                              cur_mp_t)
     torch.cuda.synchronize()
     assert int(st5.item()) == api.MCS_OK and int(gn5.item()) == n5
@@ -313,7 +269,7 @@ def test_track_previous_frame_chain_from_the_extractor(api, oa, cams):
 
 def test_call_does_not_wait_for_the_stream(api, oa, frames, cams):
     import torch
-    s = _parity_scene(api, oa, cams, frames)
+    s = parity_scene(api, oa, cams, frames)
     m = api.cORBmatcher(0.8, False, 32, True)
     hn, hout = _host(m, s)
     d = _dev(api, m, s, run=False)
@@ -321,9 +277,9 @@ def test_call_does_not_wait_for_the_stream(api, oa, frames, cams):
     st = torch.cuda.Stream()
     with torch.cuda.stream(st):
         torch.cuda._sleep(400_000_000)                  # a few hundred milliseconds of work ahead of the call
-        res = _launch(m, d, stream=st)
+        res = launch_frames(m, d, stream=st)
         busy = st.query()
     assert busy is False
     st.synchronize()
-    gn, gout, status, _ = _collect(api, d, *res)
+    gn, gout, status, _ = collect(api, d, *res)
     assert gn == hn and status == api.MCS_OK and np.array_equal(gout, hout)

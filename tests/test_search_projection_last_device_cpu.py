@@ -4,7 +4,7 @@ import ctypes as C
 
 import numpy as np
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
+from device_frames import FAKE, declared_symbols
 
 
 def _search(api, cams, cur=(FAKE, 1, 4, 0), last=(FAKE, 1, 4, 0), n_cams=4, capacity=2016, dim=32, models=None, masks=FAKE, n_levels=8,
@@ -59,7 +59,6 @@ def _sized(api, cam, w, h):
 
 
 def test_symbol_is_declared_and_exported(api):
-    from test_cabi_symbols import declared_symbols
     assert "mcs_search_by_projection_last_device" in declared_symbols()
     assert hasattr(api.lib(), "mcs_search_by_projection_last_device")
     assert hasattr(api.cORBmatcher, "SearchByProjectionLastDevice")

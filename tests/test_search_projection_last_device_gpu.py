@@ -7,89 +7,11 @@ import numpy as np
 import pytest
 
 import acceptance_model as am
-import test_ref_match_cpu as T
-from test_search_projection_device_gpu import FILL, _flip, _per_cam
+from device_frames import SIZES, flip, frames, keep_cameras, on_device, rm  # noqa: F401  (frames, rm: fixtures)
+from device_searches import collect, device_last, launch_last
+from search_scenes import make_scene, parity_scene
 
 pytestmark = pytest.mark.gpu
-frames = T.frames
-BIG_ID = 1 << 30            # last_mp value of the slots beyond a camera's count: reading one would raise status
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
-
-
-def _pack(Fc, Fl, layout, cap, dim, first_image=2):
-    """-> (cur, last) packed-frame descriptors (tensor, n_parts, part_images, first_image)"""
-    import torch
-    from multicol_slam_b200 import rig
-    pc, pl = _per_cam(Fc), _per_cam(Fl)
-    nc = len(pc)
-    t = lambda b: torch.from_numpy(b).cuda()  # noqa: E731
-    if layout == "single":         # decoys before and after each frame's cameras
-        k, d, m = pc[0]
-        decoy = (k[::-1].copy(), d[::-1].copy(), None if m is None else m[::-1].copy())
-        imgs = [decoy] * first_image + pc + [decoy]
-        return (t(rig.pack(imgs, cap, dim)), 1, len(imgs), first_image), (t(rig.pack([decoy] + pl, cap, dim)), 1, nc + 1, 1)
-    if layout == "parts":          # n_cams one-image buffers back to back, as the allgather leaves them
-        return tuple((t(np.concatenate([rig.pack([p], cap, dim) for p in per])), nc, 1, 0) for per in (pc, pl))
-    b = t(rig.pack(pl + pc, cap, dim))        # "shared": the two frames are consecutive images of one buffer
-    return (b, 1, 2 * nc, nc), (b, 1, 2 * nc, 0)
-
-
-def _device_last(api, m, Fc, Fl, rig_cur, mp_cur, mp_last, outlier, world, bad, th, layout="single", cap=None, stream=None,
-                 last_keys=None, run=True):
-    """mcs_search_by_projection_last_device on host arrays -> (nmatches, contiguous cur_mp, status, diag); last_keys replaces the
-    last frame's packed keypoints (the host composition keeps Fl's)"""
-    import torch
-    cc = [int((Fc.key_cam == c).sum()) for c in range(len(Fc.cam_w))]
-    cl = [int((Fl.key_cam == c).sum()) for c in range(len(Fl.cam_w))]
-    cap = cap or max(cc + cl) + 5
-    dim = Fc.desc.shape[1]
-    if last_keys is not None:
-        Fl = api.Frame(last_keys, Fl.key_cam, Fl.desc, Fl.dmask, list(zip(Fl.cam_w, Fl.cam_h)), Fl.scale_factors)
-    cur, last = _pack(Fc, Fl, layout, cap, dim)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    d = dict(cur=cur, last=last, cap=cap, cc=cc,
-             masks_t=t(np.stack(rig_cur.masks)), last_mp_t=t(api.contiguous_to_slots(mp_last, cl, cap, fill=BIG_ID)),
-             outlier_t=None if outlier is None else t(api.contiguous_to_slots(outlier, cl, cap, fill=1).astype(np.uint8)),
-             world_t=t(np.asarray(world, np.float64).reshape(-1, 3)), bad_t=None if bad is None else t(np.asarray(bad, np.uint8)),
-             cur_mp_t=t(api.contiguous_to_slots(mp_cur, cc, cap, fill=FILL)))
-    if not run:
-        return d
-    res = _launch(m, d, rig_cur, Fc.scale_factors, th, stream)
-    torch.cuda.synchronize()
-    return _collect(api, d, *res)
-
-
-def _launch(m, d, rig_cur, sf, th, stream=None):
-    return m.SearchByProjectionLastDevice(d["cur"], d["last"], d["cap"], rig_cur, d["masks_t"], sf, d["last_mp_t"], d["world_t"], th,
-                                          d["cur_mp_t"], bad_t=d["bad_t"], last_outlier_t=d["outlier_t"], stream=stream, diag=True)
-
-
-def _collect(api, d, n_t, st_t, fm_t, diag_t):
-    out, cap, cc = fm_t.cpu().numpy(), d["cap"], d["cc"]
-    assert np.all(np.concatenate([out[c * cap + cc[c]:(c + 1) * cap] for c in range(len(cc))]) == FILL)
-    return int(n_t.item()), api.slots_to_contiguous(out, cc, cap), int(st_t.item()), diag_t.cpu().numpy()
-
-
-def _parity_scene(api, oa, cams, frames, seed=61):
-    """the scene of test_ref_match_cpu.py::test_projection_searches_between_frames_equal_reference"""
-    F1, F2 = frames
-    sc = T.make_scene(api, oa, cams, F1, seed, npts=600)
-    n = 600
-    mp1 = np.full(len(F1.keys), -1, np.int32); mp1[sc["src"]] = np.arange(n)
-    mp1[sc["src"][5]] = mp1[sc["src"][4]]                       # one map point on two last-frame keypoints: searched twice
-    rng = np.random.default_rng(9)
-    M_t2 = sc["M_t"].copy()
-    M_t2[:3, 3] += [0.004, -0.003, 0.002]
-    rig2 = api.Rig(cams, sc["M_c"], M_t2)
-    mp2 = np.full(len(F2.keys), -1, np.int32)
-    mp2[rng.choice(len(F2.keys), 80, replace=False)] = rng.choice(n, 80, replace=False)      # pre-assigned current keypoints
-    outlier = (rng.random(len(F1.keys)) < 0.1).astype(np.uint8)
-    return dict(sc=sc, F1=F1, F2=F2, mp1=mp1, mp2=mp2, rig2=rig2, M_t2=M_t2, outlier=outlier)
 
 
 def _host(m, s, th, oa=None, mp1=None, F1=None, world=None):
@@ -102,7 +24,7 @@ def _host(m, s, th, oa=None, mp1=None, F1=None, world=None):
 @pytest.mark.parametrize("layout", ["single", "parts", "shared"])
 @pytest.mark.parametrize("masks", [False, True])
 def test_parity_with_host_oracle_and_reference(api, oa, rm, frames, cams, masks, layout, th):
-    s = _parity_scene(api, oa, cams, frames)
+    s = parity_scene(api, oa, cams, frames)
     m = api.cORBmatcher(0.8, False, 32, masks)
     hn, hout = _host(m, s, th)
     on, oout = _host(m, s, th, oa=oa)
@@ -114,7 +36,7 @@ def test_parity_with_host_oracle_and_reference(api, oa, rm, frames, cams, masks,
         k2 = rm.KF(s["F2"], cams, M_c=sc["M_c"], M_t=s["M_t2"], mp=s["mp2"])
         rn, rout = rm.search_by_projection_last(k2, k1, table, th, 0.8, masks)
         assert rn == hn and np.array_equal(rout, hout)
-    gn, gout, status, diag = _device_last(api, m, s["F2"], s["F1"], s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"],
+    gn, gout, status, diag = device_last(api, m, s["F2"], s["F1"], s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"],
                                           s["sc"]["bad"], th, layout=layout)
     assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
     assert np.array_equal(gout[s["mp2"] >= 0], s["mp2"][s["mp2"] >= 0])        # pre-assigned keypoints keep their map point
@@ -123,19 +45,14 @@ def test_parity_with_host_oracle_and_reference(api, oa, rm, frames, cams, masks,
 
 def test_empty_cameras_and_untouched_slots(api, oa, frames, cams):
     """camera 1 has no keypoints in either frame, camera 2 none in the last frame; slots beyond each count stay as they were"""
-    s = _parity_scene(api, oa, cams, frames)
-    sel = lambda F, keep: np.flatnonzero(np.isin(F.key_cam, keep))  # noqa: E731
-
-    def sub(F, keep):
-        i = sel(F, keep)
-        return api.Frame(F.keys[i], F.key_cam[i], F.desc[i], F.dmask[i], list(zip(F.cam_w, F.cam_h)), F.scale_factors), i
-    F1, i1 = sub(s["F1"], [0])
-    F2, i2 = sub(s["F2"], [0, 2])
+    s = parity_scene(api, oa, cams, frames)
+    F1, i1 = keep_cameras(api, s["F1"], [0])
+    F2, i2 = keep_cameras(api, s["F2"], [0, 2])
     s.update(F1=F1, F2=F2, mp1=s["mp1"][i1], mp2=s["mp2"][i2], outlier=s["outlier"][i1])
     m = api.cORBmatcher(0.8, False, 32, True)
     hn, hout = _host(m, s, 50.0)
     for layout in ("single", "parts", "shared"):
-        gn, gout, status, _ = _device_last(api, m, F2, F1, s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"], s["sc"]["bad"],
+        gn, gout, status, _ = device_last(api, m, F2, F1, s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"], s["sc"]["bad"],
                                            50.0, layout=layout)
         assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout) and hn > 20
 
@@ -143,7 +60,7 @@ def test_empty_cameras_and_untouched_slots(api, oa, frames, cams):
 def test_edge_queries(api, oa, frames, cams):
     """last-frame keypoints at octave 0 (min_level -1) and at the top octave; map points behind the camera, outside the mask and at
     non-finite positions; windows without candidates (th = 1)"""
-    s = _parity_scene(api, oa, cams, frames, seed=62)
+    s = parity_scene(api, oa, cams, frames, seed=62)
     rng = np.random.default_rng(23)
     F1 = s["F1"]
     keys = F1.keys.copy()
@@ -167,7 +84,7 @@ def test_edge_queries(api, oa, frames, cams):
             hn, hout = _host(m, s, th, F1=F1e, world=world)
             on, oout = _host(m, s, th, oa=oa, F1=F1e, world=world)
             assert hn == on and np.array_equal(hout, oout)
-            gn, gout, status, _ = _device_last(api, m, s["F2"], F1e, s["rig2"], s["mp2"], s["mp1"], s["outlier"], world, s["sc"]["bad"], th)
+            gn, gout, status, _ = device_last(api, m, s["F2"], F1e, s["rig2"], s["mp2"], s["mp1"], s["outlier"], world, s["sc"]["bad"], th)
             assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
             assert th != 50.0 or hn > 50
 
@@ -179,16 +96,16 @@ def test_descriptor_sizes(api, oa, cams, dim, masks):
     ex = oa.OracleExtractor(nfeatures=350, do_dbrief=True, learn_masks=True, desc_size=dim)
     streams = [synth.texture_stream(cams[c], 2, seed=60 + c) for c in range(3)]
     sf = [float(ex.info.scale_factor[l]) for l in range(8)]
-    fr = [api.Frame.from_cameras([ex.extract(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], T.SIZES, sf)
+    fr = [api.Frame.from_cameras([ex.extract(streams[c][t], synth.mirror_mask(cams[c]), cams[c]) for c in range(3)], SIZES, sf)
           for t in range(2)]
     assert fr[0].desc.shape[1] == dim
-    s = _parity_scene(api, oa, cams, fr, seed=63 + dim)
+    s = parity_scene(api, oa, cams, fr, seed=63 + dim)
     m = api.cORBmatcher(0.8, False, dim, masks)
     hn, hout = _host(m, s, 50.0)
     on, oout = _host(m, s, 50.0, oa=oa)
     assert hn == on and np.array_equal(hout, oout) and hn > 20
     for layout in ("single", "parts"):
-        gn, gout, status, _ = _device_last(api, m, s["F2"], s["F1"], s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"],
+        gn, gout, status, _ = device_last(api, m, s["F2"], s["F1"], s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"],
                                            s["sc"]["bad"], 50.0, layout=layout)
         assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
 
@@ -207,15 +124,15 @@ def _chain_scene(api, cams, rng, n_last=20, n_cur=30, dim=32):
     kc = np.zeros(n_cur, api.KEYPOINT_DTYPE)
     kc["x"] = u0 + rng.uniform(-40, 40, n_cur); kc["y"] = v0 + rng.uniform(-40, 40, n_cur)        # over several grid cells
     kc["octave"] = rng.integers(0, 3, n_cur)
-    dc = np.stack([_flip(rng, base, k + 1) for k in rng.permutation(n_cur)])
+    dc = np.stack([flip(rng, base, k + 1) for k in rng.permutation(n_cur)])
     # camera 1: an ordinary independent scene; camera 2: no keypoints in either frame
     k1 = np.zeros(120, api.KEYPOINT_DTYPE)
     k1["x"] = rng.uniform(100, 650, 120); k1["y"] = rng.uniform(60, 420, 120); k1["octave"] = rng.integers(0, 4, 120)
     d1 = rng.integers(0, 256, (120, dim)).astype(np.uint8)
     e = np.zeros(0, api.KEYPOINT_DTYPE), np.zeros((0, dim), np.uint8), None
     sf = np.cumprod([1.0] + [1.2000000476837158] * 7)
-    Fl = api.Frame.from_cameras([(kl, np.tile(base, (n_last, 1)), None), (k1, d1, None), e], T.SIZES, sf)
-    Fc = api.Frame.from_cameras([(kc, dc, None), (k1[::-1].copy(), d1[::-1].copy(), None), e], T.SIZES, sf)
+    Fl = api.Frame.from_cameras([(kl, np.tile(base, (n_last, 1)), None), (k1, d1, None), e], SIZES, sf)
+    Fc = api.Frame.from_cameras([(kc, dc, None), (k1[::-1].copy(), d1[::-1].copy(), None), e], SIZES, sf)
     # camera-1 map points: on the rays of their last keypoints, seen again in the current frame
     rays = np.array([api.img_to_world(cams[1], float(k["x"]), float(k["y"])) for k in k1])
     w1 = rays * rng.uniform(2.0, 8.0, 120)[:, None]
@@ -243,13 +160,13 @@ def test_long_dependency_chain_runs_the_walk(api, oa):
     cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
     assert pn == hn and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts", "shared"):
-        gn, gout, status, diag = _device_last(api, m, Fc, Fl, rig, mp_cur, mp_last, None, world, bad, 50.0, layout=layout)
+        gn, gout, status, diag = device_last(api, m, Fc, Fl, rig, mp_cur, mp_last, None, world, bad, 50.0, layout=layout)
         assert status == api.MCS_OK and gn == hn and np.array_equal(gout, hout)
         assert diag.tolist() == pdiag          # rounds run, walk start, queries and rescans as the model of the rounds and walk has them
 
 
 def test_invalid_ids_and_octaves_drop_only_their_query(api, oa, frames, cams):
-    s = _parity_scene(api, oa, cams, frames)
+    s = parity_scene(api, oa, cams, frames)
     m = api.cORBmatcher(0.8, False, 32, True)
     rig2, F1, sc = s["rig2"], s["F1"], s["sc"]
     live = [i for i in range(len(F1.keys)) if s["mp1"][i] >= 0 and not sc["bad"][s["mp1"][i]] and not s["outlier"][i] and
@@ -268,7 +185,7 @@ def test_invalid_ids_and_octaves_drop_only_their_query(api, oa, frames, cams):
         dropped = s["mp1"].copy()
         dropped[ids if kind == "id" else (octs if kind == "octave" else pick)] = -1
         hn, hout = _host(m, s, 50.0, mp1=dropped)
-        gn, gout, status, _ = _device_last(api, m, s["F2"], F1, rig2, s["mp2"], mp1, s["outlier"], sc["world"], sc["bad"], 50.0,
+        gn, gout, status, _ = device_last(api, m, s["F2"], F1, rig2, s["mp2"], mp1, s["outlier"], sc["world"], sc["bad"], 50.0,
                                            last_keys=keys)
         assert status == api.MCS_ERR_INVALID and gn == hn and np.array_equal(gout, hout), kind
 
@@ -287,7 +204,7 @@ def test_tracking_chain_from_the_extractor(api, oa, cams):
     imgs = torch.zeros((6, H, pitch), dtype=torch.uint8, device="cuda")
     for t in range(2):
         for c in range(3):
-            imgs[3 * t + c, :, :W] = torch.from_numpy(np.ascontiguousarray(streams[c][t]).reshape(H, W)).cuda()
+            imgs[3 * t + c, :, :W] = on_device(np.ascontiguousarray(streams[c][t]).reshape(H, W))
     masks = np.stack([synth.mirror_mask(c) for c in cams])
     cap = ex.capacity
     packed = torch.zeros(rigmod.packed_layout(6, cap, 32)[1], dtype=torch.uint8, device="cuda")
@@ -297,9 +214,9 @@ def test_tracking_chain_from_the_extractor(api, oa, cams):
     kps = v["kps"].cpu().numpy().view(api.KEYPOINT_DTYPE).reshape(6, cap)
     sf = [float(ex.info.scale_factor[l]) for l in range(8)]
     Fs = [api.Frame.from_cameras([(kps[i, :counts[i]], v["desc"][i, :counts[i]].cpu().numpy(), v["dmask"][i, :counts[i]].cpu().numpy())
-                                  for i in range(3 * t, 3 * t + 3)], T.SIZES, sf) for t in range(2)]
+                                  for i in range(3 * t, 3 * t + 3)], SIZES, sf) for t in range(2)]
     Fl, Fc = Fs
-    sc = T.make_scene(api, oa, cams, Fl, 71, npts=min(700, len(Fl.keys)))
+    sc = make_scene(api, oa, cams, Fl, 71, npts=min(700, len(Fl.keys)))
     rig1 = sc["rig"]
     M_t2 = sc["M_t"].copy()
     M_t2[:3, 3] += [0.003, 0.002, -0.004]
@@ -308,16 +225,15 @@ def test_tracking_chain_from_the_extractor(api, oa, cams):
     nrm = world - rig1.M_t[:3, 3]
     nrm /= np.linalg.norm(nrm, axis=1)[:, None]
     m = api.cORBmatcher(0.8, False, 32, True)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    masks_t, world_t, nrm_t, dmin_t, dmax_t = t(masks), t(world), t(nrm), t(sc["min_d"]), t(sc["max_d"])
-    desc_t, dmask_t = t(sc["desc"]), t(sc["dmask"])
+    masks_t, world_t, nrm_t, dmin_t, dmax_t = on_device(masks), on_device(world), on_device(nrm), on_device(sc["min_d"]), on_device(sc["max_d"])
+    desc_t, dmask_t = on_device(sc["desc"]), on_device(sc["dmask"])
     zeros = np.zeros(n, np.uint8)
     # 1. the last frame's map points: local-map search at the last pose
     g = api.project_mappoints(rig1.MtMc_inv, rig1.MtMc, cams, masks, world, nrm, sc["min_d"], sc["max_d"], sf)
     n1, fmp_last = m.SearchByProjection(Fl, api.MapPoints(zeros, *g, sc["desc"], sc["dmask"]), 3.0)
     proj = api.project_mappoints_device(rig1.MtMc_inv, rig1.MtMc, cams, masks_t, world_t, nrm_t, dmin_t, dmax_t, sf)
     fm_last_t = torch.full((3 * cap,), -1, dtype=torch.int32, device="cuda")
-    gn1, st1, _ = m.SearchByProjectionDevice(packed, 1, 6, 0, 3, cap, T.SIZES, sf, api.MapPointsDevice(None, *proj, desc_t, dmask_t), 3.0,
+    gn1, st1, _ = m.SearchByProjectionDevice(packed, 1, 6, 0, 3, cap, SIZES, sf, api.MapPointsDevice(None, *proj, desc_t, dmask_t), 3.0,
                                              fm_last_t)
     torch.cuda.synchronize()
     assert int(st1.item()) == api.MCS_OK and int(gn1.item()) == n1 and n1 > 100
@@ -334,7 +250,7 @@ def test_tracking_chain_from_the_extractor(api, oa, cams):
     g2 = api.project_mappoints(rig2.MtMc_inv, rig2.MtMc, cams, masks, world, nrm, sc["min_d"], sc["max_d"], sf)
     n3, fmp_cur = m.SearchByProjection(Fc, api.MapPoints(zeros, *g2, sc["desc"], sc["dmask"]), 3.0, mp_cur.copy())
     proj2 = api.project_mappoints_device(rig2.MtMc_inv, rig2.MtMc, cams, masks_t, world_t, nrm_t, dmin_t, dmax_t, sf)
-    gn3, st3, _ = m.SearchByProjectionDevice(packed, 1, 6, 3, 3, cap, T.SIZES, sf, api.MapPointsDevice(None, *proj2, desc_t, dmask_t), 3.0,
+    gn3, st3, _ = m.SearchByProjectionDevice(packed, 1, 6, 3, 3, cap, SIZES, sf, api.MapPointsDevice(None, *proj2, desc_t, dmask_t), 3.0,
                                              cur_mp_t)
     torch.cuda.synchronize()
     assert int(st3.item()) == api.MCS_OK and int(gn3.item()) == n3
@@ -343,18 +259,18 @@ def test_tracking_chain_from_the_extractor(api, oa, cams):
 
 def test_call_does_not_wait_for_the_stream(api, oa, frames, cams):
     import torch
-    s = _parity_scene(api, oa, cams, frames)
+    s = parity_scene(api, oa, cams, frames)
     m = api.cORBmatcher(0.8, False, 32, True)
     hn, hout = _host(m, s, 50.0)
-    d = _device_last(api, m, s["F2"], s["F1"], s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"], s["sc"]["bad"], 50.0,
+    d = device_last(api, m, s["F2"], s["F1"], s["rig2"], s["mp2"], s["mp1"], s["outlier"], s["sc"]["world"], s["sc"]["bad"], 50.0,
                      run=False)
     torch.cuda.synchronize()
     st = torch.cuda.Stream()
     with torch.cuda.stream(st):
         torch.cuda._sleep(400_000_000)                  # a few hundred milliseconds of work ahead of the call
-        res = _launch(m, d, s["rig2"], s["F2"].scale_factors, 50.0, stream=st)
+        res = launch_last(m, d, s["rig2"], s["F2"].scale_factors, 50.0, stream=st)
         busy = st.query()
     assert busy is False
     st.synchronize()
-    gn, gout, status, _ = _collect(api, d, *res)
+    gn, gout, status, _ = collect(api, d, *res)
     assert gn == hn and status == api.MCS_OK and np.array_equal(gout, hout)

@@ -14,12 +14,9 @@ import time
 import numpy as np
 import pytest
 
-from test_fuse_device_cpu import fuse_scene, host_fuse
-from test_fuse_device_gpu import _counts, _dev_map, _device, _replay, _targets
-from test_search_projection_device_gpu import _collect, _launch, _prepare
-import test_ref_match_cpu as T
-
-frames = T.frames
+from device_frames import counts, frames  # noqa: F401  (frames: a fixture)
+from device_searches import dev_map, device_projection, device_scw, fuse_device, fuse_replay, fuse_targets, launch_projection, projection_inputs
+from search_scenes import fuse_scene, host_fuse, host_scw
 
 TILE = 2048                 # entries per count / fill block (kQbTile)
 PASS = 1024 * TILE          # entries one pass of the single-CTA scan covers: 2^21
@@ -133,15 +130,6 @@ def _report(label, n_entries, nq, diag, t):
           f"{diag[1]}, rescans {diag[3]}; {t:.1f} s")
 
 
-def _device_search(api, m, per, sf, mps, th=1.0):
-    import torch
-    d = _prepare(api, per, mps, layout="parts")
-    n_t, st_t, fm_t, diag_t = _launch(m, d, [(W, H)] * len(per), sf, th)
-    torch.cuda.synchronize()
-    n, fmp, st = _collect(api, d, n_t, st_t, fm_t)
-    return n, fmp, st, diag_t.cpu().numpy()
-
-
 # (n_points * n_cams): 1024 blocks less one entry, 1024 full blocks, 1025 blocks, three passes (the last partial), five passes
 SIZES = [(PASS - 1, 7), (PASS, 4), (PASS + 1, 3), (2 * PASS + 17, 3), (5 * 1_678_000, 5)]
 
@@ -160,7 +148,7 @@ def test_search_by_projection_past_one_scan_pass(api, n_entries, nc):
         assert counts[e - 2] == 0 and counts[e - 1] == full(e - 1) and (e == nb or counts[e] == full(e))
     m = api.cORBmatcher(0.8, False, DIM, False)
     hn, hfmp = m.SearchByProjection(F, mps, 1.0)
-    gn, gfmp, status, diag = _device_search(api, m, per, F.scale_factors, mps)
+    gn, gfmp, status, diag = device_projection(api, m, per, [(W, H)] * len(per), F.scale_factors, mps, 1.0, layout="parts")
     _report("SearchByProjection", n_entries, int(diag[2]), diag, time.time() - t0)
     assert status == api.MCS_OK
     assert diag[2] == offsets[-1], _query_count_message(diag[2], offsets)
@@ -179,7 +167,7 @@ def _split_search(api, m, per, sf, mps, chunk):
     point indices, so the new ones are shifted back to the whole map's"""
     import torch
     n = len(mps.bad)
-    d = _prepare(api, per, api.MapPoints(mps.bad[:1], mps.in_view[:1], mps.level[:1], mps.proj_x[:1], mps.proj_y[:1], mps.view_cos[:1],
+    d = projection_inputs(api, per, api.MapPoints(mps.bad[:1], mps.in_view[:1], mps.level[:1], mps.proj_x[:1], mps.proj_y[:1], mps.view_cos[:1],
                                            mps.desc[:1]), layout="parts")
     full = api.MapPointsDevice.from_host(mps, d["packed"].device)
     total, worst = 0, 0
@@ -188,14 +176,14 @@ def _split_search(api, m, per, sf, mps, chunk):
         d["mdev"] = api.MapPointsDevice(full.bad[a:b], full.in_view[a:b], full.level[a:b], full.proj_x[a:b], full.proj_y[a:b],
                                         full.view_cos[a:b], full.desc[a:b])
         before = d["fm_t"].clone()
-        n_t, st_t, fm_t, diag_t = _launch(m, d, [(W, H)] * len(per), sf, 1.0)
+        n_t, st_t, fm_t, diag_t = launch_projection(m, d, [(W, H)] * len(per), sf, 1.0)
         torch.cuda.synchronize()
         assert int(st_t.item()) == api.MCS_OK
         new = fm_t != before
         fm_t[new] += a
         total += int(n_t.item())
         worst = max(worst, int(diag_t[0].item()))
-    return total, api.slots_to_contiguous(d["fm_t"].cpu().numpy(), d["counts"], d["cap"]), worst
+    return total, api.slots_to_contiguous(d["fm_t"].cpu().numpy(), d["cc"], d["cap"]), worst
 
 
 @pytest.mark.gpu
@@ -209,7 +197,7 @@ def test_search_by_projection_at_the_bound(api):
     t0 = time.time()
     F, per, mps, valid = _projection_scene(api, n_entries, nc, seed=24)
     m = api.cORBmatcher(0.8, False, DIM, False)
-    gn, gfmp, status, diag = _device_search(api, m, per, F.scale_factors, mps)
+    gn, gfmp, status, diag = device_projection(api, m, per, [(W, H)] * len(per), F.scale_factors, mps, 1.0, layout="parts")
     _report("SearchByProjection at the bound", n_entries, int(diag[2]), diag, time.time() - t0)
     offsets = scan_model(valid.reshape(-1))[1]
     assert status == api.MCS_OK and diag[2] == offsets[-1], _query_count_message(diag[2], offsets)
@@ -224,7 +212,7 @@ def test_search_by_projection_at_the_bound(api):
     mdev = api.MapPointsDevice(None, torch.ones((npts, nc4), dtype=torch.uint8, device=dev), z(torch.int32, npts, nc4),
                                *(z(torch.float64, npts, nc4) for _ in range(3)), z(torch.uint8, npts, DIM))
     assert mdev.view().n_points * nc4 == BOUND
-    d = _prepare(api, per[:1] * nc4, mdev, layout="parts")
+    d = projection_inputs(api, per[:1] * nc4, mdev, layout="parts")
     out = tuple(torch.full((k,), -777, dtype=torch.int32, device=dev) for k in (1, 1, 4))
     before = d["fm_t"].clone()
     with pytest.raises(api.McsError, match=r"more than 2\^24 - 1 \(map point, camera\) entries") as err:
@@ -251,11 +239,11 @@ def test_fuse_past_one_scan_pass(api, oa, frames, cams, variant):
     s = fuse_scene(api, oa, cams, KF, variant)
     nc = len(cams)
     m = api.cORBmatcher(0.6, False, 32, True)
-    cap = max(_counts(KF)) + 3
-    dm = _dev_map(s)
+    cap = max(counts(KF)) + 3
+    dm = dev_map(s)
     # one key frame at the scene's pose: its hits pick the queries.  Every query with a hit and every fourth without one, repeated,
     # so that more than an eighth of the entries hit and the hits outgrow one scan pass below the 2^24 entry bound.
-    h1, n1, st1, _ = _device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], dm, cap, "single", variant, Scw=s["Scw"])
+    h1, n1, st1, _ = fuse_device(api, m, [KF], [s["sc"]["rig"]], [None], s["points"], dm, cap, "single", variant, Scw=s["Scw"])
     assert st1 == api.MCS_OK and n1 > 50
     hit_q = np.unique(h1[:, 1])
     base = np.union1d(hit_q, np.setdiff1d(np.arange(len(s["points"])), hit_q)[::4])
@@ -267,11 +255,11 @@ def test_fuse_past_one_scan_pass(api, oa, frames, cams, variant):
     _fits(n_kf * per_kf * (33 + QUERY_BYTES + 12), f"{n_kf * per_kf} Fuse entries")
     kstar = PASS // per_kf + 1                    # its entries all lie past entry 2^21
     assert kstar < n_kf
-    rigs = _targets(api, cams, s["sc"], n_kf, 21)
+    rigs = fuse_targets(api, cams, s["sc"], n_kf, 21)
     rigs[kstar] = s["sc"]["rig"]
     pts = np.tile(s["points"][base], reps).astype(np.int32)
     t0 = time.time()
-    hits, n, status, _ = _device(api, m, [KF] * n_kf, rigs, [None] * n_kf, pts, dm, cap, "parts", variant, Scw=s["Scw"])
+    hits, n, status, _ = fuse_device(api, m, [KF] * n_kf, rigs, [None] * n_kf, pts, dm, cap, "parts", variant, Scw=s["Scw"])
     t_batch = time.time() - t0
     assert status == api.MCS_OK
     e = _entries(hits, n_q, nc, cap)
@@ -284,7 +272,7 @@ def test_fuse_past_one_scan_pass(api, oa, frames, cams, variant):
     sep, total = [], 0
     for a in range(0, n_kf, step):
         b = min(n_kf, a + step)
-        h, nn, st, _ = _device(api, m, [KF] * (b - a), rigs[a:b], [None] * (b - a), pts, dm, cap, "parts", variant, Scw=s["Scw"])
+        h, nn, st, _ = fuse_device(api, m, [KF] * (b - a), rigs[a:b], [None] * (b - a), pts, dm, cap, "parts", variant, Scw=s["Scw"])
         assert st == api.MCS_OK
         h = h.copy()
         h[:, 0] += a
@@ -300,7 +288,7 @@ def test_fuse_past_one_scan_pass(api, oa, frames, cams, variant):
     if variant == 0:
         sk["cur"] = dict(s["cur"], rays=np.tile(s["cur"]["rays"][base], (reps, 1)))
     hn, hops, hmp = host_fuse(api, m, KF, sk, variant)
-    dn, dops, dmp = _replay(m, KF, sk, variant, hits, cap, k=kstar)
+    dn, dops, dmp = fuse_replay(m, KF, sk, variant, hits, cap, k=kstar)
     assert dn == hn and np.array_equal(dops, hops) and np.array_equal(dmp, hmp) and len(hops) > 50
     # and that key frame's hits == the single-key-frame call's, replica by replica
     mine = hits[hits[:, 0] == kstar][:, 1:]
@@ -365,8 +353,6 @@ def _scw_scene(api, cams, seed=7):
 def test_search_by_projection_scw_past_one_scan_pass(api, cams):
     """mcs_search_by_projection_scw_device with n_q = 2.4 M entries (1172 blocks) == its host mirror, bit for bit, and its query
     count == the model's over the entries the host projection passes"""
-    from test_sim3_searches_device_cpu import host_scw
-    from test_sim3_searches_device_gpu import device_scw
     n = SCW_CAMS * SCW_KEYS
     _fits(n * (QUERY_BYTES + 4 * 8 + 2 * 28 + 2 * DIM + 16), f"{n} Scw entries")
     t0 = time.time()

@@ -5,17 +5,10 @@ methods (recorded in tests/golden/ref_tape_sim3_searches_device_cpu.*) on the sc
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
+from device_frames import FAKE, frames, taped_rm  # noqa: F401  (frames: a fixture)
+from search_scenes import host_scw, host_sim3, reference_scw, reference_sim3, scw_scene, sim3_scene
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
-frames = T.frames
-
-
-@pytest.fixture(scope="module")
-def rm():
-    """the reference's own matcher, live while recording and replayed from tests/golden/ref_tape_sim3_searches_device_cpu.* otherwise"""
-    import ref_tape
-    return ref_tape.module("ref_match_api", "sim3_searches_device_cpu", T.TAPE_LIMIT)
+rm = taped_rm("sim3_searches_device_cpu")
 
 
 def _frame(fr):
@@ -110,106 +103,6 @@ def test_symbols_are_declared_and_exported(api):
     for name in ("mcs_search_by_sim3_device", "mcs_search_by_projection_scw_device"):
         assert f"int  {name}(" in hdr and hasattr(api.lib(), name)
     assert callable(api.cORBmatcher.SearchBySim3Device) and callable(api.cORBmatcher.SearchByProjectionKFScwDevice)
-
-
-# ---- the scenes ------------------------------------------------------------------------------------------------------------------
-def second_view(api, KF, seed):
-    """another key frame over the same keypoints: positions jittered by up to half a pixel, a few descriptor bits flipped"""
-    rng = np.random.default_rng(seed)
-    keys = KF.keys.copy()
-    keys["x"] += rng.uniform(-0.5, 0.5, len(keys)).astype(np.float32)
-    keys["y"] += rng.uniform(-0.5, 0.5, len(keys)).astype(np.float32)
-    return api.Frame(keys, KF.key_cam.copy(), T.flip_bits(rng, KF.desc, 3), KF.dmask.copy(), list(zip(KF.cam_w, KF.cam_h)), KF.scale_factors)
-
-
-def sim3_scene(api, oa, cams, KF1, seed=51, s12=1.01):
-    """SearchBySim3 between KF1 and a second view KF2 of its keypoints from a rig pose a few centimetres away.  KF1 carries map points
-    0..299 on its keypoints' rays, KF2 points 300..599 a few millimetres from them with descriptor variants of their own; a few
-    bad points; the Sim3 is the true relative pose with s12 != 1.  Ten KF1 keypoints are matched beforehand to KF2 points whose
-    keypoint in KF2 (obs_idx) is then vbAlreadyMatched2."""
-    sc1 = T.make_scene(api, oa, cams, KF1, seed, npts=300)
-    KF2 = second_view(api, KF1, seed + 1)
-    rng = np.random.default_rng(seed + 2)
-    M_t2 = sc1["M_t"].copy()
-    M_t2[:3, 3] += [0.012, -0.008, 0.006]
-    a = 0.002
-    Rz = np.array([[np.cos(a), -np.sin(a), 0], [np.sin(a), np.cos(a), 0], [0, 0, 1.0]])
-    M_t2[:3, :3] = api._mm(Rz, M_t2[:3, :3])
-    rig2 = api.Rig(cams, sc1["M_c"], M_t2)
-    world2 = sc1["world"] + rng.normal(0, 0.003, sc1["world"].shape)
-    world = np.concatenate([sc1["world"], world2])
-    desc = np.concatenate([sc1["desc"], T.flip_bits(rng, KF2.desc[sc1["src"]], 30)])
-    dmask = np.concatenate([sc1["dmask"], KF2.dmask[sc1["src"]]])
-    bad = np.concatenate([sc1["bad"], np.roll(sc1["bad"], 7)])
-    # distance ranges whose predicted level is the point's keypoint octave + 1 (ratio 1.1 * scale factor): the window's levels
-    # {l - 1, l} keep the keypoint, so that most queries find it
-    cam = KF1.key_cam[sc1["src"]]
-    depth = np.array([np.linalg.norm(api._mm(sc1["rig"].MtMc_inv[int(c)], np.append(x, 1.0))[:3]) for c, x in zip(cam, sc1["world"])])
-    min1 = depth / (1.1 * np.asarray(KF1.scale_factors)[KF1.keys["octave"][sc1["src"]]])
-    min_d = np.concatenate([min1, min1])
-    max_d = min_d * 12.0
-    mp1 = np.full(len(KF1.keys), -1, np.int32); mp1[sc1["src"]] = np.arange(300)
-    mp2 = np.full(len(KF2.keys), -1, np.int32); mp2[sc1["src"]] = 300 + np.arange(300)
-    T12 = api._mm(api.inv_rigid(sc1["M_t"]), M_t2)                 # KF2's rig frame -> KF1's: T1w * Tw2
-    pre = np.full(len(KF1.keys), -1, np.int32)
-    some = rng.choice(sc1["src"], 10, replace=False)
-    pre[some] = 300 + rng.choice(300, 10, replace=False)
-    obs_idx = np.concatenate([sc1["src"], sc1["src"]]).astype(np.int32)
-    return dict(KF1=KF1, KF2=KF2, rig1=sc1["rig"], rig2=rig2, M_c=sc1["M_c"], M_t1=sc1["M_t"], M_t2=M_t2, world=world, desc=desc,
-                dmask=dmask, bad=bad, min_d=min_d, max_d=max_d, mp1=mp1, mp2=mp2, s12=s12, R12=T12[:3, :3].copy(), t12=T12[:3, 3].copy(),
-                pre=pre, obs_idx=obs_idx)
-
-
-def reference_sim3(rm, cams, s, th, masks):
-    obs_kf = np.concatenate([np.zeros(300, np.int32), np.ones(300, np.int32)])
-    table = rm.MPTable(3, s["desc"], dmask=s["dmask"], bad=s["bad"], world_pos=s["world"], min_dist=s["min_d"], max_dist=s["max_d"],
-                       obs_kf=obs_kf, obs_idx=s["obs_idx"])
-    k1 = rm.KF(s["KF1"], cams, M_c=s["M_c"], M_t=s["M_t1"], mp=s["mp1"])
-    k2 = rm.KF(s["KF2"], cams, M_c=s["M_c"], M_t=s["M_t2"], mp=s["mp2"])
-    return rm.search_by_sim3(k1, k2, table, s["s12"], s["R12"], s["t12"], th, s["pre"], 0.6, masks)
-
-
-def host_sim3(m, s, th, _sw=None, **kw):
-    return m.SearchBySim3(s["KF1"], s["rig1"], s["mp1"], s["KF2"], s["rig2"], s["mp2"], s["world"], s["min_d"], s["max_d"], s["bad"],
-                          s["desc"], s["dmask"], s["s12"], s["R12"], s["t12"], th, matches12=kw.get("pre", s["pre"]),
-                          obs_idx2=s["obs_idx"], _sw=_sw)
-
-
-def scw_scene(api, oa, cams, F, seed=33, cam0_only=True, scale=1.25):
-    """SearchByProjection(pKF, Scw, vpPoints, vpMatched, th): loop points on the key frame's rays (entry i of vpPoints projects near
-    keypoint src[i]), some NULL and some bad; vpMatched holds taken keypoints, some of them holding points of the list (already found).
-    cam0_only: the key frame keeps camera 0's keypoints alone, where the reference's descriptor reads stay defined (contiguous id ==
-    row)."""
-    if cam0_only:
-        sel = np.flatnonzero(F.key_cam == 0)
-        KF = api.Frame(F.keys[sel], F.key_cam[sel], F.desc[sel], F.dmask[sel], T.SIZES, F.scale_factors)
-    else:
-        KF = F
-    n_keys = len(KF.keys)
-    sc = T.make_scene(api, oa, cams, KF, seed, npts=min(n_keys - 5, 400))
-    n = len(sc["world"])
-    rng = np.random.default_rng(seed + 1)
-    points = np.arange(n, dtype=np.int32)
-    points[rng.random(n) < 0.05] = -1
-    matched = np.full(n_keys, -1, np.int32)
-    taken = rng.choice(n_keys, 40, replace=False)
-    matched[taken] = rng.choice(n, 40, replace=False)                # points of the list, now already found
-    Scw = api.inv_rigid(sc["M_t"]).copy()
-    Scw[:3, :3] *= scale
-    Scw[:3, 3] *= scale
-    return dict(KF=KF, sc=sc, rig=sc["rig"], M_c=sc["M_c"], M_t=sc["M_t"], world=sc["world"], desc=sc["desc"], dmask=sc["dmask"], bad=sc["bad"],
-                min_d=sc["min_d"], max_d=sc["max_d"], points=points, matched=matched, Scw=Scw)
-
-
-def reference_scw(rm, cams, s, masks):
-    table = rm.MPTable(3, s["desc"], dmask=s["dmask"], bad=s["bad"], world_pos=s["world"], min_dist=s["min_d"], max_dist=s["max_d"])
-    return rm.search_by_projection_scw(rm.KF(s["KF"], cams, M_c=s["M_c"], M_t=s["M_t"]), table, s["Scw"], s["points"], s["matched"], 10,
-                                       0.6, masks)
-
-
-def host_scw(m, s, _sw=None, **kw):
-    return m.SearchByProjectionKFScw(s["KF"], s["rig"], s["Scw"], kw.get("points", s["points"]), kw.get("matched", s["matched"]), s["world"],
-                                     s["min_d"], s["max_d"], kw.get("bad", s["bad"]), s["desc"], s["dmask"], th=kw.get("th", 10), _sw=_sw)
 
 
 @pytest.mark.parametrize("th", [7.5, 10.0])

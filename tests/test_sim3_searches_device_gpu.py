@@ -6,60 +6,25 @@ is integer: bit for bit."""
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
-from test_fuse_device_gpu import BIG_ID, GUARD, _counts, _pack_kfs
-from test_sim3_searches_device_cpu import host_scw, host_sim3, reference_scw, reference_sim3, scw_scene, sim3_scene
+from device_frames import BIG_ID, GUARD, SIZES, counts, flip_bits, frames, from_slots, on_device, pack_frames, rm, to_slots, widen, widener  # noqa: F401
+from device_searches import dev_map, device_scw
+from search_scenes import host_scw, host_sim3, make_scene, reference_scw, reference_sim3, scw_scene, sim3_scene
 
 pytestmark = pytest.mark.gpu
-frames = T.frames
-
-
-@pytest.fixture(scope="module")
-def rm():
-    import ref_match_api
-    return ref_match_api if ref_match_api.available() else None
-
-
-def _t(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def _slots(api, F, row, cap, fill):
-    return _t(api.contiguous_to_slots(np.asarray(row, np.int32), _counts(F), cap, fill=fill))
-
-
-def _dev_map(s):
-    return dict(world_t=_t(np.asarray(s["world"], np.float64)), min_t=_t(np.asarray(s["min_d"], np.float64)),
-                max_t=_t(np.asarray(s["max_d"], np.float64)), desc_t=_t(s["desc"]), dmask_t=_t(s["dmask"]), bad_t=_t(np.asarray(s["bad"], np.uint8)))
-
-
-def _back(api, F, t, cap):
-    """a slot-indexed row back to contiguous order, after checking that no slot at or beyond a camera's count was written"""
-    a = t.cpu().numpy().reshape(-1, cap)
-    for c, n in enumerate(_counts(F)):
-        assert (a[c, n:] == GUARD).all()
-    return api.slots_to_contiguous(a.reshape(-1), _counts(F), cap)
-
-
-def _widen(api, F, dim):
-    w = (lambda d: np.ascontiguousarray(d[:, :16])) if dim == 16 else (lambda d: np.ascontiguousarray(np.concatenate([d, d ^ 0x5A], 1)))
-    return api.Frame(F.keys, F.key_cam, w(F.desc), w(F.dmask), list(zip(F.cam_w, F.cam_h)), F.scale_factors), w
 
 
 def _sim3_at(api, s, dim):
     if dim == 32:
         return s
-    K1, w = _widen(api, s["KF1"], dim)
-    K2, _ = _widen(api, s["KF2"], dim)
-    return dict(s, KF1=K1, KF2=K2, desc=w(s["desc"]), dmask=w(s["dmask"]))
+    w = widener(dim)
+    return dict(s, KF1=widen(api, s["KF1"], dim), KF2=widen(api, s["KF2"], dim), desc=w(s["desc"]), dmask=w(s["dmask"]))
 
 
 def _scw_at(api, s, dim):
     if dim == 32:
         return s
-    K, w = _widen(api, s["KF"], dim)
-    return dict(s, KF=K, desc=w(s["desc"]), dmask=w(s["dmask"]))
+    w = widener(dim)
+    return dict(s, KF=widen(api, s["KF"], dim), desc=w(s["desc"]), dmask=w(s["dmask"]))
 
 
 def device_sim3(api, m, s, cap, layout, th=7.5, already2=True, pre=None, mp1=None, mp2=None, stream=None):
@@ -67,41 +32,26 @@ def device_sim3(api, m, s, cap, layout, th=7.5, already2=True, pre=None, mp1=Non
     import torch
     KF1, KF2 = s["KF1"], s["KF2"]
     if KF1 is KF2 and layout == "same":
-        kf1 = kf2 = _pack_kfs([KF1], cap, "single")[0]
+        kf1 = kf2 = pack_frames([KF1], cap, layout="single")[0]
     else:
-        kf1, kf2 = _pack_kfs([KF1, KF2], cap, "parts" if layout == "same" else layout)
+        kf1, kf2 = pack_frames([KF1, KF2], cap, layout="parts" if layout == "same" else layout)
     pre = s["pre"] if pre is None else pre
     a2 = np.zeros(len(KF2.keys), np.uint8)
     for i in np.flatnonzero(pre >= 0):
         j = int(s["obs_idx"][pre[i]]) if pre[i] < len(s["obs_idx"]) else -1
         if 0 <= j < len(KF2.keys):
             a2[j] = 1
-    dm = _dev_map(s)
-    m12_t = _slots(api, KF1, pre, cap, GUARD)
-    masks_t = _t(np.stack(s["rig1"].masks))
+    dm = dev_map(s, bad=s["bad"])
+    m12_t = to_slots(api, KF1, pre, cap, GUARD)
+    masks_t = on_device(np.stack(s["rig1"].masks))
     n, st, out = m.SearchBySim3Device(kf1, kf2, cap, s["rig1"], s["rig2"], masks_t, KF1.scale_factors,
-                                      _slots(api, KF1, s["mp1"] if mp1 is None else mp1, cap, BIG_ID),
-                                      _slots(api, KF2, s["mp2"] if mp2 is None else mp2, cap, BIG_ID), dm["world_t"], dm["min_t"], dm["max_t"],
+                                      to_slots(api, KF1, s["mp1"] if mp1 is None else mp1, cap, BIG_ID),
+                                      to_slots(api, KF2, s["mp2"] if mp2 is None else mp2, cap, BIG_ID), dm["world_t"], dm["min_t"], dm["max_t"],
                                       dm["desc_t"], dm["dmask_t"], s["s12"], s["R12"], s["t12"], th, m12_t,
-                                      already2_t=_t(api.contiguous_to_slots(a2, _counts(KF2), cap, fill=1).astype(np.uint8)) if already2 else None,
+                                      already2_t=to_slots(api, KF2, a2, cap, 1, dtype=np.uint8) if already2 else None,
                                       bad_t=dm["bad_t"], stream=stream)
     torch.cuda.synchronize()
-    return int(n.item()), int(st.item()), _back(api, KF1, out, cap)
-
-
-def device_scw(api, m, s, cap, layout, points=None, matched=None, th=10, stream=None):
-    """SearchByProjectionKFScwDevice on the scene -> (nmatches, status, vpMatched in contiguous order, diag)"""
-    import torch
-    KF = s["KF"]
-    (kf,) = _pack_kfs([KF], cap, layout)
-    dm = _dev_map(s)
-    pts = s["points"] if points is None else points
-    matched_t = _slots(api, KF, s["matched"] if matched is None else matched, cap, GUARD)
-    n, st, out, diag = m.SearchByProjectionKFScwDevice(kf, cap, s["rig"], s["Scw"], _t(np.stack(s["rig"].masks)), KF.scale_factors,
-                                                       _t(np.asarray(pts, np.int32)), dm["world_t"], dm["min_t"], dm["max_t"], dm["desc_t"],
-                                                       dm["dmask_t"], th, matched_t, bad_t=dm["bad_t"], stream=stream, diag=True)
-    torch.cuda.synchronize()
-    return int(n.item()), int(st.item()), _back(api, KF, out, cap), diag.cpu().numpy()
+    return int(n.item()), int(st.item()), from_slots(api, out, counts(KF1), cap, GUARD)
 
 
 # ---- SearchBySim3 ---------------------------------------------------------------------------------------------------------------
@@ -113,7 +63,7 @@ def test_sim3_parity(api, oa, rm, frames, cams, masks, dim, layout):
     s = _sim3_at(api, sim3_scene(api, oa, cams, frames[0]), dim)
     m = api.cORBmatcher(0.6, False, dim, masks)
     hn, h12 = host_sim3(m, s, 7.5)
-    cap = max(_counts(s["KF1"])) + 5
+    cap = max(counts(s["KF1"])) + 5
     dn, st, d12 = device_sim3(api, m, s, cap, layout)
     assert st == api.MCS_OK and dn == hn and np.array_equal(d12, h12) and dn > 30
     if rm and dim == 32:
@@ -139,7 +89,7 @@ def test_sim3_same_key_frame_in_one_buffer(api, oa, frames, cams):
     s = dict(s, KF2=s["KF1"])
     m = api.cORBmatcher(0.6, False, 32, True)
     hn, h12 = host_sim3(m, s, 7.5)
-    dn, st, d12 = device_sim3(api, m, s, max(_counts(s["KF1"])) + 1, "same")
+    dn, st, d12 = device_sim3(api, m, s, max(counts(s["KF1"])) + 1, "same")
     assert st == api.MCS_OK and dn == hn > 30 and np.array_equal(d12, h12)
 
 
@@ -150,7 +100,7 @@ def test_sim3_invalid_ids_and_edges(api, oa, frames, cams):
     s = sim3_scene(api, oa, cams, frames[0])
     m = api.cORBmatcher(0.6, False, 32, False)
     n_pts = len(s["world"])
-    cap = max(_counts(s["KF1"]))                                        # the fullest camera exactly at capacity
+    cap = max(counts(s["KF1"]))                                        # the fullest camera exactly at capacity
     for which in ("mp1", "mp2", "pre"):
         row = (s["pre"] if which == "pre" else s[which]).copy()
         k = int(np.flatnonzero(s["mp1"] >= 0)[3]) if which != "mp2" else int(np.flatnonzero(s["mp2"] >= 0)[5])
@@ -248,7 +198,7 @@ def z_edge_scene(api, oa, cams, F):
     that projects back onto keypoint i at rig z 0.1, so a kept probe agrees.  Returns the scene and the probes' z class per keypoint
     (0: zero, 1: +ulp, 2: -ulp, -1: no probe)."""
     rays, _, _ = oa.frame_prepare(F.keys, F.key_cam, cams)
-    M_c = T.make_scene(api, oa, cams, F, 61, npts=10)["M_c"].copy()
+    M_c = make_scene(api, oa, cams, F, 61, npts=10)["M_c"].copy()
     M_c[0] = np.eye(4)
     M_c[0, 2, 3] = -0.1
     rig = api.Rig(cams, M_c, np.eye(4))
@@ -266,7 +216,7 @@ def z_edge_scene(api, oa, cams, F):
         x[2] = (0.0, 2 * tiny, -2 * tiny)[k % 3]                     # p3Dc2.z = X.z / 2: 0, +ulp, -ulp
         world[i], world[n + i] = x, (lam2 * r - back) / 2.0
         depth[i], depth[n + i] = lam, lam2
-        desc[i], desc[n + i] = T.flip_bits(rng, F.desc[[i, i]], 4)
+        desc[i], desc[n + i] = flip_bits(rng, F.desc[[i, i]], 4)
         mp1[i], mp2[i], zcls[i] = i, n + i, k % 3
     oct_ = np.concatenate([F.keys["octave"], F.keys["octave"]])
     min_d = depth / (1.1 * np.asarray(F.scale_factors)[oct_])
@@ -281,7 +231,7 @@ def test_sim3_distance_and_level_edges(api, oa, frames, cams):
     agreement.  The device equals the mirror on the kept scene and on each flipped one."""
     s = sim3_scene(api, oa, cams, frames[0])
     m = api.cORBmatcher(0.6, False, 32, False)
-    cap = max(_counts(s["KF1"])) + 2
+    cap = max(counts(s["KF1"])) + 2
     kept, flipped, edited = distance_edge_scenes(api, s)
     assert all(len(v) >= 8 for v in edited.values()), {k: len(v) for k, v in edited.items()}
     hn, h12 = host_sim3(m, kept, 7.5)
@@ -303,7 +253,7 @@ def test_sim3_rig_frame_z_edge(api, oa, frames, cams):
         p4 = api._mm(api.inv_rigid(s["M_c"][0]), np.append(s["world"][i] / 2.0, 1.0))
         assert 0.1 - 1e-12 < p4[2] < 0.1 + 1e-12
     hn, h12 = host_sim3(m, s, 7.5)
-    dn, st, d12 = device_sim3(api, m, s, max(_counts(s["KF1"])) + 1, "single")
+    dn, st, d12 = device_sim3(api, m, s, max(counts(s["KF1"])) + 1, "single")
     assert st == api.MCS_OK and dn == hn and np.array_equal(d12, h12)
     agree = d12 == s["mp2"]
     assert (agree & (zcls == 0)).sum() >= 10 and (agree & (zcls == 1)).sum() >= 10
@@ -319,7 +269,7 @@ def test_scw_parity(api, oa, rm, frames, cams, masks, dim, layout):
     s = _scw_at(api, scw_scene(api, oa, cams, frames[0]), dim)
     m = api.cORBmatcher(0.6, False, dim, masks)
     hn, hm = host_scw(m, s)
-    cap = max(_counts(s["KF"])) + 3
+    cap = max(counts(s["KF"])) + 3
     dn, st, dmatched, diag = device_scw(api, m, s, cap, layout)
     assert st == api.MCS_OK and dn == hn > 50 and np.array_equal(dmatched, hm)
     if rm and dim == 32:
@@ -337,8 +287,8 @@ def scw_model(api, oa, m, s, rows=True, drop=True, zero="contiguous", points=Non
     pts = s["points"] if points is None else points
     out = (s["matched"] if matched is None else matched).copy()
     found = set(int(x) for x in out if x >= 0)
-    counts = np.asarray(_counts(KF))
-    first = np.concatenate([[0], np.cumsum(counts)])
+    n_cam = counts(KF)
+    first = np.concatenate([[0], np.cumsum(n_cam)])
     rig = api._sim3_rig(s["rig"], s["Scw"])
     sf = np.asarray(KF.scale_factors)
     dist = (lambda a, b, ma, mb: api.DescriptorDistance64Masked(a, b, ma, mb, KF.desc.shape[1])) if m.havingMasks else \
@@ -372,7 +322,7 @@ def scw_model(api, oa, m, s, rows=True, drop=True, zero="contiguous", points=Non
             d = dist(s["desc"][p], KF.desc[r], s["dmask"][p], KF.dmask[r])
             if d < best:
                 best, bi = d, idx
-        z = {"contiguous": 0, "slot0": 0 if counts[0] else -1, None: -1}[zero]
+        z = {"contiguous": 0, "slot0": 0 if n_cam[0] else -1, None: -1}[zero]
         if best <= m.TH_LOW_ and bi >= 0 and bi != z:
             out[bi] = p
             n += 1
@@ -384,7 +334,7 @@ def quirk_scene(api, oa, cams, F, empty_cam0=False, seed=71):
     entry's position is the point's camera), with keypoint i's descriptor a few bits off; entry 0 sits on keypoint 0 exactly"""
     if empty_cam0:
         sel = np.flatnonzero(F.key_cam != 0)
-        F = api.Frame(F.keys[sel], F.key_cam[sel], F.desc[sel], F.dmask[sel], T.SIZES, F.scale_factors)
+        F = api.Frame(F.keys[sel], F.key_cam[sel], F.desc[sel], F.dmask[sel], SIZES, F.scale_factors)
     s = scw_scene(api, oa, cams, F, seed=seed, cam0_only=False, scale=1.0)
     KF, sc = s["KF"], s["sc"]
     rays, _, _ = oa.frame_prepare(KF.keys, KF.key_cam, cams)
@@ -392,7 +342,7 @@ def quirk_scene(api, oa, cams, F, empty_cam0=False, seed=71):
     rng = np.random.default_rng(seed)
     depth = rng.uniform(2.0, 5.0, n)
     world = np.stack([api._mm(sc["rig"].MtMc[int(KF.key_cam[k])], np.append(rays[k] * depth[k], 1.0))[:3] for k in range(n)])
-    desc = T.flip_bits(rng, KF.desc, 6)
+    desc = flip_bits(rng, KF.desc, 6)
     desc[0] = KF.desc[0]
     oct_ = KF.keys["octave"]
     min_d = depth / (1.1 * np.asarray(KF.scale_factors)[oct_])        # level octave + 1: the window keeps the octave
@@ -411,7 +361,7 @@ def test_scw_quirks_each_matter(api, oa, frames, cams, masks):
     m = api.cORBmatcher(0.6, False, 32, masks)
     for empty in (False, True):
         s = quirk_scene(api, oa, cams, frames[0], empty_cam0=empty)
-        cap = max(_counts(s["KF"])) + 2
+        cap = max(counts(s["KF"])) + 2
         hn, hm = host_scw(m, s)
         mn, mm = scw_model(api, oa, m, s)
         dn, st, dmatched, _ = device_scw(api, m, s, cap, "single")
@@ -429,12 +379,12 @@ def test_scw_entries_past_the_keypoints(api, oa, frames, cams):
     m = api.cORBmatcher(0.6, False, 32, True)
     n_keys = len(s["KF"].keys)
     extra = np.concatenate([s["points"], np.full(n_keys - len(s["points"]), -1, np.int32), np.arange(20, dtype=np.int32)])
-    dn, st, dmatched, diag = device_scw(api, m, s, max(_counts(s["KF"])) + 1, "parts", points=extra)
+    dn, st, dmatched, diag = device_scw(api, m, s, max(counts(s["KF"])) + 1, "parts", points=extra)
     hn, hm = host_scw(m, s)
     assert st == api.MCS_ERR_INVALID and dn == hn and np.array_equal(dmatched, hm)
     # NULL, bad or already found entries past the count never reach the camera look-up: no status
     tail = np.concatenate([s["points"], np.full(n_keys - len(s["points"]) + 5, -1, np.int32)])
-    dn, st, dmatched, _ = device_scw(api, m, s, max(_counts(s["KF"])) + 1, "parts", points=tail)
+    dn, st, dmatched, _ = device_scw(api, m, s, max(counts(s["KF"])) + 1, "parts", points=tail)
     assert st == api.MCS_OK and dn == hn and np.array_equal(dmatched, hm)
 
 
@@ -454,7 +404,7 @@ def contention_scene(api, oa, cams, F, L=40):
         keys["octave"][k] = 0
         b = bits.copy(); b[:3 * k] ^= 1
         desc[k] = np.packbits(b)
-    KF = api.Frame(keys, KF.key_cam, desc, dmask, T.SIZES, KF.scale_factors)
+    KF = api.Frame(keys, KF.key_cam, desc, dmask, SIZES, KF.scale_factors)
     rays, _, _ = oa.frame_prepare(keys, KF.key_cam, cams)
     n = len(keys)
     world = np.zeros((n, 3)); qdesc = np.zeros_like(desc); min_d = np.ones(n); pts = np.full(n, -1, np.int32)
@@ -475,7 +425,7 @@ def test_scw_dense_contention(api, oa, frames, cams, masks):
     s = contention_scene(api, oa, cams, frames[0])
     m = api.cORBmatcher(0.6, False, 32, masks)
     hn, hm = host_scw(m, s)
-    dn, st, dmatched, diag = device_scw(api, m, s, max(_counts(s["KF"])) + 1, "single")
+    dn, st, dmatched, diag = device_scw(api, m, s, max(counts(s["KF"])) + 1, "single")
     assert st == api.MCS_OK and dn == hn and np.array_equal(dmatched, hm) and hn >= 30
     assert diag[0] == api.lib().mcs_search_by_projection_max_rounds() and diag[1] >= 0 and diag[2] >= 30, diag
 
@@ -486,7 +436,7 @@ def test_scw_edges(api, oa, frames, cams):
     s = scw_scene(api, oa, cams, frames[0])
     m = api.cORBmatcher(0.6, False, 32, False)
     n_pts = len(s["world"])
-    cap = max(_counts(s["KF"]))
+    cap = max(counts(s["KF"]))
     pts = s["points"].copy()
     pts[7] = n_pts + 3
     dn, st, dm_, _ = device_scw(api, m, s, cap, "single", points=pts)

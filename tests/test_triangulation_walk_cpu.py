@@ -5,19 +5,13 @@ mutant of the model told apart from the sequential loop by some scene, in its ma
 import numpy as np
 import pytest
 
-import test_ref_match_cpu as T
 import triangulation_model as tm
-from test_search_for_triangulation_device_cpu import reference_tri
+from device_frames import counts, taped_rm
+from search_scenes import reference_tri
 
 SPECS = tm.catalogue()
 _cache = {}
-
-
-@pytest.fixture(scope="module")
-def rm():
-    """the reference's own matcher, live while recording and replayed from tests/golden/ref_tape_triangulation_walk_cpu.*"""
-    import ref_tape
-    return ref_tape.module("ref_match_api", "triangulation_walk_cpu", T.TAPE_LIMIT)
+rm = taped_rm("triangulation_walk_cpu")
 
 
 def scene(api, oa, cams, spec):
@@ -166,7 +160,7 @@ def test_capacity_bound(api, oa, cams):
     """a camera with count == capacity == 65535 free KF2 rows: a winner at compact index 65534 from the list, and one in the last
     stride of tr_scan from a rescan, both in the last database chunk"""
     (spec, s, p), = _runs(api, oa, cams, "capacity")
-    assert tm.counts(s["nbs"][0])[0] == s["cap"] == tm.CAPACITY and (s["mps"][0] == -1).all()
+    assert counts(s["nbs"][0])[0] == s["cap"] == tm.CAPACITY and (s["mps"][0] == -1).all()
     chunk, splits = tm.chunk_of(s["cap"], 3)
     by_win = {r["win"]: r for r in p["record"][0]}
     assert by_win[tm.CAPACITY - 1]["rule"] == "list_win"

@@ -7,7 +7,8 @@ import numpy as np
 import pytest
 
 import triangulation_model as tm
-from test_search_for_triangulation_device_gpu import POISON, assert_same, device_call, host_call
+from device_frames import POISON
+from device_searches import assert_same_tri, device_tri, host_tri
 
 pytestmark = pytest.mark.gpu
 SPECS = tm.catalogue()
@@ -25,12 +26,12 @@ def test_device_equals_model(api, oa, cams, spec):
         chunk, splits = tm.chunk_of(cap, 3, torch.cuda.get_device_properties(0).multi_processor_count)
         rows = s["tie_rows"] if spec[0] == "ties" else [s["scan_row"], tm.CAPACITY - 1]
         assert splits >= 2 and (rows[0] < chunk <= rows[-1] if spec[0] == "ties" else min(rows) >= (splits - 1) * chunk)
-    host = host_call(api, m, F1, F2, s["mp1"], s["mps"][0], cams, cap, s["E"], s["epi"])
+    host = host_tri(api, m, F1, F2, s["mp1"], s["mps"][0], cams, cap, s["E"], s["epi"])
     live = np.array([v is not None for v in p["slots"]])
     want = np.where(live, p["slots"], POISON).astype(np.int64)
     assert host[0] == p["n"] and np.array_equal(host[1][live], want[live])
     for layout in ("single", "parts", "joint"):
-        dev = device_call(api, m, F1, F2, s["mp1"], s["mps"][0], cams, cap, s["E"], layout, s["epi"])
-        assert_same(api, F1, dev, host, cap)
+        dev = device_tri(api, m, F1, F2, s["mp1"], s["mps"][0], cams, cap, s["E"], layout, s["epi"])
+        assert_same_tri(api, F1, dev, host, cap)
         assert dev[0] == p["n"] and np.array_equal(dev[1], want), layout
         assert dev[2].tolist() == p["diag"], (layout, dev[2].tolist(), p["diag"])

@@ -2,7 +2,7 @@
 and without a device the call fails with MCS_ERR_NO_DEVICE."""
 import numpy as np
 
-FAKE = 0x10000      # stands for a device pointer: never dereferenced by the host
+from device_frames import FAKE, declared_symbols
 
 
 def _search(api, cur=(FAKE, 1, 4, 0), last=(FAKE, 1, 4, 0), n_cams=4, capacity=2016, dim=32, sizes=None, last_mp=FAKE, n_points=1000,
@@ -44,7 +44,6 @@ def test_window_search_device_validation(api):
 
 
 def test_symbol_is_declared_and_exported(api):
-    from test_cabi_symbols import declared_symbols
     assert "mcs_window_search_device" in declared_symbols()
     assert hasattr(api.lib(), "mcs_window_search_device")
     assert hasattr(api.cORBmatcher, "WindowSearchDevice")

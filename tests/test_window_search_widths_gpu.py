@@ -8,9 +8,10 @@ import numpy as np
 import pytest
 
 import acceptance_model as am
-
-from test_search_projection_device_gpu import _device_search, _per_cam, _sizes
-from test_window_edges_cpu import EMPTY_CAM, SF, edge_scene, flip, projection_scene, second_frame
+from device_frames import flip, on_device, per_cam, sizes
+from device_searches import device_projection
+from match_scenes import random_rig
+from window_edge_scenes import EMPTY_CAM, SF, edge_scene, projection_scene, second_frame
 
 pytestmark = pytest.mark.gpu
 
@@ -274,7 +275,7 @@ def test_device_search_on_edge_scenes(api, oa, dim, masked, layout):
         sc = edge_scene(kind, dim)
         F = sc.frame
         mps = projection_scene(F, dim, masked, seed=dim + j)
-        per = _per_cam(F)
+        per = per_cam(F)
         assert len(per[EMPTY_CAM][0]) == 0
         cap = max(len(p[0]) for p in per) + 7 + 10 * j
         assert cap % 32 != 0
@@ -283,7 +284,7 @@ def test_device_search_on_edge_scenes(api, oa, dim, masked, layout):
             s = None if start is None else start.copy()
             n, fmp = m.SearchByProjection(F, mps, th, s)
             on, ofmp = oa.search_by_projection(F, mps, th, 0.8, m.TH_HIGH_, masked, None if start is None else start.copy())
-            gn, gfmp, status, diag = _device_search(api, m, per, _sizes(F), F.scale_factors, mps, th,
+            gn, gfmp, status, diag = device_projection(api, m, per, sizes(F), F.scale_factors, mps, th,
                                                     pre=None if start is None else start.copy(), layout=layout, cap=cap)
             assert status == api.MCS_OK and n == on == gn and np.array_equal(fmp, ofmp) and np.array_equal(gfmp, fmp)
             assert n > 100 and diag[2] == int(((mps.in_view != 0) & (mps.bad[:, None] == 0)).sum())
@@ -296,7 +297,7 @@ def test_device_search_from_the_extractor(api, oa, cams, dim, masked):
     import torch
     from multicol_slam_b200 import rig, synth
     ex = api.mdBRIEFextractorOct(nfeatures=1200, do_dBrief=True, learnMasks=masked, descSize=dim)
-    imgs = torch.from_numpy(np.stack([synth.frame(cams[c], 400 + c) for c in range(3)])).cuda()
+    imgs = on_device(np.stack([synth.frame(cams[c], 400 + c) for c in range(3)]))
     mk = np.stack([synth.mirror_mask(c) for c in cams])
     cap = ex.capacity
     packed = torch.zeros(rig.packed_layout(3, cap, dim)[1], dtype=torch.uint8, device="cuda")
@@ -324,12 +325,10 @@ def test_device_search_from_the_extractor(api, oa, cams, dim, masked):
 @width
 def test_device_projection_chain(api, oa, cams, dim):
     """project_mappoints_device -> the device search == project_mappoints -> the host search, at descriptor size dim"""
-    import torch
     from multicol_slam_b200 import synth
-    from test_match_gpu import _random_rig
     rng = np.random.default_rng(12 + dim)
     n = 15000
-    mtmc, inv = _random_rig(rng, 3)
+    mtmc, inv = random_rig(rng, 3)
     masks = np.stack([synth.mirror_mask(c) for c in cams])
     pos = rng.normal(size=(n, 3)); pos *= (rng.uniform(1.5, 12.0, n) / np.linalg.norm(pos, axis=1))[:, None]
     nrm = rng.normal(size=(n, 3)); nrm /= np.linalg.norm(nrm, axis=1)[:, None]
@@ -337,14 +336,13 @@ def test_device_projection_chain(api, oa, cams, dim):
     F = natural(api, cams, dim, True)[0]
     sf = F.scale_factors
     g = api.project_mappoints(inv, mtmc, cams, masks, pos, nrm, dmin, dmax, sf)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()  # noqa: E731
-    d = api.project_mappoints_device(inv, mtmc, cams, t(masks), t(pos), t(nrm), t(dmin), t(dmax), sf)
+    d = api.project_mappoints_device(inv, mtmc, cams, on_device(masks), on_device(pos), on_device(nrm), on_device(dmin), on_device(dmax), sf)
     src = rng.integers(0, len(F.keys), n)
     desc, dmask = F.desc[src].copy(), F.dmask[rng.integers(0, len(F.keys), n)].copy()
     m = api.cORBmatcher(0.8, False, dim, True)
     ng, fg = m.SearchByProjection(F, api.MapPoints(np.zeros(n, np.uint8), *g, desc, dmask), 3.0)
-    mdev = api.MapPointsDevice(None, *d, t(desc), t(dmask))
-    gn, gf, status, _ = _device_search(api, m, _per_cam(F), _sizes(F), sf, mdev, 3.0)
+    mdev = api.MapPointsDevice(None, *d, on_device(desc), on_device(dmask))
+    gn, gf, status, _ = device_projection(api, m, per_cam(F), sizes(F), sf, mdev, 3.0)
     assert status == api.MCS_OK and gn == ng and np.array_equal(gf, fg) and ng > 50
 
 
@@ -394,7 +392,7 @@ def test_device_long_dependency_chain(api, oa, dim):
     cap_rounds = api.lib().mcs_search_by_projection_max_rounds()
     assert pn == n and np.array_equal(pfmp, fmp) and pdiag[0] == cap_rounds and pdiag[1] >= 0 and pdiag[3] > 0
     for layout in ("single", "parts"):
-        gn, gfmp, status, diag = _device_search(api, m, _per_cam(F), _sizes(F), SF, mps, 3.0, pre=pre.copy(), layout=layout)
+        gn, gfmp, status, diag = device_projection(api, m, per_cam(F), sizes(F), SF, mps, 3.0, pre=pre.copy(), layout=layout)
         assert status == api.MCS_OK and gn == n and np.array_equal(gfmp, fmp)
         assert diag.tolist() == pdiag
 
@@ -430,7 +428,7 @@ def test_device_list_edge(api, oa, dim, masked, n_cand, taken):
     on, ofmp = oa.search_by_projection(F, mps, 1.0, 0.8, m.TH_HIGH_, masked, pre.copy())
     assert n == on and np.array_equal(fmp, ofmp)
     assert n == (0 if (taken and n_cand == 9) else 1)
-    gn, gfmp, status, diag = _device_search(api, m, _per_cam(F), _sizes(F), SF, mps, 1.0, pre=pre.copy())
+    gn, gfmp, status, diag = device_projection(api, m, per_cam(F), sizes(F), SF, mps, 1.0, pre=pre.copy())
     assert status == api.MCS_OK and gn == n and np.array_equal(gfmp, fmp)
     assert (diag[3] > 0) == (taken and n_cand == 9)
 
@@ -461,7 +459,7 @@ def test_device_full_capacity_whole_image(api, oa, dim):
     assert n == on and np.array_equal(fmp, ofmp) and n == nmp
     _, start, items = oa.frame_prepare(F.keys, F.key_cam, _one_cam(W, H))
     assert len(items) == cap and start[-1] == cap
-    gn, gfmp, status, diag = _device_search(api, m, _per_cam(F), _sizes(F), SF, mps, th, cap=cap, first_image=1)
+    gn, gfmp, status, diag = device_projection(api, m, per_cam(F), sizes(F), SF, mps, th, cap=cap, first_image=1)
     assert status == api.MCS_OK and gn == n and np.array_equal(gfmp, fmp)
 
 
@@ -495,7 +493,7 @@ def test_every_window_and_level_ratio_instantiation_launched(api):
                 api.window_search(F, sc.queries[:64], sc.qdesc, sc.qmask if masked else None, max_cand=4096)
                 m = api.cORBmatcher(0.8, False, dim, masked)
                 mps = projection_scene(F, dim, masked, seed=1, nmp=200)
-                _device_search(api, m, _per_cam(F), _sizes(F), F.scale_factors, mps, 3.0)
+                device_projection(api, m, per_cam(F), sizes(F), F.scale_factors, mps, 3.0)
                 rng = np.random.default_rng(0)
                 d1, d2 = F.desc[:200], F.desc[200:400]
                 fv = (np.array([2], np.int32), np.array([0, 200], np.int32), np.arange(200, dtype=np.int32))

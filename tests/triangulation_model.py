@@ -16,6 +16,9 @@ import ctypes as C
 
 import numpy as np
 
+from device_frames import counts
+from search_scenes import epipolar_residual, essential, rig_of
+
 K = 8                        # kTopKMax: list length per query
 TOPK_THREADS, DB_TILE = 128, 256     # kTopkThreads (query rows per list CTA), kDbTile
 SCAN_THREADS = 256 - 32      # tr_scan's scanning threads (warps 1 .. of the walk's CTA)
@@ -164,10 +167,6 @@ def to_slots(s, m12):
     return out
 
 
-def counts(F):
-    return [int((F.key_cam == c).sum()) for c in range(len(F.cam_w))]
-
-
 def chunk_of(capacity, n_cams, sms=H100_SMS):
     """launch_search_for_triangulation's database chunk of seg_lists_kernel<CamSegs> (a multiple of kDbTile) and the number of
     chunks: list_plan(sms, ceil(capacity / 128) * n_cams, capacity) in match_kernels.cu, the one plan of the K-best list kernels"""
@@ -255,7 +254,7 @@ def pass_pixels(api, cams, E):
         n = E[c, c] @ r1
         r2 = r1 - (r1 @ n) / (n @ n) * n
         px = f32(*api.world_to_img(cams[c], *r2))
-        res = residual(api, r1, np.array(api.img_to_world(cams[c], *px)), E[c, c])
+        res = epipolar_residual(api, r1, np.array(api.img_to_world(cams[c], *px)), E[c, c])
         assert res < 1e-9, (c, res)
         out.append(px)
     return out
@@ -270,18 +269,12 @@ def fail_pixels(api, cams, E):
         for x in range(60, 700, 40):
             for y in range(40, 450, 40):
                 r2 = np.array(api.img_to_world(cams[c], float(x), float(y)))
-                v = residual(api, r1, r2, E[c, c])
+                v = epipolar_residual(api, r1, r2, E[c, c])
                 if v > best:
                     best, bp = v, (float(x), float(y))
         assert best > 0.05, best
         out.append(bp)
     return out
-
-
-def residual(api, r1, r2, E):
-    """(nom * nom) / den of CheckDistEpipolarLine, the host's arithmetic"""
-    from test_search_for_triangulation_device_gpu import residual as res
-    return res(api, r1, r2, E)
 
 
 def finish(api, oa, P, cams, rig1, rig2, E, cap_extra=0, epi=1e-2, cap=None, **info):
@@ -299,7 +292,6 @@ def th_low_of(dim, masked):
 
 
 def _geometry(api, cams, seed):
-    from test_search_for_triangulation_device_cpu import essential, rig_of
     rng = np.random.default_rng(1000 + seed)
     rig1 = rig_of(api, cams, [0, 0, 0])
     rig2 = rig_of(api, cams, rng.uniform(0.02, 0.05, 3) * rng.choice([-1, 1], 3))
@@ -458,7 +450,7 @@ def _epi(api, oa, cams, P, rig1, rig2, E, var):
         P.query(c, b)
     r1 = np.array(api.img_to_world(cams[0], *PIX[0]))
     r2 = np.array(api.img_to_world(cams[0], *near))
-    res = residual(api, r1, r2, E[0, 0])
+    res = epipolar_residual(api, r1, r2, E[0, 0])
     assert 1e-8 < res < 1e-3, res
     epi = res if var == "at" else float(np.nextafter(res, np.inf))
     return finish(api, oa, P, cams, rig1, rig2, E, epi=epi, cls="epi", var=var, near_row=j)

@@ -62,9 +62,7 @@ def main():
                 dmask=np.where(rng.random((n_kf, NS, dim)) < 0.85, 0xFF, rng.integers(0, 256, (n_kf, NS, dim))).astype(np.uint8),
                 octave=rng.integers(0, nl, (n_kf, NS)).astype(np.int32), kf_counts=counts, ow=rng.uniform(-5, 5, (n_kf, 3)),
                 kf_bad=np.zeros(n_kf, np.int32))
-    bufs, frames = S.packed_frames(base, "one")
-    packed = torch.from_numpy(bufs[0]).cuda()
-    kfs = [((packed, a, b, c), base["ow"][k], 0) for k, (_, a, b, c) in enumerate(frames)]
+    kfs = [(fr, base["ow"][k], 0) for k, fr in enumerate(S.packed_frames(base, "one"))]
     res = {"card": _card(), "n_kf": n_kf, "n_cams": nc, "capacity": cap, "dim": dim, "masks": True}
     for name, n_points in (("process_new_keyframe", 8000), ("local_ba", 30000)):
         obs, ref, X, bad = batch(rng, n_points, n_kf, nc, cap, counts)
