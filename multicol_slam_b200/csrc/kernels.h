@@ -13,9 +13,9 @@ struct DescribeArgs {
 };
 
 cudaError_t upload_constants(const signed char* pairs, const signed char* du, const signed char* dv);
-void launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_t* src, size_t src_img_bytes,
-                     uint8_t* dst, uint8_t* dst_blur, const uint8_t* mask0, int mask_w, size_t mask_bytes,
-                     const int* cam_of_image, const uint8_t* tile_flags, uint32_t* raw, int* raw_count, cudaStream_t st);
+cudaError_t launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_t* src, size_t src_img_bytes,
+                            uint8_t* dst, uint8_t* dst_blur, const uint8_t* mask0, int mask_w, size_t mask_bytes,
+                            const int* cam_of_image, const uint8_t* tile_flags, uint32_t* raw, int* raw_count, cudaStream_t st);
 cudaError_t launch_octree(const PyramidGeom& G, const PyramidGeom* G_dev, int n_images, const uint32_t* raw,
                           const int* raw_count, uint16_t* node_of, uint32_t* sel_xys, int* sel_count, int* status,
                           cudaStream_t st, int level_lo = 0, int level_count = -1);

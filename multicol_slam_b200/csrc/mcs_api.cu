@@ -186,7 +186,7 @@ int plan_geometry(mcs_extractor* ex, int W, int H, int in_stride, std::vector<in
         std::vector<int16_t> xofs(g.w), xa0(g.w), xa1(g.w), yofs(g.h), yb0(g.h), yb1(g.h), mx(g.w), my(g.h);
         if (l) {
             const double scale_x = 1.0 / ((double)g.w / g.sw), scale_y = 1.0 / ((double)g.h / g.sh);
-            // the staged source region of a 72x40 tile must fit 176 x 88 bytes: (72*s + 17) <= 176, (40*s + 2) <= 88
+            // the staged source region of a 72x72 tile must fit kSrcWB x kSrcH = 176 x 152 bytes: (72*s + 17) <= 176, (72*s + 2) <= 152
             if (scale_x > 2.08 || scale_y > 2.08) return mcs_fail(MCS_ERR_UNSUPPORTED, "scale factors above 2 are not supported");
             for (int dx = 0; dx < g.w; ++dx) {
                 float fx = (float)((dx + 0.5) * scale_x - 0.5);
@@ -227,6 +227,7 @@ int plan_geometry(mcs_extractor* ex, int W, int H, int in_stride, std::vector<in
                 bh = std::max(bh, hi - lo + 1);
             }
             g.box_w = (bw + 15) & ~15; g.box_h = bh;
+            if (g.box_w > kSrcWB || g.box_h > kSrcH) return mcs_fail(MCS_ERR_UNSUPPORTED, "K1 source region larger than its staging");
         }
         // FAST cell grid (ref :876-949, SURVEY Appendix A.6)
         std::vector<int16_t> cellx(g.w, -1), celly(g.h, -1);
@@ -428,8 +429,8 @@ int enqueue_kernels(mcs_extractor* ex, int n_images, const uint8_t* images_dev, 
     for (int l = 0; l < G.nlevels; ++l) {
         const uint8_t* src = l ? ex->lvl[l - 1].p : images_dev;
         const size_t src_bytes = l ? G.lv[l - 1].img_bytes : (size_t)stride * H;
-        launch_pyr_fast(G, l, n_images, src, src_bytes, ex->lvl[l].p, ex->blur[l].p, ex->masks.p, W, (size_t)W * H,
-                        coi_d, ex->tile_flags.p, ex->raw.p, ex->raw_count.p, st);
+        CUDA_CHECK(launch_pyr_fast(G, l, n_images, src, src_bytes, ex->lvl[l].p, ex->blur[l].p, ex->masks.p, W, (size_t)W * H,
+                                   coi_d, ex->tile_flags.p, ex->raw.p, ex->raw_count.p, st));
     }
     CUDA_CHECK(cudaGetLastError());
     if (ex->profiling) CUDA_CHECK(cudaEventRecord(ex->ev[1], st));

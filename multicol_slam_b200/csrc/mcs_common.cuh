@@ -12,10 +12,12 @@ constexpr int kHalfPatch = 16;   // HALF_PATCH_SIZE (ref :84)
 constexpr int kMaxLevels = MCS_MAX_LEVELS;
 
 // K1 tiling: one CTA produces a TW x TH tile of level l (+ kHalo ring kept in shared memory)
-constexpr int kTW = 64, kTH = 32, kHalo = 4;
+constexpr int kTW = 64, kTH = 64, kHalo = 4;
 constexpr int kTileW = kTW + 2 * kHalo;     // 72
-constexpr int kTileH = kTH + 2 * kHalo;     // 40
-constexpr int kSrcH = 88;                   // staged source rows, enough for scale factors <= 2
+constexpr int kTileH = kTH + 2 * kHalo;     // 72
+// staged source region of a tile (the level's TMA box): at most kSrcH rows of kSrcWB bytes, enough for scale factors <= 2.08
+// (72 * 2.08 + 17 <= 176 bytes, 72 * 2.08 + 2 <= 152 rows).  K1 sizes the staging per level, box_h rows, not for the largest scale.
+constexpr int kSrcWB = 176, kSrcH = 152;
 constexpr int kMaxNodes = 2048;             // octree nodes alive at once (>= max(quota + 8, 4 * nodes_ini) of every level)
 
 // Per-level geometry + look-up tables (device pointers into one blob built by the host).

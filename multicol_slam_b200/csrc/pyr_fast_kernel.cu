@@ -3,10 +3,10 @@
 // (ref src/mdBRIEFextractorOct.cpp:1158-1201 ComputePyramid, :863-949 cell loop, :1301 boxFilter; OpenCV
 // resize / boxFilter / FAST arithmetic restated in SURVEY.md Appendix A.1 / A.3 / A.5).
 //
-// One CTA owns a 64x32 tile of level l.  The source region of level l-1 is staged in shared memory with 128-bit
-// loads, the tile (+4 px ring, REFLECT_101 at the image border) is resized once and kept in three shared forms:
-// bytes (for the stores) and two 16-bit-per-pixel copies offset by one pixel, so that ANY horizontally adjacent
-// pixel pair is one aligned 32-bit word.  Blur and FAST then run on pixel PAIRS with the packed 16x2 integer
+// One CTA owns a 64x64 tile of level l.  The source region of level l-1 is staged in shared memory by TMA (or 128-bit
+// loads), the tile (+4 px ring, REFLECT_101 at the image border) is resized once and kept in two shared 16-bit-per-pixel
+// copies offset by one pixel, so that ANY horizontally adjacent pixel pair is one aligned 32-bit word (the level's bytes are
+// stored from the even copy).  Blur and FAST then run on pixel PAIRS with the packed 16x2 integer
 // SIMD of sm_90a (16x2 adds, DPX three-way min / max):
 //   * box blur: 5 packed loads + 4 packed adds give the horizontal 5-sums of two pixels;
 //   * FAST: E_k = ring_k - centre (packed), 9-arc minima / maxima by two 3-input min (max) levels
@@ -14,6 +14,7 @@
 //     pixel pair: score = max over arcs of max(min9(E), -max9(E)) - 1, corner iff that maximum exceeds the threshold.
 // The kernel is bound by integer issue rate, not by HBM (DESIGN.md, K1): on the order of a hundred thread-instructions per
 // pixel against a few bytes of DRAM traffic.
+#include <algorithm>
 #include <cstring>
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -57,15 +58,26 @@ __device__ __forceinline__ int ctaid_x() { int v; asm volatile("mov.u32 %0, %%ct
 __device__ __forceinline__ int ctaid_y() { int v; asm volatile("mov.u32 %0, %%ctaid.y;" : "=r"(v)); return v; }
 __device__ __forceinline__ int ctaid_z() { int v; asm volatile("mov.u32 %0, %%ctaid.z;" : "=r"(v)); return v; }
 
-// resident CTAs per SM the register budget is cut for: 5 allows 48 registers, enough for FAST without spills (6 CTAs at 40
-// registers spilled and measured the same time on H100, DESIGN.md §6)
+// Phase split of the kernel's time: tools/k1_split.py --split builds this file with -DMCS_K1_SPLIT_EXIT=n into a library of its own,
+// whose CTAs return after the staging and the tables (1), after the resize (2) or after FAST (3).  The shipped build has no exit.
+#ifdef MCS_K1_SPLIT_EXIT
+#define K1_SPLIT_EXIT(n) if (MCS_K1_SPLIT_EXIT == (n)) return
+#else
+#define K1_SPLIT_EXIT(n)
+#endif
+
+// resident CTAs per SM the register budget is cut for: 5 allows 48 registers, enough for FAST without spills.  Shared memory
+// (23 KB of pixel tiles and tables plus 17.3 KB of staging at scale 1.2) also allows 5 (DESIGN.md, K1)
 constexpr int kMinBlocks = 5;
 constexpr int kThreads = 256;
-constexpr int kSrcWB = 176;                 // staged source row stride (bytes, multiple of 16)
-constexpr int kT8S = 80;                    // byte tile row stride
 constexpr int kT16S = 72;                   // 16-bit tile row stride (elements)
 constexpr int kScoreS = 68;                 // score tile row stride in 16-bit elements (66 used)
-// corner slots per warp: a warp owns kTH/8 tile rows.  Inside a FAST cell two strict 3x3 maxima are never adjacent in a row, but the
+// the score tile and the packed row sums reuse the staging area, which is dead once the tile has been resized
+constexpr int kScoreBytes = (kTH + 2) * kScoreS * 2;
+constexpr int kRowSumBytes = (kTH + 4) * (kTW / 2) * 4;
+constexpr int kStagingMin = kScoreBytes + kRowSumBytes;
+static_assert(kScoreBytes % 16 == 0, "row sums start 16-byte aligned");
+// corner slots per warp: a warp owns kTH/8 = 8 tile rows.  Inside a FAST cell two strict 3x3 maxima are never adjacent in a row, but the
 // NMS counts a neighbour in another cell as 0, so the last pixel of a cell and the first of the next can both be maxima.  Cells are
 // at least 30 px wide (nCols = int(width / 30), checked by build_geometry), so a 64-px row meets at most 4 cells and holds at most
 // sum ceil(piece / 2) <= (64 + 4) / 2 = 34 maxima (tests/test_k1_bounds_cpu.py runs every level width)
@@ -126,12 +138,10 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
                 const uint8_t* __restrict__ mask0, const int mask_w, const size_t mask_bytes,
                 const int* __restrict__ cam_of_image, const uint8_t* __restrict__ tile_flags, const int tiles_total,
                 uint32_t* __restrict__ raw, const size_t raw_img_stride, int* __restrict__ raw_count) {
-    __shared__ __align__(128) uint8_t s_src[kSrcH * kSrcWB];
+    extern __shared__ __align__(128) uint8_t s_src[];                  // staged source rows: box_h x kSrcWB bytes (launcher)
     __shared__ __align__(8) uint64_t s_bar;
-    __shared__ __align__(16) uint8_t s_t8[kTileH * kT8S];
     __shared__ __align__(16) uint16_t s_a0[kTileH * kT16S];          // s_a0[y][x]   = px(x)
     __shared__ __align__(16) uint16_t s_a1[kTileH * kT16S];          // s_a1[y][i]   = px(i+1)
-    __shared__ __align__(16) uint32_t s_h[(kTH + 4) * (kTW / 2)];    // packed horizontal 5-sums of pixel pairs
     __shared__ uint32_t s_ml[kTW / 2], s_mr[kTW / 2], s_mu[kTH], s_md[kTH];   // NMS lane masks (same-cell neighbours)
     __shared__ int16_t s_xs0[kTileW], s_xs1[kTileW], s_xa0[kTileW], s_xa1[kTileW];
     __shared__ int16_t s_ys0[kTileH], s_ys1[kTileH], s_yb0[kTileH], s_yb1[kTileH];
@@ -142,11 +152,12 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
     // 16-bit score tile; it reuses the source staging area, which is dead once the tile has been resized.  The NMS forms the
     // odd-aligned score pairs from two aligned words with a byte permute.
     uint16_t* s_s0 = (uint16_t*)s_src;                                  // s_s0[y][x] = score(x),   x = score-tile column
+    uint32_t* s_h = (uint32_t*)(s_src + kScoreBytes);                   // packed horizontal 5-sums of pixel pairs
     // corner list, one segment per warp (no atomics while collecting): lives in the 16-bit pixel tile, which is dead once the FAST
     // margins are computed (phases b, c; the barrier before phase d separates them from phase e)
     uint32_t* s_list = (uint32_t*)s_a0;
     static_assert((kThreads / 32) * kWarpCorners * 4 <= kTileH * kT16S * 2, "corner list must fit into the dead pixel tile");
-    static_assert((kTH + 2) * kScoreS * 2 <= kSrcH * kSrcWB, "score tile must fit into the staging area");
+    // the launcher sizes the staging area to at least kStagingMin
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int b = blockIdx.z;
     const int X0 = blockIdx.x * kTW, Y0 = blockIdx.y * kTH;
@@ -186,17 +197,17 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         s_xs0[tid] = (int16_t)(sx - sx_base);
         s_xs1[tid] = (int16_t)(min(sx + 1, g.sw - 1) - sx_base);
         s_xa0[tid] = g.xa0[rx]; s_xa1[tid] = g.xa1[rx];
-    } else if (tid >= 96 && tid < 96 + kTileH) {
-        const int t = tid - 96;
+    } else if (tid >= kTileW && tid < kTileW + kTileH) {
+        const int t = tid - kTileW;
         const int ry = min(max(reflect101(Y0 - kHalo + t, g.h), ya), yb);
         const int sy = g.yofs[ry];
         s_ys0[t] = (int16_t)(min(max(sy, 0), g.sh - 1) - sy_lo);
         s_ys1[t] = (int16_t)(min(max(sy + 1, 0), g.sh - 1) - sy_lo);
         s_yb0[t] = g.yb0[ry]; s_yb1[t] = g.yb1[ry];
-    } else if (tid >= 144 && tid < 144 + kTW + 2) {
-        const int x = X0 - 1 + tid - 144;
+    } else if (tid >= kTileW + kTileH && tid < kTileW + kTileH + kTW + 2) {
+        const int x = X0 - 1 + tid - (kTileW + kTileH);
         const int16_t c = (x >= 0 && x < g.w) ? g.cellx[x] : (int16_t)-1;
-        s_cellx[tid - 144] = c;
+        s_cellx[tid - (kTileW + kTileH)] = c;
         in_cells = c >= 0;
     }
     if (tid < kTH + 2) {
@@ -204,13 +215,14 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         const int16_t c = (y >= 0 && y < g.h) ? g.celly[y] : (int16_t)-1;
         s_celly[tid] = c;
         in_cells = in_cells && c >= 0;
-    } else if (tid >= 64 && tid < 64 + kTW) {
-        const int x = X0 + tid - 64;
-        s_mx[tid - 64] = x < g.w ? g.mx0[x] : (int16_t)0;
-    } else if (tid >= 128 && tid < 128 + kTH) {
-        const int y = Y0 + tid - 128;
-        s_my[tid - 128] = y < g.h ? g.my0[y] : (int16_t)0;
+    } else if (tid >= 96 && tid < 96 + kTW) {
+        const int x = X0 + tid - 96;
+        s_mx[tid - 96] = x < g.w ? g.mx0[x] : (int16_t)0;
+    } else if (tid >= 96 + kTW && tid < 96 + kTW + kTH) {
+        const int y = Y0 + tid - (96 + kTW);
+        s_my[tid - (96 + kTW)] = y < g.h ? g.my0[y] : (int16_t)0;
     }
+    static_assert(kTileW + kTileH + kTW + 2 <= kThreads && kTH + 2 <= 96 && 96 + kTW + kTH <= kThreads, "one table entry per thread");
     // ---- stage the source rows: by TMA (above), or -- caller images with an unaligned base / stride -- 16-byte chunks per warp ----
     if (!use_tma) {
         const int nrows = sy_hi - sy_lo + 1;
@@ -240,6 +252,7 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
     // every pixel of the score tile (tile + 1 ring) lies inside some FAST cell, and so inside the level: FAST needs no per-pixel test
     const bool fast_inner = __syncthreads_and(in_cells);
     if (use_tma) mbar_wait(&s_bar, 0);
+    K1_SPLIT_EXIT(1);
     const int wb = use_tma ? g.box_w : kSrcWB;                          // row stride of the staged region in bytes
 
     if (level == 0 && ctaid_x() * kTW >= kHalo && ctaid_x() * kTW + kTW + kHalo <= g.w) {
@@ -255,19 +268,19 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
                 const uint32_t* r = (const uint32_t*)(s_row + s_ys0[ty] * wb);
                 const uint32_t w = r[0], wn = r[1];                         // pixels 4q .. 4q+3, 4q+4 .. 4q+7
                 const uint32_t a0 = __byte_perm(w, 0u, 0x4140), a1 = __byte_perm(w, 0u, 0x4342);
-                *(uint32_t*)(s_t8 + ty * kT8S + 4 * q) = w;
                 *(uint2*)(s_a0 + ty * kT16S + 4 * q) = make_uint2(a0, a1);
                 *(uint2*)(s_a1 + ty * kT16S + 4 * q) = make_uint2(__byte_perm(w, 0u, 0x4241), __byte_perm(a1, wn, 0x1412));
             }
         }
-    } else if (tid < (kTileW / 2) * 7) {
+    } else if (tid < (kTileW / 2) * (kThreads / (kTileW / 2))) {
         // ---- bilinear resize (OpenCV 11-bit fixed point) into the three tile forms; a thread owns a pixel-pair column ----
+        constexpr int kRG = kThreads / (kTileW / 2);
         const int pc = tid % (kTileW / 2), rg = tid / (kTileW / 2);      // 36 pair columns x 7 row groups
         const int tx = 2 * pc;
         const int xs00 = s_xs0[tx], xs01 = s_xs1[tx], xs10 = s_xs0[tx + 1], xs11 = s_xs1[tx + 1];
         const int a00 = s_xa0[tx], a01 = s_xa1[tx], a10 = s_xa0[tx + 1], a11 = s_xa1[tx + 1];
 #pragma unroll
-        for (int ty = rg; ty < kTileH; ty += 7) {
+        for (int ty = rg; ty < kTileH; ty += kRG) {
             const uint8_t* r0 = s_src + s_ys0[ty] * wb;
             const uint8_t* r1 = s_src + s_ys1[ty] * wb;
             const int b0 = s_yb0[ty], b1 = s_yb1[ty];
@@ -281,13 +294,13 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
                 v1 = (((b0 * (h10 >> 4)) >> 16) + ((b1 * (h11 >> 4)) >> 16) + 2) >> 2;
                 v0 = min(max(v0, 0), 255); v1 = min(max(v1, 0), 255);
             }
-            *(uint16_t*)(s_t8 + ty * kT8S + tx) = (uint16_t)(v0 | (v1 << 8));
             *(uint32_t*)(s_a0 + ty * kT16S + tx) = (uint32_t)v0 | ((uint32_t)v1 << 16);
             if (tx > 0) s_a1[ty * kT16S + tx - 1] = (uint16_t)v0;
             s_a1[ty * kT16S + tx] = (uint16_t)v1;
         }
     }
     __syncthreads();
+    K1_SPLIT_EXIT(2);
 
     // same-cell masks for the packed NMS: pair column j holds pixels x = 2j, 2j+1 (score-tile columns x+1, x+2)
     if (tid < kTW / 2) {
@@ -300,14 +313,16 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         s_md[y] = s_celly[y + 2] == s_celly[y + 1] ? 0xFFFFFFFFu : 0u;
     }
     uint8_t* dimg = dst + (size_t)b * g.img_bytes;
-    // ---- (a) store the unblurred tile, 4 px per thread ----
+    // ---- (a) store the unblurred tile, 4 px per thread, packed from the even 16-bit copy ----
 #pragma unroll
     for (int i = tid; i < kTH * (kTW / 4); i += kThreads) {
         const int y = i >> 4, x4 = (i & 15) * 4;
-        if (Y0 + y < g.h && X0 + x4 < g.pitch)
-            *(uint32_t*)(dimg + (size_t)(Y0 + y) * g.pitch + X0 + x4) = *(const uint32_t*)(s_t8 + (y + kHalo) * kT8S + x4 + kHalo);
+        if (Y0 + y < g.h && X0 + x4 < g.pitch) {
+            const uint2 p = *(const uint2*)(s_a0 + (y + kHalo) * kT16S + x4 + kHalo);
+            *(uint32_t*)(dimg + (size_t)(Y0 + y) * g.pitch + X0 + x4) = __byte_perm(p.x, p.y, 0x6420);
+        }
     }
-    // ---- (b) packed horizontal 5-sums of pixel pairs (rows Y0-2 .. Y0+33) ----
+    // ---- (b) packed horizontal 5-sums of pixel pairs (rows Y0-2 .. Y0+kTH+1) ----
 #pragma unroll
     for (int i = tid; i < (kTH + 4) * (kTW / 2); i += kThreads) {
         const int y = i >> 5, j = i & 31;
@@ -318,7 +333,7 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
     // ---- (c) FAST scores of pixel pairs on the tile + 1 ring: score-tile row y, pair j = score-tile columns 2j, 2j+1, centre
     // pixel px = tile col 3+2j (odd) -> word j+1 of the odd copy, pair (px+1, px+2) -> word j+2 of the even copy ----
     constexpr int kPJ = (kTW + 2) / 2;                          // 33 pairs per score-tile row
-    static_assert(kTH % 8 == 0 && kTW == 64, "FAST: one lane per pair column, a warp per score-tile row");
+    static_assert(kTH % 8 == 0 && kTW == 64 && kThreads == 256, "FAST: one lane per pair column, a warp per score-tile row");
     if (s_flag != 0) {                                          // CTA-uniform
         const unsigned th2 = (unsigned)fast_th * 0x00010001u;   // 1 <= fast_th <= 254 (checked by the host)
         // score of pair j on row y; pixels outside every FAST cell get a threshold no margin exceeds (margins are at most 255)
@@ -340,7 +355,7 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
             for (int k = 0; k < kTH / 8; ++k)                   // 8 rows further: 8 * kT16S / 2 words in the pixel tiles
                 sc[k * 4 * kScoreS] = score(o + k * 4 * kT16S, e + k * 4 * kT16S, cells(wid + 8 * k, lane));
         }
-        // the rest: rows 32, 33 (warps 0, 1) and pair column 32 of every row (threads 64 .. 97)
+        // the rest: rows kTH, kTH + 1 (warps 0, 1) and pair column 32 of every row (threads 64 .. 64 + kTH + 1)
         if (tid < 2 * 32 + kTH + 2) {
             const int y = tid < 64 ? kTH + (tid >> 5) : tid - 64, j = tid < 64 ? lane : kPJ - 1;
             const uint32_t* o = (const uint32_t*)(s_a1 + (y + kHalo - 1) * kT16S) + (j + 1);
@@ -349,6 +364,7 @@ pyr_fast_kernel(const __grid_constant__ CUtensorMap src_map, const int use_tma,
         }
     }
     __syncthreads();
+    K1_SPLIT_EXIT(3);
     const int tx0 = ctaid_x() * kTW, ty0 = ctaid_y() * kTH, img = ctaid_z();   // X0, Y0, b again (see ctaid_x)
     uint8_t* bimg = dst_blur + (size_t)img * g.img_bytes;
 
@@ -440,15 +456,20 @@ void launch_repitch(const uint8_t* src, int src_stride, uint8_t* dst, int dst_pi
     repitch_kernel<<<(unsigned)rows, 256, 0, st>>>(src, src_stride, dst, dst_pitch, width, rows);
 }
 
-void launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_t* src, size_t src_img_bytes,
-                     uint8_t* dst, uint8_t* dst_blur, const uint8_t* mask0, int mask_w, size_t mask_bytes,
-                     const int* cam_of_image, const uint8_t* tile_flags, uint32_t* raw, int* raw_count, cudaStream_t st) {
+cudaError_t launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_t* src, size_t src_img_bytes,
+                            uint8_t* dst, uint8_t* dst_blur, const uint8_t* mask0, int mask_w, size_t mask_bytes,
+                            const int* cam_of_image, const uint8_t* tile_flags, uint32_t* raw, int* raw_count, cudaStream_t st) {
     const LevelGeom& g = G.lv[level];
+    // staging sized for this level's source region (box_w <= kSrcWB, box_h <= kSrcH: build_geometry refuses larger), so that
+    // levels at small scale factors keep 4 CTAs per SM.  The opt-in above 48 KB is per device: set on every launch.
+    const int staging = std::max(g.box_h * kSrcWB, kStagingMin);
+    cudaError_t e = cudaFuncSetAttribute(pyr_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSrcH * kSrcWB);
+    if (e != cudaSuccess) return e;
     dim3 grid(g.tiles_x, g.tiles_y, n_images);
     const int aligned = (((uintptr_t)src & 15) == 0 && (g.spitch & 15) == 0 && (src_img_bytes & 15) == 0) ? 1 : 0;
     // tensor map of the source: (row bytes, rows, images), box = the level's staged region.  Encoding is a host-side table fill
     // (no driver round trip), done per launch because the base address and the batch size are per call.  Sources with an
-    // unaligned base or stride, and boxes larger than the staging buffer, are staged with __ldg instead (use_tma = 0).
+    // unaligned base or stride are staged with __ldg instead (use_tma = 0).
     CUtensorMap map;
     std::memset(&map, 0, sizeof(map));
     int use_tma = 0;
@@ -458,7 +479,7 @@ void launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr) != cudaSuccess || qr != cudaDriverEntryPointSuccess) fn = nullptr;
         return (PFN_cuTensorMapEncodeTiled_v12000)fn;
     }();
-    if (encode && aligned && g.box_w * g.box_h <= kSrcH * kSrcWB) {
+    if (encode && aligned) {
         const cuuint64_t dims[3] = {(cuuint64_t)g.spitch, (cuuint64_t)g.sh, (cuuint64_t)n_images};
         const cuuint64_t strides[2] = {(cuuint64_t)g.spitch, (cuuint64_t)src_img_bytes};
         const cuuint32_t box[3] = {(cuuint32_t)g.box_w, (cuuint32_t)g.box_h, 1u};
@@ -466,9 +487,10 @@ void launch_pyr_fast(const PyramidGeom& G, int level, int n_images, const uint8_
         use_tma = encode(&map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, (void*)src, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
     }
-    pyr_fast_kernel<<<grid, kThreads, 0, st>>>(map, use_tma, g, level, G.nlevels, G.fast_threshold, aligned, src, src_img_bytes, dst, dst_blur,
-                                               mask0, mask_w, mask_bytes, cam_of_image, tile_flags, G.tiles_total, raw, G.raw_total,
-                                               raw_count);
+    pyr_fast_kernel<<<grid, kThreads, staging, st>>>(map, use_tma, g, level, G.nlevels, G.fast_threshold, aligned, src, src_img_bytes, dst,
+                                                     dst_blur, mask0, mask_w, mask_bytes, cam_of_image, tile_flags, G.tiles_total, raw,
+                                                     G.raw_total, raw_count);
+    return cudaGetLastError();
 }
 
 }  // namespace mcs
