@@ -10,26 +10,9 @@ turn a case into an easy one."""
 import numpy as np
 import pytest
 
-from extract_cases import TILE_H, TILE_W, WARPS, axis_cells, boundary_lattice, cams_for, run_batch
+from extract_cases import axis_cells, boundary_lattice, boundary_lattice_target, cams_for, fullest_segment, run_batch
 
 pytestmark = pytest.mark.gpu
-
-WARP_SEGMENT_BEFORE_FIX = 128              # corner slots per warp when K1 assumed one strict maximum per pixel pair of a row
-
-
-def warp_segments(raw):
-    """level-0 raw corners (x, y, score) -> {(tile x, tile y, warp): corners}, the way K1 collects them"""
-    seg = {}
-    for x, y, _ in raw:
-        key = (int(x) // TILE_W, int(y) // TILE_H, (int(y) % TILE_H) % WARPS)
-        seg[key] = seg.get(key, 0) + 1
-    return seg
-
-
-def overflowing_segments(raw):
-    """warp segments holding more corners than the old 128-slot segment while the next warp of the same tile holds corners too"""
-    seg = warp_segments(raw)
-    return [k for k, v in seg.items() if v > WARP_SEGMENT_BEFORE_FIX and seg.get((k[0], k[1], k[2] + 1), 0) > 0], seg
 
 
 @pytest.mark.parametrize("mode", ["orb", "dbrief", "mdbrief"])
@@ -41,8 +24,7 @@ def test_dense_lattice_cell_boundaries(api, oa, cams, w, h, nlevels, mode):
     masks = np.stack([np.ones((h, w), np.uint8)] * 3)
     res = run_batch(api, oa, imgs, masks, cs, [0, 1, 2], 2000 if w > 1000 else 1000, mode, nlevels=nlevels)
     for i, (_, raw) in enumerate(res):
-        hit, seg = overflowing_segments(raw)
-        assert hit, f"image {i}: no warp segment above {WARP_SEGMENT_BEFORE_FIX} with a non-empty next warp (max {max(seg.values())})"
+        assert fullest_segment(raw) == boundary_lattice_target(w), f"image {i}: fullest warp segment before a non-empty one"
 
 
 def test_dense_lattice_device_unaligned(api, oa, cams):
@@ -64,7 +46,7 @@ def test_dense_lattice_device_unaligned(api, oa, cams):
     kps = out["kps"].cpu().numpy().view(api.KEYPOINT_DTYPE).reshape(3, -1)
     for i in range(3):
         ok, od, om = oe.extract(imgs[i], masks[i], cs[i])
-        assert overflowing_segments(oe.debug_read(0, 3))[0]
+        assert fullest_segment(oe.debug_read(0, 3)) == boundary_lattice_target(w)
         assert np.array_equal(ex.debug_read(0, 3, i), oe.debug_read(0, 3)), f"image {i}: raw corners level 0"
         n = counts[i]
         assert n == len(ok) and kps[i, :n].tobytes() == ok.tobytes()

@@ -1,30 +1,17 @@
 """K1 (pyr_fast_kernel) collects the strict per-cell 3x3 maxima of FAST scores in fixed buffers: a shared-memory segment of
-kWarpCorners slots per warp (a warp owns 4 rows of a 64x32 tile), and a raw corner list of raw_cap entries per level and image.
+kWarpCorners slots per warp (a warp owns 8 rows of a 64x64 tile), and a raw corner list of raw_cap entries per level and image.
 Both are sized from the FAST cell grid.  The NMS treats a neighbour in another cell as 0 (cv::FAST runs per cell), so two maxima
 can touch across a cell edge; inside a cell they cannot.  These checks run the cell grid of every level width and height the
 extractor accepts and compare the worst case with the sizes the kernel and the host use."""
 import math
-import pathlib
-import re
 
 import numpy as np
 
-CSRC = pathlib.Path(__file__).resolve().parents[1] / "multicol_slam_b200" / "csrc"
+from k1_geometry import ROWS_PER_WARP, constants
+
 EDGE = 25
 MIN_B = EDGE - 3
 LEVEL_SIZES = range(2 * EDGE + 8, 4096)    # the host refuses levels below 58 px and images of 4096 px or more
-
-
-def constants():
-    """kTW, kTH, kThreads and kWarpCorners as the kernel source states them (C integer arithmetic)"""
-    common = (CSRC / "mcs_common.cuh").read_text()
-    kern = (CSRC / "pyr_fast_kernel.cu").read_text()
-    c = {k: int(re.search(rf"\b{k} = (\d+)", common).group(1)) for k in ("kTW", "kTH")}
-    c["kThreads"] = int(re.search(r"constexpr int kThreads = (\d+);", kern).group(1))
-    expr = re.search(r"constexpr int kWarpCorners = ([^;]+);", kern).group(1)
-    assert re.fullmatch(r"[\w\s()+*/-]+", expr)
-    c["kWarpCorners"] = eval(expr.replace("/", "//"), {"__builtins__": {}}, dict(c))
-    return c
 
 
 def axis_cells(n, x_axis):
@@ -71,17 +58,16 @@ def test_cells_are_at_least_30_px_wide():
 
 def test_warp_segment_holds_the_worst_tile_rows():
     c = constants()
-    rows_per_warp = c["kTH"] // (c["kThreads"] // 32)
     worst = 0
     for n in LEVEL_SIZES:
         cell = axis_cells(n, True)
         if cell is None:
             continue
         m = tile_row_maxima(cell, c["kTW"])
-        assert rows_per_warp * m <= c["kWarpCorners"], f"level width {n}: {rows_per_warp} rows of {m} maxima"
+        assert ROWS_PER_WARP * m <= c["kWarpCorners"], f"level width {n}: {ROWS_PER_WARP} rows of {m} maxima"
         worst = max(worst, m)
     assert worst == c["kTW"] // 2 + 2                                   # the bound is reached: it is not loose
-    assert rows_per_warp * worst > rows_per_warp * (c["kTW"] // 2)      # one maximum per pixel pair would not be enough
+    assert ROWS_PER_WARP * worst > ROWS_PER_WARP * (c["kTW"] // 2)      # one maximum per pixel pair would not be enough
 
 
 def raw_cap(w, h):

@@ -1,8 +1,9 @@
 """GPU parity of K1 (pyr_fast_kernel) at the boundaries between its code paths, every stage against the CPU oracle at every level.
 
 K1 copies level 0 word by word where a tile's columns and ring need no reflection, and scores FAST without per-pixel cell tests
-where the tile and its ring lie inside the cell grid; the other tiles take the general paths.  Level sizes one pixel above and
-below a multiple of the 64x32 tile put a tile of one or two columns / rows at the right and bottom edges, and the first and last
+where the tile and its ring lie inside the cell grid; the other tiles take the general paths.  Level-0 widths (769, 767, 641,
+703) and heights (449, 511) one pixel above and below a multiple of the 64x64 tile put a tile of one or 63 columns / rows at the
+right and bottom edges (tests/test_k1_tile64_gpu.py covers heights at every level), and the first and last
 tiles of each level touch exactly one image edge and the edge of the cell grid.  Binary noise makes every pixel pair of such a
 tile matter: corners everywhere, saturated margins, and maxima on both sides of every cell edge."""
 import numpy as np

@@ -4,60 +4,22 @@ the level's TMA box and refuses a level whose box exceeds kSrcWB x kSrcH.  These
 (OpenCV INTER_LINEAR source offsets) for the shipped and tested geometries and for scale factors up to 2, so that none of them is
 refused, and check that the config-2 levels (scale 1.2) stage few enough rows for five CTAs per SM."""
 import math
-import pathlib
-import re
 
 import numpy as np
 import pytest
 
-CSRC = pathlib.Path(__file__).resolve().parents[1] / "multicol_slam_b200" / "csrc"
-
-
-def constants():
-    common = (CSRC / "mcs_common.cuh").read_text()
-    return {k: int(re.search(rf"\b{k} = (\d+)", common).group(1)) for k in ("kTW", "kTH", "kHalo", "kSrcWB", "kSrcH")}
-
-
-def src_offsets(n, sn):
-    """source row / column of every output pixel of a level (the host's resize table, float arithmetic as in build_geometry)"""
-    scale = 1.0 / (n / sn)
-    f = ((np.arange(n) + 0.5) * scale - 0.5).astype(np.float32)
-    return np.floor(f).astype(np.int64), scale
-
-
-def level_boxes(W, H, sf, nlevels):
-    """(w, h, box_w, box_h) of every level above 0 as build_geometry computes them"""
-    c = constants()
-    inv, isf = 1.0 / float(np.float32(sf)), 1.0
-    sw, sh, out = W, H, []
-    for _ in range(1, nlevels):
-        isf *= inv
-        w, h = round(W * isf), round(H * isf)
-        xofs, sx = src_offsets(w, sw)
-        yofs, sy = src_offsets(h, sh)
-        assert sx <= 2.08 and sy <= 2.08
-        xofs = np.clip(xofs, 0, sw - 1)              # the host clamps columns; rows are clamped where they are used
-        bw = bh = 1
-        for t in range(0, w, c["kTW"]):
-            xa, xb = max(t - c["kHalo"], 0), min(t + c["kTW"] + c["kHalo"], w) - 1
-            bw = max(bw, min(xofs[xb] + 1, sw - 1) - (xofs[xa] & ~15) + 1)
-        for t in range(0, h, c["kTH"]):
-            ya, yb = max(t - c["kHalo"], 0), min(t + c["kTH"] + c["kHalo"], h) - 1
-            lo, hi = min(max(yofs[ya], 0), sh - 1), min(max(yofs[yb] + 1, 0), sh - 1)
-            bh = max(bh, hi - lo + 1)
-        out.append((w, h, (bw + 15) & ~15, bh))
-        sw, sh = w, h
-    return out
+from k1_geometry import constants, level_boxes
 
 
 GEOMETRIES = [(754, 480, 1.2, 8), (1280, 720, 1.2, 8), (1920, 1080, 1.2, 8), (333, 211, 1.2, 4), (754, 480, 1.5, 5),
-              (754, 480, 2.0, 3), (754, 480, 1.1, 8), (754, 480, 1.33, 6), (705, 577, 1.2, 8), (833, 383, 1.2, 8), (420, 269, 1.2, 8)]
+              (754, 480, 2.0, 3), (754, 480, 1.1, 8), (754, 480, 1.33, 6), (705, 577, 1.2, 8), (833, 383, 1.2, 8), (420, 269, 1.2, 8),
+              (1001, 997, 2.0, 4), (999, 963, 2.0, 4), (754, 480, 1.385, 6)]
 
 
 @pytest.mark.parametrize("W,H,sf,nl", GEOMETRIES)
 def test_tested_geometries_fit_the_staging(W, H, sf, nl):
     c = constants()
-    for w, h, bw, bh in level_boxes(W, H, sf, nl):
+    for w, h, bw, bh, *_ in level_boxes(W, H, sf, nl):
         assert bw <= c["kSrcWB"] and bh <= c["kSrcH"], (w, h, bw, bh)
 
 
@@ -68,7 +30,7 @@ def test_scale_factors_up_to_2_fit_the_staging():
     for sf in np.linspace(1.05, 2.0, 20):
         for W, H in ((754, 480), (1280, 720), (1001, 997)):
             nl = max(2, min(8, int(math.log(min(W, H) / 80) / math.log(sf)) + 1))
-            for w, h, bw, bh in level_boxes(W, H, float(sf), nl):
+            for w, h, bw, bh, *_ in level_boxes(W, H, float(sf), nl):
                 assert bw <= c["kSrcWB"] and bh <= c["kSrcH"], (sf, W, H, w, h, bw, bh)
                 worst = max(worst, bh)
     assert worst > c["kSrcH"] - 8                  # scale 2 comes close to the buffer: kSrcH is not loose
@@ -79,6 +41,5 @@ def test_config2_levels_stage_few_rows():
     after the resize.  With 23 KB of pixel tiles and tables that is 41 KB per CTA, five 256-thread CTAs per SM"""
     c = constants()
     boxes = level_boxes(754, 480, 1.2, 8)
-    score_and_row_sums = (c["kTH"] + 2) * 68 * 2 + (c["kTH"] + 4) * (c["kTW"] // 2) * 4
-    assert max(bh for *_, bh in boxes) <= 90
-    assert max(bh for *_, bh in boxes) * c["kSrcWB"] <= score_and_row_sums
+    assert max(b.box_h for b in boxes) <= 90
+    assert max(b.box_h for b in boxes) * c["kSrcWB"] <= c["kStagingMin"]
